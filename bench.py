@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- headline benchmark of the MDE hot path (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W                    # our arm (CUDA, sm_100a)
+    python bench.py --gpus N --steps K --warmup W                    # our arm (CUDA, sm_90a)
     python bench.py --impl reference --gpus N --steps K --warmup W   # the reference's CPU path, host cores
 
 A "step" is one iteration of MDE.embed(): >= 1 fused evaluation of the whole edge list (value + gradient),
@@ -16,7 +16,15 @@ N > 1   BASELINE.json configs[4] (C5): synthetic SBM, n = 10 000 000, m = 2, Pus
         (`single_gpu`: the weak-scaling base), C2 cut into N shards (`c2_sharded`: the latency cost of the
         exchange on a 560 KB gradient) and a `parity` object.
 
-JSON keys beyond the base contract: `roofline` (fused distortion kernel, cold L2, CUDA events), `cpu_baseline`
+The timed region is exactly K solver steps, split into up to REPEATS windows; the line reports the median time per
+step over those windows.  `--dump-outputs DIR` writes, after the timed steps, what the timed path computed: the
+embedding after its last step and the per-iteration statistics of the solve, as DIR/<name>.npy (float32 / float64).
+All inputs are generated from fixed seeds, so two builds run with the same arguments can be compared output for
+output: the library's default gradient scatter on the sorted-SoA layout has no float atomics (per-edge
+contributions, summed per node in a fixed order), so the timed solve computes the same bits in every run.
+
+JSON keys beyond the base contract: `gpu` (device name and power limit), `roofline` (fused distortion kernel, cold
+L2, CUDA events), `cpu_baseline`
 (the unmodified reference on the host cores, bounded sample), `e2e` (public API with pinned HOST buffers, copies
 inside the timed region), `gpu_launches`, `clocks`, `iters_per_sec`, `reference_torch_cuda`,
 `parity_at_equal_iterations`.
@@ -38,7 +46,8 @@ if REPO not in sys.path:
 
 N_ITEMS, EMBED_DIM, K_NEIGHBORS = 70000, 2, 15
 C5_N, C5_SHARD_EDGES, C5_BLOCK = 10_000_000, 25_000_000, 10_000
-REPEATS = 5          # timed windows of K steps each; the line reports the median window
+REPEATS = 5          # the K timed steps are split into (up to) this many windows; the line reports the median
+DUMP_LIMIT_BYTES = 64 << 20  # --dump-outputs: larger outputs are replaced by a fixed, seeded sample of their rows
 E2E_CALLS = 15       # wall-clock end-to-end calls (host-side noise -- e.g. the nvidia-smi sampler taking driver locks -- has
                      # a heavy tail at 4 ms per call: the median of 15 is stable where the median of 5 was not)
 CPU_THREADS = 16     # ATen's CPU scatter_add / index kernels stop scaling near 16 threads (r01: 16 beat 32, 128)
@@ -111,7 +120,7 @@ def make_config(world):
                             "PushAndPull(Log1p(1.5), Log(1.0)), Centered" % (N_ITEMS, EMBED_DIM, K_NEIGHBORS),
                 "n_items": N_ITEMS, "embedding_dim": EMBED_DIM, "memory_size": 10,
                 "parallelism": "1 GPU",
-                "l2": "solver loop runs L2-warm (working set ~26 MB < 126 MB L2); roofline kernel timed cold (512 MB flush)"}
+                "l2": "solver loop runs L2-warm (working set ~26 MB < 50 MB L2); roofline kernel timed cold (512 MB flush)"}
     return {"workload": "C5: synthetic SBM, n=%d, m=2, %d edges per shard x %d shards (one shard per GPU), "
                         "PushAndPull(Log1p(1.5), Log(1.0)), Centered" % (C5_N, C5_SHARD_EDGES, world),
             "n_items": C5_N, "embedding_dim": 2, "memory_size": 10,
@@ -153,7 +162,7 @@ class ClockSampler(threading.Thread):
 
 
 # ------------------------------------------------------------------------------------------
-# reference arms (the UNMODIFIED reference from baseline/_ref; the numpy oracle port only if it did not travel)
+# reference arms (the UNMODIFIED reference via oracle/ref_loader.py; the numpy oracle port when it is absent)
 # ------------------------------------------------------------------------------------------
 def cpu_reference_run(n, m, edges, w, X0, iters, warm):
     """`warm` untimed + `iters` timed embed iterations of the reference on the host cores, `CPU_THREADS` torch
@@ -188,7 +197,7 @@ def cpu_reference_run(n, m, edges, w, X0, iters, warm):
 
 def cuda_reference_run(edges, w, X0, iters, dev):
     """The reference's own torch-CUDA path (device='cuda') on the same GPU: the denominator of the
-    north_star's '10x the reference's torch-CUDA embed() steps/sec'.  None when baseline/_ref is absent."""
+    north_star's '10x the reference's torch-CUDA embed() steps/sec'.  None when the reference is absent."""
     import torch
     from oracle.ref_loader import load_reference
     ref = load_reference()
@@ -249,16 +258,22 @@ def reference_arm(args, rank, world, K, W):
 # ------------------------------------------------------------------------------------------
 # our arm
 # ------------------------------------------------------------------------------------------
-def timed_windows(solver, K, repeats, barrier, torch, dev, world):
-    """`repeats` windows of exactly K solver iterations, each bracketed by barrier + synchronize, CUDA events
+def window_steps(K, repeats=REPEATS):
+    """K steps split into min(repeats, K) windows of near-equal length."""
+    nw = max(1, min(repeats, K))
+    return [K // nw + (1 if i < K % nw else 0) for i in range(nw)]
+
+
+def timed_windows(solver, steps, barrier, torch, dev, world):
+    """One window per entry of `steps` (solver iterations), each bracketed by barrier + synchronize, CUDA events
     on the launching stream; the max over ranks of every window.  Returns (list of ms, iterations done)."""
     out = []
     done = 0
-    for _ in range(repeats):
+    for k in steps:
         barrier()
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record()
-        done, _ = solver.run(K)
+        done, _ = solver.run(k)
         ev1.record()
         barrier()
         ms = ev0.elapsed_time(ev1)
@@ -271,14 +286,36 @@ def timed_windows(solver, K, repeats, barrier, torch, dev, world):
     return out, done
 
 
-def load_profile(key):
-    """dram traffic of the dominant kernel from the committed ncu artifact (profiles/r02_kernel_profile.json,
-    written by tools/ncu_extract.py from the --set full capture); None when the artifact has no such entry."""
+def ms_per_step(windows, steps):
+    return float(np.median([ms / k for ms, k in zip(windows, steps)]))
+
+
+def gpu_identity(dev):
+    """Name and power limit of the GPU the numbers were measured on (part of every absolute number)."""
+    import torch
+    out = {"name": torch.cuda.get_device_name(dev), "power_limit_w": None, "sm_max_mhz": None}
     try:
-        prof = json.load(open(os.path.join(REPO, "profiles", "r02_kernel_profile.json")))
-        return prof.get(key)
+        r = subprocess.run(["nvidia-smi", "-i", str(dev.index or 0), "--query-gpu=power.limit,clocks.max.sm",
+                            "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=10)
+        pl, mhz = [c.strip() for c in r.stdout.strip().split(",")]
+        out["power_limit_w"], out["sm_max_mhz"] = float(pl), float(mhz)
     except Exception:
-        return None
+        pass
+    return out
+
+
+def dump_outputs(path, arrays):
+    """Write each array as path/<name>.npy in float32 / float64.  An array larger than DUMP_LIMIT_BYTES / 4 is
+    replaced by the rows of a fixed seeded sample (the same rows in every run with the same arguments)."""
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        a = a.astype(np.float32 if a.dtype == np.float32 else np.float64)
+        if a.nbytes > DUMP_LIMIT_BYTES // 4:
+            rows = int(DUMP_LIMIT_BYTES // 4 // (a.nbytes // a.shape[0]))
+            keep = np.sort(np.random.default_rng(0).choice(a.shape[0], rows, replace=False))
+            a = a[keep]
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 def c3_shaped_roofline(torch, dev, lib, _lib, pm):
@@ -299,7 +336,7 @@ def c3_shaped_roofline(torch, dev, lib, _lib, pm):
     mde._layout()
     torch.cuda.synchronize(dev)
     build_s = time.perf_counter() - t0
-    r = kernel_roofline(mde, X, m, int(e.shape[0]), n, torch, dev, lib, _lib, True, "C3_shaped", reps=10)
+    r = kernel_roofline(mde, X, m, int(e.shape[0]), n, torch, dev, lib, _lib, True, reps=10)
     kind = int(lib.mde_edges_kind(mde._layout().handle))
     r["kernel"] = {0: "distortion_quad_kernel<m=2, fused, L_HUBER> (sorted-SoA layout)",
                    2: "distortion_pull_kernel<m=2, fused, L_HUBER> (pull-record layout)",
@@ -312,17 +349,17 @@ def c3_shaped_roofline(torch, dev, lib, _lib, pm):
     return r
 
 
-def kernel_roofline(mde, X0d, m, p_local, n, torch, dev, lib, _lib, cold, profile_key, reps=20):
+def kernel_roofline(mde, X0d, m, p_local, n, torch, dev, lib, _lib, cold, reps=20):
     peaks = {}
     try:
         peaks = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350 GB/s"
     lay = mde._layout()
     grad = torch.zeros_like(X0d)
-    flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev) if cold else None  # > 126 MB L2
+    flush = torch.empty(512 << 20, dtype=torch.uint8, device=dev) if cold else None  # > 50 MB L2
     times = []
     st = torch.cuda.current_stream(dev).cuda_stream
     for it in range((reps + 4) if cold else 10):
@@ -340,17 +377,13 @@ def kernel_roofline(mde, X0d, m, p_local, n, torch, dev, lib, _lib, cold, profil
     b_alg = p_local * 12 + 2 * n * m * 4 + 8
     achieved = b_alg / (k_ms * 1e-3) / 1e9
     kind = int(lib.mde_edges_kind(lay.handle))  # the layout / kernel family the library picked for this workload
-    prof = load_profile("%s:%s" % (profile_key, {0: "soa", 1: "tiles", 2: "pull", 3: "ell"}.get(kind, "?")))
-    kernel = {0: "distortion_quad_kernel<m=2, fused, LOG1P|LOG, fast-math> (sorted-SoA layout)",
+    kernel = {0: "distortion_quad_kernel<m=2, fused, LOG1P|LOG, fast-math> + node_gather_kernel (sorted-SoA layout)",
               1: "distortion_tile_kernel<m=2, fused, LOG1P|LOG, fast-math> (tile-record layout, push)",
               2: "distortion_pull_kernel<m=2, fused, LOG1P|LOG, fast-math> (pull-record layout)",
               3: "distortion_ell_kernel<m=2, fused, LOG1P|LOG, fast-math> (ELL pull records, one lane per owner)"
               }.get(kind, "?")
     return {"bound": "hbm", "kernel": kernel,
             "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-            "traffic": None if prof is None else prof.get("dram_bytes"),
-            "traffic_source": None if prof is None else prof.get("source"),
-            "ncu_duration_us": None if prof is None else prof.get("ncu_duration_us"),  # same capture, cold caches
             "peak_source": peak_src, "algorithmic_bytes": b_alg, "kernel_ms": k_ms,
             "timing": ("CUDA events around one launch, 512 MB L2 flush before each, mean of 20" if cold else
                        "CUDA events around one launch, inputs larger than L2, mean of 6")}
@@ -368,6 +401,8 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--cpu-iters", type=int, default=30)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what they computed as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -407,18 +442,22 @@ def ours_single(args, K, W, torch, pm, _lib, lib, dev, barrier):
     mde = pm.MDE(N_ITEMS, EMBED_DIM, torch.tensor(edges, device=dev), f, pm.Centered(), device=dev)
     X0d = torch.tensor(X0, device=dev)
 
-    # -- device-resident throughput: W warm-up, then REPEATS windows of K timed iterations ----------------
-    solver = mde._solver(mde.constraint, 10, REPEATS * K + W + 8)
+    # -- device-resident throughput: W warm-up, then K timed iterations in up to REPEATS windows ----------
+    solver = mde._solver(mde.constraint, 10, K + W + 8)
     sampler = ClockSampler(dev.index or 0)
     solver.begin(X0d, 0.0)
     solver.run(W)
     barrier()
     sampler.start()
     launches0 = lib.mde_launch_count()
-    windows, done = timed_windows(solver, K, REPEATS, barrier, torch, dev, 1)
-    launches = (lib.mde_launch_count() - launches0) / REPEATS
-    ms = float(np.median(windows))
+    steps = window_steps(K)
+    windows, done = timed_windows(solver, steps, barrier, torch, dev, 1)
+    launches = lib.mde_launch_count() - launches0  # over the K timed steps
+    ms = ms_per_step(windows, steps)
     avg, res, pct, stp, fe = solver.stats(done)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"embedding": solver.x_view().cpu().numpy(), "average_distortions": avg,
+                                         "residual_norms": res, "step_sizes": stp})
 
     # -- end to end through the public API with pinned HOST buffers ---------------------------------------
     X0h = torch.tensor(X0).pin_memory()
@@ -438,7 +477,7 @@ def ours_single(args, K, W, torch, pm, _lib, lib, dev, barrier):
     h2d = X0h.numel() * 4
     d2h = out_h.numel() * 4 + 4 * 8 * e2e_iters + 48 * (e2e_iters // 64 + 2)  # X, statistics, status words
 
-    roofline = kernel_roofline(mde, X0d, EMBED_DIM, p, N_ITEMS, torch, dev, lib, _lib, True, "C2")
+    roofline = kernel_roofline(mde, X0d, EMBED_DIM, p, N_ITEMS, torch, dev, lib, _lib, True)
     roofline_c3 = None
     try:  # an extra measurement must never cost the bench line
         roofline_c3 = c3_shaped_roofline(torch, dev, lib, _lib, pm)
@@ -471,14 +510,14 @@ def ours_single(args, K, W, torch, pm, _lib, lib, dev, barrier):
                          "rel_diff_first": abs(ours_traj[0] - rt[0]) / abs(rt[0]),
                          "rel_diff_last": abs(ours_traj[k_cmp - 1] - rt[k_cmp - 1]) / abs(rt[k_cmp - 1])}
 
-    ips = K / (ms * 1e-3)
+    ips = 1e3 / ms
     cfg = make_config(1)  # identical in both arms (the driver compares it); run details go to top-level keys
     line = {
         "metric": "embed_edges_per_sec", "value": ips * p, "unit": "edges/s", "n_gpus": 1, "steps": K,
-        "warmup": W, "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak",
-        "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": cfg,
-        "iters_per_sec": ips, "timed_windows_ms": windows, "func_evals_total": int(fe),
-        "edges_total": p, "edges_per_gpu": p, "repeats": REPEATS,
+        "warmup": W, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak",
+        "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": cfg, "gpu": gpu_identity(dev),
+        "iters_per_sec": ips, "timed_windows_ms": windows, "timed_window_steps": steps, "func_evals_total": int(fe),
+        "edges_total": p, "edges_per_gpu": p,
         "average_distortion_after_%d_iterations" % done: float(avg[-1]) if len(avg) else None,
         "e2e": {"value": e2e_iters / e2e_s * p, "unit": "edges/s", "iters_per_sec": e2e_iters / e2e_s,
                 "h2d_bytes_per_step": h2d / max(e2e_iters, 1), "d2h_bytes_per_step": d2h / max(e2e_iters, 1),
@@ -526,7 +565,7 @@ def ours_sharded(args, K, W, rank, world, torch, tdist, pm, pdist, _lib, lib, de
     e1.record()
     torch.cuda.synchronize(dev)
     solo_ms = e0.elapsed_time(e1) / Kb
-    roofline = kernel_roofline(solo, X0d, m, p_local, n, torch, dev, lib, _lib, False, "C5_shard") if rank == 0 else None
+    roofline = kernel_roofline(solo, X0d, m, p_local, n, torch, dev, lib, _lib, False) if rank == 0 else None
     tt = torch.tensor([solo_ms], device=dev)
     tdist.all_reduce(tt, op=tdist.ReduceOp.MAX)
     solo_ms = float(tt.item())
@@ -536,7 +575,7 @@ def ours_sharded(args, K, W, rank, world, torch, tdist, pm, pdist, _lib, lib, de
 
     # -- the sharded solve ----------------------------------------------------------------------------------
     mde = build(True)
-    solver = mde._solver(mde.constraint, 10, REPEATS * K + W + 8)
+    solver = mde._solver(mde.constraint, 10, K + W + 8)
     sampler = ClockSampler(dev.index or 0) if rank == 0 else None
     solver.begin(X0d, 0.0)
     solver.run(W)
@@ -544,11 +583,15 @@ def ours_sharded(args, K, W, rank, world, torch, tdist, pm, pdist, _lib, lib, de
     if sampler:
         sampler.start()
     launches0 = lib.mde_launch_count()
-    windows, done = timed_windows(solver, K, REPEATS, barrier, torch, dev, world)
-    launches = (lib.mde_launch_count() - launches0) / REPEATS
+    steps = window_steps(K)
+    windows, done = timed_windows(solver, steps, barrier, torch, dev, world)
+    launches = lib.mde_launch_count() - launches0  # over the K timed steps
     clocks = sampler.stop() if sampler else None
-    ms = float(np.median(windows))
+    ms = ms_per_step(windows, steps)
     avg, res, pct, stp, fe = solver.stats(done)
+    if args.dump_outputs and rank == 0:  # X is replicated: every rank holds the same iterate
+        dump_outputs(args.dump_outputs, {"embedding": solver.x_view().cpu().numpy(), "average_distortions": avg,
+                                         "residual_norms": res, "step_sizes": stp})
 
     # -- parity: the library's peer-memory all-reduce against NCCL on the same per-shard partials; replicas agree ---
     lay = mde._layout()
@@ -599,7 +642,7 @@ def ours_sharded(args, K, W, rank, world, torch, tdist, pm, pdist, _lib, lib, de
         s2 = m2._solver(m2.constraint, 10, 3 * 100 + 16)
         s2.begin(torch.tensor(initial_iterate(0), device=dev), 0.0)
         s2.run(5)
-        w2ms, _ = timed_windows(s2, 100, 3, barrier, torch, dev, world)
+        w2ms, _ = timed_windows(s2, [100] * 3, barrier, torch, dev, world)
         c2 = {"workload": "C2 (1.55 M edges) cut into %d edge shards" % world, "ms_per_step": float(np.median(w2ms)) / 100,
               "iters_per_sec": 100 / (float(np.median(w2ms)) * 1e-3)}
     except Exception as ex:  # pragma: no cover
@@ -607,14 +650,14 @@ def ours_sharded(args, K, W, rank, world, torch, tdist, pm, pdist, _lib, lib, de
 
     if rank != 0:
         return 0
-    ips = K / (ms * 1e-3)
+    ips = 1e3 / ms
     cfg = make_config(world)  # identical in both arms (the driver compares it); run details go to top-level keys
     line = {
         "metric": "embed_edges_per_sec", "value": ips * p_total, "unit": "edges/s", "n_gpus": world, "steps": K,
-        "warmup": W, "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak",
-        "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": cfg,
-        "iters_per_sec": ips, "timed_windows_ms": windows, "func_evals_total": int(fe),
-        "edges_total": p_total, "edges_per_gpu": p_local, "repeats": REPEATS,
+        "warmup": W, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak",
+        "vs_baseline": None, "dtype": "f32", "data": "synthetic", "config": cfg, "gpu": gpu_identity(dev),
+        "iters_per_sec": ips, "timed_windows_ms": windows, "timed_window_steps": steps, "func_evals_total": int(fe),
+        "edges_total": p_total, "edges_per_gpu": p_local,
         "allreduce": "peer-memory kernels (cudaIpc + flag handshake, graph-captured)" if peer else "NCCL host hook",
         "single_gpu": {"what": "rank-local shard (%d edges, n=%d) solved alone on one GPU, max over ranks" % (p_local, n),
                        "ms_per_step": solo_ms, "value": p_local / (solo_ms * 1e-3), "unit": "edges/s"},

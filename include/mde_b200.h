@@ -1,5 +1,5 @@
 /*
- * mde_b200.h -- C ABI of the B200-native MDE hot path (libmde_b200.so).
+ * mde_b200.h -- C ABI of the H100-native (sm_90a) MDE hot path (libmde_b200.so).
  *
  * The reference (cvxgrp/pymde v0.2.1) has no FFI of its own: its hot path is a chain of
  * torch ops behind Python call boundaries.  Each entry point below replaces one of those
@@ -195,7 +195,7 @@ typedef struct mde_solver_opts {
   int32_t max_iter;         /* capacity of the statistics arrays */
   int32_t mode;             /* 0 = host-stepped line search; 1 = CUDA graph per iteration with IF / WHILE
                                conditional nodes; 2 = flat graph of gated "steps" (one closure evaluation each),
-                               no conditional nodes -- the fastest on B200 */
+                               no conditional nodes (the default) */
   int64_t n_anchors;        /* MDE_CONSTRAINT_ANCHORED */
   const int64_t* anchors;   /* device (n_anchors,) */
   const float* anchor_values; /* device (n_anchors, m) */
@@ -252,7 +252,7 @@ int mde_solver_comm_connect(mde_solver_t* s, int rank, const void* handles, int6
  * force below 10 000 rows, the approximate pynndescent above; a third-party dependency either way).  X is a device
  * row-major n x d fp32 matrix.  For every row i the k rows nearest to it in Euclidean distance (i itself excluded)
  * are written to idx_out[i*k .. i*k+k) in ascending distance with their exact fp32 SQUARED distances in d2_out.
- * Cross terms run on the tensor cores (tcgen05, bf16 hi/lo split, fp32 accumulate in TMEM) with a running
+ * Cross terms run on the tensor cores (wgmma, bf16 hi/lo split, fp32 accumulate in registers) with a running
  * top-32 per row; the 32 candidates are re-ranked with exact fp32 distances, so the result is that of a brute-force
  * fp32 search (equal-distance ties aside).  1 <= k <= mde_knn_max_k() (24), k <= n - 1.  `ws`: 1024-byte aligned
  * device scratch of mde_knn_ws_bytes(n, d) bytes.  Asynchronous on `stream`. */

@@ -1,8 +1,9 @@
 """TEST INFRASTRUCTURE ONLY -- loader for the UNMODIFIED reference (cvxgrp/pymde).
 
-Imports the reference `pymde` package either from `baseline/_ref` (a
-`pip install --target` of /root/reference, git-ignored, travels to the GPU box)
-or, when that is absent, straight from /root/reference (this container only).
+Imports the reference `pymde` package from the directory named by the environment variable
+PYMDE_REFERENCE (a checkout of cvxgrp/pymde with its Cython extension built) or, when that is
+unset, from `oracle/_ref` or `baseline/_ref` (both git-ignored; e.g. a `pip install --target` of it).  Tests never need it: what they compare against is stored
+under tests/golden/ (tests/golden/make_golden.py, make_api_golden.py).
 
 The reference eagerly imports matplotlib (pymde/__init__.py:17 ->
 pymde/experiment_utils.py:1-3) and pynndescent (pymde/preprocess/data_matrix.py:116),
@@ -17,7 +18,8 @@ import types
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _REPO = os.path.dirname(_HERE)
-_CANDIDATES = [os.path.join(_REPO, "baseline", "_ref"), "/root/reference"]
+_CANDIDATES = [c for c in (os.environ.get("PYMDE_REFERENCE"), os.path.join(_REPO, "oracle", "_ref"),
+                            os.path.join(_REPO, "baseline", "_ref")) if c]
 
 
 def _stub(name, **attrs):

@@ -1,4 +1,4 @@
-"""pymde_b200 -- a Blackwell (sm_100a) native solver for Minimum-Distortion Embedding,
+"""pymde_b200 -- a Hopper (H100, sm_90a) native solver for Minimum-Distortion Embedding,
 drop-in for the hot path of cvxgrp/pymde: MDE / .embed() / average_distortion /
 preserve_neighbors / preserve_distances / penalties / losses / Centered / Standardized.
 

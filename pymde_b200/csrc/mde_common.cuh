@@ -1,4 +1,4 @@
-// mde_common.cuh -- shared device helpers for the B200 (sm_100a) MDE hot path.
+// mde_common.cuh -- shared device helpers for the H100 (sm_90a) MDE hot path.
 //
 // Distortion functions follow cvxgrp/pymde v0.2.1 pymde/functions/penalties.py:112-400 and
 // pymde/functions/losses.py:61-239; the reference differentiates them with torch autograd,
@@ -29,7 +29,7 @@ extern unsigned long long g_launch_count;  // host-side counter (mde_launch_coun
     if (_e != cudaSuccess) return (int)_e;         \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM; the persistent grids assume it (a 114-SM PCIe part runs a partial second wave)
 constexpr unsigned kFull = 0xffffffffu;
 
 struct FnDev {
@@ -204,7 +204,7 @@ __device__ __forceinline__ void edge_value(const FnDev& fn, float d, float a, fl
 // ------------------------------------------------------------------------------------------
 // fast path for the recipe default PushAndPull(Log1p(1.5), Log(1.0)) (pymde/recipes.py:224-225):
 // MUFU approximations (rsqrt / sqrt / rcp / lg2 / ex2, <= 2 ulp each) instead of the IEEE
-// sequences.  The kernel is instruction-issue bound (profiles/r01_ncu_summary.md), and only the
+// sequences.  The kernel is instruction-issue bound, and only the
 // SUM of the per-edge losses has to agree with the reference to 1e-5: a 1e-7 absolute error per edge
 // is far inside that.  Inputs: squared distance d2.  Outputs: f_k and g_k = f'_k / (p d).
 // ------------------------------------------------------------------------------------------

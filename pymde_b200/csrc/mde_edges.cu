@@ -98,6 +98,70 @@ __device__ __forceinline__ void red_row_fx(long long* __restrict__ F, int r, con
     atomicAdd(reinterpret_cast<unsigned long long*>(F + (int64_t)r * M + c), (unsigned long long)q);
   }
 }
+template <int M>
+__device__ __forceinline__ void store_row(float* __restrict__ C, int64_t k, const float (&v)[M]) {
+  if constexpr (M == 2) *reinterpret_cast<float2*>(C + 2 * k) = make_float2(v[0], v[1]);
+  else if constexpr (M == 4) *reinterpret_cast<float4*>(C + 4 * k) = make_float4(v[0], v[1], v[2], v[3]);
+  else {
+#pragma unroll
+    for (int c = 0; c < M; ++c) C[k * M + c] = v[c];
+  }
+}
+// grad[i] += sum over the node's incident edges of +-contribution.  kGatherLanes lanes per node, lane l takes the
+// entries l, l + 8, ... of the node's list in order and the lanes are combined by a fixed shuffle tree: no atomics,
+// and the same summation order in every run.
+constexpr int kGatherLanes = 8;
+template <int M>
+__global__ void __launch_bounds__(256)
+node_gather_kernel(const int* __restrict__ flag, const float* __restrict__ C, const uint32_t* __restrict__ inc,
+                   const int64_t* __restrict__ off, int64_t n, float* __restrict__ grad) {
+  if (flag != nullptr && *flag == 0) return;
+  const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t i = gid / kGatherLanes;
+  const int l = (int)(gid % kGatherLanes);
+  float acc[M];
+#pragma unroll
+  for (int c = 0; c < M; ++c) acc[c] = 0.0f;
+  if (i < n) {
+    const int64_t j1 = __ldg(off + i + 1);
+#pragma unroll 2
+    for (int64_t j = __ldg(off + i) + l; j < j1; j += kGatherLanes) {
+      const uint32_t w = __ldg(inc + j);
+      const int64_t k = (int64_t)(w >> 1);
+      const float sg = (w & 1u) ? -1.0f : 1.0f;
+      if constexpr (M == 2) {
+        const float2 v = __ldg(reinterpret_cast<const float2*>(C) + k);
+        acc[0] += sg * v.x; acc[1] += sg * v.y;
+      } else if constexpr (M == 4) {
+        const float4 v = __ldg(reinterpret_cast<const float4*>(C) + k);
+        acc[0] += sg * v.x; acc[1] += sg * v.y; acc[2] += sg * v.z; acc[3] += sg * v.w;
+      } else {
+#pragma unroll
+        for (int c = 0; c < M; ++c) acc[c] += sg * __ldg(C + k * M + c);
+      }
+    }
+  }
+#pragma unroll
+  for (int o = kGatherLanes / 2; o > 0; o >>= 1) {
+#pragma unroll
+    for (int c = 0; c < M; ++c) acc[c] += __shfl_xor_sync(kFull, acc[c], o, kGatherLanes);
+  }
+  if (i < n && l == 0) {
+#pragma unroll
+    for (int c = 0; c < M; ++c) grad[i * M + c] += acc[c];
+  }
+}
+// incidence entries of the sorted edges: (node, (k << 1) | endpoint is dst); the per-node counts on the side
+__global__ void inc_keys_kernel(const int32_t* __restrict__ src, const int32_t* __restrict__ dst, int64_t p,
+                                uint32_t* __restrict__ keys, uint32_t* __restrict__ vals, int* __restrict__ count) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= 2 * p) return;
+  const int64_t k = j < p ? j : j - p;
+  const int node = j < p ? src[k] : dst[k];
+  keys[j] = (uint32_t)node;
+  vals[j] = ((uint32_t)k << 1) | (j < p ? 0u : 1u);
+  atomicAdd(count + node, 1);
+}
 __global__ void fx_zero_kernel(const int* __restrict__ flag, long long* __restrict__ F, int64_t count) {
   if (flag != nullptr && *flag == 0) return;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -143,9 +207,7 @@ distortion_small_kernel(const int32_t* __restrict__ src, const int32_t* __restri
     float a[kRounds], b[kRounds];
     bool ok[kRounds];
     // Out-of-range lanes re-read the last edge (index clamp) instead of selecting zeros: every lane
-    // then holds valid row indices and no address is formed from a predicated value.  (A zero-select
-    // on the 64-bit row offset compiled to `CS2R Rd, SRZ` + predicated IMAD.WIDE, which ptxas 12.9
-    // under-stalls on sm_100a -- see profiles/r01_ptxas_cs2r_hazard.md.)
+    // then holds valid row indices and no address is formed from a predicated value.
 #pragma unroll
     for (int r = 0; r < kRounds; ++r) {
       int64_t k = base + r * 32 + lane;
@@ -223,7 +285,7 @@ distortion_quad_kernel(const int32_t* __restrict__ src, const int32_t* __restric
                        const int32_t* __restrict__ perm, const float* __restrict__ gext,
                        int64_t p, const float* __restrict__ X, float* __restrict__ grad,
                        double* __restrict__ loss_partials, FnDev fn, float inv_p,
-                       const int* __restrict__ flag, long long* __restrict__ fx) {
+                       const int* __restrict__ flag, long long* __restrict__ fx, float* __restrict__ cb) {
   if (flag != nullptr && *flag == 0) return;
   constexpr int E = 4 * NQ;  // consecutive edges owned by a thread per iteration
   const int64_t nquads = (p + 3) >> 2;
@@ -316,6 +378,10 @@ distortion_quad_kernel(const int32_t* __restrict__ src, const int32_t* __restric
         float v[M];
 #pragma unroll
         for (int c = 0; c < M; ++c) v[c] = live ? g * diff[c] : 0.0f;
+        if (cb) {  // contribution stored, gathered per node afterwards
+          if (ok) store_row<M>(cb, 4 * (u * NQ) + e, v);
+          continue;
+        }
         if (live) { if (fx) red_row_fx<M>(fx, t[e], v, -1.0f); else red_row<M>(grad, t[e], v, -1.0f); }
         if (s[e] != cur) {  // run of equal src ended: flush its sum
           if (fx) red_row_fx<M>(fx, cur, acc, 1.0f); else red_row<M>(grad, cur, acc, 1.0f);
@@ -327,7 +393,7 @@ distortion_quad_kernel(const int32_t* __restrict__ src, const int32_t* __restric
         for (int c = 0; c < M; ++c) acc[c] += v[c];
       }
     }
-    if (MODE != 1) { if (fx) red_row_fx<M>(fx, cur, acc, 1.0f); else red_row<M>(grad, cur, acc, 1.0f); }
+    if (MODE != 1 && !cb) { if (fx) red_row_fx<M>(fx, cur, acc, 1.0f); else red_row<M>(grad, cur, acc, 1.0f); }
     if (FAST) { lsum += (double)lsum_f; lsum_f = 0.0f; }
   }
   if (MODE != 2) {
@@ -581,6 +647,8 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
     fx_zero_kernel<<<zb, 256, 0, st>>>(flag, fxp, cnt);
     ++g_launch_count;
   }
+  // default on the sorted-SoA layout: per-edge contributions + fixed-order per-node gather (quad kernel only)
+  float* cbp = (!fxp && e->cb && MODE != 1 && m == e->m_hint && small_kernel_variant() != 1) ? e->cb : nullptr;
 #define SMALLK(MM, FA, FR)                                                                            \
   distortion_small_kernel<MM, MODE, FA, FR><<<nb, kSmallThreads, 0, st>>>(                            \
       e->src, e->dst, e->par0, e->has_par1 ? e->par1 : nullptr, e->perm, gext, p, X, grad,           \
@@ -589,7 +657,7 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
 #define QUADK_(MM, FA, FR, FAST, NQV)                                                                 \
   distortion_quad_kernel<MM, MODE, FA, FR, FAST, NQV><<<nb, kQuadThreads, 0, st>>>(                   \
       e->src, e->dst, e->par0, e->has_par1 ? e->par1 : nullptr, e->perm, gext, p, X, grad,           \
-      e->loss_partials, e->fn, inv_p, flag, fxp)
+      e->loss_partials, e->fn, inv_p, flag, fxp, cbp)
 #define QUADK(MM, FA, FR, FAST)                                                                       \
   if (FAST && quad_nq() == 2) { nb = loss_blocks_quad(p, 2); QUADK_(MM, FA, FR, FAST, 2); }           \
   else { nb = loss_blocks_quad(p, 1); QUADK_(MM, FA, FR, FAST, 1); }
@@ -666,6 +734,14 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
     const int64_t cnt = e->n * m;
     int zb = (int)((cnt + 255) / 256); if (zb > kNumSMs * 8) zb = kNumSMs * 8;
     fx_apply_kernel<<<zb, 256, 0, st>>>(flag, fxp, grad, cnt);
+    MDE_LAUNCH_CHECK();
+  }
+  if (cbp) {
+    const unsigned gb = (unsigned)((e->n * kGatherLanes + 255) / 256);
+    if (m == 1) node_gather_kernel<1><<<gb, 256, 0, st>>>(flag, cbp, e->inc, e->inc_off, e->n, grad);
+    else if (m == 2) node_gather_kernel<2><<<gb, 256, 0, st>>>(flag, cbp, e->inc, e->inc_off, e->n, grad);
+    else if (m == 3) node_gather_kernel<3><<<gb, 256, 0, st>>>(flag, cbp, e->inc, e->inc_off, e->n, grad);
+    else node_gather_kernel<4><<<gb, 256, 0, st>>>(flag, cbp, e->inc, e->inc_off, e->n, grad);
     MDE_LAUNCH_CHECK();
   }
   if (nblocks_out) *nblocks_out = nb;
@@ -747,11 +823,10 @@ int mde_edges_create_ex(mde_edges_t** out, const int64_t* edges, int64_t p, int6
   bool dense = false, want_ell = false;
 #define TRY(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { rc = (int)_e; goto fail; } } while (0)
   TRY(cudaMalloc(&e->loss_partials, sizeof(double) * kMaxLossBlocks));
-  // Layout choice (measured on B200, profiles/r02_kernels.md): the SM's L1 -> L2 request path (~1 sector request per
-  // cycle) bounds the gather / scatter; the tile kernels trade requests for instructions (pull: every edge is
-  // evaluated from both ends) and win once an owner's run inside a tile is long, i.e. on dense graphs
-  // (C3: 447 edges per node, 2.0x faster); on sparse ones (C2: 22, C5: 10) the sorted-SoA quad kernel is as fast or
-  // faster, and needs half the layout memory.
+  // Layout choice: the SM's L1 -> L2 request path (~1 sector request per cycle) bounds the gather / scatter; the
+  // tile kernels trade requests for instructions (pull: every edge is evaluated from both ends) and win once an
+  // owner's run inside a tile is long, i.e. on dense graphs (C3: 447 edges per node); on sparse ones (C2: 22, C5: 10)
+  // the sorted-SoA quad kernel needs half the layout memory and no more requests per edge.
   dense = (p / n_items) >= 64;
   pref = layout_pref();
   {  // MDE_B200_DETERMINISTIC=1: order-independent (fixed-point) gradient accumulation; sorted-SoA layout, m <= 4
@@ -761,8 +836,8 @@ int mde_edges_create_ex(mde_edges_t** out, const int64_t* edges, int64_t p, int6
       TRY(cudaMalloc(&e->fx, sizeof(long long) * n_items * embedding_dim));
     }
   }
-  // dense graphs: ELL pull records next to the sorted-SoA arrays (C3-shaped: 110 us against 129 us for the flat pull
-  // records, profiles/r02_kernels.md) whenever the ELL builder accepts the shape (n < 2^24, <= 32 neighbour tiles);
+  // dense graphs: ELL pull records next to the sorted-SoA arrays (fewer instructions per entry than the flat pull
+  // records) whenever the ELL builder accepts the shape (n < 2^24, <= 32 neighbour tiles);
   // MDE_B200_LAYOUT=ell asks for them on any graph
   want_ell = embedding_dim >= 1 && embedding_dim <= 4 && !par1 && !e->det && (pref == 4 || (pref == 0 && dense)) &&
              ell_supported(n_items, embedding_dim);
@@ -806,6 +881,39 @@ int mde_edges_create_ex(mde_edges_t** out, const int64_t* edges, int64_t p, int6
   }
   cudaFree(keys_in); cudaFree(keys_out); cudaFree(vals_in); cudaFree(vals_out); cudaFree(tmp);
   keys_in = keys_out = nullptr; vals_in = vals_out = nullptr; tmp = nullptr;
+  if (!e->det && !want_ell && embedding_dim >= 1 && embedding_dim <= 4 && 2 * p < (1ll << 31)) {
+    // incidence lists of the sorted edges: a stable radix sort by node keeps each node's entries in the order
+    // (src entries by k, then dst entries by k), so the per-node gather adds in the same order in every run
+    uint32_t *ik = nullptr, *ik2 = nullptr, *iv = nullptr;
+    int* cnt = nullptr;
+    const int64_t q = 2 * p;
+    size_t tb2 = 0, sb = 0;
+    int bits = 1;
+    while (bits < 32 && (1ll << bits) < n_items) ++bits;
+    TRY(cudaMalloc(&e->cb, sizeof(float) * p * embedding_dim));
+    TRY(cudaMalloc(&e->inc, sizeof(uint32_t) * q));
+    TRY(cudaMalloc(&e->inc_off, sizeof(int64_t) * (n_items + 1)));
+    TRY(cudaMalloc(&ik, sizeof(uint32_t) * q));
+    TRY(cudaMalloc(&ik2, sizeof(uint32_t) * q));
+    TRY(cudaMalloc(&iv, sizeof(uint32_t) * q));
+    TRY(cudaMalloc(&cnt, sizeof(int) * (n_items + 1)));
+    TRY(cudaMemsetAsync(cnt, 0, sizeof(int) * (n_items + 1), st));
+    inc_keys_kernel<<<ceil_div_i64(q, 256), 256, 0, st>>>(e->src, e->dst, p, ik, iv, cnt);
+    ++g_launch_count;
+    TRY(cudaPeekAtLastError());
+    TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb2, ik, ik2, iv, e->inc, (int)q, 0, bits, st));
+    TRY(cub::DeviceScan::ExclusiveSum(nullptr, sb, cnt, e->inc_off, (int)(n_items + 1), st));
+    if (sb > tb2) tb2 = sb;
+    TRY(cudaMalloc(&tmp, tb2));
+    TRY(cub::DeviceRadixSort::SortPairs(tmp, tb2, ik, ik2, iv, e->inc, (int)q, 0, bits, st));
+    sb = tb2;
+    TRY(cub::DeviceScan::ExclusiveSum(tmp, sb, cnt, e->inc_off, (int)(n_items + 1), st));
+    TRY(cudaStreamSynchronize(st));
+    cudaFree(ik); cudaFree(ik2); cudaFree(iv); cudaFree(cnt); cudaFree(tmp);
+    tmp = nullptr;
+    e->m_hint = embedding_dim;
+    e->nbytes += p * embedding_dim * 4 + q * 4 + (n_items + 1) * 8;
+  }
   if (want_ell) {
     // ELL pull records next to the sorted-SoA arrays (kind 3); MDE_E_UNSUPPORTED leaves the layout at kind 0
     rc = ell_build(e, fn, embedding_dim, st);
@@ -828,7 +936,7 @@ fail:
 int mde_edges_destroy(mde_edges_t* e) {
   if (!e) return 0;
   cudaFree(e->src); cudaFree(e->dst); cudaFree(e->perm); cudaFree(e->par0); cudaFree(e->par1);
-  cudaFree(e->loss_partials); cudaFree(e->fx);
+  cudaFree(e->loss_partials); cudaFree(e->fx); cudaFree(e->cb); cudaFree(e->inc); cudaFree(e->inc_off);
   tiled_free(e);
   pull_free(e);
   ell_free(e);

@@ -39,6 +39,12 @@ struct mde_edges {
   int64_t nbytes = 0;
   int det = 0;               // deterministic mode: gradient contributions accumulate in 64-bit fixed point
   long long* fx = nullptr;   // [n * m_hint] fixed-point accumulator (det only)
+  // sorted-SoA layout, m_hint <= 4: the quad kernel stores every edge's contribution in `cb` (no atomics) and
+  // node_gather_kernel sums a node's incident contributions in the fixed order of `inc` -- a gradient that is the same
+  // bits from run to run
+  float* cb = nullptr;          // [p * m_hint] contribution of sorted edge k (added at src, subtracted at dst)
+  uint32_t* inc = nullptr;      // [2 p] (k << 1) | (node is dst), grouped by node: src entries by k, then dst entries by k
+  int64_t* inc_off = nullptr;   // [n + 1]
   // ---- kind 1 ----
   int m_hint = 0;          // embedding dimension the tile size was chosen for
   int rb = 0;              // log2(R): dst tile rows
@@ -66,7 +72,7 @@ struct mde_edges {
 
 namespace mde {
 
-constexpr int kMaxLossBlocks = 148 * 16;
+constexpr int kMaxLossBlocks = kNumSMs * 16;
 constexpr int kWtEdges = 128;                 // slots per warp-tile
 constexpr int kWtWords = 3 * kWtEdges;        // 32-bit words per record
 constexpr int kWtBytes = kWtWords * 4;        // 1536

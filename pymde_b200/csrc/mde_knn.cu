@@ -1,16 +1,17 @@
 // mde_knn.cu -- exact k-nearest neighbours of the rows of a data matrix (SURVEY section 8 row f3).
 //
 // Replaces the neighbour search of pymde/preprocess/data_matrix.py:91-178 (scikit-learn brute force below 10 000
-// rows, pynndescent above) by an exact search whose cross terms run on the 5th-generation tensor cores:
+// rows, pynndescent above) by an exact search whose cross terms run on the Hopper tensor cores (wgmma):
 //
 //   prep     X (n x d fp32) -> Xh, Xl (n_pad x K_pad bf16, x = hi + lo to 2^-16), ||x||^2 (fp32; +inf on padding)
-//   tiles    one CTA per 128 query rows sweeps ALL candidates in tiles of 256:
-//              TMA (cp.async.bulk.tensor.2d, 128-byte swizzle) stages 64-wide K blocks of the hi and lo parts of both
-//              operands in shared memory (2 stages x 96 KB), one elected thread issues
-//              tcgen05.mma.cta_group::1.kind::f16  D[128 x 256] += Ah Bh^T + Ah Bl^T + Al Bh^T   (fp32 in TMEM),
-//              and four epilogue warps read the finished accumulator with tcgen05.ld (the second accumulator is
-//              being filled meanwhile: 2 x 256 TMEM columns), form ||x||^2 - 2 q.x and keep, per query row, the
-//              KK = 32 smallest in a thread-private list.  The n x n distance matrix never exists.
+//   tiles    one CTA per 128 query rows sweeps ALL candidates in tiles of 128:
+//              a producer warp stages 64-wide K blocks of the hi and lo parts of both operands in shared memory with
+//              TMA (cp.async.bulk.tensor.2d, 128-byte swizzle; 2 stages x 64 KB, mbarrier pipeline), and two consumer
+//              warpgroups (64 query rows each) issue
+//              wgmma.mma_async.m64n128k16.f32.bf16.bf16  D[64 x 128] += Ah Bh^T + Ah Bl^T + Al Bh^T   (fp32 registers),
+//              stage the finished accumulator in shared memory, form ||x||^2 - 2 q.x and keep, per query row, the
+//              KK = 32 smallest in thread-private lists (two threads per row, merged at the end).  The n x n distance
+//              matrix never exists.
 //   re-rank  exact fp32 sum (q - x)^2 of the KK candidates of a row (one warp per row), k smallest, ascending.
 //
 // The bf16 x 3 split leaves an error of ~2^-16 |q||x| on a cross term, far below the gap between the k-th and the
@@ -31,21 +32,26 @@ using namespace mde;
 
 namespace {
 
-constexpr int kTileM = 128;                 // query rows per CTA = TMEM lanes
-constexpr int kTileN = 256;                 // candidates per accumulator = TMEM columns
+constexpr int kTileM = 128;                 // query rows per CTA (two warpgroups of 64)
+constexpr int kTileN = 128;                 // candidates per tile = wgmma N
 constexpr int kBlockK = 64;                 // bf16 elements per 128-byte swizzle row
-constexpr int kUmmaK = 16;                  // K of one tcgen05.mma.kind::f16
+constexpr int kWgmmaK = 16;                 // K of one wgmma.m64n128k16
 constexpr int kStages = 2;
 constexpr int kKK = 32;                     // candidates kept per row before the exact re-rank
 constexpr int kMaxK = 24;
 constexpr int kRowBytes = kBlockK * 2;      // 128
-constexpr int kABytes = kTileM * kRowBytes; // 16 KB: one 128-row operand block (hi or lo)
-constexpr int kStageBytes = 6 * kABytes;    // A hi, A lo, B hi (2 x 128 rows), B lo (2 x 128 rows) = 96 KB
-constexpr int kThreads = 256;               // warp 0: TMA, warp 1: MMA, warp 2: TMEM allocation, warps 4-7: epilogue
-constexpr int kSmemBytes = kStages * kStageBytes + 1024 /* alignment slack */ + 2 * kTileN * 4 /* norms */ + 128;
+constexpr int kOpBytes = 128 * kRowBytes;   // 16 KB: one 128-row operand block (hi or lo)
+constexpr int kStageBytes = 4 * kOpBytes;   // A hi, A lo, B hi, B lo = 64 KB
+constexpr int kConsumerWarps = 8;           // warps 0-7: two consumer warpgroups; warp 8: TMA producer
+constexpr int kThreads = (kConsumerWarps + 1) * 32;
+constexpr int kAccStride = kTileN + 2;      // floats per staged accumulator row: the scan's column reads are conflict-free
+constexpr int kSmemBytes = kStages * kStageBytes + 1024 /* alignment slack */ + kTileM * kAccStride * 4 +
+                           2 * kTileN * 4 /* norms */ + 64 /* barriers */;
+static_assert(kTileM == 128 && kTileN == 128, "one TMA box (64 x 128) serves both operands");
+static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 
 // ---------------------------------------------------------------------------------------------------------------
-// PTX wrappers (tcgen05 / tensor TMA); mbarriers come from mde_tma.cuh
+// PTX wrappers (wgmma / tensor TMA); mbarriers come from mde_tma.cuh
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int x, int y, uint32_t bar) {
   asm volatile(
@@ -56,53 +62,36 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void named_bar_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
-__device__ __forceinline__ void tmem_free(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, both operands K-major; issued by ONE thread for the CTA
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accumulator registers across the asynchronous wgmma window
+__device__ __forceinline__ void fence_operand(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+
+// D[64 x 128] (+)= A[smem, 64 x 16] * B[smem, 128 x 16]^T, both operands K-major; issued by the whole warpgroup.
+// Accumulator fragment: d[4 j + {0, 1}] = (row 16 w + lane / 4, col 8 j + 2 (lane % 4) + {0, 1}), d[4 j + {2, 3}] the
+// same columns of row + 8 (w = warp within the warpgroup).
+__device__ __forceinline__ void wgmma_bf16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives on the mbarrier once every tcgen05.mma issued so far by this thread has completed
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// 32 consecutive fp32 columns of this thread's TMEM lane
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
-// Shared-memory matrix descriptor of a K-major operand block staged by TMA with the 128-byte swizzle: rows of 128
-// bytes, 8-row groups 1024 bytes apart (SBO), one swizzle atom along K (LBO unused), descriptor version 1 (sm_100),
-// layout type 2 = SWIZZLE_128B.  Field layout: cute/arch/mma_sm100_desc.hpp (UMMA::SmemDescriptor).
+// Shared-memory matrix descriptor (sm_90 wgmma) of a K-major operand block staged by TMA with the 128-byte swizzle:
+// rows of 128 bytes, 8-row groups 1024 bytes apart (stride byte offset), one swizzle atom along K (leading byte
+// offset unused), layout type 1 = SWIZZLE_128B in bits 62-63.  Blocks start 1024-aligned (base offset 0).
 __device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 46) | (2ull << 61);
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 62);
 }
-// Instruction descriptor (UMMA::InstrDescriptor): fp32 accumulate, bf16 x bf16, both K-major, M = 128, N = 256
-constexpr uint32_t kInstrDesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(kTileN >> 3) << 17) | ((uint32_t)(kTileM >> 4) << 24);
 
 // ---------------------------------------------------------------------------------------------------------------
 // prep: bf16 hi / lo split (zero padded to n_pad x k_pad) and squared norms (+inf on padded rows)
@@ -127,6 +116,20 @@ knn_prep_kernel(const float* __restrict__ X, int64_t n, int d, int64_t n_pad, in
   if (lane == 0) norms[row] = (row < n) ? acc : __int_as_float(0x7f800000);
 }
 
+// Replace the worst of the KK kept candidates by (dist, col) and find the new worst.  Static indices only, so the
+// lists stay in registers.
+__device__ __forceinline__ void keep_candidate(float (&bd)[kKK], int (&bi)[kKK], float dist, int col, float& thr,
+                                               int& worst) {
+#pragma unroll
+  for (int q = 0; q < kKK; ++q) {
+    if (q == worst) { bd[q] = dist; bi[q] = col; }
+  }
+  float m = bd[0]; int w = 0;
+#pragma unroll
+  for (int q = 1; q < kKK; ++q) { if (bd[q] > m) { m = bd[q]; w = q; } }
+  thr = m; worst = w;
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // tiles: tensor-core cross terms + running top-KK per query row
 // ---------------------------------------------------------------------------------------------------------------
@@ -135,118 +138,126 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
                 const float* __restrict__ norms, int64_t n, int64_t n_pad, int k_pad, int32_t* __restrict__ cand_idx,
                 float* __restrict__ cand_val) {
   extern __shared__ uint8_t smem_raw[];
-  // carve: [stages x 96 KB, 1024-aligned] | norms[2][256] | barriers | tmem base
+  // carve: [stages x 64 KB, 1024-aligned] | staged accumulators [128][kAccStride] | norms[2][128] | barriers
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
-  float* s_norm = reinterpret_cast<float*>(gen + kStages * kStageBytes);
-  uint64_t* s_bar = reinterpret_cast<uint64_t*>(gen + kStages * kStageBytes + 2 * kTileN * 4);
+  float* s_acc = reinterpret_cast<float*>(gen + kStages * kStageBytes);
+  float* s_norm = s_acc + kTileM * kAccStride;
+  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_norm + 2 * kTileN);
   const uint32_t bar0 = smem_u32(s_bar);
-  // barriers: full[s] = bar0 + 8 s, empty[s] = bar0 + 16 + 8 s, tfull[a] = bar0 + 32 + 8 a, tempty[a] = bar0 + 48 + 8 a
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(s_bar + 8);
+  // barriers: full[s] = bar0 + 8 s (TMA bytes landed), empty[s] = bar0 + 16 + 8 s (every consumer warp is done)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_kb = k_pad / kBlockK;
   const int num_tiles = (int)(n_pad / kTileN);
   const int row0 = blockIdx.x * kTileM;
 
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kStages; ++s) { mbar_init(bar0 + 8 * s, 1); mbar_init(bar0 + 16 + 8 * s, 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(bar0 + 32 + 8 * a, 1); mbar_init(bar0 + 48 + 8 * a, 4); }
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kStages; ++s) { mbar_init(bar0 + 8 * s, 1); mbar_init(bar0 + 16 + 8 * s, kConsumerWarps); }
     fence_mbar_init();
-  } else if (warp == 2) {
-    tmem_alloc(smem_u32(s_tmem), 512);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *s_tmem;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kConsumerWarps) {
     // ===== TMA producer =====
-    int stage = 0; uint32_t phase = 0;
-    for (int t = 0; t < num_tiles; ++t) {
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(bar0 + 16 + 8 * stage, phase ^ 1);  // slot released by the MMA thread
-        const uint32_t full = bar0 + 8 * stage;
-        const uint32_t dst = base + stage * kStageBytes;
-        mbar_expect_tx(full, kStageBytes);
-        tma_load_2d(dst, &map_h, kb * kBlockK, row0, full);
-        tma_load_2d(dst + kABytes, &map_l, kb * kBlockK, row0, full);
-        tma_load_2d(dst + 2 * kABytes, &map_h, kb * kBlockK, t * kTileN, full);
-        tma_load_2d(dst + 3 * kABytes, &map_h, kb * kBlockK, t * kTileN + kTileM, full);
-        tma_load_2d(dst + 4 * kABytes, &map_l, kb * kBlockK, t * kTileN, full);
-        tma_load_2d(dst + 5 * kABytes, &map_l, kb * kBlockK, t * kTileN + kTileM, full);
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1 && lane == 0) {
-    // ===== MMA issuer =====
-    int stage = 0; uint32_t phase = 0;
-    for (int t = 0; t < num_tiles; ++t) {
-      const int a = t & 1;
-      mbar_wait(bar0 + 48 + 8 * a, (uint32_t)((t >> 1) & 1) ^ 1);  // accumulator drained by the epilogue
-      tc_fence_after();
-      const uint32_t tacc = tmem + (uint32_t)(a * kTileN);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(bar0 + 8 * stage, phase);  // operands landed
-        tc_fence_after();
-        const uint32_t sa = base + stage * kStageBytes;
-        const uint64_t ah = smem_desc_sw128(sa), al = smem_desc_sw128(sa + kABytes);
-        const uint64_t bh = smem_desc_sw128(sa + 2 * kABytes), bl = smem_desc_sw128(sa + 4 * kABytes);
-#pragma unroll
-        for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-          const uint64_t adv = (uint64_t)((k * kUmmaK * 2) >> 4);  // 32 bytes per K step inside the swizzle atom
-          umma_bf16(tacc, ah + adv, bh + adv, kInstrDesc, (kb | k) != 0);
-          umma_bf16(tacc, ah + adv, bl + adv, kInstrDesc, 1u);
-          umma_bf16(tacc, al + adv, bh + adv, kInstrDesc, 1u);
-        }
-        umma_commit(bar0 + 16 + 8 * stage);                 // frees the smem slot when these MMAs are done
-        if (kb == num_kb - 1) umma_commit(bar0 + 32 + 8 * a);  // accumulator complete
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue: thread <-> query row (TMEM lane) =====
-    const int et = threadIdx.x - 128;            // 0..127
-    const int row = row0 + et;
-    const uint32_t lane_base = (uint32_t)((warp & 3) * 32) << 16;
-    float bd[kKK];
-    int bi[kKK];
-#pragma unroll
-    for (int q = 0; q < kKK; ++q) { bd[q] = __int_as_float(0x7f800000); bi[q] = -1; }
-    float thr = __int_as_float(0x7f800000);
-    int worst = 0;
-    for (int t = 0; t < num_tiles; ++t) {
-      const int a = t & 1;
-      float* sn = s_norm + a * kTileN;
-      // norms of this tile's candidates (the buffer of tile t - 2 was released by the barrier below)
-      sn[et] = __ldg(norms + (int64_t)t * kTileN + et);
-      sn[et + 128] = __ldg(norms + (int64_t)t * kTileN + 128 + et);
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      mbar_wait(bar0 + 32 + 8 * a, (uint32_t)((t >> 1) & 1));
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < kTileN / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tmem + lane_base + (uint32_t)(a * kTileN + c * 32), v);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const float dist = fmaf(-2.0f, __uint_as_float(v[i]), sn[c * 32 + i]);
-          if (dist < thr) {
-            const int col = t * kTileN + c * 32 + i;
-            if (col != row) {
-              bd[worst] = dist; bi[worst] = col;
-              float m = bd[0]; int w = 0;
-#pragma unroll
-              for (int q = 1; q < kKK; ++q) { if (bd[q] > m) { m = bd[q]; w = q; } }
-              thr = m; worst = w;
-            }
-          }
+    if (lane == 0) {
+      int stage = 0; uint32_t phase = 0;
+      for (int t = 0; t < num_tiles; ++t) {
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(bar0 + 16 + 8 * stage, phase ^ 1);  // slot released by the consumers
+          const uint32_t full = bar0 + 8 * stage;
+          const uint32_t dst = base + stage * kStageBytes;
+          mbar_expect_tx(full, kStageBytes);
+          tma_load_2d(dst, &map_h, kb * kBlockK, row0, full);
+          tma_load_2d(dst + kOpBytes, &map_l, kb * kBlockK, row0, full);
+          tma_load_2d(dst + 2 * kOpBytes, &map_h, kb * kBlockK, t * kTileN, full);
+          tma_load_2d(dst + 3 * kOpBytes, &map_l, kb * kBlockK, t * kTileN, full);
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
-      tc_fence_before();
+    }
+    return;
+  }
+
+  // ===== consumers: warpgroup wg owns query rows row0 + 64 wg .. + 63 =====
+  const int wg = warp >> 2;
+  const int et = threadIdx.x & 127;            // thread within the warpgroup
+  float* acc_s = s_acc + wg * 64 * kAccStride;
+  float* sn = s_norm + wg * kTileN;
+  // scan: two threads per query row, columns half, half + 2, half + 4, ...
+  const int lrow = et >> 1, half = et & 1;
+  const int row = row0 + wg * 64 + lrow;
+  // accumulator fragment rows / columns of this thread (see wgmma_bf16)
+  const int frow = 16 * (warp & 3) + (lane >> 2), fcol = 2 * (lane & 3);
+
+  float bd[kKK];
+  int bi[kKK];
+#pragma unroll
+  for (int q = 0; q < kKK; ++q) { bd[q] = __int_as_float(0x7f800000); bi[q] = -1; }
+  float thr = __int_as_float(0x7f800000);
+  int worst = 0;
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+
+  int stage = 0; uint32_t phase = 0;
+  for (int t = 0; t < num_tiles; ++t) {
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(bar0 + 8 * stage, phase);  // operands landed
+      const uint32_t sa = base + stage * kStageBytes;
+      const uint64_t ah = smem_desc_sw128(sa + wg * 64 * kRowBytes), al = smem_desc_sw128(sa + kOpBytes + wg * 64 * kRowBytes);
+      const uint64_t bh = smem_desc_sw128(sa + 2 * kOpBytes), bl = smem_desc_sw128(sa + 3 * kOpBytes);
+#pragma unroll
+      for (int i = 0; i < 64; ++i) fence_operand(acc[i]);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
+        const uint64_t adv = (uint64_t)((k * kWgmmaK * 2) >> 4);  // 32 bytes per K step inside the swizzle atom
+        wgmma_bf16(acc, ah + adv, bh + adv, (kb | k) != 0);
+        wgmma_bf16(acc, ah + adv, bl + adv, 1u);
+        wgmma_bf16(acc, al + adv, bh + adv, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait_all();
+#pragma unroll
+      for (int i = 0; i < 64; ++i) fence_operand(acc[i]);
       __syncwarp();
-      if (lane == 0) mbar_arrive(bar0 + 48 + 8 * a);  // 4 warps -> accumulator free
+      if (lane == 0) mbar_arrive(bar0 + 16 + 8 * stage);  // this warp no longer reads the slot
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+    // the previous tile's scan of acc_s / sn is finished by every thread of the warpgroup
+    named_bar_sync(1 + wg, 128);
+#pragma unroll
+    for (int j = 0; j < kTileN / 8; ++j) {
+      *reinterpret_cast<float2*>(acc_s + frow * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(acc_s + (frow + 8) * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+    sn[et] = __ldg(norms + (int64_t)t * kTileN + et);
+    named_bar_sync(1 + wg, 128);
+    const float* arow = acc_s + lrow * kAccStride;
+#pragma unroll 4
+    for (int i = 0; i < kTileN / 2; ++i) {
+      const int c = 2 * i + half;
+      const float dist = fmaf(-2.0f, arow[c], sn[c]);
+      if (dist < thr) {
+        const int col = t * kTileN + c;
+        if (col != row) keep_candidate(bd, bi, dist, col, thr, worst);
+      }
+    }
+  }
+  // merge the two half-row lists: the odd-column thread hands its list to the even-column thread
+  named_bar_sync(1 + wg, 128);
+  float* xd = acc_s + lrow * kAccStride;
+  int* xi = reinterpret_cast<int*>(xd + kKK);
+  if (half) {
+#pragma unroll
+    for (int q = 0; q < kKK; ++q) { xd[q] = bd[q]; xi[q] = bi[q]; }
+  }
+  named_bar_sync(1 + wg, 128);
+  if (!half) {
+    for (int q = 0; q < kKK; ++q) {
+      const float dist = xd[q];
+      if (dist < thr) keep_candidate(bd, bi, dist, xi[q], thr, worst);
     }
     if (row < n) {
 #pragma unroll
@@ -256,9 +267,6 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_free(tmem, 512);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -275,12 +275,14 @@ distortion_pull_kernel(const PullArgs a) {
       }
     }
     // WAR on the slot: the next record may only be requested once EVERY lane's loads have returned.  A lane
-    // issues the ballot only after it has consumed one element of each vector load (scoreboard wait), and the ballot
-    // completes only when all lanes have issued it; its result feeds a never-taken branch so it cannot be removed.
+    // issues the ballot only after it has consumed one element of EACH load (scoreboard wait), and the ballot
+    // completes only when all lanes have issued it.  Its result guards a never-taken fence: the compiler can neither
+    // drop the ballot (in every mode) nor move the refill's asm above that branch.
     {
-      unsigned chk = __float_as_uint(w[EPL - 1]) ^ __float_as_uint(w[3]) ^ op[EPL / 2 - 1] ^ np_[EPL / 2 - 1] ^
-                     (unsigned)(own_base ^ cnt ^ cls);
-      if (__ballot_sync(kFull, chk == 0x7fc12345u) == 0x80000001u) lsum += 1e-300;
+      unsigned chk = op[EPL / 2 - 1] ^ np_[EPL / 2 - 1] ^ (unsigned)(own_base ^ cnt ^ cls);
+#pragma unroll
+      for (int h = 0; h < EPL / 4; ++h) chk ^= __float_as_uint(w[4 * h + 3]);  // one element of every weight load
+      if (__ballot_sync(kFull, chk == 0x7fc12345u) == 0x80000001u) __threadfence_block();
     }
     if (lane == 0 && t + kPullWarps < wt1) {  // refill the slot: the record is in registers now
       mbar_expect_tx(my_bar, kRecBytes);
@@ -525,13 +527,13 @@ int pull_build(mde_edges* e, const int64_t* edges, const float* par0, const mde_
   const int64_t p2 = 2 * p;
   int rb = (m <= 2) ? 13 : 12;  // X tile of 64 KB (m = 1: 32 KB)
   { const int r = penv_int("MDE_B200_TILE_RB", 0); if (r >= 8 && r <= 15) rb = r; }
-  // entries per lane per warp-tile: 8 amortises the per-record work (C3-shaped: 125 vs 135 us) but needs enough
-  // records to keep 32 warps x 148 SMs busy; smaller problems take 4 (C2: 18.4 vs 22.5 us)
+  // entries per lane per warp-tile: 8 amortises the per-record work but needs enough
+  // records to keep 32 warps on every SM busy; smaller problems take 4
   int epl = (p2 / 256 >= 8ll * kPullWarps * kNumSMs) ? 8 : 4;
   { const int ev = penv_int("MDE_B200_PULL_EPL", 0); if (ev == 4 || ev == 8) epl = ev; }
   const int NE = 32 * epl, kRecWords = rec_words(epl), kRecBytes = rec_bytes(epl);
   if (rb > 16 || pull_smem_bytes(rb, m, epl) > 227u * 1024u) return MDE_E_UNSUPPORTED;
-  int64_t l2_bytes = (int64_t)penv_int("MDE_B200_STILE_MB", 48) << 20;
+  int64_t l2_bytes = (int64_t)penv_int("MDE_B200_STILE_MB", 24) << 20;  // src super-tile budget: see tiled_build
   int ss = rb;
   while (((int64_t)1 << (ss + 1)) * m * 8 <= l2_bytes && ss < 30) ++ss;
   const int64_t R = (int64_t)1 << rb, S = (int64_t)1 << ss;
@@ -541,8 +543,7 @@ int pull_build(mde_edges* e, const int64_t* edges, const float* par0, const mde_
   // Hybrid (MDE_B200_PULL_REP=push; off by default): repulsive edges of PushAndPull are uniformly random pairs -- an
   // owner has ~1 of them per neighbour tile, so mirroring them doubles the work without creating runs.  Stored ONCE
   // ("push" entries: neighbour row from the shared tile, far-endpoint contribution as one global red) they cut the
-  // instructions by 20 % (7.8 M -> 6.2 M at C2) but add 0.9 M L2 requests for the reds: 22.5 us against 20.5 us
-  // mirrored (profiles/r02_kernels.md), so mirroring stays the default.
+  // instructions by a fifth but add one L2 request per repulsive edge for the reds, so mirroring stays the default.
   int hybrid = 0;
   { const char* ev = getenv("MDE_B200_PULL_REP"); if (ev && !strcmp(ev, "push") && fn->push_pull) hybrid = 1; }
   PKeyBits kb;

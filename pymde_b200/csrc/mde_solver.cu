@@ -4,7 +4,7 @@
 // _strong_wolfe (pymde/lbfgs.py:44-253), the value_and_grad closure (pymde/optim.py:100-105)
 // and the per-iteration callback/statistics (pymde/optim.py:94-96,139-173).
 //
-// Design (B200-first):
+// Design:
 //  * every vector (X, x_init, d, g, g_prev, the S/Y history ring) and every scalar (loss,
 //    g.d, Wolfe bracket, Gram matrix of the history, statistics) lives in HBM; the host
 //    only enqueues kernels and reads one 32-byte status word per line-search trial
@@ -1143,9 +1143,8 @@ __global__ void iter_end_kernel(SolverState* __restrict__ S, cudaGraphConditiona
 }
 
 // ---------------------------------------------------------------------------------------
-// mode 2: the solve as a flat chain of identical "steps" (no conditional graph nodes: on B200 an IF node
-// costs ~10 us and a one-trip WHILE node ~16 us, a dependent kernel node 1.4 us --
-// profiles/r01_graph_overheads.txt).  A step = direction kernels (gated) -> axpy -> retraction (gated)
+// mode 2: the solve as a flat chain of identical "steps" (no conditional graph nodes: an IF or WHILE node costs
+// several times a dependent kernel node, tools/microbench/graph_overheads.cu measures them).  A step = direction kernels (gated) -> axpy -> retraction (gated)
 // -> scatter kernel -> tangent projection -> dots + epilogue; it performs exactly one closure evaluation.
 // The epilogue (last block of the dots kernel) advances a small phase machine and writes the gates the
 // next step's kernels read:
@@ -1259,7 +1258,7 @@ static_assert(sizeof(SolverState) % sizeof(double) == 0 && offsetof(SolverState,
 
 // Fixed-order reduction of the head kernel's partial rows (kHeadCols doubles each, 16-byte aligned) into out[]:
 // thread (segment, column pair) loads its rows as double2 -- all loads of a thread in flight together, one L2 round
-// trip for <= 296 rows -- and adds them with two independent accumulators; then thread k combines the segments
+// trip for <= 2 kNumSMs rows -- and adds them with two independent accumulators; then thread k combines the segments
 // serially.  Dependent fp64 chains are what the one-block stage waits for (DADD + SHFL trees cost ~100 cycles a
 // level with 8 resident warps), so there is no shuffle tree here.  Column `kmax` is a maximum, the others sums.
 __device__ void reduce_head_rows(const double* __restrict__ part, int nb, double* __restrict__ out, int kmax) {

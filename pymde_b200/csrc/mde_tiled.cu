@@ -16,7 +16,7 @@
 //     src) keeps its run sum in registers and issues one global red per run, as in the quad kernel.
 //
 // Global L2 requests per edge drop from ~3.3 (2 row gathers + 1.3 reds) to the src side only
-// (~0.2 sector reads + <= 1 red); measured numbers: profiles/r02_*.
+// (~0.2 sector reads + <= 1 red).
 #include <cub/cub.cuh>
 #include <algorithm>
 #include <cstdlib>
@@ -63,7 +63,7 @@ __device__ __forceinline__ TRow<M> ldg_row(const float* __restrict__ X, int r) {
 }
 
 // (x, y) += (a, b) on an 8-byte aligned shared-memory pair: ONE 64-bit CAS per attempt (fp32 add has no native
-// shared-memory atomic on sm_100a -- atomicAdd(float*) itself compiles to LDS + FADD + ATOMS.CAST.SPIN)
+// shared-memory atomic on sm_90a -- atomicAdd(float*) itself compiles to LDS + FADD + ATOMS.CAST.SPIN)
 __device__ __forceinline__ void smem_add2(float* p, float a, float b) {
   unsigned long long* q = reinterpret_cast<unsigned long long*>(p);
   unsigned long long old = *q, assumed;
@@ -333,10 +333,11 @@ distortion_tile_kernel(const TileArgs a) {
       asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(a4.x), "=f"(a4.y), "=f"(a4.z), "=f"(a4.w) : "r"(q + 1024u));
     }
     // WAR on the slot: the next record may only be requested once EVERY lane's loads have returned (a lane issues
-    // the ballot after consuming one element of each vector load; the result feeds a never-taken branch)
+    // the ballot after consuming one element of each vector load; the result guards a never-taken fence, so the
+    // ballot survives in every mode and the refill's asm stays behind it)
     {
       const unsigned chk = (unsigned)(s4.w ^ t4.w) ^ __float_as_uint(a4.w);
-      if (__ballot_sync(kFull, chk == 0x7fc12345u) == 0x80000001u) lsum += 1e-300;
+      if (__ballot_sync(kFull, chk == 0x7fc12345u) == 0x80000001u) __threadfence_block();
     }
     if (lane == 0 && t + kTileWarps < wt1) {  // refill the slot: the record is in registers now
       mbar_expect_tx(my_bar, kWtBytes);
@@ -516,8 +517,9 @@ int tiled_build(mde_edges* e, const int64_t* edges, const float* par0, const mde
   int gred = 0;
   { const char* ev = getenv("MDE_B200_TILE_SCATTER"); if (ev && !strcmp(ev, "global")) gred = 1; }
   if (tile_smem_bytes(rb, m, gred) > 227u * 1024u) return MDE_E_UNSUPPORTED;
-  // src super-tile: X + gradient rows of one super-tile (2 * m * 4 bytes per row) stay L2-resident
-  int64_t l2_bytes = (int64_t)env_int("MDE_B200_STILE_MB", 48) << 20;
+  // src super-tile: X + gradient rows of one super-tile (2 * m * 4 bytes per row) stay L2-resident; 24 MB leaves
+  // about half of the H100's 50 MB L2 to the streamed records and the destination side
+  int64_t l2_bytes = (int64_t)env_int("MDE_B200_STILE_MB", 24) << 20;
   int ss = rb;
   while (((int64_t)1 << (ss + 1)) * m * 8 <= l2_bytes && ss < 30) ++ss;
   const int64_t R = (int64_t)1 << rb, S = (int64_t)1 << ss;

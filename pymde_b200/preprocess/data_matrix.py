@@ -1,6 +1,6 @@
 """Problem construction from a data matrix (interface of pymde/preprocess/data_matrix.py).
 
-k-nearest neighbours are computed EXACTLY on the GPU by the library's own kernel (`mde_knn`: tcgen05 tensor-core
+k-nearest neighbours are computed EXACTLY on the GPU by the library's own kernel (`mde_knn`: wgmma tensor-core
 cross terms with a running top-32 per row and an exact fp32 re-rank, csrc/mde_knn.cu) for k <= 24; larger k uses row
 chunks of a library GEMM + top-k.  The reference uses scikit-learn brute force below 10 000 rows and the approximate
 pynndescent above (data_matrix.py:125-143)."""
@@ -26,7 +26,7 @@ def _to_device_matrix(data, device):
 
 def knn_device(X, k):
     """(indices [n, k] int32, squared distances [n, k] fp32) of the k nearest rows of every row of the CUDA fp32
-    matrix X, ascending; the tcgen05 kernel behind `mde_knn` (include/mde_b200.h)."""
+    matrix X, ascending; the wgmma kernel behind `mde_knn` (include/mde_b200.h)."""
     from .. import _lib
     lib = _lib.load()
     X = X.contiguous()

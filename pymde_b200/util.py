@@ -1,4 +1,4 @@
-"""Host-side utilities of the B200 MDE path (API surface of pymde/util.py kept where it matters).
+"""Host-side utilities of the CUDA MDE path (API surface of pymde/util.py kept where it matters).
 
 Everything numerical here is CUDA-only: tensors must live on a CUDA device; there is no CPU
 fallback for the hot path (pymde_b200._lib raises if the extension is missing)."""
@@ -24,7 +24,7 @@ def cuda_device(device=None):
     dev = torch.device(device) if not isinstance(device, torch.device) else device
     if dev.type != "cuda":
         raise ValueError(
-            "pymde_b200 runs the MDE hot path on CUDA (sm_100a) only; got device %r. "
+            "pymde_b200 runs the MDE hot path on CUDA (sm_90a) only; got device %r. "
             "There is no CPU fallback." % (device,))
     if not torch.cuda.is_available():
         raise RuntimeError("pymde_b200 needs a CUDA device (torch.cuda.is_available() is False)")

@@ -1,11 +1,11 @@
 """Generate golden fixtures by RUNNING THE UNMODIFIED REFERENCE (cvxgrp/pymde v0.2.1).
 
-Run in the build container (where /root/reference or baseline/_ref exists):
+Run with the reference importable (oracle/ref_loader.py):
 
-    python tests/golden/make_golden.py
+    PYMDE_REFERENCE=<reference checkout with its Cython extension built> python tests/golden/make_golden.py
 
 Outputs (committed): tests/golden/functions.npz, evals.npz, projections.npz,
-trajectories.npz.  The GPU box has no reference; tests there read these files.
+trajectories.npz.  Tests read these files; none of them needs the reference.
 Every array is produced by reference code paths only:
   functions    f(d) and autograd df/dd   pymde/functions/{penalties,losses}.py
   evals        MDE.average_distortion + backward   pymde/average_distortion.py:36-80

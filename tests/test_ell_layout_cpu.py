@@ -226,7 +226,7 @@ def test_cta_ranges_are_cost_balanced_on_the_bench_workload():
     edges, w = bench.c2_edges(0)
     e = np.sort(edges, axis=1)
     rc, lay = build(bench.N_ITEMS, 2, e, w, True)
-    assert rc == 0 and lay["ncta"] == 148
+    assert rc == 0 and lay["ncta"] == 132          # one CTA per SM of an H100 SXM
     rec, off = lay["rec"], lay["rec_off"].astype(np.int64) * 16
     hdr = np.stack([np.frombuffer(rec[o:o + 16].tobytes(), dtype=np.int32) for o in off[:-1]])
     W, cls, K = hdr[:, 0], hdr[:, 1], hdr[:, 2]
@@ -239,6 +239,6 @@ def test_cta_ranges_are_cost_balanced_on_the_bench_workload():
         tot.append(cost[a:b].sum() + 6000 * tiles if b > a else 0)
     tot = np.array(tot, dtype=np.float64)
     busy = tot[tot > 0]
-    assert len(busy) >= 146                      # at most the tail CTAs stay empty
+    assert len(busy) >= 130                      # at most the tail CTAs stay empty
     assert busy.max() <= 1.12 * busy.mean(), (busy.max(), busy.mean())
     assert lay["npadded"] <= 1.15 * lay["nentries"]  # pads: 11 % at C2

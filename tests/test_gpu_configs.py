@@ -90,7 +90,7 @@ def test_c2slice_converged_value_within_the_references_own_spread(c2slice):
     spread = refs.max() - refs.min()
     assert spread > 1e-5 * refs.mean()  # (documents why a 1e-5 comparison of end points is not defined here)
     final = mde.average_distortion(X).item()
-    # not worse than the reference's own worst run (it may be better: 0.1511 against 0.1520-0.1530 on B200), and the
+    # not worse than the reference's own worst run (it may be better), and the
     # same basin: within 2 % of the reference's best
     assert final <= refs.max() + 2 * spread, (final, refs)
     assert final >= 0.98 * refs.min(), (final, refs)

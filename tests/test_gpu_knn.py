@@ -1,4 +1,4 @@
-"""Row f3: the tcgen05 k-nearest-neighbour kernel (`mde_knn`, csrc/mde_knn.cu) against an fp64 brute force.
+"""Row f3: the wgmma k-nearest-neighbour kernel (`mde_knn`, csrc/mde_knn.cu) against an fp64 brute force.
 
 The reference's neighbour search (pymde/preprocess/data_matrix.py:91-178) delegates to scikit-learn / pynndescent;
 its contract is "the k nearest rows in Euclidean distance", which is what is checked here: identical neighbour sets

@@ -1,4 +1,4 @@
-"""mde_knn (tcgen05 cross terms + running top-32 + exact re-rank) against an fp64 brute force, and timed against the
+"""mde_knn (wgmma cross terms + running top-32 + exact re-rank) against an fp64 brute force, and timed against the
 library-GEMM + torch.topk path it replaces.  Usage: python tools/knn_check.py [small|full]"""
 import json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,7 +1,7 @@
 // Microbenchmark: what do the pieces of the solver's iteration graph cost on this GPU?
 //   chain of dependent small kernels, IF node (not taken), WHILE node with one trip, a WHILE node that loops
 //   on the device, and back-to-back launches of a one-kernel graph.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o graph_overheads graph_overheads.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o graph_overheads graph_overheads.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>
