@@ -277,6 +277,38 @@ int mde_graph_hops(const int32_t* indptr, const int32_t* indices, int64_t n, int
                    float* out_len, int64_t cap, unsigned long long* count_dev, void* ws, int64_t ws_bytes,
                    void* stream);
 
+/* Shortest paths of a WEIGHTED undirected graph (SURVEY section 8 row f4).  Replaces the chunked scipy Dijkstra of
+ * pymde/preprocess/graph.py:345-474 (and its per-source helper, pymde/preprocess/graph.py:311-335).  Device CSR:
+ * int32 indptr[n+1], indices[nnz], fp32 weights[nnz] (NULL = unit weights); both directions of every edge present,
+ * entries positive and finite, duplicates allowed (the shorter wins).  Lengths are fp64 sums of the widened
+ * weights, so they equal scipy's dijkstra bit for bit after the cast to fp32.  Same output contract as
+ * mde_graph_hops: for every source s in [s_begin, s_end) and every node v > s with length <= max_length (<= 0 or
+ * inf: unlimited), the triple (s, v, length) is kept when the same counter-based hash of (seed, s, v) falls under
+ * `retain` (one seed selects the same pairs in both engines), appended unsorted to out_src / out_dst / out_len
+ * (capacity `cap`); *count_dev (caller zeroes it) receives the total, and the caller re-runs with larger buffers
+ * when it exceeds `cap`.  Sources run in batches of B (a multiple of 32), the largest that `ws_bytes` holds:
+ * `ws` >= mde_graph_sssp_ws_bytes(n, 32) bytes of device scratch; mde_graph_sssp_ws_bytes(n, B) is the size for
+ * batches of B (-1 if B is not a positive multiple of 32).  Per batch the work is proportional to the
+ * (source, node) pairs the searches reach.  Blocking (one status read per few relaxation rounds, at most n
+ * rounds per batch). */
+int64_t mde_graph_sssp_ws_bytes(int64_t n, int batch);
+int mde_graph_sssp(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n,
+                   int64_t s_begin, int64_t s_end, double max_length, double retain, uint64_t seed, int32_t* out_src,
+                   int32_t* out_dst, float* out_len, int64_t cap, unsigned long long* count_dev, void* ws,
+                   int64_t ws_bytes, void* stream);
+
+/* k nearest neighbours of every node under the shortest-path metric of the same CSR (weights NULL = unit).
+ * Replaces pymde/preprocess/graph.py:503-586 (chunked Dijkstra with limit = max_distance, then a partition per
+ * row).  For every node s, the k smallest (length, node index) pairs in lexicographic order, s itself excluded,
+ * length <= max_distance (<= 0 or inf: unlimited), go to out_idx[s*k .. s*k+k) (int32) and out_len (fp32),
+ * ascending; rows with fewer than k such nodes are padded with -1 / +inf.  Ties break by node index, so the result
+ * is fully determined.  1 <= k <= mde_graph_knn_max_k() (64).  `ws` >= mde_graph_knn_ws_bytes(n, 32) bytes; the
+ * batch is derived from `ws_bytes` as for mde_graph_sssp.  Blocking. */
+int mde_graph_knn_max_k(void);
+int64_t mde_graph_knn_ws_bytes(int64_t n, int batch);
+int mde_graph_knn(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n, int k,
+                  double max_distance, int32_t* out_idx, float* out_len, void* ws, int64_t ws_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -92,6 +92,14 @@ SIGNATURES = {
     "mde_graph_hops": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_double,
                                  C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                  C.c_int64, C.c_void_p]),
+    "mde_graph_sssp_ws_bytes": (C.c_int64, [C.c_int64, C.c_int]),
+    "mde_graph_sssp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_double,
+                                 C.c_double, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                 C.c_void_p, C.c_int64, C.c_void_p]),
+    "mde_graph_knn_max_k": (C.c_int, []),
+    "mde_graph_knn_ws_bytes": (C.c_int64, [C.c_int64, C.c_int]),
+    "mde_graph_knn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_double, C.c_void_p,
+                                C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "mde_solver_comm_export": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64]),
     "mde_solver_comm_connect": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]),
 }

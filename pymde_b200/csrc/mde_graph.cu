@@ -11,12 +11,18 @@
 // finished shortest path of `level` hops; it is kept when a counter-based hash of (seed, s, v) falls under
 // `retain` and appended through one warp-aggregated atomic per warp.  The output order depends on the schedule
 // (the SET of triples does not); the caller sorts by (s, v).
+//
+// Weighted graphs (mde_graph_sssp) and the graph k-nearest neighbours (mde_graph_knn) use a frontier-driven
+// Bellman-Ford engine further down.
 #include <cstdint>
 #include <cstdlib>
+
+#include <cooperative_groups.h>
 
 #include "mde_common.cuh"
 
 using namespace mde;
+namespace cg = cooperative_groups;
 
 namespace {
 
@@ -101,11 +107,385 @@ hops_level_kernel(const int32_t* __restrict__ indptr, const int32_t* __restrict_
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// Weighted shortest paths (mde_graph_sssp) and graph k-nearest neighbours (mde_graph_knn).
+//
+// Algorithm: frontier-driven Bellman-Ford over a batch of B sources.  The batch owns one distance tile
+// dist[v * B + b] (fp64 bit patterns; ~0 = not reached).  A queue holds the (node, source) entries improved in the
+// last round; one thread per entry pushes its length to the node's neighbours with a 64-bit atomicMin.  Non-negative
+// doubles order like their unsigned bit patterns, x -> fl(x + w) is monotone and never decreases for w >= 0, so any
+// relaxation order reaches the same least fixed point: per node, the minimum fp64 fold-sum over paths -- exactly what
+// scipy's Dijkstra computes on the float64-widened weights.  The result is schedule-free, bit for bit.  Chosen over
+// delta-stepping for its simplicity: the recipes' searches are either radius-bounded (k-NN: a few rounds) or
+// sampled all-pairs, where every (source, node) entry is settled anyway and the extra re-relaxations of plain
+// Bellman-Ford stay a small factor.
+//
+// Locality: nothing per batch costs O(n * B) unless the search touches that many entries.  Every entry reached for
+// the first time (atomicMin returns ~0) is appended once to a `touched` list; emission, k-NN selection and the reset
+// of the tile for the next batch walk that list.  The tile and the queue stamps are initialised once per call.
+// A per-entry stamp (the round that last queued it) keeps each entry at most once in a queue, so every queue fits in
+// n * B slots.  Queue entries are packed (v << 32) | b.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr unsigned long long kUnreached = ~0ull;
+constexpr int kRelaxThreads = 256;
+constexpr int kRelaxBlocks = kNumSMs * 8;   // fixed grid: the queue length lives on the device
+constexpr int kRoundsPerCheck = 4;          // rounds launched between two reads of the queue length
+constexpr int kKnnMaxK = 64;
+
+// device-side counters: queue lengths (3-slot rotation, see sssp_relax_kernel) and the touched-list length
+struct PathCounters {
+  unsigned long long queue[3];
+  unsigned long long touched;
+};
+
+struct PathWs {
+  PathCounters* ctr;
+  unsigned long long* dist;   // [n * B]
+  uint64_t* touched;          // [n * B] packed entries
+  uint64_t* queue[2];         // [n * B] each; after convergence queue[0] doubles as the k-NN segment buffer
+  int* stamp;                 // [n * B]
+  int* seg_count;             // [B]
+  unsigned long long* seg_off;  // [B + 1]
+  unsigned long long* seg_cur;  // [B]
+};
+
+constexpr int64_t kMaxBatch = 1 << 20;
+
+inline int64_t align_up(int64_t x) { return (x + 255) & ~int64_t(255); }
+
+inline int64_t path_ws_bytes(int64_t n, int64_t B) {
+  const int64_t nb = n * B;
+  return align_up(sizeof(PathCounters)) + 4 * align_up(nb * 8) + align_up(nb * 4) + align_up(B * 4) +
+         align_up(B * 8) + align_up((B + 1) * 8) + 256;
+}
+
+// largest multiple of 32 (at most the rounded-up source count) whose workspace fits; 0 if not even 32 fits
+inline int64_t path_batch(int64_t n, int64_t nsrc, int64_t ws_bytes) {
+  int64_t most = ((nsrc + 31) / 32) * 32;
+  if (most > kMaxBatch) most = kMaxBatch;
+  if (ws_bytes < path_ws_bytes(n, 32)) return 0;
+  int64_t lo = 32, hi = most < 32 ? 32 : most;
+  while (lo < hi) {  // binary search over multiples of 32
+    const int64_t mid = ((lo + hi + 32) / 64) * 32;
+    if (mid > lo && path_ws_bytes(n, mid) <= ws_bytes) lo = mid; else hi = mid - 32;
+  }
+  return lo;
+}
+
+inline PathWs path_ws(void* ws, int64_t n, int64_t B) {
+  uintptr_t p = ((uintptr_t)ws + 255) & ~uintptr_t(255);
+  const int64_t nb = n * B;
+  PathWs w;
+  w.ctr = reinterpret_cast<PathCounters*>(p); p += align_up(sizeof(PathCounters));
+  w.dist = reinterpret_cast<unsigned long long*>(p); p += align_up(nb * 8);
+  w.touched = reinterpret_cast<uint64_t*>(p); p += align_up(nb * 8);
+  w.queue[0] = reinterpret_cast<uint64_t*>(p); p += align_up(nb * 8);
+  w.queue[1] = reinterpret_cast<uint64_t*>(p); p += align_up(nb * 8);
+  w.stamp = reinterpret_cast<int*>(p); p += align_up(nb * 4);
+  w.seg_count = reinterpret_cast<int*>(p); p += align_up(B * 4);
+  w.seg_cur = reinterpret_cast<unsigned long long*>(p); p += align_up(B * 8);
+  w.seg_off = reinterpret_cast<unsigned long long*>(p);
+  return w;
+}
+
+// warp-aggregated append: one atomic per group of lanes that reach the call together
+__device__ __forceinline__ unsigned long long append_slot(unsigned long long* ctr) {
+  cg::coalesced_group g = cg::coalesced_threads();
+  unsigned long long base = 0ull;
+  if (g.thread_rank() == 0) base = atomicAdd(ctr, (unsigned long long)g.size());
+  return g.shfl(base, 0) + g.thread_rank();
+}
+
+__global__ void sssp_seed_kernel(PathWs w, int64_t B, int64_t s0, int nsrc) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b == 0) {
+    w.ctr->queue[1] = (unsigned long long)nsrc;  // round 1 reads slot 1 and appends to slot 2
+    w.ctr->queue[2] = 0ull;
+    w.ctr->touched = (unsigned long long)nsrc;
+  }
+  if (b >= nsrc) return;
+  const int64_t v = s0 + b;
+  const uint64_t e = ((uint64_t)v << 32) | (uint32_t)b;
+  w.dist[v * B + b] = 0ull;  // bit pattern of +0.0
+  w.stamp[v * B + b] = 1;
+  w.touched[b] = e;
+  w.queue[1][b] = e;
+}
+
+// Round r: relax every entry queued for round r (queue[r & 1], length in slot r % 3) and queue the improved entries
+// for round r + 1 (queue[(r + 1) & 1], slot (r + 1) % 3).  Slot (r + 2) % 3 was round r - 1's input and is zeroed
+// here for round r + 1's appends, so rounds run back to back without host work in between.
+__global__ void __launch_bounds__(kRelaxThreads)
+sssp_relax_kernel(const int32_t* __restrict__ indptr, const int32_t* __restrict__ indices,
+                  const float* __restrict__ weights, PathWs w, int64_t B, double max_len, int round) {
+  const unsigned long long nin = w.ctr->queue[round % 3];
+  unsigned long long* nout = &w.ctr->queue[(round + 1) % 3];
+  if (blockIdx.x == 0 && threadIdx.x == 0) w.ctr->queue[(round + 2) % 3] = 0ull;
+  // (a select, not w.queue[round & 1]: indexing the by-value parameter array would copy it to the stack)
+  const uint64_t* __restrict__ qin = (round & 1) ? w.queue[1] : w.queue[0];
+  uint64_t* __restrict__ qout = (round & 1) ? w.queue[0] : w.queue[1];
+  const int next = round + 1;
+  for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < nin;
+       i += (unsigned long long)gridDim.x * blockDim.x) {
+    const uint64_t e = qin[i];
+    const int64_t u = (int64_t)(e >> 32);
+    const int64_t b = (int64_t)(e & 0xffffffffull);
+    const double du = __longlong_as_double((long long)w.dist[u * B + b]);
+    const int p0 = indptr[u], p1 = indptr[u + 1];
+    for (int p = p0; p < p1; ++p) {
+      const int64_t v = indices[p];
+      const double nd = du + (weights ? (double)weights[p] : 1.0);
+      if (!(nd <= max_len)) continue;
+      const unsigned long long bits = (unsigned long long)__double_as_longlong(nd);
+      unsigned long long* slot = &w.dist[v * B + b];
+      if (bits >= *slot) continue;  // a stale read is never below the current value: safe to skip
+      const unsigned long long old = atomicMin(slot, bits);
+      if (bits >= old) continue;
+      const uint64_t ev = ((uint64_t)v << 32) | (uint64_t)b;
+      if (old == kUnreached) w.touched[append_slot(&w.ctr->touched)] = ev;
+      if (atomicExch(&w.stamp[v * B + b], next) != next) qout[append_slot(nout)] = ev;
+    }
+  }
+}
+
+// Shortest-path emission (same rule and hash as hops_level_kernel) fused with the reset of the touched entries.
+__global__ void __launch_bounds__(256)
+sssp_emit_reset_kernel(PathWs w, int64_t B, int64_t n, int64_t s0, uint64_t seed, uint64_t thresh,
+                       int32_t* __restrict__ out_src, int32_t* __restrict__ out_dst, float* __restrict__ out_len,
+                       int64_t cap, unsigned long long* __restrict__ count) {
+  const unsigned long long nt = w.ctr->touched;
+  const int lane = threadIdx.x & 31;
+  const unsigned long long warp0 = ((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) & ~31ull;
+  const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
+  for (unsigned long long base = warp0; base < nt; base += stride) {  // warp-uniform trip count
+    const unsigned long long i = base + lane;
+    bool keep = false;
+    int64_t s = 0, v = 0;
+    float len = 0.0f;
+    if (i < nt) {
+      const uint64_t e = w.touched[i];
+      v = (int64_t)(e >> 32);
+      const int64_t b = (int64_t)(e & 0xffffffffull);
+      s = s0 + b;
+      len = (float)__longlong_as_double((long long)w.dist[v * B + b]);
+      w.dist[v * B + b] = kUnreached;
+      w.stamp[v * B + b] = 0;
+      keep = v > s && (thresh == ~0ull || splitmix64(seed ^ ((uint64_t)s * (uint64_t)n + (uint64_t)v)) < thresh);
+    }
+    const unsigned ballot = __ballot_sync(kFull, keep);
+    unsigned long long pos = 0ull;
+    if (lane == 0 && ballot) pos = atomicAdd(count, (unsigned long long)__popc(ballot));
+    pos = __shfl_sync(kFull, pos, 0) + (unsigned long long)__popc(ballot & ((1u << lane) - 1u));
+    if (keep && (int64_t)pos < cap) {
+      out_src[pos] = (int32_t)s;
+      out_dst[pos] = (int32_t)v;
+      out_len[pos] = len;
+    }
+  }
+}
+
+// k-NN selection, step 1: entries per source (the source itself excluded)
+__global__ void knn_count_kernel(PathWs w, int64_t s0) {
+  const unsigned long long nt = w.ctr->touched;
+  for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < nt;
+       i += (unsigned long long)gridDim.x * blockDim.x) {
+    const uint64_t e = w.touched[i];
+    const int64_t b = (int64_t)(e & 0xffffffffull);
+    if ((int64_t)(e >> 32) != s0 + b) atomicAdd(&w.seg_count[b], 1);
+  }
+}
+
+// step 2: exclusive scan of the B counts (one block of 1024 threads, contiguous chunks per thread)
+__global__ void __launch_bounds__(1024) knn_scan_kernel(PathWs w, int B) {
+  __shared__ unsigned long long warp_tot[32];
+  const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
+  const int chunk = (B + 1023) / 1024;
+  const int c0 = t * chunk, c1 = min(B, c0 + chunk);
+  unsigned long long sum = 0ull;
+  for (int c = c0; c < c1; ++c) sum += (unsigned long long)w.seg_count[c];
+  unsigned long long incl = sum;
+#pragma unroll
+  for (int off = 1; off < 32; off <<= 1) {
+    const unsigned long long o = __shfl_up_sync(kFull, incl, off);
+    if (lane >= off) incl += o;
+  }
+  if (lane == 31) warp_tot[wid] = incl;
+  __syncthreads();
+  if (wid == 0) {
+    unsigned long long x = warp_tot[lane];
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const unsigned long long o = __shfl_up_sync(kFull, x, off);
+      if (lane >= off) x += o;
+    }
+    warp_tot[lane] = x;  // inclusive over warps
+  }
+  __syncthreads();
+  unsigned long long run = incl - sum + (wid > 0 ? warp_tot[wid - 1] : 0ull);
+  for (int c = c0; c < c1; ++c) {
+    w.seg_off[c] = run;
+    w.seg_cur[c] = run;
+    run += w.seg_count[c];
+  }
+  if (t == 1023) w.seg_off[B] = warp_tot[31];
+}
+
+// step 3: node indices grouped by source (order within a group is irrelevant: selection keys are unique)
+__global__ void knn_scatter_kernel(PathWs w, int64_t s0) {
+  const unsigned long long nt = w.ctr->touched;
+  int32_t* seg = reinterpret_cast<int32_t*>(w.queue[0]);
+  for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < nt;
+       i += (unsigned long long)gridDim.x * blockDim.x) {
+    const uint64_t e = w.touched[i];
+    const int64_t v = (int64_t)(e >> 32), b = (int64_t)(e & 0xffffffffull);
+    if (v != s0 + b) seg[atomicAdd(&w.seg_cur[b], 1ull)] = (int32_t)v;
+  }
+}
+
+__device__ __forceinline__ bool key_less(unsigned long long d0, int v0, unsigned long long d1, int v1) {
+  return d0 < d1 || (d0 == d1 && v0 < v1);
+}
+
+// step 4: one warp per source; k rounds of a warp-wide minimum of (length, node) above the last one chosen
+__global__ void __launch_bounds__(256)
+knn_select_kernel(PathWs w, int64_t B, int64_t s0, int nsrc, int k, int32_t* __restrict__ out_idx,
+                  float* __restrict__ out_len) {
+  const int b = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  const int lane = threadIdx.x & 31;
+  if (b >= nsrc) return;
+  const int32_t* seg = reinterpret_cast<const int32_t*>(w.queue[0]);
+  const int64_t lo = (int64_t)w.seg_off[b], hi = (int64_t)w.seg_off[b + 1];
+  unsigned long long last_d = 0ull;
+  int last_v = -1;
+  int32_t* oi = out_idx + (s0 + b) * (int64_t)k;
+  float* ol = out_len + (s0 + b) * (int64_t)k;
+  for (int j = 0; j < k; ++j) {
+    unsigned long long best_d = kUnreached;
+    int best_v = 0x7fffffff;
+    for (int64_t i = lo + lane; i < hi; i += 32) {
+      const int v = seg[i];
+      const unsigned long long d = w.dist[(int64_t)v * B + b];
+      if (key_less(last_d, last_v, d, v) && key_less(d, v, best_d, best_v)) { best_d = d; best_v = v; }
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      const unsigned long long od = __shfl_xor_sync(kFull, best_d, off);
+      const int ov = __shfl_xor_sync(kFull, best_v, off);
+      if (key_less(od, ov, best_d, best_v)) { best_d = od; best_v = ov; }
+    }
+    if (lane == 0) {
+      const bool found = best_d != kUnreached;
+      oi[j] = found ? best_v : -1;
+      ol[j] = found ? (float)__longlong_as_double((long long)best_d) : __int_as_float(0x7f800000);
+    }
+    last_d = best_d;
+    last_v = best_v;
+  }
+}
+
+__global__ void path_reset_kernel(PathWs w, int64_t B) {
+  const unsigned long long nt = w.ctr->touched;
+  for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < nt;
+       i += (unsigned long long)gridDim.x * blockDim.x) {
+    const uint64_t e = w.touched[i];
+    const int64_t idx = (int64_t)(e >> 32) * B + (int64_t)(e & 0xffffffffull);
+    w.dist[idx] = kUnreached;
+    w.stamp[idx] = 0;
+  }
+}
+
+// Runs the batches of [s_begin, s_end).  `finish(s0, nsrc)` enqueues the per-batch emission / selection and MUST
+// leave the tile reset.  Blocking: one read of the queue length every kRoundsPerCheck rounds, at most n rounds.
+template <class Finish>
+int run_batches(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n, int64_t s_begin,
+                int64_t s_end, double max_len, const PathWs& w, int64_t B, cudaStream_t st, Finish finish) {
+  MDE_CUDA_TRY(cudaMemsetAsync(w.dist, 0xff, (size_t)(n * B) * sizeof(unsigned long long), st));
+  MDE_CUDA_TRY(cudaMemsetAsync(w.stamp, 0, (size_t)(n * B) * sizeof(int), st));
+  unsigned long long* pending = nullptr;
+  MDE_CUDA_TRY(cudaMallocHost(&pending, sizeof(unsigned long long)));
+  int rc = 0;
+  for (int64_t s0 = s_begin; s0 < s_end && !rc; s0 += B) {
+    const int nsrc = (int)((s_end - s0) < B ? (s_end - s0) : B);
+    sssp_seed_kernel<<<(nsrc + 255) / 256, 256, 0, st>>>(w, B, s0, nsrc);
+    ++g_launch_count;
+    for (int64_t r = 1; r <= n; ++r) {
+      sssp_relax_kernel<<<kRelaxBlocks, kRelaxThreads, 0, st>>>(indptr, indices, weights, w, B, max_len, (int)r);
+      ++g_launch_count;
+      if (r % kRoundsPerCheck != 0 && r != n) continue;
+      cudaError_t err = cudaMemcpyAsync(pending, &w.ctr->queue[(r + 1) % 3], sizeof(unsigned long long),
+                                        cudaMemcpyDeviceToHost, st);
+      if (err == cudaSuccess) err = cudaStreamSynchronize(st);
+      if (err != cudaSuccess) { rc = (int)err; break; }
+      if (*pending == 0ull) break;  // no entry improved in the last round: the batch has converged
+    }
+    if (!rc) rc = finish(s0, nsrc);
+  }
+  cudaFreeHost(pending);
+  if (!rc) { cudaError_t e = cudaStreamSynchronize(st); if (e == cudaSuccess) e = cudaPeekAtLastError(); rc = (int)e; }
+  return rc;
+}
+
+inline double length_limit(double max_length) {
+  return (max_length > 0.0 && max_length < INFINITY) ? max_length : INFINITY;
+}
+
 }  // namespace
 
 extern "C" {
 
 int64_t mde_graph_hops_ws_bytes(int64_t n) { return 3 * n * kWords * (int64_t)sizeof(uint64_t) + 64; }
+
+int64_t mde_graph_sssp_ws_bytes(int64_t n, int batch) {
+  if (n < 1 || batch < 32 || batch % 32) return -1;
+  return path_ws_bytes(n, batch);
+}
+
+int64_t mde_graph_knn_ws_bytes(int64_t n, int batch) { return mde_graph_sssp_ws_bytes(n, batch); }
+
+int mde_graph_knn_max_k(void) { return kKnnMaxK; }
+
+int mde_graph_sssp(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n, int64_t s_begin,
+                   int64_t s_end, double max_length, double retain, uint64_t seed, int32_t* out_src,
+                   int32_t* out_dst, float* out_len, int64_t cap, unsigned long long* count_dev, void* ws,
+                   int64_t ws_bytes, void* stream) {
+  if (!indptr || !indices || n < 1 || n >= (1ll << 31) || s_begin < 0 || s_end > n || s_begin > s_end ||
+      !count_dev || !ws || cap < 0 || (cap > 0 && (!out_src || !out_dst || !out_len)))
+    return MDE_E_INVALID;
+  const int64_t B = path_batch(n, s_end - s_begin, ws_bytes);
+  if (B < 32) return MDE_E_INVALID;
+  if (s_begin == s_end) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const PathWs w = path_ws(ws, n, B);
+  const uint64_t thresh = (retain >= 1.0) ? ~0ull : (uint64_t)(retain * 18446744073709551616.0);
+  return run_batches(indptr, indices, weights, n, s_begin, s_end, length_limit(max_length), w, B, st,
+                     [&](int64_t s0, int) -> int {
+                       sssp_emit_reset_kernel<<<kRelaxBlocks, 256, 0, st>>>(w, B, n, s0, seed, thresh, out_src,
+                                                                            out_dst, out_len, cap, count_dev);
+                       ++g_launch_count;
+                       return 0;
+                     });
+}
+
+int mde_graph_knn(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n, int k,
+                  double max_distance, int32_t* out_idx, float* out_len, void* ws, int64_t ws_bytes, void* stream) {
+  if (!indptr || !indices || n < 1 || n >= (1ll << 31) || k < 1 || k > kKnnMaxK || !out_idx || !out_len || !ws)
+    return MDE_E_INVALID;
+  const int64_t B = path_batch(n, n, ws_bytes);
+  if (B < 32) return MDE_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  const PathWs w = path_ws(ws, n, B);
+  return run_batches(indptr, indices, weights, n, 0, n, length_limit(max_distance), w, B, st,
+                     [&](int64_t s0, int nsrc) -> int {
+                       MDE_CUDA_TRY(cudaMemsetAsync(w.seg_count, 0, (size_t)B * sizeof(int), st));
+                       knn_count_kernel<<<kRelaxBlocks, 256, 0, st>>>(w, s0);
+                       knn_scan_kernel<<<1, 1024, 0, st>>>(w, (int)B);
+                       knn_scatter_kernel<<<kRelaxBlocks, 256, 0, st>>>(w, s0);
+                       knn_select_kernel<<<(nsrc * 32 + 255) / 256, 256, 0, st>>>(w, B, s0, nsrc, k, out_idx, out_len);
+                       path_reset_kernel<<<kRelaxBlocks, 256, 0, st>>>(w, B);
+                       g_launch_count += 5;
+                       return 0;
+                     });
+}
 
 int mde_graph_hops(const int32_t* indptr, const int32_t* indices, int64_t n, int64_t s_begin, int64_t s_end,
                    int max_length, double retain, uint64_t seed, int32_t* out_src, int32_t* out_dst,

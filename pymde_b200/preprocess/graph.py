@@ -142,34 +142,63 @@ class EdgeListGraph(object):
         return Graph.from_edges(self.edges.cpu().numpy(), self.distances.cpu().numpy(), n_items=self._n)
 
 
-def shortest_paths_device(graph, max_length=None, retain_fraction=1.0, device=None, seed=None):
-    """Hop-count shortest paths of an UNWEIGHTED graph on the GPU (`mde_graph_hops`: bit-parallel multi-source BFS,
-    256 sources per pass over the adjacency).  Same contract as `shortest_paths` -- pairs (i < j) within `max_length`
-    hops, each kept with probability `retain_fraction` -- but the sample is drawn by a counter-based hash seeded from
-    the module RNG, and the result stays on the device as an `EdgeListGraph`."""
-    import ctypes as C
-    from .. import _lib, util
-    A = graph.adjacency_matrix if isinstance(graph, Graph) else Graph(graph).adjacency_matrix
+_PATH_WS_BUDGET = 8 << 30  # device scratch of the weighted engine: caps its batch of sources
+
+
+def _is_unweighted(A):
+    return bool((A.data == 1.0).all())
+
+
+def _device_csr(A, dev):
+    """Undirected device CSR of `A` for the weighted engine: the entries of A and of A^T (the semantics of scipy's
+    `dijkstra(directed=False)`, also for an asymmetric A), with parallel entries reduced to the shortest one --
+    the same shortest paths as keeping them all, at half the relaxations for a symmetric A.  (scipy's Dijkstra
+    treats parallel entries the same way for float64 data, but sums them when it converts another dtype.)  int32
+    indptr and indices, fp32 weights.  Negative weights raise ValueError (scipy's Dijkstra rejects them too)."""
+    if A.nnz and float(A.data.min()) < 0:
+        raise ValueError("shortest paths need non-negative edge weights")
     n = A.shape[0]
-    dev = util.cuda_device(device)
-    lib = _lib.load()
-    indptr = torch.tensor(A.indptr.astype(np.int32), device=dev)
-    indices = torch.tensor(A.indices.astype(np.int32), device=dev)
-    ws = torch.empty(int(lib.mde_graph_hops_ws_bytes(n)), dtype=torch.uint8, device=dev)
-    if seed is None:
-        seed = int(util.np_rng().integers(0, 2 ** 62))
+    coo = A.tocoo()
+    r = torch.tensor(coo.row.astype(np.int64), device=dev)
+    c = torch.tensor(coo.col.astype(np.int64), device=dev)
+    w = torch.tensor(coo.data.astype(np.float32), device=dev)
+    r, c, w = torch.cat([r, c]), torch.cat([c, r]), torch.cat([w, w])
+    order = torch.argsort(w, stable=True)          # within one (row, col) key the shortest entry comes first
+    key = (r * n + c)[order]
+    order = order[torch.argsort(key, stable=True)]
+    key, w = (r * n + c)[order], w[order]
+    first = torch.ones_like(key, dtype=torch.bool)
+    first[1:] = key[1:] != key[:-1]
+    key, w = key[first], w[first]
+    rows = key // n
+    indptr = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+    indptr[1:] = torch.cumsum(torch.bincount(rows, minlength=n), 0)
+    return indptr.int(), (key % n).int(), w.contiguous()
+
+
+def _path_ws(ws_bytes_fn, n, nsrc, dev):
+    """Scratch for the weighted engine: the batch of sources grows with the memory it is given (fewer batches,
+    fewer synchronising rounds), up to a quarter of the free device memory or _PATH_WS_BUDGET."""
+    per32 = int(ws_bytes_fn(n, 64)) - int(ws_bytes_fn(n, 32))
+    free = torch.cuda.mem_get_info(dev)[0]
+    budget = min(_PATH_WS_BUDGET, free // 4)
+    batch = max(32, min((nsrc + 31) // 32 * 32, int(budget // max(per32, 1)) * 32))
+    return torch.empty(int(ws_bytes_fn(n, batch)), dtype=torch.uint8, device=dev)
+
+
+def _collect_pairs(run, n, retain_fraction, dev):
+    """Shared tail of the shortest-path engines: `run(src, dst, len, cap, count)` appends (s, v, length) triples;
+    the buffers are sized from the expected sample, the call is repeated with larger ones when they overflowed (the
+    same seed draws the same sample), and the result is sorted by (s, v) into an `EdgeListGraph`."""
     expected = min(1.0, float(retain_fraction)) * n * (n - 1) / 2
     cap = int(expected * 1.02 + 4 * (expected ** 0.5) + 1024)
-    limit = 0 if (max_length is None or not np.isfinite(max_length)) else int(max_length)
     while True:
         src = torch.empty(cap, dtype=torch.int32, device=dev)
         dst = torch.empty(cap, dtype=torch.int32, device=dev)
         ln = torch.empty(cap, dtype=torch.float32, device=dev)
         count = torch.zeros(1, dtype=torch.int64, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(lib.mde_graph_hops(indptr.data_ptr(), indices.data_ptr(), n, 0, n, limit, float(retain_fraction),
-                                          C.c_uint64(seed), src.data_ptr(), dst.data_ptr(), ln.data_ptr(), cap,
-                                          count.data_ptr(), ws.data_ptr(), ws.numel(), util.stream_ptr(dev)))
+            run(src, dst, ln, cap, count)
         got = int(count.item())
         if got <= cap:
             break
@@ -177,6 +206,76 @@ def shortest_paths_device(graph, max_length=None, retain_fraction=1.0, device=No
     src, dst, ln = src[:got].long(), dst[:got].long(), ln[:got]
     order = torch.argsort(src * n + dst)
     return EdgeListGraph(torch.stack([src[order], dst[order]], 1), ln[order], n)
+
+
+def shortest_paths_device(graph, max_length=None, retain_fraction=1.0, device=None, seed=None):
+    """Shortest paths on the GPU.  Same contract as `shortest_paths` -- pairs (i < j) within `max_length`, each kept
+    with probability `retain_fraction` -- but the sample is drawn by a counter-based hash seeded from the module RNG,
+    and the result stays on the device as an `EdgeListGraph`.  Unweighted graphs use hop counts (`mde_graph_hops`:
+    bit-parallel multi-source BFS, 256 sources per pass over the adjacency); weighted ones `mde_graph_sssp`
+    (batched frontier Bellman-Ford with fp64 lengths, equal to scipy's Dijkstra after the cast to fp32).  The same
+    seed selects the same pairs in both engines."""
+    import ctypes as C
+    from .. import _lib, util
+    A = graph.adjacency_matrix if isinstance(graph, Graph) else Graph(graph).adjacency_matrix
+    n = A.shape[0]
+    dev = util.cuda_device(device)
+    lib = _lib.load()
+    if seed is None:
+        seed = int(util.np_rng().integers(0, 2 ** 62))
+    unlimited = max_length is None or not np.isfinite(max_length)
+    if _is_unweighted(A):
+        indptr = torch.tensor(A.indptr.astype(np.int32), device=dev)
+        indices = torch.tensor(A.indices.astype(np.int32), device=dev)
+        ws = torch.empty(int(lib.mde_graph_hops_ws_bytes(n)), dtype=torch.uint8, device=dev)
+        limit = 0 if unlimited else int(max_length)
+
+        def run(src, dst, ln, cap, count):
+            _lib.check(lib.mde_graph_hops(indptr.data_ptr(), indices.data_ptr(), n, 0, n, limit, float(retain_fraction),
+                                          C.c_uint64(seed), src.data_ptr(), dst.data_ptr(), ln.data_ptr(), cap,
+                                          count.data_ptr(), ws.data_ptr(), ws.numel(), util.stream_ptr(dev)))
+    else:
+        indptr, indices, weights = _device_csr(A, dev)
+        ws = _path_ws(lib.mde_graph_sssp_ws_bytes, n, n, dev)
+        limit = 0.0 if unlimited else float(max_length)
+
+        def run(src, dst, ln, cap, count):
+            _lib.check(lib.mde_graph_sssp(indptr.data_ptr(), indices.data_ptr(), weights.data_ptr(), n, 0, n, limit,
+                                          float(retain_fraction), C.c_uint64(seed), src.data_ptr(), dst.data_ptr(),
+                                          ln.data_ptr(), cap, count.data_ptr(), ws.data_ptr(), ws.numel(),
+                                          util.stream_ptr(dev)))
+    return _collect_pairs(run, n, retain_fraction, dev)
+
+
+def k_nearest_neighbors_device(graph, k, max_distance=None, device=None):
+    """k-nearest-neighbour graph under the shortest-path metric, on the GPU (`mde_graph_knn`).  Every node's k
+    nearest nodes within `max_distance` (ties broken by node index), as undirected pairs (i < j) sorted by (i, j);
+    a pair that is a neighbour in both directions gets weight 2, otherwise 1 -- the edges and weights that
+    `k_nearest_neighbors` gives when no lengths tie.  Returns an `EdgeListGraph` on the device."""
+    from .. import _lib, util
+    A = graph.adjacency_matrix if isinstance(graph, Graph) else Graph(graph).adjacency_matrix
+    n = A.shape[0]
+    k = int(k)
+    dev = util.cuda_device(device)
+    lib = _lib.load()
+    if not 1 <= k <= int(lib.mde_graph_knn_max_k()):
+        raise ValueError("k must be between 1 and %d" % int(lib.mde_graph_knn_max_k()))
+    indptr, indices, weights = _device_csr(A, dev)
+    wptr = None if _is_unweighted(A) else weights.data_ptr()
+    ws = _path_ws(lib.mde_graph_knn_ws_bytes, n, n, dev)
+    idx = torch.empty(n * k, dtype=torch.int32, device=dev)
+    ln = torch.empty(n * k, dtype=torch.float32, device=dev)
+    limit = 0.0 if (max_distance is None or not np.isfinite(max_distance)) else float(max_distance)
+    with torch.cuda.device(dev):
+        _lib.check(lib.mde_graph_knn(indptr.data_ptr(), indices.data_ptr(), wptr, n, k, limit, idx.data_ptr(),
+                                     ln.data_ptr(), ws.data_ptr(), ws.numel(), util.stream_ptr(dev)))
+    dst = idx.long()
+    src = torch.arange(n, device=dev).repeat_interleave(k)
+    found = dst >= 0
+    src, dst = src[found], dst[found]
+    key = torch.minimum(src, dst) * n + torch.maximum(src, dst)
+    key, counts = torch.unique_consecutive(torch.sort(key)[0], return_counts=True)
+    return EdgeListGraph(torch.stack([key // n, key % n], 1), counts.float(), n)
 
 
 def shortest_paths(graph, max_length=None, retain_fraction=1.0, n_workers=None, verbose=False):
