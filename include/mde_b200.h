@@ -261,6 +261,26 @@ int mde_knn_ws_bytes(int64_t n, int d, size_t* bytes);
 int mde_knn(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
             void* stream);
 
+/* The same search on a sparse data matrix, without densifying it (pymde/preprocess/data_matrix.py:19,99 accepts
+ * scipy.sparse input).  Device CSR of an n x d matrix: int64 indptr[n+1] (indptr[0] = 0, indptr[n] = nnz), int32
+ * indices[nnz] strictly increasing within a row and below d, fp32 values[nnz]; nnz may exceed 2^31.  Output contract
+ * of mde_knn, except that the distances are the exact squared distances summed in fp64 and rounded once to fp32, and
+ * the k rows are the k smallest (distance, index) pairs in lexicographic order: the result is fully determined,
+ * ties included.  Cross terms run on the tensor cores over the 64-feature blocks both tiles occupy (features ordered
+ * by descending document frequency); nothing n x d sized is allocated.  1 <= k <= mde_knn_max_k() (24),
+ * k <= n - 1.  `ws`: 1024-byte aligned device scratch of mde_knn_csr_ws_bytes(n, d, nnz) bytes (about 20 bytes per
+ * non-zero and 260 per row, plus 20 per feature and the sort's scratch).  MDE_E_INVALID also when the CSR is malformed (checked on the device).
+ * Blocking (one status read after the check). */
+int mde_knn_csr_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes);
+int mde_knn_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
+                int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream);
+/* Euclidean distances ||x_a - x_b|| of p row pairs (device int64 pairs[p][2]) of the same CSR, into out[p] (fp32):
+ * a sorted merge of the two rows summed in fp64, sqrt in fp64, one rounding (pymde/preprocess/data_matrix.py:59-70
+ * takes the norm of the difference in scipy).  MDE_E_INVALID for a malformed CSR or a pair index outside [0, n).
+ * Blocking. */
+int mde_pair_dist_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                      const int64_t* pairs, int64_t p, float* out, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * Problem construction next to the path (SURVEY section 8 row f4).
  * Hop-count shortest paths of an UNWEIGHTED undirected graph given as a symmetric CSR adjacency (device int32

@@ -88,6 +88,11 @@ SIGNATURES = {
     "mde_knn_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                           C.c_void_p]),
+    "mde_knn_csr_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.POINTER(C.c_size_t)]),
+    "mde_knn_csr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_void_p,
+                              C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_pair_dist_csr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int64,
+                                    C.c_void_p, C.c_void_p]),
     "mde_graph_hops_ws_bytes": (C.c_int64, [C.c_int64]),
     "mde_graph_hops": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_double,
                                  C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,

@@ -1,0 +1,513 @@
+// mde_knn_sparse.cu -- exact k-nearest neighbours and pair distances of the rows of a CSR data matrix (SURVEY
+// section 8 row f3, sparse input).
+//
+// The reference hands a scipy.sparse matrix to pynndescent for the k-NN and to scipy for the distances of sampled
+// pairs (pymde/preprocess/data_matrix.py:59-70).  Densifying costs n d 4 bytes, which a TF-IDF or count matrix
+// cannot afford, so this file works from the CSR arrays alone (int64 indptr, int32 indices strictly increasing within
+// a row, fp32 values):
+//
+//   prep     validate the CSR, ||x||^2 (fp64 sums, fp32; +inf on padding rows) and a column histogram; a permutation
+//            of the features by descending document frequency (CUB radix sort); every row re-sorted under it (one
+//            radix sort on the key (row, new column)); one occupancy bitmap per 128-row tile with one bit per
+//            64-feature K block.  Frequent features land in the first K blocks, so most tiles touch few of the rest.
+//   tiles    one CTA per 128 query rows sweeps every candidate tile, as knn_tile_kernel in mde_knn.cu does.  For a
+//            (query tile, candidate tile) pair only the K blocks set in both bitmaps are visited; a pair with none has
+//            cross terms of exactly 0.  All 256 threads build each 128 x 64 operand block (bf16 hi and lo of both
+//            tiles) straight from CSR: a thread owns one row, zeroes its 128-byte swizzled rows with 16-byte stores
+//            and scatters the row's entries of the block, its cursor advancing monotonically through the visited
+//            blocks.  fence.proxy.async makes these generic-proxy writes visible to wgmma (async proxy); block j's
+//            scatter into one stage overlaps the wgmmas of block j - 1 on the other.  Two consumer warpgroups issue
+//            wgmma.m64n128k16 with Ah Bh^T + Ah Bl^T + Al Bh^T and keep a running top-32 per row, ordered by
+//            (approximate distance, index).
+//   re-rank  sum (q - x)^2 over each candidate by a sorted merge of the two rows, in fp64, rounded once to fp32; the
+//            k smallest by (distance, index).  The result is fully determined, ties included.
+//
+// mde_pair_dist_csr: ||a - b|| of given pairs by the same sorted merge, fp64, sqrt in fp64, one rounding.
+#include <cub/cub.cuh>
+#include <cuda_bf16.h>
+
+#include <climits>
+#include <cstdint>
+
+#include "mde_common.cuh"
+#include "mde_tma.cuh"
+#include "mde_wgmma.cuh"
+
+using namespace mde;
+
+namespace {
+
+constexpr int kTileM = 128;                 // query rows per CTA (two warpgroups of 64)
+constexpr int kTileN = 128;                 // candidates per tile = wgmma N
+constexpr int kBlockK = 64;                 // bf16 elements per 128-byte swizzle row
+constexpr int kWgmmaK = 16;
+constexpr int kStages = 2;
+constexpr int kKK = 32;                     // candidates kept per row before the exact re-rank
+constexpr int kMaxK = 24;
+constexpr int kRowBytes = kBlockK * 2;      // 128
+constexpr int kOpBytes = 128 * kRowBytes;   // 16 KB: one 128-row operand block (hi or lo)
+constexpr int kStageBytes = 4 * kOpBytes;   // A hi, A lo, B hi, B lo = 64 KB
+constexpr int kThreads = 256;               // two warpgroups: each thread builds one operand row, each warpgroup
+                                            // consumes 64 query rows
+constexpr int kChunkWords = 128;            // bitmap words intersected per pass (4096 K blocks)
+constexpr int kAccStride = kTileN + 2;
+constexpr int kSmemBytes = kStages * kStageBytes + 1024 /* alignment slack */ + kTileM * kAccStride * 4 +
+                           kTileN * 4 /* norms */ + kChunkWords * 32 * 4 /* visited-block list */;
+static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
+
+constexpr float kInf = __builtin_huge_valf();
+
+__device__ __forceinline__ bool before(float d1, int i1, float d2, int i2) { return d1 < d2 || (d1 == d2 && i1 < i2); }
+
+// Replace the worst of the KK kept candidates by (dist, col); the new worst is the largest (distance, index).
+__device__ __forceinline__ void keep_candidate(float (&bd)[kKK], int (&bi)[kKK], float dist, int col, float& thr,
+                                               int& thi, int& worst) {
+#pragma unroll
+  for (int q = 0; q < kKK; ++q) {
+    if (q == worst) { bd[q] = dist; bi[q] = col; }
+  }
+  float m = bd[0]; int mi = bi[0], w = 0;
+#pragma unroll
+  for (int q = 1; q < kKK; ++q) {
+    if (before(m, mi, bd[q], bi[q])) { m = bd[q]; mi = bi[q]; w = q; }
+  }
+  thr = m; thi = mi; worst = w;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// prep
+// ---------------------------------------------------------------------------------------------------------------
+// One warp per row: checks the row's CSR (bounds, indices in [0, d), strictly increasing) and sets *bad otherwise;
+// optionally counts each column and writes the fp32-rounded fp64 squared norm.  Padding rows get +inf norms.
+__global__ void __launch_bounds__(256)
+csr_check_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
+                 const float* __restrict__ values, int64_t n, int d, int64_t nnz, int64_t n_pad,
+                 int* __restrict__ bad, int32_t* __restrict__ col_count, float* __restrict__ norms) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= n) {
+    if (norms && row < n_pad && lane == 0) norms[row] = kInf;
+    return;
+  }
+  const int64_t b = indptr[row], e = indptr[row + 1];
+  if (b < 0 || e < b || e > nnz || (row == 0 && b != 0) || (row == n - 1 && e != nnz)) {
+    if (lane == 0) atomicOr(bad, 1);
+    return;
+  }
+  double acc = 0.0;
+  bool ok = true;
+  for (int64_t p = b + lane; p < e; p += 32) {
+    const int c = indices[p];
+    if (c < 0 || c >= d || (p > b && indices[p - 1] >= c)) { ok = false; continue; }
+    if (col_count) atomicAdd(col_count + c, 1);
+    const double x = values[p];
+    acc += x * x;
+  }
+  if (!__all_sync(kFull, ok) && lane == 0) atomicOr(bad, 1);
+  if (norms) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
+    if (lane == 0) norms[row] = (float)acc;
+  }
+}
+
+__global__ void iota_kernel(int32_t* __restrict__ v, int d) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < d) v[i] = i;
+}
+
+__global__ void invert_perm_kernel(const int32_t* __restrict__ col_sorted, int d, int32_t* __restrict__ perm) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < d) perm[col_sorted[i]] = i;
+}
+
+// One warp per row: sort keys (row << col_bits | new column) and the tile occupancy bitmaps.
+__global__ void __launch_bounds__(256)
+csr_keys_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
+                const int32_t* __restrict__ perm, int64_t n, int col_bits, int nwords, uint64_t* __restrict__ keys,
+                uint32_t* __restrict__ bitmap) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= n) return;
+  uint32_t* bm = bitmap + (row / kTileM) * nwords;
+  const int64_t e = indptr[row + 1];
+  for (int64_t p = indptr[row] + lane; p < e; p += 32) {
+    const int c = perm[indices[p]];
+    keys[p] = ((uint64_t)row << col_bits) | (uint32_t)c;
+    const int kb = c / kBlockK;
+    atomicOr(bm + (kb >> 5), 1u << (kb & 31));
+  }
+}
+
+__global__ void key_to_col_kernel(const uint64_t* __restrict__ keys, int64_t nnz, uint64_t mask,
+                                  int32_t* __restrict__ cols) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < nnz) cols[i] = (int32_t)(keys[i] & mask);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// tiles
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kThreads, 1)
+knn_csr_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
+                    const float* __restrict__ vals, const float* __restrict__ norms,
+                    const uint32_t* __restrict__ bitmap, int nwords, int64_t n, int num_tiles,
+                    int32_t* __restrict__ cand_idx, float* __restrict__ cand_val) {
+  extern __shared__ uint8_t smem_raw[];
+  // carve: [stages x 64 KB, 1024-aligned] | staged accumulators [128][kAccStride] | norms[128] | visited blocks
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
+  float* s_acc = reinterpret_cast<float*>(gen + kStages * kStageBytes);
+  float* s_norm = s_acc + kTileM * kAccStride;
+  int* s_list = reinterpret_cast<int*>(s_norm + kTileN);
+  using Scan = cub::BlockScan<int, kThreads>;
+  __shared__ typename Scan::TempStorage scan_tmp;
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int64_t row0 = (int64_t)blockIdx.x * kTileM;
+  const uint32_t* abm = bitmap + (int64_t)blockIdx.x * nwords;
+
+  // ----- builder role: thread tid owns operand row tid & 127 of A (query tile, tid < 128) or B (candidate tile)
+  const bool is_b = tid >= 128;
+  const int orow = tid & 127;
+  const uint32_t my_off = (is_b ? 2 * kOpBytes : 0) + orow * kRowBytes;
+  const int swz = orow & 7;
+  int64_t a_beg = 0, a_end = 0;
+  if (!is_b && row0 + orow < n) { a_beg = indptr[row0 + orow]; a_end = indptr[row0 + orow + 1]; }
+
+  // ----- consumer role: warpgroup wg owns query rows row0 + 64 wg .. + 63
+  const int wg = warp >> 2;
+  const int et = tid & 127;
+  float* acc_s = s_acc + wg * 64 * kAccStride;
+  const int lrow = et >> 1, half = et & 1;
+  const int64_t row = row0 + wg * 64 + lrow;
+  const int frow = 16 * (warp & 3) + (lane >> 2), fcol = 2 * (lane & 3);
+
+  float bd[kKK];
+  int bi[kKK];
+#pragma unroll
+  for (int q = 0; q < kKK; ++q) { bd[q] = kInf; bi[q] = INT_MAX; }
+  float thr = kInf;
+  int thi = INT_MAX, worst = 0;
+  float acc[64];
+
+  int stage = 0;
+  for (int t = 0; t < num_tiles; ++t) {
+    int64_t p = a_beg, end = a_end;
+    if (is_b) {
+      const int64_t r = (int64_t)t * kTileN + orow;
+      p = end = 0;
+      if (r < n) { p = indptr[r]; end = indptr[r + 1]; }
+    }
+    int cur = p < end ? cols[p] : INT_MAX;
+    const uint32_t* bbm = bitmap + (int64_t)t * nwords;
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+
+    for (int w0 = 0; w0 < nwords; w0 += kChunkWords) {
+      __syncthreads();  // every thread is done with s_list (and, on the first chunk, with the last tile's scan)
+      uint32_t m = 0;
+      if (tid < kChunkWords && w0 + tid < nwords) m = __ldg(abm + w0 + tid) & __ldg(bbm + w0 + tid);
+      int pos, total;
+      Scan(scan_tmp).ExclusiveSum(__popc(m), pos, total);
+      for (; m; m &= m - 1) s_list[pos++] = (w0 + tid) * 32 + (__ffs(m) - 1);
+      __syncthreads();
+      for (int i = 0; i < total; ++i) {
+        const int lo = s_list[i] * kBlockK, hi = lo + kBlockK;
+        // the stage was last read by the wgmmas of block i - 2, which every warpgroup waited for before the
+        // barrier of block i - 1
+        uint8_t* rh = gen + stage * kStageBytes + my_off;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+          reinterpret_cast<uint4*>(rh)[c] = make_uint4(0, 0, 0, 0);
+          reinterpret_cast<uint4*>(rh + kOpBytes)[c] = make_uint4(0, 0, 0, 0);
+        }
+        while (cur < hi) {
+          if (cur >= lo) {
+            const float x = vals[p];
+            const __nv_bfloat16 h = __float2bfloat16_rn(x);
+            const __nv_bfloat16 l = __float2bfloat16_rn(x - __bfloat162float(h));
+            const int k = cur - lo;
+            const int off = (((k >> 3) ^ swz) << 4) | ((k & 7) << 1);
+            *reinterpret_cast<__nv_bfloat16*>(rh + off) = h;
+            *reinterpret_cast<__nv_bfloat16*>(rh + kOpBytes + off) = l;
+          }
+          ++p;
+          cur = p < end ? cols[p] : INT_MAX;
+        }
+        fence_proxy_async();  // generic-proxy stores above, read next by wgmma (async proxy)
+        wgmma_wait_all();     // this warpgroup's wgmmas of block i - 1 are done with the other stage
+        __syncthreads();
+        const uint32_t sa = base + stage * kStageBytes;
+        const uint64_t ah = smem_desc_sw128(sa + wg * 64 * kRowBytes);
+        const uint64_t al = smem_desc_sw128(sa + kOpBytes + wg * 64 * kRowBytes);
+        const uint64_t bh = smem_desc_sw128(sa + 2 * kOpBytes), bl = smem_desc_sw128(sa + 3 * kOpBytes);
+#pragma unroll
+        for (int q = 0; q < 64; ++q) fence_operand(acc[q]);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
+          const uint64_t adv = (uint64_t)((k * kWgmmaK * 2) >> 4);
+          wgmma_bf16(acc, ah + adv, bh + adv, 1u);
+          wgmma_bf16(acc, ah + adv, bl + adv, 1u);
+          wgmma_bf16(acc, al + adv, bh + adv, 1u);
+        }
+        wgmma_commit();
+        stage ^= 1;
+      }
+    }
+    wgmma_wait_all();
+#pragma unroll
+    for (int q = 0; q < 64; ++q) fence_operand(acc[q]);
+#pragma unroll
+    for (int j = 0; j < kTileN / 8; ++j) {
+      *reinterpret_cast<float2*>(acc_s + frow * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(acc_s + (frow + 8) * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+    if (tid < kTileN) s_norm[tid] = __ldg(norms + (int64_t)t * kTileN + tid);
+    __syncthreads();
+    const float* arow = acc_s + lrow * kAccStride;
+#pragma unroll 4
+    for (int i = 0; i < kTileN / 2; ++i) {
+      const int c = 2 * i + half;
+      const float dist = fmaf(-2.0f, arow[c], s_norm[c]);
+      const int col = t * kTileN + c;
+      if (before(dist, col, thr, thi) && col != row && col < n) keep_candidate(bd, bi, dist, col, thr, thi, worst);
+    }
+  }
+  // merge the two half-row lists: the odd-column thread hands its list to the even-column thread
+  __syncthreads();
+  float* xd = acc_s + lrow * kAccStride;
+  int* xi = reinterpret_cast<int*>(xd + kKK);
+  if (half) {
+#pragma unroll
+    for (int q = 0; q < kKK; ++q) { xd[q] = bd[q]; xi[q] = bi[q]; }
+  }
+  __syncthreads();
+  if (!half) {
+    for (int q = 0; q < kKK; ++q) {
+      if (before(xd[q], xi[q], thr, thi)) keep_candidate(bd, bi, xd[q], xi[q], thr, thi, worst);
+    }
+    if (row < n) {
+#pragma unroll
+      for (int q = 0; q < kKK; ++q) {
+        cand_idx[row * kKK + q] = bi[q] == INT_MAX ? -1 : bi[q];
+        cand_val[row * kKK + q] = bd[q];
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// exact distances: sorted merge of two CSR rows, fp64
+// ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ double merge_dist2(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
+                                              const float* __restrict__ vals, int64_t a, int64_t b) {
+  int64_t p = indptr[a], q = indptr[b];
+  const int64_t pe = indptr[a + 1], qe = indptr[b + 1];
+  double acc = 0.0;
+  while (p < pe && q < qe) {
+    const int cp = cols[p], cq = cols[q];
+    double t;
+    if (cp == cq) { t = (double)vals[p] - (double)vals[q]; ++p; ++q; }
+    else if (cp < cq) { t = vals[p]; ++p; }
+    else { t = vals[q]; ++q; }
+    acc = fma(t, t, acc);
+  }
+  for (; p < pe; ++p) { const double t = vals[p]; acc = fma(t, t, acc); }
+  for (; q < qe; ++q) { const double t = vals[q]; acc = fma(t, t, acc); }
+  return acc;
+}
+
+// One warp per row, lane q re-ranks candidate q; the k smallest (distance, index) in ascending order.
+__global__ void __launch_bounds__(256)
+knn_csr_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
+                      const float* __restrict__ vals, int64_t n, const int32_t* __restrict__ cand_idx, int k,
+                      int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= n) return;
+  const int c = cand_idx[row * kKK + lane];
+  const float my_d = c >= 0 ? (float)merge_dist2(indptr, cols, vals, row, c) : kInf;
+  const int mine = c >= 0 ? c : INT_MAX;  // missing candidates last
+  int rank = 0;
+  for (int q = 0; q < kKK; ++q) {
+    const float od = __shfl_sync(kFull, my_d, q);
+    const int oi = __shfl_sync(kFull, mine, q);
+    if (before(od, oi, my_d, mine)) ++rank;
+  }
+  if (rank < k) {
+    out_idx[row * k + rank] = mine;
+    out_d2[row * k + rank] = my_d;
+  }
+}
+
+// One thread per pair (the rows of a pair are walked in column order: the same fp64 sum every run).
+__global__ void __launch_bounds__(256)
+pair_dist_csr_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
+                     const float* __restrict__ vals, int64_t n, const int64_t* __restrict__ pairs, int64_t p,
+                     float* __restrict__ out, int* __restrict__ bad) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= p) return;
+  const int64_t a = pairs[2 * i], b = pairs[2 * i + 1];
+  if (a < 0 || a >= n || b < 0 || b >= n) { atomicOr(bad, 1); return; }
+  out[i] = (float)sqrt(merge_dist2(indptr, cols, vals, a, b));
+}
+
+int bits_for(uint64_t count) {  // bits needed to hold 0 .. count - 1
+  int b = 0;
+  while (b < 64 && (1ull << b) < count) ++b;
+  return b;
+}
+
+struct CsrKnnLayout {
+  int64_t n_pad; int num_tiles, nwords, row_bits, col_bits;
+  size_t off_flag, off_norm, off_ci, off_cv, off_cnt, off_cnt_s, off_iota, off_col_s, off_perm, off_bm, off_kin,
+      off_kout, off_val, off_tmp, tmp_bytes, total;
+};
+
+int csr_knn_layout(int64_t n, int d, int64_t nnz, CsrKnnLayout* L) {
+  L->n_pad = (n + kTileN - 1) / kTileN * kTileN;
+  L->num_tiles = (int)(L->n_pad / kTileN);
+  const int64_t nkb = ((int64_t)d + kBlockK - 1) / kBlockK;
+  L->nwords = (int)((nkb + 31) / 32);
+  L->row_bits = bits_for((uint64_t)n);
+  L->col_bits = bits_for((uint64_t)d);
+  // CUB scratch of the two sorts (a query: no device work)
+  size_t t1 = 0, t2 = 0;
+  MDE_CUDA_TRY(cub::DeviceRadixSort::SortPairsDescending(nullptr, t1, (const int32_t*)nullptr, (int32_t*)nullptr,
+                                                         (const int32_t*)nullptr, (int32_t*)nullptr, d));
+  MDE_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t2, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                                               (const float*)nullptr, (float*)nullptr, (int64_t)nnz, 0,
+                                               L->row_bits + L->col_bits));
+  L->tmp_bytes = t1 > t2 ? t1 : t2;
+  auto up = [](size_t x) { return (x + 1023) / 1024 * 1024; };
+  size_t o = 0;
+  L->off_flag = o; o = up(o + 4);
+  L->off_norm = o; o = up(o + (size_t)L->n_pad * 4);
+  L->off_ci = o; o = up(o + (size_t)n * kKK * 4);
+  L->off_cv = o; o = up(o + (size_t)n * kKK * 4);
+  L->off_cnt = o; o = up(o + (size_t)d * 4);
+  L->off_cnt_s = o; o = up(o + (size_t)d * 4);
+  L->off_iota = o; o = up(o + (size_t)d * 4);
+  L->off_col_s = o; o = up(o + (size_t)d * 4);
+  L->off_perm = o; o = up(o + (size_t)d * 4);
+  L->off_bm = o; o = up(o + (size_t)L->num_tiles * L->nwords * 4);
+  L->off_kin = o; o = up(o + (size_t)nnz * 8);  // after the sort: the re-sorted column indices (int32)
+  L->off_kout = o; o = up(o + (size_t)nnz * 8);
+  L->off_val = o; o = up(o + (size_t)nnz * 4);
+  L->off_tmp = o; o = up(o + L->tmp_bytes);
+  L->total = o;
+  return 0;
+}
+
+// Runs csr_check_kernel and reads the verdict back (blocking).
+int check_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
+              int64_t n_pad, int* flag_dev, int32_t* col_count, float* norms, cudaStream_t st) {
+  MDE_CUDA_TRY(cudaMemsetAsync(flag_dev, 0, sizeof(int), st));
+  csr_check_kernel<<<(unsigned)((n_pad + 7) / 8), 256, 0, st>>>(indptr, indices, values, n, d, nnz, n_pad, flag_dev,
+                                                              col_count, norms);
+  MDE_LAUNCH_CHECK();
+  int flag = 0;
+  MDE_CUDA_TRY(cudaMemcpyAsync(&flag, flag_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
+  MDE_CUDA_TRY(cudaStreamSynchronize(st));
+  return flag ? MDE_E_INVALID : 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mde_knn_csr_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes) {
+  if (!bytes || n < 2 || d < 1 || nnz < 0) return MDE_E_INVALID;
+  CsrKnnLayout L;
+  int rc = csr_knn_layout(n, d, nnz, &L);
+  if (rc) return rc;
+  *bytes = L.total;
+  return 0;
+}
+
+int mde_knn_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
+                int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream) {
+  if (!indptr || !idx_out || !d2_out || !ws || n < 2 || d < 1 || nnz < 0 || k < 1 || k > kMaxK || k > n - 1)
+    return MDE_E_INVALID;
+  if (nnz > 0 && (!indices || !values)) return MDE_E_INVALID;
+  if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
+  CsrKnnLayout L;
+  int rc = csr_knn_layout(n, d, nnz, &L);
+  if (rc) return rc;
+  if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* w = static_cast<uint8_t*>(ws);
+  int* flag = reinterpret_cast<int*>(w + L.off_flag);
+  float* norms = reinterpret_cast<float*>(w + L.off_norm);
+  int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
+  float* cv = reinterpret_cast<float*>(w + L.off_cv);
+  int32_t* cnt = reinterpret_cast<int32_t*>(w + L.off_cnt);
+  int32_t* cnt_s = reinterpret_cast<int32_t*>(w + L.off_cnt_s);
+  int32_t* iota = reinterpret_cast<int32_t*>(w + L.off_iota);
+  int32_t* col_s = reinterpret_cast<int32_t*>(w + L.off_col_s);
+  int32_t* perm = reinterpret_cast<int32_t*>(w + L.off_perm);
+  uint32_t* bm = reinterpret_cast<uint32_t*>(w + L.off_bm);
+  uint64_t* kin = reinterpret_cast<uint64_t*>(w + L.off_kin);
+  uint64_t* kout = reinterpret_cast<uint64_t*>(w + L.off_kout);
+  int32_t* cols = reinterpret_cast<int32_t*>(w + L.off_kin);
+  float* vals = reinterpret_cast<float*>(w + L.off_val);
+  void* tmp = w + L.off_tmp;
+  size_t tmp_bytes = L.tmp_bytes;
+
+  MDE_CUDA_TRY(cudaMemsetAsync(cnt, 0, (size_t)d * 4, st));
+  if ((rc = check_csr(indptr, indices, values, n, d, nnz, L.n_pad, flag, cnt, norms, st))) return rc;
+  // features by descending document frequency (stable: equal counts keep column order)
+  iota_kernel<<<(d + 255) / 256, 256, 0, st>>>(iota, d);
+  MDE_LAUNCH_CHECK();
+  MDE_CUDA_TRY(cub::DeviceRadixSort::SortPairsDescending(tmp, tmp_bytes, cnt, cnt_s, iota, col_s, d, 0, 32, st));
+  invert_perm_kernel<<<(d + 255) / 256, 256, 0, st>>>(col_s, d, perm);
+  MDE_LAUNCH_CHECK();
+  MDE_CUDA_TRY(cudaMemsetAsync(bm, 0, (size_t)L.num_tiles * L.nwords * 4, st));
+  if (nnz > 0) {
+    csr_keys_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(indptr, indices, perm, n, L.col_bits, L.nwords, kin, bm);
+    MDE_LAUNCH_CHECK();
+    tmp_bytes = L.tmp_bytes;
+    MDE_CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, kin, kout, values, vals, (int64_t)nnz, 0,
+                                                 L.row_bits + L.col_bits, st));
+    key_to_col_kernel<<<(unsigned)((nnz + 255) / 256), 256, 0, st>>>(kout, nnz, (1ull << L.col_bits) - 1, cols);
+    MDE_LAUNCH_CHECK();
+  }
+  static bool attr_set = false;
+  if (!attr_set) {
+    MDE_CUDA_TRY(cudaFuncSetAttribute(knn_csr_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+    attr_set = true;
+  }
+  knn_csr_tile_kernel<<<(unsigned)L.num_tiles, kThreads, kSmemBytes, st>>>(indptr, cols, vals, norms, bm, L.nwords, n,
+                                                                           L.num_tiles, ci, cv);
+  MDE_LAUNCH_CHECK();
+  knn_csr_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(indptr, cols, vals, n, ci, k, idx_out, d2_out);
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+
+int mde_pair_dist_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                      const int64_t* pairs, int64_t p, float* out, void* stream) {
+  if (!indptr || n < 1 || d < 1 || p < 0 || (p > 0 && (!pairs || !out))) return MDE_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  int64_t nnz = 0;
+  MDE_CUDA_TRY(cudaMemcpyAsync(&nnz, indptr + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  MDE_CUDA_TRY(cudaStreamSynchronize(st));
+  if (nnz < 0 || (nnz > 0 && (!indices || !values))) return MDE_E_INVALID;
+  int* flag = nullptr;
+  MDE_CUDA_TRY(cudaMallocAsync(reinterpret_cast<void**>(&flag), sizeof(int), st));
+  int rc = check_csr(indptr, indices, values, n, d, nnz, n, flag, nullptr, nullptr, st);
+  if (!rc && p > 0) {
+    pair_dist_csr_kernel<<<(unsigned)((p + 255) / 256), 256, 0, st>>>(indptr, indices, values, n, pairs, p, out, flag);
+    MDE_LAUNCH_CHECK();
+    int bad = 0;
+    MDE_CUDA_TRY(cudaMemcpyAsync(&bad, flag, sizeof(int), cudaMemcpyDeviceToHost, st));
+    MDE_CUDA_TRY(cudaStreamSynchronize(st));
+    if (bad) rc = MDE_E_INVALID;
+  }
+  MDE_CUDA_TRY(cudaFreeAsync(flag, st));
+  return rc;
+}
+
+}  // extern "C"

@@ -3,7 +3,8 @@
 k-nearest neighbours are computed EXACTLY on the GPU by the library's own kernel (`mde_knn`: wgmma tensor-core
 cross terms with a running top-32 per row and an exact fp32 re-rank, csrc/mde_knn.cu) for k <= 24; larger k uses row
 chunks of a library GEMM + top-k.  The reference uses scikit-learn brute force below 10 000 rows and the approximate
-pynndescent above (data_matrix.py:125-143)."""
+pynndescent above (data_matrix.py:125-143).  A scipy.sparse matrix is searched without densifying it (`mde_knn_csr`,
+csrc/mde_knn_sparse.cu), and its pair distances come from sorted merges of CSR rows (`mde_pair_dist_csr`)."""
 import ctypes as C
 import os
 
@@ -22,6 +23,63 @@ def _to_device_matrix(data, device):
     if isinstance(data, np.ndarray):
         data = torch.from_numpy(np.ascontiguousarray(data))
     return data.to(device=device, dtype=torch.float32)
+
+
+def _to_device_csr(data, device):
+    """Canonical CSR of a scipy.sparse matrix on `device`: (indptr int64 [n+1], indices int32 [nnz], values fp32
+    [nnz], (n, d)), with duplicates summed and the indices of every row sorted, uploaded once."""
+    A = sp.csr_matrix(data, copy=True)
+    A.sum_duplicates()  # also sorts the indices of every row
+    indptr = torch.from_numpy(A.indptr.astype(np.int64))
+    indices = torch.from_numpy(A.indices.astype(np.int32))
+    values = torch.from_numpy(A.data.astype(np.float32))
+    return (indptr.to(device), indices.to(device), values.to(device)), A.shape
+
+
+def knn_sparse_device(csr, shape, k):
+    """(indices [n, k] int32, squared distances [n, k] fp32) of the k nearest rows of every row of a device CSR
+    matrix from `_to_device_csr`, ascending by (distance, index); the kernel behind `mde_knn_csr`
+    (include/mde_b200.h)."""
+    from .. import _lib
+    lib = _lib.load()
+    indptr, indices, values = csr
+    n, d = shape
+    nnz = int(indices.shape[0])
+    dev = indptr.device
+    need = C.c_size_t(0)
+    _lib.check(lib.mde_knn_csr_ws_bytes(int(n), int(d), nnz, C.byref(need)))
+    ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=dev)
+    off = (-ws.data_ptr()) % 1024
+    idx = torch.empty((n, k), dtype=torch.int32, device=dev)
+    d2 = torch.empty((n, k), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream().cuda_stream
+        _lib.check(lib.mde_knn_csr(indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), int(n), int(d), nnz,
+                                   int(k), idx.data_ptr(), d2.data_ptr(), ws.data_ptr() + off, need.value, stream))
+        torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
+    return idx, d2
+
+
+def _pair_dist_csr(csr, shape, pairs):
+    """||x_a - x_b|| (fp32, fp64 sums) of the device int64 row pairs [p, 2] of a device CSR matrix."""
+    from .. import _lib
+    lib = _lib.load()
+    indptr, indices, values = csr
+    pairs = pairs.to(dtype=torch.int64).contiguous()
+    out = torch.empty(pairs.shape[0], dtype=torch.float32, device=pairs.device)
+    with torch.cuda.device(pairs.device):
+        stream = torch.cuda.current_stream().cuda_stream
+        _lib.check(lib.mde_pair_dist_csr(indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), int(shape[0]),
+                                         int(shape[1]), pairs.data_ptr(), int(pairs.shape[0]), out.data_ptr(),
+                                         stream))
+    return out
+
+
+def _knn_graph(idx, d2, n, max_distance, dev):
+    keep = torch.ones_like(d2, dtype=torch.bool) if max_distance is None else d2.sqrt() <= max_distance
+    i = torch.arange(n, device=dev)[:, None].expand_as(idx)
+    e = torch.stack([i[keep], idx[keep].long()], 1).cpu()
+    return Graph.from_edges(e, None, n_items=n)
 
 
 def knn_device(X, k):
@@ -48,17 +106,21 @@ def knn_device(X, k):
 def k_nearest_neighbors(data, k, max_distance=None, verbose=False, device=None, chunk_rows=None):
     """Graph whose edges join each row to its k nearest rows (Euclidean); reciprocal pairs get weight 2."""
     dev = util.cuda_device(device)
+    from .. import _lib
+    use_kernel = chunk_rows is None and os.environ.get("PYMDE_B200_KNN", "kernel") != "gemm"
+    if sp.issparse(data):
+        n = data.shape[0]
+        k = int(min(k, n - 1))
+        if use_kernel and 1 <= k <= _lib.load().mde_knn_max_k():
+            csr, shape = _to_device_csr(data, dev)
+            idx, d2 = knn_sparse_device(csr, shape, k)
+            return _knn_graph(idx, d2, n, max_distance, dev)
     X = _to_device_matrix(data, dev)
     n = X.shape[0]
     k = int(min(k, n - 1))
-    from .. import _lib
-    if (chunk_rows is None and 1 <= k <= _lib.load().mde_knn_max_k()
-            and os.environ.get("PYMDE_B200_KNN", "kernel") != "gemm"):
+    if use_kernel and 1 <= k <= _lib.load().mde_knn_max_k():
         idx, d2 = knn_device(X, k)
-        keep = torch.ones_like(d2, dtype=torch.bool) if max_distance is None else d2.sqrt() <= max_distance
-        i = torch.arange(n, device=dev)[:, None].expand_as(idx)
-        e = torch.stack([i[keep], idx[keep].long()], 1).cpu()
-        return Graph.from_edges(e, None, n_items=n)
+        return _knn_graph(idx, d2, n, max_distance, dev)
     sq = (X * X).sum(1)
     rows = chunk_rows or max(256, min(n, int(2 ** 27 // max(n, 1))))
     src, dst = [], []
@@ -77,13 +139,19 @@ def k_nearest_neighbors(data, k, max_distance=None, verbose=False, device=None, 
 def distances(data, retain_fraction=1.0, verbose=False, device=None):
     """Graph of pairwise Euclidean distances: all (n choose 2) pairs, or a uniform sample of them."""
     dev = util.cuda_device(device)
-    X = _to_device_matrix(data, dev)
-    n = X.shape[0]
+    if sp.issparse(data):
+        csr, shape = _to_device_csr(data, dev)
+        n = shape[0]
+    else:
+        X = _to_device_matrix(data, dev)
+        n = X.shape[0]
     n_all = n * (n - 1) // 2
     if retain_fraction >= 1.0:
         edges = torch.triu_indices(n, n, 1, device=dev).T
     else:
         edges = sample_edges(n, int(retain_fraction * n_all), device=dev)
+    if sp.issparse(data):
+        return Graph.from_edges(edges.cpu(), _pair_dist_csr(csr, shape, edges).cpu(), n_items=n)
     out = torch.empty(edges.shape[0], dtype=torch.float32, device=dev)
     step = 1 << 22
     for s0 in range(0, edges.shape[0], step):
