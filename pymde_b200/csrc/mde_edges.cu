@@ -590,37 +590,31 @@ int loss_blocks_small(int64_t p) {
   return (int)nb;
 }
 
-int quad_nq() {  // consecutive quads per thread: MDE_B200_NQ=1|2 (experimental A/B switch; default 1)
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("MDE_B200_NQ"); v = (e && e[0] == '2') ? 2 : 1; }
-  return v;
+// A/B switches for measurements, read when a layout is created (mde_edges::kvar / nq / qbps):
+//   MDE_B200_KERNEL=strided   the lane-strided kernel with the warp segmented reduction (sorted SoA)
+//   MDE_B200_KERNEL=precise   the thread-contiguous / tile kernels with IEEE math instead of the MUFU forms
+//   MDE_B200_NQ=2             two consecutive quads per thread in the FAST quad kernel (default 1)
+//   MDE_B200_QUAD_BPS=k       blocks per SM in the quad kernel's grid cap (default 4 = one resident wave)
+static void read_kernel_switches(mde_edges* e) {
+  const char* ev = getenv("MDE_B200_KERNEL");
+  e->kvar = 0;
+  if (ev && !strcmp(ev, "strided")) e->kvar = 1;
+  if (ev && !strcmp(ev, "precise")) e->kvar = 2;
+  ev = getenv("MDE_B200_NQ");
+  e->nq = (ev && ev[0] == '2') ? 2 : 1;
+  ev = getenv("MDE_B200_QUAD_BPS");
+  int v = ev ? atoi(ev) : 4;
+  if (v < 1) v = 1;
+  if (v > 16) v = 16;
+  e->qbps = v;
 }
 
-int quad_grid_cap() {  // blocks per SM in the grid cap: MDE_B200_QUAD_BPS (default 4 = one resident wave)
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("MDE_B200_QUAD_BPS"); v = e ? atoi(e) : 4; if (v < 1) v = 1; if (v > 16) v = 16; }
-  return v;
-}
-
-int loss_blocks_quad(int64_t p, int nq) {
+int loss_blocks_quad(int64_t p, int nq, int bps) {
   int64_t per_block = (int64_t)kQuadThreads * 4 * nq;
   int64_t nb = (p + per_block - 1) / per_block;
   if (nb < 1) nb = 1;
-  if (nb > kNumSMs * quad_grid_cap()) nb = kNumSMs * quad_grid_cap();
+  if (nb > kNumSMs * bps) nb = kNumSMs * bps;
   return (int)nb;
-}
-
-// A/B switch for measurements: MDE_B200_KERNEL=strided selects the lane-strided kernel with the warp
-// segmented reduction; MDE_B200_KERNEL=precise keeps the thread-contiguous kernel but IEEE math.
-int small_kernel_variant() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MDE_B200_KERNEL");
-    v = 0;
-    if (e && !strcmp(e, "strided")) v = 1;
-    if (e && !strcmp(e, "precise")) v = 2;
-  }
-  return v;
 }
 
 int loss_blocks_wide(int64_t p, int G) {
@@ -640,7 +634,7 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
   int nb;
   // deterministic mode (m <= 4, sorted-SoA layout): zero the fixed-point buffer, accumulate into it, add it to grad
   long long* fxp = nullptr;
-  if (e->det && MODE != 1 && m <= 4 && m <= e->m_hint && small_kernel_variant() != 1) {
+  if (e->det && MODE != 1 && m <= 4 && m <= e->m_hint && e->kvar != 1) {
     fxp = e->fx;
     const int64_t cnt = e->n * m;
     int zb = (int)((cnt + 255) / 256); if (zb > kNumSMs * 8) zb = kNumSMs * 8;
@@ -648,7 +642,7 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
     ++g_launch_count;
   }
   // default on the sorted-SoA layout: per-edge contributions + fixed-order per-node gather (quad kernel only)
-  float* cbp = (!fxp && e->cb && MODE != 1 && m == e->m_hint && small_kernel_variant() != 1) ? e->cb : nullptr;
+  float* cbp = (!fxp && e->cb && MODE != 1 && m == e->m_hint && e->kvar != 1) ? e->cb : nullptr;
 #define SMALLK(MM, FA, FR)                                                                            \
   distortion_small_kernel<MM, MODE, FA, FR><<<nb, kSmallThreads, 0, st>>>(                            \
       e->src, e->dst, e->par0, e->has_par1 ? e->par1 : nullptr, e->perm, gext, p, X, grad,           \
@@ -659,14 +653,14 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
       e->src, e->dst, e->par0, e->has_par1 ? e->par1 : nullptr, e->perm, gext, p, X, grad,           \
       e->loss_partials, e->fn, inv_p, flag, fxp, cbp)
 #define QUADK(MM, FA, FR, FAST)                                                                       \
-  if (FAST && quad_nq() == 2) { nb = loss_blocks_quad(p, 2); QUADK_(MM, FA, FR, FAST, 2); }           \
-  else { nb = loss_blocks_quad(p, 1); QUADK_(MM, FA, FR, FAST, 1); }
+  if (FAST && e->nq == 2) { nb = loss_blocks_quad(p, 2, e->qbps); QUADK_(MM, FA, FR, FAST, 2); }       \
+  else { nb = loss_blocks_quad(p, 1, e->qbps); QUADK_(MM, FA, FR, FAST, 1); }
 #define SMALL(MM)                                                                                     \
-  if (small_kernel_variant() != 1) {                                                                  \
-    nb = loss_blocks_quad(p, 1);                                                                      \
+  if (e->kvar != 1) {                                                                                 \
+    nb = loss_blocks_quad(p, 1, e->qbps);                                                             \
     const int fa = e->fn.fn_att, fr = e->fn.fn_rep, pp = e->fn.push_pull;                             \
     const bool hot = pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG && e->fn.a0 == 1.5f &&          \
-                     e->fn.r0 == 1.0f && small_kernel_variant() == 0;                                 \
+                     e->fn.r0 == 1.0f && e->kvar == 0;                                                \
     if constexpr (MODE == 0 && (MM == 2 || MM == 3)) {                                                \
       if (hot) { QUADK(MM, MDE_FN_P_LOG1P, MDE_FN_P_LOG, true); }                                     \
       else if (pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG) { QUADK(MM, MDE_FN_P_LOG1P, MDE_FN_P_LOG, false); } \
@@ -814,6 +808,7 @@ int mde_edges_create_ex(mde_edges_t** out, const int64_t* edges, int64_t p, int6
   mde_edges* e = new (std::nothrow) mde_edges();
   if (!e) return MDE_E_ALLOC;
   e->p = p; e->n = n_items; e->p_total = p_total; e->fn = to_dev(*fn); e->has_par1 = par1 != nullptr;
+  read_kernel_switches(e);
 
   uint64_t *keys_in = nullptr, *keys_out = nullptr;
   int32_t *vals_in = nullptr, *vals_out = nullptr;

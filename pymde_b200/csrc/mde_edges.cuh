@@ -37,6 +37,10 @@ struct mde_edges {
   mde::FnDev fn;
   int has_par1 = 0;
   int64_t nbytes = 0;
+  // kernel switches, resolved once when the layout is created (layouts built with different settings coexist):
+  int kvar = 0;              // MDE_B200_KERNEL: 0 default, 1 strided (sorted SoA), 2 precise (no MUFU math)
+  int nq = 1;                // MDE_B200_NQ: consecutive quads per thread of the FAST quad kernel (1 or 2)
+  int qbps = 4;              // MDE_B200_QUAD_BPS: blocks per SM in the quad kernel's grid cap (1..16)
   int det = 0;               // deterministic mode: gradient contributions accumulate in 64-bit fixed point
   long long* fx = nullptr;   // [n * m_hint] fixed-point accumulator (det only)
   // sorted-SoA layout, m_hint <= 4: the quad kernel stores every edge's contribution in `cb` (no atomics) and

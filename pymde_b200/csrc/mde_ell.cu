@@ -558,12 +558,10 @@ size_t ell_smem_bytes(int rb, int m) {
 }
 
 template <int M>
-const void* eselect_m(const FnDev& fn) {
+const void* eselect_m(const FnDev& fn, bool precise) {
   const int fa = fn.fn_att, fr = fn.fn_rep, pp = fn.push_pull;
 #define EK(FA, FR, FAST) reinterpret_cast<const void*>(&distortion_ell_kernel<M, FA, FR, FAST>)
   if constexpr (M == 2 || M == 3) {
-    const char* ev = getenv("MDE_B200_KERNEL");
-    const bool precise = ev && !strcmp(ev, "precise");
     const bool hot = pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG && fn.a0 == 1.5f && fn.r0 == 1.0f && !precise;
     if (hot) return EK(MDE_FN_P_LOG1P, MDE_FN_P_LOG, true);
     if (pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG) return EK(MDE_FN_P_LOG1P, MDE_FN_P_LOG, false);
@@ -574,12 +572,14 @@ const void* eselect_m(const FnDev& fn) {
   return EK(-1, -1, false);
 #undef EK
 }
-const void* eselect_kernel(const FnDev& fn, int m) {
+// `precise`: mde_edges::kvar == 2 (MDE_B200_KERNEL=precise, read when the layout was created)
+const void* eselect_kernel(const mde_edges* e, int m) {
+  const bool precise = e->kvar == 2;
   switch (m) {
-    case 1: return eselect_m<1>(fn);
-    case 2: return eselect_m<2>(fn);
-    case 3: return eselect_m<3>(fn);
-    case 4: return eselect_m<4>(fn);
+    case 1: return eselect_m<1>(e->fn, precise);
+    case 2: return eselect_m<2>(e->fn, precise);
+    case 3: return eselect_m<3>(e->fn, precise);
+    case 4: return eselect_m<4>(e->fn, precise);
   }
   return nullptr;
 }
@@ -824,7 +824,7 @@ int ell_build(mde_edges* e, const mde_fn_t* fn, int m, cudaStream_t st) {
   const int64_t p = e->p, n = e->n;
   int rc = ell_check_shape(n, p, m, rb);
   if (rc) return rc;
-  const void* k = eselect_kernel(e->fn, m);
+  const void* k = eselect_kernel(e, m);
   if (!k) return MDE_E_UNSUPPORTED;
   if ((rc = econfigure_kernel(k))) return rc;
   const char* bev = getenv("MDE_B200_ELL_BUILD");
@@ -885,7 +885,7 @@ int ell_launch(const mde_edges* e, const float* X, int m, float* grad, int* nblo
   a.loss_partials = e->loss_partials; a.flag = flag; a.fn = e->fn; a.inv_p = 1.0f / (float)e->p_total;
   a.n = e->n; a.rb = e->rb;
   a.x_vec_ok = ((reinterpret_cast<uintptr_t>(X) & 15u) == 0) ? 1 : 0;
-  const void* k = eselect_kernel(e->fn, m);
+  const void* k = eselect_kernel(e, m);
   if (!k) return MDE_E_UNSUPPORTED;
   int rc = econfigure_kernel(k);
   if (rc) return rc;

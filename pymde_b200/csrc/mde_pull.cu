@@ -471,11 +471,9 @@ const void* pkptr(int epl) {
 }
 
 template <int M, int MODE>
-const void* pselect_m(const FnDev& fn, int epl) {
+const void* pselect_m(const FnDev& fn, int epl, bool precise) {
   const int fa = fn.fn_att, fr = fn.fn_rep, pp = fn.push_pull;
   if constexpr (MODE == 0 && (M == 2 || M == 3)) {
-    const char* ev = getenv("MDE_B200_KERNEL");
-    const bool precise = ev && !strcmp(ev, "precise");
     const bool hot = pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG && fn.a0 == 1.5f && fn.r0 == 1.0f && !precise;
     if (hot) return pkptr<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOG, true>(epl);
     if (pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG) return pkptr<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOG, false>(epl);
@@ -488,19 +486,21 @@ const void* pselect_m(const FnDev& fn, int epl) {
   return pkptr<M, MODE, -1, -1, false>(epl);
 }
 template <int MODE>
-const void* pselect_mode(const FnDev& fn, int m, int epl) {
+const void* pselect_mode(const FnDev& fn, int m, int epl, bool precise) {
   switch (m) {
-    case 1: return pselect_m<1, MODE>(fn, epl);
-    case 2: return pselect_m<2, MODE>(fn, epl);
-    case 3: return pselect_m<3, MODE>(fn, epl);
-    case 4: return pselect_m<4, MODE>(fn, epl);
+    case 1: return pselect_m<1, MODE>(fn, epl, precise);
+    case 2: return pselect_m<2, MODE>(fn, epl, precise);
+    case 3: return pselect_m<3, MODE>(fn, epl, precise);
+    case 4: return pselect_m<4, MODE>(fn, epl, precise);
   }
   return nullptr;
 }
-const void* pselect_kernel(const FnDev& fn, int m, int mode, int epl) {
-  if (mode == 0) return pselect_mode<0>(fn, m, epl);
-  if (mode == 1) return pselect_mode<1>(fn, m, epl);
-  return pselect_mode<2>(fn, m, epl);
+// `precise`: mde_edges::kvar == 2 (MDE_B200_KERNEL=precise, read when the layout was created)
+const void* pselect_kernel(const mde_edges* e, int m, int mode, int epl) {
+  const bool precise = e->kvar == 2;
+  if (mode == 0) return pselect_mode<0>(e->fn, m, epl, precise);
+  if (mode == 1) return pselect_mode<1>(e->fn, m, epl, precise);
+  return pselect_mode<2>(e->fn, m, epl, precise);
 }
 int pconfigure_kernel(const void* k) {
   static std::vector<const void*> done;
@@ -684,7 +684,7 @@ int pull_build(mde_edges* e, const int64_t* edges, const float* par0, const mde_
     if (bad) { rc = MDE_E_UNSUPPORTED; goto done; }  // a warp-tile spans more than 65 536 owner rows (very sparse)
     e->fn = to_dev(*fn);
     for (int mode = 0; mode < 3; ++mode) {
-      const void* k = pselect_kernel(e->fn, m, mode, epl);
+      const void* k = pselect_kernel(e, m, mode, epl);
       if (!k) { rc = MDE_E_UNSUPPORTED; goto done; }
       if ((rc = pconfigure_kernel(k))) goto done;
     }
@@ -716,7 +716,7 @@ int pull_launch(int mode, const mde_edges* e, const float* X, int m, float* grad
   a.cta_wt0 = e->cta_wt0; a.cta_bkt0 = e->cta_bkt0; a.X = X; a.grad = grad; a.loss_partials = e->loss_partials;
   a.flag = flag; a.fn = e->fn; a.inv_p = 1.0f / (float)e->p_total; a.n = e->n; a.rb = e->rb;
   a.x_vec_ok = ((reinterpret_cast<uintptr_t>(X) & 15u) == 0) ? 1 : 0;
-  const void* k = pselect_kernel(e->fn, m, mode, e->epl);
+  const void* k = pselect_kernel(e, m, mode, e->epl);
   if (!k) return MDE_E_UNSUPPORTED;
   int rc = pconfigure_kernel(k);
   if (rc) return rc;

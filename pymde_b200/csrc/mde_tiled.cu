@@ -639,13 +639,12 @@ done:
 template <int M, int MODE, int FA, int FR, bool FAST>
 static const void* kptr() { return reinterpret_cast<const void*>(&distortion_tile_kernel<M, MODE, FA, FR, FAST>); }
 
-// hot function combinations get compile-time ids (fused mode, m = 2 / 3), the rest use the run-time table
+// hot function combinations get compile-time ids (fused mode, m = 2 / 3), the rest use the run-time table;
+// `precise` (mde_edges::kvar == 2, MDE_B200_KERNEL=precise) keeps the hot combination off the MUFU math
 template <int M, int MODE>
-static const void* select_m(const FnDev& fn) {
+static const void* select_m(const FnDev& fn, bool precise) {
   const int fa = fn.fn_att, fr = fn.fn_rep, pp = fn.push_pull;
   if constexpr (MODE == 0 && (M == 2 || M == 3)) {
-    static int precise = -1;
-    if (precise < 0) { const char* ev = getenv("MDE_B200_KERNEL"); precise = (ev && !strcmp(ev, "precise")) ? 1 : 0; }
     const bool hot = pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG && fn.a0 == 1.5f && fn.r0 == 1.0f && !precise;
     if (hot) return kptr<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOG, true>();
     if (pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG) return kptr<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOG, false>();
@@ -659,20 +658,21 @@ static const void* select_m(const FnDev& fn) {
 }
 
 template <int MODE>
-static const void* select_mode(const FnDev& fn, int m) {
+static const void* select_mode(const FnDev& fn, int m, bool precise) {
   switch (m) {
-    case 1: return select_m<1, MODE>(fn);
-    case 2: return select_m<2, MODE>(fn);
-    case 3: return select_m<3, MODE>(fn);
-    case 4: return select_m<4, MODE>(fn);
+    case 1: return select_m<1, MODE>(fn, precise);
+    case 2: return select_m<2, MODE>(fn, precise);
+    case 3: return select_m<3, MODE>(fn, precise);
+    case 4: return select_m<4, MODE>(fn, precise);
   }
   return nullptr;
 }
 
-static const void* select_kernel(const FnDev& fn, int m, int mode) {
-  if (mode == 0) return select_mode<0>(fn, m);
-  if (mode == 1) return select_mode<1>(fn, m);
-  return select_mode<2>(fn, m);
+static const void* select_kernel(const mde_edges* e, int m, int mode) {
+  const bool precise = e->kvar == 2;
+  if (mode == 0) return select_mode<0>(e->fn, m, precise);
+  if (mode == 1) return select_mode<1>(e->fn, m, precise);
+  return select_mode<2>(e->fn, m, precise);
 }
 
 // dynamic shared memory above 48 KB needs an opt-in per kernel; done once per kernel, at layout build for the
@@ -688,7 +688,7 @@ static int configure_kernel(const void* k) {
 
 int tiled_configure(const mde_edges* e, int m) {
   for (int mode = 0; mode < 3; ++mode) {
-    const void* k = select_kernel(e->fn, m, mode);
+    const void* k = select_kernel(e, m, mode);
     if (!k) return MDE_E_UNSUPPORTED;
     int rc = configure_kernel(k);
     if (rc) return rc;
@@ -708,7 +708,7 @@ int tiled_launch(int mode, const mde_edges* e, const float* X, int m, float* gra
   a.x_vec_ok = ((reinterpret_cast<uintptr_t>(X) & 15u) == 0) ? 1 : 0;
   a.g_vec_ok = ((reinterpret_cast<uintptr_t>(grad) & 15u) == 0) ? 1 : 0;
   a.gred = e->gred;
-  const void* k = select_kernel(e->fn, m, mode);
+  const void* k = select_kernel(e, m, mode);
   if (!k) return MDE_E_UNSUPPORTED;
   int rc = configure_kernel(k);
   if (rc) return rc;

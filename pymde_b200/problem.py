@@ -349,7 +349,15 @@ class MDE(torch.nn.Module):
             raise ValueError("pymde_b200 evaluates CUDA tensors only; move X to %s" % (self.device,))
         if X.dtype != torch.float32:
             raise ValueError("the CUDA path computes in float32; got %s" % X.dtype)
-        return X if X.is_contiguous() else X.contiguous()
+        if not X.is_contiguous():
+            return X.contiguous()
+        # the kernels load a row of m = 2 as one float2 and rows of m % 4 == 0 as float4s: a contiguous view that
+        # starts inside a row of its storage (e.g. buf[1:].view(n, m)) is copied to storage aligned for those loads
+        m = X.shape[1] if X.dim() == 2 else 1
+        align = 16 if m % 4 == 0 else (8 if m == 2 else 4)
+        if X.data_ptr() % align != 0:
+            return X.clone(memory_format=torch.contiguous_format)
+        return X
 
     # ---- evaluation API ---------------------------------------------------------------------
     def differences(self, X):

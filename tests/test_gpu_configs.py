@@ -4,7 +4,10 @@
             runs of the unmodified reference to convergence with 1 / 4 / 8 threads, and 300 non-converged iterations)
   C3 shape  n = 44 682, 2e7 sampled pairs, losses.Huber, Standardized          -- value + gradient vs the C oracle
   C4 slice  n = 200 000, m = 128, 3e6 edges, PushAndPull (wide kernel)          -- value + gradient vs the C oracle
-  C5 shape  n = 1e7, 5e7 SBM edges, PushAndPull (tile layouts, super-tiles)     -- value + gradient vs the C oracle
+  C5 shape  n = 1e7, 5e7 SBM edges, PushAndPull on the automatic layout (sorted SoA: 5 edges per node is below the
+            dense-graph threshold), forced SoA and tile records (default geometry: 1221 neighbour tiles, 10 super-tiles;
+            pull records refuse this graph: its edges between blocks leave more than 65 536 owner rows inside one
+            warp-tile)                                                            -- value + gradient vs the C oracle
 Tolerances: value 1e-5 relative (north_star), gradient 3e-5 of its largest entry (fp32 sums of up to 1e3 terms)."""
 import hashlib
 import os
@@ -155,9 +158,10 @@ def test_c4_slice_m128_wide_kernel():
     _check_against_oracle(mde, X, e.cpu().numpy(), spec)
 
 
-@pytest.mark.parametrize("layout", [None, "soa"])
-def test_c5_shape_1e7_nodes(layout, monkeypatch):
+@pytest.mark.parametrize("layout,kind", [(None, 0), ("soa", 0), ("tiles", 1)], ids=["None", "soa", "tiles"])
+def test_c5_shape_1e7_nodes(layout, kind, monkeypatch):
     import pymde_b200 as pm
+    from pymde_b200 import _lib
     if layout:
         monkeypatch.setenv("MDE_B200_LAYOUT", layout)
     n, m = 10_000_000, 2
@@ -171,6 +175,7 @@ def test_c5_shape_1e7_nodes(layout, monkeypatch):
     X -= X.mean(0)
     spec = O.FnSpec(O.P_LOG1P, w, (1.5, 0, 0), fn_rep=O.P_LOG, rep=(1.0, 0, 0))
     _check_against_oracle(mde, X, edges, spec)
+    assert _lib.load().mde_edges_kind(mde._layout().handle) == kind
     # size-independent properties: the gradient of a translation-invariant objective sums to zero per column
     Xg = X.clone().requires_grad_(True)
     mde.average_distortion(Xg).backward()
