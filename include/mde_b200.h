@@ -193,9 +193,9 @@ typedef struct mde_solver_opts {
   int32_t constraint;       /* MDE_CONSTRAINT_* */
   int32_t memory_size;      /* L-BFGS history (optim.py:110) */
   int32_t max_iter;         /* capacity of the statistics arrays */
-  int32_t mode;             /* 0 = host-stepped line search; 1 = CUDA graph per iteration with IF / WHILE
-                               conditional nodes; 2 = flat graph of gated "steps" (one closure evaluation each),
-                               no conditional nodes (the default) */
+  int32_t mode;             /* must be 2: flat CUDA graphs of gated "steps" (one closure evaluation each), no
+                               conditional nodes.  0 and 1 (retired drivers) give MDE_E_UNSUPPORTED, any other
+                               value MDE_E_INVALID. */
   int64_t n_anchors;        /* MDE_CONSTRAINT_ANCHORED */
   const int64_t* anchors;   /* device (n_anchors,) */
   const float* anchor_values; /* device (n_anchors, m) */
@@ -217,7 +217,7 @@ int mde_solver_begin_ex(mde_solver_t* s, const float* X0, double eps, int max_it
  * SolverError. */
 int mde_solver_run(mde_solver_t* s, int iters, int* iters_done, int* converged, void* stream);
 
-/* Diagnostics: %globaltimer stamps (ns) of the last step that started an iteration (mode 2, late-epilogue chain):
+/* Diagnostics: %globaltimer stamps (ns) of the last step that started an iteration:
  * [0] entry of the head kernel's last block, [1] its scalar stage begins, [2] solver state staged in shared memory,
  * [3] partials reduced, [4] previous step finished / phase chosen, [5] history update + two-loop done,
  * [6] before the state is written back, [7] first block of the vector kernel that follows.  No reference counterpart. */

@@ -7,8 +7,8 @@
 // Design:
 //  * every vector (X, x_init, d, g, g_prev, the S/Y history ring) and every scalar (loss,
 //    g.d, Wolfe bracket, Gram matrix of the history, statistics) lives in HBM; the host
-//    only enqueues kernels and reads one 32-byte status word per line-search trial
-//    (mode 0) or per batch of iterations (mode 1, CUDA graph with a device-side while loop);
+//    only launches CUDA graphs of identical "steps" (one closure evaluation each, every kernel
+//    gated by a device-side phase machine) and reads one 48-byte status word per batch of steps;
 //  * the two-loop recursion is done on the (2h+1)^2 Gram matrix ("vector-free" L-BFGS):
 //    ONE pass computes all 5h+4 dot products and writes the new (s, y) pair, ONE pass forms
 //    d = cg*g + sum cs_j s_j + cy_j y_j (and snapshots g_prev, x_init, g.d, |d|, |X|).
@@ -50,7 +50,7 @@ constexpr int kMaxSlices = (kMaxMemory + kPairsPerSlice - 1) / kPairsPerSlice;  
 constexpr int kHeadAcc = kDotsPerSlice + 12;  // step_head_kernel: + g.d, g.g, |g|_1, column sums of g and X (+ pad): fp32 accumulators
 constexpr int kHeadCols = kHeadAcc + 6;       // columns of a partial row: + loss, (g.d, d.d, X.X, max|d|) of the vec kernel, pad (even)
 constexpr int kStatusInts = 12;
-enum { PH_DIR = 0, PH_TRIAL = 1, PH_FRESH = 2, PH_MAT = 3 };  // mode 2: phase of a step
+enum { PH_DIR = 0, PH_TRIAL = 1, PH_FRESH = 2, PH_MAT = 3 };  // phase of a step
 
 struct alignas(16) HeadDesc {  // what every block of the next head kernel needs, in 64 bytes (4 broadcast loads)
   int pend, phase, count, n_iter;
@@ -68,31 +68,26 @@ struct SolverState {
   int ls_active;   // line search wants another trial
   int stop_after;  // residual <= eps seen at the start of this iteration
   int pad0;        // low word of func_evals
-  // ---- mode 2 (flat step graph) ----
+  // ---- step phase machine ----
   int paused;      // stopped at iter_limit; mde_solver_run resumes it
   int phase;       // what the next step does (PH_*)
   int iter_limit;  // pause when `iter` reaches it
-  int pend;        // late-epilogue steps: 1 = the previous step executed phase `phase`, its bookkeeping is pending
-  int g_dir;       // gates of the next step, written by the step epilogue: direction kernels run
-  int g_eval;      //   closure evaluation (scatter kernel, tangent projection, dots) runs
-  int g_mat;       //   the axpy materialises the ACCEPTED point (no evaluation follows)
+  int pend;        // 1 = the previous step executed phase `phase`, its bookkeeping is pending
+  int g_eval;      // gates of the next step, written by the head kernel's epilogue: closure evaluation runs
   int g_proj;      //   the iterate moved: retraction kernels run
+  unsigned int ticket;  // last-block-done counter of the head kernel
   // ---- scalars ----
   double eps;
   double loss;     // f at the current iterate (cached loss, lbfgs.py:418-426,550)
   double gg, g1;   // ||g||^2 and ||g||_1 of the gradient buffer
-  float gtd;       // g.d
-  float dmax;      // max |d|
   double dd, xx;   // ||d||^2, ||X||^2 at iteration start
-  unsigned int tickets[4];   // last-block-done counters of the fused vector+scalar kernels
-  float mu_x[4], mu_d[4];  // column means of x_init and d (Centered, m in {1,2,4}: fused into the trial axpy)
+  float mu_x[4], mu_d[4];  // column means of x_init and d (Centered, m in {1,2,4}: fused into the vec kernel)
   double t_last;   // state["t"]
   double t_eval;   // step of the most recent trial evaluation
   long long func_evals;
   int max_stats;
   int world;
   double *avg, *resid, *pct, *steplen;
-  // ---- late-epilogue steps ----
   double t_cur;                      // step length the current step's vec kernel applies (t0 / ls.t / ls.t_accept)
   double cs_g[4], cs_d[4];           // column sums of g_prev and d (tracked through the two-loop coefficients)
   double cs_S[kSlots][4], cs_Y[kSlots][4];  // ... and of the stored pairs
@@ -109,13 +104,11 @@ __device__ __forceinline__ bool off(const int* flag) { return *flag == 0; }
 // 16 independent coalesced loads (through L2: the partials may come from other SMs of the same launch).
 // Stage 2: one warp per output combines the S segment sums with a fixed shuffle tree.  The summation order
 // depends only on (nb, K, blockDim), so scalars are bit-reproducible for a given launch shape.
-template <bool MAXLAST>
 __device__ void reduce_partials(const double* __restrict__ part, int nb, int K, double* out) {
   __shared__ double red_buf[256];
   const int T = blockDim.x < 256 ? blockDim.x : 256;
-  const int S = T / K;  // segments (K <= 44 < T)
+  const int S = T / K;  // segments (K < T)
   const int k = threadIdx.x % K, seg = threadIdx.x / K;
-  const bool is_max = MAXLAST && (k == K - 1);
   if (threadIdx.x < S * K) {
     constexpr int U = 16;
     double s = 0.0;
@@ -124,21 +117,20 @@ __device__ void reduce_partials(const double* __restrict__ part, int nb, int K, 
 #pragma unroll
       for (int u = 0; u < U; ++u) {
         const int b = b0 + u * S;
-        v[u] = (b < nb) ? __ldcg(part + (int64_t)b * K + k) : 0.0;  // 0 is neutral for the sums and for max |.|
+        v[u] = (b < nb) ? __ldcg(part + (int64_t)b * K + k) : 0.0;
       }
 #pragma unroll
-      for (int u = 0; u < U; ++u) s = is_max ? fmax(s, v[u]) : s + v[u];
+      for (int u = 0; u < U; ++u) s += v[u];
     }
     red_buf[seg * K + k] = s;
   }
   __syncthreads();
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = (int)(blockDim.x >> 5);
   for (int kk = w; kk < K; kk += nw) {  // warp-uniform trip count
-    const bool mx = MAXLAST && (kk == K - 1);
     double s = 0.0;
-    for (int q = lane; q < S; q += 32) { const double v = red_buf[q * K + kk]; s = mx ? fmax(s, v) : s + v; }
+    for (int q = lane; q < S; q += 32) s += red_buf[q * K + kk];
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) { const double v = __shfl_xor_sync(kFull, s, o); s = mx ? fmax(s, v) : s + v; }
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(kFull, s, o);
     if (lane == 0) out[kk] = s;
   }
   __syncthreads();
@@ -162,132 +154,16 @@ __device__ bool last_block_done(unsigned int* counter) {
   return s_last != 0;
 }
 
-struct Tail {              // what a fused scalar epilogue needs
-  int fuse;                // 0: separate scalar kernel follows; 1: run the epilogue in the last block
-  int mode;                // grad_dots: 1 = line-search update, 2 = fresh evaluation
+struct Tail {              // what the head kernel's scalar epilogue needs
   const double* lpart;     // loss partials of the distortion launch
   int nl;
   const float* tail;       // (hi, lo) of the all-reduced loss (multi-GPU)
   double p_total;
-  int64_t n_rows;
   double inv_n;            // 1 / n_rows
-  cudaGraphConditionalHandle h_while;
 };
 
-__device__ void direction_scalar_body(SolverState* __restrict__ S, const double* __restrict__ part, int nblocks,
-                                      unsigned char* smem);
-__device__ void ls_init_body(SolverState* __restrict__ S, const double* __restrict__ part, int nblocks,
-                             int64_t n_rows, cudaGraphConditionalHandle h_while);
-__device__ void ls_update_body(SolverState* __restrict__ S, const double* __restrict__ lpart, int nl,
-                               const float* __restrict__ tail, const double* __restrict__ dpart, int nd,
-                               double p_total, cudaGraphConditionalHandle h_while);
-__device__ void fresh_finish_body(SolverState* __restrict__ S, const double* __restrict__ lpart, int nl,
-                                  const float* __restrict__ tail, const double* __restrict__ dpart, int nd,
-                                  double p_total);
-__device__ void iter_end_body(SolverState* __restrict__ S, cudaGraphConditionalHandle h_if_next);
-__device__ void step_end_body(SolverState* __restrict__ S, const double* __restrict__ lpart, int nl,
-                              const float* __restrict__ tail, const double* __restrict__ dpart, int nd,
-                              double p_total);
-
-constexpr int kScalarSmemBytes = (int)(sizeof(double) * (kMaxSlices * kDotsPerSlice + 5 * kSlots) + 64 + sizeof(LbfgsState));
-
 // ---------------------------------------------------------------------------------------
-// P1: candidate pair + all dot products of the history against (y_c, s_c, g)
-// ---------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kVecThreads, 2)
-lbfgs_dots_kernel(SolverState* __restrict__ S, const float* __restrict__ g, const float* __restrict__ gprev,
-                  const float* __restrict__ d, float* __restrict__ Sb, float* __restrict__ Yb,
-                  int64_t npad, double* __restrict__ part, Tail tl, const int* __restrict__ gate) {
-  if (off(&S->active)) return;
-  if (gate != nullptr && off(gate)) return;
-  // reduction tile: 27 rows x 256 threads of fp32 partials (used twice: 54 sums), later the scalar epilogue's scratch
-  constexpr int kHalf = kDotsPerSlice / 2;
-  __shared__ __align__(16) unsigned char raw[sizeof(float) * kHalf * kVecThreads];
-  static_assert(sizeof(raw) >= kScalarSmemBytes, "scalar epilogue must fit in the reduction tile");
-  __shared__ const float* sp[kPairsPerSlice];
-  __shared__ const float* yp[kPairsPerSlice];
-  const int slice = blockIdx.y;
-  const int count = S->lb.count;
-  const bool skip = (S->lb.n_iter == 0) || (slice > 0 && slice * kPairsPerSlice >= count);
-  if (!skip) {
-  const float t = (float)S->t_last;
-  float* sc = Sb + (int64_t)S->lb.cand * npad;
-  float* yc = Yb + (int64_t)S->lb.cand * npad;
-  if (threadIdx.x < kPairsPerSlice) {
-    const int lj = slice * kPairsPerSlice + threadIdx.x;
-    const int q = (lj < count) ? S->lb.order[lj] : 0;
-    sp[threadIdx.x] = Sb + (int64_t)q * npad;
-    yp[threadIdx.x] = Yb + (int64_t)q * npad;
-  }
-  __syncthreads();
-  int nval = count - slice * kPairsPerSlice;  // pairs of this slice (block-uniform)
-  if (nval > kPairsPerSlice) nval = kPairsPerSlice;
-  // fp32 per-thread partial sums (at the bench size a thread owns ONE float4; at 1e7 rows ~130): the block and
-  // grid stages below run in fp64.  The reference accumulates the same dot products in fp32 end to end.
-  float acc[kDotsPerSlice];
-#pragma unroll
-  for (int k = 0; k < kDotsPerSlice; ++k) acc[k] = 0.0f;
-  const int64_t n4 = npad >> 2;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
-    const float4 G = reinterpret_cast<const float4*>(g)[i];
-    const float4 P = reinterpret_cast<const float4*>(gprev)[i];
-    const float4 D = reinterpret_cast<const float4*>(d)[i];
-    const float gv[4] = {G.x, G.y, G.z, G.w};
-    const float yv[4] = {G.x - P.x, G.y - P.y, G.z - P.z, G.w - P.w};
-    const float sv[4] = {D.x * t, D.y * t, D.z * t, D.w * t};
-    if (slice == 0) {
-      reinterpret_cast<float4*>(yc)[i] = make_float4(yv[0], yv[1], yv[2], yv[3]);
-      reinterpret_cast<float4*>(sc)[i] = make_float4(sv[0], sv[1], sv[2], sv[3]);
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        acc[0] += yv[q] * sv[q]; acc[1] += yv[q] * yv[q];
-        acc[2] += sv[q] * gv[q]; acc[3] += yv[q] * gv[q];
-      }
-    }
-#pragma unroll
-    for (int j = 0; j < kPairsPerSlice; ++j) {
-      if (j < nval) {
-        const float4 A = reinterpret_cast<const float4*>(sp[j])[i];
-        const float4 B = reinterpret_cast<const float4*>(yp[j])[i];
-        const float av[4] = {A.x, A.y, A.z, A.w};
-        const float bv[4] = {B.x, B.y, B.z, B.w};
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          acc[4 + 5 * j + 0] += av[q] * yv[q];
-          acc[4 + 5 * j + 1] += bv[q] * yv[q];
-          acc[4 + 5 * j + 2] += sv[q] * bv[q];
-          acc[4 + 5 * j + 3] += av[q] * gv[q];
-          acc[4 + 5 * j + 4] += bv[q] * gv[q];
-        }
-      }
-    }
-  }
-  // block reduction through a transposed shared-memory tile, two halves of 27 sums: each warp sums whole rows in
-  // fp64 (8 conflict-free loads per lane + one shuffle tree per row)
-  float (*tile)[kVecThreads] = reinterpret_cast<float (*)[kVecThreads]>(raw);
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  double* o = part + ((int64_t)slice * gridDim.x + blockIdx.x) * kDotsPerSlice;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    if (h) __syncthreads();
-#pragma unroll
-    for (int k = 0; k < kHalf; ++k) tile[k][threadIdx.x] = acc[h * kHalf + k];
-    __syncthreads();
-    for (int k = w; k < kHalf; k += kVecThreads / 32) {
-      double sum = 0.0;
-#pragma unroll
-      for (int q = 0; q < kVecThreads / 32; ++q) sum += (double)tile[k][lane + 32 * q];
-      sum = warp_sum(sum);
-      if (lane == 0) o[h * kHalf + k] = sum;
-    }
-  }
-  }  // !skip
-  if (tl.fuse && last_block_done(&S->tickets[0])) direction_scalar_body(S, part, gridDim.x, raw);
-}
-
-// ---------------------------------------------------------------------------------------
-// S1: statistics of the iteration start + history update + two-loop in Gram form
+// history update + two-loop in Gram form
 // ---------------------------------------------------------------------------------------
 // Block-cooperative version of mde_logic.h::lbfgs_direction (same decisions, same formulas): thread 0
 // takes the accept / evict decision, all threads move the Gram matrices, warp 0 runs the two-loop
@@ -393,251 +269,6 @@ __device__ void lbfgs_direction_block(LbfgsState& B, double* dots, double ys, do
   }
 }
 
-__device__ void direction_scalar_body(SolverState* __restrict__ S, const double* __restrict__ part, int nblocks,
-                                      unsigned char* smem) {
-  // carve: history state (Gram matrices included) | block sums | per-pair dots | flags
-  LbfgsState& sB = *reinterpret_cast<LbfgsState*>(smem);
-  double* sums = reinterpret_cast<double*>(smem + sizeof(LbfgsState));
-  double* dots = sums + kMaxSlices * kDotsPerSlice;
-  int* flags = reinterpret_cast<int*>(dots + 5 * kSlots);
-  static_assert(sizeof(LbfgsState) % sizeof(double) == 0, "LbfgsState must be a whole number of doubles");
-  static_assert(kMaxMemory <= 32, "the two-loop recursion maps one pair per lane");
-  // The history state is staged through registers so that its loads are in flight together with the loads of
-  // the reductions below (both come from L2; issuing them back to back hides one round trip).
-  constexpr int kStateDoubles = (int)(sizeof(LbfgsState) / sizeof(double));
-  constexpr int kStatePerThread = (kStateDoubles + 255) / 256;
-  const int count = S->lb.count;
-  const int n_iter = S->lb.n_iter;
-  double stage[kStatePerThread];
-  {
-    const double* src = reinterpret_cast<const double*>(&S->lb);
-#pragma unroll
-    for (int q = 0; q < kStatePerThread; ++q) {
-      const int k = (int)threadIdx.x + q * 256;
-      stage[q] = (threadIdx.x < 256 && k < kStateDoubles) ? __ldcg(src + k) : 0.0;
-    }
-  }
-  int slices = (count + kPairsPerSlice - 1) / kPairsPerSlice;
-  if (slices < 1) slices = 1;
-  if (n_iter > 0) {
-    for (int s = 0; s < slices; ++s)
-      reduce_partials<false>(part + (int64_t)s * nblocks * kDotsPerSlice, nblocks, kDotsPerSlice,
-                             sums + s * kDotsPerSlice);
-  }
-  {
-    double* dst = reinterpret_cast<double*>(&sB);
-#pragma unroll
-    for (int q = 0; q < kStatePerThread; ++q) {
-      const int k = (int)threadIdx.x + q * 256;
-      if (threadIdx.x < 256 && k < kStateDoubles) dst[k] = stage[q];
-    }
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    // callback of LBFGS.step (optim.py:94-96): loss and ||X.grad||_F at the iteration start
-    const int it = S->iter;
-    const double resid = (double)sqrtf((float)S->gg);
-    if (it < S->max_stats) { S->avg[it] = S->loss; S->resid[it] = resid; }
-    S->stop_after = (resid <= S->eps) ? 1 : 0;
-  }
-  if (threadIdx.x < count) {
-    const int j = threadIdx.x;
-    const double* b = sums + (j / kPairsPerSlice) * kDotsPerSlice + 4 + 5 * (j % kPairsPerSlice);
-    dots[j] = b[0]; dots[kSlots + j] = b[1]; dots[2 * kSlots + j] = b[2]; dots[3 * kSlots + j] = b[3];
-    dots[4 * kSlots + j] = b[4];
-  }
-  __syncthreads();
-  if (n_iter > 0) lbfgs_direction_block(sB, dots, sums[0], sums[1], sums[2], sums[3], flags);
-  else lbfgs_direction_block(sB, dots, 0.0, 0.0, 0.0, 0.0, flags);
-  __syncthreads();
-  {
-    double* dst = reinterpret_cast<double*>(&S->lb);
-    const double* src = reinterpret_cast<const double*>(&sB);
-    for (int k = threadIdx.x; k < (int)(sizeof(LbfgsState) / sizeof(double)); k += blockDim.x) dst[k] = src[k];
-  }
-}
-
-__global__ void __launch_bounds__(256)
-direction_scalar_kernel(SolverState* __restrict__ S, const double* __restrict__ part, int nblocks) {
-  if (off(&S->active)) return;
-  __shared__ __align__(16) unsigned char raw[kScalarSmemBytes];
-  direction_scalar_body(S, part, nblocks, raw);
-}
-
-// ---------------------------------------------------------------------------------------
-// P2: d = cg*g + sum_j cs_j S_j + cy_j Y_j ; g_prev = g ; x_init = X ; partial g.d, d.d, X.X, max|d|
-// ---------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kVecThreads)
-direction_apply_kernel(SolverState* __restrict__ S, const float* __restrict__ g, float* __restrict__ gprev,
-                       float* __restrict__ d, const float* __restrict__ X, float* __restrict__ xinit,
-                       const float* __restrict__ Sb, const float* __restrict__ Yb, int64_t npad,
-                       double* __restrict__ part, int mcols, Tail tl, const int* __restrict__ gate) {
-  if (off(&S->active)) return;
-  if (gate != nullptr && off(gate)) return;
-  __shared__ float cs[kMaxMemory], cy[kMaxMemory];
-  __shared__ const float* ps[kMaxMemory];
-  __shared__ const float* py[kMaxMemory];
-  const int count = S->lb.count;
-  const float cg = (float)S->lb.cg;
-  if (threadIdx.x < count) {
-    cs[threadIdx.x] = (float)S->lb.cs[threadIdx.x];
-    cy[threadIdx.x] = (float)S->lb.cy[threadIdx.x];
-    int q = S->lb.order[threadIdx.x];
-    ps[threadIdx.x] = Sb + (int64_t)q * npad;
-    py[threadIdx.x] = Yb + (int64_t)q * npad;
-  }
-  __syncthreads();
-  constexpr int KA = 11;  // g.d, d.d, X.X, column sums of X (4) and of d (4)
-  double acc[KA];
-  float fa[KA];
-#pragma unroll
-  for (int k = 0; k < KA; ++k) { acc[k] = 0.0; fa[k] = 0.0f; }
-  float mx = 0.0f;
-  const int64_t n4 = npad >> 2;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  int cnt = 0;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
-    float4 G = reinterpret_cast<const float4*>(g)[i];
-    float4 Xv = reinterpret_cast<const float4*>(X)[i];
-    float r[4] = {cg * G.x, cg * G.y, cg * G.z, cg * G.w};
-    for (int j = 0; j < count; ++j) {
-      float4 A = reinterpret_cast<const float4*>(ps[j])[i];
-      float4 B = reinterpret_cast<const float4*>(py[j])[i];
-      r[0] += cs[j] * A.x + cy[j] * B.x; r[1] += cs[j] * A.y + cy[j] * B.y;
-      r[2] += cs[j] * A.z + cy[j] * B.z; r[3] += cs[j] * A.w + cy[j] * B.w;
-    }
-    reinterpret_cast<float4*>(d)[i] = make_float4(r[0], r[1], r[2], r[3]);
-    reinterpret_cast<float4*>(gprev)[i] = G;
-    reinterpret_cast<float4*>(xinit)[i] = Xv;
-    fa[0] += G.x * r[0] + G.y * r[1] + G.z * r[2] + G.w * r[3];
-    fa[1] += r[0] * r[0] + r[1] * r[1] + r[2] * r[2] + r[3] * r[3];
-    fa[2] += Xv.x * Xv.x + Xv.y * Xv.y + Xv.z * Xv.z + Xv.w * Xv.w;
-    mx = fmaxf(mx, fmaxf(fmaxf(fabsf(r[0]), fabsf(r[1])), fmaxf(fabsf(r[2]), fabsf(r[3]))));
-    // column sums (rows are m floats; 4 % m == 0 so element q of a float4 belongs to column q % m)
-    if (mcols == 1) {
-      fa[3] += Xv.x + Xv.y + Xv.z + Xv.w; fa[7] += r[0] + r[1] + r[2] + r[3];
-    } else if (mcols == 2) {
-      fa[3] += Xv.x + Xv.z; fa[4] += Xv.y + Xv.w; fa[7] += r[0] + r[2]; fa[8] += r[1] + r[3];
-    } else if (mcols == 4) {
-      fa[3] += Xv.x; fa[4] += Xv.y; fa[5] += Xv.z; fa[6] += Xv.w;
-      fa[7] += r[0]; fa[8] += r[1]; fa[9] += r[2]; fa[10] += r[3];
-    }
-    if (++cnt == 16) {
-#pragma unroll
-      for (int k = 0; k < KA; ++k) { acc[k] += (double)fa[k]; fa[k] = 0.0f; }
-      cnt = 0;
-    }
-  }
-#pragma unroll
-  for (int k = 0; k < KA; ++k) acc[k] += (double)fa[k];
-  __shared__ double sm[KA * 32];
-  __shared__ float smx[32];
-  block_sum<KA>(acc, sm);
-  mx = warp_max(mx);
-  if ((threadIdx.x & 31) == 0) smx[threadIdx.x >> 5] = mx;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float m2 = 0.0f;
-    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) m2 = fmaxf(m2, smx[w]);
-    double* o = part + (int64_t)blockIdx.x * (KA + 1);
-#pragma unroll
-    for (int k = 0; k < KA; ++k) o[k] = acc[k];
-    o[KA] = (double)m2;
-  }
-  if (tl.fuse && last_block_done(&S->tickets[1])) ls_init_body(S, part, gridDim.x, tl.n_rows, tl.h_while);
-}
-
-// S2: finalize g.d, |d|, |X|; initial step; arm the line search (lbfgs.py:521-549)
-__device__ void ls_init_body(SolverState* __restrict__ S, const double* __restrict__ part, int nblocks,
-                             int64_t n_rows, cudaGraphConditionalHandle h_while) {
-  __shared__ double out[12];
-  reduce_partials<true>(part, nblocks, 12, out);
-  if (threadIdx.x == 0) {
-    S->gtd = (float)out[0]; S->dd = out[1]; S->xx = out[2]; S->dmax = (float)out[11];
-    const double inv_n = 1.0 / (double)n_rows;
-#pragma unroll
-    for (int c = 0; c < 4; ++c) { S->mu_x[c] = (float)(out[3 + c] * inv_n); S->mu_d[c] = (float)(out[7 + c] * inv_n); }
-    double t0 = 1.0;
-    if (S->lb.n_iter == 1) {  // t = min(1, 1/||g||_1) * lr
-      float inv = 1.0f / (float)S->g1;
-      t0 = (inv < 1.0f) ? (double)inv : 1.0;
-    }
-    LsState L;
-    ls_begin(L, t0, S->loss, (float)out[0], (float)out[11]);
-    S->ls = L;
-    S->ls_active = 1;
-    if (h_while) cudaGraphSetConditional(h_while, 1u);  // enter the device-side trial loop
-  }
-}
-
-__global__ void __launch_bounds__(256)
-ls_init_kernel(SolverState* __restrict__ S, const double* __restrict__ part, int nblocks, int64_t n_rows,
-               cudaGraphConditionalHandle h_while) {
-  if (off(&S->active)) return;
-  ls_init_body(S, part, nblocks, n_rows, h_while);
-}
-
-// graph mode: gate of the IF node around the fresh evaluation
-__global__ void fresh_gate_kernel(const SolverState* __restrict__ S, cudaGraphConditionalHandle h_if) {
-  if (threadIdx.x == 0) cudaGraphSetConditional(h_if, (S->active && S->need_fresh) ? 1u : 0u);
-}
-
-// ---------------------------------------------------------------------------------------
-// trial point: X = x_init + t*d  (LBFGS._add_grad, lbfgs.py:350-357); FINAL uses t_accept
-// ---------------------------------------------------------------------------------------
-// center_m = 0: plain axpy.  center_m in {1,2,4}: the Centered projection (constraints.py:106-111) is
-// folded in analytically, mean(x_init + t d) = mean(x_init) + t mean(d) with both means taken in the
-// direction pass, so a trial point costs one pass and no reduction.  `gz` (trial only): gradient buffer
-// zeroed in the same pass for the scatter kernel that follows.
-template <bool FINAL>
-__global__ void __launch_bounds__(kVecThreads)
-trial_axpy_kernel(SolverState* __restrict__ S, const float* __restrict__ xinit, const float* __restrict__ d,
-                  float* __restrict__ X, int64_t npad, int64_t nvalid, int center_m, float* __restrict__ gz,
-                  int fuse_end, cudaGraphConditionalHandle h_if_next) {
-  if (off(&S->active)) return;
-  if (!FINAL && off(&S->ls_active)) return;
-  const float t = FINAL ? (float)S->ls.t_accept : (float)S->ls.t;
-  // FINAL: the accepted step is usually the last trial evaluated -- X already holds exactly
-  // project(x_init + t d) (same kernel, same inputs, deterministic), so only the epilogue is needed.
-  const bool same_point = FINAL && center_m != 0 && (S->ls.t_accept == S->t_eval);
-  float mu[4] = {0.f, 0.f, 0.f, 0.f};
-  if (center_m == 1) { float v = S->mu_x[0] + t * S->mu_d[0]; mu[0] = mu[1] = mu[2] = mu[3] = v; }
-  else if (center_m == 2) {
-    float v0 = S->mu_x[0] + t * S->mu_d[0], v1 = S->mu_x[1] + t * S->mu_d[1];
-    mu[0] = mu[2] = v0; mu[1] = mu[3] = v1;
-  } else if (center_m == 4) {
-#pragma unroll
-    for (int c = 0; c < 4; ++c) mu[c] = S->mu_x[c] + t * S->mu_d[c];
-  }
-  const int64_t n4 = npad >> 2;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4 + 1 && !same_point; i += stride) {
-    if (i < n4) {
-      float4 A = reinterpret_cast<const float4*>(xinit)[i];
-      float4 D = reinterpret_cast<const float4*>(d)[i];
-      float4 R = make_float4(fmaf(t, D.x, A.x) - mu[0], fmaf(t, D.y, A.y) - mu[1], fmaf(t, D.z, A.z) - mu[2],
-                             fmaf(t, D.w, A.w) - mu[3]);
-      if (center_m != 0 && 4 * i + 3 >= nvalid) {  // keep the zero padding behind the last row
-        if (4 * i + 0 >= nvalid) R.x = 0.f;
-        if (4 * i + 1 >= nvalid) R.y = 0.f;
-        if (4 * i + 2 >= nvalid) R.z = 0.f;
-        if (4 * i + 3 >= nvalid) R.w = 0.f;
-      }
-      reinterpret_cast<float4*>(X)[i] = R;
-    }
-    if (!FINAL && gz != nullptr) reinterpret_cast<float4*>(gz)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-  if (FINAL && fuse_end && last_block_done(&S->tickets[3])) iter_end_body(S, h_if_next);
-}
-
-__global__ void __launch_bounds__(kVecThreads)
-zero_kernel(const int* flag, float* __restrict__ p, int64_t n4) {
-  if (off(flag)) return;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride)
-    reinterpret_cast<float4*>(p)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-}
-
 // anchored constraint (pymde/constraints.py:114-164): overwrite / zero anchor rows
 __global__ void anchor_rows_kernel(const int* flag, float* __restrict__ Z, const int64_t* __restrict__ anchors,
                                    const float* __restrict__ values, int64_t na, int m) {
@@ -648,7 +279,7 @@ __global__ void anchor_rows_kernel(const int* flag, float* __restrict__ Z, const
   Z[a * m + (i % m)] = values ? values[i] : 0.0f;
 }
 
-// mode 2, multi-GPU: the all-reduced [gradient | loss] becomes the solver's gradient buffer -- only when the
+// multi-GPU: the all-reduced [gradient | loss] becomes the solver's gradient buffer -- only when the
 // step really evaluated (the all-reduce itself cannot be gated, so it works on a staging buffer)
 __global__ void __launch_bounds__(kVecThreads)
 gated_copy_kernel(const int* flag, const float* __restrict__ src, float* __restrict__ dst, int64_t n4) {
@@ -663,7 +294,7 @@ __global__ void __launch_bounds__(256)
 pack_loss_kernel(const int* flag, const double* __restrict__ lpart, int nl, float* __restrict__ tail) {
   if (off(flag)) return;
   __shared__ double out[1];
-  reduce_partials<false>(lpart, nl, 1, out);
+  reduce_partials(lpart, nl, 1, out);
   if (threadIdx.x == 0) {
     float hi = (float)out[0];
     tail[0] = hi;
@@ -941,188 +572,8 @@ allreduce_push_kernel(const int* __restrict__ flag, Comm c, int64_t npad, int* _
   if (s_last) comm_signal(STAGE == 0 ? c.fa : c.fb, c, ep);
 }
 
-// T5: partial g.d, g.g, |g|_1
-__global__ void __launch_bounds__(kVecThreads)
-grad_dots_kernel(const int* flag, const float* __restrict__ g, const float* __restrict__ d, int64_t npad,
-                 double* __restrict__ part, SolverState* __restrict__ S, Tail tl) {
-  if (tl.mode == 3) {  // mode 2 step: `flag` is the evaluation gate; PH_MAT has no evaluation, only the epilogue
-    if (off(&S->active)) return;
-    if (S->g_mat) {  // the epilogue rewrites the gates: run it once every block has read them
-      if (last_block_done(&S->tickets[2])) step_end_body(S, tl.lpart, tl.nl, tl.tail, part, gridDim.x, tl.p_total);
-      return;
-    }
-  }
-  if (off(flag)) return;
-  double acc[3] = {0.0, 0.0, 0.0};
-  float fa[3] = {0.0f, 0.0f, 0.0f};
-  const int64_t n4 = npad >> 2;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  int cnt = 0;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
-    float4 G = reinterpret_cast<const float4*>(g)[i];
-    float4 D = reinterpret_cast<const float4*>(d)[i];
-    fa[0] += G.x * D.x + G.y * D.y + G.z * D.z + G.w * D.w;
-    fa[1] += G.x * G.x + G.y * G.y + G.z * G.z + G.w * G.w;
-    fa[2] += fabsf(G.x) + fabsf(G.y) + fabsf(G.z) + fabsf(G.w);
-    if (++cnt == 16) {
-      for (int k = 0; k < 3; ++k) { acc[k] += (double)fa[k]; fa[k] = 0.0f; }
-      cnt = 0;
-    }
-  }
-  for (int k = 0; k < 3; ++k) acc[k] += (double)fa[k];
-  __shared__ double sm[3 * 32];
-  block_sum<3>(acc, sm);
-  if (threadIdx.x == 0) {
-    double* o = part + (int64_t)blockIdx.x * 3;
-    o[0] = acc[0]; o[1] = acc[1]; o[2] = acc[2];
-  }
-  if (tl.fuse && last_block_done(&S->tickets[2])) {
-    if (tl.mode == 1) ls_update_body(S, tl.lpart, tl.nl, tl.tail, part, gridDim.x, tl.p_total, tl.h_while);
-    else if (tl.mode == 3) step_end_body(S, tl.lpart, tl.nl, tl.tail, part, gridDim.x, tl.p_total);
-    else fresh_finish_body(S, tl.lpart, tl.nl, tl.tail, part, gridDim.x, tl.p_total);
-  }
-}
-
-// loss of one evaluation as the reference sees it: fp32 mean, then float(...)
-__device__ double eval_loss(const SolverState* S, const double* lpart, int nl, const float* tail, double* smem1,
-                            double p_total) {
-  double sum;
-  if (S->world > 1) {
-    sum = (double)tail[0] + (double)tail[1];
-    __syncthreads();
-  } else {
-    reduce_partials<false>(lpart, nl, 1, smem1);
-    sum = smem1[0];
-  }
-  return (double)(float)(sum / p_total);
-}
-
-// Both reductions an evaluation needs in ONE pass: loss partials of the scatter launch (nl x 1) and the
-// (g.d, g.g, |g|_1) partials of the dots pass (nd x 3).  Same thread mapping and summation order as two
-// reduce_partials calls (bit-identical results), but the loads of both are in flight together and there
-// are two block barriers instead of four.  blockDim.x == 256.  out4 = [loss sum, g.d, g.g, |g|_1].
-__device__ void reduce_loss_and_dots(const double* __restrict__ lpart, int nl, const double* __restrict__ dpart,
-                                     int nd, double* out4) {
-  __shared__ double buf_a[256], buf_b[256];
-  constexpr int U = 4, SB = 85;  // 85 segments x 3 outputs = 255 threads for the dots
-  const int t = threadIdx.x;
-  const int kb = t % 3, segb = t / 3;
-  const bool useb = t < 3 * SB;
-  double a = 0.0, b = 0.0;
-  for (int it = 0;; ++it) {
-    const int ia0 = t + it * U * 256, ib0 = segb + it * U * SB;
-    if (ia0 >= nl && (!useb || ib0 >= nd)) break;
-    double va[U], vb[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) { const int i = ia0 + u * 256; va[u] = (i < nl) ? __ldcg(lpart + i) : 0.0; }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int i = ib0 + u * SB;
-      vb[u] = (useb && i < nd) ? __ldcg(dpart + (int64_t)i * 3 + kb) : 0.0;
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) a += va[u];
-#pragma unroll
-    for (int u = 0; u < U; ++u) b += vb[u];
-  }
-  buf_a[t] = a;
-  buf_b[t] = b;  // index seg * 3 + k == t for t < 255
-  __syncthreads();
-  const int lane = t & 31, w = t >> 5;
-  if (w == 0) {
-    double v = 0.0;
-    for (int q = lane; q < 256; q += 32) v += buf_a[q];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-    if (lane == 0) out4[0] = v;
-  } else if (w <= 3) {
-    const int k = w - 1;
-    double v = 0.0;
-    for (int q = lane; q < SB; q += 32) v += buf_b[q * 3 + k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-    if (lane == 0) out4[1 + k] = v;
-  }
-  __syncthreads();
-}
-
-// loss and (g.d, g.g, |g|_1) of one evaluation -> out3[0..2], returns the loss as the reference sees it
-__device__ double eval_reductions(const SolverState* S, const double* lpart, int nl, const float* tail,
-                                  const double* dpart, int nd, double p_total, double* out3) {
-  __shared__ double r4[4];
-  if (S->world > 1 || blockDim.x != 256) {
-    __shared__ double l1[1];
-    const double loss = eval_loss(S, lpart, nl, tail, l1, p_total);
-    reduce_partials<false>(dpart, nd, 3, out3);
-    return loss;
-  }
-  reduce_loss_and_dots(lpart, nl, dpart, nd, r4);
-  if (threadIdx.x < 3) out3[threadIdx.x] = r4[1 + threadIdx.x];
-  const double loss = (double)(float)(r4[0] / p_total);
-  __syncthreads();
-  return loss;
-}
-
-// S(fresh): closure() at the current iterate (lbfgs.py:426), no line search involved
-__device__ void fresh_finish_body(SolverState* __restrict__ S, const double* __restrict__ lpart, int nl,
-                                  const float* __restrict__ tail, const double* __restrict__ dpart, int nd,
-                                  double p_total) {
-  __shared__ double out[3];
-  const double loss = eval_reductions(S, lpart, nl, tail, dpart, nd, p_total, out);
-  if (threadIdx.x == 0) {
-    S->loss = loss; S->gg = out[1]; S->g1 = out[2];
-    S->func_evals += 1;
-    S->pad0 = (int)S->func_evals;
-  }
-}
-
-__global__ void __launch_bounds__(256)
-fresh_finish_kernel(SolverState* __restrict__ S, const double* __restrict__ lpart, int nl,
-                    const float* __restrict__ tail, const double* __restrict__ dpart, int nd, double p_total) {
-  if (off(&S->active) || off(&S->need_fresh)) return;
-  fresh_finish_body(S, lpart, nl, tail, dpart, nd, p_total);
-}
-
-// S(trial): feed (f_new, g.d) to the Wolfe state machine; decide the next step or finish
-__device__ void ls_update_body(SolverState* __restrict__ S, const double* __restrict__ lpart, int nl,
-                               const float* __restrict__ tail, const double* __restrict__ dpart, int nd,
-                               double p_total, cudaGraphConditionalHandle h_while) {
-  __shared__ double out[3];
-  const double loss = eval_reductions(S, lpart, nl, tail, dpart, nd, p_total, out);
-  if (threadIdx.x == 0) {
-    S->gg = out[1]; S->g1 = out[2];
-    S->func_evals += 1;
-    S->pad0 = (int)S->func_evals;
-    LsState L = S->ls;  // work on a register copy: the state machine touches ~30 fields
-    S->t_eval = L.t;
-    const bool finite = isfinite(out[1]);
-    ls_on_result(L, loss, (float)out[0], finite);
-    S->ls = L;
-    if (L.phase == LS_DONE) {
-      S->ls_active = 0;
-      if (L.error) { S->error = MDE_E_NAN; S->active = 0; }
-      S->t_last = L.t_accept;
-      S->loss = (double)(float)L.f_accept;  // _cached_loss is an fp32 tensor (lbfgs.py:550)
-    }
-    if (h_while) cudaGraphSetConditional(h_while, (S->ls_active && S->active) ? 1u : 0u);
-  }
-}
-
-__global__ void __launch_bounds__(256)
-ls_update_kernel(SolverState* __restrict__ S, const double* __restrict__ lpart, int nl,
-                 const float* __restrict__ tail, const double* __restrict__ dpart, int nd, double p_total,
-                 cudaGraphConditionalHandle h_while) {
-  if (off(&S->active) || off(&S->ls_active)) {
-    if (h_while && threadIdx.x == 0) cudaGraphSetConditional(h_while, 0u);
-    return;
-  }
-  ls_update_body(S, lpart, nl, tail, dpart, nd, p_total, h_while);
-}
-
-// S5: end of iteration (optim.py:135-173)
-// `h_if_next`: in a graph that chains several iterations, the gate of the NEXT iteration's fresh-evaluation
-// IF node is set here instead of by a separate one-thread kernel (0 = none).
-__device__ void iter_end_body(SolverState* __restrict__ S, cudaGraphConditionalHandle h_if_next) {
+// end of iteration (optim.py:135-173)
+__device__ void iter_end_body(SolverState* __restrict__ S) {
   if (threadIdx.x != 0) return;
   const int it = S->iter;
   const double h = S->ls.t_accept;
@@ -1134,66 +585,13 @@ __device__ void iter_end_body(SolverState* __restrict__ S, cudaGraphConditionalH
   else if (h == 0.0) { lbfgs_reset(S->lb, S->lb.memory); S->need_fresh = 1; }  // opt.reset()
   else S->need_fresh = 0;
   if (S->iter >= S->max_stats) S->active = 0;
-  if (h_if_next) cudaGraphSetConditional(h_if_next, (S->active && S->need_fresh) ? 1u : 0u);
-}
-
-__global__ void iter_end_kernel(SolverState* __restrict__ S, cudaGraphConditionalHandle h_if_next) {
-  if (off(&S->active)) return;  // the next IF handle keeps its default (0): nothing runs any more
-  iter_end_body(S, h_if_next);
 }
 
 // ---------------------------------------------------------------------------------------
-// mode 2: the solve as a flat chain of identical "steps" (no conditional graph nodes: an IF or WHILE node costs
-// several times a dependent kernel node, tools/microbench/graph_overheads.cu measures them).  A step = direction kernels (gated) -> axpy -> retraction (gated)
-// -> scatter kernel -> tangent projection -> dots + epilogue; it performs exactly one closure evaluation.
-// The epilogue (last block of the dots kernel) advances a small phase machine and writes the gates the
-// next step's kernels read:
-//   PH_FRESH  closure at the current iterate (lbfgs n_iter == 0)           -> PH_DIR
-//   PH_DIR    new direction + first line-search trial                      -> PH_TRIAL | PH_MAT | end of iteration
-//   PH_TRIAL  another trial of the same line search                        -> PH_TRIAL | PH_MAT | end of iteration
-//   PH_MAT    X = retract(x_init + t_accept d) when the accepted step is not the last one evaluated
-//             (otherwise X already holds it bit for bit); no evaluation     -> end of iteration
-// End of iteration (iter_end_body) -> PH_DIR, or PH_FRESH after a reset, or pause at iter_limit.
-// ---------------------------------------------------------------------------------------
-__device__ void set_phase(SolverState* __restrict__ S, int ph) {
-  S->phase = ph;
-  S->need_fresh = (ph == PH_FRESH) ? 1 : 0;
-  const int on = S->active;
-  S->g_dir = (on && ph == PH_DIR) ? 1 : 0;
-  S->g_eval = (on && ph != PH_MAT) ? 1 : 0;
-  S->g_mat = (on && ph == PH_MAT) ? 1 : 0;
-  S->g_proj = (on && ph != PH_FRESH) ? 1 : 0;
-}
-
-__device__ void step_end_body(SolverState* __restrict__ S, const double* __restrict__ lpart, int nl,
-                              const float* __restrict__ tail, const double* __restrict__ dpart, int nd,
-                              double p_total) {
-  const int ph = S->phase;  // uniform over the block
-  if (ph == PH_FRESH) fresh_finish_body(S, lpart, nl, tail, dpart, nd, p_total);
-  else if (ph != PH_MAT) ls_update_body(S, lpart, nl, tail, dpart, nd, p_total, 0);
-  if (threadIdx.x != 0) return;
-  if (S->error == MDE_E_COMM) S->active = 0;  // a peer never arrived: stop instead of timing out once per step
-  int next = ph;
-  bool end_of_iteration = false;
-  if (ph == PH_FRESH) next = PH_DIR;
-  else if (ph == PH_MAT) end_of_iteration = true;
-  else if (S->ls_active) next = PH_TRIAL;
-  else if (S->active) {  // line search finished (on SolverError `active` is already 0)
-    if (S->ls.t_accept == S->t_eval) end_of_iteration = true;
-    else next = PH_MAT;
-  }
-  if (end_of_iteration) {
-    iter_end_body(S, 0);
-    next = S->need_fresh ? PH_FRESH : PH_DIR;
-    if (S->active && S->iter >= S->iter_limit) { S->active = 0; S->paused = 1; }
-  }
-  set_phase(S, next);
-}
-
-// ---------------------------------------------------------------------------------------
-// mode 2, "late epilogue" steps (default; MDE_B200_LATE=0 keeps the chain above).  A step is
+// The solve as a flat chain of identical "steps" (no conditional graph nodes: an IF or WHILE node costs several
+// times a dependent kernel node, tools/microbench/graph_overheads.cu measures them).  A step is
 //     head -> vec -> [retraction kernels] -> scatter [-> all-reduce] [-> tangent projection]
-// with ONE scalar stage, in the head kernel's last block:
+// and performs exactly one closure evaluation, with ONE scalar stage, in the head kernel's last block:
 //   head  reads g, g_prev, d, X and the history once: (g.d, g.g, |g|_1) of the evaluation the previous step left
 //         pending, the history dots of the iteration that would start if that trial is accepted, column sums of g and
 //         X (Centered).  Its blocks also fold the previous scatter launch's loss partials and the previous vec
@@ -1202,11 +600,25 @@ __device__ void step_end_body(SolverState* __restrict__ S, const double* __restr
 //         step's phase, and when an iteration starts: history update, two-loop, first step length, column means.
 //   vec   PH_DIR: d = H g, g_prev = g, x_init = X and the first trial X = x_init + t0 d in ONE pass (t0 does not
 //         depend on g.d: lbfgs.py:521-530); PH_TRIAL / PH_MAT: X = x_init + t d; every phase but PH_MAT: g = 0.
-// 3 kernels and one one-block epilogue per evaluation instead of 5 and 3.  The history dots are SPECULATIVE (they
-// assume the trial just evaluated, t = t_cur, is accepted, which the strong-Wolfe search does ~9 times out of 10);
-// when it asks for another trial they are unused, when it accepts an earlier point (PH_MAT) the step after the
-// materialisation recomputes them with the accepted t.
+// The epilogue advances a small phase machine and writes the gates the next step's kernels read:
+//   PH_FRESH  closure at the current iterate (lbfgs n_iter == 0)           -> PH_DIR
+//   PH_DIR    new direction + first line-search trial                      -> PH_TRIAL | PH_MAT | end of iteration
+//   PH_TRIAL  another trial of the same line search                        -> PH_TRIAL | PH_MAT | end of iteration
+//   PH_MAT    X = retract(x_init + t_accept d) when the accepted step is not the last one evaluated
+//             (otherwise X already holds it bit for bit); no evaluation     -> end of iteration
+// End of iteration (iter_end_body) -> PH_DIR, or PH_FRESH after a reset, or pause at iter_limit.
+// The history dots are SPECULATIVE (they assume the trial just evaluated, t = t_cur, is accepted, which the
+// strong-Wolfe search does ~9 times out of 10); when it asks for another trial they are unused, when it accepts an
+// earlier point (PH_MAT) the step after the materialisation recomputes them with the accepted t.
 // ---------------------------------------------------------------------------------------
+__device__ void set_phase(SolverState* __restrict__ S, int ph) {
+  S->phase = ph;
+  S->need_fresh = (ph == PH_FRESH) ? 1 : 0;
+  const int on = S->active;
+  S->g_eval = (on && ph != PH_MAT) ? 1 : 0;
+  S->g_proj = (on && ph != PH_FRESH) ? 1 : 0;
+}
+
 constexpr int kColG = kDotsPerSlice + 3;   // 57: column sums of g (4)
 constexpr int kColX = kDotsPerSlice + 7;   // 61: column sums of X (4)
 constexpr int kColLoss = kHeadAcc;         // 66: loss partial sum of the pending evaluation
@@ -1247,7 +659,7 @@ __device__ void ls_apply(SolverState* __restrict__ S, double loss, double gtd, d
   }
 }
 
-// The scalar stage of a late-epilogue step (last block of the head kernel).  The whole SolverState (history Gram
+// The scalar stage of a step (last block of the head kernel).  The whole SolverState (history Gram
 // matrices included, ~21 KB) is staged into shared memory with one cooperative copy, the phase machine, the
 // line search and the two-loop recursion run on that copy, and it is written back once at the end: the serial
 // part never waits for an L2 round trip.
@@ -1346,8 +758,7 @@ __device__ void step_head_body(SolverState* __restrict__ S, const double* __rest
       if (prev == PH_FRESH) fresh_apply(sS, loss, gg, g1);
       else if (prev != PH_MAT) {
         if (prev == PH_DIR) {  // the line-search init the vec kernel could not do (lbfgs.py:521-549)
-          sS->gtd = (float)sums[kColVec]; sS->dd = sums[kColVec + 1]; sS->xx = sums[kColVec + 2];
-          sS->dmax = (float)sums[kColVec + 3];
+          sS->dd = sums[kColVec + 1]; sS->xx = sums[kColVec + 2];
           ls_begin(sS->ls, sS->t_cur, sS->loss, (float)sums[kColVec], (float)sums[kColVec + 3]);
           sS->ls_active = 1;
         }
@@ -1364,7 +775,7 @@ __device__ void step_head_body(SolverState* __restrict__ S, const double* __rest
         else next = PH_MAT;
       }
       if (end_of_iteration) {
-        iter_end_body(sS, 0);
+        iter_end_body(sS);
         next = sS->need_fresh ? PH_FRESH : PH_DIR;
         if (sS->active && sS->iter >= sS->iter_limit) { sS->active = 0; sS->paused = 1; }
       }
@@ -1615,10 +1026,10 @@ step_head_kernel(SolverState* __restrict__ S, const float* __restrict__ g, const
       if (lane == 4) o[kHeadCols - 1] = 0.0;
     }
   }
-  if (last_block_done(&S->tickets[0])) step_head_body(S, part, gridDim.x, tl, raw, t, count, t_entry);
+  if (last_block_done(&S->ticket)) step_head_body(S, part, gridDim.x, tl, raw, t, count, t_entry);
 }
 
-// the vector kernel of a late-epilogue step (see above).  `gz` is the buffer the scatter kernel adds into: g itself
+// the vector kernel of a step (see above).  `gz` is the buffer the scatter kernel adds into: g itself
 // on one GPU (zeroed AFTER this thread has read its elements), the peer-visible partial buffer on several.
 __global__ void __launch_bounds__(kVecThreads)
 step_vec_kernel(SolverState* __restrict__ S, const float* g, float* __restrict__ gprev, float* __restrict__ d,
@@ -1719,7 +1130,7 @@ step_vec_kernel(SolverState* __restrict__ S, const float* g, float* __restrict__
   }
 }
 
-// mode 2: (re)arm the solver for iterations up to `limit`
+// (re)arm the solver for iterations up to `limit`
 __global__ void resume_kernel(SolverState* __restrict__ S, int limit) {
   if (threadIdx.x != 0) return;
   S->iter_limit = limit;
@@ -1728,61 +1139,19 @@ __global__ void resume_kernel(SolverState* __restrict__ S, int limit) {
   set_phase(S, S->phase);
 }
 
-// mode 2: the axpy of a step.  PH_DIR / PH_TRIAL: trial point x_init + t d (and g = 0 for the scatter that
-// follows); PH_MAT: accepted point x_init + t_accept d; PH_FRESH: only g = 0.  Centered with m in {1,2,4}
-// is applied on the fly like trial_axpy_kernel.
-__global__ void __launch_bounds__(kVecThreads)
-step_axpy_kernel(SolverState* __restrict__ S, const float* __restrict__ xinit, const float* __restrict__ d,
-                 float* __restrict__ X, int64_t npad, int64_t nvalid, int center_m, float* __restrict__ gz,
-                 const Comm* __restrict__ comm) {
-  if (off(&S->active)) return;
-  const bool mat = S->g_mat != 0;
-  if (comm != nullptr && !mat) comm_wait_readers_fwd(comm, &S->error);  // gz is the peer-visible partial buffer
-  const bool move = S->g_proj != 0;  // every phase but PH_FRESH
-  if (move && !mat && off(&S->ls_active)) return;
-  const float t = mat ? (float)S->ls.t_accept : (float)S->ls.t;
-  float mu[4] = {0.f, 0.f, 0.f, 0.f};
-  if (center_m == 1) { float v = S->mu_x[0] + t * S->mu_d[0]; mu[0] = mu[1] = mu[2] = mu[3] = v; }
-  else if (center_m == 2) {
-    float v0 = S->mu_x[0] + t * S->mu_d[0], v1 = S->mu_x[1] + t * S->mu_d[1];
-    mu[0] = mu[2] = v0; mu[1] = mu[3] = v1;
-  } else if (center_m == 4) {
-#pragma unroll
-    for (int c = 0; c < 4; ++c) mu[c] = S->mu_x[c] + t * S->mu_d[c];
-  }
-  const int64_t n4 = npad >> 2;
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4 + 1; i += stride) {
-    if (move && i < n4) {
-      float4 A = reinterpret_cast<const float4*>(xinit)[i];
-      float4 D = reinterpret_cast<const float4*>(d)[i];
-      float4 R = make_float4(fmaf(t, D.x, A.x) - mu[0], fmaf(t, D.y, A.y) - mu[1], fmaf(t, D.z, A.z) - mu[2],
-                             fmaf(t, D.w, A.w) - mu[3]);
-      if (center_m != 0 && 4 * i + 3 >= nvalid) {  // keep the zero padding behind the last row
-        if (4 * i + 0 >= nvalid) R.x = 0.f;
-        if (4 * i + 1 >= nvalid) R.y = 0.f;
-        if (4 * i + 2 >= nvalid) R.z = 0.f;
-        if (4 * i + 3 >= nvalid) R.w = 0.f;
-      }
-      reinterpret_cast<float4*>(X)[i] = R;
-    }
-    if (!mat) reinterpret_cast<float4*>(gz)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
-}
-
 __global__ void init_state_kernel(SolverState* S, double eps, int memory, int max_stats, int world,
                                   double* avg, double* resid, double* pct, double* steplen) {
   if (threadIdx.x != 0) return;
   S->active = 1; S->converged = 0; S->iter = 0; S->error = 0; S->need_fresh = 1; S->ls_active = 0;
-  S->stop_after = 0; S->pad0 = 0; S->eps = eps; S->loss = 0.0; S->gg = 0.0; S->g1 = 0.0; S->gtd = 0.0f;
-  S->dmax = 0.0f; S->dd = 0.0; S->xx = 0.0; S->t_last = 0.0; S->t_eval = 0.0; S->func_evals = 0;
+  S->stop_after = 0; S->pad0 = 0; S->eps = eps; S->loss = 0.0; S->gg = 0.0; S->g1 = 0.0;
+  S->dd = 0.0; S->xx = 0.0; S->t_last = 0.0; S->t_eval = 0.0; S->func_evals = 0;
   S->max_stats = max_stats; S->world = world;
   S->paused = 0; S->iter_limit = max_stats; S->pend = 0;
   S->t_cur = 0.0;
   for (int c = 0; c < 4; ++c) { S->cs_g[c] = 0.0; S->cs_d[c] = 0.0; S->mu_x[c] = 0.0f; S->mu_d[c] = 0.0f; }
   for (int q = 0; q < kSlots; ++q) for (int c = 0; c < 4; ++c) { S->cs_S[q][c] = 0.0; S->cs_Y[q][c] = 0.0; }
-  set_phase(S, PH_FRESH);  // mode 2 (sets need_fresh = 1 as well)
-  for (int k = 0; k < 4; ++k) S->tickets[k] = 0u;
+  set_phase(S, PH_FRESH);  // (sets need_fresh = 1 as well)
+  S->ticket = 0u;
   S->avg = avg; S->resid = resid; S->pct = pct; S->steplen = steplen;
   lbfgs_reset(S->lb, memory);
   ls_begin(S->ls, 0.0, 0.0, 0.0f, 0.0f);
@@ -1807,19 +1176,16 @@ struct mde_solver {
   SolverState* S = nullptr;          // device
   int* status_host = nullptr;        // pinned, kStatusInts ints
   float *X = nullptr, *xinit = nullptr, *d = nullptr, *g = nullptr, *gprev = nullptr, *Sb = nullptr, *Yb = nullptr;
-  float* gpart = nullptr;            // mode 2, multi-GPU: this rank's partial [gradient | loss] before the all-reduce
-  double *dpart = nullptr;           // dot partials
-  double *vpart = nullptr;           // late-epilogue steps: (g.d, d.d, X.X, max|d|) partials of the vec kernel
+  float* gpart = nullptr;            // multi-GPU: this rank's partial [gradient | loss] before the all-reduce
+  double *dpart = nullptr;           // partial rows of the head kernel
+  double *vpart = nullptr;           // (g.d, d.d, X.X, max|d|) partials of the vec kernel
   double *stats = nullptr;           // 4 * max_iter doubles
   void* projws = nullptr;
   ProjWs pw{};
-  int fuse = 1;                      // scalar epilogues run in the last block of the vector kernels
-  int center_m = 0;                  // {1,2,4}: Centered projection fused into the trial axpy
+  int center_m = 0;                  // {1,2,4}: Centered projection fused into the vec kernel
   int nl = 0;                        // loss-partial blocks of the distortion launch
   int nvb = 0;                       // vector-pass blocks
-  int host_need_fresh = 1;
   int host_active = 0;
-  int host_evals = 0;                // func_evals already accounted in the launch counter (mode 1)
   mde_allreduce_fn allreduce = nullptr;
   void* allreduce_user = nullptr;
   // peer-memory all-reduce (world_size > 1): one cudaMalloc region [partial buffer | flags | epoch | ticket],
@@ -1833,24 +1199,14 @@ struct mde_solver {
   void* peer_base[kMaxWorld] = {nullptr};
   int64_t* anchors = nullptr;
   float* anchor_values = nullptr;
-  // mode 1: one CUDA graph per iteration with an IF node (fresh evaluation) and a WHILE node (trials)
-  cudaGraph_t graph = nullptr;
-  cudaGraphExec_t graph_exec = nullptr;
-  // the same iteration chained `unroll` times in one graph: one graph launch per `unroll` iterations
-  cudaGraph_t graph_u = nullptr;
-  cudaGraphExec_t graph_exec_u = nullptr;
-  int unroll = 1;
-  // mode 2: flat step graphs (one step / steps_per_graph steps), no conditional nodes
+  // flat step graphs (one step / steps_per_graph steps), no conditional nodes
   int steps_per_graph = 8;           // MDE_B200_STEPS (1..64)
-  int late = 0;                      // mode 2: evaluation bookkeeping rides in the next step's head kernel (MDE_B200_LATE=0: off)
   cudaGraph_t step_graph = nullptr, steps_graph = nullptr;
   cudaGraphExec_t step_exec = nullptr, steps_exec = nullptr;
   int step_kernels = 0;              // kernel nodes per step
   int host_iter = 0;                 // iterations completed (last status read)
   int cur_max_iter = 0;              // iteration cap of the current solve (<= opts.max_iter)
-  cudaStream_t cap_stream = nullptr, cap_stream2 = nullptr;
-  cudaGraphConditionalHandle h_if = 0, h_while = 0, h_if_next = 0;  // capture-time only
-  int graph_kernels_fixed = 0, graph_kernels_trial = 0, graph_kernels_fresh = 0;
+  cudaStream_t cap_stream = nullptr;
 };
 
 namespace {
@@ -1861,46 +1217,12 @@ int read_status(mde_solver* s, cudaStream_t st) {
   return 0;
 }
 
-// project the iterate onto the constraint set (project_callback, lbfgs.py:368-372)
-int enqueue_project(mde_solver* s, cudaStream_t st) {
-  const int* act = &s->S->active;
-  switch (s->opts.constraint) {
-    case MDE_CONSTRAINT_CENTERED:
-      if (s->center_m) return 0;  // already applied by trial_axpy_kernel
-      return enqueue_project_centered(s->X, s->n, s->m, s->pw, act, st);
-    case MDE_CONSTRAINT_STANDARDIZED: return enqueue_project_standardized(s->X, s->n, s->m, s->pw, act, st);
-    case MDE_CONSTRAINT_ANCHORED: {
-      int64_t tot = s->opts.n_anchors * s->m;
-      if (tot > 0) {
-        anchor_rows_kernel<<<(int)((tot + 255) / 256), 256, 0, st>>>(act, s->X, s->anchors, s->anchor_values,
-                                                                    s->opts.n_anchors, s->m);
-        MDE_LAUNCH_CHECK();
-      }
-      return 0;
-    }
-  }
-  return MDE_E_INVALID;
-}
-
-// closure: value_and_grad at s->X (optim.py:100-105); `flag` gates the kernels
-Tail make_tail(mde_solver* s, int mode) {
-  Tail tl;
-  tl.fuse = s->fuse; tl.mode = mode;
-  tl.lpart = loss_partials_ptr(s->edges); tl.nl = s->nl; tl.tail = s->g + s->npad;
-  tl.p_total = (double)edges_p_total(s->edges); tl.n_rows = s->n; tl.inv_n = 1.0 / (double)s->n; tl.h_while = s->h_while;
-  return tl;
-}
-
-int enqueue_eval(mde_solver* s, const int* flag, bool zero_g, int tail_mode, cudaStream_t st, bool with_dots = true) {
+// closure: value_and_grad at s->X (optim.py:100-105) into the gradient buffer the vec kernel zeroed; `flag` gates
+// the kernels.  (g.d, g.g, |g|_1) and the loss are reduced by the next step's head kernel.
+int enqueue_eval(mde_solver* s, const int* flag, cudaStream_t st) {
   // several GPUs: scatter into this rank's partial buffer (peer-visible), then all-reduce into g
   const bool multi = s->opts.world_size > 1;
-  const bool staged = multi && s->opts.mode == 2;  // (the peer-memory path exists in mode 2 only)
-  float* target = staged ? s->gpart : s->g;
-  if (zero_g) {
-    const int64_t n4 = (s->npad + 4) >> 2;  // gradient + (hi, lo) tail
-    zero_kernel<<<vec_blocks(n4), kVecThreads, 0, st>>>(flag, target, n4);
-    MDE_LAUNCH_CHECK();
-  }
+  float* target = multi ? s->gpart : s->g;
   int rc = distortion_fused_flag(s->edges, s->X, s->m, target, &s->nl, flag, st);
   if (rc) return rc;
   if (multi) {
@@ -1932,11 +1254,9 @@ int enqueue_eval(mde_solver* s, const int* flag, bool zero_g, int tail_mode, cud
       if (!s->allreduce) return MDE_E_INVALID;
       rc = s->allreduce(s->allreduce_user, target, s->npad + 4, (void*)st);
       if (rc) return rc;
-      if (staged) {
-        const int64_t n4 = (s->npad + 4) >> 2;
-        gated_copy_kernel<<<vec_blocks(n4), kVecThreads, 0, st>>>(flag, s->gpart, s->g, n4);
-        MDE_LAUNCH_CHECK();
-      }
+      const int64_t n4 = (s->npad + 4) >> 2;
+      gated_copy_kernel<<<vec_blocks(n4), kVecThreads, 0, st>>>(flag, s->gpart, s->g, n4);
+      MDE_LAUNCH_CHECK();
     }
   }
   const int* act = flag;
@@ -1951,97 +1271,24 @@ int enqueue_eval(mde_solver* s, const int* flag, bool zero_g, int tail_mode, cud
       MDE_LAUNCH_CHECK();
     }
   }
-  if (!with_dots) return 0;  // late-epilogue steps: the next step's head kernel computes them
-  Tail tl = make_tail(s, tail_mode);
-  grad_dots_kernel<<<s->nvb, kVecThreads, 0, st>>>(flag, s->g, s->d, s->npad, s->dpart, s->S, tl);
-  MDE_LAUNCH_CHECK();
   return 0;
 }
 
-int enqueue_fresh(mde_solver* s, cudaStream_t st) {
-  int rc = enqueue_eval(s, &s->S->need_fresh, true, 2, st);
-  if (rc) return rc;
-  if (!s->fuse) {
-    fresh_finish_kernel<<<1, 256, 0, st>>>(s->S, loss_partials_ptr(s->edges), s->nl, s->g + s->npad, s->dpart,
-                                           s->nvb, (double)edges_p_total(s->edges));
-    MDE_LAUNCH_CHECK();
-  }
-  return 0;
-}
-
-int enqueue_direction(mde_solver* s, cudaStream_t st, const int* gate = nullptr) {
-  int slices = (s->opts.memory_size + kPairsPerSlice - 1) / kPairsPerSlice;
-  dim3 grid(s->nvb, slices);
-  Tail tl = make_tail(s, 0);
-  lbfgs_dots_kernel<<<grid, kVecThreads, 0, st>>>(s->S, s->g, s->gprev, s->d, s->Sb, s->Yb, s->npad, s->dpart, tl,
-                                                  gate);
-  MDE_LAUNCH_CHECK();
-  if (!s->fuse) {
-    direction_scalar_kernel<<<1, 256, 0, st>>>(s->S, s->dpart, s->nvb);
-    MDE_LAUNCH_CHECK();
-  }
-  direction_apply_kernel<<<s->nvb, kVecThreads, 0, st>>>(s->S, s->g, s->gprev, s->d, s->X, s->xinit, s->Sb,
-                                                         s->Yb, s->npad, s->dpart, s->center_m, tl, gate);
-  MDE_LAUNCH_CHECK();
-  if (!s->fuse) {
-    ls_init_kernel<<<1, 256, 0, st>>>(s->S, s->dpart, s->nvb, s->n, s->h_while);
-    MDE_LAUNCH_CHECK();
-  }
-  return 0;
-}
-
-int enqueue_trial(mde_solver* s, cudaStream_t st) {
-  trial_axpy_kernel<false><<<s->nvb, kVecThreads, 0, st>>>(s->S, s->xinit, s->d, s->X, s->npad, s->N, s->center_m, s->g, 0, 0);
-  MDE_LAUNCH_CHECK();
-  int rc = enqueue_project(s, st);
-  if (rc) return rc;
-  rc = enqueue_eval(s, &s->S->ls_active, false, 1, st);
-  if (rc) return rc;
-  if (!s->fuse) {
-    ls_update_kernel<<<1, 256, 0, st>>>(s->S, loss_partials_ptr(s->edges), s->nl, s->g + s->npad, s->dpart, s->nvb,
-                                        (double)edges_p_total(s->edges), s->h_while);
-    MDE_LAUNCH_CHECK();
-  }
-  return 0;
-}
-
-int enqueue_finish(mde_solver* s, cudaStream_t st) {
-  // iter_end may ride in the axpy's last block only when no projection kernel follows (it can clear `active`)
-  const int fuse_end = (s->fuse && s->opts.constraint == MDE_CONSTRAINT_CENTERED && s->center_m) ? 1 : 0;
-  trial_axpy_kernel<true><<<s->nvb, kVecThreads, 0, st>>>(s->S, s->xinit, s->d, s->X, s->npad, s->N, s->center_m,
-                                                          nullptr, fuse_end, s->h_if_next);
-  MDE_LAUNCH_CHECK();
-  int rc = enqueue_project(s, st);
-  if (rc) return rc;
-  if (!fuse_end) {
-    iter_end_kernel<<<1, 32, 0, st>>>(s->S, s->h_if_next);
-    MDE_LAUNCH_CHECK();
-  }
-  return 0;
-}
-
-// mode 2: one step (see step_end_body).  Every kernel is gated on the device; the chain has no host decision.
+// one step (see the phase machine above).  Every kernel is gated on the device; the chain has no host decision.
 int enqueue_step(mde_solver* s, cudaStream_t st) {
   SolverState* S = s->S;
   int rc = 0;
-  if (s->late) {
-    int slices = (s->opts.memory_size + kPairsPerSlice - 1) / kPairsPerSlice;
-    dim3 grid(s->nvb, slices);
-    Tail tl = make_tail(s, 3);
-    step_head_kernel<<<grid, kVecThreads, 0, st>>>(S, s->g, s->gprev, s->d, s->X, s->Sb, s->Yb, s->npad, s->center_m,
-                                                   s->dpart, s->vpart, tl);
-    MDE_LAUNCH_CHECK();
-    step_vec_kernel<<<s->nvb, kVecThreads, 0, st>>>(S, s->g, s->gprev, s->d, s->X, s->xinit, s->Sb, s->Yb, s->npad,
-                                                    s->N, s->center_m, s->opts.world_size > 1 ? s->gpart : s->g,
-                                                    s->comm_connected ? s->comm_dev : nullptr, s->vpart);
-    MDE_LAUNCH_CHECK();
-  } else {
-    if ((rc = enqueue_direction(s, st, &S->g_dir))) return rc;
-    step_axpy_kernel<<<s->nvb, kVecThreads, 0, st>>>(S, s->xinit, s->d, s->X, s->npad, s->N, s->center_m,
-                                                     s->opts.world_size > 1 ? s->gpart : s->g,
-                                                     s->comm_connected ? s->comm_dev : nullptr);
-    MDE_LAUNCH_CHECK();
-  }
+  const int slices = (s->opts.memory_size + kPairsPerSlice - 1) / kPairsPerSlice;
+  Tail tl;
+  tl.lpart = loss_partials_ptr(s->edges); tl.nl = s->nl; tl.tail = s->g + s->npad;
+  tl.p_total = (double)edges_p_total(s->edges); tl.inv_n = 1.0 / (double)s->n;
+  step_head_kernel<<<dim3(s->nvb, slices), kVecThreads, 0, st>>>(S, s->g, s->gprev, s->d, s->X, s->Sb, s->Yb, s->npad,
+                                                                 s->center_m, s->dpart, s->vpart, tl);
+  MDE_LAUNCH_CHECK();
+  step_vec_kernel<<<s->nvb, kVecThreads, 0, st>>>(S, s->g, s->gprev, s->d, s->X, s->xinit, s->Sb, s->Yb, s->npad,
+                                                  s->N, s->center_m, s->opts.world_size > 1 ? s->gpart : s->g,
+                                                  s->comm_connected ? s->comm_dev : nullptr, s->vpart);
+  MDE_LAUNCH_CHECK();
   switch (s->opts.constraint) {  // retraction of the moved iterate (project_callback, lbfgs.py:368-372)
     case MDE_CONSTRAINT_CENTERED:
       if (!s->center_m && (rc = enqueue_project_centered(s->X, s->n, s->m, s->pw, &S->g_proj, st))) return rc;
@@ -2060,14 +1307,14 @@ int enqueue_step(mde_solver* s, cudaStream_t st) {
     }
     default: return MDE_E_INVALID;
   }
-  return enqueue_eval(s, &S->g_eval, false, 3, st, !s->late);
+  return enqueue_eval(s, &S->g_eval, st);
 }
 
 int build_step_graph(mde_solver* s, int steps, cudaGraph_t* graph_out, cudaGraphExec_t* exec_out) {
 #define GTRY(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) return (int)_e; } while (0)
   if (!s->cap_stream) GTRY(cudaStreamCreateWithFlags(&s->cap_stream, cudaStreamNonBlocking));
   const unsigned long long l0 = g_launch_count;
-  if (s->late && s->nl == 0) {
+  if (s->nl == 0) {
     // the head kernel of a step reads the loss partials of the PREVIOUS step's scatter launch: their count is
     // known once one evaluation has been enqueued, so capture one throw-away step first
     cudaGraph_t tmp = nullptr;
@@ -2092,90 +1339,6 @@ int build_step_graph(mde_solver* s, int steps, cudaGraph_t* graph_out, cudaGraph
 #undef GTRY
 }
 
-// One iteration as a CUDA graph:
-//   fresh_gate -> IF(need_fresh){ evaluate at X } -> direction (P1,S1,P2,S2) -> WHILE(ls_active){ trial }
-//   -> accepted step + projection + iter_end.
-// The conditional handles are written on the device (cudaGraphSetConditional), so the host never reads
-// a scalar during an iteration.
-int build_iteration_graph(mde_solver* s, int copies, cudaGraph_t* graph_out, cudaGraphExec_t* exec_out) {
-#define GTRY(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) return (int)_e; } while (0)
-  if (!s->cap_stream) GTRY(cudaStreamCreateWithFlags(&s->cap_stream, cudaStreamNonBlocking));
-  if (!s->cap_stream2) GTRY(cudaStreamCreateWithFlags(&s->cap_stream2, cudaStreamNonBlocking));
-  cudaStream_t st = s->cap_stream, st2 = s->cap_stream2;
-  cudaStreamCaptureStatus cs;
-  cudaGraph_t cg = nullptr;
-  const cudaGraphNode_t* deps = nullptr;
-  size_t nd = 0;
-  int rc;
-  const unsigned long long l0 = g_launch_count;
-  GTRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeRelaxed));
-  // every conditional node owns its handles (default 0 at each graph launch); the kernels enqueued
-  // below capture them by value
-  cudaGraphConditionalHandle hif[8], hwh[8];
-  GTRY(cudaStreamGetCaptureInfo_v2(st, &cs, nullptr, &cg, &deps, &nd));
-  for (int copy = 0; copy < copies; ++copy) {
-    GTRY(cudaGraphConditionalHandleCreate(&hif[copy], cg, 0, cudaGraphCondAssignDefault));
-    GTRY(cudaGraphConditionalHandleCreate(&hwh[copy], cg, 0, cudaGraphCondAssignDefault));
-  }
-  for (int copy = 0; copy < copies; ++copy) {
-  s->h_if = hif[copy]; s->h_while = hwh[copy];
-  s->h_if_next = (copy + 1 < copies) ? hif[copy + 1] : 0;
-  if (copy == 0) {  // later copies: the gate is set by the previous copy's iter_end
-    fresh_gate_kernel<<<1, 32, 0, st>>>(s->S, s->h_if);
-    ++g_launch_count;
-    GTRY(cudaPeekAtLastError());
-  }
-  {  // IF node: closure() at the current iterate when lbfgs n_iter == 0
-    GTRY(cudaStreamGetCaptureInfo_v2(st, &cs, nullptr, &cg, &deps, &nd));
-    cudaGraphNodeParams np = {};
-    np.type = cudaGraphNodeTypeConditional;
-    np.conditional.handle = s->h_if;
-    np.conditional.type = cudaGraphCondTypeIf;
-    np.conditional.size = 1;
-    cudaGraphNode_t node;
-    GTRY(cudaGraphAddNode(&node, cg, deps, nd, &np));
-    cudaGraph_t body = np.conditional.phGraph_out[0];
-    GTRY(cudaStreamBeginCaptureToGraph(st2, body, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed));
-    const unsigned long long a = g_launch_count;
-    rc = enqueue_fresh(s, st2);
-    s->graph_kernels_fresh = (int)(g_launch_count - a);
-    cudaError_t e = cudaStreamEndCapture(st2, nullptr);
-    if (rc) return rc;
-    GTRY(e);
-    GTRY(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));
-  }
-  if ((rc = enqueue_direction(s, st))) return rc;
-  {  // WHILE node: line-search trials
-    GTRY(cudaStreamGetCaptureInfo_v2(st, &cs, nullptr, &cg, &deps, &nd));
-    cudaGraphNodeParams np = {};
-    np.type = cudaGraphNodeTypeConditional;
-    np.conditional.handle = s->h_while;
-    np.conditional.type = cudaGraphCondTypeWhile;
-    np.conditional.size = 1;
-    cudaGraphNode_t node;
-    GTRY(cudaGraphAddNode(&node, cg, deps, nd, &np));
-    cudaGraph_t body = np.conditional.phGraph_out[0];
-    GTRY(cudaStreamBeginCaptureToGraph(st2, body, nullptr, nullptr, 0, cudaStreamCaptureModeRelaxed));
-    const unsigned long long a = g_launch_count;
-    rc = enqueue_trial(s, st2);
-    s->graph_kernels_trial = (int)(g_launch_count - a);
-    cudaError_t e = cudaStreamEndCapture(st2, nullptr);
-    if (rc) return rc;
-    GTRY(e);
-    GTRY(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));
-  }
-  if ((rc = enqueue_finish(s, st))) return rc;
-  }  // copies
-  GTRY(cudaStreamEndCapture(st, graph_out));
-  GTRY(cudaGraphInstantiate(exec_out, *graph_out, 0));
-  s->h_if = s->h_while = s->h_if_next = 0;
-  if (copies == 1)  // kernels of one iteration outside the conditional bodies (gate included)
-    s->graph_kernels_fixed = (int)(g_launch_count - l0) - s->graph_kernels_trial - s->graph_kernels_fresh;
-  g_launch_count = l0;  // capture enqueued nothing; launches are counted per graph launch
-  return 0;
-#undef GTRY
-}
-
 }  // namespace
 
 extern "C" {
@@ -2187,8 +1350,8 @@ int mde_solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m
   if (opts->constraint == MDE_CONSTRAINT_STANDARDIZED && m > kWideMaxM) return MDE_E_UNSUPPORTED;
   if (opts->constraint < 0 || opts->constraint > MDE_CONSTRAINT_ANCHORED) return MDE_E_INVALID;
   if (opts->max_iter < 1) return MDE_E_INVALID;
-  if (opts->mode < 0 || opts->mode > 2) return MDE_E_INVALID;
-  if (opts->mode == 1 && opts->world_size > 1) return MDE_E_UNSUPPORTED;  // the NCCL hook is called from the host
+  if (opts->mode == 0 || opts->mode == 1) return MDE_E_UNSUPPORTED;  // retired drivers (host-stepped, conditional graph)
+  if (opts->mode != 2) return MDE_E_INVALID;
   if (n != edges_n(e)) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   mde_solver* s = new (std::nothrow) mde_solver();
@@ -2247,14 +1410,7 @@ int mde_solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m
   }
   s->nvb = vec_blocks(s->npad >> 2);
   if (opts->constraint == MDE_CONSTRAINT_CENTERED && (m == 1 || m == 2 || m == 4)) s->center_m = m;
-  { const char* ev = getenv("MDE_B200_FUSE"); if (ev && ev[0] == '0') s->fuse = 0; }
-  if (opts->mode == 2) {
-    s->fuse = 1;  // the phase machine lives in the fused epilogues
-    s->late = 1;
-    const char* ev = getenv("MDE_B200_LATE");
-    if (ev && ev[0] == '0') s->late = 0;
-  }
-  if (opts->mode == 2 && opts->world_size == 1) {  // several GPUs: graphs are built by mde_solver_comm_connect
+  if (opts->world_size == 1) {  // several GPUs: graphs are built by mde_solver_comm_connect
     s->nl = 0;
     TRY(cudaStreamSynchronize(st));
     rc = build_step_graph(s, 1, &s->step_graph, &s->step_exec);
@@ -2264,19 +1420,6 @@ int mde_solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m
     if (s->steps_per_graph > 64) s->steps_per_graph = 64;
     rc = build_step_graph(s, s->steps_per_graph, &s->steps_graph, &s->steps_exec);
     if (rc) goto fail;
-  }
-  if (opts->mode == 1) {
-    s->nl = 0;
-    TRY(cudaStreamSynchronize(st));
-    rc = build_iteration_graph(s, 1, &s->graph, &s->graph_exec);
-    if (rc) goto fail;
-    { const char* ev = getenv("MDE_B200_UNROLL"); if (ev) s->unroll = atoi(ev); }
-    if (s->unroll < 1) s->unroll = 1;
-    if (s->unroll > 8) s->unroll = 8;
-    if (s->unroll > 1) {
-      rc = build_iteration_graph(s, s->unroll, &s->graph_u, &s->graph_exec_u);
-      if (rc) goto fail;
-    }
   }
   *out = s;
   return 0;
@@ -2295,16 +1438,11 @@ int mde_solver_destroy(mde_solver_t* s) {
   cudaFree(s->comm_region); cudaFree(s->comm_dev);
   cudaFree(s->Sb); cudaFree(s->Yb); cudaFree(s->dpart); cudaFree(s->vpart); cudaFree(s->stats); cudaFree(s->projws);
   cudaFree(s->anchors); cudaFree(s->anchor_values);
-  if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
-  if (s->graph) cudaGraphDestroy(s->graph);
   if (s->step_exec) cudaGraphExecDestroy(s->step_exec);
   if (s->step_graph) cudaGraphDestroy(s->step_graph);
   if (s->steps_exec) cudaGraphExecDestroy(s->steps_exec);
   if (s->steps_graph) cudaGraphDestroy(s->steps_graph);
-  if (s->graph_exec_u) cudaGraphExecDestroy(s->graph_exec_u);
-  if (s->graph_u) cudaGraphDestroy(s->graph_u);
   if (s->cap_stream) cudaStreamDestroy(s->cap_stream);
-  if (s->cap_stream2) cudaStreamDestroy(s->cap_stream2);
   delete s;
   return 0;
 }
@@ -2328,7 +1466,6 @@ int mde_solver_comm_connect(mde_solver_t* s, int rank, const void* handles, int6
       handle_stride < (int64_t)sizeof(cudaIpcMemHandle_t))
     return MDE_E_INVALID;
   if (s->comm_connected) return MDE_E_INVALID;
-  if (s->opts.mode != 2) return MDE_E_UNSUPPORTED;  // host-stepped modes keep the host hook
   cudaStream_t st = (cudaStream_t)stream;
   const int W = s->opts.world_size;
   Comm c{};
@@ -2363,17 +1500,14 @@ int mde_solver_comm_connect(mde_solver_t* s, int rank, const void* handles, int6
   MDE_CUDA_TRY(cudaMemcpyAsync(s->comm_dev, &s->comm, sizeof(Comm), cudaMemcpyHostToDevice, st));
   MDE_CUDA_TRY(cudaStreamSynchronize(st));
   s->comm_connected = 1;
-  if (s->opts.mode == 2) {  // the sharded solve runs the same flat step graphs as one GPU
-    s->nl = 0;
-    int rc = build_step_graph(s, 1, &s->step_graph, &s->step_exec);
-    if (rc) return rc;
-    { const char* ev = getenv("MDE_B200_STEPS"); if (ev) s->steps_per_graph = atoi(ev); }
-    if (s->steps_per_graph < 1) s->steps_per_graph = 1;
-    if (s->steps_per_graph > 64) s->steps_per_graph = 64;
-    rc = build_step_graph(s, s->steps_per_graph, &s->steps_graph, &s->steps_exec);
-    if (rc) return rc;
-  }
-  return 0;
+  // the sharded solve runs the same flat step graphs as one GPU
+  s->nl = 0;
+  int rc = build_step_graph(s, 1, &s->step_graph, &s->step_exec);
+  if (rc) return rc;
+  { const char* ev = getenv("MDE_B200_STEPS"); if (ev) s->steps_per_graph = atoi(ev); }
+  if (s->steps_per_graph < 1) s->steps_per_graph = 1;
+  if (s->steps_per_graph > 64) s->steps_per_graph = 64;
+  return build_step_graph(s, s->steps_per_graph, &s->steps_graph, &s->steps_exec);
 }
 
 int mde_solver_begin(mde_solver_t* s, const float* X0, double eps, void* stream) {
@@ -2390,14 +1524,12 @@ int mde_solver_begin_ex(mde_solver_t* s, const float* X0, double eps, int max_it
   init_state_kernel<<<1, 32, 0, st>>>(s->S, eps, s->opts.memory_size, max_iter, s->opts.world_size, s->stats,
                                       s->stats + mi, s->stats + 2 * mi, s->stats + 3 * mi);
   MDE_LAUNCH_CHECK();
-  s->host_need_fresh = 1;
   s->host_active = 1;
-  s->host_evals = 0;
   s->host_iter = 0;
   return 0;
 }
 
-// globaltimer stamps (ns) of the last late-epilogue head kernel that started an iteration: [0] last block's entry,
+// globaltimer stamps (ns) of the last head kernel that started an iteration: [0] last block's entry,
 // [1] epilogue entry, [2] state staged, [3] partials reduced, [4] previous step finished, [5] direction done,
 // [6] before write-back, [7] the vec kernel's first block.  Diagnostics only (tools/solver_times.py).
 int mde_solver_debug_times(mde_solver_t* s, unsigned long long* out8, void* stream) {
@@ -2411,95 +1543,49 @@ int mde_solver_run(mde_solver_t* s, int iters, int* iters_done, int* converged, 
   if (!s) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   int rc = 0;
-  if (s->opts.mode == 2) {
-    // flat step graphs: the device pauses itself at `target`; the host only keeps the queue fed.  A step is
-    // one closure evaluation, an iteration takes >= 1 of them, so launching `remaining` steps never overshoots
-    // by more than the gated (early-exit) kernels of the surplus steps.
-    if (!s->host_active || iters <= 0) {
-      if ((rc = read_status(s, st))) return rc;
-      if (iters_done) *iters_done = s->status_host[2];
-      if (converged) *converged = s->status_host[1];
-      return 0;
-    }
-    int target = s->host_iter + iters;
-    if (target > s->cur_max_iter) target = s->cur_max_iter;
-    resume_kernel<<<1, 32, 0, st>>>(s->S, target);
-    MDE_LAUNCH_CHECK();
-    for (int round = 0;; ++round) {
-      if (round > (1 << 18)) return MDE_E_INVALID;
-      int remaining = target - s->host_iter;
-      if (remaining < 1) remaining = 1;
-      long long steps = 0;
-      const int spg = s->steps_per_graph;
-      if (s->opts.world_size > 1 && !s->steps_exec) {
-        // host-hook all-reduce: stream-launched steps; every rank enqueues the same number of steps (same `remaining`: the replicated state machines agree)
-        int n_steps = remaining + remaining / 8 + (round > 0 ? 1 : 0) + s->late;
-        if (n_steps > 64) n_steps = 64;
-        for (int b = 0; b < n_steps; ++b) { if ((rc = enqueue_step(s, st))) return rc; }
-      } else if (remaining >= spg) {
-        int graphs = (remaining + remaining / 8 + s->late) / spg;
-        if (graphs * spg > 96) graphs = 96 / spg > 0 ? 96 / spg : 1;  // <= ~96 steps in flight per status read
-        for (int b = 0; b < graphs; ++b) MDE_CUDA_TRY(cudaGraphLaunch(s->steps_exec, st));
-        steps = (long long)graphs * spg;
-      } else {
-        const int singles = remaining + remaining / 4 + (round > 0 ? 1 : 0) + s->late;
-        for (int b = 0; b < singles; ++b) MDE_CUDA_TRY(cudaGraphLaunch(s->step_exec, st));
-        steps = singles;
-      }
-      g_launch_count += (unsigned long long)steps * s->step_kernels;  // (stream-launched steps count themselves)
-      if ((rc = read_status(s, st))) return rc;
-      s->host_iter = s->status_host[2];
-      if (s->status_host[3]) { s->host_active = 0; if (iters_done) *iters_done = s->status_host[2]; return s->status_host[3]; }
-      if (!s->status_host[0]) {              // paused at the target, converged, or out of iterations
-        s->host_active = s->status_host[8];  // only a pause can be resumed
-        break;
-      }
-    }
-    if (iters_done) *iters_done = s->status_host[2];
-    if (converged) *converged = s->status_host[1];
-    return 0;
-  }
-  if (s->opts.mode == 1) {
-    // device-driven: one graph launch per iteration, status read back once per batch.  Launches
-    // after convergence are no-ops (every kernel checks the device-side `active` flag).
-    int left = iters;
-    while (left > 0 && s->host_active) {
-      const int batch = left < 16 ? left : 16;
-      int b = 0, chained = 0;
-      for (; s->unroll > 1 && b + s->unroll <= batch; b += s->unroll, ++chained)
-        MDE_CUDA_TRY(cudaGraphLaunch(s->graph_exec_u, st));
-      for (; b < batch; ++b) MDE_CUDA_TRY(cudaGraphLaunch(s->graph_exec, st));
-      left -= batch;
-      if ((rc = read_status(s, st))) return rc;
-      s->host_active = s->status_host[0];
-      // kernels executed by the graphs: fixed part per launch + one trial body per evaluation
-      g_launch_count += (unsigned long long)batch * s->graph_kernels_fixed +
-                        (unsigned long long)(s->status_host[7] - s->host_evals) * s->graph_kernels_trial;
-      g_launch_count -= (unsigned long long)chained * (s->unroll - 1);  // chained copies carry no gate kernel
-      s->host_evals = s->status_host[7];
-      if (s->status_host[3]) { if (iters_done) *iters_done = s->status_host[2]; return s->status_host[3]; }
-    }
+  // flat step graphs: the device pauses itself at `target`; the host only keeps the queue fed.  A step is
+  // one closure evaluation, an iteration takes >= 1 of them, so launching `remaining` steps never overshoots
+  // by more than the gated (early-exit) kernels of the surplus steps.
+  if (!s->host_active || iters <= 0) {
     if ((rc = read_status(s, st))) return rc;
     if (iters_done) *iters_done = s->status_host[2];
     if (converged) *converged = s->status_host[1];
     return 0;
   }
-  for (int it = 0; it < iters && s->host_active; ++it) {
-    if (s->host_need_fresh) { if ((rc = enqueue_fresh(s, st))) return rc; }
-    if ((rc = enqueue_direction(s, st))) return rc;
-    for (int trial = 0;; ++trial) {  // <= 10 back-offs + 25 search steps + ~85 fallback steps
-      if (trial > 256) return MDE_E_INVALID;
-      if ((rc = enqueue_trial(s, st))) return rc;
-      if ((rc = read_status(s, st))) return rc;
-      if (!s->status_host[5] || !s->status_host[0]) break;  // ls_active / active
+  int target = s->host_iter + iters;
+  if (target > s->cur_max_iter) target = s->cur_max_iter;
+  resume_kernel<<<1, 32, 0, st>>>(s->S, target);
+  MDE_LAUNCH_CHECK();
+  for (int round = 0;; ++round) {
+    if (round > (1 << 18)) return MDE_E_INVALID;
+    int remaining = target - s->host_iter;
+    if (remaining < 1) remaining = 1;
+    long long steps = 0;
+    const int spg = s->steps_per_graph;
+    if (s->opts.world_size > 1 && !s->steps_exec) {
+      // host-hook all-reduce: stream-launched steps; every rank enqueues the same number of steps (same `remaining`: the replicated state machines agree)
+      int n_steps = remaining + remaining / 8 + (round > 0 ? 1 : 0) + 1;
+      if (n_steps > 64) n_steps = 64;
+      for (int b = 0; b < n_steps; ++b) { if ((rc = enqueue_step(s, st))) return rc; }
+    } else if (remaining >= spg) {
+      int graphs = (remaining + remaining / 8 + 1) / spg;
+      if (graphs * spg > 96) graphs = 96 / spg > 0 ? 96 / spg : 1;  // <= ~96 steps in flight per status read
+      for (int b = 0; b < graphs; ++b) MDE_CUDA_TRY(cudaGraphLaunch(s->steps_exec, st));
+      steps = (long long)graphs * spg;
+    } else {
+      const int singles = remaining + remaining / 4 + (round > 0 ? 1 : 0) + 1;
+      for (int b = 0; b < singles; ++b) MDE_CUDA_TRY(cudaGraphLaunch(s->step_exec, st));
+      steps = singles;
     }
+    g_launch_count += (unsigned long long)steps * s->step_kernels;  // (stream-launched steps count themselves)
+    if ((rc = read_status(s, st))) return rc;
+    s->host_iter = s->status_host[2];
     if (s->status_host[3]) { s->host_active = 0; if (iters_done) *iters_done = s->status_host[2]; return s->status_host[3]; }
-    if ((rc = enqueue_finish(s, st))) return rc;
-    if ((rc = read_status(s, st))) return rc;
-    s->host_need_fresh = s->status_host[4];
-    s->host_active = s->status_host[0];
+    if (!s->status_host[0]) {              // paused at the target, converged, or out of iterations
+      s->host_active = s->status_host[8];  // only a pause can be resumed
+      break;
+    }
   }
-  if ((rc = read_status(s, st))) return rc;
   if (iters_done) *iters_done = s->status_host[2];
   if (converged) *converged = s->status_host[1];
   return 0;

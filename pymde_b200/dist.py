@@ -7,11 +7,11 @@ every rank holds bit-identical gradient and loss, the device-resident L-BFGS sta
 replicated and (thanks to fixed-order reductions) takes identical decisions on every rank.
 
 Two transports for the solver's all-reduce:
-  * peer memory (default, mode 2): the library's own kernels sum the ranks' partial buffers over
+  * peer memory (default): the library's own kernels sum the ranks' partial buffers over
     NVLink (cudaIpc-mapped, flag handshake, rank-ordered sums) inside the same CUDA graph as the
     rest of the step.  `torch.distributed` is used ONCE, to exchange the 64-byte IPC handles.
   * host hook (`make_allreduce`): an NCCL all-reduce enqueued from Python between two kernels --
-    kept for host-stepped solver modes and as an A/B reference.
+    the transport used when no exchange function is given (ranks without cudaIpc peer access).
 Evaluations outside the solver (`MDE.average_distortion`, gradients through autograd) are
 all-reduced with `torch.distributed` so that a sharded MDE behaves like the global problem."""
 import os

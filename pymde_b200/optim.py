@@ -6,7 +6,6 @@ distortion function and constraint the CUDA path supports, the whole solve -- L-
 strong-Wolfe line search, projections, statistics -- runs device-resident through
 `mde_solver_*` (include/mde_b200.h); X is updated in place and returned."""
 import ctypes as C
-import os
 import time
 
 import numpy as np
@@ -41,18 +40,10 @@ class SolveStats(object):
         p.text(self.__str__())
 
 
-# 2 = flat CUDA graph of gated "steps" (one closure evaluation each; a device-side phase machine decides what
-# every kernel of the next step does, no conditional graph nodes, scalars never leave the device) -- default;
-# 1 = one CUDA graph per iteration with an IF node (fresh evaluation) and a WHILE node (line-search trials);
-# 0 = host-stepped line search (one status read per trial).  Edge-sharded multi-GPU solves use 0 (the NCCL
-# hook is called from the host).
-DEFAULT_MODE = int(os.environ.get("PYMDE_B200_SOLVER_MODE", "2"))
-
-
 class DeviceSolver(object):
     """Owner of one `mde_solver_t`."""
 
-    def __init__(self, layout, n, m, constraint, memory_size, max_iter, world_size=1, allreduce=None, mode=None,
+    def __init__(self, layout, n, m, constraint, memory_size, max_iter, world_size=1, allreduce=None,
                  exchange=None, rank=0):
         lib = _lib.load()
         self.lib = lib
@@ -63,11 +54,8 @@ class DeviceSolver(object):
         opts.constraint = int(constraint._solver_id)
         opts.memory_size = int(memory_size)
         opts.max_iter = max(int(max_iter), 1)
-        opts.mode = DEFAULT_MODE if mode is None else int(mode)
-        if int(world_size) > 1 and opts.mode == 1:  # conditional-node graphs cannot host the NCCL hook
-            opts.mode = 0
+        opts.mode = 2  # the only driver: flat CUDA graphs of gated steps
         opts.world_size = int(world_size)
-        self.mode = opts.mode
         self._keep = []
         if opts.constraint == _lib.CONSTRAINT_ANCHORED:
             anchors = constraint.anchors.to(device=self.device, dtype=torch.int64).contiguous()
@@ -84,7 +72,7 @@ class DeviceSolver(object):
         self.max_iter = opts.max_iter
         self._cb = None
         self.peer_memory = False
-        if int(world_size) > 1 and exchange is not None and opts.mode == 2:
+        if int(world_size) > 1 and exchange is not None:
             # peer-memory all-reduce: export this rank's cudaIpc handle, gather everybody's, map the peers
             # (pymde_b200/dist.py::exchange_handles); the solve then runs graph-captured like on one GPU
             mine = (C.c_ubyte * _lib.IPC_HANDLE_BYTES)()

@@ -322,7 +322,7 @@ class MDE(torch.nn.Module):
         stamp = ()
         if isinstance(constraint, constraints.Anchored):  # anchor indices / values are copied at solver creation
             stamp = self._tensor_stamp(constraint.anchors, constraint.values)
-        key = (int(memory_size), optim.DEFAULT_MODE, stamp)
+        key = (int(memory_size), stamp)
         cur = self.__dict__["_device_solver"]
         if cur is None or cur[2] is not constraint or cur[0] != key or cur[1].max_iter < int(max_iter):
             if cur is not None:

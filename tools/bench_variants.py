@@ -1,5 +1,5 @@
-"""A/B timing of solver build variants on the bench workload (C2) and the Standardized variant:
-MDE_B200_UNROLL = iterations chained per CUDA-graph launch.  Not the headline bench (bench.py is)."""
+"""A/B timing of MDE_B200_STEPS (steps per solver graph launch) on the bench workload (C2) and the
+Standardized variant.  Not the headline bench (bench.py is)."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -14,11 +14,7 @@ ITERS = int(os.environ.get("VARIANT_ITERS", "400"))
 
 
 def run(cons, env):
-    from pymde_b200 import optim
-    for k in ("MDE_B200_UNROLL", "MDE_B200_STEPS"):
-        os.environ.pop(k, None)
-    env = dict(env)
-    optim.DEFAULT_MODE = int(env.pop("MODE", "1"))
+    os.environ.pop("MDE_B200_STEPS", None)
     os.environ.update(env)
     f = pm.penalties.PushAndPull(wt, pm.penalties.Log1p, pm.penalties.Log)
     mde = pm.MDE(bench.N_ITEMS, 2, et, f, cons, device=dev)
@@ -33,11 +29,10 @@ def run(cons, env):
     return best, fe / done, avg[0], avg[-1], done
 
 
-VARIANTS = [{"MODE": "1", "MDE_B200_UNROLL": "4"}, {"MODE": "2"}, {"MODE": "2", "MDE_B200_STEPS": "16"},
-            {"MODE": "2", "MDE_B200_STEPS": "32"}, {"MODE": "2"}]
+VARIANTS = [{}, {"MDE_B200_STEPS": "16"}, {"MDE_B200_STEPS": "32"}, {}]
 for cname, cons in (("centered", pm.Centered()), ("standardized", pm.Standardized())):
     for env in VARIANTS:
-        tag = " ".join("%s=%s" % (k.replace("MDE_B200_", ""), v) for k, v in sorted(env.items())) or "mode1"
+        tag = " ".join("%s=%s" % (k.replace("MDE_B200_", ""), v) for k, v in sorted(env.items())) or "STEPS=8"
         try:
             r = run(cons, env)
             print("%-13s %-12s %8.0f it/s  evals/iter %.2f  loss %.6f -> %.6f  (%d iterations)" % ((cname, tag) + r), flush=True)

@@ -1,4 +1,4 @@
-"""Where a late-epilogue step spends its time: %globaltimer stamps of the head kernel's scalar stage (see
+"""Where a solver step spends its time: %globaltimer stamps of the head kernel's scalar stage (see
 mde_solver_debug_times in include/mde_b200.h) on the C2-shaped bench problem, sampled after runs of different length."""
 import ctypes as C, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
