@@ -12,7 +12,9 @@
 // Algorithmic bytes per fused evaluation: p*(8+4k) + 2*n*m*4 + 8  (SURVEY section 8d).
 //
 // Kernel shapes
-//   m <= 4 : one thread per edge, 32 consecutive sorted edges per warp round; the lhs
+//   m <= 4, default (fused value + gradient and external coefficients): distortion_owner_kernel walks the directed
+//            entries `ent` grouped by owner node, 8 lanes per node, sum in registers, one write per row, no atomics.
+//   m <= 4, value only / MDE_B200_DETERMINISTIC / other m: one thread per edge (quad or strided kernel); the lhs
 //            contributions (sorted => runs of equal src) are summed with a warp segmented
 //            reduction and issued as ONE vector red per run; rhs contributions go out as
 //            vector reds (REDG.E.ADD.F32x2/x4).
@@ -98,59 +100,6 @@ __device__ __forceinline__ void red_row_fx(long long* __restrict__ F, int r, con
     atomicAdd(reinterpret_cast<unsigned long long*>(F + (int64_t)r * M + c), (unsigned long long)q);
   }
 }
-template <int M>
-__device__ __forceinline__ void store_row(float* __restrict__ C, int64_t k, const float (&v)[M]) {
-  if constexpr (M == 2) *reinterpret_cast<float2*>(C + 2 * k) = make_float2(v[0], v[1]);
-  else if constexpr (M == 4) *reinterpret_cast<float4*>(C + 4 * k) = make_float4(v[0], v[1], v[2], v[3]);
-  else {
-#pragma unroll
-    for (int c = 0; c < M; ++c) C[k * M + c] = v[c];
-  }
-}
-// grad[i] += sum over the node's incident edges of +-contribution.  kGatherLanes lanes per node, lane l takes the
-// entries l, l + 8, ... of the node's list in order and the lanes are combined by a fixed shuffle tree: no atomics,
-// and the same summation order in every run.
-constexpr int kGatherLanes = 8;
-template <int M>
-__global__ void __launch_bounds__(256)
-node_gather_kernel(const int* __restrict__ flag, const float* __restrict__ C, const uint32_t* __restrict__ inc,
-                   const int64_t* __restrict__ off, int64_t n, float* __restrict__ grad) {
-  if (flag != nullptr && *flag == 0) return;
-  const int64_t gid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const int64_t i = gid / kGatherLanes;
-  const int l = (int)(gid % kGatherLanes);
-  float acc[M];
-#pragma unroll
-  for (int c = 0; c < M; ++c) acc[c] = 0.0f;
-  if (i < n) {
-    const int64_t j1 = __ldg(off + i + 1);
-#pragma unroll 2
-    for (int64_t j = __ldg(off + i) + l; j < j1; j += kGatherLanes) {
-      const uint32_t w = __ldg(inc + j);
-      const int64_t k = (int64_t)(w >> 1);
-      const float sg = (w & 1u) ? -1.0f : 1.0f;
-      if constexpr (M == 2) {
-        const float2 v = __ldg(reinterpret_cast<const float2*>(C) + k);
-        acc[0] += sg * v.x; acc[1] += sg * v.y;
-      } else if constexpr (M == 4) {
-        const float4 v = __ldg(reinterpret_cast<const float4*>(C) + k);
-        acc[0] += sg * v.x; acc[1] += sg * v.y; acc[2] += sg * v.z; acc[3] += sg * v.w;
-      } else {
-#pragma unroll
-        for (int c = 0; c < M; ++c) acc[c] += sg * __ldg(C + k * M + c);
-      }
-    }
-  }
-#pragma unroll
-  for (int o = kGatherLanes / 2; o > 0; o >>= 1) {
-#pragma unroll
-    for (int c = 0; c < M; ++c) acc[c] += __shfl_xor_sync(kFull, acc[c], o, kGatherLanes);
-  }
-  if (i < n && l == 0) {
-#pragma unroll
-    for (int c = 0; c < M; ++c) grad[i * M + c] += acc[c];
-  }
-}
 // incidence entries of the sorted edges: (node, (k << 1) | endpoint is dst); the per-node counts on the side
 __global__ void inc_keys_kernel(const int32_t* __restrict__ src, const int32_t* __restrict__ dst, int64_t p,
                                 uint32_t* __restrict__ keys, uint32_t* __restrict__ vals, int* __restrict__ count) {
@@ -161,6 +110,18 @@ __global__ void inc_keys_kernel(const int32_t* __restrict__ src, const int32_t* 
   keys[j] = (uint32_t)node;
   vals[j] = ((uint32_t)k << 1) | (j < p ? 0u : 1u);
   atomicAdd(count + node, 1);
+}
+// directed entries in the order of `inc`: (neighbour row | endpoint is dst << 31, bits of par0[k])
+__global__ void ent_fill_kernel(const uint32_t* __restrict__ inc, const int32_t* __restrict__ src,
+                                const int32_t* __restrict__ dst, const float* __restrict__ par0, int64_t q,
+                                uint2* __restrict__ ent) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= q) return;
+  const uint32_t w = inc[j];
+  const int64_t k = (int64_t)(w >> 1);
+  const uint32_t is_dst = w & 1u;
+  const uint32_t nbr = (uint32_t)(is_dst ? src[k] : dst[k]);
+  ent[j] = make_uint2(nbr | (is_dst << 31), __float_as_uint(par0[k]));
 }
 __global__ void fx_zero_kernel(const int* __restrict__ flag, long long* __restrict__ F, int64_t count) {
   if (flag != nullptr && *flag == 0) return;
@@ -278,6 +239,37 @@ distortion_small_kernel(const int32_t* __restrict__ src, const int32_t* __restri
 // ------------------------------------------------------------------------------------------
 static constexpr int kQuadThreads = 256;
 
+// One edge's loss term f and gradient contribution v = g (x_src - x_dst) (added at src, subtracted at dst).  The quad
+// kernel and the owner kernel both evaluate edges through this function, so they produce the same floats.  MODE 2
+// takes g = a; MODE 1 leaves v unset.  d = 0: the reference replaces the non-finite g by 1 and the difference vector
+// is 0.  Returns whether v is live (v = 0 otherwise).  `v` must be rounded on its own before it is summed: the owner
+// kernel adds it with __fadd_rn, so that no contraction fuses g * diff into the accumulation.
+template <int M, int MODE, int FA, int FR, bool FAST>
+__device__ __forceinline__ bool edge_contribution(const Row<M>& xs, const Row<M>& xd, float a, float b, const FnDev& fn,
+                                                  float inv_p, bool ok, float& f, float (&v)[M]) {
+  float diff[M];
+  float d2 = 0.0f;
+#pragma unroll
+  for (int c = 0; c < M; ++c) { diff[c] = xs.v[c] - xd.v[c]; d2 += diff[c] * diff[c]; }
+  float g;
+  f = 0.0f;
+  if (MODE == 2) {
+    g = a;
+  } else if (FAST) {
+    edge_coeff_fast_log1p_log(d2, a, inv_p, f, g);
+  } else {
+    const float d = sqrtf(d2);
+    if (MODE == 0) edge_coeff<FA, FR>(fn, d, a, b, inv_p, f, g);
+    else { edge_value<FA, FR>(fn, d, a, b, f); g = 0.0f; }
+  }
+  const bool live = ok && (FAST ? (d2 > 0.0f) : true);
+  if (MODE != 1) {
+#pragma unroll
+    for (int c = 0; c < M; ++c) v[c] = live ? g * diff[c] : 0.0f;
+  }
+  return live;
+}
+
 template <int M, int MODE, int FA, int FR, bool FAST, int NQ>
 __global__ void __launch_bounds__(kQuadThreads)
 distortion_quad_kernel(const int32_t* __restrict__ src, const int32_t* __restrict__ dst,
@@ -285,7 +277,7 @@ distortion_quad_kernel(const int32_t* __restrict__ src, const int32_t* __restric
                        const int32_t* __restrict__ perm, const float* __restrict__ gext,
                        int64_t p, const float* __restrict__ X, float* __restrict__ grad,
                        double* __restrict__ loss_partials, FnDev fn, float inv_p,
-                       const int* __restrict__ flag, long long* __restrict__ fx, float* __restrict__ cb) {
+                       const int* __restrict__ flag, long long* __restrict__ fx) {
   if (flag != nullptr && *flag == 0) return;
   constexpr int E = 4 * NQ;  // consecutive edges owned by a thread per iteration
   const int64_t nquads = (p + 3) >> 2;
@@ -357,31 +349,10 @@ distortion_quad_kernel(const int32_t* __restrict__ src, const int32_t* __restric
 #pragma unroll
     for (int e = 0; e < E; ++e) {
       const bool ok = (4 * (u * NQ) + e) < p;
-      float diff[M];
-      float d2 = 0.0f;
-#pragma unroll
-      for (int c = 0; c < M; ++c) { diff[c] = xi[e].v[c] - xj[e].v[c]; d2 += diff[c] * diff[c]; }
-      float g, f = 0.0f;
-      if (MODE == 2) {
-        g = a[e];
-      } else if (FAST) {
-        edge_coeff_fast_log1p_log(d2, a[e], inv_p, f, g);
-      } else {
-        const float d = sqrtf(d2);
-        if (MODE == 0) edge_coeff<FA, FR>(fn, d, a[e], b[e], inv_p, f, g);
-        else { edge_value<FA, FR>(fn, d, a[e], b[e], f); g = 0.0f; }
-      }
+      float f, v[M];
+      const bool live = edge_contribution<M, MODE, FA, FR, FAST>(xi[e], xj[e], a[e], b[e], fn, inv_p, ok, f, v);
       if (MODE != 2 && ok) { if (FAST) lsum_f += f; else lsum += (double)f; }
       if (MODE != 1) {
-        // d = 0: the reference replaces the non-finite g by 1 and the difference vector is 0
-        const bool live = ok && (FAST ? (d2 > 0.0f) : true);
-        float v[M];
-#pragma unroll
-        for (int c = 0; c < M; ++c) v[c] = live ? g * diff[c] : 0.0f;
-        if (cb) {  // contribution stored, gathered per node afterwards
-          if (ok) store_row<M>(cb, 4 * (u * NQ) + e, v);
-          continue;
-        }
         if (live) { if (fx) red_row_fx<M>(fx, t[e], v, -1.0f); else red_row<M>(grad, t[e], v, -1.0f); }
         if (s[e] != cur) {  // run of equal src ended: flush its sum
           if (fx) red_row_fx<M>(fx, cur, acc, 1.0f); else red_row<M>(grad, cur, acc, 1.0f);
@@ -393,8 +364,147 @@ distortion_quad_kernel(const int32_t* __restrict__ src, const int32_t* __restric
         for (int c = 0; c < M; ++c) acc[c] += v[c];
       }
     }
-    if (MODE != 1 && !cb) { if (fx) red_row_fx<M>(fx, cur, acc, 1.0f); else red_row<M>(grad, cur, acc, 1.0f); }
+    if (MODE != 1) { if (fx) red_row_fx<M>(fx, cur, acc, 1.0f); else red_row<M>(grad, cur, acc, 1.0f); }
     if (FAST) { lsum += (double)lsum_f; lsum_f = 0.0f; }
+  }
+  if (MODE != 2) {
+    __shared__ double sm[32];
+    double v1[1] = {lsum};
+    block_sum<1>(v1, sm);
+    if (threadIdx.x == 0) loss_partials[blockIdx.x] = v1[0];
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// m <= 4, owner-complete pass over the directed entries of the sorted-SoA layout (MODE 0 and 2).  kOwnerLanes lanes
+// per node: lane l evaluates the entries l, l + 8, ... of the node's list in order and keeps their sum in registers,
+// the lanes are combined by a fixed shuffle tree and the row is written once.  Every edge is evaluated at both of its
+// ends, with the same operands, so each contribution is the same float at both; no atomics and no second pass, so
+// the gradient is the same bits in every run.  The loss counts each edge once, at its src-end entry, in fp64.
+// ------------------------------------------------------------------------------------------
+static constexpr int kOwnerLanes = 8;
+static constexpr int kOwnerThreads = 256;
+static constexpr int kOwnerNodes = kOwnerThreads / kOwnerLanes;  // nodes per block and trip
+static constexpr int kOwnerBatch = 4;  // entries per lane whose loads are issued before the first of them is added
+static constexpr int kOwnerHub = 128;  // longer lists are evaluated by the whole warp (same entries per lane, same order)
+
+template <int M, int MODE, int FA, int FR, bool FAST>
+__global__ void __launch_bounds__(kOwnerThreads)
+distortion_owner_kernel(const uint2* __restrict__ ent, const uint32_t* __restrict__ inc,
+                        const int64_t* __restrict__ off, const float* __restrict__ par1,
+                        const int32_t* __restrict__ perm, const float* __restrict__ gext, int64_t n,
+                        const float* __restrict__ X, float* __restrict__ grad, double* __restrict__ loss_partials,
+                        FnDev fn, float inv_p, const int* __restrict__ flag) {
+  static_assert(MODE == 0 || MODE == 2, "value-only evaluations run on the quad kernel");
+  if (flag != nullptr && *flag == 0) return;
+  const int lane = threadIdx.x & 31, l = lane % kOwnerLanes;
+  const bool need_k = MODE == 2 || par1 != nullptr;  // par1[k] and gext[perm[k]] are indexed by the sorted edge
+  double lsum = 0.0;
+  // one entry: record, coefficient a, second parameter b.  Past the end of a list the owner's own row stands in
+  // (masked by the caller), so every address stays valid.  Entry indices fit in int: the layout needs 2 p < 2^31.
+  auto fetch = [&](int j, bool in, int own, uint2& w, float& a, float& b) {
+    w = in ? __ldg(ent + j) : make_uint2((uint32_t)own, 0u);
+    a = __uint_as_float(w.y);
+    b = 0.0f;
+    if (need_k) {
+      const uint32_t k = in ? (__ldg(inc + j) >> 1) : 0u;
+      if (MODE == 2) a = __ldg(gext + __ldg(perm + k));
+      else b = __ldg(par1 + k);
+    }
+  };
+  // the edge's difference is x_src - x_dst at both ends; returns the signed contribution to the owner's row
+  auto contribution = [&](const Row<M>& xo, const Row<M>& xn, uint2 w, float a, float b, bool in, float (&v)[M]) {
+    const bool at_dst = (w.x >> 31) != 0;
+    Row<M> xs, xd;
+#pragma unroll
+    for (int c = 0; c < M; ++c) {
+      xs.v[c] = at_dst ? xn.v[c] : xo.v[c];
+      xd.v[c] = at_dst ? xo.v[c] : xn.v[c];
+    }
+    float f;
+    edge_contribution<M, MODE, FA, FR, FAST>(xs, xd, a, b, fn, inv_p, true, f, v);
+    if (MODE != 2 && in && !at_dst) lsum += (double)f;
+#pragma unroll
+    for (int c = 0; c < M; ++c) v[c] = at_dst ? -v[c] : v[c];
+  };
+  // the trip count is uniform across the block: the shuffles and the block sum need every lane
+  for (int64_t i0 = (int64_t)blockIdx.x * kOwnerNodes; i0 < n; i0 += (int64_t)gridDim.x * kOwnerNodes) {
+    const int64_t il = i0 + threadIdx.x / kOwnerLanes;
+    const bool node = il < n;
+    const int i = node ? (int)il : 0;
+    float acc[M];
+#pragma unroll
+    for (int c = 0; c < M; ++c) acc[c] = 0.0f;
+    const int j0 = node ? (int)__ldg(off + i) : 0, j1 = node ? (int)__ldg(off + i + 1) : 0;
+    const bool hub = j1 - j0 > kOwnerHub;
+    if (node && !hub) {
+      const Row<M> xo = load_row<M>(X, i);
+      for (int j = j0 + l; j < j1; j += kOwnerLanes * kOwnerBatch) {
+        // the loads of kOwnerBatch entries go out before the first add; the adds keep the list order
+        uint2 w[kOwnerBatch];
+        float a[kOwnerBatch], b[kOwnerBatch];
+#pragma unroll
+        for (int u = 0; u < kOwnerBatch; ++u) fetch(j + u * kOwnerLanes, j + u * kOwnerLanes < j1, i, w[u], a[u], b[u]);
+        Row<M> xn[kOwnerBatch];
+#pragma unroll
+        for (int u = 0; u < kOwnerBatch; ++u) xn[u] = load_row<M>(X, (int)(w[u].x & 0x7fffffffu));
+#pragma unroll
+        for (int u = 0; u < kOwnerBatch; ++u) {
+          if (j + u * kOwnerLanes < j1) {
+            float v[M];
+            contribution(xo, xn[u], w[u], a[u], b[u], true, v);
+#pragma unroll
+            for (int c = 0; c < M; ++c) acc[c] = __fadd_rn(acc[c], v[c]);
+          }
+        }
+      }
+    }
+    // hubs: the whole warp evaluates 32 consecutive entries of one hub's list per round, and lane l of the hub's
+    // group adds those at l, l + 8, l + 16, l + 24 -- the entries and the order of the loop above, with 4x the lanes
+    // doing the math.  Two rounds ahead are in flight during a round's math and shuffles: the entry record of round
+    // r + 2 and the neighbour row of round r + 1 (whose record arrived during round r - 1).
+    unsigned hubs = __ballot_sync(kFull, hub && l == 0);
+    while (hubs) {
+      const int g0 = __ffs(hubs) - 1;  // lane 0 of the hub's group
+      hubs &= hubs - 1;
+      const int ih = __shfl_sync(kFull, i, g0);
+      const int h0 = __shfl_sync(kFull, j0, g0), h1 = __shfl_sync(kFull, j1, g0);
+      const bool mine = (lane & ~(kOwnerLanes - 1)) == g0;
+      const Row<M> xo = load_row<M>(X, ih);
+      uint2 w0, w1;
+      float a0, b0, a1, b1;
+      fetch(h0 + lane, h0 + lane < h1, ih, w0, a0, b0);
+      fetch(h0 + 32 + lane, h0 + 32 + lane < h1, ih, w1, a1, b1);
+      Row<M> x0 = load_row<M>(X, (int)(w0.x & 0x7fffffffu));
+      for (int hb = h0; hb < h1; hb += 32) {
+        const Row<M> x1 = load_row<M>(X, (int)(w1.x & 0x7fffffffu));
+        uint2 w2;
+        float a2, b2;
+        fetch(hb + 64 + lane, hb + 64 + lane < h1, ih, w2, a2, b2);
+        float v[M];
+        contribution(xo, x0, w0, a0, b0, hb + lane < h1, v);
+#pragma unroll
+        for (int q = 0; q < 32 / kOwnerLanes; ++q) {
+          const int from = l + q * kOwnerLanes;
+#pragma unroll
+          for (int c = 0; c < M; ++c) {
+            const float t = __shfl_sync(kFull, v[c], from);
+            if (mine && hb + from < h1) acc[c] = __fadd_rn(acc[c], t);
+          }
+        }
+        w0 = w1; a0 = a1; b0 = b1; x0 = x1;
+        w1 = w2; a1 = a2; b1 = b2;
+      }
+    }
+#pragma unroll
+    for (int o = kOwnerLanes / 2; o > 0; o >>= 1) {
+#pragma unroll
+      for (int c = 0; c < M; ++c) acc[c] += __shfl_xor_sync(kFull, acc[c], o, kOwnerLanes);
+    }
+    if (node && l == 0) {
+#pragma unroll
+      for (int c = 0; c < M; ++c) grad[(int64_t)i * M + c] += acc[c];
+    }
   }
   if (MODE != 2) {
     __shared__ double sm[32];
@@ -617,6 +727,14 @@ int loss_blocks_quad(int64_t p, int nq, int bps) {
   return (int)nb;
 }
 
+// the owner kernel's grid depends on n alone; beyond kMaxLossBlocks blocks it strides over the nodes
+int loss_blocks_owner(int64_t n) {
+  int64_t nb = (n + kOwnerNodes - 1) / kOwnerNodes;
+  if (nb < 1) nb = 1;
+  if (nb > kMaxLossBlocks) nb = kMaxLossBlocks;
+  return (int)nb;
+}
+
 int loss_blocks_wide(int64_t p, int G) {
   int64_t groups_per_block = kWideThreads / G;
   int64_t per_block = groups_per_block * kWideSlice;
@@ -641,8 +759,8 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
     fx_zero_kernel<<<zb, 256, 0, st>>>(flag, fxp, cnt);
     ++g_launch_count;
   }
-  // default on the sorted-SoA layout: per-edge contributions + fixed-order per-node gather (quad kernel only)
-  float* cbp = (!fxp && e->cb && MODE != 1 && m == e->m_hint && e->kvar != 1) ? e->cb : nullptr;
+  // default on the sorted-SoA layout: the owner kernel over the directed entries, in place of the quad kernel
+  const bool owner = !fxp && e->ent && MODE != 1 && m == e->m_hint && e->kvar != 1;
 #define SMALLK(MM, FA, FR)                                                                            \
   distortion_small_kernel<MM, MODE, FA, FR><<<nb, kSmallThreads, 0, st>>>(                            \
       e->src, e->dst, e->par0, e->has_par1 ? e->par1 : nullptr, e->perm, gext, p, X, grad,           \
@@ -651,9 +769,17 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
 #define QUADK_(MM, FA, FR, FAST, NQV)                                                                 \
   distortion_quad_kernel<MM, MODE, FA, FR, FAST, NQV><<<nb, kQuadThreads, 0, st>>>(                   \
       e->src, e->dst, e->par0, e->has_par1 ? e->par1 : nullptr, e->perm, gext, p, X, grad,           \
-      e->loss_partials, e->fn, inv_p, flag, fxp, cbp)
+      e->loss_partials, e->fn, inv_p, flag, fxp)
+#define OWNERK(MM, FA, FR, FAST)                                                                      \
+  if constexpr (MODE != 1) {                                                                         \
+    nb = loss_blocks_owner(e->n);                                                                    \
+    distortion_owner_kernel<MM, MODE, FA, FR, FAST><<<nb, kOwnerThreads, 0, st>>>(                    \
+        e->ent, e->inc, e->inc_off, e->has_par1 ? e->par1 : nullptr, e->perm, gext, e->n, X, grad,   \
+        e->loss_partials, e->fn, inv_p, flag);                                                       \
+  }
 #define QUADK(MM, FA, FR, FAST)                                                                       \
-  if (FAST && e->nq == 2) { nb = loss_blocks_quad(p, 2, e->qbps); QUADK_(MM, FA, FR, FAST, 2); }       \
+  if (owner) { OWNERK(MM, FA, FR, FAST) }                                                             \
+  else if (FAST && e->nq == 2) { nb = loss_blocks_quad(p, 2, e->qbps); QUADK_(MM, FA, FR, FAST, 2); }  \
   else { nb = loss_blocks_quad(p, 1, e->qbps); QUADK_(MM, FA, FR, FAST, 1); }
 #define SMALL(MM)                                                                                     \
   if (e->kvar != 1) {                                                                                 \
@@ -670,6 +796,11 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
       else if (!pp && fa == MDE_FN_L_QUADRATIC) { QUADK(MM, MDE_FN_L_QUADRATIC, MDE_FN_L_QUADRATIC, false); }     \
       else if (!pp && fa == MDE_FN_L_WEIGHTED_QUADRATIC) { QUADK(MM, MDE_FN_L_WEIGHTED_QUADRATIC, MDE_FN_L_WEIGHTED_QUADRATIC, false); } \
       else if (!pp && fa == MDE_FN_L_HUBER) { QUADK(MM, MDE_FN_L_HUBER, MDE_FN_L_HUBER, false); }                 \
+      else { QUADK(MM, -1, -1, false); }                                                              \
+    } else if constexpr (MODE == 0) {                                                                 \
+      /* m = 1, 4: the owner kernel evaluates every edge twice, so the recipe default PushAndPull(Log1p, Log) \
+         gets compile-time ids there (IEEE math, as the run-time table) instead of two out-of-line calls */ \
+      if (owner && pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG) { OWNERK(MM, MDE_FN_P_LOG1P, MDE_FN_P_LOG, false) } \
       else { QUADK(MM, -1, -1, false); }                                                              \
     } else { QUADK(MM, -1, -1, false); }                                                              \
   } else {                                                                                            \
@@ -721,6 +852,7 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
 #undef SMALL_STRIDED
 #undef QUADK
 #undef QUADK_
+#undef OWNERK
 #undef SMALLK
 #undef WIDE
   MDE_LAUNCH_CHECK();
@@ -728,14 +860,6 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
     const int64_t cnt = e->n * m;
     int zb = (int)((cnt + 255) / 256); if (zb > kNumSMs * 8) zb = kNumSMs * 8;
     fx_apply_kernel<<<zb, 256, 0, st>>>(flag, fxp, grad, cnt);
-    MDE_LAUNCH_CHECK();
-  }
-  if (cbp) {
-    const unsigned gb = (unsigned)((e->n * kGatherLanes + 255) / 256);
-    if (m == 1) node_gather_kernel<1><<<gb, 256, 0, st>>>(flag, cbp, e->inc, e->inc_off, e->n, grad);
-    else if (m == 2) node_gather_kernel<2><<<gb, 256, 0, st>>>(flag, cbp, e->inc, e->inc_off, e->n, grad);
-    else if (m == 3) node_gather_kernel<3><<<gb, 256, 0, st>>>(flag, cbp, e->inc, e->inc_off, e->n, grad);
-    else node_gather_kernel<4><<<gb, 256, 0, st>>>(flag, cbp, e->inc, e->inc_off, e->n, grad);
     MDE_LAUNCH_CHECK();
   }
   if (nblocks_out) *nblocks_out = nb;
@@ -878,14 +1002,14 @@ int mde_edges_create_ex(mde_edges_t** out, const int64_t* edges, int64_t p, int6
   keys_in = keys_out = nullptr; vals_in = vals_out = nullptr; tmp = nullptr;
   if (!e->det && !want_ell && embedding_dim >= 1 && embedding_dim <= 4 && 2 * p < (1ll << 31)) {
     // incidence lists of the sorted edges: a stable radix sort by node keeps each node's entries in the order
-    // (src entries by k, then dst entries by k), so the per-node gather adds in the same order in every run
+    // (src entries by k, then dst entries by k), so the owner kernel adds in the same order in every run
     uint32_t *ik = nullptr, *ik2 = nullptr, *iv = nullptr;
     int* cnt = nullptr;
     const int64_t q = 2 * p;
     size_t tb2 = 0, sb = 0;
     int bits = 1;
     while (bits < 32 && (1ll << bits) < n_items) ++bits;
-    TRY(cudaMalloc(&e->cb, sizeof(float) * p * embedding_dim));
+    TRY(cudaMalloc(&e->ent, sizeof(uint2) * q));
     TRY(cudaMalloc(&e->inc, sizeof(uint32_t) * q));
     TRY(cudaMalloc(&e->inc_off, sizeof(int64_t) * (n_items + 1)));
     TRY(cudaMalloc(&ik, sizeof(uint32_t) * q));
@@ -903,11 +1027,14 @@ int mde_edges_create_ex(mde_edges_t** out, const int64_t* edges, int64_t p, int6
     TRY(cub::DeviceRadixSort::SortPairs(tmp, tb2, ik, ik2, iv, e->inc, (int)q, 0, bits, st));
     sb = tb2;
     TRY(cub::DeviceScan::ExclusiveSum(tmp, sb, cnt, e->inc_off, (int)(n_items + 1), st));
+    ent_fill_kernel<<<ceil_div_i64(q, 256), 256, 0, st>>>(e->inc, e->src, e->dst, e->par0, q, e->ent);
+    ++g_launch_count;
+    TRY(cudaPeekAtLastError());
     TRY(cudaStreamSynchronize(st));
     cudaFree(ik); cudaFree(ik2); cudaFree(iv); cudaFree(cnt); cudaFree(tmp);
     tmp = nullptr;
     e->m_hint = embedding_dim;
-    e->nbytes += p * embedding_dim * 4 + q * 4 + (n_items + 1) * 8;
+    e->nbytes += q * 8 + q * 4 + (n_items + 1) * 8;
   }
   if (want_ell) {
     // ELL pull records next to the sorted-SoA arrays (kind 3); MDE_E_UNSUPPORTED leaves the layout at kind 0
@@ -931,7 +1058,7 @@ fail:
 int mde_edges_destroy(mde_edges_t* e) {
   if (!e) return 0;
   cudaFree(e->src); cudaFree(e->dst); cudaFree(e->perm); cudaFree(e->par0); cudaFree(e->par1);
-  cudaFree(e->loss_partials); cudaFree(e->fx); cudaFree(e->cb); cudaFree(e->inc); cudaFree(e->inc_off);
+  cudaFree(e->loss_partials); cudaFree(e->fx); cudaFree(e->ent); cudaFree(e->inc); cudaFree(e->inc_off);
   tiled_free(e);
   pull_free(e);
   ell_free(e);

@@ -43,12 +43,12 @@ struct mde_edges {
   int qbps = 4;              // MDE_B200_QUAD_BPS: blocks per SM in the quad kernel's grid cap (1..16)
   int det = 0;               // deterministic mode: gradient contributions accumulate in 64-bit fixed point
   long long* fx = nullptr;   // [n * m_hint] fixed-point accumulator (det only)
-  // sorted-SoA layout, m_hint <= 4: the quad kernel stores every edge's contribution in `cb` (no atomics) and
-  // node_gather_kernel sums a node's incident contributions in the fixed order of `inc` -- a gradient that is the same
-  // bits from run to run
-  float* cb = nullptr;          // [p * m_hint] contribution of sorted edge k (added at src, subtracted at dst)
+  // sorted-SoA layout, m_hint <= 4: every edge is stored again as two directed entries grouped by owner node, and the
+  // owner kernel visits each node's entries in this fixed order, keeps the sum in registers and writes the row once
+  // (no atomics) -- a gradient that is the same bits from run to run
   uint32_t* inc = nullptr;      // [2 p] (k << 1) | (node is dst), grouped by node: src entries by k, then dst entries by k
-  int64_t* inc_off = nullptr;   // [n + 1]
+  uint2* ent = nullptr;         // [2 p] in the order of inc: (neighbour row | (node is dst) << 31, bits of par0[k])
+  int64_t* inc_off = nullptr;   // [n + 1] first entry of node i in inc / ent
   // ---- kind 1 ----
   int m_hint = 0;          // embedding dimension the tile size was chosen for
   int rb = 0;              // log2(R): dst tile rows
