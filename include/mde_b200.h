@@ -274,6 +274,19 @@ int mde_knn(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2
 int mde_knn_csr_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes);
 int mde_knn_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
                 int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream);
+/* The same two searches for 1 <= k <= mde_knn_wide_max_k() (64), k <= n - 1: arguments, output contract, tie rules
+ * and return codes of mde_knn and mde_knn_csr (the CSR check included).  A running top-96 per row, kept in shared
+ * memory, feeds the exact re-rank.  For k <= 24 the result is that of mde_knn / mde_knn_csr, which remain the faster
+ * searches there.  `ws`: 1024-byte aligned device scratch of mde_knn_wide_ws_bytes(n, d) or
+ * mde_knn_csr_wide_ws_bytes(n, d, nnz) bytes (256 more bytes per row than the narrow searches).  mde_knn_wide is
+ * asynchronous on `stream`, mde_knn_csr_wide blocking as mde_knn_csr. */
+int mde_knn_wide_max_k(void);
+int mde_knn_wide_ws_bytes(int64_t n, int d, size_t* bytes);
+int mde_knn_wide(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                 size_t ws_bytes, void* stream);
+int mde_knn_csr_wide_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes);
+int mde_knn_csr_wide(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                     int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream);
 /* Euclidean distances ||x_a - x_b|| of p row pairs (device int64 pairs[p][2]) of the same CSR, into out[p] (fp32):
  * a sorted merge of the two rows summed in fp64, sqrt in fp64, one rounding (pymde/preprocess/data_matrix.py:59-70
  * takes the norm of the difference in scipy).  MDE_E_INVALID for a malformed CSR or a pair index outside [0, n).

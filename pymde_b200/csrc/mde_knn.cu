@@ -18,6 +18,10 @@
 // (k + 8)-th neighbour of real data, and the re-rank removes it from the result: the neighbour lists are those of a
 // brute-force fp32 search (ties and fp32 rounding aside).  k <= 24.
 //
+// mde_knn_wide (24 < k <= 64): knn_wide_tile_kernel does the same sweep for 64 query rows per CTA with one consumer
+// warpgroup and keeps KK = 96 candidates per row in shared memory (mde_knn_select.cuh); knn_wide_rerank_kernel
+// re-ranks all 96 with the arithmetic above.
+//
 // Hangs are not an option on a shared GPU: every mbarrier wait is bounded (mde_tma.cuh) and traps.
 #include <cuda.h>  // CUtensorMap and its enums (types only: the encoder is fetched with cudaGetDriverEntryPoint)
 #include <cuda_bf16.h>
@@ -26,6 +30,7 @@
 #include <cstdlib>
 
 #include "mde_common.cuh"
+#include "mde_knn_select.cuh"
 #include "mde_tma.cuh"
 #include "mde_wgmma.cuh"
 
@@ -50,6 +55,17 @@ constexpr int kSmemBytes = kStages * kStageBytes + 1024 /* alignment slack */ + 
                            2 * kTileN * 4 /* norms */ + 64 /* barriers */;
 static_assert(kTileM == 128 && kTileN == 128, "one TMA box (64 x 128) serves both operands");
 static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
+
+// wide search (k <= 64): 64 query rows per CTA, one consumer warpgroup, running top-96 lists in shared memory
+constexpr int kWideTileM = 64;
+constexpr int kAOpBytes = kWideTileM * kRowBytes;          // 8 KB: one 64-row query operand block (hi or lo)
+constexpr int kWideStageBytes = 2 * kAOpBytes + 2 * kOpBytes;  // A hi, A lo, B hi, B lo = 48 KB
+constexpr int kWideConsumerWarps = 4;                       // warps 0-3: one consumer warpgroup; warp 4: TMA producer
+constexpr int kWideThreads = (kWideConsumerWarps + 1) * 32;
+constexpr int kWideSmemBytes = kStages * kWideStageBytes + 1024 /* alignment slack */ +
+                               kWideTileM * kAccStride * 4 + kTileN * 4 /* norms */ +
+                               kWideTileM * kWideListStride * 8 /* lists */ + 64 /* barriers */;
+static_assert(kWideSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 
 // ---------------------------------------------------------------------------------------------------------------
 // PTX wrappers (tensor TMA); mbarriers come from mde_tma.cuh, wgmma from mde_wgmma.cuh
@@ -278,14 +294,190 @@ knn_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* 
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// wide tiles (k <= 64): as knn_tile_kernel for 64 query rows, one running top-96 per row in shared memory
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kWideThreads, 1)
+knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant__ CUtensorMap map_al,
+                     const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_l,
+                     const float* __restrict__ norms, int64_t n, int64_t n_pad, int k_pad,
+                     int32_t* __restrict__ cand_idx, float* __restrict__ cand_val) {
+  extern __shared__ uint8_t smem_raw[];
+  // carve: [stages x 48 KB, 1024-aligned] | staged accumulators [64][kAccStride] | norms[128] |
+  //        list distances [64][kWideListStride] | list indices [64][kWideListStride] | barriers
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
+  float* s_acc = reinterpret_cast<float*>(gen + kStages * kWideStageBytes);
+  float* s_norm = s_acc + kWideTileM * kAccStride;
+  float* s_ld = s_norm + kTileN;
+  int* s_li = reinterpret_cast<int*>(s_ld + kWideTileM * kWideListStride);
+  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_li + kWideTileM * kWideListStride);
+  const uint32_t bar0 = smem_u32(s_bar);
+  // barriers: full[s] = bar0 + 8 s (TMA bytes landed), empty[s] = bar0 + 16 + 8 s (every consumer warp is done)
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int num_kb = k_pad / kBlockK;
+  const int num_tiles = (int)(n_pad / kTileN);
+  const int row0 = blockIdx.x * kWideTileM;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kStages; ++s) { mbar_init(bar0 + 8 * s, 1); mbar_init(bar0 + 16 + 8 * s, kWideConsumerWarps); }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (warp == kWideConsumerWarps) {
+    // ===== TMA producer =====
+    if (lane == 0) {
+      int stage = 0; uint32_t phase = 0;
+      for (int t = 0; t < num_tiles; ++t) {
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(bar0 + 16 + 8 * stage, phase ^ 1);  // slot released by the consumers
+          const uint32_t full = bar0 + 8 * stage;
+          const uint32_t dst = base + stage * kWideStageBytes;
+          mbar_expect_tx(full, kWideStageBytes);
+          tma_load_2d(dst, &map_ah, kb * kBlockK, row0, full);
+          tma_load_2d(dst + kAOpBytes, &map_al, kb * kBlockK, row0, full);
+          tma_load_2d(dst + 2 * kAOpBytes, &map_h, kb * kBlockK, t * kTileN, full);
+          tma_load_2d(dst + 2 * kAOpBytes + kOpBytes, &map_l, kb * kBlockK, t * kTileN, full);
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+
+  // ===== consumers: the warpgroup owns query rows row0 .. row0 + 63, two adjacent lanes per row =====
+  const int et = threadIdx.x;
+  const int lrow = et >> 1, half = et & 1;
+  const int row = row0 + lrow;
+  const int frow = 16 * warp + (lane >> 2), fcol = 2 * (lane & 3);
+  WideList list;
+  list.init(s_ld + lrow * kWideListStride, s_li + lrow * kWideListStride, half);
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+
+  int stage = 0; uint32_t phase = 0;
+  for (int t = 0; t < num_tiles; ++t) {
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(bar0 + 8 * stage, phase);  // operands landed
+      const uint32_t sa = base + stage * kWideStageBytes;
+      const uint64_t ah = smem_desc_sw128(sa), al = smem_desc_sw128(sa + kAOpBytes);
+      const uint64_t bh = smem_desc_sw128(sa + 2 * kAOpBytes), bl = smem_desc_sw128(sa + 2 * kAOpBytes + kOpBytes);
+#pragma unroll
+      for (int i = 0; i < 64; ++i) fence_operand(acc[i]);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
+        const uint64_t adv = (uint64_t)((k * kWgmmaK * 2) >> 4);
+        wgmma_bf16(acc, ah + adv, bh + adv, (kb | k) != 0);
+        wgmma_bf16(acc, ah + adv, bl + adv, 1u);
+        wgmma_bf16(acc, al + adv, bh + adv, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait_all();
+#pragma unroll
+      for (int i = 0; i < 64; ++i) fence_operand(acc[i]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar0 + 16 + 8 * stage);  // this warp no longer reads the slot
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+    // the previous tile's scan of s_acc / s_norm is finished by every consumer thread
+    named_bar_sync(1, 128);
+#pragma unroll
+    for (int j = 0; j < kTileN / 8; ++j) {
+      *reinterpret_cast<float2*>(s_acc + frow * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(s_acc + (frow + 8) * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+    s_norm[et] = __ldg(norms + (int64_t)t * kTileN + et);
+    named_bar_sync(1, 128);
+    // both lanes of the row offer every column, in column order
+    const float2* arow = reinterpret_cast<const float2*>(s_acc + lrow * kAccStride);
+    const float2* sn = reinterpret_cast<const float2*>(s_norm);
+#pragma unroll 2
+    for (int i = 0; i < kTileN / 2; ++i) {
+      const float2 a = arow[i], s = sn[i];
+      const int col = t * kTileN + 2 * i;
+      if (col != row && col < n) list.offer(fmaf(-2.0f, a.x, s.x), col);
+      if (col + 1 != row && col + 1 < n) list.offer(fmaf(-2.0f, a.y, s.y), col + 1);
+    }
+  }
+  if (row < n) list.store(cand_idx + (int64_t)row * kWideKK, cand_val + (int64_t)row * kWideKK);
+}
+
+// Exact fp32 squared distances of a row's 96 candidates (the arithmetic of knn_rerank_kernel), the k smallest in
+// ascending order; lane q owns candidates q, q + 32 and q + 64, ranks are taken over all 96.
+__global__ void __launch_bounds__(256)
+knn_wide_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
+                       int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= n) return;
+  constexpr int kPer = kWideKK / 32;
+  int mine[kPer];
+  float my_d[kPer];
+  const float* xq = X + row * d;
+#pragma unroll
+  for (int s = 0; s < kPer; ++s) {
+    mine[s] = cand_idx[row * kWideKK + 32 * s + lane];
+    my_d[s] = __int_as_float(0x7f800000);
+    for (int q = 0; q < 32; ++q) {
+      const int c = __shfl_sync(kFull, mine[s], q);
+      if (c < 0) continue;  // (warp-uniform)
+      const float* xc = X + (int64_t)c * d;
+      float acc = 0.0f;
+      for (int j = lane; j < d; j += 32) { const float t = xq[j] - xc[j]; acc = fmaf(t, t, acc); }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
+      if (lane == q) my_d[s] = acc;
+    }
+  }
+  // rank of each owned (distance, index) among the 96: ties broken by index, missing candidates last
+  int rank[kPer] = {};
+#pragma unroll
+  for (int s2 = 0; s2 < kPer; ++s2) {
+    for (int q = 0; q < 32; ++q) {
+      const float od = __shfl_sync(kFull, my_d[s2], q);
+      const int oi = __shfl_sync(kFull, mine[s2], q);
+#pragma unroll
+      for (int s = 0; s < kPer; ++s) {
+        if ((q != lane || s2 != s) && (od < my_d[s] || (od == my_d[s] && (unsigned)oi < (unsigned)mine[s]))) ++rank[s];
+      }
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < kPer; ++s) {
+    if (rank[s] < k) {
+      out_idx[row * k + rank[s]] = mine[s];
+      out_d2[row * k + rank[s]] = my_d[s];
+    }
+  }
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-int make_map(EncodeTiledFn enc, CUtensorMap* map, void* ptr, int64_t n_pad, int k_pad) {
+// cuTensorMapEncodeTiled, fetched once through the runtime (no link-time libcuda dependency)
+int tensor_map_encoder(EncodeTiledFn* out) {
+  static EncodeTiledFn enc = nullptr;
+  if (!enc) {
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    MDE_CUDA_TRY(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
+    if (!fn || qres != cudaDriverEntryPointSuccess) return MDE_E_UNSUPPORTED;
+    enc = (EncodeTiledFn)fn;
+  }
+  *out = enc;
+  return 0;
+}
+
+// Tensor map of an n_pad x k_pad bf16 operand, loaded in boxes of box_rows x 64 (128-byte swizzle).
+int make_map(EncodeTiledFn enc, CUtensorMap* map, void* ptr, int64_t n_pad, int k_pad, int box_rows = kTileM) {
   const cuuint64_t dims[2] = {(cuuint64_t)k_pad, (cuuint64_t)n_pad};
   const cuuint64_t strides[1] = {(cuuint64_t)k_pad * 2};
-  const cuuint32_t box[2] = {(cuuint32_t)kBlockK, (cuuint32_t)kTileM};
+  const cuuint32_t box[2] = {(cuuint32_t)kBlockK, (cuuint32_t)box_rows};
   const cuuint32_t estr[2] = {1, 1};
   const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ptr, dims, strides, box, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -298,7 +490,8 @@ struct KnnLayout {
   size_t off_h, off_l, off_norm, off_ci, off_cv, total;
 };
 
-KnnLayout knn_layout(int64_t n, int d) {
+// kk: candidates kept per row (kKK, or kWideKK for the wide search)
+KnnLayout knn_layout(int64_t n, int d, int kk = kKK) {
   KnnLayout L;
   L.n_pad = (n + kTileN - 1) / kTileN * kTileN;
   L.k_pad = (d + kBlockK - 1) / kBlockK * kBlockK;
@@ -307,8 +500,8 @@ KnnLayout knn_layout(int64_t n, int d) {
   L.off_h = o; o = up(o + (size_t)L.n_pad * L.k_pad * 2);
   L.off_l = o; o = up(o + (size_t)L.n_pad * L.k_pad * 2);
   L.off_norm = o; o = up(o + (size_t)L.n_pad * 4);
-  L.off_ci = o; o = up(o + (size_t)n * kKK * 4);
-  L.off_cv = o; o = up(o + (size_t)n * kKK * 4);
+  L.off_ci = o; o = up(o + (size_t)n * kk * 4);
+  L.off_cv = o; o = up(o + (size_t)n * kk * 4);
   L.total = o;
   return L;
 }
@@ -332,14 +525,9 @@ int mde_knn(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2
   const KnnLayout L = knn_layout(n, d);
   if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
-  static EncodeTiledFn enc = nullptr;
-  if (!enc) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    MDE_CUDA_TRY(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-    if (!fn || qres != cudaDriverEntryPointSuccess) return MDE_E_UNSUPPORTED;
-    enc = (EncodeTiledFn)fn;
-  }
+  EncodeTiledFn enc = nullptr;
+  int rc;
+  if ((rc = tensor_map_encoder(&enc))) return rc;
   uint8_t* w = static_cast<uint8_t*>(ws);
   __nv_bfloat16* Xh = reinterpret_cast<__nv_bfloat16*>(w + L.off_h);
   __nv_bfloat16* Xl = reinterpret_cast<__nv_bfloat16*>(w + L.off_l);
@@ -347,7 +535,6 @@ int mde_knn(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2
   int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
   float* cv = reinterpret_cast<float*>(w + L.off_cv);
   CUtensorMap mh, ml;
-  int rc;
   if ((rc = make_map(enc, &mh, Xh, L.n_pad, L.k_pad))) return rc;
   if ((rc = make_map(enc, &ml, Xl, L.n_pad, L.k_pad))) return rc;
   knn_prep_kernel<<<(unsigned)((L.n_pad + 7) / 8), 256, 0, st>>>(X, n, d, L.n_pad, L.k_pad, Xh, Xl, norms);
@@ -361,6 +548,53 @@ int mde_knn(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2
   knn_tile_kernel<<<grid, kThreads, kSmemBytes, st>>>(mh, ml, norms, n, L.n_pad, L.k_pad, ci, cv);
   MDE_LAUNCH_CHECK();
   knn_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(X, n, d, ci, k, idx_out, d2_out);
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+
+int mde_knn_wide_max_k(void) { return kWideMaxK; }
+
+int mde_knn_wide_ws_bytes(int64_t n, int d, size_t* bytes) {
+  if (!bytes || n < 2 || d < 1) return MDE_E_INVALID;
+  *bytes = knn_layout(n, d, kWideKK).total;
+  return 0;
+}
+
+int mde_knn_wide(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                 size_t ws_bytes, void* stream) {
+  if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > kWideMaxK || k > n - 1)
+    return MDE_E_INVALID;
+  if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
+  const KnnLayout L = knn_layout(n, d, kWideKK);
+  if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  EncodeTiledFn enc = nullptr;
+  int rc;
+  if ((rc = tensor_map_encoder(&enc))) return rc;
+  uint8_t* w = static_cast<uint8_t*>(ws);
+  __nv_bfloat16* Xh = reinterpret_cast<__nv_bfloat16*>(w + L.off_h);
+  __nv_bfloat16* Xl = reinterpret_cast<__nv_bfloat16*>(w + L.off_l);
+  float* norms = reinterpret_cast<float*>(w + L.off_norm);
+  int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
+  float* cv = reinterpret_cast<float*>(w + L.off_cv);
+  CUtensorMap mah, mal, mh, ml;  // query operand in 64-row boxes, candidate operand in 128-row boxes
+  if ((rc = make_map(enc, &mah, Xh, L.n_pad, L.k_pad, kWideTileM))) return rc;
+  if ((rc = make_map(enc, &mal, Xl, L.n_pad, L.k_pad, kWideTileM))) return rc;
+  if ((rc = make_map(enc, &mh, Xh, L.n_pad, L.k_pad))) return rc;
+  if ((rc = make_map(enc, &ml, Xl, L.n_pad, L.k_pad))) return rc;
+  knn_prep_kernel<<<(unsigned)((L.n_pad + 7) / 8), 256, 0, st>>>(X, n, d, L.n_pad, L.k_pad, Xh, Xl, norms);
+  MDE_LAUNCH_CHECK();
+  static bool attr_set = false;
+  if (!attr_set) {
+    MDE_CUDA_TRY(cudaFuncSetAttribute(knn_wide_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      kWideSmemBytes));
+    attr_set = true;
+  }
+  const unsigned grid = (unsigned)((n + kWideTileM - 1) / kWideTileM);
+  knn_wide_tile_kernel<<<grid, kWideThreads, kWideSmemBytes, st>>>(mah, mal, mh, ml, norms, n, L.n_pad, L.k_pad, ci,
+                                                                   cv);
+  MDE_LAUNCH_CHECK();
+  knn_wide_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(X, n, d, ci, k, idx_out, d2_out);
   MDE_LAUNCH_CHECK();
   return 0;
 }

@@ -1,0 +1,68 @@
+// mde_knn_select.cuh -- the running top-96 of the wide k-nearest-neighbour tile kernels (mde_knn.cu,
+// mde_knn_sparse.cu; k <= 64).
+//
+// One list of kWideKK (distance, index) pairs per query row lives in shared memory; it is too large for registers
+// next to the 64 fp32 wgmma accumulators.  Two adjacent lanes (a "pair", half = lane & 1) own a row.  Both offer
+// every candidate of the row in the same order with the same values, so both take the same branches.  Lane `half`
+// owns the slots of its parity: it writes the slot it replaces (when the slot is its own) and scans only its own
+// slots for the new worst, and the two partial worsts meet through one shuffle.  Candidates are ordered by
+// (distance, index); the worst is the largest, so the list after a sweep depends on nothing but the order of the
+// offers, never on timing.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include <climits>
+
+namespace mde {
+
+constexpr int kWideKK = 96;          // candidates kept per row before the exact re-rank
+constexpr int kWideMaxK = 64;        // leaves >= 32 spare candidates for the bf16 x 3 error of the cross terms
+constexpr int kWideListStride = 98;  // words per row list: the 32 lanes of a warp (16 rows) hit 32 different banks
+
+__device__ __forceinline__ bool knn_before(float d1, int i1, float d2, int i2) {
+  return d1 < d2 || (d1 == d2 && i1 < i2);
+}
+
+// Per-lane copy of its row's threshold: the worst kept pair and its slot (identical in both lanes of the pair).
+struct WideList {
+  float* d;    // this row's distances [kWideKK] in shared memory
+  int* i;      // this row's indices [kWideKK]; INT_MAX marks an empty slot
+  int half;    // 0 or 1: the parity of the slots this lane owns
+  float thr;   // worst kept pair (thr, thi) in slot `worst`
+  int thi, worst;
+
+  __device__ __forceinline__ void init(float* row_d, int* row_i, int lane_half) {
+    d = row_d; i = row_i; half = lane_half;
+    for (int j = half; j < kWideKK; j += 2) { d[j] = __builtin_huge_valf(); i[j] = INT_MAX; }
+    thr = __builtin_huge_valf(); thi = INT_MAX; worst = 0;
+  }
+
+  // Keep (dist, col) if it comes before the worst kept pair.  Both lanes of the pair call this with the same
+  // arguments (pair-uniform branches).
+  __device__ __forceinline__ void offer(float dist, int col) {
+    if (!knn_before(dist, col, thr, thi)) return;
+    if ((worst & 1) == half) { d[worst] = dist; i[worst] = col; }
+    float m = d[half]; int mi = i[half], w = half;
+    for (int j = half + 2; j < kWideKK; j += 2) {
+      const float v = d[j]; const int vi = i[j];
+      if (knn_before(m, mi, v, vi)) { m = v; mi = vi; w = j; }
+    }
+    const unsigned pair = 3u << ((threadIdx.x & 31) & 30);
+    const float om = __shfl_xor_sync(pair, m, 1);
+    const int omi = __shfl_xor_sync(pair, mi, 1), ow = __shfl_xor_sync(pair, w, 1);
+    // the larger (distance, index); equal pairs (empty slots) resolve to the lower slot, so both lanes agree
+    if (knn_before(m, mi, om, omi) || (!knn_before(om, omi, m, mi) && ow < w)) { m = om; mi = omi; w = ow; }
+    thr = m; thi = mi; worst = w;
+  }
+
+  // This lane's slots to the row's candidate arrays (empty slots as index -1, distance +inf).
+  __device__ __forceinline__ void store(int32_t* cand_idx, float* cand_val) const {
+    for (int j = half; j < kWideKK; j += 2) {
+      cand_idx[j] = i[j] == INT_MAX ? -1 : i[j];
+      cand_val[j] = d[j];
+    }
+  }
+};
+
+}  // namespace mde

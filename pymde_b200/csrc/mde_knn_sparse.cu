@@ -22,6 +22,9 @@
 //   re-rank  sum (q - x)^2 over each candidate by a sorted merge of the two rows, in fp64, rounded once to fp32; the
 //            k smallest by (distance, index).  The result is fully determined, ties included.
 //
+// mde_knn_csr_wide (24 < k <= 64): the same preparation; knn_csr_wide_tile_kernel sweeps 64 query rows per CTA and
+// keeps KK = 96 candidates per row in shared memory (mde_knn_select.cuh); the re-rank merges all 96.
+//
 // mde_pair_dist_csr: ||a - b|| of given pairs by the same sorted merge, fp64, sqrt in fp64, one rounding.
 #include <cub/cub.cuh>
 #include <cuda_bf16.h>
@@ -30,6 +33,7 @@
 #include <cstdint>
 
 #include "mde_common.cuh"
+#include "mde_knn_select.cuh"
 #include "mde_tma.cuh"
 #include "mde_wgmma.cuh"
 
@@ -54,6 +58,18 @@ constexpr int kAccStride = kTileN + 2;
 constexpr int kSmemBytes = kStages * kStageBytes + 1024 /* alignment slack */ + kTileM * kAccStride * 4 +
                            kTileN * 4 /* norms */ + kChunkWords * 32 * 4 /* visited-block list */;
 static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
+
+// wide search (k <= 64): 64 query rows per CTA, running top-96 lists in shared memory
+constexpr int kWideTileM = 64;
+constexpr int kAOpBytes = kWideTileM * kRowBytes;              // 8 KB: one 64-row query operand block (hi or lo)
+constexpr int kWideStageBytes = 2 * kAOpBytes + 2 * kOpBytes;  // A hi, A lo, B hi, B lo = 48 KB
+constexpr int kWideBuilders = kWideTileM + kTileN;             // 192: one builder thread per operand row
+constexpr int kWideThreads = 256;                              // two warpgroups, one per 64-candidate half of a tile
+constexpr int kWideSmemBytes = kStages * kWideStageBytes + 1024 /* alignment slack */ +
+                               kWideTileM * kAccStride * 4 + kTileN * 4 /* norms */ +
+                               kChunkWords * 32 * 4 /* visited-block list */ +
+                               kWideTileM * kWideListStride * 8 /* lists */;
+static_assert(kWideSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 
 constexpr float kInf = __builtin_huge_valf();
 
@@ -342,6 +358,186 @@ knn_csr_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __restr
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// wide tiles (k <= 64): as knn_csr_tile_kernel for 64 query rows, one running top-96 per row in shared memory; the
+// two warpgroups issue wgmma.m64n64k16 on the two halves of the candidate tile
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kWideThreads, 1)
+knn_csr_wide_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
+                         const float* __restrict__ vals, const float* __restrict__ norms,
+                         const uint32_t* __restrict__ bitmap, int nwords, int64_t n, int num_tiles,
+                         int32_t* __restrict__ cand_idx, float* __restrict__ cand_val) {
+  extern __shared__ uint8_t smem_raw[];
+  // carve: [stages x 48 KB, 1024-aligned] | staged accumulators [64][kAccStride] | norms[128] | visited blocks |
+  //        list distances [64][kWideListStride] | list indices [64][kWideListStride]
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
+  float* s_acc = reinterpret_cast<float*>(gen + kStages * kWideStageBytes);
+  float* s_norm = s_acc + kWideTileM * kAccStride;
+  int* s_list = reinterpret_cast<int*>(s_norm + kTileN);
+  float* s_ld = reinterpret_cast<float*>(s_list + kChunkWords * 32);
+  int* s_li = reinterpret_cast<int*>(s_ld + kWideTileM * kWideListStride);
+  using Scan = cub::BlockScan<int, kWideThreads>;
+  __shared__ typename Scan::TempStorage scan_tmp;
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int64_t row0 = (int64_t)blockIdx.x * kWideTileM;
+  // the query rows use the bitmap of their 128-row tile: a superset of their own blocks (a block only the other
+  // half of that tile occupies is built with zero query rows and adds exactly 0)
+  const uint32_t* abm = bitmap + (row0 / kTileM) * nwords;
+
+  // ----- builder role: thread tid owns operand row tid of A (query rows, tid < 64) or row tid - 64 of B (up to
+  // tid 191); warps 6 and 7 build nothing
+  const bool builder = tid < kWideBuilders;  // (warp-uniform)
+  const bool is_b = tid >= kWideTileM;
+  const int orow = is_b ? tid - kWideTileM : tid;
+  const uint32_t my_off = (is_b ? 2 * kAOpBytes : 0) + orow * kRowBytes;
+  const uint32_t lo_off = is_b ? kOpBytes : kAOpBytes;  // from the hi block to the lo block of the operand
+  const int swz = orow & 7;
+  int64_t a_beg = 0, a_end = 0;
+  if (!is_b && row0 + orow < n) { a_beg = indptr[row0 + orow]; a_end = indptr[row0 + orow + 1]; }
+
+  // ----- consumer role: warpgroup wg multiplies the 64 query rows by candidates 64 wg .. 64 wg + 63 of the tile;
+  // the scanners, threads 0-127, own the query rows, two adjacent lanes per row
+  const int wg = warp >> 2;
+  const bool scanner = tid < 128;  // (warp-uniform)
+  const int lrow = (tid & 127) >> 1, half = tid & 1;
+  const int64_t row = row0 + lrow;
+  const int frow = 16 * (warp & 3) + (lane >> 2), fcol = 64 * wg + 2 * (lane & 3);
+  WideList list;
+  if (scanner) list.init(s_ld + lrow * kWideListStride, s_li + lrow * kWideListStride, half);
+  float acc[32];
+
+  int stage = 0;
+  for (int t = 0; t < num_tiles; ++t) {
+    int64_t p = a_beg, end = a_end;
+    if (is_b) {
+      const int64_t r = (int64_t)t * kTileN + orow;
+      p = end = 0;
+      if (builder && r < n) { p = indptr[r]; end = indptr[r + 1]; }
+    }
+    int cur = p < end ? cols[p] : INT_MAX;
+    const uint32_t* bbm = bitmap + (int64_t)t * nwords;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[i] = 0.0f;
+
+    for (int w0 = 0; w0 < nwords; w0 += kChunkWords) {
+      __syncthreads();  // every thread is done with s_list (and, on the first chunk, with the last tile's scan)
+      uint32_t m = 0;
+      if (tid < kChunkWords && w0 + tid < nwords) m = __ldg(abm + w0 + tid) & __ldg(bbm + w0 + tid);
+      int pos, total;
+      Scan(scan_tmp).ExclusiveSum(__popc(m), pos, total);
+      for (; m; m &= m - 1) s_list[pos++] = (w0 + tid) * 32 + (__ffs(m) - 1);
+      __syncthreads();
+      for (int i = 0; i < total; ++i) {
+        const int lo = s_list[i] * kBlockK, hi = lo + kBlockK;
+        // the stage was last read by the wgmmas of block i - 2, which the consumers waited for before the barrier
+        // of block i - 1
+        uint8_t* rh = gen + stage * kWideStageBytes + my_off;
+        if (builder) {
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {
+            reinterpret_cast<uint4*>(rh)[c] = make_uint4(0, 0, 0, 0);
+            reinterpret_cast<uint4*>(rh + lo_off)[c] = make_uint4(0, 0, 0, 0);
+          }
+        }
+        while (cur < hi) {
+          if (cur >= lo) {
+            const float x = vals[p];
+            const __nv_bfloat16 h = __float2bfloat16_rn(x);
+            const __nv_bfloat16 l = __float2bfloat16_rn(x - __bfloat162float(h));
+            const int k = cur - lo;
+            const int off = (((k >> 3) ^ swz) << 4) | ((k & 7) << 1);
+            *reinterpret_cast<__nv_bfloat16*>(rh + off) = h;
+            *reinterpret_cast<__nv_bfloat16*>(rh + lo_off + off) = l;
+          }
+          ++p;
+          cur = p < end ? cols[p] : INT_MAX;
+        }
+        fence_proxy_async();  // generic-proxy stores above, read next by wgmma (async proxy)
+        wgmma_wait_all();     // this warpgroup's wgmmas of block i - 1 are done with the other stage
+        __syncthreads();
+        const uint32_t sa = base + stage * kWideStageBytes;
+        const uint64_t ah = smem_desc_sw128(sa), al = smem_desc_sw128(sa + kAOpBytes);
+        const uint64_t bh = smem_desc_sw128(sa + 2 * kAOpBytes + wg * 64 * kRowBytes);
+        const uint64_t bl = smem_desc_sw128(sa + 2 * kAOpBytes + kOpBytes + wg * 64 * kRowBytes);
+#pragma unroll
+        for (int q = 0; q < 32; ++q) fence_operand(acc[q]);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
+          const uint64_t adv = (uint64_t)((k * kWgmmaK * 2) >> 4);
+          wgmma_bf16_n64(acc, ah + adv, bh + adv, 1u);
+          wgmma_bf16_n64(acc, ah + adv, bl + adv, 1u);
+          wgmma_bf16_n64(acc, al + adv, bh + adv, 1u);
+        }
+        wgmma_commit();
+        stage ^= 1;
+      }
+    }
+    wgmma_wait_all();
+#pragma unroll
+    for (int q = 0; q < 32; ++q) fence_operand(acc[q]);
+#pragma unroll
+    for (int j = 0; j < 64 / 8; ++j) {
+      *reinterpret_cast<float2*>(s_acc + frow * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(s_acc + (frow + 8) * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+    if (tid < kTileN) s_norm[tid] = __ldg(norms + (int64_t)t * kTileN + tid);
+    __syncthreads();
+    if (scanner) {
+      // both lanes of the row offer every column, in column order
+      const float2* arow = reinterpret_cast<const float2*>(s_acc + lrow * kAccStride);
+      const float2* sn = reinterpret_cast<const float2*>(s_norm);
+#pragma unroll 2
+      for (int i = 0; i < kTileN / 2; ++i) {
+        const float2 a = arow[i], s = sn[i];
+        const int col = t * kTileN + 2 * i;
+        if (col != row && col < n) list.offer(fmaf(-2.0f, a.x, s.x), col);
+        if (col + 1 != row && col + 1 < n) list.offer(fmaf(-2.0f, a.y, s.y), col + 1);
+      }
+    }
+  }
+  if (scanner && row < n) list.store(cand_idx + row * kWideKK, cand_val + row * kWideKK);
+}
+
+// One warp per row, lane q re-ranks candidates q, q + 32 and q + 64 by the merge of knn_csr_rerank_kernel; the k
+// smallest (distance, index) of the 96 in ascending order.
+__global__ void __launch_bounds__(256)
+knn_csr_wide_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
+                           const float* __restrict__ vals, int64_t n, const int32_t* __restrict__ cand_idx, int k,
+                           int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= n) return;
+  constexpr int kPer = kWideKK / 32;
+  float my_d[kPer];
+  int mine[kPer];
+#pragma unroll
+  for (int s = 0; s < kPer; ++s) {
+    const int c = cand_idx[row * kWideKK + 32 * s + lane];
+    my_d[s] = c >= 0 ? (float)merge_dist2(indptr, cols, vals, row, c) : kInf;
+    mine[s] = c >= 0 ? c : INT_MAX;  // missing candidates last
+  }
+  int rank[kPer] = {};
+#pragma unroll
+  for (int s2 = 0; s2 < kPer; ++s2) {
+    for (int q = 0; q < 32; ++q) {
+      const float od = __shfl_sync(kFull, my_d[s2], q);
+      const int oi = __shfl_sync(kFull, mine[s2], q);
+#pragma unroll
+      for (int s = 0; s < kPer; ++s) rank[s] += before(od, oi, my_d[s], mine[s]);
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < kPer; ++s) {
+    if (rank[s] < k) {
+      out_idx[row * k + rank[s]] = mine[s];
+      out_d2[row * k + rank[s]] = my_d[s];
+    }
+  }
+}
+
 // One thread per pair (the rows of a pair are walked in column order: the same fp64 sum every run).
 __global__ void __launch_bounds__(256)
 pair_dist_csr_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
@@ -366,7 +562,8 @@ struct CsrKnnLayout {
       off_kout, off_val, off_tmp, tmp_bytes, total;
 };
 
-int csr_knn_layout(int64_t n, int d, int64_t nnz, CsrKnnLayout* L) {
+// kk: candidates kept per row (kKK, or kWideKK for the wide search)
+int csr_knn_layout(int64_t n, int d, int64_t nnz, CsrKnnLayout* L, int kk = kKK) {
   L->n_pad = (n + kTileN - 1) / kTileN * kTileN;
   L->num_tiles = (int)(L->n_pad / kTileN);
   const int64_t nkb = ((int64_t)d + kBlockK - 1) / kBlockK;
@@ -385,8 +582,8 @@ int csr_knn_layout(int64_t n, int d, int64_t nnz, CsrKnnLayout* L) {
   size_t o = 0;
   L->off_flag = o; o = up(o + 4);
   L->off_norm = o; o = up(o + (size_t)L->n_pad * 4);
-  L->off_ci = o; o = up(o + (size_t)n * kKK * 4);
-  L->off_cv = o; o = up(o + (size_t)n * kKK * 4);
+  L->off_ci = o; o = up(o + (size_t)n * kk * 4);
+  L->off_cv = o; o = up(o + (size_t)n * kk * 4);
   L->off_cnt = o; o = up(o + (size_t)d * 4);
   L->off_cnt_s = o; o = up(o + (size_t)d * 4);
   L->off_iota = o; o = up(o + (size_t)d * 4);
@@ -414,6 +611,48 @@ int check_csr(const int64_t* indptr, const int32_t* indices, const float* values
   return flag ? MDE_E_INVALID : 0;
 }
 
+// The preparation both tile kernels read (workspace carved by csr_knn_layout at w): validates the CSR (blocking
+// status read), writes the norms, the feature permutation, the rows re-sorted under it (cols / vals at off_kin /
+// off_val) and the per-tile occupancy bitmaps.
+int prepare_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
+                const CsrKnnLayout& L, uint8_t* w, cudaStream_t st) {
+  int* flag = reinterpret_cast<int*>(w + L.off_flag);
+  float* norms = reinterpret_cast<float*>(w + L.off_norm);
+  int32_t* cnt = reinterpret_cast<int32_t*>(w + L.off_cnt);
+  int32_t* cnt_s = reinterpret_cast<int32_t*>(w + L.off_cnt_s);
+  int32_t* iota = reinterpret_cast<int32_t*>(w + L.off_iota);
+  int32_t* col_s = reinterpret_cast<int32_t*>(w + L.off_col_s);
+  int32_t* perm = reinterpret_cast<int32_t*>(w + L.off_perm);
+  uint32_t* bm = reinterpret_cast<uint32_t*>(w + L.off_bm);
+  uint64_t* kin = reinterpret_cast<uint64_t*>(w + L.off_kin);
+  uint64_t* kout = reinterpret_cast<uint64_t*>(w + L.off_kout);
+  int32_t* cols = reinterpret_cast<int32_t*>(w + L.off_kin);
+  float* vals = reinterpret_cast<float*>(w + L.off_val);
+  void* tmp = w + L.off_tmp;
+  size_t tmp_bytes = L.tmp_bytes;
+
+  MDE_CUDA_TRY(cudaMemsetAsync(cnt, 0, (size_t)d * 4, st));
+  int rc;
+  if ((rc = check_csr(indptr, indices, values, n, d, nnz, L.n_pad, flag, cnt, norms, st))) return rc;
+  // features by descending document frequency (stable: equal counts keep column order)
+  iota_kernel<<<(d + 255) / 256, 256, 0, st>>>(iota, d);
+  MDE_LAUNCH_CHECK();
+  MDE_CUDA_TRY(cub::DeviceRadixSort::SortPairsDescending(tmp, tmp_bytes, cnt, cnt_s, iota, col_s, d, 0, 32, st));
+  invert_perm_kernel<<<(d + 255) / 256, 256, 0, st>>>(col_s, d, perm);
+  MDE_LAUNCH_CHECK();
+  MDE_CUDA_TRY(cudaMemsetAsync(bm, 0, (size_t)L.num_tiles * L.nwords * 4, st));
+  if (nnz > 0) {
+    csr_keys_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(indptr, indices, perm, n, L.col_bits, L.nwords, kin, bm);
+    MDE_LAUNCH_CHECK();
+    tmp_bytes = L.tmp_bytes;
+    MDE_CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, kin, kout, values, vals, (int64_t)nnz, 0,
+                                                 L.row_bits + L.col_bits, st));
+    key_to_col_kernel<<<(unsigned)((nnz + 255) / 256), 256, 0, st>>>(kout, nnz, (1ull << L.col_bits) - 1, cols);
+    MDE_LAUNCH_CHECK();
+  }
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -439,41 +678,13 @@ int mde_knn_csr(const int64_t* indptr, const int32_t* indices, const float* valu
   if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   uint8_t* w = static_cast<uint8_t*>(ws);
-  int* flag = reinterpret_cast<int*>(w + L.off_flag);
-  float* norms = reinterpret_cast<float*>(w + L.off_norm);
+  if ((rc = prepare_csr(indptr, indices, values, n, d, nnz, L, w, st))) return rc;
+  const float* norms = reinterpret_cast<const float*>(w + L.off_norm);
   int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
   float* cv = reinterpret_cast<float*>(w + L.off_cv);
-  int32_t* cnt = reinterpret_cast<int32_t*>(w + L.off_cnt);
-  int32_t* cnt_s = reinterpret_cast<int32_t*>(w + L.off_cnt_s);
-  int32_t* iota = reinterpret_cast<int32_t*>(w + L.off_iota);
-  int32_t* col_s = reinterpret_cast<int32_t*>(w + L.off_col_s);
-  int32_t* perm = reinterpret_cast<int32_t*>(w + L.off_perm);
-  uint32_t* bm = reinterpret_cast<uint32_t*>(w + L.off_bm);
-  uint64_t* kin = reinterpret_cast<uint64_t*>(w + L.off_kin);
-  uint64_t* kout = reinterpret_cast<uint64_t*>(w + L.off_kout);
-  int32_t* cols = reinterpret_cast<int32_t*>(w + L.off_kin);
-  float* vals = reinterpret_cast<float*>(w + L.off_val);
-  void* tmp = w + L.off_tmp;
-  size_t tmp_bytes = L.tmp_bytes;
-
-  MDE_CUDA_TRY(cudaMemsetAsync(cnt, 0, (size_t)d * 4, st));
-  if ((rc = check_csr(indptr, indices, values, n, d, nnz, L.n_pad, flag, cnt, norms, st))) return rc;
-  // features by descending document frequency (stable: equal counts keep column order)
-  iota_kernel<<<(d + 255) / 256, 256, 0, st>>>(iota, d);
-  MDE_LAUNCH_CHECK();
-  MDE_CUDA_TRY(cub::DeviceRadixSort::SortPairsDescending(tmp, tmp_bytes, cnt, cnt_s, iota, col_s, d, 0, 32, st));
-  invert_perm_kernel<<<(d + 255) / 256, 256, 0, st>>>(col_s, d, perm);
-  MDE_LAUNCH_CHECK();
-  MDE_CUDA_TRY(cudaMemsetAsync(bm, 0, (size_t)L.num_tiles * L.nwords * 4, st));
-  if (nnz > 0) {
-    csr_keys_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(indptr, indices, perm, n, L.col_bits, L.nwords, kin, bm);
-    MDE_LAUNCH_CHECK();
-    tmp_bytes = L.tmp_bytes;
-    MDE_CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, kin, kout, values, vals, (int64_t)nnz, 0,
-                                                 L.row_bits + L.col_bits, st));
-    key_to_col_kernel<<<(unsigned)((nnz + 255) / 256), 256, 0, st>>>(kout, nnz, (1ull << L.col_bits) - 1, cols);
-    MDE_LAUNCH_CHECK();
-  }
+  const uint32_t* bm = reinterpret_cast<const uint32_t*>(w + L.off_bm);
+  const int32_t* cols = reinterpret_cast<const int32_t*>(w + L.off_kin);
+  const float* vals = reinterpret_cast<const float*>(w + L.off_val);
   static bool attr_set = false;
   if (!attr_set) {
     MDE_CUDA_TRY(cudaFuncSetAttribute(knn_csr_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
@@ -483,6 +694,49 @@ int mde_knn_csr(const int64_t* indptr, const int32_t* indices, const float* valu
                                                                            L.num_tiles, ci, cv);
   MDE_LAUNCH_CHECK();
   knn_csr_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(indptr, cols, vals, n, ci, k, idx_out, d2_out);
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+
+int mde_knn_csr_wide_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes) {
+  if (!bytes || n < 2 || d < 1 || nnz < 0) return MDE_E_INVALID;
+  CsrKnnLayout L;
+  int rc = csr_knn_layout(n, d, nnz, &L, kWideKK);
+  if (rc) return rc;
+  *bytes = L.total;
+  return 0;
+}
+
+int mde_knn_csr_wide(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                     int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream) {
+  if (!indptr || !idx_out || !d2_out || !ws || n < 2 || d < 1 || nnz < 0 || k < 1 || k > kWideMaxK || k > n - 1)
+    return MDE_E_INVALID;
+  if (nnz > 0 && (!indices || !values)) return MDE_E_INVALID;
+  if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
+  CsrKnnLayout L;
+  int rc = csr_knn_layout(n, d, nnz, &L, kWideKK);
+  if (rc) return rc;
+  if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* w = static_cast<uint8_t*>(ws);
+  if ((rc = prepare_csr(indptr, indices, values, n, d, nnz, L, w, st))) return rc;
+  const float* norms = reinterpret_cast<const float*>(w + L.off_norm);
+  int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
+  float* cv = reinterpret_cast<float*>(w + L.off_cv);
+  const uint32_t* bm = reinterpret_cast<const uint32_t*>(w + L.off_bm);
+  const int32_t* cols = reinterpret_cast<const int32_t*>(w + L.off_kin);
+  const float* vals = reinterpret_cast<const float*>(w + L.off_val);
+  static bool attr_set = false;
+  if (!attr_set) {
+    MDE_CUDA_TRY(cudaFuncSetAttribute(knn_csr_wide_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      kWideSmemBytes));
+    attr_set = true;
+  }
+  const unsigned grid = (unsigned)((n + kWideTileM - 1) / kWideTileM);
+  knn_csr_wide_tile_kernel<<<grid, kWideThreads, kWideSmemBytes, st>>>(indptr, cols, vals, norms, bm, L.nwords, n,
+                                                                        L.num_tiles, ci, cv);
+  MDE_LAUNCH_CHECK();
+  knn_csr_wide_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(indptr, cols, vals, n, ci, k, idx_out, d2_out);
   MDE_LAUNCH_CHECK();
   return 0;
 }

@@ -27,6 +27,19 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[64], uint64_t adesc, uint6
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
+// D[64 x 64] (+)= A[smem, 64 x 16] * B[smem, 64 x 16]^T: the same fragment layout with j < 8.
+__device__ __forceinline__ void wgmma_bf16_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+
 // Shared-memory matrix descriptor (sm_90 wgmma) of a K-major operand block in the 128-byte swizzle layout (the one
 // TMA writes with CU_TENSOR_MAP_SWIZZLE_128B): rows of 128 bytes, 8-row groups 1024 bytes apart (stride byte
 // offset), one swizzle atom along K (leading byte offset unused), layout type 1 = SWIZZLE_128B in bits 62-63.

@@ -1,10 +1,12 @@
 """Problem construction from a data matrix (interface of pymde/preprocess/data_matrix.py).
 
-k-nearest neighbours are computed EXACTLY on the GPU by the library's own kernel (`mde_knn`: wgmma tensor-core
-cross terms with a running top-32 per row and an exact fp32 re-rank, csrc/mde_knn.cu) for k <= 24; larger k uses row
-chunks of a library GEMM + top-k.  The reference uses scikit-learn brute force below 10 000 rows and the approximate
-pynndescent above (data_matrix.py:125-143).  A scipy.sparse matrix is searched without densifying it (`mde_knn_csr`,
-csrc/mde_knn_sparse.cu), and its pair distances come from sorted merges of CSR rows (`mde_pair_dist_csr`)."""
+k-nearest neighbours are computed EXACTLY on the GPU by the library's own kernels (`mde_knn`: wgmma tensor-core
+cross terms with a running top-32 per row and an exact fp32 re-rank, csrc/mde_knn.cu) for k <= 24, and by their wide
+variants (`mde_knn_wide`: a running top-96 per row in shared memory) for 24 < k <= 64; larger k uses row chunks of a
+library GEMM + top-k.  The reference uses scikit-learn brute force below 10 000 rows and the approximate pynndescent
+above (data_matrix.py:125-143).  A scipy.sparse matrix is searched without densifying it for k <= 64 (`mde_knn_csr`,
+`mde_knn_csr_wide`, csrc/mde_knn_sparse.cu), and its pair distances come from sorted merges of CSR rows
+(`mde_pair_dist_csr`)."""
 import ctypes as C
 import os
 
@@ -38,24 +40,27 @@ def _to_device_csr(data, device):
 
 def knn_sparse_device(csr, shape, k):
     """(indices [n, k] int32, squared distances [n, k] fp32) of the k nearest rows of every row of a device CSR
-    matrix from `_to_device_csr`, ascending by (distance, index); the kernel behind `mde_knn_csr`
-    (include/mde_b200.h)."""
+    matrix from `_to_device_csr`, ascending by (distance, index); the kernel behind `mde_knn_csr` for k <= 24 and
+    `mde_knn_csr_wide` for 24 < k <= 64 (include/mde_b200.h)."""
     from .. import _lib
     lib = _lib.load()
+    wide = k > lib.mde_knn_max_k()
+    ws_bytes, search = ((lib.mde_knn_csr_wide_ws_bytes, lib.mde_knn_csr_wide) if wide
+                        else (lib.mde_knn_csr_ws_bytes, lib.mde_knn_csr))
     indptr, indices, values = csr
     n, d = shape
     nnz = int(indices.shape[0])
     dev = indptr.device
     need = C.c_size_t(0)
-    _lib.check(lib.mde_knn_csr_ws_bytes(int(n), int(d), nnz, C.byref(need)))
+    _lib.check(ws_bytes(int(n), int(d), nnz, C.byref(need)))
     ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=dev)
     off = (-ws.data_ptr()) % 1024
     idx = torch.empty((n, k), dtype=torch.int32, device=dev)
     d2 = torch.empty((n, k), dtype=torch.float32, device=dev)
     with torch.cuda.device(dev):
         stream = torch.cuda.current_stream().cuda_stream
-        _lib.check(lib.mde_knn_csr(indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), int(n), int(d), nnz,
-                                   int(k), idx.data_ptr(), d2.data_ptr(), ws.data_ptr() + off, need.value, stream))
+        _lib.check(search(indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), int(n), int(d), nnz, int(k),
+                          idx.data_ptr(), d2.data_ptr(), ws.data_ptr() + off, need.value, stream))
         torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
     return idx, d2
 
@@ -84,21 +89,24 @@ def _knn_graph(idx, d2, n, max_distance, dev):
 
 def knn_device(X, k):
     """(indices [n, k] int32, squared distances [n, k] fp32) of the k nearest rows of every row of the CUDA fp32
-    matrix X, ascending; the wgmma kernel behind `mde_knn` (include/mde_b200.h)."""
+    matrix X, ascending; the wgmma kernel behind `mde_knn` for k <= 24 and `mde_knn_wide` for 24 < k <= 64
+    (include/mde_b200.h)."""
     from .. import _lib
     lib = _lib.load()
+    wide = k > lib.mde_knn_max_k()
+    ws_bytes, search = (lib.mde_knn_wide_ws_bytes, lib.mde_knn_wide) if wide else (lib.mde_knn_ws_bytes, lib.mde_knn)
     X = X.contiguous()
     n, d = X.shape
     need = C.c_size_t(0)
-    _lib.check(lib.mde_knn_ws_bytes(int(n), int(d), C.byref(need)))
+    _lib.check(ws_bytes(int(n), int(d), C.byref(need)))
     ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=X.device)
     off = (-ws.data_ptr()) % 1024
     idx = torch.empty((n, k), dtype=torch.int32, device=X.device)
     d2 = torch.empty((n, k), dtype=torch.float32, device=X.device)
     with torch.cuda.device(X.device):
         stream = torch.cuda.current_stream().cuda_stream
-        _lib.check(lib.mde_knn(X.data_ptr(), int(n), int(d), int(k), idx.data_ptr(), d2.data_ptr(),
-                               ws.data_ptr() + off, need.value, stream))
+        _lib.check(search(X.data_ptr(), int(n), int(d), int(k), idx.data_ptr(), d2.data_ptr(), ws.data_ptr() + off,
+                          need.value, stream))
         torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
     return idx, d2
 
@@ -111,14 +119,14 @@ def k_nearest_neighbors(data, k, max_distance=None, verbose=False, device=None, 
     if sp.issparse(data):
         n = data.shape[0]
         k = int(min(k, n - 1))
-        if use_kernel and 1 <= k <= _lib.load().mde_knn_max_k():
+        if use_kernel and 1 <= k <= _lib.load().mde_knn_wide_max_k():
             csr, shape = _to_device_csr(data, dev)
             idx, d2 = knn_sparse_device(csr, shape, k)
             return _knn_graph(idx, d2, n, max_distance, dev)
     X = _to_device_matrix(data, dev)
     n = X.shape[0]
     k = int(min(k, n - 1))
-    if use_kernel and 1 <= k <= _lib.load().mde_knn_max_k():
+    if use_kernel and 1 <= k <= _lib.load().mde_knn_wide_max_k():
         idx, d2 = knn_device(X, k)
         return _knn_graph(idx, d2, n, max_distance, dev)
     sq = (X * X).sum(1)

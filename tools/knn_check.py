@@ -1,6 +1,8 @@
-"""mde_knn (wgmma cross terms + running top-32 + exact re-rank) against an fp64 brute force, and timed against the
-library-GEMM + torch.topk path it replaces.  Usage: python tools/knn_check.py [small|full]"""
-import json, os, sys, time
+"""mde_knn (wgmma cross terms + running top-32 + exact re-rank; mde_knn_wide and its top-96 for 24 < k <= 64) against
+an fp64 brute force, and timed against the library-GEMM + torch.topk path it replaces.  At k <= 24 the full run also
+times mde_knn_wide on the same matrix.  One JSON line per shape, with the GPU name and power limit read in the same run.
+Usage: python tools/knn_check.py [small|full] [k]   (k: the neighbours of the full run, default 15)"""
+import json, os, subprocess, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
 from pymde_b200.preprocess import data_matrix as dm
@@ -29,6 +31,34 @@ def gemm_path(X, k, rows=8192):
     return torch.cat(out)
 
 
+def gpu_identity():
+    out = {"gpu": torch.cuda.get_device_name(dev), "power_limit_w": None}
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=10)
+        out["power_limit_w"] = float(r.stdout.strip())
+    except Exception:
+        pass
+    return out
+
+
+def wide_only(X, k):
+    """mde_knn_wide at any k <= 64 (knn_device takes it only above 24)."""
+    import ctypes as C
+    from pymde_b200 import _lib
+    lib = _lib.load()
+    n, d = X.shape
+    need = C.c_size_t(0)
+    _lib.check(lib.mde_knn_wide_ws_bytes(n, d, C.byref(need)))
+    ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=X.device)
+    idx = torch.empty((n, k), dtype=torch.int32, device=X.device)
+    d2 = torch.empty((n, k), dtype=torch.float32, device=X.device)
+    _lib.check(lib.mde_knn_wide(X.data_ptr(), n, d, k, idx.data_ptr(), d2.data_ptr(),
+                                ws.data_ptr() + (-ws.data_ptr()) % 1024, need.value, None))
+    torch.cuda.synchronize()
+    return idx, d2
+
+
 def check(n, d, k, seed, clustered, time_it=False):
     g = torch.Generator(device=dev).manual_seed(seed)
     if clustered:  # MNIST-like: non-negative, many exact zeros, cluster structure
@@ -53,7 +83,12 @@ def check(n, d, k, seed, clustered, time_it=False):
            "kth_distance_max_rel_err_vs_fp64": rel, "rows_with_identical_sets": same, "ascending": ok_sorted,
            "returned_d2_max_rel_err": d2rel, "self_in_list": bool((got == rows[:, None]).any())}
     if time_it:
-        for name, fn in (("kernel_ms", lambda: dm.knn_device(X, k)), ("gemm_topk_ms", lambda: gemm_path(X, k))):
+        arms = [("kernel_ms", lambda: dm.knn_device(X, k)), ("gemm_topk_ms", lambda: gemm_path(X, k))]
+        if k <= 24:
+            arms.append(("wide_kernel_ms", lambda: wide_only(X, k)))
+            wi, wd = wide_only(X, k)
+            rec["wide_d2_identical"] = bool(torch.equal(wd, d2))
+        for name, fn in arms:
             fn(); torch.cuda.synchronize()
             ts = []
             for _ in range(3):
@@ -61,13 +96,16 @@ def check(n, d, k, seed, clustered, time_it=False):
             rec[name] = min(ts)
         flops = 3 * 2.0 * n * n * ((d + 63) // 64 * 64)
         rec["tensor_tflops_at_kernel_ms"] = flops / (rec["kernel_ms"] * 1e-3) / 1e12
+        rec.update(gpu_identity())
     print(json.dumps(rec), flush=True)
     return rec
 
 
 mode = sys.argv[1] if len(sys.argv) > 1 else "small"
+k_full = int(sys.argv[2]) if len(sys.argv) > 2 else 15
 check(1000, 64, 5, 0, False)
 check(3000, 100, 15, 1, False)
 check(5000, 784, 15, 2, True)
+check(5000, 784, 40, 2, True)
 if mode == "full":
-    check(70000, 784, 15, 3, True, time_it=True)
+    check(70000, 784, k_full, 3, True, time_it=True)
