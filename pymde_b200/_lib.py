@@ -72,6 +72,7 @@ SIGNATURES = {
     "mde_project_ws_bytes": (C.c_int64, [C.c_int64, C.c_int]),
     "mde_project_centered": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
     "mde_project_standardized": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
+    "mde_project_status": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.c_void_p]),
     "mde_tangent_standardized": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
     "mde_solver_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int,
                                     C.POINTER(mde_solver_opts_t), C.c_void_p]),

@@ -22,10 +22,14 @@ __device__ __forceinline__ bool inactive(const int* active) { return active != n
 
 // ---- moments: column sums of X and G[a][b] = sum_r Z[r][a] * X[r][b] --------------------------
 // partial layout per block: [m sums][m*m products]
+//
+// shift (GRAM only, nullable): the retraction passes X itself and gets the sums and products of X - s, s =
+// proj_shift(X), stored in shift_out.  Far from the origin, G - n mu mu^T would cancel most of the fp32 digits of G;
+// the shifted rows are as small as the spread of the data, and a constant column gives an exactly zero Gram row.
 template <int M, bool GRAM>
 __global__ void __launch_bounds__(kProjThreads)
 moments_small_kernel(const float* __restrict__ Z, const float* __restrict__ X, int64_t n,
-                     double* __restrict__ partials, const int* active) {
+                     double* __restrict__ partials, const float* shift, double* shift_out, const int* active) {
   if (inactive(active)) return;
   constexpr int K = GRAM ? (M + M * M) : M;
   float acc[K];
@@ -34,6 +38,17 @@ moments_small_kernel(const float* __restrict__ Z, const float* __restrict__ X, i
   double dacc[K];
 #pragma unroll
   for (int k = 0; k < K; ++k) dacc[k] = 0.0;
+  float s[M];
+#pragma unroll
+  for (int c = 0; c < M; ++c) s[c] = 0.0f;
+  if (GRAM && shift) {
+#pragma unroll
+    for (int c = 0; c < M; ++c) s[c] = proj_shift(shift, n, M, c);
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+#pragma unroll
+      for (int c = 0; c < M; ++c) shift_out[c] = (double)s[c];
+    }
+  }
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   int cnt = 0;
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += stride) {
@@ -42,7 +57,7 @@ moments_small_kernel(const float* __restrict__ Z, const float* __restrict__ X, i
     for (int c = 0; c < M; ++c) x[c] = X[r * M + c];
     if (GRAM) {
 #pragma unroll
-      for (int c = 0; c < M; ++c) z[c] = Z[r * M + c];
+      for (int c = 0; c < M; ++c) { x[c] -= s[c]; z[c] = Z[r * M + c] - s[c]; }
     }
 #pragma unroll
     for (int c = 0; c < M; ++c) acc[c] += x[c];
@@ -73,19 +88,25 @@ moments_small_kernel(const float* __restrict__ Z, const float* __restrict__ X, i
 template <bool GRAM>
 __global__ void __launch_bounds__(kProjThreads)
 moments_warp_kernel(const float* __restrict__ Z, const float* __restrict__ X, int64_t n, int m,
-                    double* __restrict__ partials, const int* active) {
+                    double* __restrict__ partials, const float* shift, double* shift_out, const int* active) {
   if (inactive(active)) return;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
   float sum = 0.0f;
   float acc[32];
 #pragma unroll
   for (int b = 0; b < 32; ++b) acc[b] = 0.0f;
+  float s = 0.0f;  // see moments_small_kernel
+  if (GRAM && shift && lane < m) {
+    s = proj_shift(shift, n, m, lane);
+    if (blockIdx.x == 0 && w == 0) shift_out[lane] = (double)s;
+  }
   const int64_t stride = (int64_t)gridDim.x * nw;
   for (int64_t r = (int64_t)blockIdx.x * nw + w; r < n; r += stride) {
     float x = (lane < m) ? X[r * m + lane] : 0.0f;
+    if (GRAM) x -= s;
     sum += x;
     if (GRAM) {
-      float z = (lane < m) ? Z[r * m + lane] : 0.0f;
+      float z = (lane < m) ? Z[r * m + lane] - s : 0.0f;
 #pragma unroll
       for (int b = 0; b < 32; ++b) {
         float xb = __shfl_sync(kFull, x, b);
@@ -208,12 +229,13 @@ __device__ void jacobi_eig_warp(double* A, double* V, int m) {
   __syncwarp();
 }
 
-// MODE 0: mean only.  MODE 1: mean + W = sqrt(n) (Gc)^(-1/2), Gc = G - n mu mu^T.
-// MODE 2: mat = G / n (tangent).
+// MODE 0: mean only.  MODE 1: the partials are moments of X - s (s = shift), d = mean(X - s):
+// mean = s + d and W = sqrt(n) (Gc)^(-1/2), Gc = G_s - n d d^T.  MODE 2: mat = G / n (tangent).
 template <int MODE>
 __global__ void __launch_bounds__(256)
 proj_finalize_kernel(const double* __restrict__ partials, int nblocks, int64_t n, int m,
-                     double* __restrict__ mean, double* __restrict__ mat, int* status, const int* active) {
+                     double* __restrict__ mean, const double* __restrict__ shift, double* __restrict__ mat,
+                     int* status, const int* active) {
   if (inactive(active)) return;
   __shared__ double sA[kProjMaxM * kProjMaxM];
   __shared__ double sV[kProjMaxM * kProjMaxM];
@@ -235,8 +257,11 @@ proj_finalize_kernel(const double* __restrict__ partials, int nblocks, int64_t n
     }
   }
   __syncthreads();
-  if (MODE != 2) {
+  if (MODE == 0) {
     for (int k = threadIdx.x; k < m; k += blockDim.x) mean[k] = sMu[k];
+  }
+  if (MODE == 1) {
+    for (int k = threadIdx.x; k < m; k += blockDim.x) mean[k] = shift[k] + sMu[k];
   }
   if (MODE == 0) return;
   if (MODE == 2) {
@@ -257,8 +282,16 @@ proj_finalize_kernel(const double* __restrict__ partials, int nblocks, int64_t n
     }
     __syncwarp();
     jacobi_eig_warp(sA, sV, m);
-    bool bad = false;
-    for (int k = 0; k < m; ++k) { double l = sA[k * m + k]; if (!(l > 0.0) || !isfinite(l)) bad = true; }
+    // The de-meaned X has rank <= n - 1.  A Gram that is singular in exact arithmetic keeps eigenvalues of the
+    // order of its rounding, of either sign: the test is relative to the largest.
+    bool bad = n <= (int64_t)m;
+    double lmin = sA[0], lmax = sA[0];
+    for (int k = 0; k < m; ++k) {
+      const double l = sA[k * m + k];
+      if (!isfinite(l)) bad = true;
+      lmin = fmin(lmin, l); lmax = fmax(lmax, l);
+    }
+    if (!(lmin > kProjRankTol * lmax)) bad = true;
     if (threadIdx.x == 0 && status) *status = bad ? 1 : 0;
     const double sq = sqrt((double)n);
     for (int k = threadIdx.x; k < m * m; k += 32) {
@@ -350,21 +383,23 @@ int blocks_for_rows(int64_t n, int rows_per_block) {
   return (int)nb;
 }
 
+// shift: null, or the row (X[0]) the retraction's Gram is taken around (see moments_small_kernel)
 template <bool GRAM>
-int launch_moments(const float* Z, const float* X, int64_t n, int m, const ProjWs& w, const int* active,
-                   int* nblocks, cudaStream_t st) {
+int launch_moments(const float* Z, const float* X, int64_t n, int m, const float* shift, const ProjWs& w,
+                   const int* active, int* nblocks, cudaStream_t st) {
   int nb;
+  double* so = w.shift;
   if (m <= 4) {
     nb = blocks_for_rows(n, kProjThreads);
     switch (m) {
-      case 1: moments_small_kernel<1, GRAM><<<nb, kProjThreads, 0, st>>>(Z, X, n, w.partials, active); break;
-      case 2: moments_small_kernel<2, GRAM><<<nb, kProjThreads, 0, st>>>(Z, X, n, w.partials, active); break;
-      case 3: moments_small_kernel<3, GRAM><<<nb, kProjThreads, 0, st>>>(Z, X, n, w.partials, active); break;
-      default: moments_small_kernel<4, GRAM><<<nb, kProjThreads, 0, st>>>(Z, X, n, w.partials, active); break;
+      case 1: moments_small_kernel<1, GRAM><<<nb, kProjThreads, 0, st>>>(Z, X, n, w.partials, shift, so, active); break;
+      case 2: moments_small_kernel<2, GRAM><<<nb, kProjThreads, 0, st>>>(Z, X, n, w.partials, shift, so, active); break;
+      case 3: moments_small_kernel<3, GRAM><<<nb, kProjThreads, 0, st>>>(Z, X, n, w.partials, shift, so, active); break;
+      default: moments_small_kernel<4, GRAM><<<nb, kProjThreads, 0, st>>>(Z, X, n, w.partials, shift, so, active); break;
     }
   } else {
     nb = blocks_for_rows(n, kProjThreads / 32);
-    moments_warp_kernel<GRAM><<<nb, kProjThreads, 0, st>>>(Z, X, n, m, w.partials, active);
+    moments_warp_kernel<GRAM><<<nb, kProjThreads, 0, st>>>(Z, X, n, m, w.partials, shift, so, active);
   }
   MDE_LAUNCH_CHECK();
   *nblocks = nb;
@@ -408,8 +443,8 @@ int enqueue_colmean_wide(const float* X, int64_t n, int m, const ProjWs& w, cons
 int enqueue_project_centered(float* X, int64_t n, int m, const ProjWs& w, const int* active, cudaStream_t st) {
   int nb = 0, rc;
   if (m <= kProjMaxM) {
-    if ((rc = launch_moments<false>(X, X, n, m, w, active, &nb, st))) return rc;
-    proj_finalize_kernel<0><<<1, 256, 0, st>>>(w.partials, nb, n, m, w.mean, w.mat, w.status, active);
+    if ((rc = launch_moments<false>(X, X, n, m, nullptr, w, active, &nb, st))) return rc;
+    proj_finalize_kernel<0><<<1, 256, 0, st>>>(w.partials, nb, n, m, w.mean, w.shift, w.mat, w.status, active);
     MDE_LAUNCH_CHECK();
   } else if ((rc = enqueue_colmean_wide(X, n, m, w, active, st))) return rc;
   int64_t total = n * m;
@@ -425,8 +460,8 @@ int enqueue_project_standardized(float* X, int64_t n, int m, const ProjWs& w, co
   if (proj_wide(m)) return enqueue_project_standardized_wide(X, n, m, w, active, st);
   if (m > kProjMaxM) return MDE_E_UNSUPPORTED;
   int nb = 0, rc;
-  if ((rc = launch_moments<true>(X, X, n, m, w, active, &nb, st))) return rc;
-  proj_finalize_kernel<1><<<1, 256, 0, st>>>(w.partials, nb, n, m, w.mean, w.mat, w.status, active);
+  if ((rc = launch_moments<true>(X, X, n, m, X, w, active, &nb, st))) return rc;
+  proj_finalize_kernel<1><<<1, 256, 0, st>>>(w.partials, nb, n, m, w.mean, w.shift, w.mat, w.status, active);
   MDE_LAUNCH_CHECK();
   return launch_rowmat<0>(X, X, n, m, w, active, st);
 }
@@ -436,8 +471,8 @@ int enqueue_tangent_standardized(const float* X, float* Z, int64_t n, int m, con
   if (proj_wide(m)) return enqueue_tangent_standardized_wide(X, Z, n, m, w, active, st);
   if (m > kProjMaxM) return MDE_E_UNSUPPORTED;
   int nb = 0, rc;
-  if ((rc = launch_moments<true>(Z, X, n, m, w, active, &nb, st))) return rc;
-  proj_finalize_kernel<2><<<1, 256, 0, st>>>(w.partials, nb, n, m, w.mean, w.mat, w.status, active);
+  if ((rc = launch_moments<true>(Z, X, n, m, nullptr, w, active, &nb, st))) return rc;
+  proj_finalize_kernel<2><<<1, 256, 0, st>>>(w.partials, nb, n, m, w.mean, w.shift, w.mat, w.status, active);
   MDE_LAUNCH_CHECK();
   return launch_rowmat<1>(X, Z, n, m, w, active, st);
 }
@@ -460,6 +495,15 @@ int mde_project_standardized(float* X, int64_t n, int m, void* ws, void* stream)
   if (!X || !ws || n < 1 || m < 1) return MDE_E_INVALID;
   if (m > kWideMaxM) return MDE_E_UNSUPPORTED;
   return enqueue_project_standardized(X, n, m, proj_ws_carve(ws, m), nullptr, (cudaStream_t)stream);
+}
+
+int mde_project_status(const void* ws, int m, int* status, void* stream) {
+  if (!ws || !status || m < 1) return MDE_E_INVALID;
+  const ProjWs w = proj_ws_carve(const_cast<void*>(ws), m);
+  const cudaStream_t st = (cudaStream_t)stream;
+  MDE_CUDA_TRY(cudaMemcpyAsync(status, w.status, sizeof(int), cudaMemcpyDeviceToHost, st));
+  MDE_CUDA_TRY(cudaStreamSynchronize(st));
+  return 0;
 }
 
 int mde_tangent_standardized(const float* X, float* Z, int64_t n, int m, void* ws, void* stream) {

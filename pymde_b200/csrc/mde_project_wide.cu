@@ -7,7 +7,8 @@
 //
 //   gram      P[rb] = Z[rows rb]^T X[rows rb]   64 x 64 output tiles, 4 x 4 per thread, fp32 inside a row block
 //   reduce    G = sum_rb P[rb]                  fp64 across row blocks (fixed order)
-//   retraction:   A = (G - n mu mu^T) / n ;  W = A^(-1/2) by the coupled Newton-Schulz iteration
+//   retraction:   G is the Gram of X - s (s = proj_shift, near the column mean) ;  A = (G - n (mu - s)(mu - s)^T) / n ;
+//                 W = A^(-1/2) by the coupled Newton-Schulz iteration
 //                     Y_0 = A / c, Z_0 = I ;  T = (3 I - Z Y) / 2 ;  Y <- Y T ;  Z <- T Z      (Z -> sqrt(c) A^(-1/2))
 //                 in fp64 with c = ||A||_inf >= lambda_max (so the iteration converges for every positive definite
 //                 A); an embedding that is already nearly standardized -- every trial point of the solver -- has
@@ -28,15 +29,26 @@ __device__ __forceinline__ bool inactive(const int* active) { return active != n
 constexpr int kGT = 64;   // Gram output tile
 constexpr int kGK = 16;   // rows per shared-memory stage
 
-// P[rb][a][b] = sum over the rows of row block rb of Z[r][a] X[r][b];  grid = (tiles*tiles, row blocks)
+// P[rb][a][b] = sum over the rows of row block rb of (Z[r][a] - s[a]) (X[r][b] - s[b]);  grid = (tiles*tiles, row
+// blocks).  s = proj_shift(shift) (nullable; the retraction passes X, and s goes to shift_out): the products of the shifted rows
+// keep the fp32 digits that G - n mu mu^T would cancel when the columns sit far from the origin.
 __global__ void __launch_bounds__(256)
 gram_wide_kernel(const float* __restrict__ Z, const float* __restrict__ X, int64_t n, int m, int tiles,
-                 int64_t rows_per_block, float* __restrict__ P, const int* active) {
+                 int64_t rows_per_block, float* __restrict__ P, const float* shift, double* shift_out,
+                 const int* active) {
   if (inactive(active)) return;
   __shared__ __align__(16) float sA[kGK][kGT + 4];
   __shared__ __align__(16) float sB[kGK][kGT + 4];
   const int ta = blockIdx.x / tiles, tb = blockIdx.x % tiles;
   const int ty = threadIdx.x >> 4, tx = threadIdx.x & 15;
+  // every element this thread stages lies in column threadIdx.x & 63 of the two tiles
+  float sa = 0.0f, sb = 0.0f;
+  if (shift) {
+    const int ca = ta * kGT + (threadIdx.x & 63), cb = tb * kGT + (threadIdx.x & 63);
+    if (ca < m) sa = proj_shift(shift, n, m, ca);
+    if (cb < m) sb = proj_shift(shift, n, m, cb);
+    if (blockIdx.y == 0 && tb == 0 && threadIdx.x < kGT && ca < m) shift_out[ca] = (double)sa;
+  }
   const int64_t r0 = (int64_t)blockIdx.y * rows_per_block;
   int64_t r1 = r0 + rows_per_block;
   if (r1 > n) r1 = n;
@@ -53,8 +65,8 @@ gram_wide_kernel(const float* __restrict__ Z, const float* __restrict__ X, int64
       const int kk = e >> 6, c = e & 63;
       const int64_t row = r + kk;
       const int ca = ta * kGT + c, cb = tb * kGT + c;
-      sA[kk][c] = (row < r1 && ca < m) ? Z[row * m + ca] : 0.0f;
-      sB[kk][c] = (row < r1 && cb < m) ? X[row * m + cb] : 0.0f;
+      sA[kk][c] = (row < r1 && ca < m) ? Z[row * m + ca] - sa : 0.0f;
+      sB[kk][c] = (row < r1 && cb < m) ? X[row * m + cb] - sb : 0.0f;
     }
     __syncthreads();
 #pragma unroll
@@ -102,19 +114,23 @@ tangent_mat_kernel(const double* __restrict__ G, int64_t mm, double inv_n, float
   if (k < mm) wf[k] = (float)(G[k] * inv_n);
 }
 
-// retraction: A = sym(G - n mu mu^T) / n, c = ||A||_inf, Y0 = A / c, Z0 = I, flags cleared.  One block.
+// retraction: A = sym(G_s - n d d^T) / n with d = mu - s (G_s is the Gram of X - s), c = ||A||_inf, Y0 = A / c,
+// Z0 = I, flags cleared.  One block.
 __global__ void __launch_bounds__(1024)
-ns_init_kernel(const double* __restrict__ G, const double* __restrict__ mean, int64_t n, int m, double* __restrict__ Y0,
-               double* __restrict__ Z0, double* __restrict__ scal, int* __restrict__ nsflag, int* status,
-               const int* active) {
+ns_init_kernel(const double* __restrict__ G, const double* __restrict__ mean, const double* __restrict__ shift,
+               int64_t n, int m, double* __restrict__ Y0, double* __restrict__ Z0, double* __restrict__ scal,
+               int* __restrict__ nsflag, int* status, const int* active) {
   if (inactive(active)) return;
   __shared__ double s_row[kWideMaxM];
+  __shared__ double s_d[kWideMaxM];
   __shared__ double s_c;
   const double dn = (double)n;
+  for (int a = threadIdx.x; a < m; a += blockDim.x) s_d[a] = mean[a] - shift[a];
+  __syncthreads();
   for (int a = threadIdx.x; a < m; a += blockDim.x) {
     double rs = 0.0;
     for (int b = 0; b < m; ++b) {
-      const double v = 0.5 * (G[(int64_t)a * m + b] + G[(int64_t)b * m + a]) - dn * mean[a] * mean[b];
+      const double v = 0.5 * (G[(int64_t)a * m + b] + G[(int64_t)b * m + a]) - dn * s_d[a] * s_d[b];
       rs += fabs(v);
     }
     s_row[a] = rs / dn;
@@ -122,7 +138,7 @@ ns_init_kernel(const double* __restrict__ G, const double* __restrict__ mean, in
   __syncthreads();
   if (threadIdx.x == 0) {
     double c = 0.0;
-    bool bad = false;
+    bool bad = n <= (int64_t)m;  // the de-meaned X has rank <= n - 1
     for (int a = 0; a < m; ++a) { c = fmax(c, s_row[a]); if (!isfinite(s_row[a])) bad = true; }
     if (!(c > 0.0)) { bad = true; c = 1.0; }
     s_c = c;
@@ -134,7 +150,7 @@ ns_init_kernel(const double* __restrict__ G, const double* __restrict__ mean, in
   const double ic = 1.0 / (s_c * dn);
   for (int k = threadIdx.x; k < m * m; k += blockDim.x) {
     const int a = k / m, b = k % m;
-    Y0[k] = (0.5 * (G[(int64_t)a * m + b] + G[(int64_t)b * m + a]) - dn * mean[a] * mean[b]) * ic;
+    Y0[k] = (0.5 * (G[(int64_t)a * m + b] + G[(int64_t)b * m + a]) - dn * s_d[a] * s_d[b]) * ic;
     Z0[k] = (a == b) ? 1.0 : 0.0;
   }
 }
@@ -280,7 +296,8 @@ rowmat_wide_kernel(const float* __restrict__ X, float* __restrict__ Y, int64_t n
   }
 }
 
-int launch_gram(const float* Z, const float* X, int64_t n, int m, const ProjWs& w, const int* active, cudaStream_t st) {
+int launch_gram(const float* Z, const float* X, int64_t n, int m, const float* shift, const ProjWs& w,
+                const int* active, cudaStream_t st) {
   const int tiles = (m + kGT - 1) / kGT;
   int rb = wide_row_blocks(m);
   const int64_t max_rb = (n + 255) / 256;  // at least 256 rows per block
@@ -290,7 +307,7 @@ int launch_gram(const float* Z, const float* X, int64_t n, int m, const ProjWs& 
   rows_per_block = (rows_per_block + kGK - 1) / kGK * kGK;
   rb = (int)((n + rows_per_block - 1) / rows_per_block);
   dim3 grid(tiles * tiles, rb);
-  gram_wide_kernel<<<grid, 256, 0, st>>>(Z, X, n, m, tiles, rows_per_block, w.fpart, active);
+  gram_wide_kernel<<<grid, 256, 0, st>>>(Z, X, n, m, tiles, rows_per_block, w.fpart, shift, w.shift, active);
   MDE_LAUNCH_CHECK();
   const int64_t mm = (int64_t)m * m;
   gram_reduce_kernel<<<(unsigned)((mm + 255) / 256), 256, 0, st>>>(w.fpart, rb, mm, w.gram, active);
@@ -323,12 +340,12 @@ int enqueue_project_standardized_wide(float* X, int64_t n, int m, const ProjWs& 
   if (!proj_wide(m) || !w.fpart) return MDE_E_UNSUPPORTED;
   int rc;
   if ((rc = enqueue_colmean_wide(X, n, m, w, active, st))) return rc;
-  if ((rc = launch_gram(X, X, n, m, w, active, st))) return rc;
+  if ((rc = launch_gram(X, X, n, m, X, w, active, st))) return rc;
   const int64_t mm = (int64_t)m * m;
   double* Yb[2] = {w.ns, w.ns + mm};
   double* Zb[2] = {w.ns + 2 * mm, w.ns + 3 * mm};
   double* T = w.ns + 4 * mm;
-  ns_init_kernel<<<1, 1024, 0, st>>>(w.gram, w.mean, n, m, Yb[0], Zb[0], w.scal, w.nsflag, w.status, active);
+  ns_init_kernel<<<1, 1024, 0, st>>>(w.gram, w.mean, w.shift, n, m, Yb[0], Zb[0], w.scal, w.nsflag, w.status, active);
   MDE_LAUNCH_CHECK();
   const int g = (m + 31) / 32;
   const double tol = 1e-9 * (double)m, tol2 = tol * tol;
@@ -354,7 +371,7 @@ int enqueue_tangent_standardized_wide(const float* X, float* Z, int64_t n, int m
                                       const int* active, cudaStream_t st) {
   if (!proj_wide(m) || !w.fpart) return MDE_E_UNSUPPORTED;
   int rc;
-  if ((rc = launch_gram(Z, X, n, m, w, active, st))) return rc;
+  if ((rc = launch_gram(Z, X, n, m, nullptr, w, active, st))) return rc;
   const int64_t mm = (int64_t)m * m;
   tangent_mat_kernel<<<(unsigned)((mm + 255) / 256), 256, 0, st>>>(w.gram, mm, 1.0 / (double)n, w.wf, active);
   MDE_LAUNCH_CHECK();

@@ -2,6 +2,7 @@
 
 Everything numerical here is CUDA-only: tensors must live on a CUDA device; there is no CPU
 fallback for the hot path (pymde_b200._lib raises if the extension is missing)."""
+import ctypes
 import numbers
 
 import numpy as np
@@ -203,7 +204,11 @@ def proj_standardized(X, demean=False, inplace=False):
 
     m <= 32: fused Gram + on-device Jacobi kernels; 32 < m <= 256: tiled Gram, Newton-Schulz inverse square root
     and row kernel (csrc/mde_project_wide.cu) -- both behind mde_project_standardized.  Larger m: the same Gram /
-    eigen formulation with the m x m eigenproblem handed to cuSOLVER through torch."""
+    eigen formulation with the m x m eigenproblem handed to cuSOLVER through torch.
+
+    Raises SolverError when X (de-meaned if asked) is numerically rank deficient: a constant or duplicated column,
+    n <= m with demean, or a Gram too ill conditioned for the device's Newton-Schulz iteration.  X may have been
+    overwritten by then when inplace is set."""
     if X.device.type != "cuda":
         raise ValueError("pymde_b200.util.proj_standardized needs a CUDA tensor")
     out = X if inplace else X.detach().clone()
@@ -213,14 +218,20 @@ def proj_standardized(X, demean=False, inplace=False):
     lib = _lib.load()
     if m <= 256 and demean:
         ws = Workspace.get(out.device, lib.mde_project_ws_bytes(n, m))
-        _lib.check(lib.mde_project_standardized(out.data_ptr(), n, m, ws.data_ptr(), stream_ptr(out.device)))
+        stream = stream_ptr(out.device)
+        _lib.check(lib.mde_project_standardized(out.data_ptr(), n, m, ws.data_ptr(), stream))
+        status = ctypes.c_int(0)
+        _lib.check(lib.mde_project_status(ws.data_ptr(), m, ctypes.byref(status), stream))
+        if status.value:
+            raise SolverError("Gram matrix is not positive definite")
         return out
     with torch.no_grad():
         Z = out.double()
         if demean:
             Z = Z - Z.mean(dim=0)
         lam, Q = torch.linalg.eigh(Z.T @ Z)
-        if not bool((lam > 0).all()):
+        # relative: an exactly singular Gram keeps eigenvalues of the order of its rounding, of either sign
+        if not bool(lam[0] > 1e-12 * lam[-1]):
             raise SolverError("Gram matrix is not positive definite")
         W = (Q * lam.rsqrt()) @ Q.T * (float(n) ** 0.5)
         out.copy_((Z @ W).float())
