@@ -237,6 +237,35 @@ int mde_solver_stats(mde_solver_t* s, double* average_distortions_host, double* 
                      double* step_size_percents_host, double* step_lengths_host, int64_t* func_evals_host,
                      void* stream);
 
+/* Distortion functions that are arbitrary callables (pymde/problem.py:36-193 accepts any (p,) -> (p,) torch function):
+ * the solver runs the caller's part of every evaluation between two of its own gated kernels,
+ *     distances d (caller's edge order) -> caller: fpp, loss -> g_k = fpp_k / d_k (non-finite g -> 1) -> gradient scatter
+ * where fpp = d mean_k f(d_k) / d d (fp32) and loss = sum_k f(d_k) (one fp64 value); the loss takes the route of a
+ * built-in loss (a non-finite one ends in MDE_E_NAN where the reference raises SolverError).  The caller's part is
+ * given in one of two forms:
+ *   graph  a cudaGraph_t (as void*) that reads d and writes fpp and loss, with kernel, memset and memcpy nodes only
+ *          (anything else: MDE_E_UNSUPPORTED).  It is added as a child node to every step of the solver's CUDA graphs
+ *          and, unlike the solver's kernels, it is not gated: in the surplus steps after the device paused it runs
+ *          again on a stale d, and nothing reads its result.  The graph is copied; its buffers must outlive the solver.
+ *   hook   fn(user, d, fpp, loss, stream), called on the host at every evaluation, must enqueue the same work on
+ *          `stream` and return 0 (non-zero is returned by mde_solver_run).  Steps are then stream-launched.
+ * Exactly one of `graph` and `fn` is set.  d and fpp hold mde_edges_count(e) floats. */
+typedef int (*mde_external_fn)(void* user, const float* d, float* fpp, double* loss, void* stream);
+typedef struct mde_external {
+  float* d;             /* written by the solver, read by the caller's part */
+  float* fpp;           /* written by the caller's part, read by the solver */
+  double* loss;         /* written by the caller's part, read by the solver */
+  void* graph;          /* cudaGraph_t, or NULL */
+  mde_external_fn fn;   /* or NULL */
+  void* user;
+} mde_external_t;
+/* One GPU only (opts->world_size == 1). */
+int mde_solver_create_external(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m,
+                               const mde_solver_opts_t* opts, const mde_external_t* ext, void* stream);
+/* Replace the caller's part of a solver made by mde_solver_create_external and rebuild its step graphs (a callable
+ * captured anew).  Blocking. */
+int mde_solver_set_external(mde_solver_t* s, const mde_external_t* ext, void* stream);
+
 /* Multi-GPU hook (world_size > 1): after every distortion launch the solver calls
  * `fn(user, buf, count, stream)` which must sum the float32 buffer in place across ranks
  * on `stream` (an NCCL all-reduce).  buf = [partial gradient (n*m) | loss hi | loss lo]. */

@@ -44,6 +44,13 @@ class mde_ell_host_t(C.Structure):
 
 
 ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p)
+# (user, d, fpp, loss, stream) -> int: the caller's part of an evaluation of a callable distortion function
+EXTERNAL_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p)
+
+
+class mde_external_t(C.Structure):
+    _fields_ = [("d", C.c_void_p), ("fpp", C.c_void_p), ("loss", C.c_void_p), ("graph", C.c_void_p),
+                ("fn", EXTERNAL_FN), ("user", C.c_void_p)]
 
 # name -> (restype, argtypes); every symbol include/mde_b200.h declares
 SIGNATURES = {
@@ -85,6 +92,9 @@ SIGNATURES = {
     "mde_solver_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.POINTER(C.c_int64), C.c_void_p]),
     "mde_solver_set_allreduce": (C.c_int, [C.c_void_p, ALLREDUCE_FN, C.c_void_p]),
+    "mde_solver_create_external": (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int,
+                                             C.POINTER(mde_solver_opts_t), C.POINTER(mde_external_t), C.c_void_p]),
+    "mde_solver_set_external": (C.c_int, [C.c_void_p, C.POINTER(mde_external_t), C.c_void_p]),
     "mde_knn_max_k": (C.c_int, []),
     "mde_knn_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,

@@ -654,7 +654,8 @@ __global__ void edge_outputs_kernel(const int32_t* __restrict__ src, const int32
                                     const float* __restrict__ par0, const float* __restrict__ par1,
                                     const int32_t* __restrict__ perm, int64_t p, int m,
                                     const float* __restrict__ X, float* __restrict__ distances,
-                                    float* __restrict__ distortions, FnDev fn) {
+                                    float* __restrict__ distortions, FnDev fn, const int* flag) {
+  if (flag && *flag == 0) return;  // gated inside the device solver's steps (callable distortion functions)
   int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= p) return;
   int s = src[k], t = dst[k];
@@ -880,6 +881,26 @@ int distortion_fused_flag(const mde_edges* e, const float* X, int m, float* grad
   if (e->kind == 1) return tiled_launch(0, e, X, m, grad, nullptr, nblocks, flag, st);
   return launch_distortion<0>(e, X, m, grad, nullptr, nblocks, flag, st);
 }
+// the device solver's evaluation of a callable distortion function (mde_solver.cu): distances in the caller's edge
+// order, then the gradient scatter of the caller-ordered coefficients g; both gated by `flag`
+int edge_distances_flag(const mde_edges* e, const float* X, int m, float* distances, const int* flag,
+                        cudaStream_t st) {
+  if (e->kind == 2) return pull_edge_outputs(e, X, m, distances, nullptr, st, flag);
+  if (e->kind == 1) return tiled_edge_outputs(e, X, m, distances, nullptr, st, flag);
+  int tb = 256, nb = ceil_div_i64(e->p, tb);
+  edge_outputs_kernel<0><<<nb, tb, 0, st>>>(e->src, e->dst, e->par0, nullptr, e->perm, e->p, m, X, distances, nullptr,
+                                            e->fn, flag);
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+int scatter_external_flag(const mde_edges* e, const float* X, int m, const float* g, float* grad, const int* flag,
+                          cudaStream_t st) {
+  if (e->kind == 2) return pull_launch(2, e, X, m, grad, g, nullptr, flag, st);
+  if (e->kind == 1) return tiled_launch(2, e, X, m, grad, g, nullptr, flag, st);
+  return launch_distortion<2>(e, X, m, grad, g, nullptr, flag, st);
+}
+double* loss_partials_mut(const mde_edges* e) { return e->loss_partials; }
+int64_t edges_p(const mde_edges* e) { return e->p; }
 int64_t edges_p_total(const mde_edges* e) { return e->p_total; }
 const double* loss_partials_ptr(const mde_edges* e) { return e->loss_partials; }
 int64_t edges_n(const mde_edges* e) { return e->n; }
@@ -1115,7 +1136,7 @@ int mde_edge_outputs(const mde_edges_t* e, const float* X, int m, float* distanc
   if (e->kind == 1) return tiled_edge_outputs(e, X, m, distances, distortions, st);
   int tb = 256, nb = ceil_div_i64(e->p, tb);
   edge_outputs_kernel<0><<<nb, tb, 0, st>>>(e->src, e->dst, e->par0, e->has_par1 ? e->par1 : nullptr,
-                                            e->perm, e->p, m, X, distances, distortions, e->fn);
+                                            e->perm, e->p, m, X, distances, distortions, e->fn, nullptr);
   MDE_LAUNCH_CHECK();
   return 0;
 }

@@ -89,7 +89,7 @@ void tiled_free(mde_edges* e);
 int tiled_launch(int mode, const mde_edges* e, const float* X, int m, float* grad, const float* gext,
                  int* nblocks_out, const int* flag, cudaStream_t st);
 int tiled_edge_outputs(const mde_edges* e, const float* X, int m, float* distances, float* distortions,
-                       cudaStream_t st);
+                       cudaStream_t st, const int* flag = nullptr);  // flag: gate (nullptr: always runs)
 
 // pull kernel (mde_pull.cu)
 int pull_build(mde_edges* e, const int64_t* edges, const float* par0, const mde_fn_t* fn, int embedding_dim,
@@ -98,7 +98,7 @@ void pull_free(mde_edges* e);
 int pull_launch(int mode, const mde_edges* e, const float* X, int m, float* grad, const float* gext,
                 int* nblocks_out, const int* flag, cudaStream_t st);
 int pull_edge_outputs(const mde_edges* e, const float* X, int m, float* distances, float* distortions,
-                      cudaStream_t st);
+                      cudaStream_t st, const int* flag = nullptr);  // flag: gate (nullptr: always runs)
 
 // ELL pull kernel (mde_ell.cu): fused value + gradient only; everything else runs on the sorted-SoA kernels
 bool ell_supported(int64_t n_items, int embedding_dim);  // shape accepted by the ELL builder (before any allocation)

@@ -425,7 +425,8 @@ __global__ void pull_scatter_kernel(const uint64_t* __restrict__ keys, const uin
 __global__ void pull_outputs_kernel(const int32_t* __restrict__ rec, const int32_t* __restrict__ perm,
                                     const int32_t* __restrict__ wt_tile, int rb, int epl, int64_t nslots, int m,
                                     const float* __restrict__ X, float* __restrict__ distances,
-                                    float* __restrict__ distortions, FnDev fn) {
+                                    float* __restrict__ distortions, FnDev fn, const int* flag) {
+  if (flag && *flag == 0) return;
   const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= nslots) return;
   const int o = perm[k];
@@ -728,11 +729,11 @@ int pull_launch(int mode, const mde_edges* e, const float* X, int m, float* grad
 }
 
 int pull_edge_outputs(const mde_edges* e, const float* X, int m, float* distances, float* distortions,
-                      cudaStream_t st) {
+                      cudaStream_t st, const int* flag) {
   const int64_t nslots = e->nwt * 32 * e->epl;
   const int tb = 256;
   pull_outputs_kernel<<<ceil_div_i64(nslots, tb), tb, 0, st>>>(e->rec, e->perm, e->wt_tile, e->rb, e->epl, nslots, m, X,
-                                                              distances, distortions, e->fn);
+                                                              distances, distortions, e->fn, flag);
   MDE_LAUNCH_CHECK();
   return 0;
 }

@@ -34,7 +34,13 @@ int distortion_fused(const mde_edges* e, const float* X, int m, float* grad, int
 int distortion_fused_flag(const mde_edges* e, const float* X, int m, float* grad, int* nblocks,
                           const int* flag, cudaStream_t st);
 const double* loss_partials_ptr(const mde_edges* e);
+double* loss_partials_mut(const mde_edges* e);
+int edge_distances_flag(const mde_edges* e, const float* X, int m, float* distances, const int* flag,
+                        cudaStream_t st);
+int scatter_external_flag(const mde_edges* e, const float* X, int m, const float* g, float* grad, const int* flag,
+                          cudaStream_t st);
 int64_t edges_n(const mde_edges* e);
+int64_t edges_p(const mde_edges* e);
 int64_t edges_p_total(const mde_edges* e);
 }  // namespace mde
 
@@ -300,6 +306,21 @@ pack_loss_kernel(const int* flag, const double* __restrict__ lpart, int nl, floa
     tail[0] = hi;
     tail[1] = (float)(out[0] - (double)hi);
   }
+}
+
+// callable distortion function: the coefficients g_k = f'(d_k) / d_k the scatter takes (the caller's torch code left
+// fpp = d mean f / d d), non-finite g replaced by 1 like the reference (pymde/average_distortion.py:55-62), and the loss
+// sum f(d).sum() in the layout's first loss-partial slot, where the next head kernel reads it (one partial)
+__global__ void __launch_bounds__(256)
+ext_coeff_kernel(const int* flag, const float* __restrict__ fpp, const float* __restrict__ d,
+                 const double* __restrict__ loss, float* __restrict__ g, double* __restrict__ lpart, int64_t p) {
+  if (off(flag)) return;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < p; k += stride) {
+    const float v = __fdiv_rn(fpp[k], d[k]);  // IEEE division: the same floats as the torch path
+    g[k] = isfinite(v) ? v : 1.0f;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) lpart[0] = *loss;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1199,6 +1220,9 @@ struct mde_solver {
   void* peer_base[kMaxWorld] = {nullptr};
   int64_t* anchors = nullptr;
   float* anchor_values = nullptr;
+  mde_external_t ext{};              // callable distortion function (ext.d != nullptr), see mde_solver_create_external
+  float* gcoef = nullptr;            // (p,) caller-ordered coefficients of the scatter
+  int64_t p = 0;
   // flat step graphs (one step / steps_per_graph steps), no conditional nodes
   int steps_per_graph = 8;           // MDE_B200_STEPS (1..64)
   cudaGraph_t step_graph = nullptr, steps_graph = nullptr;
@@ -1217,13 +1241,41 @@ int read_status(mde_solver* s, cudaStream_t st) {
   return 0;
 }
 
+// callable distortion function: distances -> the caller's torch code -> coefficients -> scatter.  The caller's part is
+// either a CUDA graph, added as a child node of the step graph being captured on `st` (it is not gated: in the surplus
+// steps after the device paused it recomputes fpp and loss from a stale d, and nothing reads them), or a host hook
+// that enqueues the torch ops on `st` (stream-launched steps).
+int enqueue_external(mde_solver* s, const int* flag, cudaStream_t st) {
+  const mde_external_t& x = s->ext;
+  int rc = edge_distances_flag(s->edges, s->X, s->m, x.d, flag, st);
+  if (rc) return rc;
+  if (x.graph) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    cudaGraph_t g = nullptr;
+    const cudaGraphNode_t* deps = nullptr;
+    size_t nd = 0;
+    MDE_CUDA_TRY(cudaStreamGetCaptureInfo(st, &cs, nullptr, &g, &deps, &nd));
+    if (cs != cudaStreamCaptureStatusActive) return MDE_E_INVALID;  // graph mode runs inside the step graphs only
+    cudaGraphNode_t node = nullptr;
+    MDE_CUDA_TRY(cudaGraphAddChildGraphNode(&node, g, deps, nd, (cudaGraph_t)x.graph));
+    MDE_CUDA_TRY(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));
+  } else {
+    if ((rc = x.fn(x.user, x.d, x.fpp, x.loss, (void*)st))) return rc;
+  }
+  int nb = (int)((s->p + 255) / 256);
+  if (nb > kVecBlocks) nb = kVecBlocks;
+  ext_coeff_kernel<<<nb, 256, 0, st>>>(flag, x.fpp, x.d, x.loss, s->gcoef, loss_partials_mut(s->edges), s->p);
+  MDE_LAUNCH_CHECK();
+  return scatter_external_flag(s->edges, s->X, s->m, s->gcoef, s->g, flag, st);
+}
+
 // closure: value_and_grad at s->X (optim.py:100-105) into the gradient buffer the vec kernel zeroed; `flag` gates
 // the kernels.  (g.d, g.g, |g|_1) and the loss are reduced by the next step's head kernel.
 int enqueue_eval(mde_solver* s, const int* flag, cudaStream_t st) {
   // several GPUs: scatter into this rank's partial buffer (peer-visible), then all-reduce into g
   const bool multi = s->opts.world_size > 1;
   float* target = multi ? s->gpart : s->g;
-  int rc = distortion_fused_flag(s->edges, s->X, s->m, target, &s->nl, flag, st);
+  int rc = s->ext.d ? enqueue_external(s, flag, st) : distortion_fused_flag(s->edges, s->X, s->m, target, &s->nl, flag, st);
   if (rc) return rc;
   if (multi) {
     pack_loss_kernel<<<1, 256, 0, st>>>(flag, loss_partials_ptr(s->edges), s->nl, target + s->npad);
@@ -1339,12 +1391,58 @@ int build_step_graph(mde_solver* s, int steps, cudaGraph_t* graph_out, cudaGraph
 #undef GTRY
 }
 
-}  // namespace
+void destroy_step_graphs(mde_solver* s) {
+  if (s->step_exec) cudaGraphExecDestroy(s->step_exec);
+  if (s->step_graph) cudaGraphDestroy(s->step_graph);
+  if (s->steps_exec) cudaGraphExecDestroy(s->steps_exec);
+  if (s->steps_graph) cudaGraphDestroy(s->steps_graph);
+  s->step_exec = s->steps_exec = nullptr;
+  s->step_graph = s->steps_graph = nullptr;
+}
 
-extern "C" {
+// the one-step and the steps_per_graph-step graphs (one GPU, or several once connected)
+int build_step_graphs(mde_solver* s) {
+  int rc = build_step_graph(s, 1, &s->step_graph, &s->step_exec);
+  if (rc) return rc;
+  { const char* ev = getenv("MDE_B200_STEPS"); if (ev) s->steps_per_graph = atoi(ev); }
+  if (s->steps_per_graph < 1) s->steps_per_graph = 1;
+  if (s->steps_per_graph > 64) s->steps_per_graph = 64;
+  return build_step_graph(s, s->steps_per_graph, &s->steps_graph, &s->steps_exec);
+}
 
-int mde_solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m, const mde_solver_opts_t* opts,
-                      void* stream) {
+// a graph the solver can embed as a child node: kernel, memset and memcpy nodes only (no memory-allocation nodes)
+int check_external(const mde_external_t* x) {
+  if (!x->d || !x->fpp || !x->loss || (!x->graph) == (!x->fn)) return MDE_E_INVALID;
+  if (!x->graph) return 0;
+  cudaGraph_t g = (cudaGraph_t)x->graph;
+  size_t n = 0;
+  MDE_CUDA_TRY(cudaGraphGetNodes(g, nullptr, &n));
+  if (n == 0) return MDE_E_INVALID;
+  cudaGraphNode_t* nodes = new (std::nothrow) cudaGraphNode_t[n];
+  if (!nodes) return MDE_E_ALLOC;
+  int rc = 0;
+  cudaError_t e = cudaGraphGetNodes(g, nodes, &n);
+  for (size_t i = 0; e == cudaSuccess && i < n && !rc; ++i) {
+    cudaGraphNodeType t;
+    e = cudaGraphNodeGetType(nodes[i], &t);
+    if (e == cudaSuccess && t != cudaGraphNodeTypeKernel && t != cudaGraphNodeTypeMemset && t != cudaGraphNodeTypeMemcpy)
+      rc = MDE_E_UNSUPPORTED;
+  }
+  delete[] nodes;
+  return e != cudaSuccess ? (int)e : rc;
+}
+
+// (re)build the step graphs around the external part x: graph mode captures them with x's graph inside, hook mode
+// runs stream-launched steps and has no step graphs
+int attach_external(mde_solver* s, const mde_external_t* x) {
+  destroy_step_graphs(s);
+  s->ext = *x;
+  s->nl = 1;  // the loss arrives as one partial (ext_coeff_kernel)
+  return x->graph ? build_step_graphs(s) : 0;
+}
+
+int solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m, const mde_solver_opts_t* opts,
+                  const mde_external_t* ext, void* stream) {
   if (!out || !e || !opts || n < 1 || m < 1) return MDE_E_INVALID;
   if (opts->memory_size < 1 || opts->memory_size > kMaxMemory) return MDE_E_UNSUPPORTED;
   if (opts->constraint == MDE_CONSTRAINT_STANDARDIZED && m > kWideMaxM) return MDE_E_UNSUPPORTED;
@@ -1410,16 +1508,15 @@ int mde_solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m
   }
   s->nvb = vec_blocks(s->npad >> 2);
   if (opts->constraint == MDE_CONSTRAINT_CENTERED && (m == 1 || m == 2 || m == 4)) s->center_m = m;
-  if (opts->world_size == 1) {  // several GPUs: graphs are built by mde_solver_comm_connect
+  if (ext) {  // the descriptor is in place before the first capture
+    s->p = edges_p(e);
+    TRY(cudaMalloc(&s->gcoef, sizeof(float) * s->p));
+    TRY(cudaStreamSynchronize(st));
+    if ((rc = attach_external(s, ext))) goto fail;
+  } else if (opts->world_size == 1) {  // several GPUs: graphs are built by mde_solver_comm_connect
     s->nl = 0;
     TRY(cudaStreamSynchronize(st));
-    rc = build_step_graph(s, 1, &s->step_graph, &s->step_exec);
-    if (rc) goto fail;
-    { const char* ev = getenv("MDE_B200_STEPS"); if (ev) s->steps_per_graph = atoi(ev); }
-    if (s->steps_per_graph < 1) s->steps_per_graph = 1;
-    if (s->steps_per_graph > 64) s->steps_per_graph = 64;
-    rc = build_step_graph(s, s->steps_per_graph, &s->steps_graph, &s->steps_exec);
-    if (rc) goto fail;
+    if ((rc = build_step_graphs(s))) goto fail;
   }
   *out = s;
   return 0;
@@ -1427,6 +1524,31 @@ fail:
   mde_solver_destroy(s);
   return rc;
 #undef TRY
+}
+
+}  // namespace
+
+extern "C" {
+
+int mde_solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m, const mde_solver_opts_t* opts,
+                      void* stream) {
+  return solver_create(out, e, n, m, opts, nullptr, stream);
+}
+
+int mde_solver_create_external(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m,
+                               const mde_solver_opts_t* opts, const mde_external_t* ext, void* stream) {
+  if (!ext || !opts || opts->world_size != 1) return MDE_E_INVALID;
+  const int rc = check_external(ext);
+  if (rc) return rc;
+  return solver_create(out, e, n, m, opts, ext, stream);
+}
+
+int mde_solver_set_external(mde_solver_t* s, const mde_external_t* ext, void* stream) {
+  if (!s || !ext || !s->ext.d) return MDE_E_INVALID;
+  int rc = check_external(ext);
+  if (rc) return rc;
+  MDE_CUDA_TRY(cudaStreamSynchronize((cudaStream_t)stream));  // no step that embeds the old part is in flight
+  return attach_external(s, ext);
 }
 
 int mde_solver_destroy(mde_solver_t* s) {
@@ -1437,11 +1559,8 @@ int mde_solver_destroy(mde_solver_t* s) {
   for (int q = 0; q < kMaxWorld; ++q) if (s->peer_base[q]) cudaIpcCloseMemHandle(s->peer_base[q]);
   cudaFree(s->comm_region); cudaFree(s->comm_dev);
   cudaFree(s->Sb); cudaFree(s->Yb); cudaFree(s->dpart); cudaFree(s->vpart); cudaFree(s->stats); cudaFree(s->projws);
-  cudaFree(s->anchors); cudaFree(s->anchor_values);
-  if (s->step_exec) cudaGraphExecDestroy(s->step_exec);
-  if (s->step_graph) cudaGraphDestroy(s->step_graph);
-  if (s->steps_exec) cudaGraphExecDestroy(s->steps_exec);
-  if (s->steps_graph) cudaGraphDestroy(s->steps_graph);
+  cudaFree(s->anchors); cudaFree(s->anchor_values); cudaFree(s->gcoef);
+  destroy_step_graphs(s);
   if (s->cap_stream) cudaStreamDestroy(s->cap_stream);
   delete s;
   return 0;
@@ -1502,12 +1621,7 @@ int mde_solver_comm_connect(mde_solver_t* s, int rank, const void* handles, int6
   s->comm_connected = 1;
   // the sharded solve runs the same flat step graphs as one GPU
   s->nl = 0;
-  int rc = build_step_graph(s, 1, &s->step_graph, &s->step_exec);
-  if (rc) return rc;
-  { const char* ev = getenv("MDE_B200_STEPS"); if (ev) s->steps_per_graph = atoi(ev); }
-  if (s->steps_per_graph < 1) s->steps_per_graph = 1;
-  if (s->steps_per_graph > 64) s->steps_per_graph = 64;
-  return build_step_graph(s, s->steps_per_graph, &s->steps_graph, &s->steps_exec);
+  return build_step_graphs(s);
 }
 
 int mde_solver_begin(mde_solver_t* s, const float* X0, double eps, void* stream) {
@@ -1562,8 +1676,9 @@ int mde_solver_run(mde_solver_t* s, int iters, int* iters_done, int* converged, 
     if (remaining < 1) remaining = 1;
     long long steps = 0;
     const int spg = s->steps_per_graph;
-    if (s->opts.world_size > 1 && !s->steps_exec) {
-      // host-hook all-reduce: stream-launched steps; every rank enqueues the same number of steps (same `remaining`: the replicated state machines agree)
+    if (!s->steps_exec) {
+      // host hook (all-reduce, or a callable distortion function in hook mode): stream-launched steps; every rank
+      // enqueues the same number of steps (same `remaining`: the replicated state machines agree)
       int n_steps = remaining + remaining / 8 + (round > 0 ? 1 : 0) + 1;
       if (n_steps > 64) n_steps = 64;
       for (int b = 0; b < n_steps; ++b) { if ((rc = enqueue_step(s, st))) return rc; }

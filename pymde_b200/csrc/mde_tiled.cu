@@ -458,7 +458,8 @@ __global__ void scatter_records_kernel(const uint64_t* __restrict__ keys, const 
 
 __global__ void tiled_outputs_kernel(const int32_t* __restrict__ rec, const int32_t* __restrict__ perm, int64_t nslots,
                                      int m, const float* __restrict__ X, float* __restrict__ distances,
-                                     float* __restrict__ distortions, FnDev fn) {
+                                     float* __restrict__ distortions, FnDev fn, const int* flag) {
+  if (flag && *flag == 0) return;
   const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= nslots) return;
   const int o = perm[k];
@@ -720,11 +721,11 @@ int tiled_launch(int mode, const mde_edges* e, const float* X, int m, float* gra
 }
 
 int tiled_edge_outputs(const mde_edges* e, const float* X, int m, float* distances, float* distortions,
-                       cudaStream_t st) {
+                       cudaStream_t st, const int* flag) {
   const int64_t nslots = e->nwt * kWtEdges;
   const int tb = 256;
   tiled_outputs_kernel<<<ceil_div_i64(nslots, tb), tb, 0, st>>>(e->rec, e->perm, nslots, m, X, distances, distortions,
-                                                               e->fn);
+                                                               e->fn, flag);
   MDE_LAUNCH_CHECK();
   return 0;
 }

@@ -4,7 +4,8 @@
 `(X, SolveStats)`.  When `objective_fn` is the bound `MDE.average_distortion` of a problem whose
 distortion function and constraint the CUDA path supports, the whole solve -- L-BFGS history,
 strong-Wolfe line search, projections, statistics -- runs device-resident through
-`mde_solver_*` (include/mde_b200.h); X is updated in place and returned."""
+`mde_solver_*` (include/mde_b200.h); X is updated in place and returned.  A distortion function that is
+an arbitrary callable runs on the same solver, its torch code inside every step (pymde_b200/external.py)."""
 import ctypes as C
 import time
 
@@ -44,7 +45,7 @@ class DeviceSolver(object):
     """Owner of one `mde_solver_t`."""
 
     def __init__(self, layout, n, m, constraint, memory_size, max_iter, world_size=1, allreduce=None,
-                 exchange=None, rank=0):
+                 exchange=None, rank=0, external=None):
         lib = _lib.load()
         self.lib = lib
         self.layout = layout  # keep the edge layout alive
@@ -65,9 +66,15 @@ class DeviceSolver(object):
             opts.anchor_values = values.data_ptr()
             self._keep += [anchors, values]
         handle = C.c_void_p()
+        self._ext = None  # pymde_b200.external.UserPart of a callable distortion function
         with torch.cuda.device(self.device):
-            _lib.check(lib.mde_solver_create(C.byref(handle), layout.handle, self.n, self.m, C.byref(opts),
-                                             util.stream_ptr(self.device)))
+            if external is None:
+                _lib.check(lib.mde_solver_create(C.byref(handle), layout.handle, self.n, self.m, C.byref(opts),
+                                                 util.stream_ptr(self.device)))
+            else:
+                self._attach(external, lambda x: lib.mde_solver_create_external(
+                    C.byref(handle), layout.handle, self.n, self.m, C.byref(opts), C.byref(x),
+                    util.stream_ptr(self.device)))
         self.handle = handle
         self.max_iter = opts.max_iter
         self._cb = None
@@ -86,6 +93,25 @@ class DeviceSolver(object):
         elif allreduce is not None:
             self._cb = _lib.ALLREDUCE_FN(allreduce)
             _lib.check(lib.mde_solver_set_allreduce(self.handle, self._cb, None))
+
+    def _attach(self, ext, call):
+        rc = call(ext.descriptor())
+        if rc == _lib.MDE_E_UNSUPPORTED and ext.mode == "graph":  # node types the solver cannot embed
+            ext.use_hook()
+            rc = call(ext.descriptor())
+        _lib.check(rc)
+        self._ext = ext  # after the library let go of the previous part: its graph and buffers may be freed now
+
+    def set_external(self, ext):
+        """Run the solves from now on with the callable's part `ext` (captured anew for every embed())."""
+        with torch.cuda.device(self.device):
+            self._attach(ext, lambda x: self.lib.mde_solver_set_external(self.handle, C.byref(x),
+                                                                        util.stream_ptr(self.device)))
+
+    @property
+    def external_mode(self):
+        """"graph" or "hook" for a callable distortion function, None for a table function."""
+        return None if self._ext is None else self._ext.mode
 
     def close(self):
         if getattr(self, "handle", None):
@@ -111,6 +137,8 @@ class DeviceSolver(object):
         with torch.cuda.device(self.device):
             rc = self.lib.mde_solver_run(self.handle, int(iters), C.byref(done), C.byref(conv),
                                          util.stream_ptr(self.device))
+        if self._ext is not None:
+            self._ext.raise_error()
         if rc == _lib.MDE_E_NAN:
             raise util.SolverError("Function or gradient evaluation returned NaN/inf.")
         _lib.check(rc)
@@ -168,7 +196,11 @@ def lbfgs(X, objective_fn, constraint, eps, max_iter, memory_size, use_line_sear
     start_time = time.time()
     layout = mde._layout()
     n, m = X.shape
-    solver = mde._solver(constraint, memory_size, max_iter)
+    external = None
+    if not mde._is_table_function():  # a callable: its torch part is captured again for every solve
+        from .external import UserPart
+        external = UserPart(mde.distortion_function, layout.p, layout.device)
+    solver = mde._solver(constraint, memory_size, max_iter, external)
     solver.begin(X, eps, max_iter)
     snapshots, times = [], []
     digits = len(str(max_iter))
