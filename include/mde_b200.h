@@ -70,7 +70,8 @@ typedef struct mde_fn {
 } mde_fn_t;
 
 /* constraint ids -- pymde/constraints.py */
-enum { MDE_CONSTRAINT_CENTERED = 0, MDE_CONSTRAINT_STANDARDIZED = 1, MDE_CONSTRAINT_ANCHORED = 2 };
+enum { MDE_CONSTRAINT_CENTERED = 0, MDE_CONSTRAINT_STANDARDIZED = 1, MDE_CONSTRAINT_ANCHORED = 2,
+       MDE_CONSTRAINT_CUSTOM = 3 /* caller-defined projections: mde_solver_create_custom only */ };
 
 typedef struct mde_edges mde_edges_t;   /* device-resident edge layout (one shard) */
 typedef struct mde_solver mde_solver_t; /* device-resident projected L-BFGS state */
@@ -265,6 +266,39 @@ int mde_solver_create_external(mde_solver_t** out, const mde_edges_t* e, int64_t
 /* Replace the caller's part of a solver made by mde_solver_create_external and rebuild its step graphs (a callable
  * captured anew).  Blocking. */
 int mde_solver_set_external(mde_solver_t* s, const mde_external_t* ext, void* stream);
+
+/* Constraints whose projections the caller defines (pymde/constraints.py:7-91, any Constraint subclass), on the
+ * device solver (opts->constraint == MDE_CONSTRAINT_CUSTOM).  The caller's projections run on its own staging
+ * buffers, never in place on the solver's iterate X or gradient g:
+ *     retraction  [X -> u] -> caller: retract(u) in place -> [u -> X]      after the iterate moved
+ *     tangent     [X -> xt, g -> gt] -> caller: tangent(xt, gt), gt in place -> [gt -> g]   after every evaluation
+ * The bracketed copies are gated like the solver's own kernels (a step at the current iterate does not retract;
+ * the retraction of an accepted earlier trial does not evaluate); the caller's part is not gated, so in the steps
+ * after the device paused it runs again on stale staging buffers and nothing reads its result.  A projection that
+ * yields non-finite values ends, through the loss, in MDE_E_NAN.  The caller's part is given either as two CUDA graphs
+ * (kernel, memset and memcpy nodes only, else MDE_E_UNSUPPORTED; added as child nodes to every step), or as a hook
+ * fn(user, which, stream), which = 0 retraction / 1 tangent, that enqueues the same work on `stream` and returns 0
+ * (non-zero is returned by mde_solver_run).  Either both graphs or fn are set.  u, xt and gt each hold at least
+ * npad = ceil(n*m / 32) * 32 floats, 16-byte aligned, rows of m floats from the start; they must outlive the solver
+ * (or the next mde_solver_set_constraint_part). */
+typedef int (*mde_constraint_fn)(void* user, int which /* 0 retract, 1 tangent */, void* stream);
+typedef struct mde_constraint_part {
+  float* u;             /* retraction: iterate in, retracted iterate out */
+  float* xt;            /* tangent projection: the iterate */
+  float* gt;            /* tangent projection: gradient in, projected gradient out */
+  void* retract_graph;  /* cudaGraph_t, or NULL */
+  void* tangent_graph;  /* cudaGraph_t, or NULL */
+  mde_constraint_fn fn; /* or NULL */
+  void* user;
+} mde_constraint_part_t;
+/* One GPU only (opts->world_size == 1, else MDE_E_INVALID).  `ext` is a callable distortion function as for
+ * mde_solver_create_external, or NULL for the layout's table function.  When any caller's part is a hook, the steps are
+ * stream-launched, and the caller's parts given as graphs are launched inside them. */
+int mde_solver_create_custom(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m,
+                             const mde_solver_opts_t* opts, const mde_external_t* ext,
+                             const mde_constraint_part_t* part, void* stream);
+/* Replace the constraint part of a solver made by mde_solver_create_custom and rebuild its step graphs.  Blocking. */
+int mde_solver_set_constraint_part(mde_solver_t* s, const mde_constraint_part_t* part, void* stream);
 
 /* Multi-GPU hook (world_size > 1): after every distortion launch the solver calls
  * `fn(user, buf, count, stream)` which must sum the float32 buffer in place across ranks

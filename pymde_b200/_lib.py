@@ -13,7 +13,7 @@ LIB_PATH = os.path.join(_HERE, "libmde_b200.so")
 # error codes (include/mde_b200.h)
 MDE_E_INVALID, MDE_E_UNSUPPORTED, MDE_E_NAN, MDE_E_ALLOC, MDE_E_COMM = -1, -2, -3, -4, -5
 IPC_HANDLE_BYTES = 64
-CONSTRAINT_CENTERED, CONSTRAINT_STANDARDIZED, CONSTRAINT_ANCHORED = 0, 1, 2
+CONSTRAINT_CENTERED, CONSTRAINT_STANDARDIZED, CONSTRAINT_ANCHORED, CONSTRAINT_CUSTOM = 0, 1, 2, 3
 
 
 class MdeError(RuntimeError):
@@ -51,6 +51,15 @@ EXTERNAL_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_
 class mde_external_t(C.Structure):
     _fields_ = [("d", C.c_void_p), ("fpp", C.c_void_p), ("loss", C.c_void_p), ("graph", C.c_void_p),
                 ("fn", EXTERNAL_FN), ("user", C.c_void_p)]
+
+
+# (user, which: 0 retract / 1 tangent, stream) -> int: the caller's part of a user-defined constraint
+CONSTRAINT_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_void_p)
+
+
+class mde_constraint_part_t(C.Structure):
+    _fields_ = [("u", C.c_void_p), ("xt", C.c_void_p), ("gt", C.c_void_p), ("retract_graph", C.c_void_p),
+                ("tangent_graph", C.c_void_p), ("fn", CONSTRAINT_FN), ("user", C.c_void_p)]
 
 # name -> (restype, argtypes); every symbol include/mde_b200.h declares
 SIGNATURES = {
@@ -95,6 +104,10 @@ SIGNATURES = {
     "mde_solver_create_external": (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int,
                                              C.POINTER(mde_solver_opts_t), C.POINTER(mde_external_t), C.c_void_p]),
     "mde_solver_set_external": (C.c_int, [C.c_void_p, C.POINTER(mde_external_t), C.c_void_p]),
+    "mde_solver_create_custom": (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p, C.c_int64, C.c_int,
+                                           C.POINTER(mde_solver_opts_t), C.POINTER(mde_external_t),
+                                           C.POINTER(mde_constraint_part_t), C.c_void_p]),
+    "mde_solver_set_constraint_part": (C.c_int, [C.c_void_p, C.POINTER(mde_constraint_part_t), C.c_void_p]),
     "mde_knn_max_k": (C.c_int, []),
     "mde_knn_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,

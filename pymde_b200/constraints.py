@@ -12,7 +12,8 @@ from . import util
 
 class Constraint(abc.ABC):
     """A generic constraint.  Subclass and implement the four methods to create your own;
-    custom constraints run through the generic (torch-tensor) solver in pymde_b200.optim."""
+    custom constraints run through the generic (torch-tensor) solver in pymde_b200.optim, or, under
+    PYMDE_B200_CONSTRAINT=device, inside the device-resident solver's steps (pymde_b200/external.py)."""
 
     @abc.abstractmethod
     def name(self) -> str:
@@ -134,6 +135,11 @@ class _Standardized(Constraint):
 
 __Centered = _Centered()
 __Standardized = _Standardized()
+
+
+def is_builtin(constraint):
+    """Is `constraint` one the device solver projects with its own kernels (not a user-defined subclass)?"""
+    return type(constraint) in (_Centered, _Standardized, Anchored)
 
 
 def Centered():

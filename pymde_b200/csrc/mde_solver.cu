@@ -1223,6 +1223,10 @@ struct mde_solver {
   mde_external_t ext{};              // callable distortion function (ext.d != nullptr), see mde_solver_create_external
   float* gcoef = nullptr;            // (p,) caller-ordered coefficients of the scatter
   int64_t p = 0;
+  mde_constraint_part_t cpart{};     // MDE_CONSTRAINT_CUSTOM: the caller's projections, see mde_solver_create_custom
+  // stream-launched steps (a caller's part is a hook): the caller's parts that are graphs, instantiated
+  // (0 distortion function, 1 retraction, 2 tangent projection)
+  cudaGraphExec_t part_exec[3] = {nullptr, nullptr, nullptr};
   // flat step graphs (one step / steps_per_graph steps), no conditional nodes
   int steps_per_graph = 8;           // MDE_B200_STEPS (1..64)
   cudaGraph_t step_graph = nullptr, steps_graph = nullptr;
@@ -1245,20 +1249,34 @@ int read_status(mde_solver* s, cudaStream_t st) {
 // either a CUDA graph, added as a child node of the step graph being captured on `st` (it is not gated: in the surplus
 // steps after the device paused it recomputes fpp and loss from a stale d, and nothing reads them), or a host hook
 // that enqueues the torch ops on `st` (stream-launched steps).
+// the caller's graph inside a step: a child node of the step graph being captured on `st`, after everything captured
+// so far; in stream-launched steps (another caller's part is a hook) a launch of its instantiation `exec`
+int add_child_graph(cudaGraph_t child, cudaGraphExec_t exec, cudaStream_t st) {
+  size_t nodes = 0;
+  MDE_CUDA_TRY(cudaGraphGetNodes(child, nullptr, &nodes));
+  if (nodes == 0) return 0;  // nothing to do (a tangent projection that returns Z as it is)
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  cudaGraph_t g = nullptr;
+  const cudaGraphNode_t* deps = nullptr;
+  size_t nd = 0;
+  MDE_CUDA_TRY(cudaStreamGetCaptureInfo(st, &cs, nullptr, &g, &deps, &nd));
+  if (cs != cudaStreamCaptureStatusActive) {
+    if (!exec) return MDE_E_INVALID;
+    MDE_CUDA_TRY(cudaGraphLaunch(exec, st));
+    return 0;
+  }
+  cudaGraphNode_t node = nullptr;
+  MDE_CUDA_TRY(cudaGraphAddChildGraphNode(&node, g, deps, nd, child));
+  MDE_CUDA_TRY(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));
+  return 0;
+}
+
 int enqueue_external(mde_solver* s, const int* flag, cudaStream_t st) {
   const mde_external_t& x = s->ext;
   int rc = edge_distances_flag(s->edges, s->X, s->m, x.d, flag, st);
   if (rc) return rc;
   if (x.graph) {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    cudaGraph_t g = nullptr;
-    const cudaGraphNode_t* deps = nullptr;
-    size_t nd = 0;
-    MDE_CUDA_TRY(cudaStreamGetCaptureInfo(st, &cs, nullptr, &g, &deps, &nd));
-    if (cs != cudaStreamCaptureStatusActive) return MDE_E_INVALID;  // graph mode runs inside the step graphs only
-    cudaGraphNode_t node = nullptr;
-    MDE_CUDA_TRY(cudaGraphAddChildGraphNode(&node, g, deps, nd, (cudaGraph_t)x.graph));
-    MDE_CUDA_TRY(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));
+    if ((rc = add_child_graph((cudaGraph_t)x.graph, s->part_exec[0], st))) return rc;
   } else {
     if ((rc = x.fn(x.user, x.d, x.fpp, x.loss, (void*)st))) return rc;
   }
@@ -1267,6 +1285,30 @@ int enqueue_external(mde_solver* s, const int* flag, cudaStream_t st) {
   ext_coeff_kernel<<<nb, 256, 0, st>>>(flag, x.fpp, x.d, x.loss, s->gcoef, loss_partials_mut(s->edges), s->p);
   MDE_LAUNCH_CHECK();
   return scatter_external_flag(s->edges, s->X, s->m, s->gcoef, s->g, flag, st);
+}
+
+// caller-defined constraint: which = 0 retraction [X -> u] -> caller -> [u -> X], which = 1 tangent projection
+// [X -> xt, g -> gt] -> caller -> [gt -> g].  The copies are gated on `flag`, the caller's part is not: it only ever
+// works on its staging buffers, so in the surplus steps after the device paused it changes nothing the solver (or the
+// resumption of a paused solve) reads.
+int enqueue_constraint_part(mde_solver* s, int which, const int* flag, cudaStream_t st) {
+  const mde_constraint_part_t& c = s->cpart;
+  const int64_t n4 = s->npad >> 2;
+  const int nb = vec_blocks(n4);
+  float* out = which == 0 ? c.u : c.gt;
+  gated_copy_kernel<<<nb, kVecThreads, 0, st>>>(flag, s->X, which == 0 ? c.u : c.xt, n4);
+  MDE_LAUNCH_CHECK();
+  if (which == 1) {
+    gated_copy_kernel<<<nb, kVecThreads, 0, st>>>(flag, s->g, c.gt, n4);
+    MDE_LAUNCH_CHECK();
+  }
+  int rc = 0;
+  if (c.fn) rc = c.fn(c.user, which, (void*)st);
+  else rc = add_child_graph((cudaGraph_t)(which == 0 ? c.retract_graph : c.tangent_graph), s->part_exec[1 + which], st);
+  if (rc) return rc;
+  gated_copy_kernel<<<nb, kVecThreads, 0, st>>>(flag, out, which == 0 ? s->X : s->g, n4);
+  MDE_LAUNCH_CHECK();
+  return 0;
 }
 
 // closure: value_and_grad at s->X (optim.py:100-105) into the gradient buffer the vec kernel zeroed; `flag` gates
@@ -1322,6 +1364,8 @@ int enqueue_eval(mde_solver* s, const int* flag, cudaStream_t st) {
                                                                   s->opts.n_anchors, s->m);
       MDE_LAUNCH_CHECK();
     }
+  } else if (s->opts.constraint == MDE_CONSTRAINT_CUSTOM) {
+    return enqueue_constraint_part(s, 1, act, st);
   }
   return 0;
 }
@@ -1357,6 +1401,9 @@ int enqueue_step(mde_solver* s, cudaStream_t st) {
       }
       break;
     }
+    case MDE_CONSTRAINT_CUSTOM:
+      if ((rc = enqueue_constraint_part(s, 0, &S->g_proj, st))) return rc;
+      break;
     default: return MDE_E_INVALID;
   }
   return enqueue_eval(s, &S->g_eval, st);
@@ -1398,6 +1445,10 @@ void destroy_step_graphs(mde_solver* s) {
   if (s->steps_graph) cudaGraphDestroy(s->steps_graph);
   s->step_exec = s->steps_exec = nullptr;
   s->step_graph = s->steps_graph = nullptr;
+  for (cudaGraphExec_t& x : s->part_exec) {
+    if (x) cudaGraphExecDestroy(x);
+    x = nullptr;
+  }
 }
 
 // the one-step and the steps_per_graph-step graphs (one GPU, or several once connected)
@@ -1410,14 +1461,12 @@ int build_step_graphs(mde_solver* s) {
   return build_step_graph(s, s->steps_per_graph, &s->steps_graph, &s->steps_exec);
 }
 
-// a graph the solver can embed as a child node: kernel, memset and memcpy nodes only (no memory-allocation nodes)
-int check_external(const mde_external_t* x) {
-  if (!x->d || !x->fpp || !x->loss || (!x->graph) == (!x->fn)) return MDE_E_INVALID;
-  if (!x->graph) return 0;
-  cudaGraph_t g = (cudaGraph_t)x->graph;
+// a graph the solver can embed as a child node: kernel, memset and memcpy nodes only (no memory-allocation nodes);
+// an empty one only where `allow_empty`
+int check_graph(cudaGraph_t g, bool allow_empty) {
   size_t n = 0;
   MDE_CUDA_TRY(cudaGraphGetNodes(g, nullptr, &n));
-  if (n == 0) return MDE_E_INVALID;
+  if (n == 0) return allow_empty ? 0 : MDE_E_INVALID;
   cudaGraphNode_t* nodes = new (std::nothrow) cudaGraphNode_t[n];
   if (!nodes) return MDE_E_ALLOC;
   int rc = 0;
@@ -1432,21 +1481,50 @@ int check_external(const mde_external_t* x) {
   return e != cudaSuccess ? (int)e : rc;
 }
 
-// (re)build the step graphs around the external part x: graph mode captures them with x's graph inside, hook mode
-// runs stream-launched steps and has no step graphs
-int attach_external(mde_solver* s, const mde_external_t* x) {
+int check_external(const mde_external_t* x) {
+  if (!x->d || !x->fpp || !x->loss || (!x->graph) == (!x->fn)) return MDE_E_INVALID;
+  return x->graph ? check_graph((cudaGraph_t)x->graph, false) : 0;
+}
+
+int check_constraint_part(const mde_constraint_part_t* c) {
+  const auto misaligned = [](const float* p) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & 15u) != 0; };
+  if (misaligned(c->u) || misaligned(c->xt) || misaligned(c->gt)) return MDE_E_INVALID;
+  if ((!c->retract_graph) != (!c->tangent_graph)) return MDE_E_INVALID;  // both graphs, or none
+  if ((!c->retract_graph) == (!c->fn)) return MDE_E_INVALID;             // graphs or a hook
+  if (c->fn) return 0;
+  const int rc = check_graph((cudaGraph_t)c->retract_graph, true);
+  return rc ? rc : check_graph((cudaGraph_t)c->tangent_graph, true);
+}
+
+// (re)build the step graphs around the caller's parts: when every part is a graph the steps are captured with those
+// graphs inside; when any part is a hook the steps are stream-launched, there are no step graphs, and the parts that
+// are graphs are instantiated to be launched inside those steps
+int rebuild_step_graphs(mde_solver* s) {
   destroy_step_graphs(s);
+  const bool hook = (s->ext.d && !s->ext.graph) || s->cpart.fn;
+  if (!hook) return build_step_graphs(s);
+  const void* parts[3] = {s->ext.graph, s->cpart.retract_graph, s->cpart.tangent_graph};
+  for (int k = 0; k < 3; ++k) {
+    size_t nodes = 0;
+    if (parts[k]) MDE_CUDA_TRY(cudaGraphGetNodes((cudaGraph_t)parts[k], nullptr, &nodes));
+    if (nodes) MDE_CUDA_TRY(cudaGraphInstantiate(&s->part_exec[k], (cudaGraph_t)parts[k], 0));
+  }
+  return 0;
+}
+
+int attach_external(mde_solver* s, const mde_external_t* x) {
   s->ext = *x;
   s->nl = 1;  // the loss arrives as one partial (ext_coeff_kernel)
-  return x->graph ? build_step_graphs(s) : 0;
+  return rebuild_step_graphs(s);
 }
 
 int solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m, const mde_solver_opts_t* opts,
-                  const mde_external_t* ext, void* stream) {
+                  const mde_external_t* ext, const mde_constraint_part_t* cpart, void* stream) {
   if (!out || !e || !opts || n < 1 || m < 1) return MDE_E_INVALID;
   if (opts->memory_size < 1 || opts->memory_size > kMaxMemory) return MDE_E_UNSUPPORTED;
   if (opts->constraint == MDE_CONSTRAINT_STANDARDIZED && m > kWideMaxM) return MDE_E_UNSUPPORTED;
-  if (opts->constraint < 0 || opts->constraint > MDE_CONSTRAINT_ANCHORED) return MDE_E_INVALID;
+  if (opts->constraint < 0 || opts->constraint > MDE_CONSTRAINT_CUSTOM) return MDE_E_INVALID;
+  if ((opts->constraint == MDE_CONSTRAINT_CUSTOM) != (cpart != nullptr)) return MDE_E_INVALID;
   if (opts->max_iter < 1) return MDE_E_INVALID;
   if (opts->mode == 0 || opts->mode == 1) return MDE_E_UNSUPPORTED;  // retired drivers (host-stepped, conditional graph)
   if (opts->mode != 2) return MDE_E_INVALID;
@@ -1508,11 +1586,16 @@ int solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m, co
   }
   s->nvb = vec_blocks(s->npad >> 2);
   if (opts->constraint == MDE_CONSTRAINT_CENTERED && (m == 1 || m == 2 || m == 4)) s->center_m = m;
+  if (cpart) s->cpart = *cpart;  // (before the first capture, like the external descriptor)
   if (ext) {  // the descriptor is in place before the first capture
     s->p = edges_p(e);
     TRY(cudaMalloc(&s->gcoef, sizeof(float) * s->p));
     TRY(cudaStreamSynchronize(st));
     if ((rc = attach_external(s, ext))) goto fail;
+  } else if (cpart) {
+    s->nl = 0;
+    TRY(cudaStreamSynchronize(st));
+    if ((rc = rebuild_step_graphs(s))) goto fail;
   } else if (opts->world_size == 1) {  // several GPUs: graphs are built by mde_solver_comm_connect
     s->nl = 0;
     TRY(cudaStreamSynchronize(st));
@@ -1532,7 +1615,7 @@ extern "C" {
 
 int mde_solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m, const mde_solver_opts_t* opts,
                       void* stream) {
-  return solver_create(out, e, n, m, opts, nullptr, stream);
+  return solver_create(out, e, n, m, opts, nullptr, nullptr, stream);
 }
 
 int mde_solver_create_external(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m,
@@ -1540,7 +1623,27 @@ int mde_solver_create_external(mde_solver_t** out, const mde_edges_t* e, int64_t
   if (!ext || !opts || opts->world_size != 1) return MDE_E_INVALID;
   const int rc = check_external(ext);
   if (rc) return rc;
-  return solver_create(out, e, n, m, opts, ext, stream);
+  return solver_create(out, e, n, m, opts, ext, nullptr, stream);
+}
+
+int mde_solver_create_custom(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m,
+                             const mde_solver_opts_t* opts, const mde_external_t* ext,
+                             const mde_constraint_part_t* part, void* stream) {
+  if (!out || !e || !part || !opts || opts->world_size != 1 || opts->constraint != MDE_CONSTRAINT_CUSTOM)
+    return MDE_E_INVALID;
+  int rc = check_constraint_part(part);
+  if (rc) return rc;
+  if (ext && (rc = check_external(ext))) return rc;
+  return solver_create(out, e, n, m, opts, ext, part, stream);
+}
+
+int mde_solver_set_constraint_part(mde_solver_t* s, const mde_constraint_part_t* part, void* stream) {
+  if (!s || !part || s->opts.constraint != MDE_CONSTRAINT_CUSTOM) return MDE_E_INVALID;
+  int rc = check_constraint_part(part);
+  if (rc) return rc;
+  MDE_CUDA_TRY(cudaStreamSynchronize((cudaStream_t)stream));  // no step that embeds the old part is in flight
+  s->cpart = *part;
+  return rebuild_step_graphs(s);
 }
 
 int mde_solver_set_external(mde_solver_t* s, const mde_external_t* ext, void* stream) {

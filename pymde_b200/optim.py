@@ -13,6 +13,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from . import constraints
 from . import util
 
 
@@ -45,14 +46,14 @@ class DeviceSolver(object):
     """Owner of one `mde_solver_t`."""
 
     def __init__(self, layout, n, m, constraint, memory_size, max_iter, world_size=1, allreduce=None,
-                 exchange=None, rank=0, external=None):
+                 exchange=None, rank=0, external=None, constraint_part=None):
         lib = _lib.load()
         self.lib = lib
         self.layout = layout  # keep the edge layout alive
         self.device = layout.device
         self.n, self.m = int(n), int(m)
         opts = _lib.mde_solver_opts_t()
-        opts.constraint = int(constraint._solver_id)
+        opts.constraint = _lib.CONSTRAINT_CUSTOM if constraint_part is not None else int(constraint._solver_id)
         opts.memory_size = int(memory_size)
         opts.max_iter = max(int(max_iter), 1)
         opts.mode = 2  # the only driver: flat CUDA graphs of gated steps
@@ -67,13 +68,18 @@ class DeviceSolver(object):
             self._keep += [anchors, values]
         handle = C.c_void_p()
         self._ext = None  # pymde_b200.external.UserPart of a callable distortion function
+        self._part = None  # pymde_b200.external.ConstraintPart of a user-defined constraint
         with torch.cuda.device(self.device):
-            if external is None:
+            if constraint_part is not None:
+                self._attach(external, constraint_part, lambda x, c: lib.mde_solver_create_custom(
+                    C.byref(handle), layout.handle, self.n, self.m, C.byref(opts), x, C.byref(c),
+                    util.stream_ptr(self.device)))
+            elif external is None:
                 _lib.check(lib.mde_solver_create(C.byref(handle), layout.handle, self.n, self.m, C.byref(opts),
                                                  util.stream_ptr(self.device)))
             else:
-                self._attach(external, lambda x: lib.mde_solver_create_external(
-                    C.byref(handle), layout.handle, self.n, self.m, C.byref(opts), C.byref(x),
+                self._attach(external, None, lambda x, c: lib.mde_solver_create_external(
+                    C.byref(handle), layout.handle, self.n, self.m, C.byref(opts), x,
                     util.stream_ptr(self.device)))
         self.handle = handle
         self.max_iter = opts.max_iter
@@ -94,24 +100,45 @@ class DeviceSolver(object):
             self._cb = _lib.ALLREDUCE_FN(allreduce)
             _lib.check(lib.mde_solver_set_allreduce(self.handle, self._cb, None))
 
-    def _attach(self, ext, call):
-        rc = call(ext.descriptor())
-        if rc == _lib.MDE_E_UNSUPPORTED and ext.mode == "graph":  # node types the solver cannot embed
-            ext.use_hook()
-            rc = call(ext.descriptor())
+    def _attach(self, ext, part, call):
+        """call(descriptor of ext or None, descriptor of part or None) installs the caller's parts.  When the
+        library refuses a graph (node types it cannot embed), the parts fall back to hook mode one at a time, the
+        constraint's first, until it accepts them."""
+        def attempt():
+            return call(None if ext is None else C.byref(ext.descriptor()),
+                        None if part is None else part.descriptor())
+        rc = attempt()
+        for p in (part, ext):
+            if rc == _lib.MDE_E_UNSUPPORTED and p is not None and p.mode == "graph":
+                p.use_hook()
+                rc = attempt()
         _lib.check(rc)
-        self._ext = ext  # after the library let go of the previous part: its graph and buffers may be freed now
+        # after the library let go of the previous parts: their graphs and buffers may be freed now
+        self._ext = ext if ext is not None else self._ext
+        self._part = part if part is not None else self._part
 
     def set_external(self, ext):
         """Run the solves from now on with the callable's part `ext` (captured anew for every embed())."""
         with torch.cuda.device(self.device):
-            self._attach(ext, lambda x: self.lib.mde_solver_set_external(self.handle, C.byref(x),
-                                                                        util.stream_ptr(self.device)))
+            self._attach(ext, None, lambda x, c: self.lib.mde_solver_set_external(self.handle, x,
+                                                                                 util.stream_ptr(self.device)))
+
+    def set_constraint_part(self, part):
+        """Run the solves from now on with the user-defined constraint's part `part` (captured anew for every
+        embed())."""
+        with torch.cuda.device(self.device):
+            self._attach(None, part, lambda x, c: self.lib.mde_solver_set_constraint_part(
+                self.handle, C.byref(c), util.stream_ptr(self.device)))
 
     @property
     def external_mode(self):
         """"graph" or "hook" for a callable distortion function, None for a table function."""
         return None if self._ext is None else self._ext.mode
+
+    @property
+    def constraint_mode(self):
+        """"graph" or "hook" for a user-defined constraint, None for a built-in one."""
+        return None if self._part is None else self._part.mode
 
     def close(self):
         if getattr(self, "handle", None):
@@ -137,8 +164,9 @@ class DeviceSolver(object):
         with torch.cuda.device(self.device):
             rc = self.lib.mde_solver_run(self.handle, int(iters), C.byref(done), C.byref(conv),
                                          util.stream_ptr(self.device))
-        if self._ext is not None:
-            self._ext.raise_error()
+        for part in (self._ext, self._part):
+            if part is not None:
+                part.raise_error()
         if rc == _lib.MDE_E_NAN:
             raise util.SolverError("Function or gradient evaluation returned NaN/inf.")
         _lib.check(rc)
@@ -196,11 +224,14 @@ def lbfgs(X, objective_fn, constraint, eps, max_iter, memory_size, use_line_sear
     start_time = time.time()
     layout = mde._layout()
     n, m = X.shape
-    external = None
+    external = part = None
     if not mde._is_table_function():  # a callable: its torch part is captured again for every solve
         from .external import UserPart
         external = UserPart(mde.distortion_function, layout.p, layout.device)
-    solver = mde._solver(constraint, memory_size, max_iter, external)
+    if not constraints.is_builtin(constraint):  # a user-defined constraint: the same, for its two projections
+        from .external import ConstraintPart
+        part = ConstraintPart(constraint, X)
+    solver = mde._solver(constraint, memory_size, max_iter, external, part)
     solver.begin(X, eps, max_iter)
     snapshots, times = [], []
     digits = len(str(max_iter))

@@ -304,15 +304,17 @@ class MDE(torch.nn.Module):
 
     def _fused_ok(self, constraint, memory_size):
         """Can the device-resident solver take this problem?  Table functions and callables alike; callables of
-        edge-sharded problems, and callables under PYMDE_B200_EXTERNAL=generic, stay on the host-stepped solver."""
+        edge-sharded problems, and callables under PYMDE_B200_EXTERNAL=generic, stay on the host-stepped solver.
+        User-defined constraints run on it only under PYMDE_B200_CONSTRAINT=device|graph|hook, on one GPU."""
+        from . import external
         if not self._is_table_function():
-            from . import external
             if not callable(self.distortion_function) or self.__dict__["_dist"] is not None:
                 return False
             if external.forced_mode() == "generic":
                 return False
-        if type(constraint) not in (constraints._Centered, constraints._Standardized, constraints.Anchored):
-            return False
+        if not constraints.is_builtin(constraint):
+            if external.constraint_mode() is None or self.__dict__["_dist"] is not None:
+                return False
         if isinstance(constraint, constraints._Standardized) and int(self.embedding_dim) > 256:
             return False
         m = int(self.embedding_dim)
@@ -320,10 +322,11 @@ class MDE(torch.nn.Module):
             return False
         return 1 <= int(memory_size) <= 32
 
-    def _solver(self, constraint, memory_size, max_iter, external=None):
+    def _solver(self, constraint, memory_size, max_iter, external=None, constraint_part=None):
         """Device solver for this problem, cached across embed() calls.  `max_iter` only sizes the statistics
         buffers, so a cached solver with enough capacity is reused (its CUDA graphs are built once, except for a
-        callable distortion function: `external`, its newly captured part, is installed and the graphs rebuilt)."""
+        callable distortion function or a user-defined constraint: `external` and `constraint_part`, their newly
+        captured parts, are installed and the graphs rebuilt)."""
         layout = self._layout()  # (re)built first: a rebuilt layout invalidates the solver that referenced the old one
         stamp = ()
         if isinstance(constraint, constraints.Anchored):  # anchor indices / values are copied at solver creation
@@ -340,11 +343,15 @@ class MDE(torch.nn.Module):
                                         world_size=1 if dist is None else dist["world_size"],
                                         allreduce=None if dist is None else dist.get("allreduce"),
                                         exchange=None if dist is None else dist.get("exchange"),
-                                        rank=0 if dist is None else dist["rank"], external=external)
+                                        rank=0 if dist is None else dist["rank"], external=external,
+                                        constraint_part=constraint_part)
             cur = (key, solver, constraint)  # holds the constraint: a recycled id() can never alias it
             self.__dict__["_device_solver"] = cur
-        elif external is not None:
-            cur[1].set_external(external)
+        else:
+            if external is not None:
+                cur[1].set_external(external)
+            if constraint_part is not None:
+                cur[1].set_constraint_part(constraint_part)
         return cur[1]
 
     def _check_X(self, X):
