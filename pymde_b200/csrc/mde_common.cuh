@@ -207,6 +207,8 @@ __device__ __forceinline__ void edge_value(const FnDev& fn, float d, float a, fl
 // sequences.  The kernel is instruction-issue bound, and only the
 // SUM of the per-edge losses has to agree with the reference to 1e-5: a 1e-7 absolute error per edge
 // is far inside that.  Inputs: squared distance d2.  Outputs: f_k and g_k = f'_k / (p d).
+// CLS 2 picks the attractive or repulsive form by the sign of w; the tile kernels pass CLS 0 (attractive) or 1
+// (repulsive) when the class of a whole warp's edges is known, and only that side is compiled.
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float fast_rsqrt(float x) { float y; asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float fast_sqrt(float x) { float y; asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
@@ -214,11 +216,12 @@ __device__ __forceinline__ float fast_rcp(float x) { float y; asm("rcp.approx.ft
 __device__ __forceinline__ float fast_lg2(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float fast_ex2(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
+template <int CLS>
 __device__ __forceinline__ void edge_coeff_fast_log1p_log(float d2, float w, float inv_p, float& f, float& g) {
   const float kLn2 = 0.69314718056f, kLog2e = 1.44269504089f;
   const float rs = fast_rsqrt(d2);          // 1/d  (inf at d2 = 0; masked by the caller)
   const float d = (d2 > 0.0f) ? d2 * rs : 0.0f;  // 0 * inf would be NaN
-  if (w >= 0.0f) {                          // attractive: w log1p(d^1.5)
+  if (CLS == 0 || (CLS == 2 && w >= 0.0f)) {  // attractive: w log1p(d^1.5)
     const float sd = fast_sqrt(d);
     const float de = d * sd;
     const float one_p = 1.0f + de;

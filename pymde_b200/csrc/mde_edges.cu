@@ -1,4 +1,5 @@
-// mde_edges.cu -- edge layout + the fused average-distortion kernel (forward + backward).
+// mde_edges.cu -- edge layout + the fused average-distortion kernel (forward + backward), the evaluation entries that
+// pick the kernels of every layout kind, and the launch helpers the tile, pull and ELL layouts share (mde_edges.cuh).
 //
 // Replaces pymde/average_distortion.py:36-80 (gather X[lhs], X[rhs]; row norms; per-edge
 // penalty; mean; scatter-add of +-g*diff) and pymde/problem.py:246-307 (per-edge outputs).
@@ -21,6 +22,7 @@
 //   m >= 5 : a group of G lanes (8/16/32) walks a contiguous slice of edges; the lhs row and
 //            its gradient accumulator stay in registers across a run.
 #include <cub/cub.cuh>
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
 #include <new>
@@ -72,21 +74,6 @@ __global__ void unpack_kernel(const uint64_t* __restrict__ keys, const int32_t* 
 // ------------------------------------------------------------------------------------------
 // m <= 4: thread-per-edge kernel
 // ------------------------------------------------------------------------------------------
-template <int M> struct Row { float v[M]; };
-
-template <int M>
-__device__ __forceinline__ Row<M> load_row(const float* __restrict__ X, int r) {
-  Row<M> o;
-  if constexpr (M == 1) { o.v[0] = __ldg(X + r); }
-  else if constexpr (M == 2) { float2 t = __ldg(reinterpret_cast<const float2*>(X) + r); o.v[0] = t.x; o.v[1] = t.y; }
-  else if constexpr (M == 4) { float4 t = __ldg(reinterpret_cast<const float4*>(X) + r); o.v[0] = t.x; o.v[1] = t.y; o.v[2] = t.z; o.v[3] = t.w; }
-  else {
-#pragma unroll
-    for (int c = 0; c < M; ++c) o.v[c] = __ldg(X + (int64_t)r * M + c);
-  }
-  return o;
-}
-
 // Deterministic mode: contributions are accumulated as 64-bit fixed point (scale 2^40, resolution 9e-13, range
 // +-8.4e6 -- the entries are f'/p-sized).  Integer addition is associative, so the sums do not depend on the order in
 // which the reds land (the float reds of the default mode, like the reference's scatter_add_, do:
@@ -136,17 +123,6 @@ __global__ void fx_apply_kernel(const int* __restrict__ flag, const long long* _
     grad[i] += (float)((double)F[i] * (1.0 / 1099511627776.0));
 }
 
-template <int M>
-__device__ __forceinline__ void red_row(float* __restrict__ G, int r, const float (&v)[M], float sgn) {
-  if constexpr (M == 1) red_add(G + r, sgn * v[0]);
-  else if constexpr (M == 2) red_add_v2(G + 2 * (int64_t)r, sgn * v[0], sgn * v[1]);
-  else if constexpr (M == 4) red_add_v4(G + 4 * (int64_t)r, sgn * v[0], sgn * v[1], sgn * v[2], sgn * v[3]);
-  else {
-#pragma unroll
-    for (int c = 0; c < M; ++c) red_add(G + (int64_t)r * M + c, sgn * v[c]);
-  }
-}
-
 // MODE 0: fused value + gradient; 1: value only; 2: external per-edge g (gradient only)
 template <int M, int MODE, int FA, int FR>
 __global__ void __launch_bounds__(kSmallThreads)
@@ -183,8 +159,8 @@ distortion_small_kernel(const int32_t* __restrict__ src, const int32_t* __restri
     Row<M> xi[kRounds], xj[kRounds];
 #pragma unroll
     for (int r = 0; r < kRounds; ++r) {
-      xi[r] = load_row<M>(X, s[r]);
-      xj[r] = load_row<M>(X, t[r]);
+      xi[r] = ldg_row<M>(X, s[r]);
+      xj[r] = ldg_row<M>(X, t[r]);
     }
 #pragma unroll
     for (int r = 0; r < kRounds; ++r) {
@@ -256,7 +232,7 @@ __device__ __forceinline__ bool edge_contribution(const Row<M>& xs, const Row<M>
   if (MODE == 2) {
     g = a;
   } else if (FAST) {
-    edge_coeff_fast_log1p_log(d2, a, inv_p, f, g);
+    edge_coeff_fast_log1p_log<2>(d2, a, inv_p, f, g);
   } else {
     const float d = sqrtf(d2);
     if (MODE == 0) edge_coeff<FA, FR>(fn, d, a, b, inv_p, f, g);
@@ -341,7 +317,7 @@ distortion_quad_kernel(const int32_t* __restrict__ src, const int32_t* __restric
     }
     Row<M> xi[E], xj[E];
 #pragma unroll
-    for (int e = 0; e < E; ++e) { xi[e] = load_row<M>(X, s[e]); xj[e] = load_row<M>(X, t[e]); }
+    for (int e = 0; e < E; ++e) { xi[e] = ldg_row<M>(X, s[e]); xj[e] = ldg_row<M>(X, t[e]); }
     float acc[M];
 #pragma unroll
     for (int c = 0; c < M; ++c) acc[c] = 0.0f;
@@ -438,7 +414,7 @@ distortion_owner_kernel(const uint2* __restrict__ ent, const uint32_t* __restric
     const int j0 = node ? (int)__ldg(off + i) : 0, j1 = node ? (int)__ldg(off + i + 1) : 0;
     const bool hub = j1 - j0 > kOwnerHub;
     if (node && !hub) {
-      const Row<M> xo = load_row<M>(X, i);
+      const Row<M> xo = ldg_row<M>(X, i);
       for (int j = j0 + l; j < j1; j += kOwnerLanes * kOwnerBatch) {
         // the loads of kOwnerBatch entries go out before the first add; the adds keep the list order
         uint2 w[kOwnerBatch];
@@ -447,7 +423,7 @@ distortion_owner_kernel(const uint2* __restrict__ ent, const uint32_t* __restric
         for (int u = 0; u < kOwnerBatch; ++u) fetch(j + u * kOwnerLanes, j + u * kOwnerLanes < j1, i, w[u], a[u], b[u]);
         Row<M> xn[kOwnerBatch];
 #pragma unroll
-        for (int u = 0; u < kOwnerBatch; ++u) xn[u] = load_row<M>(X, (int)(w[u].x & 0x7fffffffu));
+        for (int u = 0; u < kOwnerBatch; ++u) xn[u] = ldg_row<M>(X, (int)(w[u].x & 0x7fffffffu));
 #pragma unroll
         for (int u = 0; u < kOwnerBatch; ++u) {
           if (j + u * kOwnerLanes < j1) {
@@ -470,14 +446,14 @@ distortion_owner_kernel(const uint2* __restrict__ ent, const uint32_t* __restric
       const int ih = __shfl_sync(kFull, i, g0);
       const int h0 = __shfl_sync(kFull, j0, g0), h1 = __shfl_sync(kFull, j1, g0);
       const bool mine = (lane & ~(kOwnerLanes - 1)) == g0;
-      const Row<M> xo = load_row<M>(X, ih);
+      const Row<M> xo = ldg_row<M>(X, ih);
       uint2 w0, w1;
       float a0, b0, a1, b1;
       fetch(h0 + lane, h0 + lane < h1, ih, w0, a0, b0);
       fetch(h0 + 32 + lane, h0 + 32 + lane < h1, ih, w1, a1, b1);
-      Row<M> x0 = load_row<M>(X, (int)(w0.x & 0x7fffffffu));
+      Row<M> x0 = ldg_row<M>(X, (int)(w0.x & 0x7fffffffu));
       for (int hb = h0; hb < h1; hb += 32) {
-        const Row<M> x1 = load_row<M>(X, (int)(w1.x & 0x7fffffffu));
+        const Row<M> x1 = ldg_row<M>(X, (int)(w1.x & 0x7fffffffu));
         uint2 w2;
         float a2, b2;
         fetch(hb + 64 + lane, hb + 64 + lane < h1, ih, w2, a2, b2);
@@ -713,8 +689,7 @@ static void read_kernel_switches(mde_edges* e) {
   if (ev && !strcmp(ev, "precise")) e->kvar = 2;
   ev = getenv("MDE_B200_NQ");
   e->nq = (ev && ev[0] == '2') ? 2 : 1;
-  ev = getenv("MDE_B200_QUAD_BPS");
-  int v = ev ? atoi(ev) : 4;
+  int v = env_int("MDE_B200_QUAD_BPS", 4);
   if (v < 1) v = 1;
   if (v > 16) v = 16;
   e->qbps = v;
@@ -745,165 +720,200 @@ int loss_blocks_wide(int64_t p, int G) {
   return (int)nb;
 }
 
+// compile-time function pairs of the quad / owner kernels and of the strided kernel (fused mode, m = 2 / 3)
+using QuadPairs = FnList<Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>, Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOGRATIO>, Fn1<MDE_FN_P_QUADRATIC>,
+                         Fn1<MDE_FN_L_ABSOLUTE>, Fn1<MDE_FN_L_QUADRATIC>, Fn1<MDE_FN_L_WEIGHTED_QUADRATIC>,
+                         Fn1<MDE_FN_L_HUBER>>;
+using StridedPairs = FnList<Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>, Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOGRATIO>,
+                            Fn1<MDE_FN_P_QUADRATIC>, Fn1<MDE_FN_P_LOG1P>, Fn1<MDE_FN_L_ABSOLUTE>, Fn1<MDE_FN_L_QUADRATIC>,
+                            Fn1<MDE_FN_L_WEIGHTED_QUADRATIC>, Fn1<MDE_FN_L_HUBER>>;
+
+// one evaluation on the sorted-SoA layout; the launch helpers return the grid size (= loss partials)
+struct SoaLaunch {
+  const mde_edges* e;
+  const float* X;
+  int m;
+  float* grad;
+  const float* gext;
+  const int* flag;
+  cudaStream_t st;
+  float inv_p;
+  long long* fx;  // deterministic mode: the fixed-point accumulator
+  bool owner;     // the owner kernel runs in place of the quad kernel
+  const float* par1() const { return e->has_par1 ? e->par1 : nullptr; }
+};
+
+template <int M, int MODE, int FA, int FR, bool FAST>
+int launch_owner(const SoaLaunch& l) {
+  const mde_edges* e = l.e;
+  const int nb = loss_blocks_owner(e->n);
+  distortion_owner_kernel<M, MODE, FA, FR, FAST><<<nb, kOwnerThreads, 0, l.st>>>(
+      e->ent, e->inc, e->inc_off, l.par1(), e->perm, l.gext, e->n, l.X, l.grad, e->loss_partials, e->fn, l.inv_p, l.flag);
+  return nb;
+}
+
+template <int M, int MODE, int FA, int FR, bool FAST>
+int launch_quad(const SoaLaunch& l) {
+  if constexpr (MODE != 1) {
+    if (l.owner) return launch_owner<M, MODE, FA, FR, FAST>(l);
+  }
+  const mde_edges* e = l.e;
+  const int nq = (FAST && e->nq == 2) ? 2 : 1;
+  const int nb = loss_blocks_quad(e->p, nq, e->qbps);
+  auto k = nq == 2 ? &distortion_quad_kernel<M, MODE, FA, FR, FAST, 2> : &distortion_quad_kernel<M, MODE, FA, FR, FAST, 1>;
+  k<<<nb, kQuadThreads, 0, l.st>>>(e->src, e->dst, e->par0, l.par1(), e->perm, l.gext, e->p, l.X, l.grad,
+                                   e->loss_partials, e->fn, l.inv_p, l.flag, l.fx);
+  return nb;
+}
+
+template <int M, int MODE, int FA, int FR>
+int launch_strided(const SoaLaunch& l) {
+  const mde_edges* e = l.e;
+  const int nb = loss_blocks_small(e->p);
+  distortion_small_kernel<M, MODE, FA, FR><<<nb, kSmallThreads, 0, l.st>>>(
+      e->src, e->dst, e->par0, l.par1(), e->perm, l.gext, e->p, l.X, l.grad, e->loss_partials, e->fn, l.inv_p, l.flag);
+  return nb;
+}
+
+template <int M, int MODE>
+int launch_small(const SoaLaunch& l) {
+  const FnDev& fn = l.e->fn;
+  if (l.e->kvar == 1) {
+    return select_fn<M, MODE>(fn, false, StridedPairs{},
+                              [&](auto f) { using F = decltype(f); return launch_strided<M, MODE, F::FA, F::FR>(l); });
+  }
+  if constexpr (MODE == 0 && (M == 1 || M == 4)) {
+    // m = 1, 4: the owner kernel evaluates every edge twice, so the recipe default PushAndPull(Log1p, Log) gets
+    // compile-time ids there (IEEE math, as the run-time table) instead of two out-of-line calls
+    if (l.owner && Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>::matches(fn))
+      return launch_owner<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOG, false>(l);
+  }
+  return select_fn<M, MODE>(fn, fast_log1p_log(fn, l.e->kvar == 2), QuadPairs{}, [&](auto f) {
+    using F = decltype(f);
+    return launch_quad<M, MODE, F::FA, F::FR, F::FAST>(l);
+  });
+}
+
+template <int G, int CPL, int VW, int MODE>
+int launch_wide(const SoaLaunch& l) {
+  const mde_edges* e = l.e;
+  const int nb = loss_blocks_wide(e->p, G);
+  distortion_wide_kernel<G, CPL, VW, MODE><<<nb, kWideThreads, 0, l.st>>>(
+      e->src, e->dst, e->par0, l.par1(), e->perm, l.gext, e->p, l.m, l.X, l.grad, e->loss_partials, e->fn, l.inv_p,
+      l.flag);
+  return nb;
+}
+
 template <int MODE>
 int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, const float* gext,
                       int* nblocks_out, const int* flag, cudaStream_t st) {
-  const float inv_p = 1.0f / (float)e->p_total;
-  const int64_t p = e->p;
-  int nb;
+  SoaLaunch l{e, X, m, grad, gext, flag, st, 1.0f / (float)e->p_total, nullptr, false};
   // deterministic mode (m <= 4, sorted-SoA layout): zero the fixed-point buffer, accumulate into it, add it to grad
-  long long* fxp = nullptr;
   if (e->det && MODE != 1 && m <= 4 && m <= e->m_hint && e->kvar != 1) {
-    fxp = e->fx;
+    l.fx = e->fx;
     const int64_t cnt = e->n * m;
     int zb = (int)((cnt + 255) / 256); if (zb > kNumSMs * 8) zb = kNumSMs * 8;
-    fx_zero_kernel<<<zb, 256, 0, st>>>(flag, fxp, cnt);
+    fx_zero_kernel<<<zb, 256, 0, st>>>(flag, l.fx, cnt);
     ++g_launch_count;
   }
   // default on the sorted-SoA layout: the owner kernel over the directed entries, in place of the quad kernel
-  const bool owner = !fxp && e->ent && MODE != 1 && m == e->m_hint && e->kvar != 1;
-#define SMALLK(MM, FA, FR)                                                                            \
-  distortion_small_kernel<MM, MODE, FA, FR><<<nb, kSmallThreads, 0, st>>>(                            \
-      e->src, e->dst, e->par0, e->has_par1 ? e->par1 : nullptr, e->perm, gext, p, X, grad,           \
-      e->loss_partials, e->fn, inv_p, flag)
-  // hot function combinations get compile-time ids (fused mode, m = 2 / 3); the rest use the table
-#define QUADK_(MM, FA, FR, FAST, NQV)                                                                 \
-  distortion_quad_kernel<MM, MODE, FA, FR, FAST, NQV><<<nb, kQuadThreads, 0, st>>>(                   \
-      e->src, e->dst, e->par0, e->has_par1 ? e->par1 : nullptr, e->perm, gext, p, X, grad,           \
-      e->loss_partials, e->fn, inv_p, flag, fxp)
-#define OWNERK(MM, FA, FR, FAST)                                                                      \
-  if constexpr (MODE != 1) {                                                                         \
-    nb = loss_blocks_owner(e->n);                                                                    \
-    distortion_owner_kernel<MM, MODE, FA, FR, FAST><<<nb, kOwnerThreads, 0, st>>>(                    \
-        e->ent, e->inc, e->inc_off, e->has_par1 ? e->par1 : nullptr, e->perm, gext, e->n, X, grad,   \
-        e->loss_partials, e->fn, inv_p, flag);                                                       \
-  }
-#define QUADK(MM, FA, FR, FAST)                                                                       \
-  if (owner) { OWNERK(MM, FA, FR, FAST) }                                                             \
-  else if (FAST && e->nq == 2) { nb = loss_blocks_quad(p, 2, e->qbps); QUADK_(MM, FA, FR, FAST, 2); }  \
-  else { nb = loss_blocks_quad(p, 1, e->qbps); QUADK_(MM, FA, FR, FAST, 1); }
-#define SMALL(MM)                                                                                     \
-  if (e->kvar != 1) {                                                                                 \
-    nb = loss_blocks_quad(p, 1, e->qbps);                                                             \
-    const int fa = e->fn.fn_att, fr = e->fn.fn_rep, pp = e->fn.push_pull;                             \
-    const bool hot = pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG && e->fn.a0 == 1.5f &&          \
-                     e->fn.r0 == 1.0f && e->kvar == 0;                                                \
-    if constexpr (MODE == 0 && (MM == 2 || MM == 3)) {                                                \
-      if (hot) { QUADK(MM, MDE_FN_P_LOG1P, MDE_FN_P_LOG, true); }                                     \
-      else if (pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG) { QUADK(MM, MDE_FN_P_LOG1P, MDE_FN_P_LOG, false); } \
-      else if (pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOGRATIO) { QUADK(MM, MDE_FN_P_LOG1P, MDE_FN_P_LOGRATIO, false); } \
-      else if (!pp && fa == MDE_FN_P_QUADRATIC) { QUADK(MM, MDE_FN_P_QUADRATIC, MDE_FN_P_QUADRATIC, false); }     \
-      else if (!pp && fa == MDE_FN_L_ABSOLUTE) { QUADK(MM, MDE_FN_L_ABSOLUTE, MDE_FN_L_ABSOLUTE, false); }        \
-      else if (!pp && fa == MDE_FN_L_QUADRATIC) { QUADK(MM, MDE_FN_L_QUADRATIC, MDE_FN_L_QUADRATIC, false); }     \
-      else if (!pp && fa == MDE_FN_L_WEIGHTED_QUADRATIC) { QUADK(MM, MDE_FN_L_WEIGHTED_QUADRATIC, MDE_FN_L_WEIGHTED_QUADRATIC, false); } \
-      else if (!pp && fa == MDE_FN_L_HUBER) { QUADK(MM, MDE_FN_L_HUBER, MDE_FN_L_HUBER, false); }                 \
-      else { QUADK(MM, -1, -1, false); }                                                              \
-    } else if constexpr (MODE == 0) {                                                                 \
-      /* m = 1, 4: the owner kernel evaluates every edge twice, so the recipe default PushAndPull(Log1p, Log) \
-         gets compile-time ids there (IEEE math, as the run-time table) instead of two out-of-line calls */ \
-      if (owner && pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG) { OWNERK(MM, MDE_FN_P_LOG1P, MDE_FN_P_LOG, false) } \
-      else { QUADK(MM, -1, -1, false); }                                                              \
-    } else { QUADK(MM, -1, -1, false); }                                                              \
-  } else {                                                                                            \
-    SMALL_STRIDED(MM);                                                                                \
-  }
-#define SMALL_STRIDED(MM)                                                                             \
-  nb = loss_blocks_small(p);                                                                          \
-  if constexpr (MODE == 0 && (MM == 2 || MM == 3)) {                                                  \
-    const int fa = e->fn.fn_att, fr = e->fn.fn_rep, pp = e->fn.push_pull;                             \
-    if (pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG) { SMALLK(MM, MDE_FN_P_LOG1P, MDE_FN_P_LOG); }            \
-    else if (pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOGRATIO) { SMALLK(MM, MDE_FN_P_LOG1P, MDE_FN_P_LOGRATIO); } \
-    else if (!pp && fa == MDE_FN_P_QUADRATIC) { SMALLK(MM, MDE_FN_P_QUADRATIC, MDE_FN_P_QUADRATIC); }             \
-    else if (!pp && fa == MDE_FN_P_LOG1P) { SMALLK(MM, MDE_FN_P_LOG1P, MDE_FN_P_LOG1P); }                         \
-    else if (!pp && fa == MDE_FN_L_ABSOLUTE) { SMALLK(MM, MDE_FN_L_ABSOLUTE, MDE_FN_L_ABSOLUTE); }                \
-    else if (!pp && fa == MDE_FN_L_QUADRATIC) { SMALLK(MM, MDE_FN_L_QUADRATIC, MDE_FN_L_QUADRATIC); }             \
-    else if (!pp && fa == MDE_FN_L_WEIGHTED_QUADRATIC) { SMALLK(MM, MDE_FN_L_WEIGHTED_QUADRATIC, MDE_FN_L_WEIGHTED_QUADRATIC); } \
-    else if (!pp && fa == MDE_FN_L_HUBER) { SMALLK(MM, MDE_FN_L_HUBER, MDE_FN_L_HUBER); }                         \
-    else { SMALLK(MM, -1, -1); }                                                                      \
-  } else { SMALLK(MM, -1, -1); }
-#define WIDE(GG, CC, VV)                                                                              \
-  nb = loss_blocks_wide(p, GG);                                                                       \
-  distortion_wide_kernel<GG, CC, VV, MODE><<<nb, kWideThreads, 0, st>>>(                              \
-      e->src, e->dst, e->par0, e->has_par1 ? e->par1 : nullptr, e->perm, gext, p, m, X, grad,        \
-      e->loss_partials, e->fn, inv_p, flag)
-  if (m == 1) { SMALL(1); }
-  else if (m == 2) { SMALL(2); }
-  else if (m == 3) { SMALL(3); }
-  else if (m == 4) { SMALL(4); }
+  l.owner = !l.fx && e->ent && MODE != 1 && m == e->m_hint && e->kvar != 1;
+  int nb;
+  if (m == 1) nb = launch_small<1, MODE>(l);
+  else if (m == 2) nb = launch_small<2, MODE>(l);
+  else if (m == 3) nb = launch_small<3, MODE>(l);
+  else if (m == 4) nb = launch_small<4, MODE>(l);
   else if (m % 4 == 0) {
-    int mv = m / 4;
-    if (mv <= 8) { WIDE(8, 1, 4); }
-    else if (mv <= 16) { WIDE(16, 1, 4); }
-    else if (mv <= 32) { WIDE(32, 1, 4); }
-    else if (mv <= 64) { WIDE(32, 2, 4); }
-    else if (mv <= 128) { WIDE(32, 4, 4); }
-    else if (mv <= 256) { WIDE(32, 8, 4); }
+    const int mv = m / 4;
+    if (mv <= 8) nb = launch_wide<8, 1, 4, MODE>(l);
+    else if (mv <= 16) nb = launch_wide<16, 1, 4, MODE>(l);
+    else if (mv <= 32) nb = launch_wide<32, 1, 4, MODE>(l);
+    else if (mv <= 64) nb = launch_wide<32, 2, 4, MODE>(l);
+    else if (mv <= 128) nb = launch_wide<32, 4, 4, MODE>(l);
+    else if (mv <= 256) nb = launch_wide<32, 8, 4, MODE>(l);
     else return MDE_E_UNSUPPORTED;
   } else {
-    if (m <= 8) { WIDE(8, 1, 1); }
-    else if (m <= 16) { WIDE(16, 1, 1); }
-    else if (m <= 32) { WIDE(32, 1, 1); }
-    else if (m <= 64) { WIDE(32, 2, 1); }
-    else if (m <= 128) { WIDE(32, 4, 1); }
-    else if (m <= 256) { WIDE(32, 8, 1); }
-    else if (m <= 512) { WIDE(32, 16, 1); }
+    if (m <= 8) nb = launch_wide<8, 1, 1, MODE>(l);
+    else if (m <= 16) nb = launch_wide<16, 1, 1, MODE>(l);
+    else if (m <= 32) nb = launch_wide<32, 1, 1, MODE>(l);
+    else if (m <= 64) nb = launch_wide<32, 2, 1, MODE>(l);
+    else if (m <= 128) nb = launch_wide<32, 4, 1, MODE>(l);
+    else if (m <= 256) nb = launch_wide<32, 8, 1, MODE>(l);
+    else if (m <= 512) nb = launch_wide<32, 16, 1, MODE>(l);
     else return MDE_E_UNSUPPORTED;
   }
-#undef SMALL
-#undef SMALL_STRIDED
-#undef QUADK
-#undef QUADK_
-#undef OWNERK
-#undef SMALLK
-#undef WIDE
   MDE_LAUNCH_CHECK();
-  if (fxp) {
+  if (l.fx) {
     const int64_t cnt = e->n * m;
     int zb = (int)((cnt + 255) / 256); if (zb > kNumSMs * 8) zb = kNumSMs * 8;
-    fx_apply_kernel<<<zb, 256, 0, st>>>(flag, fxp, grad, cnt);
+    fx_apply_kernel<<<zb, 256, 0, st>>>(flag, l.fx, grad, cnt);
     MDE_LAUNCH_CHECK();
   }
   if (nblocks_out) *nblocks_out = nb;
   return 0;
 }
 
-// used by the solver: fused launch leaving per-block loss partials in e->loss_partials
-int distortion_fused(const mde_edges* e, const float* X, int m, float* grad, int* nblocks, cudaStream_t st) {
-  if (e->kind == 3 && m == e->m_hint) return ell_launch(e, X, m, grad, nblocks, nullptr, st);
-  if (e->kind == 2) return pull_launch(0, e, X, m, grad, nullptr, nblocks, nullptr, st);
-  if (e->kind == 1) return tiled_launch(0, e, X, m, grad, nullptr, nblocks, nullptr, st);
-  return launch_distortion<0>(e, X, m, grad, nullptr, nblocks, nullptr, st);
+int evaluate(int mode, const mde_edges* e, const float* X, int m, float* grad, const float* gext, int* nblocks_out,
+             const int* flag, cudaStream_t st) {
+  switch (e->kind) {
+    case kSoaEll:  // the fused evaluation at the layout's m; everything else on the sorted-SoA arrays
+      if (mode == 0 && m == e->m_hint) return ell_launch(e, X, m, grad, nblocks_out, flag, st);
+      break;
+    case kPull: return pull_launch(mode, e, X, m, grad, gext, nblocks_out, flag, st);
+    case kTiles: return tiled_launch(mode, e, X, m, grad, gext, nblocks_out, flag, st);
+    case kSoa: break;
+  }
+  if (mode == 0) return launch_distortion<0>(e, X, m, grad, gext, nblocks_out, flag, st);
+  if (mode == 1) return launch_distortion<1>(e, X, m, grad, gext, nblocks_out, flag, st);
+  return launch_distortion<2>(e, X, m, grad, gext, nblocks_out, flag, st);
 }
-int distortion_fused_flag(const mde_edges* e, const float* X, int m, float* grad, int* nblocks,
-                          const int* flag, cudaStream_t st) {
-  if (e->kind == 3 && m == e->m_hint) return ell_launch(e, X, m, grad, nblocks, flag, st);
-  if (e->kind == 2) return pull_launch(0, e, X, m, grad, nullptr, nblocks, flag, st);
-  if (e->kind == 1) return tiled_launch(0, e, X, m, grad, nullptr, nblocks, flag, st);
-  return launch_distortion<0>(e, X, m, grad, nullptr, nblocks, flag, st);
-}
-// the device solver's evaluation of a callable distortion function (mde_solver.cu): distances in the caller's edge
-// order, then the gradient scatter of the caller-ordered coefficients g; both gated by `flag`
-int edge_distances_flag(const mde_edges* e, const float* X, int m, float* distances, const int* flag,
-                        cudaStream_t st) {
-  if (e->kind == 2) return pull_edge_outputs(e, X, m, distances, nullptr, st, flag);
-  if (e->kind == 1) return tiled_edge_outputs(e, X, m, distances, nullptr, st, flag);
-  int tb = 256, nb = ceil_div_i64(e->p, tb);
-  edge_outputs_kernel<0><<<nb, tb, 0, st>>>(e->src, e->dst, e->par0, nullptr, e->perm, e->p, m, X, distances, nullptr,
-                                            e->fn, flag);
+
+int edge_outputs(const mde_edges* e, const float* X, int m, float* distances, float* distortions, const int* flag,
+                 cudaStream_t st) {
+  switch (e->kind) {
+    case kPull: return pull_edge_outputs(e, X, m, distances, distortions, flag, st);
+    case kTiles: return tiled_edge_outputs(e, X, m, distances, distortions, flag, st);
+    case kSoa: case kSoaEll: break;
+  }
+  const int tb = 256, nb = ceil_div_i64(e->p, tb);
+  edge_outputs_kernel<0><<<nb, tb, 0, st>>>(e->src, e->dst, e->par0, e->has_par1 ? e->par1 : nullptr, e->perm, e->p, m,
+                                            X, distances, distortions, e->fn, flag);
   MDE_LAUNCH_CHECK();
   return 0;
 }
-int scatter_external_flag(const mde_edges* e, const float* X, int m, const float* g, float* grad, const int* flag,
-                          cudaStream_t st) {
-  if (e->kind == 2) return pull_launch(2, e, X, m, grad, g, nullptr, flag, st);
-  if (e->kind == 1) return tiled_launch(2, e, X, m, grad, g, nullptr, flag, st);
-  return launch_distortion<2>(e, X, m, grad, g, nullptr, flag, st);
+
+int allow_max_smem(const void* kernel) {
+  if (!kernel) return MDE_E_UNSUPPORTED;
+  static std::vector<const void*> done;
+  if (std::find(done.begin(), done.end(), kernel) != done.end()) return 0;
+  const cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxDynSmem);
+  if (err != cudaSuccess) return (int)err;
+  done.push_back(kernel);
+  return 0;
 }
-double* loss_partials_mut(const mde_edges* e) { return e->loss_partials; }
-int64_t edges_p(const mde_edges* e) { return e->p; }
-int64_t edges_p_total(const mde_edges* e) { return e->p_total; }
-const double* loss_partials_ptr(const mde_edges* e) { return e->loss_partials; }
-int64_t edges_n(const mde_edges* e) { return e->n; }
+
+int split_ctas(int64_t nwt, const std::vector<int32_t>& bkt_wt0, std::vector<int32_t>& cta_wt0,
+               std::vector<int32_t>& cta_bkt0) {
+  const int ncta = (int)std::min<int64_t>(kNumSMs, std::max<int64_t>(1, (nwt + 1) / 2));
+  cta_wt0.resize(ncta + 1);
+  cta_bkt0.resize(ncta);
+  for (int c = 0; c <= ncta; ++c) cta_wt0[c] = (int32_t)(nwt * c / ncta);
+  for (int c = 0; c < ncta; ++c) {
+    const auto it = std::upper_bound(bkt_wt0.begin(), bkt_wt0.end(), cta_wt0[c]);
+    cta_bkt0[c] = (int32_t)(it - bkt_wt0.begin()) - 1;
+  }
+  return ncta;
+}
+
+int launch_persistent(const void* kernel, void* args, int ncta, int threads, size_t smem, int* nblocks_out,
+                      cudaStream_t st) {
+  const int rc = allow_max_smem(kernel);
+  if (rc) return rc;
+  MDE_CUDA_TRY(cudaLaunchKernel(kernel, dim3(ncta), dim3(threads), &args, smem, st));
+  MDE_LAUNCH_CHECK();
+  if (nblocks_out) *nblocks_out = ncta;
+  return 0;
+}
 
 }  // namespace mde
 
@@ -1028,8 +1038,7 @@ int mde_edges_create_ex(mde_edges_t** out, const int64_t* edges, int64_t p, int6
     int* cnt = nullptr;
     const int64_t q = 2 * p;
     size_t tb2 = 0, sb = 0;
-    int bits = 1;
-    while (bits < 32 && (1ll << bits) < n_items) ++bits;
+    const int bits = bits_for((uint64_t)(n_items - 1));
     TRY(cudaMalloc(&e->ent, sizeof(uint2) * q));
     TRY(cudaMalloc(&e->inc, sizeof(uint32_t) * q));
     TRY(cudaMalloc(&e->inc_off, sizeof(int64_t) * (n_items + 1)));
@@ -1096,12 +1105,8 @@ int mde_distortion(const mde_edges_t* e, const float* X, int m, float* grad, dou
                    void* stream) {
   if (!e || !X || m < 1) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
-  int nb = 0, rc;
-  if (e->kind == 3 && grad && m == e->m_hint) rc = ell_launch(e, X, m, grad, &nb, nullptr, st);
-  else if (e->kind == 2) rc = pull_launch(grad ? 0 : 1, e, X, m, grad, nullptr, &nb, nullptr, st);
-  else if (e->kind == 1) rc = tiled_launch(grad ? 0 : 1, e, X, m, grad, nullptr, &nb, nullptr, st);
-  else if (grad) rc = launch_distortion<0>(e, X, m, grad, nullptr, &nb, nullptr, st);
-  else rc = launch_distortion<1>(e, X, m, nullptr, nullptr, &nb, nullptr, st);
+  int nb = 0;
+  const int rc = evaluate(grad ? 0 : 1, e, X, m, grad, nullptr, &nb, nullptr, st);
   if (rc) return rc;
   if (loss_sum) {  // NULL: leave the per-block partials (kernel-only timing)
     add_partials_kernel<<<1, 256, 0, st>>>(e->loss_partials, nb, loss_sum);
@@ -1123,22 +1128,13 @@ int mde_function_eval(const mde_fn_t* fn, const float* par0, int64_t par0_len, c
 int mde_scatter_external(const mde_edges_t* e, const float* X, int m, const float* g, float* grad,
                          void* stream) {
   if (!e || !X || !g || !grad || m < 1) return MDE_E_INVALID;
-  if (e->kind == 2) return pull_launch(2, e, X, m, grad, g, nullptr, nullptr, (cudaStream_t)stream);
-  if (e->kind == 1) return tiled_launch(2, e, X, m, grad, g, nullptr, nullptr, (cudaStream_t)stream);
-  return launch_distortion<2>(e, X, m, grad, g, nullptr, nullptr, (cudaStream_t)stream);
+  return evaluate(2, e, X, m, grad, g, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 int mde_edge_outputs(const mde_edges_t* e, const float* X, int m, float* distances, float* distortions,
                      void* stream) {
   if (!e || !X || m < 1) return MDE_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (e->kind == 2) return pull_edge_outputs(e, X, m, distances, distortions, st);
-  if (e->kind == 1) return tiled_edge_outputs(e, X, m, distances, distortions, st);
-  int tb = 256, nb = ceil_div_i64(e->p, tb);
-  edge_outputs_kernel<0><<<nb, tb, 0, st>>>(e->src, e->dst, e->par0, e->has_par1 ? e->par1 : nullptr,
-                                            e->perm, e->p, m, X, distances, distortions, e->fn, nullptr);
-  MDE_LAUNCH_CHECK();
-  return 0;
+  return edge_outputs(e, X, m, distances, distortions, nullptr, (cudaStream_t)stream);
 }
 
 }  // extern "C"

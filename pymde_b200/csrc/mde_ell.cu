@@ -277,38 +277,6 @@ struct EllArgs {
   int x_vec_ok;
 };
 
-// neighbour row at BYTE offset `off` of the resident tile
-template <int M>
-__device__ __forceinline__ void e_lds_row(const float* __restrict__ Xt, uint32_t off, float (&o)[M]) {
-  const unsigned char* q = reinterpret_cast<const unsigned char*>(Xt) + off;
-  if constexpr (M == 2) { const float2 t = *reinterpret_cast<const float2*>(q); o[0] = t.x; o[1] = t.y; }
-  else if constexpr (M == 4) { const float4 t = *reinterpret_cast<const float4*>(q); o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w; }
-  else {
-#pragma unroll
-    for (int c = 0; c < M; ++c) o[c] = reinterpret_cast<const float*>(q)[c];
-  }
-}
-template <int M>
-__device__ __forceinline__ void e_ldg_row(const float* __restrict__ X, uint32_t r, float (&o)[M]) {
-  if constexpr (M == 1) { o[0] = __ldg(X + r); }
-  else if constexpr (M == 2) { const float2 t = __ldg(reinterpret_cast<const float2*>(X) + r); o[0] = t.x; o[1] = t.y; }
-  else if constexpr (M == 4) { const float4 t = __ldg(reinterpret_cast<const float4*>(X) + r); o[0] = t.x; o[1] = t.y; o[2] = t.z; o[3] = t.w; }
-  else {
-#pragma unroll
-    for (int c = 0; c < M; ++c) o[c] = __ldg(X + (size_t)r * M + c);
-  }
-}
-template <int M>
-__device__ __forceinline__ void e_red_row(float* __restrict__ G, uint32_t r, const float (&v)[M]) {
-  if constexpr (M == 1) red_add(G + r, v[0]);
-  else if constexpr (M == 2) red_add_v2(G + 2 * (size_t)r, v[0], v[1]);
-  else if constexpr (M == 4) red_add_v4(G + 4 * (size_t)r, v[0], v[1], v[2], v[3]);
-  else {
-#pragma unroll
-    for (int c = 0; c < M; ++c) red_add(G + (size_t)r * M + c, v[c]);
-  }
-}
-
 // PushAndPull(Log1p(1.5), Log(1.0)), MUFU math, class known at compile time.  Same formulas as
 // mde_common.cuh::edge_coeff_fast_log1p_log; returns the loss in log2 units (flog2 = w lg2(.), the block sum is
 // multiplied by ln 2 at the end) and gs = f'/(p d) WITHOUT the class constant (1.5/p attractive, 1/p repulsive: applied
@@ -349,13 +317,13 @@ struct EllFiniteAtZero {
 // MASK: the lane-slot row has pads (entries e >= cnt) that the generic functions must not see; rows whose 32 lane-slots
 // all hold W entries (almost all of them: lane-slots are sorted by length) run without the two selects
 template <int M, int FA, int FR, bool FAST, int CLS, bool MASK>
-__device__ __forceinline__ void ell_entry(const EllArgs& a, const float* __restrict__ Xt, const float (&xi)[M], float w,
+__device__ __forceinline__ void ell_entry(const EllArgs& a, const float* __restrict__ Xt, const Row<M>& xi, float w,
                                           uint32_t j, bool valid, float (&acc)[M], float& lf) {
   float xj[M], diff[M];
-  e_lds_row<M>(Xt, j, xj);
+  lds_row_at<M>(Xt, j, xj);
   float d2 = 0.0f;
 #pragma unroll
-  for (int c = 0; c < M; ++c) { diff[c] = xi[c] - xj[c]; d2 = fmaf(diff[c], diff[c], d2); }
+  for (int c = 0; c < M; ++c) { diff[c] = xi.v[c] - xj[c]; d2 = fmaf(diff[c], diff[c], d2); }
   float f, g;
   if constexpr (FAST) {
     ell_fast_coeff<CLS>(d2, w, f, g);  // pads: w = 0
@@ -388,7 +356,7 @@ __device__ __forceinline__ void ell_entry(const EllArgs& a, const float* __restr
 // all W entries of this lane's lane-slot, straight from the shared-memory slot
 template <int M, int FA, int FR, bool FAST, int CLS, bool MASK>
 __device__ __forceinline__ void ell_columns(const EllArgs& a, const float* __restrict__ Xt, const unsigned char* cols,
-                                            int lane, int W, int cnt, const float (&xi)[M], float (&acc)[M],
+                                            int lane, int W, int cnt, const Row<M>& xi, float (&acc)[M],
                                             float& lf) {
   const float2* wp = reinterpret_cast<const float2*>(cols) + lane;
   const uint32_t* ip = reinterpret_cast<const uint32_t*>(cols + 256) + lane;
@@ -518,8 +486,8 @@ distortion_ell_kernel(const EllArgs a) {
       const uint32_t ow = reinterpret_cast<const uint32_t*>(rec + 16)[k * 32 + lane];
       const uint32_t own = ow & kOwnMask;
       const int cnt = (int)((ow >> 24) & 0x7fu);
-      float xi[M], acc[M];
-      e_ldg_row<M>(a.X, own, xi);
+      const Row<M> xi = ldg_row<M>(a.X, own);
+      float acc[M];
 #pragma unroll
       for (int q = 0; q < M; ++q) acc[q] = 0.0f;
       float lf = 0.0f;
@@ -534,7 +502,7 @@ distortion_ell_kernel(const EllArgs a) {
       } else {
         ell_columns<M, FA, FR, false, 2, true>(a, Xt, cols + k * row_bytes, lane, W, cnt, xi, acc, lf);
       }
-      if (!(ow >> 31)) e_red_row<M>(a.grad, own, acc);
+      if (!(ow >> 31)) red_row<M>(a.grad, own, acc);
       lrec += lf;
     }
     lsum += (double)lrec;
@@ -557,46 +525,19 @@ size_t ell_smem_bytes(int rb, int m) {
          (size_t)(2 * kEllWarps + 2) * sizeof(uint64_t) + 32 * sizeof(double);
 }
 
-template <int M>
-const void* eselect_m(const FnDev& fn, bool precise) {
-  const int fa = fn.fn_att, fr = fn.fn_rep, pp = fn.push_pull;
-#define EK(FA, FR, FAST) reinterpret_cast<const void*>(&distortion_ell_kernel<M, FA, FR, FAST>)
-  if constexpr (M == 2 || M == 3) {
-    const bool hot = pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG && fn.a0 == 1.5f && fn.r0 == 1.0f && !precise;
-    if (hot) return EK(MDE_FN_P_LOG1P, MDE_FN_P_LOG, true);
-    if (pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG) return EK(MDE_FN_P_LOG1P, MDE_FN_P_LOG, false);
-    if (!pp && fa == MDE_FN_P_QUADRATIC) return EK(MDE_FN_P_QUADRATIC, MDE_FN_P_QUADRATIC, false);
-    if (!pp && fa == MDE_FN_L_QUADRATIC) return EK(MDE_FN_L_QUADRATIC, MDE_FN_L_QUADRATIC, false);
-    if (!pp && fa == MDE_FN_L_HUBER) return EK(MDE_FN_L_HUBER, MDE_FN_L_HUBER, false);
-  }
-  return EK(-1, -1, false);
-#undef EK
-}
-// `precise`: mde_edges::kvar == 2 (MDE_B200_KERNEL=precise, read when the layout was created)
-const void* eselect_kernel(const mde_edges* e, int m) {
-  const bool precise = e->kvar == 2;
-  switch (m) {
-    case 1: return eselect_m<1>(e->fn, precise);
-    case 2: return eselect_m<2>(e->fn, precise);
-    case 3: return eselect_m<3>(e->fn, precise);
-    case 4: return eselect_m<4>(e->fn, precise);
-  }
-  return nullptr;
-}
-int econfigure_kernel(const void* k) {
-  static std::vector<const void*> done;
-  if (std::find(done.begin(), done.end(), k) != done.end()) return 0;
-  cudaError_t err = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  if (err != cudaSuccess) return (int)err;
-  done.push_back(k);
-  return 0;
-}
+// compile-time function pairs of the ELL kernel
+using EllPairs = FnList<Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>, Fn1<MDE_FN_P_QUADRATIC>, Fn1<MDE_FN_L_QUADRATIC>,
+                        Fn1<MDE_FN_L_HUBER>>;
 
-int ell_default_rb(int m) { return (m <= 2) ? 13 : 12; }  // X tile of 64 KB (m = 1: 32 KB, m = 3: 48 KB)
-
-int eenv_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return e ? atoi(e) : dflt;
+const void* select_kernel(const mde_edges* e, int m) {
+  const bool fast = fast_log1p_log(e->fn, e->kvar == 2);
+  return with_small_m(m, [&](auto mc) {
+    constexpr int M = decltype(mc)::value;
+    return select_fn<M, 0>(e->fn, fast, EllPairs{}, [](auto f) {
+      using F = decltype(f);
+      return reinterpret_cast<const void*>(&distortion_ell_kernel<M, F::FA, F::FR, F::FAST>);
+    });
+  });
 }
 
 }  // namespace
@@ -612,10 +553,9 @@ void ell_free(mde_edges* e) {
 
 bool ell_supported(int64_t n, int m) {
   if (m < 1 || m > 4 || n >= (1ll << 24)) return false;
-  int rb = ell_default_rb(m);
-  { const int r = eenv_int("MDE_B200_TILE_RB", 0); if (r >= 8 && r <= 15) rb = r; }
+  const int rb = tile_rb(m);
   const int64_t R = 1ll << rb;
-  return ((n + R - 1) >> rb) <= 32 && (R - 1) * 4 * m <= 65535 && ell_smem_bytes(rb, m) <= 227u * 1024u;
+  return ((n + R - 1) >> rb) <= 32 && (R - 1) * 4 * m <= 65535 && ell_smem_bytes(rb, m) <= kMaxDynSmem;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -711,12 +651,6 @@ __global__ void ell_fill_kernel(const uint32_t* __restrict__ rec_off, const int3
   }
 }
 
-int ebits_for(uint64_t maxval) {
-  int b = 1;
-  while (b < 64 && (maxval >> b) != 0) ++b;
-  return b;
-}
-
 }  // namespace
 namespace mde {
 
@@ -749,13 +683,13 @@ int ell_build_device(int64_t n, int64_t p, int m, const int32_t* src, const int3
   ++g_launch_count;
   TRY(cudaPeekAtLastError());
   // workspace: the largest of the four CUB calls
-  TRY(cub::DeviceRadixSort::SortPairs(nullptr, need, keys_in, keys_out, vals_in, vals_out, (int)p2, 0, ebits_for((uint64_t)ng), st));
+  TRY(cub::DeviceRadixSort::SortPairs(nullptr, need, keys_in, keys_out, vals_in, vals_out, (int)p2, 0, bits_for((uint64_t)ng), st));
   tmp_bytes = need;
   TRY(cub::DeviceScan::ExclusiveSum(nullptr, need, gcount, gstart, (int)ng, st));
   tmp_bytes = std::max(tmp_bytes, need);
   TRY(cudaMalloc(&tmp, tmp_bytes));
   need = tmp_bytes;
-  TRY(cub::DeviceRadixSort::SortPairs(tmp, need, keys_in, keys_out, vals_in, vals_out, (int)p2, 0, ebits_for((uint64_t)ng), st));
+  TRY(cub::DeviceRadixSort::SortPairs(tmp, need, keys_in, keys_out, vals_in, vals_out, (int)p2, 0, bits_for((uint64_t)ng), st));
   need = tmp_bytes;
   TRY(cub::DeviceScan::ExclusiveSum(tmp, need, gcount, gstart, (int)ng, st));
   ell_group_slots_kernel<<<ceil_div_i64(ng, tb), tb, 0, st>>>(gcount, ng, gslots);
@@ -776,7 +710,7 @@ int ell_build_device(int64_t n, int64_t p, int m, const int32_t* src, const int3
   TRY(cudaPeekAtLastError());
   {
     size_t need2 = 0;
-    const int sbits = ebits_for((uint64_t)(ndt * 2 * 8));
+    const int sbits = bits_for((uint64_t)(ndt * 2 * 8));
     TRY(cub::DeviceRadixSort::SortPairs(nullptr, need2, skey, skey_o, sval, sval_o, (int)nslots, 0, sbits, st));
     if (need2 > tmp_bytes) { cudaFree(tmp); tmp = nullptr; TRY(cudaMalloc(&tmp, need2)); tmp_bytes = need2; }
     need2 = tmp_bytes;
@@ -817,16 +751,13 @@ done:
 // (MDE_B200_ELL_BUILD=host: copies them to the host and runs ell_build_host, the builder the CPU tests cover; both give the
 // same bytes); on success the layout becomes kind 3.  Returns 0, MDE_E_UNSUPPORTED (layout stays kind 0) or an error.
 int ell_build(mde_edges* e, const mde_fn_t* fn, int m, cudaStream_t st) {
-  if (e->kind != 0 || e->has_par1 || e->det || m < 1 || m > 4) return MDE_E_UNSUPPORTED;
-  int rb = ell_default_rb(m);
-  { const int r = eenv_int("MDE_B200_TILE_RB", 0); if (r >= 8 && r <= 15) rb = r; }
-  if (ell_smem_bytes(rb, m) > 227u * 1024u) return MDE_E_UNSUPPORTED;
+  if (e->kind != kSoa || e->has_par1 || e->det || m < 1 || m > 4) return MDE_E_UNSUPPORTED;
+  const int rb = tile_rb(m);
+  if (ell_smem_bytes(rb, m) > kMaxDynSmem) return MDE_E_UNSUPPORTED;
   const int64_t p = e->p, n = e->n;
   int rc = ell_check_shape(n, p, m, rb);
   if (rc) return rc;
-  const void* k = eselect_kernel(e, m);
-  if (!k) return MDE_E_UNSUPPORTED;
-  if ((rc = econfigure_kernel(k))) return rc;
+  if ((rc = allow_max_smem(select_kernel(e, m)))) return rc;
   const char* bev = getenv("MDE_B200_ELL_BUILD");
   const bool on_host = bev && !strcmp(bev, "host");
   EllHost h;
@@ -870,14 +801,14 @@ int ell_build(mde_edges* e, const mde_fn_t* fn, int m, cudaStream_t st) {
 #undef UP
   cudaError_t se = cudaStreamSynchronize(st);  // the host vectors die with this frame
   if (se != cudaSuccess) { ell_free(e); return (int)se; }
-  e->kind = 3; e->m_hint = m; e->rb = rb; e->ell_nrec = pl->nrec; e->ell_ncta = pl->ncta; e->nbkt = nbkt;
+  e->kind = kSoaEll; e->m_hint = m; e->rb = rb; e->ell_nrec = pl->nrec; e->ell_ncta = pl->ncta; e->nbkt = nbkt;
   e->nbytes += pl->rec_bytes + 4 * (pl->nrec + 1) + 4ll * (2 * nbkt + 4 * pl->ncta + 2);
   return 0;
 }
 
 int ell_launch(const mde_edges* e, const float* X, int m, float* grad, int* nblocks_out, const int* flag,
                cudaStream_t st) {
-  if (e->kind != 3 || m != e->m_hint || !grad) return MDE_E_UNSUPPORTED;
+  if (e->kind != kSoaEll || m != e->m_hint || !grad) return MDE_E_UNSUPPORTED;
   const size_t smem = ell_smem_bytes(e->rb, m);
   EllArgs a;
   a.rec = e->ell_rec; a.rec_off = e->ell_off; a.bkt_tile = e->ell_bkt_tile; a.bkt_wt0 = e->ell_bkt_wt0;
@@ -885,15 +816,7 @@ int ell_launch(const mde_edges* e, const float* X, int m, float* grad, int* nblo
   a.loss_partials = e->loss_partials; a.flag = flag; a.fn = e->fn; a.inv_p = 1.0f / (float)e->p_total;
   a.n = e->n; a.rb = e->rb;
   a.x_vec_ok = ((reinterpret_cast<uintptr_t>(X) & 15u) == 0) ? 1 : 0;
-  const void* k = eselect_kernel(e, m);
-  if (!k) return MDE_E_UNSUPPORTED;
-  int rc = econfigure_kernel(k);
-  if (rc) return rc;
-  void* args[] = {(void*)&a};
-  MDE_CUDA_TRY(cudaLaunchKernel(k, dim3(e->ell_ncta), dim3(kEllThreads), args, smem, st));
-  MDE_LAUNCH_CHECK();
-  if (nblocks_out) *nblocks_out = e->ell_ncta;
-  return 0;
+  return launch_persistent(select_kernel(e, m), &a, e->ell_ncta, kEllThreads, smem, nblocks_out, st);
 }
 
 }  // namespace mde
@@ -930,7 +853,7 @@ int mde_ell_host_layout(int64_t n_items, int64_t p, int embedding_dim, const int
                         const float* par0, int push_pull, int tile_rows_log2, int max_cta, mde_ell_host_t* out) {
   if (!src || !dst || !par0 || !out) return MDE_E_INVALID;
   EllHost h;
-  const int rb = tile_rows_log2 > 0 ? tile_rows_log2 : ell_default_rb(embedding_dim);
+  const int rb = tile_rows_log2 > 0 ? tile_rows_log2 : default_tile_rb(embedding_dim);
   const int rc = ell_build_host(n_items, p, embedding_dim, src, dst, par0, push_pull, rb, max_cta > 0 ? max_cta : kNumSMs, h);
   if (rc) return rc;
   return ell_export(h.plan, h.rec.data(), h.rb, h.nentries, out);
@@ -942,7 +865,7 @@ int mde_ell_device_layout(int64_t n_items, int64_t p, int embedding_dim, const i
   if (!src || !dst || !par0 || !out) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   mde::EllDev d;
-  const int rb = tile_rows_log2 > 0 ? tile_rows_log2 : ell_default_rb(embedding_dim);
+  const int rb = tile_rows_log2 > 0 ? tile_rows_log2 : default_tile_rb(embedding_dim);
   int rc = mde::ell_build_device(n_items, p, embedding_dim, src, dst, par0, push_pull, rb, max_cta > 0 ? max_cta : kNumSMs, d, st);
   if (rc) return rc;
   std::vector<unsigned char> host((size_t)d.plan.rec_bytes);

@@ -19,8 +19,6 @@
 // owners is summed in registers and leaves as one vector red.  Nothing is written to shared memory after the
 // tile load.
 #include <cub/cub.cuh>
-#include <algorithm>
-#include <cstdlib>
 #include <cstring>
 #include <vector>
 
@@ -36,64 +34,6 @@ constexpr int kPullThreads = kPullWarps * 32;
 // a warp-tile holds NE = 32 * EPL entries (EPL = entries per lane per iteration: 4 or 8); record = 2 NE + 4 words
 __host__ __device__ constexpr int rec_words(int epl) { return 64 * epl + 4; }
 __host__ __device__ constexpr int rec_bytes(int epl) { return rec_words(epl) * 4; }  // 1040 (EPL 4) / 2064 (EPL 8)
-
-template <int M> struct PRow { float v[M]; };
-
-template <int M>
-__device__ __forceinline__ PRow<M> p_lds_row(const float* __restrict__ Xt, int r) {
-  PRow<M> o;
-  if constexpr (M == 2) { const float2 t = reinterpret_cast<const float2*>(Xt)[r]; o.v[0] = t.x; o.v[1] = t.y; }
-  else if constexpr (M == 4) { const float4 t = reinterpret_cast<const float4*>(Xt)[r]; o.v[0] = t.x; o.v[1] = t.y; o.v[2] = t.z; o.v[3] = t.w; }
-  else {
-#pragma unroll
-    for (int c = 0; c < M; ++c) o.v[c] = Xt[r * M + c];
-  }
-  return o;
-}
-template <int M>
-__device__ __forceinline__ PRow<M> p_ldg_row(const float* __restrict__ X, int r) {
-  PRow<M> o;
-  if constexpr (M == 1) { o.v[0] = __ldg(X + r); }
-  else if constexpr (M == 2) { const float2 t = __ldg(reinterpret_cast<const float2*>(X) + r); o.v[0] = t.x; o.v[1] = t.y; }
-  else if constexpr (M == 4) { const float4 t = __ldg(reinterpret_cast<const float4*>(X) + r); o.v[0] = t.x; o.v[1] = t.y; o.v[2] = t.z; o.v[3] = t.w; }
-  else {
-#pragma unroll
-    for (int c = 0; c < M; ++c) o.v[c] = __ldg(X + (int64_t)r * M + c);
-  }
-  return o;
-}
-template <int M>
-__device__ __forceinline__ void p_red_row(float* __restrict__ G, int r, const float (&v)[M]) {
-  if constexpr (M == 1) red_add(G + r, v[0]);
-  else if constexpr (M == 2) red_add_v2(G + 2 * (int64_t)r, v[0], v[1]);
-  else if constexpr (M == 4) red_add_v4(G + 4 * (int64_t)r, v[0], v[1], v[2], v[3]);
-  else {
-#pragma unroll
-    for (int c = 0; c < M; ++c) red_add(G + (int64_t)r * M + c, v[c]);
-  }
-}
-
-// PushAndPull(Log1p(1.5), Log(1.0)) with MUFU math, one class known at compile time (0 attractive, 1 repulsive);
-// same formulas as mde_common.cuh::edge_coeff_fast_log1p_log
-template <int CLS>
-__device__ __forceinline__ void pull_fast_coeff(float d2, float w, float inv_p, float& f, float& g) {
-  const float kLn2 = 0.69314718056f, kLog2e = 1.44269504089f;
-  const float rs = fast_rsqrt(d2);
-  const float d = (d2 > 0.0f) ? d2 * rs : 0.0f;
-  if constexpr (CLS == 0) {
-    const float sd = fast_sqrt(d);
-    const float one_p = 1.0f + d * sd;
-    f = w * kLn2 * fast_lg2(one_p);
-    g = w * (1.5f * inv_p) * sd * rs * fast_rcp(one_p);
-  } else {
-    const float em = fast_ex2(-d * kLog2e);
-    float one_m = 1.0f - em;
-    const float series = d * (1.0f - d * (0.5f - d * (0.16666667f - d * 0.041666668f)));
-    one_m = (d < 0.0625f) ? series : one_m;
-    f = w * kLn2 * fast_lg2(one_m);
-    g = w * inv_p * rs * em * fast_rcp(one_m);
-  }
-}
 
 struct PullArgs {
   const int32_t* rec;
@@ -122,13 +62,13 @@ __device__ __forceinline__ void pull_quad(const PullArgs& a, const float* __rest
                                           int own_base, int cnt, const float (&w)[4], const int (&oo)[4],
                                           const int (&nl)[4], const float (&gx)[4], int& cur, float (&acc)[M],
                                           float& lsum_f, double& lsum) {
-  PRow<M> xi[4], xj[4];
+  Row<M> xi[4], xj[4];
   int own[4];
 #pragma unroll
   for (int e = 0; e < 4; ++e) {
     own[e] = own_base + oo[e];
-    xi[e] = p_ldg_row<M>(a.X, own[e]);
-    xj[e] = p_lds_row<M>(Xt, nl[e]);
+    xi[e] = ldg_row<M>(a.X, own[e]);
+    xj[e] = lds_row<M>(Xt, nl[e]);
   }
 #pragma unroll
   for (int e = 0; e < 4; ++e) {
@@ -141,7 +81,7 @@ __device__ __forceinline__ void pull_quad(const PullArgs& a, const float* __rest
     if (MODE == 2) {
       g = gx[e];
     } else if (FAST) {
-      pull_fast_coeff<CLS>(d2, w[e], a.inv_p, f, g);
+      edge_coeff_fast_log1p_log<CLS>(d2, w[e], a.inv_p, f, g);
     } else {
       const float d = sqrtf(d2);
       if (MODE == 0) edge_coeff<FA, FR>(a.fn, d, w[e], 0.0f, a.inv_p, f, g);
@@ -157,7 +97,7 @@ __device__ __forceinline__ void pull_quad(const PullArgs& a, const float* __rest
       // d = 0: the reference replaces the non-finite g by 1 and the difference vector is 0
       const bool live = ok && (FAST ? (d2 > 0.0f) : true);
       if (own[e] != cur) {  // run ended (pads repeat the last owner: they never end one)
-        p_red_row<M>(a.grad, cur, acc);
+        red_row<M>(a.grad, cur, acc);
         cur = own[e];
 #pragma unroll
         for (int c = 0; c < M; ++c) acc[c] = 0.0f;
@@ -169,7 +109,7 @@ __device__ __forceinline__ void pull_quad(const PullArgs& a, const float* __rest
         float nv[M];
 #pragma unroll
         for (int c = 0; c < M; ++c) nv[c] = -v[c];
-        p_red_row<M>(a.grad, ibase + nl[e], nv);
+        red_row<M>(a.grad, ibase + nl[e], nv);
       }
     }
   }
@@ -322,7 +262,7 @@ distortion_pull_kernel(const PullArgs a) {
         else pull_quad<M, MODE, FA, FR, FAST, 2, false>(a, Xt, (int)base, first_idx, own_base, cnt, wq, oq, nq, gx, cur, acc, lsum_f, lsum);
       }
     }
-    if (MODE != 1 && (EPL * lane) < cnt) p_red_row<M>(a.grad, cur, acc);
+    if (MODE != 1 && (EPL * lane) < cnt) red_row<M>(a.grad, cur, acc);
     if (FAST) { lsum += (double)lsum_f; lsum_f = 0.0f; }
   }
   if (first && wt0 < wt1) { enter_bucket(); first = false; }
@@ -451,65 +391,32 @@ __global__ void pull_outputs_kernel(const int32_t* __restrict__ rec, const int32
   }
 }
 
-int pbits_for(uint64_t maxval) {
-  int b = 1;
-  while (b < 64 && (maxval >> b) != 0) ++b;
-  return b;
-}
-int penv_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return e ? atoi(e) : dflt;
-}
 size_t pull_smem_bytes(int rb, int m, int epl) {
   return (size_t)((size_t)1 << rb) * m * sizeof(float) + (size_t)kPullWarps * rec_bytes(epl) +
          (size_t)(kPullWarps + 2) * sizeof(uint64_t) + 32 * sizeof(double);
 }
 
-template <int M, int MODE, int FA, int FR, bool FAST>
-const void* pkptr(int epl) {
-  if (epl == 8) return reinterpret_cast<const void*>(&distortion_pull_kernel<M, MODE, FA, FR, FAST, 8>);
-  return reinterpret_cast<const void*>(&distortion_pull_kernel<M, MODE, FA, FR, FAST, 4>);
+// compile-time function pairs of the pull kernel
+using PullPairs = FnList<Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>, Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOGRATIO>, Fn1<MDE_FN_P_QUADRATIC>,
+                         Fn1<MDE_FN_L_ABSOLUTE>, Fn1<MDE_FN_L_QUADRATIC>, Fn1<MDE_FN_L_HUBER>>;
+
+template <int MODE>
+const void* select_kernel(const mde_edges* e, int m, int epl) {
+  const bool fast = fast_log1p_log(e->fn, e->kvar == 2);
+  return with_small_m(m, [&](auto mc) {
+    constexpr int M = decltype(mc)::value;
+    return select_fn<M, MODE>(e->fn, fast, PullPairs{}, [&](auto f) {
+      using F = decltype(f);
+      if (epl == 8) return reinterpret_cast<const void*>(&distortion_pull_kernel<M, MODE, F::FA, F::FR, F::FAST, 8>);
+      return reinterpret_cast<const void*>(&distortion_pull_kernel<M, MODE, F::FA, F::FR, F::FAST, 4>);
+    });
+  });
 }
 
-template <int M, int MODE>
-const void* pselect_m(const FnDev& fn, int epl, bool precise) {
-  const int fa = fn.fn_att, fr = fn.fn_rep, pp = fn.push_pull;
-  if constexpr (MODE == 0 && (M == 2 || M == 3)) {
-    const bool hot = pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG && fn.a0 == 1.5f && fn.r0 == 1.0f && !precise;
-    if (hot) return pkptr<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOG, true>(epl);
-    if (pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG) return pkptr<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOG, false>(epl);
-    if (pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOGRATIO) return pkptr<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOGRATIO, false>(epl);
-    if (!pp && fa == MDE_FN_P_QUADRATIC) return pkptr<M, MODE, MDE_FN_P_QUADRATIC, MDE_FN_P_QUADRATIC, false>(epl);
-    if (!pp && fa == MDE_FN_L_ABSOLUTE) return pkptr<M, MODE, MDE_FN_L_ABSOLUTE, MDE_FN_L_ABSOLUTE, false>(epl);
-    if (!pp && fa == MDE_FN_L_QUADRATIC) return pkptr<M, MODE, MDE_FN_L_QUADRATIC, MDE_FN_L_QUADRATIC, false>(epl);
-    if (!pp && fa == MDE_FN_L_HUBER) return pkptr<M, MODE, MDE_FN_L_HUBER, MDE_FN_L_HUBER, false>(epl);
-  }
-  return pkptr<M, MODE, -1, -1, false>(epl);
-}
-template <int MODE>
-const void* pselect_mode(const FnDev& fn, int m, int epl, bool precise) {
-  switch (m) {
-    case 1: return pselect_m<1, MODE>(fn, epl, precise);
-    case 2: return pselect_m<2, MODE>(fn, epl, precise);
-    case 3: return pselect_m<3, MODE>(fn, epl, precise);
-    case 4: return pselect_m<4, MODE>(fn, epl, precise);
-  }
-  return nullptr;
-}
-// `precise`: mde_edges::kvar == 2 (MDE_B200_KERNEL=precise, read when the layout was created)
-const void* pselect_kernel(const mde_edges* e, int m, int mode, int epl) {
-  const bool precise = e->kvar == 2;
-  if (mode == 0) return pselect_mode<0>(e->fn, m, epl, precise);
-  if (mode == 1) return pselect_mode<1>(e->fn, m, epl, precise);
-  return pselect_mode<2>(e->fn, m, epl, precise);
-}
-int pconfigure_kernel(const void* k) {
-  static std::vector<const void*> done;
-  if (std::find(done.begin(), done.end(), k) != done.end()) return 0;
-  cudaError_t err = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  if (err != cudaSuccess) return (int)err;
-  done.push_back(k);
-  return 0;
+const void* select_kernel(const mde_edges* e, int m, int mode, int epl) {
+  if (mode == 0) return select_kernel<0>(e, m, epl);
+  if (mode == 1) return select_kernel<1>(e, m, epl);
+  return select_kernel<2>(e, m, epl);
 }
 
 }  // namespace
@@ -526,15 +433,14 @@ int pull_build(mde_edges* e, const int64_t* edges, const float* par0, const mde_
   const int64_t p = e->p, n = e->n;
   if (m < 1 || m > 4 || p >= (1ll << 30)) return MDE_E_UNSUPPORTED;
   const int64_t p2 = 2 * p;
-  int rb = (m <= 2) ? 13 : 12;  // X tile of 64 KB (m = 1: 32 KB)
-  { const int r = penv_int("MDE_B200_TILE_RB", 0); if (r >= 8 && r <= 15) rb = r; }
+  const int rb = tile_rb(m);
   // entries per lane per warp-tile: 8 amortises the per-record work but needs enough
   // records to keep 32 warps on every SM busy; smaller problems take 4
   int epl = (p2 / 256 >= 8ll * kPullWarps * kNumSMs) ? 8 : 4;
-  { const int ev = penv_int("MDE_B200_PULL_EPL", 0); if (ev == 4 || ev == 8) epl = ev; }
+  { const int ev = env_int("MDE_B200_PULL_EPL", 0); if (ev == 4 || ev == 8) epl = ev; }
   const int NE = 32 * epl, kRecWords = rec_words(epl), kRecBytes = rec_bytes(epl);
-  if (rb > 16 || pull_smem_bytes(rb, m, epl) > 227u * 1024u) return MDE_E_UNSUPPORTED;
-  int64_t l2_bytes = (int64_t)penv_int("MDE_B200_STILE_MB", 24) << 20;  // src super-tile budget: see tiled_build
+  if (rb > 16 || pull_smem_bytes(rb, m, epl) > kMaxDynSmem) return MDE_E_UNSUPPORTED;
+  int64_t l2_bytes = (int64_t)env_int("MDE_B200_STILE_MB", 24) << 20;  // src super-tile budget: see tiled_build
   int ss = rb;
   while (((int64_t)1 << (ss + 1)) * m * 8 <= l2_bytes && ss < 30) ++ss;
   const int64_t R = (int64_t)1 << rb, S = (int64_t)1 << ss;
@@ -548,9 +454,9 @@ int pull_build(mde_edges* e, const int64_t* edges, const float* par0, const mde_
   int hybrid = 0;
   { const char* ev = getenv("MDE_B200_PULL_REP"); if (ev && !strcmp(ev, "push") && fn->push_pull) hybrid = 1; }
   PKeyBits kb;
-  kb.rb = rb; kb.ss = ss; kb.sb = pbits_for((uint64_t)(n - 1)); kb.ndt = ndt;
+  kb.rb = rb; kb.ss = ss; kb.sb = bits_for((uint64_t)(n - 1)); kb.ndt = ndt;
   kb.shift_own = rb; kb.shift_bkt = kb.sb + rb;
-  const int total_bits = kb.shift_bkt + pbits_for((uint64_t)nb_all);  // bucket id nb_all = dropped mirrors
+  const int total_bits = kb.shift_bkt + bits_for((uint64_t)nb_all);  // bucket id nb_all = dropped mirrors
   if (total_bits > 64) return MDE_E_UNSUPPORTED;
 
   uint64_t *keys_in = nullptr, *keys_out = nullptr;
@@ -616,7 +522,7 @@ int pull_build(mde_edges* e, const int64_t* edges, const float* par0, const mde_
     const int64_t nwt = slot / NE;
     lb_wt0.push_back((int32_t)nwt);
     const int nlb = (int)lb_id.size();
-    const int64_t min_per_bucket = penv_int("MDE_B200_TILE_MIN", 2048);
+    const int64_t min_per_bucket = env_int("MDE_B200_TILE_MIN", 2048);
     if (nlb > 2 && p2_eff / nlb < min_per_bucket) { rc = MDE_E_UNSUPPORTED; goto done; }
     // physical order: the two classes of one (super-tile, tile) group share the resident X tile, so their warp-tiles
     // are INTERLEAVED proportionally -- pull (issue-bound) and push (red-bound) records then alternate inside every
@@ -644,14 +550,7 @@ int pull_build(mde_edges* e, const int64_t* edges, const float* par0, const mde_
     bkt_wt0.push_back((int32_t)nwt);
     const int nbkt = (int)bkt_tile.size();
 
-    const int ncta = (int)std::min<int64_t>(kNumSMs, std::max<int64_t>(1, (nwt + 1) / 2));
-    cta_wt0.resize(ncta + 1);
-    cta_bkt0.resize(ncta);
-    for (int c = 0; c <= ncta; ++c) cta_wt0[c] = (int32_t)(nwt * c / ncta);
-    for (int c = 0; c < ncta; ++c) {
-      const auto it = std::upper_bound(bkt_wt0.begin(), bkt_wt0.end(), cta_wt0[c]);
-      cta_bkt0[c] = (int32_t)(it - bkt_wt0.begin()) - 1;
-    }
+    const int ncta = split_ctas(nwt, bkt_wt0, cta_wt0, cta_bkt0);
     wt_tile.resize(nwt);
     for (int b = 0; b < nbkt; ++b)
       for (int32_t t = bkt_wt0[b]; t < bkt_wt0[b + 1]; ++t) wt_tile[t] = bkt_tile[b];
@@ -685,12 +584,10 @@ int pull_build(mde_edges* e, const int64_t* edges, const float* par0, const mde_
     if (bad) { rc = MDE_E_UNSUPPORTED; goto done; }  // a warp-tile spans more than 65 536 owner rows (very sparse)
     e->fn = to_dev(*fn);
     for (int mode = 0; mode < 3; ++mode) {
-      const void* k = pselect_kernel(e, m, mode, epl);
-      if (!k) { rc = MDE_E_UNSUPPORTED; goto done; }
-      if ((rc = pconfigure_kernel(k))) goto done;
+      if ((rc = allow_max_smem(select_kernel(e, m, mode, epl)))) goto done;
     }
     e->epl = epl;
-    e->kind = 2; e->m_hint = m; e->rb = rb; e->ss = ss; e->nwt = nwt; e->nbkt = nbkt; e->ncta = ncta;
+    e->kind = kPull; e->m_hint = m; e->rb = rb; e->ss = ss; e->nwt = nwt; e->nbkt = nbkt; e->ncta = ncta;
     e->nbytes = nwt * (kRecBytes + 4 * NE + 4) + 8 * kMaxLossBlocks + 4ll * (2 * nbkt + 2 * ncta + 2);
   }
 done:
@@ -701,7 +598,7 @@ done:
     pull_free(e);
     cudaFree(e->perm);
     e->perm = nullptr;
-    e->kind = 0;
+    e->kind = kSoa;
   }
   return rc;
 #undef TRY
@@ -709,27 +606,19 @@ done:
 
 int pull_launch(int mode, const mde_edges* e, const float* X, int m, float* grad, const float* gext,
                 int* nblocks_out, const int* flag, cudaStream_t st) {
-  if (e->kind != 2 || m < 1 || m > 4) return MDE_E_UNSUPPORTED;
+  if (e->kind != kPull || m < 1 || m > 4) return MDE_E_UNSUPPORTED;
   const size_t smem = pull_smem_bytes(e->rb, m, e->epl);
-  if (smem > 227u * 1024u) return MDE_E_UNSUPPORTED;
+  if (smem > kMaxDynSmem) return MDE_E_UNSUPPORTED;
   PullArgs a;
   a.rec = e->rec; a.perm = e->perm; a.gext = gext; a.bkt_tile = e->bkt_tile; a.bkt_wt0 = e->bkt_wt0;
   a.cta_wt0 = e->cta_wt0; a.cta_bkt0 = e->cta_bkt0; a.X = X; a.grad = grad; a.loss_partials = e->loss_partials;
   a.flag = flag; a.fn = e->fn; a.inv_p = 1.0f / (float)e->p_total; a.n = e->n; a.rb = e->rb;
   a.x_vec_ok = ((reinterpret_cast<uintptr_t>(X) & 15u) == 0) ? 1 : 0;
-  const void* k = pselect_kernel(e, m, mode, e->epl);
-  if (!k) return MDE_E_UNSUPPORTED;
-  int rc = pconfigure_kernel(k);
-  if (rc) return rc;
-  void* args[] = {(void*)&a};
-  MDE_CUDA_TRY(cudaLaunchKernel(k, dim3(e->ncta), dim3(kPullThreads), args, smem, st));
-  MDE_LAUNCH_CHECK();
-  if (nblocks_out) *nblocks_out = e->ncta;
-  return 0;
+  return launch_persistent(select_kernel(e, m, mode, e->epl), &a, e->ncta, kPullThreads, smem, nblocks_out, st);
 }
 
 int pull_edge_outputs(const mde_edges* e, const float* X, int m, float* distances, float* distortions,
-                      cudaStream_t st, const int* flag) {
+                      const int* flag, cudaStream_t st) {
   const int64_t nslots = e->nwt * 32 * e->epl;
   const int tb = 256;
   pull_outputs_kernel<<<ceil_div_i64(nslots, tb), tb, 0, st>>>(e->rec, e->perm, e->wt_tile, e->rb, e->epl, nslots, m, X,

@@ -24,25 +24,9 @@
 #include <cstring>
 #include <new>
 
-#include "mde_common.cuh"
+#include "mde_edges.cuh"
 #include "mde_logic.h"
 #include "mde_project.cuh"
-
-struct mde_edges;
-namespace mde {
-int distortion_fused(const mde_edges* e, const float* X, int m, float* grad, int* nblocks, cudaStream_t st);
-int distortion_fused_flag(const mde_edges* e, const float* X, int m, float* grad, int* nblocks,
-                          const int* flag, cudaStream_t st);
-const double* loss_partials_ptr(const mde_edges* e);
-double* loss_partials_mut(const mde_edges* e);
-int edge_distances_flag(const mde_edges* e, const float* X, int m, float* distances, const int* flag,
-                        cudaStream_t st);
-int scatter_external_flag(const mde_edges* e, const float* X, int m, const float* g, float* grad, const int* flag,
-                          cudaStream_t st);
-int64_t edges_n(const mde_edges* e);
-int64_t edges_p(const mde_edges* e);
-int64_t edges_p_total(const mde_edges* e);
-}  // namespace mde
 
 using namespace mde;
 
@@ -1273,7 +1257,7 @@ int add_child_graph(cudaGraph_t child, cudaGraphExec_t exec, cudaStream_t st) {
 
 int enqueue_external(mde_solver* s, const int* flag, cudaStream_t st) {
   const mde_external_t& x = s->ext;
-  int rc = edge_distances_flag(s->edges, s->X, s->m, x.d, flag, st);
+  int rc = edge_outputs(s->edges, s->X, s->m, x.d, nullptr, flag, st);
   if (rc) return rc;
   if (x.graph) {
     if ((rc = add_child_graph((cudaGraph_t)x.graph, s->part_exec[0], st))) return rc;
@@ -1282,9 +1266,9 @@ int enqueue_external(mde_solver* s, const int* flag, cudaStream_t st) {
   }
   int nb = (int)((s->p + 255) / 256);
   if (nb > kVecBlocks) nb = kVecBlocks;
-  ext_coeff_kernel<<<nb, 256, 0, st>>>(flag, x.fpp, x.d, x.loss, s->gcoef, loss_partials_mut(s->edges), s->p);
+  ext_coeff_kernel<<<nb, 256, 0, st>>>(flag, x.fpp, x.d, x.loss, s->gcoef, s->edges->loss_partials, s->p);
   MDE_LAUNCH_CHECK();
-  return scatter_external_flag(s->edges, s->X, s->m, s->gcoef, s->g, flag, st);
+  return evaluate(2, s->edges, s->X, s->m, s->g, s->gcoef, nullptr, flag, st);
 }
 
 // caller-defined constraint: which = 0 retraction [X -> u] -> caller -> [u -> X], which = 1 tangent projection
@@ -1317,10 +1301,11 @@ int enqueue_eval(mde_solver* s, const int* flag, cudaStream_t st) {
   // several GPUs: scatter into this rank's partial buffer (peer-visible), then all-reduce into g
   const bool multi = s->opts.world_size > 1;
   float* target = multi ? s->gpart : s->g;
-  int rc = s->ext.d ? enqueue_external(s, flag, st) : distortion_fused_flag(s->edges, s->X, s->m, target, &s->nl, flag, st);
+  int rc = s->ext.d ? enqueue_external(s, flag, st)
+                     : evaluate(0, s->edges, s->X, s->m, target, nullptr, &s->nl, flag, st);
   if (rc) return rc;
   if (multi) {
-    pack_loss_kernel<<<1, 256, 0, st>>>(flag, loss_partials_ptr(s->edges), s->nl, target + s->npad);
+    pack_loss_kernel<<<1, 256, 0, st>>>(flag, s->edges->loss_partials, s->nl, target + s->npad);
     MDE_LAUNCH_CHECK();
     if (s->comm_connected) {
       const int64_t n4 = s->npad >> 2;
@@ -1376,8 +1361,8 @@ int enqueue_step(mde_solver* s, cudaStream_t st) {
   int rc = 0;
   const int slices = (s->opts.memory_size + kPairsPerSlice - 1) / kPairsPerSlice;
   Tail tl;
-  tl.lpart = loss_partials_ptr(s->edges); tl.nl = s->nl; tl.tail = s->g + s->npad;
-  tl.p_total = (double)edges_p_total(s->edges); tl.inv_n = 1.0 / (double)s->n;
+  tl.lpart = s->edges->loss_partials; tl.nl = s->nl; tl.tail = s->g + s->npad;
+  tl.p_total = (double)s->edges->p_total; tl.inv_n = 1.0 / (double)s->n;
   step_head_kernel<<<dim3(s->nvb, slices), kVecThreads, 0, st>>>(S, s->g, s->gprev, s->d, s->X, s->Sb, s->Yb, s->npad,
                                                                  s->center_m, s->dpart, s->vpart, tl);
   MDE_LAUNCH_CHECK();
@@ -1528,7 +1513,7 @@ int solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m, co
   if (opts->max_iter < 1) return MDE_E_INVALID;
   if (opts->mode == 0 || opts->mode == 1) return MDE_E_UNSUPPORTED;  // retired drivers (host-stepped, conditional graph)
   if (opts->mode != 2) return MDE_E_INVALID;
-  if (n != edges_n(e)) return MDE_E_INVALID;
+  if (n != e->n) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   mde_solver* s = new (std::nothrow) mde_solver();
   if (!s) return MDE_E_ALLOC;
@@ -1588,7 +1573,7 @@ int solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m, co
   if (opts->constraint == MDE_CONSTRAINT_CENTERED && (m == 1 || m == 2 || m == 4)) s->center_m = m;
   if (cpart) s->cpart = *cpart;  // (before the first capture, like the external descriptor)
   if (ext) {  // the descriptor is in place before the first capture
-    s->p = edges_p(e);
+    s->p = e->p;
     TRY(cudaMalloc(&s->gcoef, sizeof(float) * s->p));
     TRY(cudaStreamSynchronize(st));
     if ((rc = attach_external(s, ext))) goto fail;

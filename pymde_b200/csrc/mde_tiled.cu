@@ -18,8 +18,6 @@
 // Global L2 requests per edge drop from ~3.3 (2 row gathers + 1.3 reds) to the src side only
 // (~0.2 sector reads + <= 1 red).
 #include <cub/cub.cuh>
-#include <algorithm>
-#include <cstdlib>
 #include <cstring>
 #include <vector>
 
@@ -32,35 +30,6 @@ namespace {
 
 constexpr int kTileWarps = 32;                    // warps per CTA (1 CTA per SM)
 constexpr int kTileThreads = kTileWarps * 32;
-
-// ------------------------------------------------------------------------------------------
-// shared-memory rows
-// ------------------------------------------------------------------------------------------
-template <int M> struct TRow { float v[M]; };
-
-template <int M>
-__device__ __forceinline__ TRow<M> lds_row(const float* __restrict__ Xt, int r) {
-  TRow<M> o;
-  if constexpr (M == 2) { const float2 t = reinterpret_cast<const float2*>(Xt)[r]; o.v[0] = t.x; o.v[1] = t.y; }
-  else if constexpr (M == 4) { const float4 t = reinterpret_cast<const float4*>(Xt)[r]; o.v[0] = t.x; o.v[1] = t.y; o.v[2] = t.z; o.v[3] = t.w; }
-  else {
-#pragma unroll
-    for (int c = 0; c < M; ++c) o.v[c] = Xt[r * M + c];
-  }
-  return o;
-}
-template <int M>
-__device__ __forceinline__ TRow<M> ldg_row(const float* __restrict__ X, int r) {
-  TRow<M> o;
-  if constexpr (M == 1) { o.v[0] = __ldg(X + r); }
-  else if constexpr (M == 2) { const float2 t = __ldg(reinterpret_cast<const float2*>(X) + r); o.v[0] = t.x; o.v[1] = t.y; }
-  else if constexpr (M == 4) { const float4 t = __ldg(reinterpret_cast<const float4*>(X) + r); o.v[0] = t.x; o.v[1] = t.y; o.v[2] = t.z; o.v[3] = t.w; }
-  else {
-#pragma unroll
-    for (int c = 0; c < M; ++c) o.v[c] = __ldg(X + (int64_t)r * M + c);
-  }
-  return o;
-}
 
 // (x, y) += (a, b) on an 8-byte aligned shared-memory pair: ONE 64-bit CAS per attempt (fp32 add has no native
 // shared-memory atomic on sm_90a -- atomicAdd(float*) itself compiles to LDS + FADD + ATOMS.CAST.SPIN)
@@ -87,17 +56,6 @@ __device__ __forceinline__ void smem_sub_row(float* __restrict__ Gt, int r, cons
   }
 }
 
-template <int M>
-__device__ __forceinline__ void red_row_g(float* __restrict__ G, int r, const float (&v)[M]) {
-  if constexpr (M == 1) red_add(G + r, v[0]);
-  else if constexpr (M == 2) red_add_v2(G + 2 * (int64_t)r, v[0], v[1]);
-  else if constexpr (M == 4) red_add_v4(G + 4 * (int64_t)r, v[0], v[1], v[2], v[3]);
-  else {
-#pragma unroll
-    for (int c = 0; c < M; ++c) red_add(G + (int64_t)r * M + c, v[c]);
-  }
-}
-
 struct TileArgs {
   const int32_t* rec;
   const int32_t* perm;
@@ -119,39 +77,13 @@ struct TileArgs {
   int gred;      // 1: dst contributions leave as global reds (no gradient tile, no CAS); the X tile may be twice as large
 };
 
-// PushAndPull(Log1p(1.5), Log(1.0)) with MUFU math (mde_common.cuh::edge_coeff_fast_log1p_log), one-sided when the
-// class of the whole warp-tile is known: CLS 0 = attractive, 1 = repulsive, 2 = per-edge select.
-template <int CLS>
-__device__ __forceinline__ void fast_coeff(float d2, float w, float inv_p, float& f, float& g) {
-  if constexpr (CLS == 2) {
-    edge_coeff_fast_log1p_log(d2, w, inv_p, f, g);
-  } else {
-    const float kLn2 = 0.69314718056f, kLog2e = 1.44269504089f;
-    const float rs = fast_rsqrt(d2);
-    const float d = (d2 > 0.0f) ? d2 * rs : 0.0f;
-    if constexpr (CLS == 0) {
-      const float sd = fast_sqrt(d);
-      const float one_p = 1.0f + d * sd;
-      f = w * kLn2 * fast_lg2(one_p);
-      g = w * (1.5f * inv_p) * sd * rs * fast_rcp(one_p);
-    } else {
-      const float em = fast_ex2(-d * kLog2e);
-      float one_m = 1.0f - em;
-      const float series = d * (1.0f - d * (0.5f - d * (0.16666667f - d * 0.041666668f)));
-      one_m = (d < 0.0625f) ? series : one_m;
-      f = w * kLn2 * fast_lg2(one_m);
-      g = w * inv_p * rs * em * fast_rcp(one_m);
-    }
-  }
-}
-
 // One thread, 4 consecutive slots of a warp-tile: src rows from global (L1-cached, sorted => neighbouring lanes
 // share sectors), dst rows and the dst gradient in the resident tile.
 template <int M, int MODE, int FA, int FR, bool FAST, int CLS>
 __device__ __forceinline__ void quad_compute(const TileArgs& a, const float* __restrict__ Xt, float* __restrict__ Gt,
                                              int ibase, const int (&s)[4], const int (&td)[4], const float (&av)[4],
                                              float& lsum_f, double& lsum) {
-  TRow<M> xi[4], xj[4];
+  Row<M> xi[4], xj[4];
   int dl[4];
 #pragma unroll
   for (int e = 0; e < 4; ++e) {
@@ -175,7 +107,7 @@ __device__ __forceinline__ void quad_compute(const TileArgs& a, const float* __r
     if (MODE == 2) {
       g = av[e];
     } else if (FAST) {
-      fast_coeff<CLS>(d2, av[e], a.inv_p, f, g);
+      edge_coeff_fast_log1p_log<CLS>(d2, av[e], a.inv_p, f, g);
     } else {
       const float d = sqrtf(d2);
       if (MODE == 0) edge_coeff<FA, FR>(a.fn, d, av[e], 0.0f, a.inv_p, f, g);
@@ -193,14 +125,14 @@ __device__ __forceinline__ void quad_compute(const TileArgs& a, const float* __r
           float nv[M];
 #pragma unroll
           for (int cc = 0; cc < M; ++cc) nv[cc] = -v[cc];
-          red_row_g<M>(a.grad, td[e], nv);
+          red_row<M>(a.grad, td[e], nv);
         } else {
           smem_sub_row<M>(Gt, dl[e], v);
         }
       }
       const int se = ok ? s[e] : cur;  // pads never break a run
       if (se != cur) {                 // run of equal src ended: flush its sum
-        red_row_g<M>(a.grad, cur, acc);
+        red_row<M>(a.grad, cur, acc);
         cur = se;
 #pragma unroll
         for (int cc = 0; cc < M; ++cc) acc[cc] = 0.0f;
@@ -209,7 +141,7 @@ __device__ __forceinline__ void quad_compute(const TileArgs& a, const float* __r
       for (int cc = 0; cc < M; ++cc) acc[cc] += v[cc];
     }
   }
-  if (MODE != 1) red_row_g<M>(a.grad, cur, acc);
+  if (MODE != 1) red_row<M>(a.grad, cur, acc);
   if (FAST) { lsum += (double)lsum_f; lsum_f = 0.0f; }
 }
 
@@ -481,27 +413,36 @@ __global__ void tiled_outputs_kernel(const int32_t* __restrict__ rec, const int3
   }
 }
 
-int bits_for(uint64_t maxval) {  // bits needed to hold values 0..maxval
-  int b = 1;
-  while (b < 64 && (maxval >> b) != 0) ++b;
-  return b;
-}
-
-int env_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return e ? atoi(e) : dflt;
-}
-
 size_t tile_smem_bytes(int rb, int m, int gred) {
   return (size_t)(gred ? 1 : 2) * ((size_t)1 << rb) * m * sizeof(float) + (size_t)kTileWarps * kWtBytes +
          (size_t)(kTileWarps + 2) * sizeof(uint64_t) + 32 * sizeof(double);
 }
 
+// compile-time function pairs of the tile kernel
+using TilePairs = FnList<Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>, Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOGRATIO>, Fn1<MDE_FN_P_QUADRATIC>,
+                         Fn1<MDE_FN_L_ABSOLUTE>, Fn1<MDE_FN_L_QUADRATIC>, Fn1<MDE_FN_L_HUBER>>;
+
+template <int MODE>
+const void* select_kernel(const mde_edges* e, int m) {
+  const bool fast = fast_log1p_log(e->fn, e->kvar == 2);
+  return with_small_m(m, [&](auto mc) {
+    constexpr int M = decltype(mc)::value;
+    return select_fn<M, MODE>(e->fn, fast, TilePairs{}, [](auto f) {
+      using F = decltype(f);
+      return reinterpret_cast<const void*>(&distortion_tile_kernel<M, MODE, F::FA, F::FR, F::FAST>);
+    });
+  });
+}
+
+const void* select_kernel(const mde_edges* e, int m, int mode) {
+  if (mode == 0) return select_kernel<0>(e, m);
+  if (mode == 1) return select_kernel<1>(e, m);
+  return select_kernel<2>(e, m);
+}
+
 }  // namespace
 
 namespace mde {
-
-int tiled_configure(const mde_edges* e, int m);
 
 void tiled_free(mde_edges* e) {
   cudaFree(e->rec); cudaFree(e->bkt_tile); cudaFree(e->bkt_wt0); cudaFree(e->cta_wt0); cudaFree(e->cta_bkt0);
@@ -513,11 +454,10 @@ void tiled_free(mde_edges* e) {
 int tiled_build(mde_edges* e, const int64_t* edges, const float* par0, const mde_fn_t* fn, int m, cudaStream_t st) {
   const int64_t p = e->p, n = e->n;
   if (m < 1 || m > 4) return MDE_E_UNSUPPORTED;
-  int rb = (m <= 2) ? 13 : 12;  // R = 8192 rows (m <= 2) / 4096 rows: X tile + gradient tile = 128 KB
-  { const int r = env_int("MDE_B200_TILE_RB", 0); if (r >= 8 && r <= 15) rb = r; }
+  const int rb = tile_rb(m);
   int gred = 0;
   { const char* ev = getenv("MDE_B200_TILE_SCATTER"); if (ev && !strcmp(ev, "global")) gred = 1; }
-  if (tile_smem_bytes(rb, m, gred) > 227u * 1024u) return MDE_E_UNSUPPORTED;
+  if (tile_smem_bytes(rb, m, gred) > kMaxDynSmem) return MDE_E_UNSUPPORTED;
   // src super-tile: X + gradient rows of one super-tile (2 * m * 4 bytes per row) stay L2-resident; 24 MB leaves
   // about half of the H100's 50 MB L2 to the streamed records and the destination side
   int64_t l2_bytes = (int64_t)env_int("MDE_B200_STILE_MB", 24) << 20;
@@ -590,14 +530,7 @@ int tiled_build(mde_edges* e, const int64_t* edges, const float* par0, const mde
     const int64_t min_per_bucket = env_int("MDE_B200_TILE_MIN", 2048);
     if (nbkt > 1 && p / nbkt < min_per_bucket) { rc = MDE_E_UNSUPPORTED; goto done; }
 
-    int ncta = (int)std::min<int64_t>(kNumSMs, std::max<int64_t>(1, (nwt + 1) / 2));
-    cta_wt0.resize(ncta + 1);
-    cta_bkt0.resize(ncta);
-    for (int cidx = 0; cidx <= ncta; ++cidx) cta_wt0[cidx] = (int32_t)(nwt * cidx / ncta);
-    for (int cidx = 0; cidx < ncta; ++cidx) {
-      const auto it = std::upper_bound(bkt_wt0.begin(), bkt_wt0.end(), cta_wt0[cidx]);
-      cta_bkt0[cidx] = (int32_t)(it - bkt_wt0.begin()) - 1;
-    }
+    const int ncta = split_ctas(nwt, bkt_wt0, cta_wt0, cta_bkt0);
 
     TRY(cudaMalloc(&e->rec, sizeof(int32_t) * nwt * kWtWords));
     TRY(cudaMalloc(&e->perm, sizeof(int32_t) * nwt * kWtEdges));
@@ -619,9 +552,11 @@ int tiled_build(mde_edges* e, const int64_t* edges, const float* par0, const mde
     TRY(cudaPeekAtLastError());
     TRY(cudaStreamSynchronize(st));
     e->fn = to_dev(*fn);
-    if ((rc = tiled_configure(e, m))) goto done;
+    for (int mode = 0; mode < 3; ++mode) {
+      if ((rc = allow_max_smem(select_kernel(e, m, mode)))) goto done;
+    }
     e->gred = gred;
-    e->kind = 1; e->m_hint = m; e->rb = rb; e->ss = ss; e->nwt = nwt; e->nbkt = nbkt; e->ncta = ncta;
+    e->kind = kTiles; e->m_hint = m; e->rb = rb; e->ss = ss; e->nwt = nwt; e->nbkt = nbkt; e->ncta = ncta;
     e->nbytes = nwt * (kWtBytes + 4 * kWtEdges) + 8 * kMaxLossBlocks + 4ll * (2 * nbkt + 2 * ncta + 2);
   }
 done:
@@ -631,77 +566,17 @@ done:
     tiled_free(e);
     cudaFree(e->perm);
     e->perm = nullptr;
-    e->kind = 0;
+    e->kind = kSoa;
   }
   return rc;
 #undef TRY
 }
 
-template <int M, int MODE, int FA, int FR, bool FAST>
-static const void* kptr() { return reinterpret_cast<const void*>(&distortion_tile_kernel<M, MODE, FA, FR, FAST>); }
-
-// hot function combinations get compile-time ids (fused mode, m = 2 / 3), the rest use the run-time table;
-// `precise` (mde_edges::kvar == 2, MDE_B200_KERNEL=precise) keeps the hot combination off the MUFU math
-template <int M, int MODE>
-static const void* select_m(const FnDev& fn, bool precise) {
-  const int fa = fn.fn_att, fr = fn.fn_rep, pp = fn.push_pull;
-  if constexpr (MODE == 0 && (M == 2 || M == 3)) {
-    const bool hot = pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG && fn.a0 == 1.5f && fn.r0 == 1.0f && !precise;
-    if (hot) return kptr<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOG, true>();
-    if (pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOG) return kptr<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOG, false>();
-    if (pp && fa == MDE_FN_P_LOG1P && fr == MDE_FN_P_LOGRATIO) return kptr<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOGRATIO, false>();
-    if (!pp && fa == MDE_FN_P_QUADRATIC) return kptr<M, MODE, MDE_FN_P_QUADRATIC, MDE_FN_P_QUADRATIC, false>();
-    if (!pp && fa == MDE_FN_L_ABSOLUTE) return kptr<M, MODE, MDE_FN_L_ABSOLUTE, MDE_FN_L_ABSOLUTE, false>();
-    if (!pp && fa == MDE_FN_L_QUADRATIC) return kptr<M, MODE, MDE_FN_L_QUADRATIC, MDE_FN_L_QUADRATIC, false>();
-    if (!pp && fa == MDE_FN_L_HUBER) return kptr<M, MODE, MDE_FN_L_HUBER, MDE_FN_L_HUBER, false>();
-  }
-  return kptr<M, MODE, -1, -1, false>();
-}
-
-template <int MODE>
-static const void* select_mode(const FnDev& fn, int m, bool precise) {
-  switch (m) {
-    case 1: return select_m<1, MODE>(fn, precise);
-    case 2: return select_m<2, MODE>(fn, precise);
-    case 3: return select_m<3, MODE>(fn, precise);
-    case 4: return select_m<4, MODE>(fn, precise);
-  }
-  return nullptr;
-}
-
-static const void* select_kernel(const mde_edges* e, int m, int mode) {
-  const bool precise = e->kvar == 2;
-  if (mode == 0) return select_mode<0>(e->fn, m, precise);
-  if (mode == 1) return select_mode<1>(e->fn, m, precise);
-  return select_mode<2>(e->fn, m, precise);
-}
-
-// dynamic shared memory above 48 KB needs an opt-in per kernel; done once per kernel, at layout build for the
-// kernels this layout will launch (never for the first time inside a stream capture)
-static int configure_kernel(const void* k) {
-  static std::vector<const void*> done;
-  if (std::find(done.begin(), done.end(), k) != done.end()) return 0;
-  cudaError_t err = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  if (err != cudaSuccess) return (int)err;
-  done.push_back(k);
-  return 0;
-}
-
-int tiled_configure(const mde_edges* e, int m) {
-  for (int mode = 0; mode < 3; ++mode) {
-    const void* k = select_kernel(e, m, mode);
-    if (!k) return MDE_E_UNSUPPORTED;
-    int rc = configure_kernel(k);
-    if (rc) return rc;
-  }
-  return 0;
-}
-
 int tiled_launch(int mode, const mde_edges* e, const float* X, int m, float* grad, const float* gext,
                  int* nblocks_out, const int* flag, cudaStream_t st) {
-  if (e->kind != 1 || m < 1 || m > 4) return MDE_E_UNSUPPORTED;
+  if (e->kind != kTiles || m < 1 || m > 4) return MDE_E_UNSUPPORTED;
   const size_t smem = tile_smem_bytes(e->rb, m, e->gred);
-  if (smem > 227u * 1024u) return MDE_E_UNSUPPORTED;  // layout built for a smaller embedding dimension
+  if (smem > kMaxDynSmem) return MDE_E_UNSUPPORTED;  // layout built for a smaller embedding dimension
   TileArgs a;
   a.rec = e->rec; a.perm = e->perm; a.gext = gext; a.bkt_tile = e->bkt_tile; a.bkt_wt0 = e->bkt_wt0;
   a.cta_wt0 = e->cta_wt0; a.cta_bkt0 = e->cta_bkt0; a.X = X; a.grad = grad; a.loss_partials = e->loss_partials;
@@ -709,19 +584,11 @@ int tiled_launch(int mode, const mde_edges* e, const float* X, int m, float* gra
   a.x_vec_ok = ((reinterpret_cast<uintptr_t>(X) & 15u) == 0) ? 1 : 0;
   a.g_vec_ok = ((reinterpret_cast<uintptr_t>(grad) & 15u) == 0) ? 1 : 0;
   a.gred = e->gred;
-  const void* k = select_kernel(e, m, mode);
-  if (!k) return MDE_E_UNSUPPORTED;
-  int rc = configure_kernel(k);
-  if (rc) return rc;
-  void* args[] = {(void*)&a};
-  MDE_CUDA_TRY(cudaLaunchKernel(k, dim3(e->ncta), dim3(kTileThreads), args, smem, st));
-  MDE_LAUNCH_CHECK();
-  if (nblocks_out) *nblocks_out = e->ncta;
-  return 0;
+  return launch_persistent(select_kernel(e, m, mode), &a, e->ncta, kTileThreads, smem, nblocks_out, st);
 }
 
 int tiled_edge_outputs(const mde_edges* e, const float* X, int m, float* distances, float* distortions,
-                       cudaStream_t st, const int* flag) {
+                       const int* flag, cudaStream_t st) {
   const int64_t nslots = e->nwt * kWtEdges;
   const int tb = 256;
   tiled_outputs_kernel<<<ceil_div_i64(nslots, tb), tb, 0, st>>>(e->rec, e->perm, nslots, m, X, distances, distortions,

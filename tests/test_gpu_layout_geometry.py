@@ -56,7 +56,7 @@ GEOMETRIES = {
 _SIZES = {"G1": (40_000, 4000), "G2": (20_000, 2000), "G3": (1_000_000, 50_000), "G4a": (40_000, 4000),
           "G4b": (40_000, 4000)}
 
-# functions: every instantiation of the kernel selectors (eselect_m, pselect_m, tiled select_m, SoA QUADK / SMALL)
+# functions: every compile-time function pair of the kernel families (select_fn in mde_edges.cuh and the pair lists)
 FNS = ("pp_fast_mixed", "pp_fast_att", "pp_fast_rep", "pp_precise_mixed", "pp_logratio", "pen_quadratic",
        "loss_absolute", "loss_quadratic", "loss_huber", "pen_cubic", "loss_logistic", "pp_quad_invpower")
 _COINCIDENT_OK = ("pen_quadratic", "loss_absolute", "loss_quadratic", "loss_huber", "pen_cubic", "loss_logistic")
