@@ -357,6 +357,22 @@ int mde_knn_wide(const float* X, int64_t n, int d, int k, int32_t* idx_out, floa
 int mde_knn_csr_wide_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes);
 int mde_knn_csr_wide(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                      int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream);
+/* APPROXIMATE k-nearest neighbours of a dense matrix by NN-descent, for n too large for the exact O(n^2 d) search.
+ * Output contract of mde_knn with "the k nearest rows" replaced by "k rows found by the search": k distinct rows per
+ * row, never the row itself, ascending by (squared distance, index), with the exact fp32 squared distances of the
+ * re-rank of mde_knn / mde_knn_wide (a pair found by both searches carries the same bits).  1 <= k <=
+ * mde_knn_approx_max_k() (64), k <= n - 1.  The result is a function of (X, k, seed) alone: identical bits from run
+ * to run, whatever the workspace held.  When n - 1 <= 32 (k <= 24) or n - 1 <= 96 (k > 24) every row's list holds
+ * every other row and the result is that of the exact search.  `ws`: 1024-byte aligned device scratch of
+ * mde_knn_approx_ws_bytes(n, d, k) bytes (about 1.1 KB per row for k <= 24, 1.9 KB for k > 24).  Return codes of
+ * mde_knn_wide (MDE_E_UNSUPPORTED for n >= 2^31 - 128).  Blocking: one 8-byte read per iteration.
+ * mde_knn_approx_ex also writes the number of NN-descent iterations to *iterations (nullable). */
+int mde_knn_approx_max_k(void);
+int mde_knn_approx_ws_bytes(int64_t n, int d, int k, size_t* bytes);
+int mde_knn_approx(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out, float* d2_out, void* ws,
+                   size_t ws_bytes, void* stream);
+int mde_knn_approx_ex(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out, float* d2_out,
+                      void* ws, size_t ws_bytes, void* stream, int* iterations);
 /* Euclidean distances ||x_a - x_b|| of p row pairs (device int64 pairs[p][2]) of the same CSR, into out[p] (fp32):
  * a sorted merge of the two rows summed in fp64, sqrt in fp64, one rounding (pymde/preprocess/data_matrix.py:59-70
  * takes the norm of the difference in scipy).  MDE_E_INVALID for a malformed CSR or a pair index outside [0, n).

@@ -43,7 +43,7 @@ constexpr int kTileN = 128;                 // candidates per tile = wgmma N
 constexpr int kBlockK = 64;                 // bf16 elements per 128-byte swizzle row
 constexpr int kWgmmaK = 16;                 // K of one wgmma.m64n128k16
 constexpr int kStages = 2;
-constexpr int kKK = 32;                     // candidates kept per row before the exact re-rank
+constexpr int kKK = kNarrowKK;              // candidates kept per row before the exact re-rank (32)
 constexpr int kMaxK = 24;
 constexpr int kRowBytes = kBlockK * 2;      // 128
 constexpr int kOpBytes = 128 * kRowBytes;   // 16 KB: one 128-row operand block (hi or lo)
@@ -259,9 +259,14 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
   }
 }
 
+}  // namespace
+
 // ---------------------------------------------------------------------------------------------------------------
 // re-rank: exact fp32 squared distances of a row's candidates, the k smallest in ascending order
+// (namespace mde, declared in mde_knn_select.cuh: mde_knn_approx.cu re-ranks its lists with the same kernels)
 // ---------------------------------------------------------------------------------------------------------------
+namespace mde {
+
 __global__ void __launch_bounds__(256)
 knn_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
                   int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
@@ -293,6 +298,10 @@ knn_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* 
     out_d2[row * k + rank] = my_d;
   }
 }
+
+}  // namespace mde
+
+namespace {
 
 // ---------------------------------------------------------------------------------------------------------------
 // wide tiles (k <= 64): as knn_tile_kernel for 64 query rows, one running top-96 per row in shared memory
@@ -406,6 +415,10 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
   if (row < n) list.store(cand_idx + (int64_t)row * kWideKK, cand_val + (int64_t)row * kWideKK);
 }
 
+}  // namespace
+
+namespace mde {
+
 // Exact fp32 squared distances of a row's 96 candidates (the arithmetic of knn_rerank_kernel), the k smallest in
 // ascending order; lane q owns candidates q, q + 32 and q + 64, ranks are taken over all 96.
 __global__ void __launch_bounds__(256)
@@ -454,6 +467,10 @@ knn_wide_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int3
     }
   }
 }
+
+}  // namespace mde
+
+namespace {
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,

@@ -1,0 +1,460 @@
+// mde_knn_approx.cu -- approximate k-nearest neighbours of the rows of a dense data matrix by NN-descent (Dong,
+// Moses and Li 2011, in the GPU form of GNND, Wang et al. 2021).  Opt-in next to the exact mde_knn / mde_knn_wide,
+// whose cost grows as n^2 d: NN-descent costs about (iterations x n x 64 staged rows x d).
+//
+// Every row keeps a list of KB (distance, index) entries, KB = 32 for k <= 24 and 96 for k <= 64, as one sorted array
+// of 64-bit keys ((fp32 distance bits << 32) | index; all ones = empty) and one "new" flag per entry.  An iteration is
+//
+//   sample   per row, the S new and S old list entries of lowest hash priority (seed, iteration, row, neighbour); the
+//            sampled new entries become old, and every sample (u -> v) is offered to v's reverse reservoir
+//   join     one CTA per row u: the union of its new and old, forward and reverse samples (<= 64 rows, deduplicated,
+//            new first) is staged in shared memory 64 features at a time; every pair (a, b) with a new member gets
+//            its squared distance on the CUDA cores and is offered to a and b when it beats the worst entry of the
+//            target's list at the start of the iteration and is not in that list already
+//   merge    per row, the list and the offers it received: duplicates dropped, the KB smallest keys kept, entries
+//            that came from offers flagged new; the number of such entries is counted
+//
+// and the host stops when fewer than 0.001 n KB entries changed or after max(5, ceil(log2 n)) iterations.  The final
+// lists go to the re-rank kernels of mde_knn (knn_rerank_kernel for 32 candidates, knn_wide_rerank_kernel for 96),
+// so the output contract and the distance arithmetic are those of the exact search.
+//
+// Determinism.  Offers and reverse samples arrive in a racy order, so they are collected in cascade reservoirs: R
+// 64-bit keys per row, all ones when empty; inserting x runs y = atomicMin(&r[i], x), x = max(x, y) down the slots.
+// Slot i ends up with the i-th smallest key offered (with multiplicity) whatever the interleaving.  Every distance
+// used inside the search is the sequential fp32 sum of fmaf((a_f - b_f)^2) over f = 0 .. d-1, a function of the
+// unordered pair alone, so a pair offered twice carries the same key and duplicates are exact.  Everything the search
+// reads is written by it first: nothing depends on the workspace's earlier contents.
+#include <cuda_runtime.h>
+
+#include <cstdint>
+
+#include "mde_common.cuh"
+#include "mde_knn_select.cuh"
+
+using namespace mde;
+
+namespace {
+
+constexpr int kS = 16;                 // new and old samples per row and direction
+constexpr int kCand = 4 * kS;          // join candidates: forward new, reverse new, forward old, reverse old
+constexpr int kRes = 32;               // offer reservoir slots per row
+constexpr int kNarrowMaxK = 24;        // k <= 24: lists of 32 and knn_rerank_kernel (as mde_knn); else 96
+constexpr int kFC = 64;                // features per staged chunk in the join
+constexpr int kJoinThreads = 128;
+constexpr int kJoinTiles = 100;        // 4 x 4 pair tiles (ta < 8 <= 16 new rows, ta <= tb < 16)
+constexpr int kDeltaInv = 1000;        // stop when fewer than n KB / 1000 entries changed
+constexpr unsigned long long kEmpty = ~0ull;
+static_assert(kRes == 32 && 2 * kS == 32, "the reservoirs of a row are reset by one warp, one slot per lane");
+static_assert(kCand == 64, "the join's pair tiles cover 16 groups of 4 candidates");
+
+__device__ __forceinline__ uint64_t mix64(uint64_t x) {  // splitmix64 finaliser
+  x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
+  x ^= x >> 27; x *= 0x94d049bb133111ebull;
+  return x ^ (x >> 31);
+}
+__device__ __forceinline__ uint64_t hash4(uint64_t seed, uint64_t a, uint64_t b, uint64_t c) {
+  return mix64(mix64(mix64(seed + 0x9e3779b97f4a7c15ull * (a + 1)) ^ b) + c);
+}
+
+// The one distance of the search: sequential fp32 sum over the features (the join's tiles add in the same order).
+__device__ __forceinline__ float seq_dist(const float* __restrict__ a, const float* __restrict__ b, int d) {
+  float acc = 0.0f;
+  for (int f = 0; f < d; ++f) { const float t = a[f] - b[f]; acc = fmaf(t, t, acc); }
+  return acc;
+}
+
+__device__ __forceinline__ unsigned long long make_key(float dist, uint32_t idx) {
+  return ((unsigned long long)__float_as_uint(dist) << 32) | idx;
+}
+
+// Cascade insertion into a reservoir of R ascending slots.  Both shortcuts are exact: a slot only ever decreases, so
+// a read r[i] <= x means the atomic would return <= x and change nothing, and x > r[R-1] (strict: an equal key must
+// still take its slot) means x is not among the R smallest.
+__device__ __forceinline__ void reservoir_insert(unsigned long long* r, int R, unsigned long long x) {
+  if (x > __ldcg(r + R - 1)) return;
+  for (int i = 0; i < R; ++i) {
+    if (__ldcg(r + i) <= x) continue;
+    const unsigned long long y = atomicMin(r + i, x);
+    x = x > y ? x : y;
+    if (x == kEmpty) return;
+  }
+}
+
+// Whether key x is in a row's sorted list.  The lists are not written during the join, so the read is stable, and a
+// pair's key depends on the pair alone, so key equality is index equality.
+template <int KB>
+__device__ __forceinline__ bool in_list(const unsigned long long* __restrict__ l, unsigned long long x) {
+  int lo = 0, hi = KB;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (__ldg(l + mid) < x) lo = mid + 1; else hi = mid; }
+  return lo < KB && __ldg(l + lo) == x;
+}
+
+__device__ __forceinline__ unsigned long long gcd_u64(unsigned long long a, unsigned long long b) {
+  while (b) { const unsigned long long t = a % b; a = b; b = t; }
+  return a;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// init: one warp per row.  The list starts with min(KB, n - 1) distinct rows: all others when n - 1 <= KB, else the
+// rows u + 1 + (a + j b) mod (n - 1) for slots j, with a and b (coprime to n - 1) hashed from (seed, u).  Resets the
+// row's reservoirs.
+// ---------------------------------------------------------------------------------------------------------------
+template <int KB>
+__global__ void __launch_bounds__(256)
+nnd_init_kernel(const float* __restrict__ X, int64_t n, int d, uint64_t seed, unsigned long long* __restrict__ keys,
+                uint8_t* __restrict__ flags, uint32_t* __restrict__ thr, unsigned long long* __restrict__ offers,
+                unsigned long long* __restrict__ rev) {
+  __shared__ unsigned long long s_k[8][KB];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t row = (int64_t)blockIdx.x * 8 + w;
+  if (row >= n) return;
+  const unsigned long long m = (unsigned long long)(n - 1);
+  unsigned long long a = 0, b = 1;
+  if (m > (unsigned long long)KB) {
+    a = hash4(seed, 0, (uint64_t)row, 0) % m;
+    b = 1 + hash4(seed, 1, (uint64_t)row, 0) % (m - 1);
+    while (gcd_u64(b, m) != 1) b = (b + 1 < m) ? b + 1 : 1;
+  }
+  const float* xr = X + row * d;
+#pragma unroll
+  for (int s = 0; s < KB / 32; ++s) {
+    const int j = lane + 32 * s;
+    unsigned long long key = kEmpty;
+    if ((unsigned long long)j < m) {
+      const unsigned long long off = (m > (unsigned long long)KB) ? 1 + (a + (unsigned long long)j * b) % m : 1 + j;
+      const int64_t c = (int64_t)(((unsigned long long)row + off) % (unsigned long long)n);
+      key = make_key(seq_dist(xr, X + c * d, d), (uint32_t)c);
+    }
+    s_k[w][j] = key;
+  }
+  __syncwarp();
+#pragma unroll
+  for (int s = 0; s < KB / 32; ++s) {
+    const int j = lane + 32 * s;
+    const unsigned long long key = s_k[w][j];
+    int rank = 0;  // keys are distinct except the empty ones, which keep their slot order
+    for (int q = 0; q < KB; ++q) {
+      const unsigned long long o = s_k[w][q];
+      rank += (o < key) || (o == key && q < j);
+    }
+    keys[row * KB + rank] = key;
+    flags[row * KB + rank] = key != kEmpty;
+    if (rank == KB - 1) thr[row] = (uint32_t)(key >> 32);
+  }
+  offers[row * kRes + lane] = kEmpty;
+  rev[row * 2 * kS + lane] = kEmpty;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// sample: one warp per row.  fwd[u] = S new then S old list entries (-1 padded) of lowest priority; the sampled new
+// entries are flagged old; each sample u -> v goes to v's reverse reservoir (new: rev[v][0, S), old: [S, 2S)) with
+// the key (priority << 32 | u).
+// ---------------------------------------------------------------------------------------------------------------
+template <int KB>
+__global__ void __launch_bounds__(256)
+nnd_sample_kernel(int64_t n, uint64_t seed, int iter, const unsigned long long* __restrict__ keys,
+                  uint8_t* __restrict__ flags, int32_t* __restrict__ fwd, unsigned long long* __restrict__ rev) {
+  __shared__ unsigned long long s_p[8][KB];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t row = (int64_t)blockIdx.x * 8 + w;
+  if (row >= n) return;
+  constexpr int P = KB / 32;
+  unsigned long long sk[P];
+  int n_new = 0, n_old = 0;
+#pragma unroll
+  for (int s = 0; s < P; ++s) {
+    const int j = lane + 32 * s;
+    const unsigned long long key = keys[row * KB + j];
+    const bool valid = key != kEmpty, is_new = valid && flags[row * KB + j];
+    const uint32_t idx = (uint32_t)key;
+    const uint32_t pr = (uint32_t)(hash4(seed, 2 + (uint64_t)iter, (uint64_t)row, idx) >> 33);  // 31 bits
+    // new entries order before old ones, each by (priority, index)
+    sk[s] = valid ? ((unsigned long long)!is_new << 63) | ((unsigned long long)pr << 32) | idx : kEmpty;
+    s_p[w][j] = sk[s];
+    n_new += __popc(__ballot_sync(kFull, is_new));
+    n_old += __popc(__ballot_sync(kFull, valid && !is_new));
+  }
+  __syncwarp();
+  int32_t* f = fwd + row * 2 * kS;
+#pragma unroll
+  for (int s = 0; s < P; ++s) {
+    if (sk[s] == kEmpty) continue;
+    int rank = 0;
+    for (int q = 0; q < KB; ++q) rank += s_p[w][q] < sk[s];
+    const bool is_new = !(sk[s] >> 63);
+    const int r = is_new ? rank : rank - n_new;
+    if (r >= kS) continue;
+    const uint32_t idx = (uint32_t)sk[s];
+    const unsigned long long rk = (sk[s] & 0x7fffffff00000000ull) | (uint64_t)row;
+    f[(is_new ? 0 : kS) + r] = (int32_t)idx;
+    if (is_new) flags[row * KB + lane + 32 * s] = 0;
+    reservoir_insert(rev + (int64_t)idx * 2 * kS + (is_new ? 0 : kS), kS, rk);
+  }
+  if (lane < kS) {
+    if (lane >= n_new) f[lane] = -1;
+  } else {
+    if (lane - kS >= n_old) f[lane] = -1;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// join: one CTA per row u.  Candidates: forward new, reverse new (slots 0..31 after compaction), forward old, reverse
+// old (slots 32..63), each row once (its first, i.e. newest, occurrence).  Thread t < 100 owns the 4 x 4 pair tile
+// (ta, tb), ta < 8 <= ... tb: every pair with a new member and a < b.  An offer that is already in the target's list
+// is dropped before it can take a reservoir slot: the closest pairs are offered again and again, and would otherwise
+// crowd the genuinely new candidates out of the reservoir.  Resets u's reverse reservoirs.
+// ---------------------------------------------------------------------------------------------------------------
+template <int KB>
+__global__ void __launch_bounds__(kJoinThreads)
+nnd_join_kernel(const float* __restrict__ X, int64_t n, int d, const unsigned long long* __restrict__ keys,
+                const int32_t* __restrict__ fwd, unsigned long long* __restrict__ rev, const uint32_t* __restrict__ thr,
+                unsigned long long* __restrict__ offers) {
+  __shared__ int s_raw[kCand];
+  __shared__ int s_idx[kCand];
+  __shared__ uint32_t s_thr[kCand];
+  __shared__ int s_cnt[2];
+  __shared__ float s_x[kCand][kFC + 1];  // odd row stride: the tiles' column reads hit distinct banks
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int64_t u = blockIdx.x;
+  if (t < kCand) {
+    const int grp = t / kS, q = t % kS;  // 0 fwd new, 1 rev new, 2 fwd old, 3 rev old
+    int c;
+    if (grp == 0 || grp == 2) {
+      c = fwd[u * 2 * kS + (grp == 0 ? 0 : kS) + q];
+    } else {
+      unsigned long long* slot = rev + u * 2 * kS + (grp == 1 ? 0 : kS) + q;
+      const unsigned long long key = *slot;
+      *slot = kEmpty;
+      c = key == kEmpty ? -1 : (int)(uint32_t)key;
+    }
+    s_raw[t] = c;
+  }
+  __syncthreads();
+  if (t < kCand) {  // warps 0 (new) and 1 (old), whole
+    const int c = s_raw[t];
+    bool valid = c >= 0;
+    for (int q = 0; q < t; ++q) valid &= s_raw[q] != c;
+    const unsigned mask = __ballot_sync(kFull, valid);
+    if (valid) {
+      const int p = warp * 32 + __popc(mask & ((1u << lane) - 1));
+      s_idx[p] = c;
+      s_thr[p] = thr[c];
+    }
+    if (lane == 0) s_cnt[warp] = __popc(mask);
+  }
+  __syncthreads();
+  const int nn = s_cnt[0], no = s_cnt[1];
+  if (nn == 0) return;  // nothing new around u
+  auto slot_valid = [&](int r) { return r < 32 ? r < nn : r - 32 < no; };
+  int ta = 0, tb = 0;
+  {
+    int q = t;
+    while (ta < 8 && q >= 16 - ta) { q -= 16 - ta; ++ta; }
+    tb = ta + q;
+  }
+  const bool active = t < kJoinTiles && 4 * ta < nn && slot_valid(4 * tb);
+  float acc[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.0f;
+  for (int f0 = 0; f0 < d; f0 += kFC) {
+    const int fc = min(kFC, d - f0);
+    __syncthreads();  // the previous chunk is consumed
+    for (int e = t; e < kCand * kFC; e += kJoinThreads) {
+      const int r = e / kFC, f = e % kFC;
+      s_x[r][f] = (f < fc && slot_valid(r)) ? __ldg(X + (int64_t)s_idx[r] * d + f0 + f) : 0.0f;
+    }
+    __syncthreads();
+    if (active) {
+#pragma unroll 4
+      for (int f = 0; f < fc; ++f) {
+        float xa[4], xb[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { xa[i] = s_x[4 * ta + i][f]; xb[i] = s_x[4 * tb + i][f]; }
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) { const float df = xa[i] - xb[j]; acc[i][j] = fmaf(df, df, acc[i][j]); }
+      }
+    }
+  }
+  if (!active) return;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int a = 4 * ta + i, b = 4 * tb + j;
+      if ((ta == tb && j <= i) || a >= nn || !slot_valid(b)) continue;
+      const uint32_t db = __float_as_uint(acc[i][j]);
+      const int ia = s_idx[a], ib = s_idx[b];
+      const unsigned long long to_a = ((unsigned long long)db << 32) | (uint32_t)ib;
+      const unsigned long long to_b = ((unsigned long long)db << 32) | (uint32_t)ia;
+      if (db < s_thr[a] && !in_list<KB>(keys + (int64_t)ia * KB, to_a)) reservoir_insert(offers + (int64_t)ia * kRes, kRes, to_a);
+      if (db < s_thr[b] && !in_list<KB>(keys + (int64_t)ib * KB, to_b)) reservoir_insert(offers + (int64_t)ib * kRes, kRes, to_b);
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// merge: one warp per row.  New list = the KB smallest of (list, offers not in the list, each once); entries from
+// offers are flagged new and counted in *changes.  Resets the row's offer reservoir and writes the threshold of the
+// next join (distance bits of the worst entry).
+// ---------------------------------------------------------------------------------------------------------------
+template <int KB>
+__global__ void __launch_bounds__(256)
+nnd_merge_kernel(int64_t n, unsigned long long* __restrict__ keys, uint8_t* __restrict__ flags,
+                 uint32_t* __restrict__ thr, unsigned long long* __restrict__ offers,
+                 unsigned long long* __restrict__ changes) {
+  __shared__ unsigned long long s_l[8][KB];
+  __shared__ unsigned long long s_r[8][kRes];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t row = (int64_t)blockIdx.x * 8 + w;
+  if (row >= n) return;
+  constexpr int P = KB / 32;
+  uint8_t fl[P];
+#pragma unroll
+  for (int s = 0; s < P; ++s) {
+    const int j = lane + 32 * s;
+    s_l[w][j] = keys[row * KB + j];
+    fl[s] = flags[row * KB + j];
+  }
+  const unsigned long long x = offers[row * kRes + lane];
+  offers[row * kRes + lane] = kEmpty;
+  s_r[w][lane] = x;
+  __syncwarp();
+  // lower bound of x in the list
+  int lo = 0, hi = KB;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (s_l[w][mid] < x) lo = mid + 1; else hi = mid; }
+  const bool fresh = x != kEmpty && (lane == 0 || s_r[w][lane - 1] != x) && !(lo < KB && s_l[w][lo] == x);
+  const unsigned vmask = __ballot_sync(kFull, fresh);
+  const int pos_x = lo + __popc(vmask & ((1u << lane) - 1));
+  const bool enters = fresh && pos_x < KB;
+  if (enters) {
+    keys[row * KB + pos_x] = x;
+    flags[row * KB + pos_x] = 1;
+    if (pos_x == KB - 1) thr[row] = (uint32_t)(x >> 32);
+  }
+#pragma unroll
+  for (int s = 0; s < P; ++s) {
+    const int j = lane + 32 * s;
+    const unsigned long long key = s_l[w][j];
+    int before = 0;
+    for (int q = 0; q < kRes; ++q) before += ((vmask >> q) & 1u) && s_r[w][q] < key;
+    const int pos = j + before;
+    if (pos < KB) {
+      keys[row * KB + pos] = key;
+      flags[row * KB + pos] = fl[s];
+      if (pos == KB - 1) thr[row] = (uint32_t)(key >> 32);
+    }
+  }
+  const int changed = __popc(__ballot_sync(kFull, enters));
+  if (lane == 0 && changed) atomicAdd(changes, (unsigned long long)changed);
+}
+
+// list keys -> the candidate indices read by the re-rank kernels (-1 for an empty slot)
+__global__ void __launch_bounds__(256)
+nnd_extract_kernel(int64_t count, const unsigned long long* __restrict__ keys, int32_t* __restrict__ cand) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  const unsigned long long key = keys[i];
+  cand[i] = key == kEmpty ? -1 : (int32_t)(uint32_t)key;
+}
+
+struct ApproxLayout {
+  int kb;
+  size_t off_keys, off_flags, off_thr, off_offers, off_rev, off_fwd, off_cand, off_changes, total;
+};
+
+ApproxLayout approx_layout(int64_t n, int k) {
+  ApproxLayout L;
+  L.kb = k <= kNarrowMaxK ? kNarrowKK : kWideKK;
+  auto up = [](size_t x) { return (x + 1023) / 1024 * 1024; };
+  const size_t nn = (size_t)n;
+  size_t o = 0;
+  L.off_keys = o; o = up(o + nn * L.kb * 8);
+  L.off_flags = o; o = up(o + nn * L.kb);
+  L.off_thr = o; o = up(o + nn * 4);
+  L.off_offers = o; o = up(o + nn * kRes * 8);
+  L.off_rev = o; o = up(o + nn * 2 * kS * 8);
+  L.off_fwd = o; o = up(o + nn * 2 * kS * 4);
+  L.off_cand = o; o = up(o + nn * L.kb * 4);
+  L.off_changes = o; o = up(o + 8);
+  L.total = o;
+  return L;
+}
+
+template <int KB>
+int run_approx(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out, float* d2_out, uint8_t* w,
+               const ApproxLayout& L, cudaStream_t st, int* iterations) {
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(w + L.off_keys);
+  uint8_t* flags = w + L.off_flags;
+  uint32_t* thr = reinterpret_cast<uint32_t*>(w + L.off_thr);
+  unsigned long long* offers = reinterpret_cast<unsigned long long*>(w + L.off_offers);
+  unsigned long long* rev = reinterpret_cast<unsigned long long*>(w + L.off_rev);
+  int32_t* fwd = reinterpret_cast<int32_t*>(w + L.off_fwd);
+  int32_t* cand = reinterpret_cast<int32_t*>(w + L.off_cand);
+  unsigned long long* changes = reinterpret_cast<unsigned long long*>(w + L.off_changes);
+  const unsigned warp_grid = (unsigned)((n + 7) / 8);
+  nnd_init_kernel<KB><<<warp_grid, 256, 0, st>>>(X, n, d, seed, keys, flags, thr, offers, rev);
+  MDE_LAUNCH_CHECK();
+  int max_iter = 5;
+  while ((1ll << max_iter) < n) ++max_iter;  // max(5, ceil(log2 n))
+  int it = 0;
+  if (n - 1 > KB) {  // else every list already holds every other row
+    for (; it < max_iter;) {
+      MDE_CUDA_TRY(cudaMemsetAsync(changes, 0, sizeof(unsigned long long), st));
+      nnd_sample_kernel<KB><<<warp_grid, 256, 0, st>>>(n, seed, it, keys, flags, fwd, rev);
+      MDE_LAUNCH_CHECK();
+      nnd_join_kernel<KB><<<(unsigned)n, kJoinThreads, 0, st>>>(X, n, d, keys, fwd, rev, thr, offers);
+      MDE_LAUNCH_CHECK();
+      nnd_merge_kernel<KB><<<warp_grid, 256, 0, st>>>(n, keys, flags, thr, offers, changes);
+      MDE_LAUNCH_CHECK();
+      unsigned long long changed = 0;
+      MDE_CUDA_TRY(cudaMemcpyAsync(&changed, changes, sizeof(changed), cudaMemcpyDeviceToHost, st));
+      MDE_CUDA_TRY(cudaStreamSynchronize(st));
+      ++it;
+      if (changed * kDeltaInv < (unsigned long long)n * KB) break;
+    }
+  }
+  if (iterations) *iterations = it;
+  const int64_t count = n * KB;
+  nnd_extract_kernel<<<(unsigned)((count + 255) / 256), 256, 0, st>>>(count, keys, cand);
+  MDE_LAUNCH_CHECK();
+  if (KB == kNarrowKK) knn_rerank_kernel<<<warp_grid, 256, 0, st>>>(X, n, d, cand, k, idx_out, d2_out);
+  else knn_wide_rerank_kernel<<<warp_grid, 256, 0, st>>>(X, n, d, cand, k, idx_out, d2_out);
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mde_knn_approx_max_k(void) { return kWideMaxK; }
+
+int mde_knn_approx_ws_bytes(int64_t n, int d, int k, size_t* bytes) {
+  if (!bytes || n < 2 || d < 1 || k < 1 || k > kWideMaxK || k > n - 1) return MDE_E_INVALID;
+  *bytes = approx_layout(n, k).total;
+  return 0;
+}
+
+int mde_knn_approx_ex(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out, float* d2_out,
+                      void* ws, size_t ws_bytes, void* stream, int* iterations) {
+  if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > kWideMaxK || k > n - 1)
+    return MDE_E_INVALID;
+  if (n >= (1ll << 31) - 128) return MDE_E_UNSUPPORTED;
+  const ApproxLayout L = approx_layout(n, k);
+  if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* w = static_cast<uint8_t*>(ws);
+  if (L.kb == kNarrowKK) return run_approx<kNarrowKK>(X, n, d, k, seed, idx_out, d2_out, w, L, st, iterations);
+  return run_approx<kWideKK>(X, n, d, k, seed, idx_out, d2_out, w, L, st, iterations);
+}
+
+int mde_knn_approx(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out, float* d2_out, void* ws,
+                   size_t ws_bytes, void* stream) {
+  return mde_knn_approx_ex(X, n, d, k, seed, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
+}
+
+}  // extern "C"

@@ -8,6 +8,10 @@
 // slots for the new worst, and the two partial worsts meet through one shuffle.  Candidates are ordered by
 // (distance, index); the worst is the largest, so the list after a sweep depends on nothing but the order of the
 // offers, never on timing.
+//
+// It also declares the two dense re-rank kernels (defined in mde_knn.cu).  The approximate search
+// (mde_knn_approx.cu) hands its final lists to them, so a pair found by the exact and the approximate search carries
+// the same fp32 distance bits.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -16,6 +20,7 @@
 
 namespace mde {
 
+constexpr int kNarrowKK = 32;        // candidates per row read by knn_rerank_kernel
 constexpr int kWideKK = 96;          // candidates kept per row before the exact re-rank
 constexpr int kWideMaxK = 64;        // leaves >= 32 spare candidates for the bf16 x 3 error of the cross terms
 constexpr int kWideListStride = 98;  // words per row list: the 32 lanes of a warp (16 rows) hit 32 different banks
@@ -64,5 +69,15 @@ struct WideList {
     }
   }
 };
+
+// Exact fp32 squared distances sum_j (q_j - x_j)^2 (lane-strided fmaf, then a butterfly) of a row's kNarrowKK
+// (knn_rerank_kernel) or kWideKK (knn_wide_rerank_kernel) candidates cand_idx[row][.], -1 for none; the k smallest by
+// (distance, index) go to out_idx / out_d2 [n][k] in ascending order.  One warp per row, 256 threads per block.
+__global__ void __launch_bounds__(256)
+knn_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
+                  int32_t* __restrict__ out_idx, float* __restrict__ out_d2);
+__global__ void __launch_bounds__(256)
+knn_wide_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
+                       int32_t* __restrict__ out_idx, float* __restrict__ out_d2);
 
 }  // namespace mde

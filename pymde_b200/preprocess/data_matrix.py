@@ -4,9 +4,12 @@ k-nearest neighbours are computed EXACTLY on the GPU by the library's own kernel
 cross terms with a running top-32 per row and an exact fp32 re-rank, csrc/mde_knn.cu) for k <= 24, and by their wide
 variants (`mde_knn_wide`: a running top-96 per row in shared memory) for 24 < k <= 64; larger k uses row chunks of a
 library GEMM + top-k.  The reference uses scikit-learn brute force below 10 000 rows and the approximate pynndescent
-above (data_matrix.py:125-143).  A scipy.sparse matrix is searched without densifying it for k <= 64 (`mde_knn_csr`,
-`mde_knn_csr_wide`, csrc/mde_knn_sparse.cu), and its pair distances come from sorted merges of CSR rows
-(`mde_pair_dist_csr`)."""
+above (data_matrix.py:125-143).  `PYMDE_B200_KNN=approx` opts in to an approximate search of dense input for k <= 64
+(`mde_knn_approx`: NN-descent, csrc/mde_knn_approx.cu), whose cost grows about linearly in n; it returns k rows
+found by the search, not necessarily the k nearest.  It pays off for large n at large d: at 10^6 rows and d = 50 the
+exact search is faster (DESIGN section 11.3).  Sparse input keeps the exact searches.  A scipy.sparse matrix is
+searched without densifying it for k <= 64 (`mde_knn_csr`, `mde_knn_csr_wide`, csrc/mde_knn_sparse.cu), and its pair
+distances come from sorted merges of CSR rows (`mde_pair_dist_csr`)."""
 import ctypes as C
 import os
 
@@ -111,11 +114,37 @@ def knn_device(X, k):
     return idx, d2
 
 
+def knn_approx_device(X, k, seed=None):
+    """(indices [n, k] int32, squared distances [n, k] fp32) of k rows found for every row of the CUDA fp32 matrix X
+    by NN-descent, ascending by (distance, index), with the exact fp32 distances of `knn_device`
+    (`mde_knn_approx`, include/mde_b200.h).  `seed` defaults to a draw from the module RNG, so `pymde_b200.seed(s)`
+    reproduces the result."""
+    from .. import _lib
+    lib = _lib.load()
+    if seed is None:
+        seed = int(util.np_rng().integers(0, 2 ** 62))
+    X = X.contiguous()
+    n, d = X.shape
+    need = C.c_size_t(0)
+    _lib.check(lib.mde_knn_approx_ws_bytes(int(n), int(d), int(k), C.byref(need)))
+    ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=X.device)
+    off = (-ws.data_ptr()) % 1024
+    idx = torch.empty((n, k), dtype=torch.int32, device=X.device)
+    d2 = torch.empty((n, k), dtype=torch.float32, device=X.device)
+    with torch.cuda.device(X.device):
+        stream = torch.cuda.current_stream().cuda_stream
+        _lib.check(lib.mde_knn_approx(X.data_ptr(), int(n), int(d), int(k), C.c_uint64(seed), idx.data_ptr(),
+                                      d2.data_ptr(), ws.data_ptr() + off, need.value, stream))
+        torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
+    return idx, d2
+
+
 def k_nearest_neighbors(data, k, max_distance=None, verbose=False, device=None, chunk_rows=None):
     """Graph whose edges join each row to its k nearest rows (Euclidean); reciprocal pairs get weight 2."""
     dev = util.cuda_device(device)
     from .. import _lib
-    use_kernel = chunk_rows is None and os.environ.get("PYMDE_B200_KNN", "kernel") != "gemm"
+    mode = os.environ.get("PYMDE_B200_KNN", "kernel")
+    use_kernel = chunk_rows is None and mode != "gemm"
     if sp.issparse(data):
         n = data.shape[0]
         k = int(min(k, n - 1))
@@ -127,7 +156,8 @@ def k_nearest_neighbors(data, k, max_distance=None, verbose=False, device=None, 
     n = X.shape[0]
     k = int(min(k, n - 1))
     if use_kernel and 1 <= k <= _lib.load().mde_knn_wide_max_k():
-        idx, d2 = knn_device(X, k)
+        # "approx" applies to dense input only: scipy.sparse input keeps the exact sparse searches above
+        idx, d2 = knn_approx_device(X, k) if mode == "approx" else knn_device(X, k)
         return _knn_graph(idx, d2, n, max_distance, dev)
     sq = (X * X).sum(1)
     rows = chunk_rows or max(256, min(n, int(2 ** 27 // max(n, 1))))
