@@ -230,6 +230,13 @@ int mde_solver_run(mde_solver_t* s, int iters, int* iters_done, int* converged, 
  * [3] partials reduced, [4] previous step finished / phase chosen, [5] history update + two-loop done,
  * [6] before the state is written back, [7] first block of the vector kernel that follows.  No reference counterpart. */
 int mde_solver_debug_times(mde_solver_t* s, unsigned long long* out8, void* stream);
+/* Diagnostics: the L-BFGS state of a solve paused between two mde_solver_run calls, copied to host buffers (blocking;
+ * MDE_E_INVALID when the solve is not paused).  g: (n*m) gradient of the last evaluation; g_prev, d: (n*m) gradient
+ * and direction of the last completed iteration; S, Y: (memory_size, n*m) receive the *count stored pairs in logical
+ * order, oldest first; *h_diag, *n_iter: the scaling of the two-loop recursion and the iterations since the last
+ * reset.  Changes no device state.  No reference counterpart. */
+int mde_solver_debug_lbfgs(mde_solver_t* s, float* g, float* g_prev, float* d, float* S, float* Y, int* count,
+                           double* h_diag, int* n_iter, void* stream);
 /* Device pointer to the current iterate (n,m). */
 float* mde_solver_x(mde_solver_t* s);
 /* Copy statistics to host arrays of length >= iterations done (blocking):

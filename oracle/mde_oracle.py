@@ -405,8 +405,12 @@ class SolveStats(object):
 
 
 def embed(X0, edges, spec, constraint, eps=1e-5, max_iter=300, memory_size=10,
-          dtype=np.float32, value_and_grad=None):
+          dtype=np.float32, value_and_grad=None, trace=None):
     """Restatement of MDE.embed -> optim.lbfgs.  Returns (X, SolveStats).
+
+    `trace`, if given, is called after every iteration with a dict of the solver state the device solver's debug
+    view reports at a pause (X, g, g_prev, d, the stored pairs S and Y oldest first, H_diag, n_iter, func_evals);
+    it changes nothing the solve computes.
 
     State kept between iterations mirrors lbfgs.py:581-588.  Note the reference quirk
     (SURVEY section 7.5): the gradient used by iteration k+1 is X.grad as left by the LAST
@@ -503,11 +507,26 @@ def embed(X0, edges, spec, constraint, eps=1e-5, max_iter=300, memory_size=10,
         pc = 100.0 * h * float(dt(np.sqrt((d.astype(np.float64) ** 2).sum()))) / float(norm_X)
         stats.step_size_percents.append(pc)
         stats.step_lengths.append(h)
-        if stats.residual_norms[-1] <= eps:  # :165
-            break
-        elif h == 0:  # :172-173 -> reset, lbfgs.py:378-388
+        stop = stats.residual_norms[-1] <= eps  # :165
+        if not stop and h == 0:  # :172-173 -> reset, lbfgs.py:378-388
             state = {"n_iter": 0}
+        if trace is not None:
+            trace(_trace_point(X, grad, prev_flat_grad, d, state, stats.func_evals))
+        if stop:
+            break
     return X, stats
+
+
+def _trace_point(X, grad, prev_flat_grad, d, state, func_evals):
+    """What the device solver's debug view (mde_solver_debug_lbfgs) reads at a pause, as copies."""
+    held = state["n_iter"] > 0
+    shape = X.shape
+    return {"X": X.copy(), "g": grad.reshape(shape).copy(), "g_prev": prev_flat_grad.reshape(shape).copy(),
+            "d": d.reshape(shape).copy(),
+            "S": [s.reshape(shape).copy() for s in state["old_stps"]] if held else [],
+            "Y": [y.reshape(shape).copy() for y in state["old_dirs"]] if held else [],
+            "H_diag": float(state["H_diag"]) if held else 1.0, "n_iter": state["n_iter"],
+            "func_evals": func_evals}
 
 
 # --------------------------------------------------------------------------------------

@@ -97,6 +97,8 @@ SIGNATURES = {
     "mde_solver_begin_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_void_p]),
     "mde_solver_run": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]),
     "mde_solver_debug_times": (C.c_int, [C.c_void_p, C.POINTER(C.c_ulonglong), C.c_void_p]),
+    "mde_solver_debug_lbfgs": (C.c_int, [C.c_void_p] + [C.c_void_p] * 5 + [C.POINTER(C.c_int), C.POINTER(C.c_double),
+                                                                          C.POINTER(C.c_int), C.c_void_p]),
     "mde_solver_x": (C.c_void_p, [C.c_void_p]),
     "mde_solver_stats": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.POINTER(C.c_int64), C.c_void_p]),

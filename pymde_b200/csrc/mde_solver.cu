@@ -1741,6 +1741,36 @@ int mde_solver_debug_times(mde_solver_t* s, unsigned long long* out8, void* stre
   return 0;
 }
 
+// L-BFGS state of a paused solve, copied as it is (no kernel, no device write): the gradient buffer, g_prev and d of
+// the last completed iteration, the stored pairs in logical order (slot order[j], first n*m floats), H_diag, n_iter.
+// Diagnostics only (tests/test_gpu_lbfgs_replay.py replays the solve from these in fp64).
+int mde_solver_debug_lbfgs(mde_solver_t* s, float* g, float* g_prev, float* d, float* S_out, float* Y_out, int* count,
+                           double* h_diag, int* n_iter, void* stream) {
+  if (!s || !g || !g_prev || !d || !S_out || !Y_out || !count || !h_diag || !n_iter) return MDE_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  int rc = read_status(s, st);
+  if (rc) return rc;
+  if (!s->host_active || !s->status_host[8]) return MDE_E_INVALID;  // only between two runs of a paused solve
+  LbfgsState* lb = new (std::nothrow) LbfgsState();
+  if (!lb) return MDE_E_ALLOC;
+  const size_t vb = sizeof(float) * (size_t)s->N;
+  cudaError_t e = cudaMemcpyAsync(lb, (const char*)s->S + offsetof(SolverState, lb), sizeof(LbfgsState),
+                                  cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(g, s->g, vb, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(g_prev, s->gprev, vb, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d, s->d, vb, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  for (int j = 0; e == cudaSuccess && j < lb->count; ++j) {
+    const int64_t q = lb->order[j];
+    e = cudaMemcpyAsync(S_out + (int64_t)j * s->N, s->Sb + q * s->npad, vb, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(Y_out + (int64_t)j * s->N, s->Yb + q * s->npad, vb, cudaMemcpyDeviceToHost, st);
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  *count = lb->count; *h_diag = lb->H_diag; *n_iter = lb->n_iter;
+  delete lb;
+  return e == cudaSuccess ? 0 : (int)e;
+}
+
 int mde_solver_run(mde_solver_t* s, int iters, int* iters_done, int* converged, void* stream) {
   if (!s) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;

@@ -83,6 +83,7 @@ class DeviceSolver(object):
                     util.stream_ptr(self.device)))
         self.handle = handle
         self.max_iter = opts.max_iter
+        self.memory_size = opts.memory_size
         self._cb = None
         self.peer_memory = False
         if int(world_size) > 1 and exchange is not None:
@@ -191,6 +192,24 @@ class DeviceSolver(object):
             _lib.check(self.lib.mde_solver_stats(self.handle, avg.ctypes.data, res.ctypes.data, pct.ctypes.data,
                                                  stp.ctypes.data, C.byref(fe), util.stream_ptr(self.device)))
         return avg, res, pct, stp, fe.value
+
+    def debug_lbfgs(self):
+        """L-BFGS state of a solve paused between two run() calls (diagnostics): a dict of CPU tensors g, g_prev, d
+        (n, m), S, Y (count, n, m) in logical order, oldest first, and the numbers count, H_diag, n_iter."""
+        nm = self.n * self.m
+        vec = [torch.empty(nm, dtype=torch.float32) for _ in range(3)]
+        S = torch.empty((self.memory_size, nm), dtype=torch.float32)
+        Y = torch.empty_like(S)
+        count, h_diag, n_iter = C.c_int(0), C.c_double(0.0), C.c_int(0)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.mde_solver_debug_lbfgs(self.handle, *[t.data_ptr() for t in vec + [S, Y]],
+                                                       C.byref(count), C.byref(h_diag), C.byref(n_iter),
+                                                       util.stream_ptr(self.device)))
+        shape = (self.n, self.m)
+        c = count.value
+        return {"g": vec[0].view(shape), "g_prev": vec[1].view(shape), "d": vec[2].view(shape),
+                "S": S[:c].view(c, *shape), "Y": Y[:c].view(c, *shape), "count": c, "H_diag": h_diag.value,
+                "n_iter": n_iter.value}
 
 
 class _PtrHolder(object):

@@ -70,18 +70,8 @@ def test_embed_matches_fp32_oracle(golden, key):
 
 
 def _knn_problem(pm, n, k, m, seed, constraint):
-    rng = np.random.default_rng(seed)
-    i = np.repeat(np.arange(n), k)
-    j = (i + rng.integers(1, 50, n * k)) % n
-    att = np.unique(np.sort(np.stack([i, j], 1), axis=1), axis=0)
-    rep = rng.integers(0, n, (len(att), 2))
-    rep = rep[rep[:, 0] != rep[:, 1]]
-    rep = np.unique(np.sort(rep, axis=1), axis=0)
-    # drop repulsive pairs that are also attractive
-    key = lambda e: e[:, 0].astype(np.int64) * n + e[:, 1]
-    rep = rep[~np.isin(key(rep), key(att))]
-    edges = np.concatenate([att, rep]).astype(np.int64)
-    w = np.concatenate([np.ones(len(att)), -np.ones(len(rep))]).astype(np.float32)
+    from tests.lbfgs_replay import knn_graph
+    edges, w = knn_graph(n, k, seed)
     f = pm.penalties.PushAndPull(torch.tensor(w, device="cuda"), pm.penalties.Log1p, pm.penalties.Log)
     return pm.MDE(n, m, torch.tensor(edges, device="cuda"), f, constraint), edges, w
 

@@ -9,6 +9,7 @@ import pytest
 
 from oracle import mde_oracle as O
 from pymde_b200 import _lib
+from tests.lbfgs_replay import explicit_two_loop
 
 LS_DONE = 5
 
@@ -86,22 +87,6 @@ def test_strong_wolfe_state_machine_matches_oracle(kind, seed):
             assert abs(f_c - float(f_ref)) <= 1e-4 * abs(float(f_ref)) + 1e-7 + 4e-5 * slope * abs(t_c)
         checked += 1
     assert checked > 20
-
-
-def explicit_two_loop(g, S, Y, H_diag):
-    """lbfgs.py:488-507 with explicit vectors (float64)."""
-    q = -g.copy()
-    h = len(S)
-    al = [0.0] * h
-    ro = [1.0 / float(Y[i] @ S[i]) for i in range(h)]
-    for i in range(h - 1, -1, -1):
-        al[i] = float(S[i] @ q) * ro[i]
-        q -= al[i] * Y[i]
-    r = q * H_diag
-    for i in range(h):
-        be = float(Y[i] @ r) * ro[i]
-        r += (al[i] - be) * S[i]
-    return r
 
 
 @pytest.mark.parametrize("memory", [1, 3, 10])
