@@ -380,6 +380,24 @@ int mde_knn_approx(const float* X, int64_t n, int d, int k, uint64_t seed, int32
                    size_t ws_bytes, void* stream);
 int mde_knn_approx_ex(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out, float* d2_out,
                       void* ws, size_t ws_bytes, void* stream, int* iterations);
+/* The same NN-descent search on a sparse data matrix, without densifying it.  Input contract of mde_knn_csr (the
+ * device CSR check included: MDE_E_INVALID when malformed); output contract of mde_knn_approx, with the distances of
+ * mde_knn_csr / mde_knn_csr_wide: the exact squared distance summed in fp64 and rounded once to fp32, which is also
+ * the distance the search itself compares, so a pair found by the exact and the approximate sparse search carries the
+ * same bits.  The result is a function of (CSR, k, seed) alone, whatever the workspace held.  When n - 1 <= 32
+ * (k <= 24) or n - 1 <= 96 (k > 24) the result is that of mde_knn_csr / mde_knn_csr_wide, ties included.
+ * 1 <= k <= mde_knn_approx_max_k() (64), k <= n - 1; MDE_E_UNSUPPORTED for n >= 2^31 - 128.  `ws`: 1024-byte aligned
+ * device scratch of mde_knn_approx_csr_ws_bytes(n, d, nnz, k) bytes: about 1.1 KB per row for k <= 24 (1.9 KB for
+ * k > 24), 36 bytes per non-zero and 20 per feature, plus 8 MB (a host-computed bound on the sort's scratch; the call
+ * returns MDE_E_ALLOC should the sort need more).  Blocking: the CSR check and one 8-byte read per iteration.
+ * mde_knn_approx_csr_ex also writes the number of NN-descent iterations to *iterations (nullable). */
+int mde_knn_approx_csr_ws_bytes(int64_t n, int d, int64_t nnz, int k, size_t* bytes);
+int mde_knn_approx_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                       int64_t nnz, int k, uint64_t seed, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
+                       void* stream);
+int mde_knn_approx_csr_ex(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                          int64_t nnz, int k, uint64_t seed, int32_t* idx_out, float* d2_out, void* ws,
+                          size_t ws_bytes, void* stream, int* iterations);
 /* Euclidean distances ||x_a - x_b|| of p row pairs (device int64 pairs[p][2]) of the same CSR, into out[p] (fp32):
  * a sorted merge of the two rows summed in fp64, sqrt in fp64, one rounding (pymde/preprocess/data_matrix.py:59-70
  * takes the norm of the difference in scipy).  MDE_E_INVALID for a malformed CSR or a pair index outside [0, n).

@@ -130,6 +130,12 @@ SIGNATURES = {
                                  C.c_void_p, C.c_size_t, C.c_void_p]),
     "mde_knn_approx_ex": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
+    "mde_knn_approx_csr_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn_approx_csr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int,
+                                     C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn_approx_csr_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int,
+                                        C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                        C.POINTER(C.c_int)]),
     "mde_pair_dist_csr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int64,
                                     C.c_void_p, C.c_void_p]),
     "mde_graph_hops_ws_bytes": (C.c_int64, [C.c_int64]),

@@ -24,11 +24,20 @@
 // used inside the search is the sequential fp32 sum of fmaf((a_f - b_f)^2) over f = 0 .. d-1, a function of the
 // unordered pair alone, so a pair offered twice carries the same key and duplicates are exact.  Everything the search
 // reads is written by it first: nothing depends on the workspace's earlier contents.
+//
+// Sparse rows (mde_knn_approx_csr).  The CSR is validated and re-sorted by prepare_csr (mde_knn_sparse.cu: features
+// by descending document frequency), and every distance of the search is merge_dist2 over those rows: the fp64 sum
+// in column order rounded once to fp32, again a function of the unordered pair alone.  Only init and join depend on
+// the row format (DenseRows, CsrRows); sample, merge, the reservoirs, the stop rule and the driver are shared.  The
+// CSR join stages its candidates' (column, value) slices in shared memory while they fit kCsrStage entries and
+// merges the others from global memory; one thread merges one pair.  The final lists go to knn_csr_rerank_kernel /
+// knn_csr_wide_rerank_kernel, so a pair found by both sparse searches carries the same bits.
 #include <cuda_runtime.h>
 
 #include <cstdint>
 
 #include "mde_common.cuh"
+#include "mde_knn_csr.cuh"
 #include "mde_knn_select.cuh"
 
 using namespace mde;
@@ -43,6 +52,8 @@ constexpr int kFC = 64;                // features per staged chunk in the join
 constexpr int kJoinThreads = 128;
 constexpr int kJoinTiles = 100;        // 4 x 4 pair tiles (ta < 8 <= 16 new rows, ta <= tb < 16)
 constexpr int kDeltaInv = 1000;        // stop when fewer than n KB / 1000 entries changed
+constexpr int kCsrJoinThreads = 256;
+constexpr int kCsrStage = 5632;        // CSR join: staged (column, value) entries per CTA (44 KB)
 constexpr unsigned long long kEmpty = ~0ull;
 static_assert(kRes == 32 && 2 * kS == 32, "the reservoirs of a row are reset by one warp, one slot per lane");
 static_assert(kCand == 64, "the join's pair tiles cover 16 groups of 4 candidates");
@@ -89,6 +100,19 @@ __device__ __forceinline__ bool in_list(const unsigned long long* __restrict__ l
   return lo < KB && __ldg(l + lo) == x;
 }
 
+// The row formats: the one distance of the search between rows a and b.
+struct DenseRows {
+  const float* X;
+  int d;
+  __device__ __forceinline__ float dist(int64_t a, int64_t b) const { return seq_dist(X + a * d, X + b * d, d); }
+};
+struct CsrRows {  // the rows as prepare_csr re-sorts them
+  const int64_t* indptr;
+  const int32_t* cols;
+  const float* vals;
+  __device__ __forceinline__ float dist(int64_t a, int64_t b) const { return (float)merge_dist2(indptr, cols, vals, a, b); }
+};
+
 __device__ __forceinline__ unsigned long long gcd_u64(unsigned long long a, unsigned long long b) {
   while (b) { const unsigned long long t = a % b; a = b; b = t; }
   return a;
@@ -99,9 +123,9 @@ __device__ __forceinline__ unsigned long long gcd_u64(unsigned long long a, unsi
 // rows u + 1 + (a + j b) mod (n - 1) for slots j, with a and b (coprime to n - 1) hashed from (seed, u).  Resets the
 // row's reservoirs.
 // ---------------------------------------------------------------------------------------------------------------
-template <int KB>
+template <int KB, class Rows>
 __global__ void __launch_bounds__(256)
-nnd_init_kernel(const float* __restrict__ X, int64_t n, int d, uint64_t seed, unsigned long long* __restrict__ keys,
+nnd_init_kernel(Rows rows, int64_t n, uint64_t seed, unsigned long long* __restrict__ keys,
                 uint8_t* __restrict__ flags, uint32_t* __restrict__ thr, unsigned long long* __restrict__ offers,
                 unsigned long long* __restrict__ rev) {
   __shared__ unsigned long long s_k[8][KB];
@@ -115,15 +139,14 @@ nnd_init_kernel(const float* __restrict__ X, int64_t n, int d, uint64_t seed, un
     b = 1 + hash4(seed, 1, (uint64_t)row, 0) % (m - 1);
     while (gcd_u64(b, m) != 1) b = (b + 1 < m) ? b + 1 : 1;
   }
-  const float* xr = X + row * d;
-#pragma unroll
+#pragma unroll 1  // one distance at a time: unrolled, the CSR merges spill
   for (int s = 0; s < KB / 32; ++s) {
     const int j = lane + 32 * s;
     unsigned long long key = kEmpty;
     if ((unsigned long long)j < m) {
       const unsigned long long off = (m > (unsigned long long)KB) ? 1 + (a + (unsigned long long)j * b) % m : 1 + j;
       const int64_t c = (int64_t)(((unsigned long long)row + off) % (unsigned long long)n);
-      key = make_key(seq_dist(xr, X + c * d, d), (uint32_t)c);
+      key = make_key(rows.dist(row, c), (uint32_t)c);
     }
     s_k[w][j] = key;
   }
@@ -198,24 +221,14 @@ nnd_sample_kernel(int64_t n, uint64_t seed, int iter, const unsigned long long* 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// join: one CTA per row u.  Candidates: forward new, reverse new (slots 0..31 after compaction), forward old, reverse
-// old (slots 32..63), each row once (its first, i.e. newest, occurrence).  Thread t < 100 owns the 4 x 4 pair tile
-// (ta, tb), ta < 8 <= ... tb: every pair with a new member and a < b.  An offer that is already in the target's list
-// is dropped before it can take a reservoir slot: the closest pairs are offered again and again, and would otherwise
-// crowd the genuinely new candidates out of the reservoir.  Resets u's reverse reservoirs.
+// join, shared by both row formats.  Candidates of row u: forward new, reverse new (slots 0..31 after compaction),
+// forward old, reverse old (slots 32..63), each row once (its first, i.e. newest, occurrence); s_cnt = (new, old)
+// counts.  Resets u's reverse reservoirs.  Called by every thread of the CTA (>= 64 threads).
 // ---------------------------------------------------------------------------------------------------------------
-template <int KB>
-__global__ void __launch_bounds__(kJoinThreads)
-nnd_join_kernel(const float* __restrict__ X, int64_t n, int d, const unsigned long long* __restrict__ keys,
-                const int32_t* __restrict__ fwd, unsigned long long* __restrict__ rev, const uint32_t* __restrict__ thr,
-                unsigned long long* __restrict__ offers) {
-  __shared__ int s_raw[kCand];
-  __shared__ int s_idx[kCand];
-  __shared__ uint32_t s_thr[kCand];
-  __shared__ int s_cnt[2];
-  __shared__ float s_x[kCand][kFC + 1];  // odd row stride: the tiles' column reads hit distinct banks
+__device__ __forceinline__ void join_candidates(int64_t u, const int32_t* __restrict__ fwd,
+                                                unsigned long long* __restrict__ rev, const uint32_t* __restrict__ thr,
+                                                int* s_raw, int* s_idx, uint32_t* s_thr, int* s_cnt) {
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
-  const int64_t u = blockIdx.x;
   if (t < kCand) {
     const int grp = t / kS, q = t % kS;  // 0 fwd new, 1 rev new, 2 fwd old, 3 rev old
     int c;
@@ -243,6 +256,40 @@ nnd_join_kernel(const float* __restrict__ X, int64_t n, int d, const unsigned lo
     if (lane == 0) s_cnt[warp] = __popc(mask);
   }
   __syncthreads();
+}
+
+// The pair (a, b) of candidate slots at distance bits db, offered to both rows: when it beats the worst entry of the
+// target's list at the start of the iteration and is not in that list already.  An offer that is already in the list
+// is dropped before it can take a reservoir slot: the closest pairs are offered again and again, and would otherwise
+// crowd the genuinely new candidates out of the reservoir.
+template <int KB>
+__device__ __forceinline__ void offer_pair(const unsigned long long* __restrict__ keys,
+                                           unsigned long long* __restrict__ offers, const int* s_idx,
+                                           const uint32_t* s_thr, int a, int b, uint32_t db) {
+  const int ia = s_idx[a], ib = s_idx[b];
+  const unsigned long long to_a = ((unsigned long long)db << 32) | (uint32_t)ib;
+  const unsigned long long to_b = ((unsigned long long)db << 32) | (uint32_t)ia;
+  if (db < s_thr[a] && !in_list<KB>(keys + (int64_t)ia * KB, to_a)) reservoir_insert(offers + (int64_t)ia * kRes, kRes, to_a);
+  if (db < s_thr[b] && !in_list<KB>(keys + (int64_t)ib * KB, to_b)) reservoir_insert(offers + (int64_t)ib * kRes, kRes, to_b);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// join of dense rows: one CTA per row u.  The candidates (join_candidates) are staged in shared memory 64 features at
+// a time; thread t < 100 owns the 4 x 4 pair tile (ta, tb), ta < 8 <= ... tb: every pair with a new member and a < b.
+// ---------------------------------------------------------------------------------------------------------------
+template <int KB>
+__global__ void __launch_bounds__(kJoinThreads)
+nnd_join_kernel(const float* __restrict__ X, int64_t n, int d, const unsigned long long* __restrict__ keys,
+                const int32_t* __restrict__ fwd, unsigned long long* __restrict__ rev, const uint32_t* __restrict__ thr,
+                unsigned long long* __restrict__ offers) {
+  __shared__ int s_raw[kCand];
+  __shared__ int s_idx[kCand];
+  __shared__ uint32_t s_thr[kCand];
+  __shared__ int s_cnt[2];
+  __shared__ float s_x[kCand][kFC + 1];  // odd row stride: the tiles' column reads hit distinct banks
+  const int t = threadIdx.x;
+  const int64_t u = blockIdx.x;
+  join_candidates(u, fwd, rev, thr, s_raw, s_idx, s_thr, s_cnt);
   const int nn = s_cnt[0], no = s_cnt[1];
   if (nn == 0) return;  // nothing new around u
   auto slot_valid = [&](int r) { return r < 32 ? r < nn : r - 32 < no; };
@@ -286,13 +333,81 @@ nnd_join_kernel(const float* __restrict__ X, int64_t n, int d, const unsigned lo
     for (int j = 0; j < 4; ++j) {
       const int a = 4 * ta + i, b = 4 * tb + j;
       if ((ta == tb && j <= i) || a >= nn || !slot_valid(b)) continue;
-      const uint32_t db = __float_as_uint(acc[i][j]);
-      const int ia = s_idx[a], ib = s_idx[b];
-      const unsigned long long to_a = ((unsigned long long)db << 32) | (uint32_t)ib;
-      const unsigned long long to_b = ((unsigned long long)db << 32) | (uint32_t)ia;
-      if (db < s_thr[a] && !in_list<KB>(keys + (int64_t)ia * KB, to_a)) reservoir_insert(offers + (int64_t)ia * kRes, kRes, to_a);
-      if (db < s_thr[b] && !in_list<KB>(keys + (int64_t)ib * KB, to_b)) reservoir_insert(offers + (int64_t)ib * kRes, kRes, to_b);
+      offer_pair<KB>(keys, offers, s_idx, s_thr, a, b, __float_as_uint(acc[i][j]));
     }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// join of CSR rows: one CTA per row u, the candidates of join_candidates.  Their (column, value) slices are staged in
+// shared memory in slot order (new rows first) while they fit kCsrStage entries; a row that does not fit is merged
+// from global memory (same values, same sum).  One thread per pair: the nn (nn - 1) / 2 new-new pairs, then the
+// nn x no new-old pairs, each one sequential merge.
+// ---------------------------------------------------------------------------------------------------------------
+template <int KB>
+__global__ void __launch_bounds__(kCsrJoinThreads)
+nnd_csr_join_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
+                    const float* __restrict__ vals, const unsigned long long* __restrict__ keys,
+                    const int32_t* __restrict__ fwd, unsigned long long* __restrict__ rev,
+                    const uint32_t* __restrict__ thr, unsigned long long* __restrict__ offers) {
+  __shared__ int s_raw[kCand];
+  __shared__ int s_idx[kCand];
+  __shared__ uint32_t s_thr[kCand];
+  __shared__ int s_cnt[2];
+  __shared__ int64_t s_beg[kCand];  // the slot's row in cols / vals
+  __shared__ int s_len[kCand];
+  __shared__ int s_off[kCand];      // its offset in s_col / s_val, or -1: read from global memory
+  __shared__ int32_t s_col[kCsrStage];
+  __shared__ float s_val[kCsrStage];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int64_t u = blockIdx.x;
+  join_candidates(u, fwd, rev, thr, s_raw, s_idx, s_thr, s_cnt);
+  const int nn = s_cnt[0], no = s_cnt[1];
+  if (nn == 0) return;  // nothing new around u
+  if (t < kCand) {
+    int64_t b = 0;
+    int len = 0;
+    if (t < 32 ? t < nn : t - 32 < no) { b = indptr[s_idx[t]]; len = (int)(indptr[s_idx[t] + 1] - b); }
+    s_beg[t] = b;
+    s_len[t] = len;
+  }
+  __syncthreads();
+  if (t == 0) {
+    int used = 0;
+    for (int r = 0; r < kCand; ++r) {
+      const int len = s_len[r];
+      s_off[r] = len <= kCsrStage - used ? used : -1;
+      if (s_off[r] >= 0) used += len;
+    }
+  }
+  __syncthreads();
+  for (int r = warp; r < kCand; r += kCsrJoinThreads / 32) {
+    const int off = s_off[r], len = s_len[r];
+    if (off < 0) continue;
+    const int64_t b = s_beg[r];
+    for (int e = lane; e < len; e += 32) { s_col[off + e] = __ldg(cols + b + e); s_val[off + e] = __ldg(vals + b + e); }
+  }
+  __syncthreads();
+  const int p1 = nn * (nn - 1) / 2, total = p1 + nn * no;
+  for (int p = t; p < total; p += kCsrJoinThreads) {
+    int a, b;
+    if (p < p1) {  // p = b (b - 1) / 2 + a, 0 <= a < b < nn
+      b = (int)((1.0f + sqrtf(1.0f + 8.0f * (float)p)) * 0.5f);
+      while (b * (b - 1) / 2 > p) --b;
+      while ((b + 1) * b / 2 <= p) ++b;
+      a = p - b * (b - 1) / 2;
+    } else {
+      const int q = p - p1;
+      a = q / no;
+      b = 32 + q % no;
+    }
+    const int oa = s_off[a], ob = s_off[b];
+    const int32_t* ca = oa >= 0 ? s_col + oa : cols + s_beg[a];
+    const float* va = oa >= 0 ? s_val + oa : vals + s_beg[a];
+    const int32_t* cb = ob >= 0 ? s_col + ob : cols + s_beg[b];
+    const float* vb = ob >= 0 ? s_val + ob : vals + s_beg[b];
+    const float dist = (float)merge_dist2_rows(ca, va, s_len[a], cb, vb, s_len[b]);
+    offer_pair<KB>(keys, offers, s_idx, s_thr, a, b, __float_as_uint(dist));
   }
 }
 
@@ -384,8 +499,62 @@ ApproxLayout approx_layout(int64_t n, int k) {
   return L;
 }
 
+// CSR search: prepare_csr's workspace (without candidate lists), then the lists.  The workspace size is host
+// arithmetic alone, so the sort scratch is reserved as a bound: 16 bytes per item of the larger sort (the alternate
+// key and value buffers take 12, CUB's look-back at most 4) plus 8 MB of histograms; the call checks CUB's exact
+// figure against it.
+struct ApproxCsrLayout {
+  CsrKnnLayout prep;
+  ApproxLayout lists;  // offsets from prep.total
+  size_t total;
+};
+
+ApproxCsrLayout approx_csr_layout(int64_t n, int d, int64_t nnz, int k) {
+  ApproxCsrLayout A;
+  const size_t items = (size_t)(nnz > (int64_t)d ? nnz : (int64_t)d);
+  csr_knn_carve(n, d, nnz, 0, 16 * items + (8u << 20), &A.prep);
+  A.lists = approx_layout(n, k);
+  A.total = A.prep.total + A.lists.total;
+  return A;
+}
+
+// The format-specific launches of the driver.
 template <int KB>
-int run_approx(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out, float* d2_out, uint8_t* w,
+int launch_join(const DenseRows& r, int64_t n, const unsigned long long* keys, const int32_t* fwd,
+                unsigned long long* rev, const uint32_t* thr, unsigned long long* offers, cudaStream_t st) {
+  nnd_join_kernel<KB><<<(unsigned)n, kJoinThreads, 0, st>>>(r.X, n, r.d, keys, fwd, rev, thr, offers);
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+template <int KB>
+int launch_join(const CsrRows& r, int64_t n, const unsigned long long* keys, const int32_t* fwd,
+                unsigned long long* rev, const uint32_t* thr, unsigned long long* offers, cudaStream_t st) {
+  nnd_csr_join_kernel<KB><<<(unsigned)n, kCsrJoinThreads, 0, st>>>(r.indptr, r.cols, r.vals, keys, fwd, rev, thr,
+                                                                    offers);
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+template <int KB>
+int launch_rerank(const DenseRows& r, int64_t n, const int32_t* cand, int k, int32_t* idx_out, float* d2_out,
+                  cudaStream_t st) {
+  const unsigned grid = (unsigned)((n + 7) / 8);
+  if (KB == kNarrowKK) knn_rerank_kernel<<<grid, 256, 0, st>>>(r.X, n, r.d, cand, k, idx_out, d2_out);
+  else knn_wide_rerank_kernel<<<grid, 256, 0, st>>>(r.X, n, r.d, cand, k, idx_out, d2_out);
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+template <int KB>
+int launch_rerank(const CsrRows& r, int64_t n, const int32_t* cand, int k, int32_t* idx_out, float* d2_out,
+                  cudaStream_t st) {
+  const unsigned grid = (unsigned)((n + 7) / 8);
+  if (KB == kNarrowKK) knn_csr_rerank_kernel<<<grid, 256, 0, st>>>(r.indptr, r.cols, r.vals, n, cand, k, idx_out, d2_out);
+  else knn_csr_wide_rerank_kernel<<<grid, 256, 0, st>>>(r.indptr, r.cols, r.vals, n, cand, k, idx_out, d2_out);
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+
+template <int KB, class Rows>
+int run_approx(const Rows& rows, int64_t n, int k, uint64_t seed, int32_t* idx_out, float* d2_out, uint8_t* w,
                const ApproxLayout& L, cudaStream_t st, int* iterations) {
   unsigned long long* keys = reinterpret_cast<unsigned long long*>(w + L.off_keys);
   uint8_t* flags = w + L.off_flags;
@@ -396,7 +565,7 @@ int run_approx(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* 
   int32_t* cand = reinterpret_cast<int32_t*>(w + L.off_cand);
   unsigned long long* changes = reinterpret_cast<unsigned long long*>(w + L.off_changes);
   const unsigned warp_grid = (unsigned)((n + 7) / 8);
-  nnd_init_kernel<KB><<<warp_grid, 256, 0, st>>>(X, n, d, seed, keys, flags, thr, offers, rev);
+  nnd_init_kernel<KB, Rows><<<warp_grid, 256, 0, st>>>(rows, n, seed, keys, flags, thr, offers, rev);
   MDE_LAUNCH_CHECK();
   int max_iter = 5;
   while ((1ll << max_iter) < n) ++max_iter;  // max(5, ceil(log2 n))
@@ -406,8 +575,8 @@ int run_approx(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* 
       MDE_CUDA_TRY(cudaMemsetAsync(changes, 0, sizeof(unsigned long long), st));
       nnd_sample_kernel<KB><<<warp_grid, 256, 0, st>>>(n, seed, it, keys, flags, fwd, rev);
       MDE_LAUNCH_CHECK();
-      nnd_join_kernel<KB><<<(unsigned)n, kJoinThreads, 0, st>>>(X, n, d, keys, fwd, rev, thr, offers);
-      MDE_LAUNCH_CHECK();
+      int rc;
+      if ((rc = launch_join<KB>(rows, n, keys, fwd, rev, thr, offers, st))) return rc;
       nnd_merge_kernel<KB><<<warp_grid, 256, 0, st>>>(n, keys, flags, thr, offers, changes);
       MDE_LAUNCH_CHECK();
       unsigned long long changed = 0;
@@ -421,10 +590,7 @@ int run_approx(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* 
   const int64_t count = n * KB;
   nnd_extract_kernel<<<(unsigned)((count + 255) / 256), 256, 0, st>>>(count, keys, cand);
   MDE_LAUNCH_CHECK();
-  if (KB == kNarrowKK) knn_rerank_kernel<<<warp_grid, 256, 0, st>>>(X, n, d, cand, k, idx_out, d2_out);
-  else knn_wide_rerank_kernel<<<warp_grid, 256, 0, st>>>(X, n, d, cand, k, idx_out, d2_out);
-  MDE_LAUNCH_CHECK();
-  return 0;
+  return launch_rerank<KB>(rows, n, cand, k, idx_out, d2_out, st);
 }
 
 }  // namespace
@@ -448,13 +614,51 @@ int mde_knn_approx_ex(const float* X, int64_t n, int d, int k, uint64_t seed, in
   if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   uint8_t* w = static_cast<uint8_t*>(ws);
-  if (L.kb == kNarrowKK) return run_approx<kNarrowKK>(X, n, d, k, seed, idx_out, d2_out, w, L, st, iterations);
-  return run_approx<kWideKK>(X, n, d, k, seed, idx_out, d2_out, w, L, st, iterations);
+  const DenseRows rows{X, d};
+  if (L.kb == kNarrowKK) return run_approx<kNarrowKK>(rows, n, k, seed, idx_out, d2_out, w, L, st, iterations);
+  return run_approx<kWideKK>(rows, n, k, seed, idx_out, d2_out, w, L, st, iterations);
 }
 
 int mde_knn_approx(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out, float* d2_out, void* ws,
                    size_t ws_bytes, void* stream) {
   return mde_knn_approx_ex(X, n, d, k, seed, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
+}
+
+int mde_knn_approx_csr_ws_bytes(int64_t n, int d, int64_t nnz, int k, size_t* bytes) {
+  if (!bytes || n < 2 || d < 1 || nnz < 0 || k < 1 || k > kWideMaxK || k > n - 1) return MDE_E_INVALID;
+  *bytes = approx_csr_layout(n, d, nnz, k).total;
+  return 0;
+}
+
+int mde_knn_approx_csr_ex(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                          int64_t nnz, int k, uint64_t seed, int32_t* idx_out, float* d2_out, void* ws,
+                          size_t ws_bytes, void* stream, int* iterations) {
+  if (!indptr || !idx_out || !d2_out || !ws || n < 2 || d < 1 || nnz < 0 || k < 1 || k > kWideMaxK || k > n - 1)
+    return MDE_E_INVALID;
+  if (nnz > 0 && (!indices || !values)) return MDE_E_INVALID;
+  if (n >= (1ll << 31) - 128) return MDE_E_UNSUPPORTED;
+  const ApproxCsrLayout A = approx_csr_layout(n, d, nnz, k);
+  if (ws_bytes < A.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
+  size_t sort_bytes = 0;
+  int rc = csr_sort_scratch(n, d, nnz, &sort_bytes);
+  if (rc) return rc;
+  if (sort_bytes > A.prep.tmp_bytes) return MDE_E_ALLOC;
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* w = static_cast<uint8_t*>(ws);
+  if ((rc = prepare_csr(indptr, indices, values, n, d, nnz, A.prep, w, st))) return rc;
+  const CsrRows rows{indptr, reinterpret_cast<const int32_t*>(w + A.prep.off_kin),
+                     reinterpret_cast<const float*>(w + A.prep.off_val)};
+  uint8_t* wl = w + A.prep.total;
+  if (A.lists.kb == kNarrowKK)
+    return run_approx<kNarrowKK>(rows, n, k, seed, idx_out, d2_out, wl, A.lists, st, iterations);
+  return run_approx<kWideKK>(rows, n, k, seed, idx_out, d2_out, wl, A.lists, st, iterations);
+}
+
+int mde_knn_approx_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                       int64_t nnz, int k, uint64_t seed, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
+                       void* stream) {
+  return mde_knn_approx_csr_ex(indptr, indices, values, n, d, nnz, k, seed, idx_out, d2_out, ws, ws_bytes, stream,
+                               nullptr);
 }
 
 }  // extern "C"

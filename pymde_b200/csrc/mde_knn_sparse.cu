@@ -33,6 +33,7 @@
 #include <cstdint>
 
 #include "mde_common.cuh"
+#include "mde_knn_csr.cuh"
 #include "mde_knn_select.cuh"
 #include "mde_tma.cuh"
 #include "mde_wgmma.cuh"
@@ -314,26 +315,13 @@ knn_csr_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __restric
   }
 }
 
+}  // namespace
+
 // ---------------------------------------------------------------------------------------------------------------
-// exact distances: sorted merge of two CSR rows, fp64
+// re-rank: merge_dist2 (mde_knn_csr.cuh) of a row's candidates, the k smallest in ascending order
+// (namespace mde, declared in mde_knn_csr.cuh: mde_knn_approx.cu re-ranks its lists with the same kernels)
 // ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ double merge_dist2(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
-                                              const float* __restrict__ vals, int64_t a, int64_t b) {
-  int64_t p = indptr[a], q = indptr[b];
-  const int64_t pe = indptr[a + 1], qe = indptr[b + 1];
-  double acc = 0.0;
-  while (p < pe && q < qe) {
-    const int cp = cols[p], cq = cols[q];
-    double t;
-    if (cp == cq) { t = (double)vals[p] - (double)vals[q]; ++p; ++q; }
-    else if (cp < cq) { t = vals[p]; ++p; }
-    else { t = vals[q]; ++q; }
-    acc = fma(t, t, acc);
-  }
-  for (; p < pe; ++p) { const double t = vals[p]; acc = fma(t, t, acc); }
-  for (; q < qe; ++q) { const double t = vals[q]; acc = fma(t, t, acc); }
-  return acc;
-}
+namespace mde {
 
 // One warp per row, lane q re-ranks candidate q; the k smallest (distance, index) in ascending order.
 __global__ void __launch_bounds__(256)
@@ -357,6 +345,10 @@ knn_csr_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __restr
     out_d2[row * k + rank] = my_d;
   }
 }
+
+}  // namespace mde
+
+namespace {
 
 // ---------------------------------------------------------------------------------------------------------------
 // wide tiles (k <= 64): as knn_csr_tile_kernel for 64 query rows, one running top-96 per row in shared memory; the
@@ -501,6 +493,10 @@ knn_csr_wide_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __re
   if (scanner && row < n) list.store(cand_idx + row * kWideKK, cand_val + row * kWideKK);
 }
 
+}  // namespace
+
+namespace mde {
+
 // One warp per row, lane q re-ranks candidates q, q + 32 and q + 64 by the merge of knn_csr_rerank_kernel; the k
 // smallest (distance, index) of the 96 in ascending order.
 __global__ void __launch_bounds__(256)
@@ -538,6 +534,10 @@ knn_csr_wide_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __
   }
 }
 
+}  // namespace mde
+
+namespace {
+
 // One thread per pair (the rows of a pair are walked in column order: the same fp64 sum every run).
 __global__ void __launch_bounds__(256)
 pair_dist_csr_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
@@ -556,28 +556,38 @@ int bits_for(uint64_t count) {  // bits needed to hold 0 .. count - 1
   return b;
 }
 
-struct CsrKnnLayout {
-  int64_t n_pad; int num_tiles, nwords, row_bits, col_bits;
-  size_t off_flag, off_norm, off_ci, off_cv, off_cnt, off_cnt_s, off_iota, off_col_s, off_perm, off_bm, off_kin,
-      off_kout, off_val, off_tmp, tmp_bytes, total;
-};
+}  // namespace
 
-// kk: candidates kept per row (kKK, or kWideKK for the wide search)
-int csr_knn_layout(int64_t n, int d, int64_t nnz, CsrKnnLayout* L, int kk = kKK) {
-  L->n_pad = (n + kTileN - 1) / kTileN * kTileN;
-  L->num_tiles = (int)(L->n_pad / kTileN);
-  const int64_t nkb = ((int64_t)d + kBlockK - 1) / kBlockK;
-  L->nwords = (int)((nkb + 31) / 32);
-  L->row_bits = bits_for((uint64_t)n);
-  L->col_bits = bits_for((uint64_t)d);
+namespace mde {
+
+int csr_sort_scratch(int64_t n, int d, int64_t nnz, size_t* bytes) {
   // CUB scratch of the two sorts (a query: no device work)
   size_t t1 = 0, t2 = 0;
   MDE_CUDA_TRY(cub::DeviceRadixSort::SortPairsDescending(nullptr, t1, (const int32_t*)nullptr, (int32_t*)nullptr,
                                                          (const int32_t*)nullptr, (int32_t*)nullptr, d));
   MDE_CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, t2, (const uint64_t*)nullptr, (uint64_t*)nullptr,
                                                (const float*)nullptr, (float*)nullptr, (int64_t)nnz, 0,
-                                               L->row_bits + L->col_bits));
-  L->tmp_bytes = t1 > t2 ? t1 : t2;
+                                               bits_for((uint64_t)n) + bits_for((uint64_t)d)));
+  *bytes = t1 > t2 ? t1 : t2;
+  return 0;
+}
+
+int csr_knn_layout(int64_t n, int d, int64_t nnz, CsrKnnLayout* L, int kk) {
+  size_t tmp = 0;
+  const int rc = csr_sort_scratch(n, d, nnz, &tmp);
+  if (rc) return rc;
+  csr_knn_carve(n, d, nnz, kk, tmp, L);
+  return 0;
+}
+
+void csr_knn_carve(int64_t n, int d, int64_t nnz, int kk, size_t tmp_bytes, CsrKnnLayout* L) {
+  L->n_pad = (n + kTileN - 1) / kTileN * kTileN;
+  L->num_tiles = (int)(L->n_pad / kTileN);
+  const int64_t nkb = ((int64_t)d + kBlockK - 1) / kBlockK;
+  L->nwords = (int)((nkb + 31) / 32);
+  L->row_bits = bits_for((uint64_t)n);
+  L->col_bits = bits_for((uint64_t)d);
+  L->tmp_bytes = tmp_bytes;
   auto up = [](size_t x) { return (x + 1023) / 1024 * 1024; };
   size_t o = 0;
   L->off_flag = o; o = up(o + 4);
@@ -595,8 +605,11 @@ int csr_knn_layout(int64_t n, int d, int64_t nnz, CsrKnnLayout* L, int kk = kKK)
   L->off_val = o; o = up(o + (size_t)nnz * 4);
   L->off_tmp = o; o = up(o + L->tmp_bytes);
   L->total = o;
-  return 0;
 }
+
+}  // namespace mde
+
+namespace {
 
 // Runs csr_check_kernel and reads the verdict back (blocking).
 int check_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
@@ -611,9 +624,10 @@ int check_csr(const int64_t* indptr, const int32_t* indices, const float* values
   return flag ? MDE_E_INVALID : 0;
 }
 
-// The preparation both tile kernels read (workspace carved by csr_knn_layout at w): validates the CSR (blocking
-// status read), writes the norms, the feature permutation, the rows re-sorted under it (cols / vals at off_kin /
-// off_val) and the per-tile occupancy bitmaps.
+}  // namespace
+
+namespace mde {
+
 int prepare_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
                 const CsrKnnLayout& L, uint8_t* w, cudaStream_t st) {
   int* flag = reinterpret_cast<int*>(w + L.off_flag);
@@ -653,7 +667,7 @@ int prepare_csr(const int64_t* indptr, const int32_t* indices, const float* valu
   return 0;
 }
 
-}  // namespace
+}  // namespace mde
 
 extern "C" {
 

@@ -7,9 +7,11 @@ library GEMM + top-k.  The reference uses scikit-learn brute force below 10 000 
 above (data_matrix.py:125-143).  `PYMDE_B200_KNN=approx` opts in to an approximate search of dense input for k <= 64
 (`mde_knn_approx`: NN-descent, csrc/mde_knn_approx.cu), whose cost grows about linearly in n; it returns k rows
 found by the search, not necessarily the k nearest.  It pays off for large n at large d: at 10^6 rows and d = 50 the
-exact search is faster (DESIGN section 11.3).  Sparse input keeps the exact searches.  A scipy.sparse matrix is
-searched without densifying it for k <= 64 (`mde_knn_csr`, `mde_knn_csr_wide`, csrc/mde_knn_sparse.cu), and its pair
-distances come from sorted merges of CSR rows (`mde_pair_dist_csr`)."""
+exact search is faster (DESIGN section 11.3).  `PYMDE_B200_KNN=approx` leaves sparse input on the exact searches.  A
+scipy.sparse matrix is searched without densifying it for k <= 64 (`mde_knn_csr`, `mde_knn_csr_wide`,
+csrc/mde_knn_sparse.cu), and its pair distances come from sorted merges of CSR rows (`mde_pair_dist_csr`).
+`PYMDE_B200_KNN_SPARSE=approx` opts in to NN-descent over the CSR rows for k <= 64 (`mde_knn_approx_csr`,
+csrc/mde_knn_approx.cu), with the distances of the exact sparse search (DESIGN section 11.4)."""
 import ctypes as C
 import os
 
@@ -64,6 +66,34 @@ def knn_sparse_device(csr, shape, k):
         stream = torch.cuda.current_stream().cuda_stream
         _lib.check(search(indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), int(n), int(d), nnz, int(k),
                           idx.data_ptr(), d2.data_ptr(), ws.data_ptr() + off, need.value, stream))
+        torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
+    return idx, d2
+
+
+def knn_approx_sparse_device(csr, shape, k, seed=None):
+    """(indices [n, k] int32, squared distances [n, k] fp32) of k rows found for every row of a device CSR matrix from
+    `_to_device_csr` by NN-descent, ascending by (distance, index), with the distances of `knn_sparse_device`
+    (`mde_knn_approx_csr`, include/mde_b200.h).  `seed` defaults to a draw from the module RNG, so
+    `pymde_b200.seed(s)` reproduces the result."""
+    from .. import _lib
+    lib = _lib.load()
+    if seed is None:
+        seed = int(util.np_rng().integers(0, 2 ** 62))
+    indptr, indices, values = csr
+    n, d = shape
+    nnz = int(indices.shape[0])
+    dev = indptr.device
+    need = C.c_size_t(0)
+    _lib.check(lib.mde_knn_approx_csr_ws_bytes(int(n), int(d), nnz, int(k), C.byref(need)))
+    ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=dev)
+    off = (-ws.data_ptr()) % 1024
+    idx = torch.empty((n, k), dtype=torch.int32, device=dev)
+    d2 = torch.empty((n, k), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream().cuda_stream
+        _lib.check(lib.mde_knn_approx_csr(indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), int(n), int(d),
+                                          nnz, int(k), C.c_uint64(seed), idx.data_ptr(), d2.data_ptr(),
+                                          ws.data_ptr() + off, need.value, stream))
         torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
     return idx, d2
 
@@ -150,7 +180,11 @@ def k_nearest_neighbors(data, k, max_distance=None, verbose=False, device=None, 
         k = int(min(k, n - 1))
         if use_kernel and 1 <= k <= _lib.load().mde_knn_wide_max_k():
             csr, shape = _to_device_csr(data, dev)
-            idx, d2 = knn_sparse_device(csr, shape, k)
+            # PYMDE_B200_KNN=approx does not reach here: sparse input has its own opt-in
+            if os.environ.get("PYMDE_B200_KNN_SPARSE") == "approx":
+                idx, d2 = knn_approx_sparse_device(csr, shape, k)
+            else:
+                idx, d2 = knn_sparse_device(csr, shape, k)
             return _knn_graph(idx, d2, n, max_distance, dev)
     X = _to_device_matrix(data, dev)
     n = X.shape[0]

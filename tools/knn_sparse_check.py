@@ -7,8 +7,13 @@ only; one JSON line per shape, each with the GPU name and power limit read in th
   (b) MNIST-like: 70 000 x 784 clipped Gaussian, ~80 % zeros, stored as CSR, timed against the dense mde_knn
   (c) (a)'s kind with 1e6 rows, run once
 
-Usage: python tools/knn_sparse_check.py [--shapes abc] [--k 15]
+--approx measures the approximate search (mde_knn_approx_csr, NN-descent) instead, on (a) and (c) at every k of
+--k: call time (one run after a warm-up on a small matrix), iterations, peak device memory, recall@k on
+--recall-rows (4 096) sampled rows against the host fp64 brute force, and on (a) the exact mde_knn_csr / mde_knn_csr_wide on the same matrix.
+
+Usage: python tools/knn_sparse_check.py [--shapes abc] [--k 15] [--approx --k 15,50]
 """
+import ctypes as C
 import argparse
 import json
 import os
@@ -21,6 +26,7 @@ import scipy.sparse as sp
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from pymde_b200 import _lib  # noqa: E402
 from pymde_b200.preprocess import data_matrix as dm  # noqa: E402
 
 dev = torch.device("cuda", 0)
@@ -153,14 +159,93 @@ def run_sparse(name, A, k, reps, host_extrapolate, extra=None):
     print(json.dumps(line), flush=True)
 
 
+def approx_call(csr, shape, k, seed=1):
+    """mde_knn_approx_csr_ex: (idx, d2, iterations)."""
+    lib = _lib.load()
+    indptr, indices, values = csr
+    n, d = shape
+    nnz = int(indices.shape[0])
+    need = C.c_size_t(0)
+    _lib.check(lib.mde_knn_approx_csr_ws_bytes(n, d, nnz, k, C.byref(need)))
+    ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=dev)
+    idx = torch.empty((n, k), dtype=torch.int32, device=dev)
+    d2 = torch.empty((n, k), dtype=torch.float32, device=dev)
+    it = C.c_int(0)
+    _lib.check(lib.mde_knn_approx_csr_ex(indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), n, d, nnz, k,
+                                         C.c_uint64(seed), idx.data_ptr(), d2.data_ptr(),
+                                         ws.data_ptr() + (-ws.data_ptr()) % 1024, need.value, None, C.byref(it)))
+    torch.cuda.synchronize()
+    return idx, d2, it.value
+
+
+def recall(idx, ref):
+    return float(np.mean([len(np.intersect1d(a, b)) for a, b in zip(idx, ref)])) / ref.shape[1]
+
+
+def run_approx(name, A, ks, with_exact, n_rows=4096):
+    """One JSON line per k; the host brute force runs once, at the largest k (its first k columns are the k-NN)."""
+    n, d = A.shape
+    csr, shape = dm._to_device_csr(A, dev)
+    rows = np.random.default_rng(1).choice(n, n_rows, replace=False)
+    t0 = time.perf_counter()
+    bi, _ = host_brute(A, rows, max(ks))
+    t_host = time.perf_counter() - t0
+    for k in ks:
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats(dev)
+        base = torch.cuda.memory_allocated(dev)
+        t0 = time.perf_counter()
+        idx, d2, it = approx_call(csr, shape, k)
+        t = time.perf_counter() - t0
+        peak = torch.cuda.max_memory_allocated(dev)
+        got = idx.cpu().numpy()
+        line = {"shape": name, "n": n, "d": d, "nnz": int(A.nnz), "k": k, "approx_s": round(t, 3),
+                "timing": "single run after a warm-up", "iterations": it, "peak_device_bytes": int(peak),
+                "peak_above_input_bytes": int(peak - base), "recall_rows": n_rows,
+                "recall": round(recall(got[rows], bi[:, :k]), 5), "host_brute_s": round(t_host, 1)}
+        if with_exact:
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            ei, ed = dm.knn_sparse_device(csr, shape, k)
+            torch.cuda.synchronize()
+            line["exact_s"] = round(time.perf_counter() - t0, 3)
+            line["exact_kernel"] = "mde_knn_csr" if k <= _lib.load().mde_knn_max_k() else "mde_knn_csr_wide"
+            line["exact_recall"] = round(recall(ei.cpu().numpy()[rows], bi[:, :k]), 5)
+            same = (torch.sort(ei.long(), 1)[0] == torch.sort(idx.long(), 1)[0]).all(1)
+            line["rows_identical_to_exact"] = float(same.float().mean())
+            line["identical_rows_bit_identical_d2"] = bool(torch.equal(d2[same].view(torch.int32),
+                                                                       ed[same].view(torch.int32)))
+            del ei, ed
+        line.update(gpu_identity())
+        print(json.dumps(line), flush=True)
+        del idx, d2
+    del csr
+    torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--shapes", default="abc")
-    ap.add_argument("--k", type=int, default=15)
+    ap.add_argument("--k", default="15", help="one k, or a comma-separated list with --approx")
     ap.add_argument("--rows-c", type=int, default=1_000_000)
     ap.add_argument("--reps-a", type=int, default=3)
+    ap.add_argument("--approx", action="store_true")
+    ap.add_argument("--recall-rows", type=int, default=4096, help="rows sampled for recall (--approx)")
     a = ap.parse_args()
     torch.cuda.init()
+    if a.approx:
+        ks = [int(k) for k in a.k.split(",")]
+        w = text_like(20_000, seed=5)
+        for k in ks:  # warm-up: module loads of both searches
+            cw, sw = dm._to_device_csr(w, dev)
+            approx_call(cw, sw, k)
+            dm.knn_sparse_device(cw, sw, k)
+        if "a" in a.shapes:
+            run_approx("a_text_like", text_like(300_000), ks, True, a.recall_rows)
+        if "c" in a.shapes:
+            run_approx("c_text_like_1e6", text_like(a.rows_c, seed=2), ks, False, a.recall_rows)
+        return
+    a.k = int(a.k)
     if "a" in a.shapes:
         run_sparse("a_text_like", text_like(300_000), a.k, a.reps_a, True)
     if "b" in a.shapes:
