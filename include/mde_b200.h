@@ -404,6 +404,26 @@ int mde_knn_approx_csr_ex(const int64_t* indptr, const int32_t* indices, const f
  * Blocking. */
 int mde_pair_dist_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                       const int64_t* pairs, int64_t p, float* out, void* stream);
+/* Neighbour lists to a weighted undirected edge list (replaces pymde/preprocess/data_matrix.py:172-178 and
+ * graph.py:75-110: Graph.from_edges of the directed pairs, then .edges / .weights).  idx: device int32 [n][k],
+ * row-major, as mde_knn*, mde_knn_approx* and mde_graph_knn write it; -1 means "no entry" and may sit anywhere in a
+ * row.  The output is every unordered pair {i, j} with at least one entry i -> j or j -> i, as int64 rows (i, j) with
+ * i < j sorted by (i, j), with the fp32 weight (number of entries i -> j) + (number of entries j -> i): 1 or 2 for the
+ * searches, and duplicates inside a row are counted too.  Two calls on one workspace: mde_knn_graph_count checks the
+ * entries and counts the pairs (*count); mde_knn_graph_emit then writes edges_out[count][2] and weights_out[count]
+ * from what the count left in `ws` (same n, k and ws; the call is skipped when count is 0).  An entry equal to its
+ * own row or outside [-1, n) gives MDE_E_INVALID (checked on the device).  No atomics order the output: the result
+ * is a function of (idx, n, k) alone, whatever the workspace held, and a row listed by every other row costs no more
+ * than its entries.  1 <= k <= mde_knn_graph_max_k() (64), n >= 1; MDE_E_UNSUPPORTED for n k >= 2^31 - 1.  `ws`:
+ * 1024-byte aligned device scratch of mde_knn_graph_ws_bytes(n, k) bytes (about 25 bytes per entry, plus 16 MB, a
+ * host-computed bound on the sort's scratch; the count returns MDE_E_ALLOC should the sort need more).  The count is
+ * blocking (one 8-byte read); the emit is asynchronous on `stream`. */
+int mde_knn_graph_max_k(void);
+int mde_knn_graph_ws_bytes(int64_t n, int k, size_t* bytes);
+int mde_knn_graph_count(const int32_t* idx, int64_t n, int k, void* ws, size_t ws_bytes, int64_t* count,
+                        void* stream);
+int mde_knn_graph_emit(int64_t n, int k, const void* ws, size_t ws_bytes, int64_t* edges_out, float* weights_out,
+                       void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Problem construction next to the path (SURVEY section 8 row f4).

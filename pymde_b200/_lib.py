@@ -138,7 +138,13 @@ SIGNATURES = {
                                         C.POINTER(C.c_int)]),
     "mde_pair_dist_csr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_int64,
                                     C.c_void_p, C.c_void_p]),
-    "mde_graph_hops_ws_bytes": (C.c_int64, [C.c_int64]),
+    "mde_knn_graph_max_k": (C.c_int, []),
+    "mde_knn_graph_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn_graph_count": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64),
+                                      C.c_void_p]),
+    "mde_knn_graph_emit": (C.c_int, [C.c_int64, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                     C.c_void_p]),
+    "mde_graph_hops_ws_bytes":(C.c_int64, [C.c_int64]),
     "mde_graph_hops": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_double,
                                  C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                  C.c_int64, C.c_void_p]),

@@ -20,7 +20,7 @@ import scipy.sparse as sp
 import torch
 
 from .. import util
-from .graph import Graph
+from .graph import EdgeListGraph, Graph
 from .preprocess import sample_edges  # noqa: F401  (the reference exposes it here as well)
 
 
@@ -169,9 +169,10 @@ def knn_approx_device(X, k, seed=None):
     return idx, d2
 
 
-def k_nearest_neighbors(data, k, max_distance=None, verbose=False, device=None, chunk_rows=None):
-    """Graph whose edges join each row to its k nearest rows (Euclidean); reciprocal pairs get weight 2."""
-    dev = util.cuda_device(device)
+def _search(data, k, dev, chunk_rows=None):
+    """The neighbour search of `k_nearest_neighbors`: (idx [n, k'], squared distances [n, k'] fp32, n) of the
+    k' = min(k, n - 1) nearest rows of every row, from the search kernels (int32 indices), or from row chunks of a
+    library GEMM + top-k (int64 indices) for k' > 64, `chunk_rows` or PYMDE_B200_KNN=gemm."""
     from .. import _lib
     mode = os.environ.get("PYMDE_B200_KNN", "kernel")
     use_kernel = chunk_rows is None and mode != "gemm"
@@ -185,32 +186,49 @@ def k_nearest_neighbors(data, k, max_distance=None, verbose=False, device=None, 
                 idx, d2 = knn_approx_sparse_device(csr, shape, k)
             else:
                 idx, d2 = knn_sparse_device(csr, shape, k)
-            return _knn_graph(idx, d2, n, max_distance, dev)
+            return idx, d2, n
     X = _to_device_matrix(data, dev)
     n = X.shape[0]
     k = int(min(k, n - 1))
     if use_kernel and 1 <= k <= _lib.load().mde_knn_wide_max_k():
         # "approx" applies to dense input only: scipy.sparse input keeps the exact sparse searches above
         idx, d2 = knn_approx_device(X, k) if mode == "approx" else knn_device(X, k)
-        return _knn_graph(idx, d2, n, max_distance, dev)
+        return idx, d2, n
     sq = (X * X).sum(1)
     rows = chunk_rows or max(256, min(n, int(2 ** 27 // max(n, 1))))
-    src, dst = [], []
+    idxs, vals = [], []
     for s0 in range(0, n, rows):
         Q = X[s0:s0 + rows]
         d2 = (sq[s0:s0 + rows, None] + sq[None, :] - 2.0 * (Q @ X.T)).clamp_(min=0)
         d2[torch.arange(Q.shape[0], device=dev), torch.arange(s0, s0 + Q.shape[0], device=dev)] = float("inf")
         val, idx = torch.topk(d2, k, dim=1, largest=False)
-        keep = torch.ones_like(val, dtype=torch.bool) if max_distance is None else val.sqrt() <= max_distance
-        i = torch.arange(s0, s0 + Q.shape[0], device=dev)[:, None].expand_as(idx)
-        src.append(i[keep]); dst.append(idx[keep])
-    e = torch.stack([torch.cat(src), torch.cat(dst)], 1).cpu()
-    return Graph.from_edges(e, None, n_items=n)
+        idxs.append(idx); vals.append(val)
+    return torch.cat(idxs), torch.cat(vals), n
 
 
-def distances(data, retain_fraction=1.0, verbose=False, device=None):
-    """Graph of pairwise Euclidean distances: all (n choose 2) pairs, or a uniform sample of them."""
+def k_nearest_neighbors(data, k, max_distance=None, verbose=False, device=None, chunk_rows=None):
+    """Graph whose edges join each row to its k nearest rows (Euclidean); reciprocal pairs get weight 2."""
     dev = util.cuda_device(device)
+    idx, d2, n = _search(data, k, dev, chunk_rows)
+    return _knn_graph(idx, d2, n, max_distance, dev)
+
+
+def k_nearest_neighbors_device(data, k, max_distance=None, device=None):
+    """The graph of `k_nearest_neighbors` -- same search, same edges and weights -- assembled on the device from the
+    neighbour lists (`graph.knn_edge_list`) and returned as an `EdgeListGraph` there.  The lists of the search
+    kernels and of PYMDE_B200_KNN=gemm qualify when min(k, n - 1) <= 64; larger k raises ValueError (use
+    `k_nearest_neighbors`, which builds the host Graph)."""
+    from .graph import knn_edge_list
+    dev = util.cuda_device(device)
+    idx, d2, n = _search(data, k, dev)
+    if max_distance is not None:
+        idx = torch.where(d2.sqrt() <= max_distance, idx, -1)  # (a NaN distance is dropped, as in _knn_graph)
+    return knn_edge_list(idx, n)
+
+
+def _pair_distances(data, retain_fraction, dev):
+    """(pairs [p, 2] int64 with i < j, Euclidean distances [p] fp32, n) of `distances`, on the device: all pairs in
+    row-major order, or `sample_edges`' sample in its draw order."""
     if sp.issparse(data):
         csr, shape = _to_device_csr(data, dev)
         n = shape[0]
@@ -223,11 +241,28 @@ def distances(data, retain_fraction=1.0, verbose=False, device=None):
     else:
         edges = sample_edges(n, int(retain_fraction * n_all), device=dev)
     if sp.issparse(data):
-        return Graph.from_edges(edges.cpu(), _pair_dist_csr(csr, shape, edges).cpu(), n_items=n)
+        return edges, _pair_dist_csr(csr, shape, edges), n
     out = torch.empty(edges.shape[0], dtype=torch.float32, device=dev)
     step = 1 << 22
     for s0 in range(0, edges.shape[0], step):
         e = edges[s0:s0 + step]
         out[s0:s0 + step] = (X[e[:, 0]] - X[e[:, 1]]).norm(dim=1)
-    g = Graph.from_edges(edges.cpu(), out.cpu(), n_items=n)
-    return g
+    return edges, out, n
+
+
+def distances(data, retain_fraction=1.0, verbose=False, device=None):
+    """Graph of pairwise Euclidean distances: all (n choose 2) pairs, or a uniform sample of them."""
+    dev = util.cuda_device(device)
+    edges, out, n = _pair_distances(data, retain_fraction, dev)
+    return Graph.from_edges(edges.cpu(), out.cpu(), n_items=n)
+
+
+def distances_device(data, retain_fraction=1.0, device=None):
+    """The graph of `distances` -- same pairs, same draws, same distance bits -- as an `EdgeListGraph` on the
+    device: the pairs sorted by (i, j), without the zero and +inf distances that `Graph` drops (NaN is kept)."""
+    dev = util.cuda_device(device)
+    edges, out, n = _pair_distances(data, retain_fraction, dev)
+    order = torch.argsort(edges[:, 0] * n + edges[:, 1])  # (the pairs are distinct: no ties)
+    edges, out = edges[order], out[order]
+    keep = (out != 0) & (out != float("inf"))
+    return EdgeListGraph(edges[keep], out[keep], n)

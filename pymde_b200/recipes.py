@@ -20,15 +20,22 @@ def _remove_anchor_anchor_edges(edges, data, anchors):
     return edges[~both], data[~both]
 
 
+_KNN_GRAPH_MAX_K = 64  # mde_knn_graph_max_k(): longer neighbour lists are assembled into a host Graph
+
+
 def preserve_distances(data, embedding_dim=2, loss=losses.Absolute, constraint=None, max_distances=5e7,
                        device=None, verbose=False):
-    """MDE problem preserving original distances (pymde/recipes.py:103-218)."""
+    """MDE problem preserving original distances (pymde/recipes.py:103-218).  For a data matrix the pair distances
+    are computed and assembled into the edge list on the device (`data_matrix.distances_device`)."""
     if not isinstance(data, (np.ndarray, torch.Tensor, Graph)) and not scipy.sparse.issparse(data):
         raise ValueError("`data` must be a np.ndarray/torch.Tensor/scipy.sparse matrix, or a pymde.Graph.")
     dev = util.cuda_device(device)
     n_items = data.n_items if isinstance(data, Graph) else data.shape[0]
     retain_fraction = max_distances / (n_items * (n_items - 1) / 2)
-    graph = preprocess.distances(data, retain_fraction=retain_fraction, verbose=verbose, device=dev)
+    if isinstance(data, Graph):
+        graph = preprocess.distances(data, retain_fraction=retain_fraction, verbose=verbose, device=dev)
+    else:
+        graph = preprocess.data_matrix.distances_device(data, retain_fraction=retain_fraction, device=dev)
     edges = graph.edges.to(dev)
     deviations = graph.distances.to(dev)
     if constraint is None:
@@ -44,7 +51,9 @@ def preserve_distances(data, embedding_dim=2, loss=losses.Absolute, constraint=N
 def preserve_neighbors(data, embedding_dim=2, attractive_penalty=penalties.Log1p, repulsive_penalty=penalties.Log,
                        constraint=None, n_neighbors=None, repulsive_fraction=None, max_distance=None,
                        init="quadratic", device=None, verbose=False):
-    """MDE problem preserving local structure (pymde/recipes.py:221-448)."""
+    """MDE problem preserving local structure (pymde/recipes.py:221-448).  For a data matrix the neighbour graph is
+    assembled on the device from the search's lists (`data_matrix.k_nearest_neighbors_device`) when
+    min(n_neighbors, n - 1) <= 64; larger n_neighbors keep the chunked GEMM search and the host `Graph`."""
     dev = util.cuda_device(device)
     if isinstance(data, Graph):
         n = data.n_items
@@ -65,7 +74,12 @@ def preserve_neighbors(data, embedding_dim=2, attractive_penalty=penalties.Log1p
     if verbose:
         problem.LOGGER.info("Computing %d-nearest neighbors, with max_distance=%s" % (n_neighbors, max_distance))
 
-    knn = preprocess.k_nearest_neighbors(data, k=n_neighbors, max_distance=max_distance, verbose=verbose, device=dev)
+    if isinstance(data, Graph) or min(n_neighbors, n - 1) > _KNN_GRAPH_MAX_K:
+        knn = preprocess.k_nearest_neighbors(data, k=n_neighbors, max_distance=max_distance, verbose=verbose,
+                                             device=dev)
+    else:
+        knn = preprocess.data_matrix.k_nearest_neighbors_device(data, n_neighbors, max_distance=max_distance,
+                                                                device=dev)
     edges = knn.edges.to(dev)
     weights = knn.weights.to(dev)
     if isinstance(constraint, constraints.Anchored):
