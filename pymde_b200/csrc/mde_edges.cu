@@ -363,9 +363,15 @@ static constexpr int kOwnerThreads = 256;
 static constexpr int kOwnerNodes = kOwnerThreads / kOwnerLanes;  // nodes per block and trip
 static constexpr int kOwnerBatch = 4;  // entries per lane whose loads are issued before the first of them is added
 static constexpr int kOwnerHub = 128;  // longer lists are evaluated by the whole warp (same entries per lane, same order)
+// Resident blocks per SM that the register allocation must allow.  The grid is two waves at 8 blocks per SM
+// (loss_blocks_owner).  The MUFU kernel at m = 2 fits 6 blocks (40 registers) without spilling, where the compiler's
+// own choice of 43 leaves 5; 8 blocks (32 registers) spill and measured slower.  Every other instantiation keeps the
+// compiler's allocation.
+template <int M, bool FAST>
+constexpr int owner_min_blocks() { return (FAST && M == 2) ? 6 : 1; }
 
 template <int M, int MODE, int FA, int FR, bool FAST>
-__global__ void __launch_bounds__(kOwnerThreads)
+__global__ void __launch_bounds__(kOwnerThreads, owner_min_blocks<M, FAST>())
 distortion_owner_kernel(const uint2* __restrict__ ent, const uint32_t* __restrict__ inc,
                         const int64_t* __restrict__ off, const float* __restrict__ par1,
                         const int32_t* __restrict__ perm, const float* __restrict__ gext, int64_t n,
@@ -374,34 +380,37 @@ distortion_owner_kernel(const uint2* __restrict__ ent, const uint32_t* __restric
   static_assert(MODE == 0 || MODE == 2, "value-only evaluations run on the quad kernel");
   if (flag != nullptr && *flag == 0) return;
   const int lane = threadIdx.x & 31, l = lane % kOwnerLanes;
-  const bool need_k = MODE == 2 || par1 != nullptr;  // par1[k] and gext[perm[k]] are indexed by the sorted edge
+  // par1[k] and gext[perm[k]] are indexed by the sorted edge.  Of the compile-time functions only WeightedQuadratic
+  // reads its second parameter, so every other pair compiles the lookup out.
+  constexpr bool kReadsPar1 = FA < 0 || FA == MDE_FN_L_WEIGHTED_QUADRATIC || FR == MDE_FN_L_WEIGHTED_QUADRATIC;
+  const bool need_k = MODE == 2 || (kReadsPar1 && par1 != nullptr);
   double lsum = 0.0;
-  // one entry: record, coefficient a, second parameter b.  Past the end of a list the owner's own row stands in
-  // (masked by the caller), so every address stays valid.  Entry indices fit in int: the layout needs 2 p < 2^31.
-  auto fetch = [&](int j, bool in, int own, uint2& w, float& a, float& b) {
-    w = in ? __ldg(ent + j) : make_uint2((uint32_t)own, 0u);
-    a = __uint_as_float(w.y);
+  // one entry: record w (w.y holds the coefficient a, the caller's in MODE 2) and second parameter b.  Past the end
+  // of a list nothing is loaded.  The records are read once per evaluation: ldg_stream.  Entry indices fit in int:
+  // the layout needs 2 p < 2^31.
+  auto fetch = [&](int j, bool in, uint2& w, float& b) {
+    w = make_uint2(0u, 0u);
     b = 0.0f;
-    if (need_k) {
-      const uint32_t k = in ? (__ldg(inc + j) >> 1) : 0u;
-      if (MODE == 2) a = __ldg(gext + __ldg(perm + k));
-      else b = __ldg(par1 + k);
+    if (in) {
+      w = ldg_stream(ent + j);
+      if (need_k) {
+        const uint32_t k = ldg_stream(inc + j) >> 1;
+        if (MODE == 2) w.y = __float_as_uint(__ldg(gext + __ldg(perm + k)));
+        else b = __ldg(par1 + k);
+      }
     }
   };
-  // the edge's difference is x_src - x_dst at both ends; returns the signed contribution to the owner's row
-  auto contribution = [&](const Row<M>& xo, const Row<M>& xn, uint2 w, float a, float b, bool in, float (&v)[M]) {
-    const bool at_dst = (w.x >> 31) != 0;
-    Row<M> xs, xd;
-#pragma unroll
-    for (int c = 0; c < M; ++c) {
-      xs.v[c] = at_dst ? xn.v[c] : xo.v[c];
-      xd.v[c] = at_dst ? xo.v[c] : xn.v[c];
-    }
+  // the neighbour's row of a fetched entry; past the end of a list no gather is issued (the value is never used)
+  auto gather = [&](uint2 w, bool in, const Row<M>& xo) {
+    return in ? ldg_row<M>(X, (int)(w.x & 0x7fffffffu)) : xo;
+  };
+  // The signed contribution of an entry to the owner's row.  The edge's difference is x_src - x_dst at both ends and
+  // the owner adds +v at the src end, -v at the dst end; rounding is symmetric in sign, so that is g (x_owner -
+  // x_neighbour) at either end, with the same d2, f and g.  The loss counts the edge at its src end.
+  auto contribution = [&](const Row<M>& xo, const Row<M>& xn, uint2 w, float b, bool in, float (&v)[M]) {
     float f;
-    edge_contribution<M, MODE, FA, FR, FAST>(xs, xd, a, b, fn, inv_p, true, f, v);
-    if (MODE != 2 && in && !at_dst) lsum += (double)f;
-#pragma unroll
-    for (int c = 0; c < M; ++c) v[c] = at_dst ? -v[c] : v[c];
+    edge_contribution<M, MODE, FA, FR, FAST>(xo, xn, __uint_as_float(w.y), b, fn, inv_p, true, f, v);
+    if (MODE != 2 && in && (w.x >> 31) == 0) lsum += (double)f;
   };
   // the trip count is uniform across the block: the shuffles and the block sum need every lane
   for (int64_t i0 = (int64_t)blockIdx.x * kOwnerNodes; i0 < n; i0 += (int64_t)gridDim.x * kOwnerNodes) {
@@ -411,24 +420,25 @@ distortion_owner_kernel(const uint2* __restrict__ ent, const uint32_t* __restric
     float acc[M];
 #pragma unroll
     for (int c = 0; c < M; ++c) acc[c] = 0.0f;
-    const int j0 = node ? (int)__ldg(off + i) : 0, j1 = node ? (int)__ldg(off + i + 1) : 0;
-    const bool hub = j1 - j0 > kOwnerHub;
+    const int j0 = node ? (int)ldg_stream(off + i) : 0, cnt = node ? (int)ldg_stream(off + i + 1) - j0 : 0;
+    const bool hub = cnt > kOwnerHub;
     if (node && !hub) {
       const Row<M> xo = ldg_row<M>(X, i);
-      for (int j = j0 + l; j < j1; j += kOwnerLanes * kOwnerBatch) {
+      // lane l holds the entries j, j + 8, ..., of which those below j + left exist
+      for (int j = j0 + l, left = cnt - l; left > 0; j += kOwnerLanes * kOwnerBatch, left -= kOwnerLanes * kOwnerBatch) {
         // the loads of kOwnerBatch entries go out before the first add; the adds keep the list order
         uint2 w[kOwnerBatch];
-        float a[kOwnerBatch], b[kOwnerBatch];
+        float b[kOwnerBatch];
 #pragma unroll
-        for (int u = 0; u < kOwnerBatch; ++u) fetch(j + u * kOwnerLanes, j + u * kOwnerLanes < j1, i, w[u], a[u], b[u]);
+        for (int u = 0; u < kOwnerBatch; ++u) fetch(j + u * kOwnerLanes, u * kOwnerLanes < left, w[u], b[u]);
         Row<M> xn[kOwnerBatch];
 #pragma unroll
-        for (int u = 0; u < kOwnerBatch; ++u) xn[u] = ldg_row<M>(X, (int)(w[u].x & 0x7fffffffu));
+        for (int u = 0; u < kOwnerBatch; ++u) xn[u] = gather(w[u], u * kOwnerLanes < left, xo);
 #pragma unroll
         for (int u = 0; u < kOwnerBatch; ++u) {
-          if (j + u * kOwnerLanes < j1) {
+          if (u * kOwnerLanes < left) {
             float v[M];
-            contribution(xo, xn[u], w[u], a[u], b[u], true, v);
+            contribution(xo, xn[u], w[u], b[u], true, v);
 #pragma unroll
             for (int c = 0; c < M; ++c) acc[c] = __fadd_rn(acc[c], v[c]);
           }
@@ -444,21 +454,21 @@ distortion_owner_kernel(const uint2* __restrict__ ent, const uint32_t* __restric
       const int g0 = __ffs(hubs) - 1;  // lane 0 of the hub's group
       hubs &= hubs - 1;
       const int ih = __shfl_sync(kFull, i, g0);
-      const int h0 = __shfl_sync(kFull, j0, g0), h1 = __shfl_sync(kFull, j1, g0);
+      const int h0 = __shfl_sync(kFull, j0, g0), h1 = h0 + __shfl_sync(kFull, cnt, g0);
       const bool mine = (lane & ~(kOwnerLanes - 1)) == g0;
       const Row<M> xo = ldg_row<M>(X, ih);
       uint2 w0, w1;
-      float a0, b0, a1, b1;
-      fetch(h0 + lane, h0 + lane < h1, ih, w0, a0, b0);
-      fetch(h0 + 32 + lane, h0 + 32 + lane < h1, ih, w1, a1, b1);
-      Row<M> x0 = ldg_row<M>(X, (int)(w0.x & 0x7fffffffu));
+      float b0, b1;
+      fetch(h0 + lane, h0 + lane < h1, w0, b0);
+      fetch(h0 + 32 + lane, h0 + 32 + lane < h1, w1, b1);
+      Row<M> x0 = gather(w0, h0 + lane < h1, xo);
       for (int hb = h0; hb < h1; hb += 32) {
-        const Row<M> x1 = ldg_row<M>(X, (int)(w1.x & 0x7fffffffu));
+        const Row<M> x1 = gather(w1, hb + 32 + lane < h1, xo);
         uint2 w2;
-        float a2, b2;
-        fetch(hb + 64 + lane, hb + 64 + lane < h1, ih, w2, a2, b2);
+        float b2;
+        fetch(hb + 64 + lane, hb + 64 + lane < h1, w2, b2);
         float v[M];
-        contribution(xo, x0, w0, a0, b0, hb + lane < h1, v);
+        contribution(xo, x0, w0, b0, hb + lane < h1, v);
 #pragma unroll
         for (int q = 0; q < 32 / kOwnerLanes; ++q) {
           const int from = l + q * kOwnerLanes;
@@ -468,8 +478,8 @@ distortion_owner_kernel(const uint2* __restrict__ ent, const uint32_t* __restric
             if (mine && hb + from < h1) acc[c] = __fadd_rn(acc[c], t);
           }
         }
-        w0 = w1; a0 = a1; b0 = b1; x0 = x1;
-        w1 = w2; a1 = a2; b1 = b2;
+        w0 = w1; b0 = b1; x0 = x1;
+        w1 = w2; b1 = b2;
       }
     }
 #pragma unroll

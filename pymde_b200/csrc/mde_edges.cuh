@@ -114,6 +114,25 @@ __device__ __forceinline__ Row<M> ldg_row(const float* __restrict__ X, I r) {
   return o;
 }
 
+// A record of a stream that a kernel reads once per launch while it gathers rows of X again and again (the owner
+// kernel's `ent`, `inc`, `inc_off`): ld.global.nc.L1::evict_first, so the stream is the first to leave L1.  No L2
+// hint: the records stay L2-resident from one evaluation to the next.
+__device__ __forceinline__ uint2 ldg_stream(const uint2* __restrict__ p) {
+  uint2 o;
+  asm("ld.global.nc.L1::evict_first.v2.u32 {%0, %1}, [%2];" : "=r"(o.x), "=r"(o.y) : "l"(p));
+  return o;
+}
+__device__ __forceinline__ uint32_t ldg_stream(const uint32_t* __restrict__ p) {
+  uint32_t o;
+  asm("ld.global.nc.L1::evict_first.u32 %0, [%1];" : "=r"(o) : "l"(p));
+  return o;
+}
+__device__ __forceinline__ int64_t ldg_stream(const int64_t* __restrict__ p) {
+  int64_t o;
+  asm("ld.global.nc.L1::evict_first.s64 %0, [%1];" : "=l"(o) : "l"(p));
+  return o;
+}
+
 // row r of a shared-memory tile
 template <int M>
 __device__ __forceinline__ Row<M> lds_row(const float* __restrict__ Xt, int r) {
