@@ -108,10 +108,14 @@ int64_t mde_edges_count(const mde_edges_t* e);
  * value-only / per-edge outputs / external coefficients on the SoA kernels).
  * MDE_B200_LAYOUT=soa|tiles|pull|ell overrides the choice (A/B measurements). */
 int mde_edges_kind(const mde_edges_t* e);
-/* 1 when the layout was created with MDE_B200_DETERMINISTIC=1 (embedding_dim <= 4): gradient contributions are
- * accumulated as 64-bit fixed point (2^-40 resolution), so value AND gradient are bit-reproducible run to run and
- * independent of the scheduling of the reds -- the reference's scatter_add_ is not (pymde/average_distortion.py:75-76).
- * Costs two 64-bit reds per row update instead of one vector red. */
+/* 1 when the layout was created with MDE_B200_DETERMINISTIC=1 and 1 <= embedding_dim <= 512: value AND gradient of
+ * fused and external-coefficient evaluations at that m are bit-reproducible run to run and independent of scheduling
+ * -- the reference's scatter_add_ is not (pymde/average_distortion.py:75-76).
+ *   m <= 4: gradient contributions are accumulated as 64-bit fixed point (2^-40 resolution); two 64-bit reds per row
+ *           update instead of one vector red.
+ *   5 <= m <= 512: owner-complete rows -- every node's directed entries are evaluated by one group of lanes in a fixed
+ *           order and its row is written once, with no atomics (lists longer than 256 entries in segments added in
+ *           order); two row gathers per edge instead of one plus a row of reds. */
 int mde_edges_deterministic(const mde_edges_t* e);
 /* bytes of device memory held by the layout */
 int64_t mde_edges_nbytes(const mde_edges_t* e);

@@ -21,6 +21,8 @@
 //            vector reds (REDG.E.ADD.F32x2/x4).
 //   m >= 5 : a group of G lanes (8/16/32) walks a contiguous slice of edges; the lhs row and
 //            its gradient accumulator stay in registers across a run.
+//   5 <= m <= 512, MDE_B200_DETERMINISTIC (fused and external coefficients): distortion_wide_owner_kernel, one group
+//            of G lanes per owner over its directed entries `ent`, one write per row, no atomics.
 #include <cub/cub.cuh>
 #include <algorithm>
 #include <cstdlib>
@@ -625,6 +627,162 @@ distortion_wide_kernel(const int32_t* __restrict__ src, const int32_t* __restric
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// 5 <= m <= 512, deterministic mode (MODE 0 and 2): owner-complete evaluation of the directed entries `ent`, with the
+// group shape of the wide kernel.  A group of G lanes walks one owner's list in order; lane l holds columns l, l + G,
+// ... of the owner row and of its gradient sum in registers.  Per entry it gathers the neighbour row, forms x_owner -
+// x_neighbour, combines the squared distance over the group with a fixed xor tree and adds g (x_owner - x_neighbour).
+// The lane-to-column partition and the tree are the same at both ends of an edge, and rounding is symmetric in sign,
+// so both ends compute the same d, f and g.  No atomics: a row is written once, the gradient is the same bits in
+// every run.  The loss counts each edge at its src-end entry, in fp64.
+// Lists longer than kWideSeg entries are cut into segments of kWideSeg (the layout's `wseg` table).  The segments are
+// work items of their own, evaluated in parallel into the scratch rows `wpart`; wide_owner_combine_kernel then adds
+// each such node's segment rows in segment order to its gradient row.
+// ------------------------------------------------------------------------------------------
+static constexpr int kWideSeg = 256;
+
+// entries per batch whose loads are issued before the first of them is added: 8 at one float of the row per lane, 4
+// at 4 floats, else 2.  What stays live across the out-of-line call of the run-time function table must fit the
+// registers the call preserves: at 2 floats per lane, 4 or 8 entries spill.
+template <int CPL, int VW>
+__host__ __device__ constexpr int wide_owner_batch() { return CPL * VW == 1 ? 8 : (CPL * VW == 4 ? 4 : 2); }
+
+template <int G, int CPL, int VW, int MODE>
+__global__ void __launch_bounds__(kWideThreads)
+distortion_wide_owner_kernel(const uint2* __restrict__ ent, const uint32_t* __restrict__ inc,
+                             const int64_t* __restrict__ off, const int4* __restrict__ seg, int nseg,
+                             float* __restrict__ part, const float* __restrict__ par1,
+                             const int32_t* __restrict__ perm, const float* __restrict__ gext, int64_t n, int m,
+                             const float* __restrict__ X, float* __restrict__ grad,
+                             double* __restrict__ loss_partials, FnDev fn, float inv_p,
+                             const int* __restrict__ flag) {
+  static_assert(MODE == 0 || MODE == 2, "value-only evaluations run on the wide kernel");
+  constexpr int B = wide_owner_batch<CPL, VW>();
+  if (flag != nullptr && *flag == 0) return;
+  const int lg = threadIdx.x % G;
+  // shuffles stay inside the G-lane group: groups of one warp walk lists of different lengths
+  const unsigned gmask = (G == 32) ? kFull : (((1u << G) - 1u) << ((threadIdx.x & 31) & ~(G - 1)));
+  const int64_t group0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) / G;
+  const int64_t ngroups = ((int64_t)gridDim.x * blockDim.x) / G;
+  const int mv = m / VW;  // columns in units of VW floats
+  const bool need_k = MODE == 2 || par1 != nullptr;
+  double lsum = 0.0;
+  // work items: the nseg segments of the long lists first (the largest items), then the n owners
+  for (int64_t item = group0; item < nseg + n; item += ngroups) {
+    int owner, jb, je;
+    float* out;
+    if (item < nseg) {
+      const int4 s = __ldg(seg + item);
+      owner = s.x; jb = s.y; je = s.z;
+      out = part + item * m;
+    } else {
+      owner = (int)(item - nseg);
+      jb = (int)ldg_stream(off + owner);
+      je = (int)ldg_stream(off + owner + 1);
+      if (je - jb > kWideSeg) continue;  // evaluated by its segments
+      out = grad + (int64_t)owner * m;
+    }
+    Vec<VW> xo[CPL], acc[CPL];
+#pragma unroll
+    for (int c = 0; c < CPL; ++c) {
+      const int col = lg + c * G;
+      xo[c] = ldv<VW>(X + (int64_t)owner * m + (col < mv ? col : mv - 1) * VW);
+#pragma unroll
+      for (int q = 0; q < VW; ++q) acc[c].v[q] = 0.0f;
+    }
+    // the trip count and every branch below are uniform across the group (same list)
+    for (int j = jb; j < je; j += B) {
+      uint2 w[B];
+      float a[B], b[B];
+#pragma unroll
+      for (int u = 0; u < B; ++u) {
+        w[u] = make_uint2(0u, 0u);
+        b[u] = 1.0f;  // as the wide kernel: only WeightedQuadratic reads b, and it always has par1
+        if (j + u < je) {
+          w[u] = ldg_stream(ent + j + u);
+          if (need_k) {
+            const uint32_t k = ldg_stream(inc + j + u) >> 1;
+            if (MODE == 2) w[u].y = __float_as_uint(__ldg(gext + __ldg(perm + k)));
+            else b[u] = __ldg(par1 + k);
+          }
+        }
+        a[u] = __uint_as_float(w[u].y);
+      }
+      Vec<VW> xn[B][CPL];
+#pragma unroll
+      for (int u = 0; u < B; ++u) {
+        const int64_t r = (int64_t)(w[u].x & 0x7fffffffu) * m;
+#pragma unroll
+        for (int c = 0; c < CPL; ++c) {
+          const int col = lg + c * G;
+          xn[u][c] = (j + u < je) ? ldv<VW>(X + r + (col < mv ? col : mv - 1) * VW) : xo[c];
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < B; ++u) {
+        if (j + u < je) {
+          Vec<VW> diff[CPL];
+          float d2 = 0.0f;
+#pragma unroll
+          for (int c = 0; c < CPL; ++c) {
+            const float keep = (lg + c * G < mv) ? 1.0f : 0.0f;
+#pragma unroll
+            for (int q = 0; q < VW; ++q) {
+              diff[c].v[q] = (xo[c].v[q] - xn[u][c].v[q]) * keep;
+              d2 += diff[c].v[q] * diff[c].v[q];
+            }
+          }
+#pragma unroll
+          for (int o = G / 2; o > 0; o >>= 1) d2 += __shfl_xor_sync(gmask, d2, o);
+          float g;
+          if (MODE == 2) {
+            g = a[u];
+          } else {
+            float f;
+            edge_coeff<-1, -1>(fn, sqrtf(d2), a[u], b[u], inv_p, f, g);
+            if (lg == 0 && (w[u].x >> 31) == 0) lsum += (double)f;
+          }
+#pragma unroll
+          for (int c = 0; c < CPL; ++c)
+#pragma unroll
+            for (int q = 0; q < VW; ++q) acc[c].v[q] = __fadd_rn(acc[c].v[q], __fmul_rn(g, diff[c].v[q]));
+        }
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < CPL; ++c) {
+      const int col = lg + c * G;
+      if (col < mv) {
+#pragma unroll
+        for (int q = 0; q < VW; ++q) {
+          if (item < nseg) out[col * VW + q] = acc[c].v[q];
+          else out[col * VW + q] += acc[c].v[q];
+        }
+      }
+    }
+  }
+  if (MODE != 2) {
+    __shared__ double sm[32];
+    double v1[1] = {lsum};
+    block_sum<1>(v1, sm);
+    if (threadIdx.x == 0) loss_partials[blockIdx.x] = v1[0];
+  }
+}
+
+// the nodes whose lists were cut into segments: grad[node] += the segment rows in segment order, one thread per
+// (node, column).  whub[h] = (node, first segment, end segment).
+__global__ void wide_owner_combine_kernel(const int4* __restrict__ whub, int nhub, const float* __restrict__ part,
+                                          int m, float* __restrict__ grad, const int* __restrict__ flag) {
+  if (flag != nullptr && *flag == 0) return;
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (int64_t)nhub * m) return;
+  const int h = (int)(t / m), c = (int)(t % m);
+  const int4 hb = __ldg(whub + h);
+  float s = __ldg(part + (int64_t)hb.y * m + c);
+  for (int q = hb.y + 1; q < hb.z; ++q) s = __fadd_rn(s, __ldg(part + (int64_t)q * m + c));
+  grad[(int64_t)hb.x * m + c] += s;
+}
+
 // sum of per-block partials, added to *out (single block; fixed order => deterministic)
 __global__ void add_partials_kernel(const double* __restrict__ partials, int nblocks, double* out) {
   __shared__ double sm[32];
@@ -804,9 +962,39 @@ int launch_small(const SoaLaunch& l) {
   });
 }
 
+// the wide owner kernel's grid depends on its work items alone (segments + owners)
+int loss_blocks_wide_owner(int64_t items, int G) {
+  const int64_t groups_per_block = kWideThreads / G;
+  int64_t nb = (items + groups_per_block - 1) / groups_per_block;
+  if (nb < 1) nb = 1;
+  if (nb > kMaxLossBlocks) nb = kMaxLossBlocks;
+  return (int)nb;
+}
+
+// deterministic mode at the layout's m >= 5: the owner-complete kernel, then (when some list was cut into segments)
+// the kernel that adds the segment rows; both honour the step gate
+template <int G, int CPL, int VW, int MODE>
+int launch_wide_owner(const SoaLaunch& l) {
+  const mde_edges* e = l.e;
+  const int nb = loss_blocks_wide_owner(e->n + e->nwseg, G);
+  distortion_wide_owner_kernel<G, CPL, VW, MODE><<<nb, kWideThreads, 0, l.st>>>(
+      e->ent, e->inc, e->inc_off, e->wseg, e->nwseg, e->wpart, l.par1(), e->perm, l.gext, e->n, l.m, l.X, l.grad,
+      e->loss_partials, e->fn, l.inv_p, l.flag);
+  if (e->nwhub > 0) {
+    ++g_launch_count;
+    const int64_t t = (int64_t)e->nwhub * l.m;
+    wide_owner_combine_kernel<<<ceil_div_i64(t, 256), 256, 0, l.st>>>(e->whub, e->nwhub, e->wpart, l.m, l.grad, l.flag);
+  }
+  return nb;
+}
+
 template <int G, int CPL, int VW, int MODE>
 int launch_wide(const SoaLaunch& l) {
   const mde_edges* e = l.e;
+  // the owner kernel is instantiated for the deterministic range m <= 512 (at most 16 floats of a row per lane)
+  if constexpr (MODE != 1 && CPL * VW <= 16) {
+    if (e->det && e->ent && l.m == e->m_hint) return launch_wide_owner<G, CPL, VW, MODE>(l);
+  }
   const int nb = loss_blocks_wide(e->p, G);
   distortion_wide_kernel<G, CPL, VW, MODE><<<nb, kWideThreads, 0, l.st>>>(
       e->src, e->dst, e->par0, l.par1(), e->perm, l.gext, e->p, l.m, l.X, l.grad, e->loss_partials, e->fn, l.inv_p,
@@ -818,8 +1006,10 @@ template <int MODE>
 int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, const float* gext,
                       int* nblocks_out, const int* flag, cudaStream_t st) {
   SoaLaunch l{e, X, m, grad, gext, flag, st, 1.0f / (float)e->p_total, nullptr, false};
-  // deterministic mode (m <= 4, sorted-SoA layout): zero the fixed-point buffer, accumulate into it, add it to grad
-  if (e->det && MODE != 1 && m <= 4 && m <= e->m_hint && e->kvar != 1) {
+  // deterministic mode (m <= 4, sorted-SoA layout): zero the fixed-point buffer, accumulate into it, add it to grad.
+  // A deterministic layout built for m >= 5 has no fixed-point buffer: it evaluates its own m on the wide owner kernel
+  // (launch_wide).
+  if (e->det && e->fx && MODE != 1 && m <= 4 && m <= e->m_hint && e->kvar != 1) {
     l.fx = e->fx;
     const int64_t cnt = e->n * m;
     int zb = (int)((cnt + 255) / 256); if (zb > kNumSMs * 8) zb = kNumSMs * 8;
@@ -989,11 +1179,15 @@ int mde_edges_create_ex(mde_edges_t** out, const int64_t* edges, int64_t p, int6
   // the sorted-SoA quad kernel needs half the layout memory and no more requests per edge.
   dense = (p / n_items) >= 64;
   pref = layout_pref();
-  {  // MDE_B200_DETERMINISTIC=1: order-independent (fixed-point) gradient accumulation; sorted-SoA layout, m <= 4
+  {  // MDE_B200_DETERMINISTIC=1, sorted-SoA layout: order-independent (fixed-point) gradient accumulation for m <= 4,
+     // owner-complete rows over the directed entries (built below) for 5 <= m <= 512
     const char* ev = getenv("MDE_B200_DETERMINISTIC");
     if (ev && ev[0] == '1' && embedding_dim >= 1 && embedding_dim <= 4) {
       e->det = 1; e->m_hint = embedding_dim; pref = 1;
       TRY(cudaMalloc(&e->fx, sizeof(long long) * n_items * embedding_dim));
+    }
+    if (ev && ev[0] == '1' && embedding_dim >= 5 && embedding_dim <= 512 && 2 * p < (1ll << 31)) {
+      e->det = 1; e->m_hint = embedding_dim; pref = 1;
     }
   }
   // dense graphs: ELL pull records next to the sorted-SoA arrays (fewer instructions per entry than the flat pull
@@ -1041,9 +1235,10 @@ int mde_edges_create_ex(mde_edges_t** out, const int64_t* edges, int64_t p, int6
   }
   cudaFree(keys_in); cudaFree(keys_out); cudaFree(vals_in); cudaFree(vals_out); cudaFree(tmp);
   keys_in = keys_out = nullptr; vals_in = vals_out = nullptr; tmp = nullptr;
-  if (!e->det && !want_ell && embedding_dim >= 1 && embedding_dim <= 4 && 2 * p < (1ll << 31)) {
+  if (((!e->det && embedding_dim >= 1 && embedding_dim <= 4) || (e->det && embedding_dim >= 5)) && !want_ell &&
+      2 * p < (1ll << 31)) {
     // incidence lists of the sorted edges: a stable radix sort by node keeps each node's entries in the order
-    // (src entries by k, then dst entries by k), so the owner kernel adds in the same order in every run
+    // (src entries by k, then dst entries by k), so the owner kernels add in the same order in every run
     uint32_t *ik = nullptr, *ik2 = nullptr, *iv = nullptr;
     int* cnt = nullptr;
     const int64_t q = 2 * p;
@@ -1075,6 +1270,30 @@ int mde_edges_create_ex(mde_edges_t** out, const int64_t* edges, int64_t p, int6
     tmp = nullptr;
     e->m_hint = embedding_dim;
     e->nbytes += q * 8 + q * 4 + (n_items + 1) * 8;
+    if (e->det) {
+      // the wide owner kernel's segments: every list longer than kWideSeg entries is cut into pieces of kWideSeg,
+      // in list order; whub[h] = (node, first segment, end segment), wseg[s] = (node, first entry, end entry)
+      std::vector<int64_t> off(n_items + 1);
+      TRY(cudaMemcpy(off.data(), e->inc_off, sizeof(int64_t) * (n_items + 1), cudaMemcpyDeviceToHost));
+      std::vector<int4> segs, hubs;
+      for (int64_t i = 0; i < n_items; ++i) {
+        if (off[i + 1] - off[i] <= kWideSeg) continue;
+        hubs.push_back(make_int4((int)i, (int)segs.size(), 0, 0));
+        for (int64_t j = off[i]; j < off[i + 1]; j += kWideSeg)
+          segs.push_back(make_int4((int)i, (int)j, (int)std::min<int64_t>(j + kWideSeg, off[i + 1]), 0));
+        hubs.back().z = (int)segs.size();
+      }
+      e->nwseg = (int)segs.size();
+      e->nwhub = (int)hubs.size();
+      if (e->nwhub > 0) {
+        TRY(cudaMalloc(&e->wseg, sizeof(int4) * segs.size()));
+        TRY(cudaMalloc(&e->whub, sizeof(int4) * hubs.size()));
+        TRY(cudaMalloc(&e->wpart, sizeof(float) * segs.size() * embedding_dim));
+        TRY(cudaMemcpy(e->wseg, segs.data(), sizeof(int4) * segs.size(), cudaMemcpyHostToDevice));
+        TRY(cudaMemcpy(e->whub, hubs.data(), sizeof(int4) * hubs.size(), cudaMemcpyHostToDevice));
+        e->nbytes += (int64_t)(segs.size() + hubs.size()) * 16 + (int64_t)segs.size() * embedding_dim * 4;
+      }
+    }
   }
   if (want_ell) {
     // ELL pull records next to the sorted-SoA arrays (kind 3); MDE_E_UNSUPPORTED leaves the layout at kind 0
@@ -1099,6 +1318,7 @@ int mde_edges_destroy(mde_edges_t* e) {
   if (!e) return 0;
   cudaFree(e->src); cudaFree(e->dst); cudaFree(e->perm); cudaFree(e->par0); cudaFree(e->par1);
   cudaFree(e->loss_partials); cudaFree(e->fx); cudaFree(e->ent); cudaFree(e->inc); cudaFree(e->inc_off);
+  cudaFree(e->wseg); cudaFree(e->whub); cudaFree(e->wpart);
   tiled_free(e);
   pull_free(e);
   ell_free(e);

@@ -50,14 +50,19 @@ struct mde_edges {
   int kvar = 0;              // MDE_B200_KERNEL: 0 default, 1 strided (sorted SoA), 2 precise (no MUFU math)
   int nq = 1;                // MDE_B200_NQ: consecutive quads per thread of the FAST quad kernel (1 or 2)
   int qbps = 4;              // MDE_B200_QUAD_BPS: blocks per SM in the quad kernel's grid cap (1..16)
-  int det = 0;               // deterministic mode: gradient contributions accumulate in 64-bit fixed point
-  long long* fx = nullptr;   // [n * m_hint] fixed-point accumulator (det only)
-  // sorted-SoA layout, m_hint <= 4: every edge is stored again as two directed entries grouped by owner node, and the
-  // owner kernel visits each node's entries in this fixed order, keeps the sum in registers and writes the row once
-  // (no atomics) -- a gradient that is the same bits from run to run
+  int det = 0;               // deterministic mode: m <= 4 fixed point (fx), 5 <= m <= 512 the wide owner kernel
+  long long* fx = nullptr;   // [n * m_hint] fixed-point accumulator (det, m_hint <= 4 only)
+  // sorted-SoA layout, m_hint <= 4 (and deterministic layouts with 5 <= m_hint <= 512): every edge is stored again as
+  // two directed entries grouped by owner node, and the owner kernels visit each node's entries in this fixed order,
+  // keep the sum in registers and write the row once (no atomics) -- a gradient that is the same bits from run to run
   uint32_t* inc = nullptr;      // [2 p] (k << 1) | (node is dst), grouped by node: src entries by k, then dst entries by k
   uint2* ent = nullptr;         // [2 p] in the order of inc: (neighbour row | (node is dst) << 31, bits of par0[k])
   int64_t* inc_off = nullptr;   // [n + 1] first entry of node i in inc / ent
+  // deterministic layouts with m_hint >= 5: lists longer than kWideSeg entries are evaluated in segments (mde_edges.cu)
+  int nwseg = 0, nwhub = 0;
+  int4* wseg = nullptr;         // [nwseg] (node, first entry, end entry) of every segment, in node and list order
+  int4* whub = nullptr;         // [nwhub] (node, first segment, end segment) of every node that has segments
+  float* wpart = nullptr;       // [nwseg * m_hint] the segments' partial gradient rows
   // ---- kind 1 ----
   int m_hint = 0;          // embedding dimension the tile size was chosen for
   int rb = 0;              // log2(R): dst tile rows
