@@ -889,8 +889,6 @@ step_head_kernel(SolverState* __restrict__ S, const float* __restrict__ g, const
   __shared__ __align__(16) unsigned char raw[(kHeadSmemBytes + 15) / 16 * 16];  // warp sums, then the scalar stage
   static_assert(sizeof(raw) >= sizeof(float) * kHeadAcc * (kVecThreads / 32), "warp sums must fit");
   static_assert(kHeadAcc == 66, "the transposing butterfly below is written for 64 + 2 accumulators");
-  __shared__ const float* sp[kPairsPerSlice];
-  __shared__ const float* yp[kPairsPerSlice];
   const unsigned long long t_entry = gtime();
   const int slice = blockIdx.y;
   // one round trip: the 64-byte descriptor the previous epilogue left (same address for every thread)
@@ -917,26 +915,38 @@ step_head_kernel(SolverState* __restrict__ S, const float* __restrict__ g, const
   if (want_grad || want_hist || slice == 0) {
     float* sc = Sb + (int64_t)h1.x * npad;
     float* yc = Yb + (int64_t)h1.x * npad;
-    if (threadIdx.x < kPairsPerSlice) {
-      const int lj = slice * kPairsPerSlice + threadIdx.x;
-      const unsigned ow[8] = {h2.x, h2.y, h2.z, h2.w, h3.x, h3.y, h3.z, h3.w};
-      unsigned word = ow[0];
-#pragma unroll
-      for (int q = 1; q < 8; ++q) if ((lj >> 2) == q) word = ow[q];
-      const int q = (lj < count && lj < 32) ? (int)((word >> (8 * (lj & 3))) & 0xffu) : 0;
-      sp[threadIdx.x] = Sb + (int64_t)q * npad;
-      yp[threadIdx.x] = Yb + (int64_t)q * npad;
-    }
-    __syncthreads();
     int nval = want_hist ? count - slice * kPairsPerSlice : 0;
     if (nval > kPairsPerSlice) nval = kPairsPerSlice;
+    // Physical slots of the slice's pairs: lane L of warp 0 picks order byte L of the descriptor with selects (no
+    // local array), one shuffle hands pair j's byte to lane j.  The pairs are read through the read-only path
+    // (LDG.CONSTANT, addresses formed from Sb / Yb, not pointers kept in shared memory) although Sb / Yb are written
+    // in this launch: slice 0 only writes the candidate slot h1.x (lb.cand), which lbfgs_update never leaves in
+    // order[0 .. count-1].
+    __shared__ int q[kPairsPerSlice];
+    if (threadIdx.x < 32) {
+      const int lane = threadIdx.x;
+      const uint4 hw = (lane < 16) ? h2 : h3;
+      const int wi = (lane >> 2) & 3;
+      const unsigned word = wi == 0 ? hw.x : (wi == 1 ? hw.y : (wi == 2 ? hw.z : hw.w));
+      const int obyte = (int)((word >> (8 * (lane & 3))) & 0xffu);
+      const int lj = slice * kPairsPerSlice + lane;
+      const int qq = __shfl_sync(kFull, obyte, lj & 31);
+      if (lane < kPairsPerSlice) q[lane] = (lj < count) ? qq : 0;
+    }
+    __syncthreads();
     const int64_t n4 = npad >> 2;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    const float4* S4 = reinterpret_cast<const float4*>(Sb);
+    const float4* Y4 = reinterpret_cast<const float4*>(Yb);
+    const float4 z4 = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    const bool gh = want_grad || want_hist;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
       const float4 G = reinterpret_cast<const float4*>(g)[i];
+      const float4 Xv = (slice == 0) ? reinterpret_cast<const float4*>(X)[i] : z4;
+      const float4 P = gh ? reinterpret_cast<const float4*>(gprev)[i] : z4;
+      const float4 D = gh ? reinterpret_cast<const float4*>(d)[i] : z4;
       const float gv[4] = {G.x, G.y, G.z, G.w};
       if (slice == 0) {
-        const float4 Xv = reinterpret_cast<const float4*>(X)[i];
         // column sums (rows are m floats; 4 % m == 0 so element q of a float4 belongs to column q % m)
         if (mcols == 1) {
           acc[kColG] += (G.x + G.y) + (G.z + G.w); acc[kColX] += (Xv.x + Xv.y) + (Xv.z + Xv.w);
@@ -947,44 +957,55 @@ step_head_kernel(SolverState* __restrict__ S, const float* __restrict__ g, const
           acc[kColX] += Xv.x; acc[kColX + 1] += Xv.y; acc[kColX + 2] += Xv.z; acc[kColX + 3] += Xv.w;
         }
       }
-      if (!(want_grad || want_hist)) continue;
-      const float4 P = reinterpret_cast<const float4*>(gprev)[i];
-      const float4 D = reinterpret_cast<const float4*>(d)[i];
       const float dv[4] = {D.x, D.y, D.z, D.w};
       const float yv[4] = {G.x - P.x, G.y - P.y, G.z - P.z, G.w - P.w};
       const float sv[4] = {D.x * t, D.y * t, D.z * t, D.w * t};
-      if (want_grad) {
+      // Every update is computed and then kept or dropped, not branched over (the branchy form spilled at 128
+      // registers).  Each accumulator keeps its FFMA chain, so the bits are the same.
+      {
+        float r0 = acc[kDotsPerSlice], r1 = acc[kDotsPerSlice + 1], r2 = acc[kDotsPerSlice + 2];
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          acc[kDotsPerSlice] += gv[q] * dv[q];
-          acc[kDotsPerSlice + 1] += gv[q] * gv[q];
-          acc[kDotsPerSlice + 2] += fabsf(gv[q]);
+        for (int e = 0; e < 4; ++e) {
+          r0 += gv[e] * dv[e];
+          r1 += gv[e] * gv[e];
+          r2 += fabsf(gv[e]);
         }
+        if (want_grad) { acc[kDotsPerSlice] = r0; acc[kDotsPerSlice + 1] = r1; acc[kDotsPerSlice + 2] = r2; }
       }
-      if (want_hist && slice == 0) {
+      const bool cand = want_hist && slice == 0;
+      if (cand) {
         reinterpret_cast<float4*>(yc)[i] = make_float4(yv[0], yv[1], yv[2], yv[3]);
         reinterpret_cast<float4*>(sc)[i] = make_float4(sv[0], sv[1], sv[2], sv[3]);
+      }
+      {
+        float r0 = acc[0], r1 = acc[1], r2 = acc[2], r3 = acc[3];
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          acc[0] += yv[q] * sv[q]; acc[1] += yv[q] * yv[q];
-          acc[2] += sv[q] * gv[q]; acc[3] += yv[q] * gv[q];
+        for (int e = 0; e < 4; ++e) {
+          r0 += yv[e] * sv[e]; r1 += yv[e] * yv[e];
+          r2 += sv[e] * gv[e]; r3 += yv[e] * gv[e];
         }
+        if (cand) { acc[0] = r0; acc[1] = r1; acc[2] = r2; acc[3] = r3; }
       }
 #pragma unroll
       for (int j = 0; j < kPairsPerSlice; ++j) {
-        if (j < nval) {
-          const float4 A = reinterpret_cast<const float4*>(sp[j])[i];
-          const float4 B = reinterpret_cast<const float4*>(yp[j])[i];
-          const float av[4] = {A.x, A.y, A.z, A.w};
-          const float bv[4] = {B.x, B.y, B.z, B.w};
+        // predicated loads rather than a branch per pair, so the compiler may issue them ahead of the FFMAs
+        const float4 A = (j < nval) ? __ldg(S4 + (int64_t)q[j] * n4 + i) : z4;
+        const float4 B = (j < nval) ? __ldg(Y4 + (int64_t)q[j] * n4 + i) : z4;
+        const float av[4] = {A.x, A.y, A.z, A.w};
+        const float bv[4] = {B.x, B.y, B.z, B.w};
+        float r0 = acc[4 + 5 * j], r1 = acc[4 + 5 * j + 1], r2 = acc[4 + 5 * j + 2], r3 = acc[4 + 5 * j + 3],
+              r4 = acc[4 + 5 * j + 4];
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            acc[4 + 5 * j + 0] += av[q] * yv[q];
-            acc[4 + 5 * j + 1] += bv[q] * yv[q];
-            acc[4 + 5 * j + 2] += sv[q] * bv[q];
-            acc[4 + 5 * j + 3] += av[q] * gv[q];
-            acc[4 + 5 * j + 4] += bv[q] * gv[q];
-          }
+        for (int e = 0; e < 4; ++e) {
+          r0 += av[e] * yv[e];
+          r1 += bv[e] * yv[e];
+          r2 += sv[e] * bv[e];
+          r3 += av[e] * gv[e];
+          r4 += bv[e] * gv[e];
+        }
+        if (j < nval) {  // a pair beyond nval is not added (adding a zero product can turn -0 into +0)
+          acc[4 + 5 * j] = r0; acc[4 + 5 * j + 1] = r1; acc[4 + 5 * j + 2] = r2; acc[4 + 5 * j + 3] = r3;
+          acc[4 + 5 * j + 4] = r4;
         }
       }
     }
