@@ -368,6 +368,19 @@ int mde_knn_wide(const float* X, int64_t n, int d, int k, int32_t* idx_out, floa
 int mde_knn_csr_wide_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes);
 int mde_knn_csr_wide(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                      int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream);
+/* The same two searches for 1 <= k <= mde_knn_long_max_k() (256), k <= n - 1: arguments, output contract, tie rules,
+ * CSR check and return codes of mde_knn_wide and mde_knn_csr_wide.  A running top-288 per row feeds the exact
+ * re-rank.  For k <= 64 the result is that of mde_knn_wide (the same distance bits; indices may differ only inside
+ * exact ties) and of mde_knn_csr_wide (identical), which remain the faster searches there.  `ws`: 1024-byte aligned
+ * device scratch of mde_knn_long_ws_bytes(n, d) or mde_knn_csr_long_ws_bytes(n, d, nnz) bytes (1536 more bytes per
+ * row than the wide searches).  mde_knn_long is asynchronous on `stream`, mde_knn_csr_long blocking as mde_knn_csr. */
+int mde_knn_long_max_k(void);
+int mde_knn_long_ws_bytes(int64_t n, int d, size_t* bytes);
+int mde_knn_long(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                 size_t ws_bytes, void* stream);
+int mde_knn_csr_long_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes);
+int mde_knn_csr_long(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                     int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream);
 /* APPROXIMATE k-nearest neighbours of a dense matrix by NN-descent, for n too large for the exact O(n^2 d) search.
  * Output contract of mde_knn with "the k nearest rows" replaced by "k rows found by the search": k distinct rows per
  * row, never the row itself, ascending by (squared distance, index), with the exact fp32 squared distances of the
@@ -428,6 +441,15 @@ int mde_knn_graph_count(const int32_t* idx, int64_t n, int k, void* ws, size_t w
                         void* stream);
 int mde_knn_graph_emit(int64_t n, int k, const void* ws, size_t ws_bytes, int64_t* edges_out, float* weights_out,
                        void* stream);
+/* The same builder for neighbour lists of 1 <= k <= mde_knn_graph_long_max_k() (256): contract, n k limit and
+ * return codes of mde_knn_graph_ws_bytes / _count / _emit, on a workspace of mde_knn_graph_long_ws_bytes(n, k)
+ * bytes (the same size). */
+int mde_knn_graph_long_max_k(void);
+int mde_knn_graph_long_ws_bytes(int64_t n, int k, size_t* bytes);
+int mde_knn_graph_long_count(const int32_t* idx, int64_t n, int k, void* ws, size_t ws_bytes, int64_t* count,
+                             void* stream);
+int mde_knn_graph_long_emit(int64_t n, int k, const void* ws, size_t ws_bytes, int64_t* edges_out,
+                            float* weights_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Problem construction next to the path (SURVEY section 8 row f4).

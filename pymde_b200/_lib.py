@@ -124,6 +124,13 @@ SIGNATURES = {
     "mde_knn_csr_wide_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.POINTER(C.c_size_t)]),
     "mde_knn_csr_wide": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn_long_max_k": (C.c_int, []),
+    "mde_knn_long_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn_long": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.c_size_t, C.c_void_p]),
+    "mde_knn_csr_long_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.POINTER(C.c_size_t)]),
+    "mde_knn_csr_long": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mde_knn_approx_max_k": (C.c_int, []),
     "mde_knn_approx_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn_approx": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_void_p, C.c_void_p,
@@ -144,6 +151,12 @@ SIGNATURES = {
                                       C.c_void_p]),
     "mde_knn_graph_emit": (C.c_int, [C.c_int64, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
                                      C.c_void_p]),
+    "mde_knn_graph_long_max_k": (C.c_int, []),
+    "mde_knn_graph_long_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn_graph_long_count": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_size_t,
+                                           C.POINTER(C.c_int64), C.c_void_p]),
+    "mde_knn_graph_long_emit": (C.c_int, [C.c_int64, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                          C.c_void_p]),
     "mde_graph_hops_ws_bytes":(C.c_int64, [C.c_int64]),
     "mde_graph_hops": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_double,
                                  C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,

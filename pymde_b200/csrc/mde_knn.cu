@@ -20,7 +20,8 @@
 //
 // mde_knn_wide (24 < k <= 64): knn_wide_tile_kernel does the same sweep for 64 query rows per CTA with one consumer
 // warpgroup and keeps KK = 96 candidates per row in shared memory (mde_knn_select.cuh); knn_wide_rerank_kernel
-// re-ranks all 96 with the arithmetic above.
+// re-ranks all 96 with the arithmetic above.  mde_knn_long (k <= 256) is the same kernel with KK = 288 and candidate
+// tiles of 64 (wgmma.m64n64k16), so that its lists fit in shared memory; knn_long_rerank_kernel re-ranks all 288.
 //
 // Hangs are not an option on a shared GPU: every mbarrier wait is bounded (mde_tma.cuh) and traps.
 #include <cuda.h>  // CUtensorMap and its enums (types only: the encoder is fetched with cudaGetDriverEntryPoint)
@@ -56,16 +57,24 @@ constexpr int kSmemBytes = kStages * kStageBytes + 1024 /* alignment slack */ + 
 static_assert(kTileM == 128 && kTileN == 128, "one TMA box (64 x 128) serves both operands");
 static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 
-// wide search (k <= 64): 64 query rows per CTA, one consumer warpgroup, running top-96 lists in shared memory
+// wide (k <= 64) and long (k <= 256) searches: 64 query rows per CTA, one consumer warpgroup, running top-KK lists in
+// shared memory, candidate tiles of TN = 128 (wide) or 64 (long) rows
 constexpr int kWideTileM = 64;
 constexpr int kAOpBytes = kWideTileM * kRowBytes;          // 8 KB: one 64-row query operand block (hi or lo)
-constexpr int kWideStageBytes = 2 * kAOpBytes + 2 * kOpBytes;  // A hi, A lo, B hi, B lo = 48 KB
 constexpr int kWideConsumerWarps = 4;                       // warps 0-3: one consumer warpgroup; warp 4: TMA producer
 constexpr int kWideThreads = (kWideConsumerWarps + 1) * 32;
-constexpr int kWideSmemBytes = kStages * kWideStageBytes + 1024 /* alignment slack */ +
-                               kWideTileM * kAccStride * 4 + kTileN * 4 /* norms */ +
-                               kWideTileM * kWideListStride * 8 /* lists */ + 64 /* barriers */;
-static_assert(kWideSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
+constexpr int kLongTileN = 64;
+
+template <int TN>
+constexpr int kWideStageBytes = 2 * kAOpBytes + 2 * TN * kRowBytes;  // A hi, A lo, B hi, B lo
+template <int KK, int TN>
+constexpr int kWideSmemBytes = kStages * kWideStageBytes<TN> + 1024 /* alignment slack */ +
+                               kWideTileM * (TN + 2) * 4 /* accumulators */ + TN * 4 /* norms */ +
+                               kWideTileM * WideList<KK>::kStride * 8 /* lists */ + 64 /* barriers */;
+// wide: 2 x 48 KB stages, 33 KB accumulators, 49 KB lists.  long: 148.5 KB of lists leave room for 2 x 32 KB stages
+// of 64-wide candidate tiles and a 16.5 KB accumulator (232 256 bytes in all)
+static_assert(kWideSmemBytes<kWideKK, kTileN> <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
+static_assert(kWideSmemBytes<kLongKK, kLongTileN> <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 
 // ---------------------------------------------------------------------------------------------------------------
 // PTX wrappers (tensor TMA); mbarriers come from mde_tma.cuh, wgmma from mde_wgmma.cuh
@@ -304,29 +313,36 @@ knn_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* 
 namespace {
 
 // ---------------------------------------------------------------------------------------------------------------
-// wide tiles (k <= 64): as knn_tile_kernel for 64 query rows, one running top-96 per row in shared memory
+// wide tiles (k <= 64, KK = 96, TN = 128) and long tiles (k <= 256, KK = 288, TN = 64): as knn_tile_kernel for 64
+// query rows, one running top-KK per row in shared memory, wgmma.m64n{TN}k16 on candidate tiles of TN rows
 // ---------------------------------------------------------------------------------------------------------------
+template <int KK, int TN>
 __global__ void __launch_bounds__(kWideThreads, 1)
 knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant__ CUtensorMap map_al,
                      const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_l,
                      const float* __restrict__ norms, int64_t n, int64_t n_pad, int k_pad,
                      int32_t* __restrict__ cand_idx, float* __restrict__ cand_val) {
+  static_assert(TN == 64 || TN == 128, "wgmma.m64n64k16 or m64n128k16");
+  constexpr int kBOpBytes = TN * kRowBytes;
+  constexpr int kStageB = kWideStageBytes<TN>;
+  constexpr int kAccS = TN + 2;  // floats per staged accumulator row: the scan's float2 reads are conflict-free
+  constexpr int kStride = WideList<KK>::kStride;
   extern __shared__ uint8_t smem_raw[];
-  // carve: [stages x 48 KB, 1024-aligned] | staged accumulators [64][kAccStride] | norms[128] |
-  //        list distances [64][kWideListStride] | list indices [64][kWideListStride] | barriers
+  // carve: [stages x kStageB, 1024-aligned] | staged accumulators [64][kAccS] | norms[TN] |
+  //        list distances [64][kStride] | list indices [64][kStride] | barriers
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
-  float* s_acc = reinterpret_cast<float*>(gen + kStages * kWideStageBytes);
-  float* s_norm = s_acc + kWideTileM * kAccStride;
-  float* s_ld = s_norm + kTileN;
-  int* s_li = reinterpret_cast<int*>(s_ld + kWideTileM * kWideListStride);
-  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_li + kWideTileM * kWideListStride);
+  float* s_acc = reinterpret_cast<float*>(gen + kStages * kStageB);
+  float* s_norm = s_acc + kWideTileM * kAccS;
+  float* s_ld = s_norm + TN;
+  int* s_li = reinterpret_cast<int*>(s_ld + kWideTileM * kStride);
+  uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_li + kWideTileM * kStride);
   const uint32_t bar0 = smem_u32(s_bar);
   // barriers: full[s] = bar0 + 8 s (TMA bytes landed), empty[s] = bar0 + 16 + 8 s (every consumer warp is done)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_kb = k_pad / kBlockK;
-  const int num_tiles = (int)(n_pad / kTileN);
+  const int num_tiles = (int)(n_pad / TN);
   const int row0 = blockIdx.x * kWideTileM;
 
   if (threadIdx.x == 0) {
@@ -343,12 +359,12 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(bar0 + 16 + 8 * stage, phase ^ 1);  // slot released by the consumers
           const uint32_t full = bar0 + 8 * stage;
-          const uint32_t dst = base + stage * kWideStageBytes;
-          mbar_expect_tx(full, kWideStageBytes);
+          const uint32_t dst = base + stage * kStageB;
+          mbar_expect_tx(full, kStageB);
           tma_load_2d(dst, &map_ah, kb * kBlockK, row0, full);
           tma_load_2d(dst + kAOpBytes, &map_al, kb * kBlockK, row0, full);
-          tma_load_2d(dst + 2 * kAOpBytes, &map_h, kb * kBlockK, t * kTileN, full);
-          tma_load_2d(dst + 2 * kAOpBytes + kOpBytes, &map_l, kb * kBlockK, t * kTileN, full);
+          tma_load_2d(dst + 2 * kAOpBytes, &map_h, kb * kBlockK, t * TN, full);
+          tma_load_2d(dst + 2 * kAOpBytes + kBOpBytes, &map_l, kb * kBlockK, t * TN, full);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
@@ -361,33 +377,39 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
   const int lrow = et >> 1, half = et & 1;
   const int row = row0 + lrow;
   const int frow = 16 * warp + (lane >> 2), fcol = 2 * (lane & 3);
-  WideList list;
-  list.init(s_ld + lrow * kWideListStride, s_li + lrow * kWideListStride, half);
-  float acc[64];
+  WideList<KK> list;
+  list.init(s_ld + lrow * kStride, s_li + lrow * kStride, half);
+  float acc[TN / 2];
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+  for (int i = 0; i < TN / 2; ++i) acc[i] = 0.0f;
 
   int stage = 0; uint32_t phase = 0;
   for (int t = 0; t < num_tiles; ++t) {
     for (int kb = 0; kb < num_kb; ++kb) {
       mbar_wait(bar0 + 8 * stage, phase);  // operands landed
-      const uint32_t sa = base + stage * kWideStageBytes;
+      const uint32_t sa = base + stage * kStageB;
       const uint64_t ah = smem_desc_sw128(sa), al = smem_desc_sw128(sa + kAOpBytes);
-      const uint64_t bh = smem_desc_sw128(sa + 2 * kAOpBytes), bl = smem_desc_sw128(sa + 2 * kAOpBytes + kOpBytes);
+      const uint64_t bh = smem_desc_sw128(sa + 2 * kAOpBytes), bl = smem_desc_sw128(sa + 2 * kAOpBytes + kBOpBytes);
 #pragma unroll
-      for (int i = 0; i < 64; ++i) fence_operand(acc[i]);
+      for (int i = 0; i < TN / 2; ++i) fence_operand(acc[i]);
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
         const uint64_t adv = (uint64_t)((k * kWgmmaK * 2) >> 4);
-        wgmma_bf16(acc, ah + adv, bh + adv, (kb | k) != 0);
-        wgmma_bf16(acc, ah + adv, bl + adv, 1u);
-        wgmma_bf16(acc, al + adv, bh + adv, 1u);
+        if constexpr (TN == 128) {
+          wgmma_bf16(acc, ah + adv, bh + adv, (kb | k) != 0);
+          wgmma_bf16(acc, ah + adv, bl + adv, 1u);
+          wgmma_bf16(acc, al + adv, bh + adv, 1u);
+        } else {
+          wgmma_bf16_n64(acc, ah + adv, bh + adv, (kb | k) != 0);
+          wgmma_bf16_n64(acc, ah + adv, bl + adv, 1u);
+          wgmma_bf16_n64(acc, al + adv, bh + adv, 1u);
+        }
       }
       wgmma_commit();
       wgmma_wait_all();
 #pragma unroll
-      for (int i = 0; i < 64; ++i) fence_operand(acc[i]);
+      for (int i = 0; i < TN / 2; ++i) fence_operand(acc[i]);
       __syncwarp();
       if (lane == 0) mbar_arrive(bar0 + 16 + 8 * stage);  // this warp no longer reads the slot
       if (++stage == kStages) { stage = 0; phase ^= 1; }
@@ -395,45 +417,46 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
     // the previous tile's scan of s_acc / s_norm is finished by every consumer thread
     named_bar_sync(1, 128);
 #pragma unroll
-    for (int j = 0; j < kTileN / 8; ++j) {
-      *reinterpret_cast<float2*>(s_acc + frow * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
-      *reinterpret_cast<float2*>(s_acc + (frow + 8) * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    for (int j = 0; j < TN / 8; ++j) {
+      *reinterpret_cast<float2*>(s_acc + frow * kAccS + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(s_acc + (frow + 8) * kAccS + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
     }
-    s_norm[et] = __ldg(norms + (int64_t)t * kTileN + et);
+    if (et < TN) s_norm[et] = __ldg(norms + (int64_t)t * TN + et);
     named_bar_sync(1, 128);
     // both lanes of the row offer every column, in column order
-    const float2* arow = reinterpret_cast<const float2*>(s_acc + lrow * kAccStride);
+    const float2* arow = reinterpret_cast<const float2*>(s_acc + lrow * kAccS);
     const float2* sn = reinterpret_cast<const float2*>(s_norm);
 #pragma unroll 2
-    for (int i = 0; i < kTileN / 2; ++i) {
+    for (int i = 0; i < TN / 2; ++i) {
       const float2 a = arow[i], s = sn[i];
-      const int col = t * kTileN + 2 * i;
+      const int col = t * TN + 2 * i;
       if (col != row && col < n) list.offer(fmaf(-2.0f, a.x, s.x), col);
       if (col + 1 != row && col + 1 < n) list.offer(fmaf(-2.0f, a.y, s.y), col + 1);
     }
   }
-  if (row < n) list.store(cand_idx + (int64_t)row * kWideKK, cand_val + (int64_t)row * kWideKK);
+  if (row < n) list.store(cand_idx + (int64_t)row * KK, cand_val + (int64_t)row * KK);
 }
 
 }  // namespace
 
 namespace mde {
 
-// Exact fp32 squared distances of a row's 96 candidates (the arithmetic of knn_rerank_kernel), the k smallest in
-// ascending order; lane q owns candidates q, q + 32 and q + 64, ranks are taken over all 96.
-__global__ void __launch_bounds__(256)
-knn_wide_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
-                       int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+// Exact fp32 squared distances of a row's KK candidates (the arithmetic of knn_rerank_kernel), the k smallest in
+// ascending order; lane q owns candidates q, q + 32, q + 64, ..., ranks are taken over all KK.
+template <int KK>
+__device__ __forceinline__ void wide_rerank_row(const float* __restrict__ X, int64_t n, int d,
+                                                const int32_t* __restrict__ cand_idx, int k,
+                                                int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= n) return;
-  constexpr int kPer = kWideKK / 32;
+  constexpr int kPer = KK / 32;
   int mine[kPer];
   float my_d[kPer];
   const float* xq = X + row * d;
 #pragma unroll
   for (int s = 0; s < kPer; ++s) {
-    mine[s] = cand_idx[row * kWideKK + 32 * s + lane];
+    mine[s] = cand_idx[row * KK + 32 * s + lane];
     my_d[s] = __int_as_float(0x7f800000);
     for (int q = 0; q < 32; ++q) {
       const int c = __shfl_sync(kFull, mine[s], q);
@@ -446,7 +469,7 @@ knn_wide_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int3
       if (lane == q) my_d[s] = acc;
     }
   }
-  // rank of each owned (distance, index) among the 96: ties broken by index, missing candidates last
+  // rank of each owned (distance, index) among the KK: ties broken by index, missing candidates last
   int rank[kPer] = {};
 #pragma unroll
   for (int s2 = 0; s2 < kPer; ++s2) {
@@ -466,6 +489,19 @@ knn_wide_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int3
       out_d2[row * k + rank[s]] = my_d[s];
     }
   }
+}
+
+__global__ void __launch_bounds__(256)
+knn_wide_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
+                       int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+  wide_rerank_row<kWideKK>(X, n, d, cand_idx, k, out_idx, out_d2);
+}
+
+// the 288 candidates of the long search, with the same arithmetic
+__global__ void __launch_bounds__(256)
+knn_long_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
+                       int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+  wide_rerank_row<kLongKK>(X, n, d, cand_idx, k, out_idx, out_d2);
 }
 
 }  // namespace mde
@@ -507,7 +543,7 @@ struct KnnLayout {
   size_t off_h, off_l, off_norm, off_ci, off_cv, total;
 };
 
-// kk: candidates kept per row (kKK, or kWideKK for the wide search)
+// kk: candidates kept per row (kKK, kWideKK for the wide search, kLongKK for the long one)
 KnnLayout knn_layout(int64_t n, int d, int kk = kKK) {
   KnnLayout L;
   L.n_pad = (n + kTileN - 1) / kTileN * kTileN;
@@ -521,6 +557,46 @@ KnnLayout knn_layout(int64_t n, int d, int kk = kKK) {
   L.off_cv = o; o = up(o + (size_t)n * kk * 4);
   L.total = o;
   return L;
+}
+
+// mde_knn_wide (KK = 96, TN = 128) and mde_knn_long (KK = 288, TN = 64): prep, tiles, re-rank of all KK candidates.
+template <int KK, int TN>
+int run_wide(const float* X, int64_t n, int d, int k, int max_k, int32_t* idx_out, float* d2_out, void* ws,
+             size_t ws_bytes, void* stream) {
+  if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > max_k || k > n - 1) return MDE_E_INVALID;
+  if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
+  const KnnLayout L = knn_layout(n, d, KK);
+  if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  EncodeTiledFn enc = nullptr;
+  int rc;
+  if ((rc = tensor_map_encoder(&enc))) return rc;
+  uint8_t* w = static_cast<uint8_t*>(ws);
+  __nv_bfloat16* Xh = reinterpret_cast<__nv_bfloat16*>(w + L.off_h);
+  __nv_bfloat16* Xl = reinterpret_cast<__nv_bfloat16*>(w + L.off_l);
+  float* norms = reinterpret_cast<float*>(w + L.off_norm);
+  int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
+  float* cv = reinterpret_cast<float*>(w + L.off_cv);
+  CUtensorMap mah, mal, mh, ml;  // query operand in 64-row boxes, candidate operand in TN-row boxes
+  if ((rc = make_map(enc, &mah, Xh, L.n_pad, L.k_pad, kWideTileM))) return rc;
+  if ((rc = make_map(enc, &mal, Xl, L.n_pad, L.k_pad, kWideTileM))) return rc;
+  if ((rc = make_map(enc, &mh, Xh, L.n_pad, L.k_pad, TN))) return rc;
+  if ((rc = make_map(enc, &ml, Xl, L.n_pad, L.k_pad, TN))) return rc;
+  knn_prep_kernel<<<(unsigned)((L.n_pad + 7) / 8), 256, 0, st>>>(X, n, d, L.n_pad, L.k_pad, Xh, Xl, norms);
+  MDE_LAUNCH_CHECK();
+  constexpr int kSmem = kWideSmemBytes<KK, TN>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    MDE_CUDA_TRY(cudaFuncSetAttribute(knn_wide_tile_kernel<KK, TN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+    attr_set = true;
+  }
+  const unsigned grid = (unsigned)((n + kWideTileM - 1) / kWideTileM);
+  knn_wide_tile_kernel<KK, TN><<<grid, kWideThreads, kSmem, st>>>(mah, mal, mh, ml, norms, n, L.n_pad, L.k_pad, ci, cv);
+  MDE_LAUNCH_CHECK();
+  if constexpr (KK == kWideKK) knn_wide_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(X, n, d, ci, k, idx_out, d2_out);
+  else knn_long_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(X, n, d, ci, k, idx_out, d2_out);
+  MDE_LAUNCH_CHECK();
+  return 0;
 }
 
 }  // namespace
@@ -579,41 +655,20 @@ int mde_knn_wide_ws_bytes(int64_t n, int d, size_t* bytes) {
 
 int mde_knn_wide(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                  size_t ws_bytes, void* stream) {
-  if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > kWideMaxK || k > n - 1)
-    return MDE_E_INVALID;
-  if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
-  const KnnLayout L = knn_layout(n, d, kWideKK);
-  if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream;
-  EncodeTiledFn enc = nullptr;
-  int rc;
-  if ((rc = tensor_map_encoder(&enc))) return rc;
-  uint8_t* w = static_cast<uint8_t*>(ws);
-  __nv_bfloat16* Xh = reinterpret_cast<__nv_bfloat16*>(w + L.off_h);
-  __nv_bfloat16* Xl = reinterpret_cast<__nv_bfloat16*>(w + L.off_l);
-  float* norms = reinterpret_cast<float*>(w + L.off_norm);
-  int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
-  float* cv = reinterpret_cast<float*>(w + L.off_cv);
-  CUtensorMap mah, mal, mh, ml;  // query operand in 64-row boxes, candidate operand in 128-row boxes
-  if ((rc = make_map(enc, &mah, Xh, L.n_pad, L.k_pad, kWideTileM))) return rc;
-  if ((rc = make_map(enc, &mal, Xl, L.n_pad, L.k_pad, kWideTileM))) return rc;
-  if ((rc = make_map(enc, &mh, Xh, L.n_pad, L.k_pad))) return rc;
-  if ((rc = make_map(enc, &ml, Xl, L.n_pad, L.k_pad))) return rc;
-  knn_prep_kernel<<<(unsigned)((L.n_pad + 7) / 8), 256, 0, st>>>(X, n, d, L.n_pad, L.k_pad, Xh, Xl, norms);
-  MDE_LAUNCH_CHECK();
-  static bool attr_set = false;
-  if (!attr_set) {
-    MDE_CUDA_TRY(cudaFuncSetAttribute(knn_wide_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      kWideSmemBytes));
-    attr_set = true;
-  }
-  const unsigned grid = (unsigned)((n + kWideTileM - 1) / kWideTileM);
-  knn_wide_tile_kernel<<<grid, kWideThreads, kWideSmemBytes, st>>>(mah, mal, mh, ml, norms, n, L.n_pad, L.k_pad, ci,
-                                                                   cv);
-  MDE_LAUNCH_CHECK();
-  knn_wide_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(X, n, d, ci, k, idx_out, d2_out);
-  MDE_LAUNCH_CHECK();
+  return run_wide<kWideKK, kTileN>(X, n, d, k, kWideMaxK, idx_out, d2_out, ws, ws_bytes, stream);
+}
+
+int mde_knn_long_max_k(void) { return kLongMaxK; }
+
+int mde_knn_long_ws_bytes(int64_t n, int d, size_t* bytes) {
+  if (!bytes || n < 2 || d < 1) return MDE_E_INVALID;
+  *bytes = knn_layout(n, d, kLongKK).total;
   return 0;
+}
+
+int mde_knn_long(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                 size_t ws_bytes, void* stream) {
+  return run_wide<kLongKK, kLongTileN>(X, n, d, k, kLongMaxK, idx_out, d2_out, ws, ws_bytes, stream);
 }
 
 }  // extern "C"

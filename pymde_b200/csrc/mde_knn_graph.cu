@@ -9,13 +9,13 @@
 // and its output is the distinct values of F_a u R_a in ascending order, each weighted by its number of occurrences
 // in both lists (scipy sums the duplicates).  The call is
 //
-//   prep       one warp per row: check the entries, bitonic-sort the row's entries > i (two per lane), keep each
-//              distinct value once with its multiplicity (F_i, acount[i] values), and write the reverse sort's input
-//              (key = v for an entry u -> v with v < u, else n; value = u)
+//   prep       one warp per row: check the entries, bitonic-sort the row's entries > i (P per lane: 2 for k <= 64,
+//              8 for k <= 256), keep each distinct value once with its multiplicity (F_i, acount[i] values), and
+//              write the reverse sort's input (key = v for an entry u -> v with v < u, else n; value = u)
 //   sort       one stable CUB radix sort of (key, value) over ceil(log2(n + 1)) bits: R_v = the rows u > v that list
 //              v, ascending, at [rev_off[v], rev_off[v + 1]) (rev_off by binary search)
 //   flags      per reverse entry p: 1 when it is the first of its run of equal u in R_v and u is not in F_v (binary
-//              search in <= 64 values); an exclusive scan gives S_R
+//              search in <= k values); an exclusive scan gives S_R
 //   offsets    cnt[i] = acount[i] + (R-only runs of row i), scanned into row_off
 //
 // and the emit pass writes every output at its rank in the union, without atomics:
@@ -38,7 +38,8 @@ using namespace mde;
 
 namespace {
 
-constexpr int kMaxK = 64;
+constexpr int kMaxK = 64;       // mde_knn_graph_*: the prep pass sorts 2 entries per lane
+constexpr int kLongMaxK = 256;  // mde_knn_graph_*_long: 8 entries per lane
 constexpr int kSentinel = INT_MAX;  // past every valid value: sorts last
 
 int bits_for(int64_t count) {  // smallest b with 2^b >= count
@@ -67,7 +68,7 @@ GraphLayout graph_layout(int64_t n, int k) {
   L.off_hdr = o; o = up(o + 16);                       // {flag, total, sort buffer}
   L.off_acount = o; o = up(o + (size_t)n * 4);
   L.off_fwd = o; o = up(o + (size_t)L.N * 4);
-  L.off_fmul = o; o = up(o + (size_t)L.N);
+  L.off_fmul = o; o = up(o + (size_t)L.N);           // multiplicity - 1 (1 .. 256 fits a byte)
   L.off_k0 = o; o = up(o + items * 4);
   L.off_k1 = o; o = up(o + items * 4);
   L.off_v0 = o; o = up(o + items * 4);
@@ -119,19 +120,21 @@ __device__ __forceinline__ int32_t search(const int32_t* __restrict__ a, int32_t
   return lo;
 }
 
-// One warp per row: the check, the forward list and the reverse sort's input.
+// One warp per row of k <= 32 P entries: the check, the forward list and the reverse sort's input.
+template <int P>
 __global__ void __launch_bounds__(256)
 knn_graph_prep_kernel(const int32_t* __restrict__ idx, int64_t n, int k, int32_t* __restrict__ flag,
                       int32_t* __restrict__ acount, int32_t* __restrict__ fwd, uint8_t* __restrict__ fmul,
                       int32_t* __restrict__ rkey, int32_t* __restrict__ rval) {
+  constexpr int kSlots = 32 * P;
   const int lane = threadIdx.x & 31;
   const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (i >= n) return;
   const int32_t* row = idx + i * k;
-  int32_t v[2];
+  int32_t v[P];
   bool bad = false;
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
+  for (int h = 0; h < P; ++h) {
     const int e = lane + 32 * h;
     const int32_t x = e < k ? __ldg(row + e) : -1;
     bad |= x == i || x < -1 || x >= n;
@@ -142,46 +145,59 @@ knn_graph_prep_kernel(const int32_t* __restrict__ idx, int64_t n, int k, int32_t
     }
   }
   if (__any_sync(kFull, bad) && lane == 0) *flag = 1;
-  // bitonic sort of the 64 slots e = lane + 32 h, ascending
+  // bitonic sort of the kSlots slots e = lane + 32 h, ascending (strides >= 32 pair registers of one lane)
 #pragma unroll
-  for (int size = 2; size <= 64; size <<= 1) {
+  for (int size = 2; size <= kSlots; size <<= 1) {
 #pragma unroll
     for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      int32_t o[2];
-      if (stride == 32) { o[0] = v[1]; o[1] = v[0]; }
-      else { o[0] = __shfl_xor_sync(kFull, v[0], stride); o[1] = __shfl_xor_sync(kFull, v[1], stride); }
+      int32_t o[P];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
+      for (int h = 0; h < P; ++h) o[h] = stride >= 32 ? v[h ^ (stride >> 5)] : __shfl_xor_sync(kFull, v[h], stride);
+#pragma unroll
+      for (int h = 0; h < P; ++h) {
         const int e = lane + 32 * h;
         const bool asc = (e & size) == 0, lower = (e & stride) == 0;
         v[h] = (lower == asc) ? min(v[h], o[h]) : max(v[h], o[h]);
       }
     }
   }
-  // distinct values with their multiplicities, compacted to the front of the row
-  const int32_t up0 = __shfl_up_sync(kFull, v[0], 1), up1 = __shfl_up_sync(kFull, v[1], 1);
-  const int32_t last0 = __shfl_sync(kFull, v[0], 31);
-  const int32_t prev[2] = {lane ? up0 : INT_MIN, lane ? up1 : last0};
-  bool head[2], valid[2];
+  // distinct values with their multiplicities, compacted to the front of the row; H[h] / V[h]: the heads / valid
+  // values among the slots lane + 32 h
+  uint32_t H[P], V[P];
+  bool head[P];
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    valid[h] = v[h] != kSentinel;
-    head[h] = valid[h] && prev[h] != v[h];
+  for (int h = 0; h < P; ++h) {
+    const int32_t up = __shfl_up_sync(kFull, v[h], 1);
+    const int32_t last = h ? __shfl_sync(kFull, v[h ? h - 1 : 0], 31) : INT_MIN;
+    const int32_t prev = lane ? up : last;
+    const bool valid = v[h] != kSentinel;
+    head[h] = valid && prev != v[h];
+    H[h] = __ballot_sync(kFull, head[h]);
+    V[h] = __ballot_sync(kFull, valid);
   }
-  const uint64_t H = (uint64_t)__ballot_sync(kFull, head[0]) | ((uint64_t)__ballot_sync(kFull, head[1]) << 32);
-  const uint64_t V = (uint64_t)__ballot_sync(kFull, valid[0]) | ((uint64_t)__ballot_sync(kFull, valid[1]) << 32);
-  const int nvalid = __popcll(V);  // the valid values are a prefix
+  int nvalid = 0, heads = 0;  // the valid values are a prefix
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    if (!head[h]) continue;
-    const int e = lane + 32 * h;
-    const uint64_t above = H & ~((2ull << e) - 1);  // (2ull << 63 wraps to 0: nothing above slot 63)
-    const int next = above ? __ffsll((long long)above) - 1 : nvalid;
-    const int r = __popcll(H & ((1ull << e) - 1));
-    fwd[i * k + r] = v[h];
-    fmul[i * k + r] = (uint8_t)(next - e);
+  for (int h = 0; h < P; ++h) { nvalid += __popc(V[h]); heads += __popc(H[h]); }
+  int below = 0;  // heads in the registers before h
+#pragma unroll
+  for (int h = 0; h < P; ++h) {
+    if (head[h]) {
+      const int e = lane + 32 * h;
+      int next = nvalid;  // the slot of the next head, or the end of the valid values
+      const uint32_t above = H[h] & ~((2u << lane) - 1);  // (2u << 31 wraps to 0: nothing above lane 31)
+      if (above) {
+        next = 32 * h + __ffs(above) - 1;
+      } else {
+#pragma unroll
+        for (int h2 = P - 1; h2 > h; --h2) if (H[h2]) next = 32 * h2 + __ffs(H[h2]) - 1;
+      }
+      const int r = below + __popc(H[h] & ((1u << lane) - 1));
+      fwd[i * k + r] = v[h];
+      fmul[i * k + r] = (uint8_t)(next - e - 1);
+    }
+    below += __popc(H[h]);
   }
-  if (lane == 0) acount[i] = __popcll(H);
+  if (lane == 0) acount[i] = heads;
 }
 
 // rev_off[v] = first p with key[p] >= v, for v in [0, n] (a binary search each: long runs of one key, or keys that
@@ -252,7 +268,7 @@ __global__ void knn_graph_emit_fwd_kernel(int64_t n, int k, const int32_t* __res
   const int64_t pos = (int64_t)row_off[i] + r + (S[lb] - S[lo]);
   edges[2 * pos] = i;
   edges[2 * pos + 1] = a;
-  weights[pos] = (float)(fmul[t] + (ub - lb));
+  weights[pos] = (float)(fmul[t] + 1 + (ub - lb));
 }
 
 // The runs of reverse entries whose row is not in the owner's forward list (one thread per reverse entry).
@@ -296,7 +312,7 @@ int graph_cub_bytes(int64_t n, int64_t N, size_t* bytes) {
   return 0;
 }
 
-bool bad_args(int64_t n, int k) { return n < 1 || k < 1 || k > kMaxK; }
+bool bad_args(int64_t n, int k, int max_k) { return n < 1 || k < 1 || k > max_k; }
 
 // The checks both calls share: every one of them is host arithmetic.
 int check_ws(int64_t n, int k, const void* ws, size_t ws_bytes, GraphLayout* L) {
@@ -306,22 +322,17 @@ int check_ws(int64_t n, int k, const void* ws, size_t ws_bytes, GraphLayout* L) 
   return 0;
 }
 
-}  // namespace
-
-extern "C" {
-
-int mde_knn_graph_max_k(void) { return kMaxK; }
-
-int mde_knn_graph_ws_bytes(int64_t n, int k, size_t* bytes) {
-  if (!bytes || bad_args(n, k)) return MDE_E_INVALID;
+// The calls of both entry families; max_k is the family's bound on k.
+int graph_ws_bytes(int64_t n, int k, int max_k, size_t* bytes) {
+  if (!bytes || bad_args(n, k, max_k)) return MDE_E_INVALID;
   if (n * k >= INT_MAX) return MDE_E_UNSUPPORTED;
   *bytes = graph_layout(n, k).total;
   return 0;
 }
 
-int mde_knn_graph_count(const int32_t* idx, int64_t n, int k, void* ws, size_t ws_bytes, int64_t* count,
-                        void* stream) {
-  if (!idx || !ws || !count || bad_args(n, k)) return MDE_E_INVALID;
+int graph_count(const int32_t* idx, int64_t n, int k, int max_k, void* ws, size_t ws_bytes, int64_t* count,
+                void* stream) {
+  if (!idx || !ws || !count || bad_args(n, k, max_k)) return MDE_E_INVALID;
   GraphLayout L;
   int rc = check_ws(n, k, ws, ws_bytes, &L);
   if (rc) return rc;
@@ -332,7 +343,10 @@ int mde_knn_graph_count(const int32_t* idx, int64_t n, int k, void* ws, size_t w
   uint8_t* w = static_cast<uint8_t*>(ws);
   const GraphBufs B = carve(w, L);
   MDE_CUDA_TRY(cudaMemsetAsync(B.hdr, 0, 16, st));
-  knn_graph_prep_kernel<<<grid_for(n * 32), 256, 0, st>>>(idx, n, k, B.hdr, B.acount, B.fwd, B.fmul, B.k0, B.v0);
+  if (k <= kMaxK)
+    knn_graph_prep_kernel<2><<<grid_for(n * 32), 256, 0, st>>>(idx, n, k, B.hdr, B.acount, B.fwd, B.fmul, B.k0, B.v0);
+  else
+    knn_graph_prep_kernel<8><<<grid_for(n * 32), 256, 0, st>>>(idx, n, k, B.hdr, B.acount, B.fwd, B.fmul, B.k0, B.v0);
   MDE_LAUNCH_CHECK();
   cub::DoubleBuffer<int32_t> kb(B.k0, B.k1), vb(B.v0, B.v1);
   size_t tb = L.tmp_bytes;
@@ -359,9 +373,9 @@ int mde_knn_graph_count(const int32_t* idx, int64_t n, int k, void* ws, size_t w
   return 0;
 }
 
-int mde_knn_graph_emit(int64_t n, int k, const void* ws, size_t ws_bytes, int64_t* edges_out, float* weights_out,
-                       void* stream) {
-  if (!ws || !edges_out || !weights_out || bad_args(n, k)) return MDE_E_INVALID;
+int graph_emit(int64_t n, int k, int max_k, const void* ws, size_t ws_bytes, int64_t* edges_out, float* weights_out,
+               void* stream) {
+  if (!ws || !edges_out || !weights_out || bad_args(n, k, max_k)) return MDE_E_INVALID;
   GraphLayout L;
   const int rc = check_ws(n, k, ws, ws_bytes, &L);
   if (rc) return rc;
@@ -375,6 +389,38 @@ int mde_knn_graph_emit(int64_t n, int k, const void* ws, size_t ws_bytes, int64_
                                                            edges_out, weights_out);
   MDE_LAUNCH_CHECK();
   return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int mde_knn_graph_max_k(void) { return kMaxK; }
+
+int mde_knn_graph_ws_bytes(int64_t n, int k, size_t* bytes) { return graph_ws_bytes(n, k, kMaxK, bytes); }
+
+int mde_knn_graph_count(const int32_t* idx, int64_t n, int k, void* ws, size_t ws_bytes, int64_t* count,
+                        void* stream) {
+  return graph_count(idx, n, k, kMaxK, ws, ws_bytes, count, stream);
+}
+
+int mde_knn_graph_emit(int64_t n, int k, const void* ws, size_t ws_bytes, int64_t* edges_out, float* weights_out,
+                       void* stream) {
+  return graph_emit(n, k, kMaxK, ws, ws_bytes, edges_out, weights_out, stream);
+}
+
+int mde_knn_graph_long_max_k(void) { return kLongMaxK; }
+
+int mde_knn_graph_long_ws_bytes(int64_t n, int k, size_t* bytes) { return graph_ws_bytes(n, k, kLongMaxK, bytes); }
+
+int mde_knn_graph_long_count(const int32_t* idx, int64_t n, int k, void* ws, size_t ws_bytes, int64_t* count,
+                             void* stream) {
+  return graph_count(idx, n, k, kLongMaxK, ws, ws_bytes, count, stream);
+}
+
+int mde_knn_graph_long_emit(int64_t n, int k, const void* ws, size_t ws_bytes, int64_t* edges_out,
+                            float* weights_out, void* stream) {
+  return graph_emit(n, k, kLongMaxK, ws, ws_bytes, edges_out, weights_out, stream);
 }
 
 }  // extern "C"

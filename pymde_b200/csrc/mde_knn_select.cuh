@@ -1,8 +1,8 @@
-// mde_knn_select.cuh -- the running top-96 of the wide k-nearest-neighbour tile kernels (mde_knn.cu,
-// mde_knn_sparse.cu; k <= 64).
+// mde_knn_select.cuh -- the running top-KK lists of the wide (KK = 96, k <= 64) and long (KK = 288, k <= 256)
+// k-nearest-neighbour tile kernels (mde_knn.cu, mde_knn_sparse.cu).
 //
-// One list of kWideKK (distance, index) pairs per query row lives in shared memory; it is too large for registers
-// next to the 64 fp32 wgmma accumulators.  Two adjacent lanes (a "pair", half = lane & 1) own a row.  Both offer
+// One list of KK (distance, index) pairs per query row lives in shared memory; it is too large for registers
+// next to the fp32 wgmma accumulators.  Two adjacent lanes (a "pair", half = lane & 1) own a row.  Both offer
 // every candidate of the row in the same order with the same values, so both take the same branches.  Lane `half`
 // owns the slots of its parity: it writes the slot it replaces (when the slot is its own) and scans only its own
 // slots for the new worst, and the two partial worsts meet through one shuffle.  Candidates are ordered by
@@ -23,23 +23,29 @@ namespace mde {
 constexpr int kNarrowKK = 32;        // candidates per row read by knn_rerank_kernel
 constexpr int kWideKK = 96;          // candidates kept per row before the exact re-rank
 constexpr int kWideMaxK = 64;        // leaves >= 32 spare candidates for the bf16 x 3 error of the cross terms
-constexpr int kWideListStride = 98;  // words per row list: the 32 lanes of a warp (16 rows) hit 32 different banks
+constexpr int kLongKK = 288;         // the same margin for the long search
+constexpr int kLongMaxK = 256;
 
 __device__ __forceinline__ bool knn_before(float d1, int i1, float d2, int i2) {
   return d1 < d2 || (d1 == d2 && i1 < i2);
 }
 
 // Per-lane copy of its row's threshold: the worst kept pair and its slot (identical in both lanes of the pair).
+template <int KK>
 struct WideList {
-  float* d;    // this row's distances [kWideKK] in shared memory
-  int* i;      // this row's indices [kWideKK]; INT_MAX marks an empty slot
+  // words per row list: KK + 2 = 2 (mod 32), so the 32 lanes of a warp (16 rows) hit 32 different banks
+  static constexpr int kStride = KK + 2;
+  static_assert(KK % 32 == 0 && kStride % 32 == 2, "lists of whole warps, conflict-free rows");
+
+  float* d;    // this row's distances [KK] in shared memory
+  int* i;      // this row's indices [KK]; INT_MAX marks an empty slot
   int half;    // 0 or 1: the parity of the slots this lane owns
   float thr;   // worst kept pair (thr, thi) in slot `worst`
   int thi, worst;
 
   __device__ __forceinline__ void init(float* row_d, int* row_i, int lane_half) {
     d = row_d; i = row_i; half = lane_half;
-    for (int j = half; j < kWideKK; j += 2) { d[j] = __builtin_huge_valf(); i[j] = INT_MAX; }
+    for (int j = half; j < KK; j += 2) { d[j] = __builtin_huge_valf(); i[j] = INT_MAX; }
     thr = __builtin_huge_valf(); thi = INT_MAX; worst = 0;
   }
 
@@ -49,7 +55,7 @@ struct WideList {
     if (!knn_before(dist, col, thr, thi)) return;
     if ((worst & 1) == half) { d[worst] = dist; i[worst] = col; }
     float m = d[half]; int mi = i[half], w = half;
-    for (int j = half + 2; j < kWideKK; j += 2) {
+    for (int j = half + 2; j < KK; j += 2) {
       const float v = d[j]; const int vi = i[j];
       if (knn_before(m, mi, v, vi)) { m = v; mi = vi; w = j; }
     }
@@ -63,7 +69,7 @@ struct WideList {
 
   // This lane's slots to the row's candidate arrays (empty slots as index -1, distance +inf).
   __device__ __forceinline__ void store(int32_t* cand_idx, float* cand_val) const {
-    for (int j = half; j < kWideKK; j += 2) {
+    for (int j = half; j < KK; j += 2) {
       cand_idx[j] = i[j] == INT_MAX ? -1 : i[j];
       cand_val[j] = d[j];
     }

@@ -24,6 +24,8 @@
 //
 // mde_knn_csr_wide (24 < k <= 64): the same preparation; knn_csr_wide_tile_kernel sweeps 64 query rows per CTA and
 // keeps KK = 96 candidates per row in shared memory (mde_knn_select.cuh); the re-rank merges all 96.
+// mde_knn_csr_long (k <= 256): the same kernel with KK = 288 on candidate tiles of 64 rows (one warpgroup); the
+// re-rank merges all 288.
 //
 // mde_pair_dist_csr: ||a - b|| of given pairs by the same sorted merge, fp64, sqrt in fp64, one rounding.
 #include <cub/cub.cuh>
@@ -60,17 +62,24 @@ constexpr int kSmemBytes = kStages * kStageBytes + 1024 /* alignment slack */ + 
                            kTileN * 4 /* norms */ + kChunkWords * 32 * 4 /* visited-block list */;
 static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 
-// wide search (k <= 64): 64 query rows per CTA, running top-96 lists in shared memory
+// wide (k <= 64) and long (k <= 256) searches: 64 query rows per CTA, running top-KK lists in shared memory,
+// candidate tiles of TN = 128 (wide) or 64 (long) rows, one warpgroup per 64 candidates of a tile
 constexpr int kWideTileM = 64;
 constexpr int kAOpBytes = kWideTileM * kRowBytes;              // 8 KB: one 64-row query operand block (hi or lo)
-constexpr int kWideStageBytes = 2 * kAOpBytes + 2 * kOpBytes;  // A hi, A lo, B hi, B lo = 48 KB
-constexpr int kWideBuilders = kWideTileM + kTileN;             // 192: one builder thread per operand row
-constexpr int kWideThreads = 256;                              // two warpgroups, one per 64-candidate half of a tile
-constexpr int kWideSmemBytes = kStages * kWideStageBytes + 1024 /* alignment slack */ +
-                               kWideTileM * kAccStride * 4 + kTileN * 4 /* norms */ +
+constexpr int kLongTileN = 64;
+
+template <int TN>
+constexpr int kWideStageBytes = 2 * kAOpBytes + 2 * TN * kRowBytes;  // A hi, A lo, B hi, B lo
+// The staged accumulators [64][TN + 2] share the stage buffers: the tile's last wgmmas are done before they are
+// written, and the next tile's first operand block is built after the scan.
+template <int KK, int TN>
+constexpr int kWideSmemBytes = kStages * kWideStageBytes<TN> + 1024 /* alignment slack */ + TN * 4 /* norms */ +
                                kChunkWords * 32 * 4 /* visited-block list */ +
-                               kWideTileM * kWideListStride * 8 /* lists */;
-static_assert(kWideSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
+                               kWideTileM * WideList<KK>::kStride * 8 /* lists */;
+// long: the 148.5 KB of lists leave 2 x 32 KB stages of 64-wide candidate tiles (CUB's scan storage is static)
+static_assert(kWideSmemBytes<kWideKK, kTileN> <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
+static_assert(kWideSmemBytes<kLongKK, kLongTileN> + 768 /* CUB scan, 672 B */ <= 227 * 1024,
+              "H100: at most 227 KB of shared memory per block, static storage included");
 
 constexpr float kInf = __builtin_huge_valf();
 
@@ -351,40 +360,51 @@ knn_csr_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __restr
 namespace {
 
 // ---------------------------------------------------------------------------------------------------------------
-// wide tiles (k <= 64): as knn_csr_tile_kernel for 64 query rows, one running top-96 per row in shared memory; the
-// two warpgroups issue wgmma.m64n64k16 on the two halves of the candidate tile
+// wide tiles (k <= 64, KK = 96, TN = 128) and long tiles (k <= 256, KK = 288, TN = 64): as knn_csr_tile_kernel for
+// 64 query rows, one running top-KK per row in shared memory; warpgroup wg issues wgmma.m64n64k16 on candidates
+// 64 wg .. 64 wg + 63 of the tile
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kWideThreads, 1)
+template <int KK, int TN>
+__global__ void __launch_bounds__(2 * TN, 1)
 knn_csr_wide_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
                          const float* __restrict__ vals, const float* __restrict__ norms,
                          const uint32_t* __restrict__ bitmap, int nwords, int64_t n, int num_tiles,
                          int32_t* __restrict__ cand_idx, float* __restrict__ cand_val) {
+  static_assert(TN == 64 || TN == 128, "one or two warpgroups");
+  constexpr int kThreadsT = 2 * TN;                  // one warpgroup per 64 candidates of a tile
+  constexpr int kBuilders = kWideTileM + TN;         // one builder thread per operand row
+  constexpr int kBOpBytes = TN * kRowBytes;
+  constexpr int kStageB = kWideStageBytes<TN>;
+  constexpr int kAccS = TN + 2;
+  constexpr int kStride = WideList<KK>::kStride;
+  static_assert(kWideTileM * kAccS * 4 <= kStages * kStageB, "the staged accumulators fit in the stage buffers");
+  static_assert(kChunkWords <= kThreadsT, "one bitmap word per thread");
   extern __shared__ uint8_t smem_raw[];
-  // carve: [stages x 48 KB, 1024-aligned] | staged accumulators [64][kAccStride] | norms[128] | visited blocks |
-  //        list distances [64][kWideListStride] | list indices [64][kWideListStride]
+  // carve: [stages x kStageB, 1024-aligned; staged accumulators [64][kAccS] at its start between tiles] | norms[TN] |
+  //        visited blocks | list distances [64][kStride] | list indices [64][kStride]
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
-  float* s_acc = reinterpret_cast<float*>(gen + kStages * kWideStageBytes);
-  float* s_norm = s_acc + kWideTileM * kAccStride;
-  int* s_list = reinterpret_cast<int*>(s_norm + kTileN);
+  float* s_acc = reinterpret_cast<float*>(gen);
+  float* s_norm = reinterpret_cast<float*>(gen + kStages * kStageB);
+  int* s_list = reinterpret_cast<int*>(s_norm + TN);
   float* s_ld = reinterpret_cast<float*>(s_list + kChunkWords * 32);
-  int* s_li = reinterpret_cast<int*>(s_ld + kWideTileM * kWideListStride);
-  using Scan = cub::BlockScan<int, kWideThreads>;
+  int* s_li = reinterpret_cast<int*>(s_ld + kWideTileM * kStride);
+  using Scan = cub::BlockScan<int, kThreadsT>;
   __shared__ typename Scan::TempStorage scan_tmp;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int64_t row0 = (int64_t)blockIdx.x * kWideTileM;
-  // the query rows use the bitmap of their 128-row tile: a superset of their own blocks (a block only the other
-  // half of that tile occupies is built with zero query rows and adds exactly 0)
+  // the query rows use the bitmap of their 128-row tile, and so do the candidate rows: a superset of their own
+  // blocks (a block only other rows of that tile occupy is built with zero rows and adds exactly 0)
   const uint32_t* abm = bitmap + (row0 / kTileM) * nwords;
 
   // ----- builder role: thread tid owns operand row tid of A (query rows, tid < 64) or row tid - 64 of B (up to
-  // tid 191); warps 6 and 7 build nothing
-  const bool builder = tid < kWideBuilders;  // (warp-uniform)
+  // tid 64 + TN - 1); with TN = 128, warps 6 and 7 build nothing
+  const bool builder = tid < kBuilders;  // (warp-uniform)
   const bool is_b = tid >= kWideTileM;
   const int orow = is_b ? tid - kWideTileM : tid;
   const uint32_t my_off = (is_b ? 2 * kAOpBytes : 0) + orow * kRowBytes;
-  const uint32_t lo_off = is_b ? kOpBytes : kAOpBytes;  // from the hi block to the lo block of the operand
+  const uint32_t lo_off = is_b ? kBOpBytes : kAOpBytes;  // from the hi block to the lo block of the operand
   const int swz = orow & 7;
   int64_t a_beg = 0, a_end = 0;
   if (!is_b && row0 + orow < n) { a_beg = indptr[row0 + orow]; a_end = indptr[row0 + orow + 1]; }
@@ -396,20 +416,20 @@ knn_csr_wide_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __re
   const int lrow = (tid & 127) >> 1, half = tid & 1;
   const int64_t row = row0 + lrow;
   const int frow = 16 * (warp & 3) + (lane >> 2), fcol = 64 * wg + 2 * (lane & 3);
-  WideList list;
-  if (scanner) list.init(s_ld + lrow * kWideListStride, s_li + lrow * kWideListStride, half);
+  WideList<KK> list;
+  if (scanner) list.init(s_ld + lrow * kStride, s_li + lrow * kStride, half);
   float acc[32];
 
   int stage = 0;
   for (int t = 0; t < num_tiles; ++t) {
     int64_t p = a_beg, end = a_end;
     if (is_b) {
-      const int64_t r = (int64_t)t * kTileN + orow;
+      const int64_t r = (int64_t)t * TN + orow;
       p = end = 0;
       if (builder && r < n) { p = indptr[r]; end = indptr[r + 1]; }
     }
     int cur = p < end ? cols[p] : INT_MAX;
-    const uint32_t* bbm = bitmap + (int64_t)t * nwords;
+    const uint32_t* bbm = bitmap + ((int64_t)t * TN / kTileM) * nwords;
 #pragma unroll
     for (int i = 0; i < 32; ++i) acc[i] = 0.0f;
 
@@ -425,7 +445,7 @@ knn_csr_wide_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __re
         const int lo = s_list[i] * kBlockK, hi = lo + kBlockK;
         // the stage was last read by the wgmmas of block i - 2, which the consumers waited for before the barrier
         // of block i - 1
-        uint8_t* rh = gen + stage * kWideStageBytes + my_off;
+        uint8_t* rh = gen + stage * kStageB + my_off;
         if (builder) {
 #pragma unroll
           for (int c = 0; c < 8; ++c) {
@@ -449,10 +469,10 @@ knn_csr_wide_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __re
         fence_proxy_async();  // generic-proxy stores above, read next by wgmma (async proxy)
         wgmma_wait_all();     // this warpgroup's wgmmas of block i - 1 are done with the other stage
         __syncthreads();
-        const uint32_t sa = base + stage * kWideStageBytes;
+        const uint32_t sa = base + stage * kStageB;
         const uint64_t ah = smem_desc_sw128(sa), al = smem_desc_sw128(sa + kAOpBytes);
         const uint64_t bh = smem_desc_sw128(sa + 2 * kAOpBytes + wg * 64 * kRowBytes);
-        const uint64_t bl = smem_desc_sw128(sa + 2 * kAOpBytes + kOpBytes + wg * 64 * kRowBytes);
+        const uint64_t bl = smem_desc_sw128(sa + 2 * kAOpBytes + kBOpBytes + wg * 64 * kRowBytes);
 #pragma unroll
         for (int q = 0; q < 32; ++q) fence_operand(acc[q]);
         wgmma_fence();
@@ -470,48 +490,50 @@ knn_csr_wide_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __re
     wgmma_wait_all();
 #pragma unroll
     for (int q = 0; q < 32; ++q) fence_operand(acc[q]);
+    __syncthreads();  // every warpgroup's wgmmas are done with the stage buffers that take the accumulators
 #pragma unroll
     for (int j = 0; j < 64 / 8; ++j) {
-      *reinterpret_cast<float2*>(s_acc + frow * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
-      *reinterpret_cast<float2*>(s_acc + (frow + 8) * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      *reinterpret_cast<float2*>(s_acc + frow * kAccS + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(s_acc + (frow + 8) * kAccS + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
     }
-    if (tid < kTileN) s_norm[tid] = __ldg(norms + (int64_t)t * kTileN + tid);
+    if (tid < TN) s_norm[tid] = __ldg(norms + (int64_t)t * TN + tid);
     __syncthreads();
     if (scanner) {
       // both lanes of the row offer every column, in column order
-      const float2* arow = reinterpret_cast<const float2*>(s_acc + lrow * kAccStride);
+      const float2* arow = reinterpret_cast<const float2*>(s_acc + lrow * kAccS);
       const float2* sn = reinterpret_cast<const float2*>(s_norm);
 #pragma unroll 2
-      for (int i = 0; i < kTileN / 2; ++i) {
+      for (int i = 0; i < TN / 2; ++i) {
         const float2 a = arow[i], s = sn[i];
-        const int col = t * kTileN + 2 * i;
+        const int col = t * TN + 2 * i;
         if (col != row && col < n) list.offer(fmaf(-2.0f, a.x, s.x), col);
         if (col + 1 != row && col + 1 < n) list.offer(fmaf(-2.0f, a.y, s.y), col + 1);
       }
     }
   }
-  if (scanner && row < n) list.store(cand_idx + row * kWideKK, cand_val + row * kWideKK);
+  if (scanner && row < n) list.store(cand_idx + row * KK, cand_val + row * KK);
 }
 
 }  // namespace
 
 namespace mde {
 
-// One warp per row, lane q re-ranks candidates q, q + 32 and q + 64 by the merge of knn_csr_rerank_kernel; the k
-// smallest (distance, index) of the 96 in ascending order.
-__global__ void __launch_bounds__(256)
-knn_csr_wide_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
-                           const float* __restrict__ vals, int64_t n, const int32_t* __restrict__ cand_idx, int k,
-                           int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+// One warp per row, lane q re-ranks candidates q, q + 32, q + 64, ... by the merge of knn_csr_rerank_kernel; the k
+// smallest (distance, index) of the KK in ascending order.
+template <int KK>
+__device__ __forceinline__ void csr_wide_rerank_row(const int64_t* __restrict__ indptr,
+                                                    const int32_t* __restrict__ cols, const float* __restrict__ vals,
+                                                    int64_t n, const int32_t* __restrict__ cand_idx, int k,
+                                                    int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= n) return;
-  constexpr int kPer = kWideKK / 32;
+  constexpr int kPer = KK / 32;
   float my_d[kPer];
   int mine[kPer];
 #pragma unroll
   for (int s = 0; s < kPer; ++s) {
-    const int c = cand_idx[row * kWideKK + 32 * s + lane];
+    const int c = cand_idx[row * KK + 32 * s + lane];
     my_d[s] = c >= 0 ? (float)merge_dist2(indptr, cols, vals, row, c) : kInf;
     mine[s] = c >= 0 ? c : INT_MAX;  // missing candidates last
   }
@@ -532,6 +554,21 @@ knn_csr_wide_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __
       out_d2[row * k + rank[s]] = my_d[s];
     }
   }
+}
+
+__global__ void __launch_bounds__(256)
+knn_csr_wide_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
+                           const float* __restrict__ vals, int64_t n, const int32_t* __restrict__ cand_idx, int k,
+                           int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+  csr_wide_rerank_row<kWideKK>(indptr, cols, vals, n, cand_idx, k, out_idx, out_d2);
+}
+
+// the 288 candidates of the long search, with the same merge
+__global__ void __launch_bounds__(256)
+knn_csr_long_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
+                           const float* __restrict__ vals, int64_t n, const int32_t* __restrict__ cand_idx, int k,
+                           int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+  csr_wide_rerank_row<kLongKK>(indptr, cols, vals, n, cand_idx, k, out_idx, out_d2);
 }
 
 }  // namespace mde
@@ -669,6 +706,60 @@ int prepare_csr(const int64_t* indptr, const int32_t* indices, const float* valu
 
 }  // namespace mde
 
+namespace {
+
+int csr_wide_ws_bytes(int64_t n, int d, int64_t nnz, int kk, size_t* bytes) {
+  if (!bytes || n < 2 || d < 1 || nnz < 0) return MDE_E_INVALID;
+  CsrKnnLayout L;
+  int rc = csr_knn_layout(n, d, nnz, &L, kk);
+  if (rc) return rc;
+  *bytes = L.total;
+  return 0;
+}
+
+// mde_knn_csr_wide (KK = 96, TN = 128) and mde_knn_csr_long (KK = 288, TN = 64): prep, tiles, re-rank of all KK.
+template <int KK, int TN>
+int run_csr_wide(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
+                 int k, int max_k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream) {
+  if (!indptr || !idx_out || !d2_out || !ws || n < 2 || d < 1 || nnz < 0 || k < 1 || k > max_k || k > n - 1)
+    return MDE_E_INVALID;
+  if (nnz > 0 && (!indices || !values)) return MDE_E_INVALID;
+  if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
+  CsrKnnLayout L;
+  int rc = csr_knn_layout(n, d, nnz, &L, KK);
+  if (rc) return rc;
+  if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* w = static_cast<uint8_t*>(ws);
+  if ((rc = prepare_csr(indptr, indices, values, n, d, nnz, L, w, st))) return rc;
+  const float* norms = reinterpret_cast<const float*>(w + L.off_norm);
+  int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
+  float* cv = reinterpret_cast<float*>(w + L.off_cv);
+  const uint32_t* bm = reinterpret_cast<const uint32_t*>(w + L.off_bm);
+  const int32_t* cols = reinterpret_cast<const int32_t*>(w + L.off_kin);
+  const float* vals = reinterpret_cast<const float*>(w + L.off_val);
+  constexpr int kSmem = kWideSmemBytes<KK, TN>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    MDE_CUDA_TRY(cudaFuncSetAttribute(knn_csr_wide_tile_kernel<KK, TN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      kSmem));
+    attr_set = true;
+  }
+  const unsigned grid = (unsigned)((n + kWideTileM - 1) / kWideTileM);
+  const int num_tiles = (int)(L.n_pad / TN);
+  knn_csr_wide_tile_kernel<KK, TN><<<grid, 2 * TN, kSmem, st>>>(indptr, cols, vals, norms, bm, L.nwords, n, num_tiles,
+                                                                ci, cv);
+  MDE_LAUNCH_CHECK();
+  if constexpr (KK == kWideKK)
+    knn_csr_wide_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(indptr, cols, vals, n, ci, k, idx_out, d2_out);
+  else
+    knn_csr_long_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(indptr, cols, vals, n, ci, k, idx_out, d2_out);
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // namespace
+
 extern "C" {
 
 int mde_knn_csr_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes) {
@@ -713,46 +804,23 @@ int mde_knn_csr(const int64_t* indptr, const int32_t* indices, const float* valu
 }
 
 int mde_knn_csr_wide_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes) {
-  if (!bytes || n < 2 || d < 1 || nnz < 0) return MDE_E_INVALID;
-  CsrKnnLayout L;
-  int rc = csr_knn_layout(n, d, nnz, &L, kWideKK);
-  if (rc) return rc;
-  *bytes = L.total;
-  return 0;
+  return csr_wide_ws_bytes(n, d, nnz, kWideKK, bytes);
 }
 
 int mde_knn_csr_wide(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                      int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream) {
-  if (!indptr || !idx_out || !d2_out || !ws || n < 2 || d < 1 || nnz < 0 || k < 1 || k > kWideMaxK || k > n - 1)
-    return MDE_E_INVALID;
-  if (nnz > 0 && (!indices || !values)) return MDE_E_INVALID;
-  if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
-  CsrKnnLayout L;
-  int rc = csr_knn_layout(n, d, nnz, &L, kWideKK);
-  if (rc) return rc;
-  if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream;
-  uint8_t* w = static_cast<uint8_t*>(ws);
-  if ((rc = prepare_csr(indptr, indices, values, n, d, nnz, L, w, st))) return rc;
-  const float* norms = reinterpret_cast<const float*>(w + L.off_norm);
-  int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
-  float* cv = reinterpret_cast<float*>(w + L.off_cv);
-  const uint32_t* bm = reinterpret_cast<const uint32_t*>(w + L.off_bm);
-  const int32_t* cols = reinterpret_cast<const int32_t*>(w + L.off_kin);
-  const float* vals = reinterpret_cast<const float*>(w + L.off_val);
-  static bool attr_set = false;
-  if (!attr_set) {
-    MDE_CUDA_TRY(cudaFuncSetAttribute(knn_csr_wide_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      kWideSmemBytes));
-    attr_set = true;
-  }
-  const unsigned grid = (unsigned)((n + kWideTileM - 1) / kWideTileM);
-  knn_csr_wide_tile_kernel<<<grid, kWideThreads, kWideSmemBytes, st>>>(indptr, cols, vals, norms, bm, L.nwords, n,
-                                                                        L.num_tiles, ci, cv);
-  MDE_LAUNCH_CHECK();
-  knn_csr_wide_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(indptr, cols, vals, n, ci, k, idx_out, d2_out);
-  MDE_LAUNCH_CHECK();
-  return 0;
+  return run_csr_wide<kWideKK, kTileN>(indptr, indices, values, n, d, nnz, k, kWideMaxK, idx_out, d2_out, ws, ws_bytes,
+                                       stream);
+}
+
+int mde_knn_csr_long_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes) {
+  return csr_wide_ws_bytes(n, d, nnz, kLongKK, bytes);
+}
+
+int mde_knn_csr_long(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                     int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream) {
+  return run_csr_wide<kLongKK, kLongTileN>(indptr, indices, values, n, d, nnz, k, kLongMaxK, idx_out, d2_out, ws,
+                                           ws_bytes, stream);
 }
 
 int mde_pair_dist_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,

@@ -1,17 +1,19 @@
 """Problem construction from a data matrix (interface of pymde/preprocess/data_matrix.py).
 
 k-nearest neighbours are computed EXACTLY on the GPU by the library's own kernels (`mde_knn`: wgmma tensor-core
-cross terms with a running top-32 per row and an exact fp32 re-rank, csrc/mde_knn.cu) for k <= 24, and by their wide
+cross terms with a running top-32 per row and an exact fp32 re-rank, csrc/mde_knn.cu) for k <= 24, by their wide
 variants (`mde_knn_wide`: a running top-96 per row in shared memory) for 24 < k <= 64; larger k uses row chunks of a
-library GEMM + top-k.  The reference uses scikit-learn brute force below 10 000 rows and the approximate pynndescent
+library GEMM + top-k, which measured faster than the long variant (`mde_knn_long`: a running top-288 per row, for
+k <= 256) on 70 000 x 784 at every k from 65 to 256 (DESIGN section 11.6).  The reference uses scikit-learn brute force below 10 000 rows and the approximate pynndescent
 above (data_matrix.py:125-143).  `PYMDE_B200_KNN=approx` opts in to an approximate search of dense input for k <= 64
 (`mde_knn_approx`: NN-descent, csrc/mde_knn_approx.cu), whose cost grows about linearly in n; it returns k rows
 found by the search, not necessarily the k nearest.  It pays off for large n at large d: at 10^6 rows and d = 50 the
-exact search is faster (DESIGN section 11.3).  `PYMDE_B200_KNN=approx` leaves sparse input on the exact searches.  A
-scipy.sparse matrix is searched without densifying it for k <= 64 (`mde_knn_csr`, `mde_knn_csr_wide`,
-csrc/mde_knn_sparse.cu), and its pair distances come from sorted merges of CSR rows (`mde_pair_dist_csr`).
-`PYMDE_B200_KNN_SPARSE=approx` opts in to NN-descent over the CSR rows for k <= 64 (`mde_knn_approx_csr`,
-csrc/mde_knn_approx.cu), with the distances of the exact sparse search (DESIGN section 11.4)."""
+exact search is faster (DESIGN section 11.3).  `PYMDE_B200_KNN=approx` leaves sparse input on the exact searches; for
+64 < k <= 256 it takes the exact `mde_knn_long`.  A scipy.sparse matrix is searched without densifying it for k <= 256
+(`mde_knn_csr`, `mde_knn_csr_wide`, `mde_knn_csr_long`, csrc/mde_knn_sparse.cu), and its pair distances come from
+sorted merges of CSR rows (`mde_pair_dist_csr`).  `PYMDE_B200_KNN_SPARSE=approx` opts in to NN-descent over the CSR
+rows for k <= 64 (`mde_knn_approx_csr`, csrc/mde_knn_approx.cu), with the distances of the exact sparse search
+(DESIGN section 11.4); a k above 64 takes the exact long search."""
 import ctypes as C
 import os
 
@@ -45,13 +47,16 @@ def _to_device_csr(data, device):
 
 def knn_sparse_device(csr, shape, k):
     """(indices [n, k] int32, squared distances [n, k] fp32) of the k nearest rows of every row of a device CSR
-    matrix from `_to_device_csr`, ascending by (distance, index); the kernel behind `mde_knn_csr` for k <= 24 and
-    `mde_knn_csr_wide` for 24 < k <= 64 (include/mde_b200.h)."""
+    matrix from `_to_device_csr`, ascending by (distance, index); the kernel behind `mde_knn_csr` for k <= 24,
+    `mde_knn_csr_wide` for 24 < k <= 64 and `mde_knn_csr_long` for 64 < k <= 256 (include/mde_b200.h)."""
     from .. import _lib
     lib = _lib.load()
-    wide = k > lib.mde_knn_max_k()
-    ws_bytes, search = ((lib.mde_knn_csr_wide_ws_bytes, lib.mde_knn_csr_wide) if wide
-                        else (lib.mde_knn_csr_ws_bytes, lib.mde_knn_csr))
+    if k > lib.mde_knn_wide_max_k():
+        ws_bytes, search = lib.mde_knn_csr_long_ws_bytes, lib.mde_knn_csr_long
+    elif k > lib.mde_knn_max_k():
+        ws_bytes, search = lib.mde_knn_csr_wide_ws_bytes, lib.mde_knn_csr_wide
+    else:
+        ws_bytes, search = lib.mde_knn_csr_ws_bytes, lib.mde_knn_csr
     indptr, indices, values = csr
     n, d = shape
     nnz = int(indices.shape[0])
@@ -122,12 +127,16 @@ def _knn_graph(idx, d2, n, max_distance, dev):
 
 def knn_device(X, k):
     """(indices [n, k] int32, squared distances [n, k] fp32) of the k nearest rows of every row of the CUDA fp32
-    matrix X, ascending; the wgmma kernel behind `mde_knn` for k <= 24 and `mde_knn_wide` for 24 < k <= 64
-    (include/mde_b200.h)."""
+    matrix X, ascending; the wgmma kernel behind `mde_knn` for k <= 24, `mde_knn_wide` for 24 < k <= 64 and
+    `mde_knn_long` for 64 < k <= 256 (include/mde_b200.h)."""
     from .. import _lib
     lib = _lib.load()
-    wide = k > lib.mde_knn_max_k()
-    ws_bytes, search = (lib.mde_knn_wide_ws_bytes, lib.mde_knn_wide) if wide else (lib.mde_knn_ws_bytes, lib.mde_knn)
+    if k > lib.mde_knn_wide_max_k():
+        ws_bytes, search = lib.mde_knn_long_ws_bytes, lib.mde_knn_long
+    elif k > lib.mde_knn_max_k():
+        ws_bytes, search = lib.mde_knn_wide_ws_bytes, lib.mde_knn_wide
+    else:
+        ws_bytes, search = lib.mde_knn_ws_bytes, lib.mde_knn
     X = X.contiguous()
     n, d = X.shape
     need = C.c_size_t(0)
@@ -172,17 +181,20 @@ def knn_approx_device(X, k, seed=None):
 def _search(data, k, dev, chunk_rows=None):
     """The neighbour search of `k_nearest_neighbors`: (idx [n, k'], squared distances [n, k'] fp32, n) of the
     k' = min(k, n - 1) nearest rows of every row, from the search kernels (int32 indices), or from row chunks of a
-    library GEMM + top-k (int64 indices) for k' > 64, `chunk_rows` or PYMDE_B200_KNN=gemm."""
+    library GEMM + top-k (int64 indices) for k' > 256, dense input with 64 < k' <= 256 (unless PYMDE_B200_KNN=approx),
+    `chunk_rows` or PYMDE_B200_KNN=gemm."""
     from .. import _lib
+    lib = _lib.load()
     mode = os.environ.get("PYMDE_B200_KNN", "kernel")
     use_kernel = chunk_rows is None and mode != "gemm"
     if sp.issparse(data):
         n = data.shape[0]
         k = int(min(k, n - 1))
-        if use_kernel and 1 <= k <= _lib.load().mde_knn_wide_max_k():
+        if use_kernel and 1 <= k <= lib.mde_knn_long_max_k():
             csr, shape = _to_device_csr(data, dev)
             # PYMDE_B200_KNN=approx does not reach here: sparse input has its own opt-in
-            if os.environ.get("PYMDE_B200_KNN_SPARSE") == "approx":
+            # NN-descent covers k <= 64; above that PYMDE_B200_KNN_SPARSE=approx takes the exact long search
+            if os.environ.get("PYMDE_B200_KNN_SPARSE") == "approx" and k <= lib.mde_knn_approx_max_k():
                 idx, d2 = knn_approx_sparse_device(csr, shape, k)
             else:
                 idx, d2 = knn_sparse_device(csr, shape, k)
@@ -190,9 +202,14 @@ def _search(data, k, dev, chunk_rows=None):
     X = _to_device_matrix(data, dev)
     n = X.shape[0]
     k = int(min(k, n - 1))
-    if use_kernel and 1 <= k <= _lib.load().mde_knn_wide_max_k():
+    if use_kernel and 1 <= k <= lib.mde_knn_wide_max_k():
         # "approx" applies to dense input only: scipy.sparse input keeps the exact sparse searches above
         idx, d2 = knn_approx_device(X, k) if mode == "approx" else knn_device(X, k)
+        return idx, d2, n
+    if use_kernel and mode == "approx" and k <= lib.mde_knn_long_max_k():
+        # above NN-descent's k the opt-in takes the exact long search (mde_knn_long); by default 64 < k <= 256 stays
+        # on the GEMM path below, which measured faster on 70 000 x 784 at k = 65 .. 256 (DESIGN section 11.6)
+        idx, d2 = knn_device(X, k)
         return idx, d2, n
     sq = (X * X).sum(1)
     rows = chunk_rows or max(256, min(n, int(2 ** 27 // max(n, 1))))
@@ -213,17 +230,34 @@ def k_nearest_neighbors(data, k, max_distance=None, verbose=False, device=None, 
     return _knn_graph(idx, d2, n, max_distance, dev)
 
 
-def k_nearest_neighbors_device(data, k, max_distance=None, device=None):
-    """The graph of `k_nearest_neighbors` -- same search, same edges and weights -- assembled on the device from the
-    neighbour lists (`graph.knn_edge_list`) and returned as an `EdgeListGraph` there.  The lists of the search
-    kernels and of PYMDE_B200_KNN=gemm qualify when min(k, n - 1) <= 64; larger k raises ValueError (use
-    `k_nearest_neighbors`, which builds the host Graph)."""
+def _device_knn_graph(data, k, max_distance, device, max_k):
+    """`k_nearest_neighbors`' graph assembled on the device; ValueError when min(k, n - 1) > max_k."""
     from .graph import knn_edge_list
+    n = data.shape[0]
+    if min(k, n - 1) > max_k:
+        raise ValueError("min(k, n - 1) must be at most %d (use k_nearest_neighbors, which builds the host Graph)"
+                         % max_k)
     dev = util.cuda_device(device)
     idx, d2, n = _search(data, k, dev)
     if max_distance is not None:
         idx = torch.where(d2.sqrt() <= max_distance, idx, -1)  # (a NaN distance is dropped, as in _knn_graph)
     return knn_edge_list(idx, n)
+
+
+def k_nearest_neighbors_device(data, k, max_distance=None, device=None):
+    """The graph of `k_nearest_neighbors` -- same search, same edges and weights -- assembled on the device from the
+    neighbour lists (`graph.knn_edge_list`) and returned as an `EdgeListGraph` there.  The lists of the search
+    kernels and of PYMDE_B200_KNN=gemm qualify when min(k, n - 1) <= 64; larger k raises ValueError (use
+    `k_nearest_neighbors_device_long` up to 256, or `k_nearest_neighbors`, which builds the host Graph)."""
+    from .. import _lib
+    return _device_knn_graph(data, k, max_distance, device, int(_lib.load().mde_knn_graph_max_k()))
+
+
+def k_nearest_neighbors_device_long(data, k, max_distance=None, device=None):
+    """`k_nearest_neighbors_device` for min(k, n - 1) <= 256 (`mde_knn_graph_long_max_k()`); larger k raises
+    ValueError."""
+    from .. import _lib
+    return _device_knn_graph(data, k, max_distance, device, int(_lib.load().mde_knn_graph_long_max_k()))
 
 
 def _pair_distances(data, retain_fraction, dev):

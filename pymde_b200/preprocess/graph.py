@@ -274,10 +274,10 @@ def k_nearest_neighbors_device(graph, k, max_distance=None, device=None):
 
 
 def knn_edge_list(idx, n):
-    """`EdgeListGraph` of the neighbour lists idx [n, k] (device int32, -1 = no entry, 1 <= k <= 64) on their
+    """`EdgeListGraph` of the neighbour lists idx [n, k] (device int32, -1 = no entry, 1 <= k <= 256) on their
     device: the edges and weights `Graph.from_edges` gives for the directed pairs (i, idx[i, s]) -- every unordered
     pair once as (i, j), i < j, sorted by (i, j), weighted by the number of entries i -> j and j -> i
-    (`mde_knn_graph_count` / `mde_knn_graph_emit`, include/mde_b200.h).  An entry equal to its own row or outside
+    (`mde_knn_graph_long_count` / `mde_knn_graph_long_emit`, include/mde_b200.h).  An entry equal to its own row or outside
     [-1, n) raises ValueError, as `Graph` does for a self edge."""
     import ctypes as C
     from .. import _lib
@@ -287,17 +287,17 @@ def knn_edge_list(idx, n):
     if idx.dim() != 2 or idx.shape[0] != n:
         raise ValueError("neighbour lists must have shape (n, k)")
     k = int(idx.shape[1])
-    if not 1 <= k <= int(lib.mde_knn_graph_max_k()):
-        raise ValueError("k must be between 1 and %d" % int(lib.mde_knn_graph_max_k()))
+    if not 1 <= k <= int(lib.mde_knn_graph_long_max_k()):
+        raise ValueError("k must be between 1 and %d" % int(lib.mde_knn_graph_long_max_k()))
     dev = idx.device
     need = C.c_size_t(0)
-    _lib.check(lib.mde_knn_graph_ws_bytes(n, k, C.byref(need)))
+    _lib.check(lib.mde_knn_graph_long_ws_bytes(n, k, C.byref(need)))
     ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=dev)
     off = (-ws.data_ptr()) % 1024
     count = C.c_int64(0)
     with torch.cuda.device(dev):
         stream = torch.cuda.current_stream().cuda_stream
-        code = lib.mde_knn_graph_count(idx.data_ptr(), n, k, ws.data_ptr() + off, need.value, C.byref(count), stream)
+        code = lib.mde_knn_graph_long_count(idx.data_ptr(), n, k, ws.data_ptr() + off, need.value, C.byref(count), stream)
         if code == _lib.MDE_E_INVALID:
             raise ValueError("neighbour lists must hold row indices in [0, n) other than the row itself, or -1")
         _lib.check(code)
@@ -305,7 +305,7 @@ def knn_edge_list(idx, n):
         edges = torch.empty((p, 2), dtype=torch.int64, device=dev)
         weights = torch.empty(p, dtype=torch.float32, device=dev)
         if p:
-            _lib.check(lib.mde_knn_graph_emit(n, k, ws.data_ptr() + off, need.value, edges.data_ptr(),
+            _lib.check(lib.mde_knn_graph_long_emit(n, k, ws.data_ptr() + off, need.value, edges.data_ptr(),
                                               weights.data_ptr(), stream))
         torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
     return EdgeListGraph(edges, weights, n)

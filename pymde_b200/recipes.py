@@ -20,7 +20,11 @@ def _remove_anchor_anchor_edges(edges, data, anchors):
     return edges[~both], data[~both]
 
 
-_KNN_GRAPH_MAX_K = 64  # mde_knn_graph_max_k(): longer neighbour lists are assembled into a host Graph
+def _knn_graph_max_k(long=False):
+    """mde_knn_graph_max_k(), or mde_knn_graph_long_max_k(): longer neighbour lists are assembled into a host Graph."""
+    from . import _lib
+    lib = _lib.load()
+    return int(lib.mde_knn_graph_long_max_k() if long else lib.mde_knn_graph_max_k())
 
 
 def preserve_distances(data, embedding_dim=2, loss=losses.Absolute, constraint=None, max_distances=5e7,
@@ -52,8 +56,9 @@ def preserve_neighbors(data, embedding_dim=2, attractive_penalty=penalties.Log1p
                        constraint=None, n_neighbors=None, repulsive_fraction=None, max_distance=None,
                        init="quadratic", device=None, verbose=False):
     """MDE problem preserving local structure (pymde/recipes.py:221-448).  For a data matrix the neighbour graph is
-    assembled on the device from the search's lists (`data_matrix.k_nearest_neighbors_device`) when
-    min(n_neighbors, n - 1) <= 64; larger n_neighbors keep the chunked GEMM search and the host `Graph`."""
+    assembled on the device from the search's lists (`data_matrix.k_nearest_neighbors_device`, or
+    `k_nearest_neighbors_device_long` above 64) when min(n_neighbors, n - 1) <= 256; larger n_neighbors keep the
+    chunked GEMM search and the host `Graph`."""
     dev = util.cuda_device(device)
     if isinstance(data, Graph):
         n = data.n_items
@@ -74,12 +79,14 @@ def preserve_neighbors(data, embedding_dim=2, attractive_penalty=penalties.Log1p
     if verbose:
         problem.LOGGER.info("Computing %d-nearest neighbors, with max_distance=%s" % (n_neighbors, max_distance))
 
-    if isinstance(data, Graph) or min(n_neighbors, n - 1) > _KNN_GRAPH_MAX_K:
+    k = min(n_neighbors, n - 1)
+    if isinstance(data, Graph) or k > _knn_graph_max_k(long=True):
         knn = preprocess.k_nearest_neighbors(data, k=n_neighbors, max_distance=max_distance, verbose=verbose,
                                              device=dev)
     else:
-        knn = preprocess.data_matrix.k_nearest_neighbors_device(data, n_neighbors, max_distance=max_distance,
-                                                                device=dev)
+        dm = preprocess.data_matrix
+        build = dm.k_nearest_neighbors_device if k <= _knn_graph_max_k() else dm.k_nearest_neighbors_device_long
+        knn = build(data, n_neighbors, max_distance=max_distance, device=dev)
     edges = knn.edges.to(dev)
     weights = knn.weights.to(dev)
     if isinstance(constraint, constraints.Anchored):
