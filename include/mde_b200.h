@@ -14,7 +14,8 @@
  *    caller's int64 edge list;
  *  - `stream` is a cudaStream_t passed as void*; all work is enqueued on it and no call
  *    synchronises the device unless documented ("blocking");
- *  - matrices are row-major contiguous float32: X[n_items][m].
+ *  - matrices are row-major contiguous float32: X[n_items][m] (the mde_knn16* searches also read
+ *    16-bit data matrices, tagged with an MDE_DTYPE_* code).
  */
 #ifndef MDE_B200_H
 #define MDE_B200_H
@@ -397,6 +398,36 @@ int mde_knn_approx(const float* X, int64_t n, int d, int k, uint64_t seed, int32
                    size_t ws_bytes, void* stream);
 int mde_knn_approx_ex(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out, float* d2_out,
                       void* ws, size_t ws_bytes, void* stream, int* iterations);
+
+/* The dense searches on a 16-bit data matrix, read in place: `X` is a device row-major n x d matrix of IEEE fp16
+ * (`dtype` = MDE_DTYPE_FP16) or bf16 (MDE_DTYPE_BF16) values; any other code is MDE_E_INVALID, checked with the other
+ * arguments before any CUDA call.  mde_knn16, mde_knn16_wide, mde_knn16_long and mde_knn16_approx(_ex) take the
+ * arguments, bounds on k, return codes, blocking behaviour and output contract of mde_knn, mde_knn_wide, mde_knn_long
+ * and mde_knn_approx(_ex), and give the bits those give on the fp32 matrix X.float(): the re-rank and NN-descent
+ * convert every element to fp32 as they read it and keep the fp32 arithmetic.  The exact searches' operand is X itself
+ * (one wgmma per 16 features, bf16 x bf16 or fp16 x fp16, against three for the bf16 hi / lo split of fp32 input); a
+ * bf16 value's lo part is exactly zero, so bf16 input gives the fp32 route's candidate lists, and fp16 input gives
+ * them up to rounding of the cross terms, so the results are equal unless more rows than the list's spare slots lie
+ * within that rounding of the k-th distance.  `ws`: 1024-byte aligned device scratch of mde_knn16_ws_bytes(n, d),
+ * mde_knn16_wide_ws_bytes(n, d), mde_knn16_long_ws_bytes(n, d) (2 n_pad k_pad bytes less than the fp32 searches,
+ * n_pad = n rounded up to 128, k_pad = d rounded up to 64: no lo operand) or mde_knn16_approx_ws_bytes(n, d, k) (that
+ * of mde_knn_approx: NN-descent keeps no copy of X) bytes.  Nothing n x d sized in fp32 is allocated. */
+#define MDE_DTYPE_FP16 1
+#define MDE_DTYPE_BF16 2
+int mde_knn16_ws_bytes(int64_t n, int d, size_t* bytes);
+int mde_knn16(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+              size_t ws_bytes, void* stream);
+int mde_knn16_wide_ws_bytes(int64_t n, int d, size_t* bytes);
+int mde_knn16_wide(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                   size_t ws_bytes, void* stream);
+int mde_knn16_long_ws_bytes(int64_t n, int d, size_t* bytes);
+int mde_knn16_long(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                   size_t ws_bytes, void* stream);
+int mde_knn16_approx_ws_bytes(int64_t n, int d, int k, size_t* bytes);
+int mde_knn16_approx(const void* X, int dtype, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out,
+                     float* d2_out, void* ws, size_t ws_bytes, void* stream);
+int mde_knn16_approx_ex(const void* X, int dtype, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out,
+                        float* d2_out, void* ws, size_t ws_bytes, void* stream, int* iterations);
 /* The same NN-descent search on a sparse data matrix, without densifying it.  Input contract of mde_knn_csr (the
  * device CSR check included: MDE_E_INVALID when malformed); output contract of mde_knn_approx, with the distances of
  * mde_knn_csr / mde_knn_csr_wide: the exact squared distance summed in fp64 and rounded once to fp32, which is also

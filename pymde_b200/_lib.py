@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libmde_b200.so")
 MDE_E_INVALID, MDE_E_UNSUPPORTED, MDE_E_NAN, MDE_E_ALLOC, MDE_E_COMM = -1, -2, -3, -4, -5
 IPC_HANDLE_BYTES = 64
 CONSTRAINT_CENTERED, CONSTRAINT_STANDARDIZED, CONSTRAINT_ANCHORED, CONSTRAINT_CUSTOM = 0, 1, 2, 3
+DTYPE_FP16, DTYPE_BF16 = 1, 2  # MDE_DTYPE_* element codes of the mde_knn16* searches
 
 
 class MdeError(RuntimeError):
@@ -137,6 +138,20 @@ SIGNATURES = {
                                  C.c_void_p, C.c_size_t, C.c_void_p]),
     "mde_knn_approx_ex": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
+    "mde_knn16_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn16": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                            C.c_size_t, C.c_void_p]),
+    "mde_knn16_wide_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn16_wide": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn16_long_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn16_long": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn16_approx_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn16_approx": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn16_approx_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_void_p,
+                                      C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
     "mde_knn_approx_csr_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn_approx_csr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int,
                                      C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

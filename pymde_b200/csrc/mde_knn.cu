@@ -23,12 +23,24 @@
 // re-ranks all 96 with the arithmetic above.  mde_knn_long (k <= 256) is the same kernel with KK = 288 and candidate
 // tiles of 64 (wgmma.m64n64k16), so that its lists fit in shared memory; knn_long_rerank_kernel re-ranks all 288.
 //
+// 16-bit input (mde_knn16, mde_knn16_wide, mde_knn16_long: IEEE fp16 or bf16, read without an fp32 copy).  The element
+// type T is a template parameter of every kernel above.  The prep copies X into a zero-padded operand of its own type
+// (no lo part) and writes the norms with the arithmetic of the fp32 prep on the upcast values; the tile kernels issue
+// one wgmma per k16 step, bf16 x bf16 or fp16 x fp16, on the stage layout and barrier protocol of the fp32 route with
+// the lo slots left empty; the re-rank converts each element to fp32 as it reads it.  For bf16 input the lo operand of
+// the fp32 route is exactly zero, so its two extra products add exact zeros and the candidate lists are the same; an
+// fp16 product is exact in fp32, so the cross terms differ from the split's by rounding alone, and the re-rank of the
+// unchanged arithmetic gives the bits of the fp32 route on X.float() (near-ties at the list's edge aside, DESIGN
+// section 11.7).
+//
 // Hangs are not an option on a shared GPU: every mbarrier wait is bounded (mde_tma.cuh) and traps.
 #include <cuda.h>  // CUtensorMap and its enums (types only: the encoder is fetched with cudaGetDriverEntryPoint)
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 
 #include <cstdint>
 #include <cstdlib>
+#include <type_traits>
 
 #include "mde_common.cuh"
 #include "mde_knn_select.cuh"
@@ -92,22 +104,67 @@ __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 
+// The tensor-core operand of an element type: fp32 is split into bf16 hi and lo parts (three products per k16 step),
+// a 16-bit element is its own operand (one product).
+template <class T>
+struct Operand {
+  using type = __nv_bfloat16;
+  static constexpr bool kSplit = true;
+  static constexpr CUtensorMapDataType kMapType = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+};
+template <>
+struct Operand<__nv_bfloat16> {
+  using type = __nv_bfloat16;
+  static constexpr bool kSplit = false;
+  static constexpr CUtensorMapDataType kMapType = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+};
+template <>
+struct Operand<__half> {
+  using type = __half;
+  static constexpr bool kSplit = false;
+  static constexpr CUtensorMapDataType kMapType = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+};
+template <class T>
+using OpT = typename Operand<T>::type;
+
+// One k16 step of the cross terms of 64 query rows and TN candidates, D (+)= Ah Bh^T (+ Ah Bl^T + Al Bh^T for fp32).
+template <class T, int TN>
+__device__ __forceinline__ void cross_step(float (&acc)[TN / 2], uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl,
+                                           uint32_t accumulate) {
+  if constexpr (std::is_same_v<T, __half>) {
+    if constexpr (TN == 128) wgmma_f16(acc, ah, bh, accumulate);
+    else wgmma_f16_n64(acc, ah, bh, accumulate);
+  } else if constexpr (TN == 128) {
+    wgmma_bf16(acc, ah, bh, accumulate);
+    if constexpr (Operand<T>::kSplit) { wgmma_bf16(acc, ah, bl, 1u); wgmma_bf16(acc, al, bh, 1u); }
+  } else {
+    wgmma_bf16_n64(acc, ah, bh, accumulate);
+    if constexpr (Operand<T>::kSplit) { wgmma_bf16_n64(acc, ah, bl, 1u); wgmma_bf16_n64(acc, al, bh, 1u); }
+  }
+}
+
 // ---------------------------------------------------------------------------------------------------------------
-// prep: bf16 hi / lo split (zero padded to n_pad x k_pad) and squared norms (+inf on padded rows)
+// prep: the operand (zero padded to n_pad x k_pad): bf16 hi / lo split of fp32 X, a copy of 16-bit X (Xl unused);
+// squared norms of the fp32 values (+inf on padded rows), the same arithmetic for every element type
 // ---------------------------------------------------------------------------------------------------------------
+template <class T>
 __global__ void __launch_bounds__(256)
-knn_prep_kernel(const float* __restrict__ X, int64_t n, int d, int64_t n_pad, int k_pad, __nv_bfloat16* __restrict__ Xh,
+knn_prep_kernel(const T* __restrict__ X, int64_t n, int d, int64_t n_pad, int k_pad, OpT<T>* __restrict__ Xh,
                 __nv_bfloat16* __restrict__ Xl, float* __restrict__ norms) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= n_pad) return;
   float acc = 0.0f;
   for (int c = lane; c < k_pad; c += 32) {
-    const float x = (row < n && c < d) ? X[row * d + c] : 0.0f;
-    const __nv_bfloat16 h = __float2bfloat16_rn(x);
-    const __nv_bfloat16 l = __float2bfloat16_rn(x - __bfloat162float(h));
-    Xh[row * k_pad + c] = h;
-    Xl[row * k_pad + c] = l;
+    const float x = (row < n && c < d) ? elem_f32(X[row * d + c]) : 0.0f;
+    if constexpr (Operand<T>::kSplit) {
+      const __nv_bfloat16 h = __float2bfloat16_rn(x);
+      const __nv_bfloat16 l = __float2bfloat16_rn(x - __bfloat162float(h));
+      Xh[row * k_pad + c] = h;
+      Xl[row * k_pad + c] = l;
+    } else {
+      Xh[row * k_pad + c] = (row < n && c < d) ? X[row * d + c] : T(0.0f);
+    }
     acc += x * x;
   }
 #pragma unroll
@@ -132,6 +189,7 @@ __device__ __forceinline__ void keep_candidate(float (&bd)[kKK], int (&bi)[kKK],
 // ---------------------------------------------------------------------------------------------------------------
 // tiles: tensor-core cross terms + running top-KK per query row
 // ---------------------------------------------------------------------------------------------------------------
+template <class T>
 __global__ void __launch_bounds__(kThreads, 1)
 knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_l,
                 const float* __restrict__ norms, int64_t n, int64_t n_pad, int k_pad, int32_t* __restrict__ cand_idx,
@@ -166,11 +224,11 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
           mbar_wait(bar0 + 16 + 8 * stage, phase ^ 1);  // slot released by the consumers
           const uint32_t full = bar0 + 8 * stage;
           const uint32_t dst = base + stage * kStageBytes;
-          mbar_expect_tx(full, kStageBytes);
+          mbar_expect_tx(full, Operand<T>::kSplit ? kStageBytes : 2 * kOpBytes);  // 16-bit input: no lo parts
           tma_load_2d(dst, &map_h, kb * kBlockK, row0, full);
-          tma_load_2d(dst + kOpBytes, &map_l, kb * kBlockK, row0, full);
+          if (Operand<T>::kSplit) tma_load_2d(dst + kOpBytes, &map_l, kb * kBlockK, row0, full);
           tma_load_2d(dst + 2 * kOpBytes, &map_h, kb * kBlockK, t * kTileN, full);
-          tma_load_2d(dst + 3 * kOpBytes, &map_l, kb * kBlockK, t * kTileN, full);
+          if (Operand<T>::kSplit) tma_load_2d(dst + 3 * kOpBytes, &map_l, kb * kBlockK, t * kTileN, full);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
@@ -212,9 +270,7 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
 #pragma unroll
       for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
         const uint64_t adv = (uint64_t)((k * kWgmmaK * 2) >> 4);  // 32 bytes per K step inside the swizzle atom
-        wgmma_bf16(acc, ah + adv, bh + adv, (kb | k) != 0);
-        wgmma_bf16(acc, ah + adv, bl + adv, 1u);
-        wgmma_bf16(acc, al + adv, bh + adv, 1u);
+        cross_step<T, kTileN>(acc, ah + adv, al + adv, bh + adv, bl + adv, (kb | k) != 0);
       }
       wgmma_commit();
       wgmma_wait_all();
@@ -276,21 +332,22 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
 // ---------------------------------------------------------------------------------------------------------------
 namespace mde {
 
+template <class T>
 __global__ void __launch_bounds__(256)
-knn_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
+knn_rerank_kernel(const T* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
                   int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= n) return;
   const int mine = cand_idx[row * kKK + lane];  // lane q owns candidate q
   float my_d = __int_as_float(0x7f800000);
-  const float* xq = X + row * d;
+  const T* xq = X + row * d;
   for (int q = 0; q < kKK; ++q) {
     const int c = __shfl_sync(kFull, mine, q);
     if (c < 0) continue;  // (warp-uniform)
-    const float* xc = X + (int64_t)c * d;
+    const T* xc = X + (int64_t)c * d;
     float acc = 0.0f;
-    for (int j = lane; j < d; j += 32) { const float t = xq[j] - xc[j]; acc = fmaf(t, t, acc); }
+    for (int j = lane; j < d; j += 32) { const float t = elem_f32(xq[j]) - elem_f32(xc[j]); acc = fmaf(t, t, acc); }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
     if (lane == q) my_d = acc;
@@ -316,7 +373,7 @@ namespace {
 // wide tiles (k <= 64, KK = 96, TN = 128) and long tiles (k <= 256, KK = 288, TN = 64): as knn_tile_kernel for 64
 // query rows, one running top-KK per row in shared memory, wgmma.m64n{TN}k16 on candidate tiles of TN rows
 // ---------------------------------------------------------------------------------------------------------------
-template <int KK, int TN>
+template <class T, int KK, int TN>
 __global__ void __launch_bounds__(kWideThreads, 1)
 knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant__ CUtensorMap map_al,
                      const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_l,
@@ -360,11 +417,11 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
           mbar_wait(bar0 + 16 + 8 * stage, phase ^ 1);  // slot released by the consumers
           const uint32_t full = bar0 + 8 * stage;
           const uint32_t dst = base + stage * kStageB;
-          mbar_expect_tx(full, kStageB);
+          mbar_expect_tx(full, Operand<T>::kSplit ? kStageB : kAOpBytes + kBOpBytes);  // 16-bit input: no lo parts
           tma_load_2d(dst, &map_ah, kb * kBlockK, row0, full);
-          tma_load_2d(dst + kAOpBytes, &map_al, kb * kBlockK, row0, full);
+          if (Operand<T>::kSplit) tma_load_2d(dst + kAOpBytes, &map_al, kb * kBlockK, row0, full);
           tma_load_2d(dst + 2 * kAOpBytes, &map_h, kb * kBlockK, t * TN, full);
-          tma_load_2d(dst + 2 * kAOpBytes + kBOpBytes, &map_l, kb * kBlockK, t * TN, full);
+          if (Operand<T>::kSplit) tma_load_2d(dst + 2 * kAOpBytes + kBOpBytes, &map_l, kb * kBlockK, t * TN, full);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
@@ -396,15 +453,7 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
 #pragma unroll
       for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
         const uint64_t adv = (uint64_t)((k * kWgmmaK * 2) >> 4);
-        if constexpr (TN == 128) {
-          wgmma_bf16(acc, ah + adv, bh + adv, (kb | k) != 0);
-          wgmma_bf16(acc, ah + adv, bl + adv, 1u);
-          wgmma_bf16(acc, al + adv, bh + adv, 1u);
-        } else {
-          wgmma_bf16_n64(acc, ah + adv, bh + adv, (kb | k) != 0);
-          wgmma_bf16_n64(acc, ah + adv, bl + adv, 1u);
-          wgmma_bf16_n64(acc, al + adv, bh + adv, 1u);
-        }
+        cross_step<T, TN>(acc, ah + adv, al + adv, bh + adv, bl + adv, (kb | k) != 0);
       }
       wgmma_commit();
       wgmma_wait_all();
@@ -443,8 +492,8 @@ namespace mde {
 
 // Exact fp32 squared distances of a row's KK candidates (the arithmetic of knn_rerank_kernel), the k smallest in
 // ascending order; lane q owns candidates q, q + 32, q + 64, ..., ranks are taken over all KK.
-template <int KK>
-__device__ __forceinline__ void wide_rerank_row(const float* __restrict__ X, int64_t n, int d,
+template <class T, int KK>
+__device__ __forceinline__ void wide_rerank_row(const T* __restrict__ X, int64_t n, int d,
                                                 const int32_t* __restrict__ cand_idx, int k,
                                                 int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
   const int lane = threadIdx.x & 31;
@@ -453,7 +502,7 @@ __device__ __forceinline__ void wide_rerank_row(const float* __restrict__ X, int
   constexpr int kPer = KK / 32;
   int mine[kPer];
   float my_d[kPer];
-  const float* xq = X + row * d;
+  const T* xq = X + row * d;
 #pragma unroll
   for (int s = 0; s < kPer; ++s) {
     mine[s] = cand_idx[row * KK + 32 * s + lane];
@@ -461,9 +510,9 @@ __device__ __forceinline__ void wide_rerank_row(const float* __restrict__ X, int
     for (int q = 0; q < 32; ++q) {
       const int c = __shfl_sync(kFull, mine[s], q);
       if (c < 0) continue;  // (warp-uniform)
-      const float* xc = X + (int64_t)c * d;
+      const T* xc = X + (int64_t)c * d;
       float acc = 0.0f;
-      for (int j = lane; j < d; j += 32) { const float t = xq[j] - xc[j]; acc = fmaf(t, t, acc); }
+      for (int j = lane; j < d; j += 32) { const float t = elem_f32(xq[j]) - elem_f32(xc[j]); acc = fmaf(t, t, acc); }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
       if (lane == q) my_d[s] = acc;
@@ -491,18 +540,38 @@ __device__ __forceinline__ void wide_rerank_row(const float* __restrict__ X, int
   }
 }
 
+template <class T>
 __global__ void __launch_bounds__(256)
-knn_wide_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
+knn_wide_rerank_kernel(const T* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
                        int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
-  wide_rerank_row<kWideKK>(X, n, d, cand_idx, k, out_idx, out_d2);
+  wide_rerank_row<T, kWideKK>(X, n, d, cand_idx, k, out_idx, out_d2);
 }
 
 // the 288 candidates of the long search, with the same arithmetic
+template <class T>
 __global__ void __launch_bounds__(256)
-knn_long_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
+knn_long_rerank_kernel(const T* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
                        int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
-  wide_rerank_row<kLongKK>(X, n, d, cand_idx, k, out_idx, out_d2);
+  wide_rerank_row<T, kLongKK>(X, n, d, cand_idx, k, out_idx, out_d2);
 }
+
+template <class T>
+int knn_dense_rerank(int kk, const T* X, int64_t n, int d, const int32_t* cand_idx, int k, int32_t* out_idx,
+                     float* out_d2, cudaStream_t st) {
+  const unsigned grid = (unsigned)((n + 7) / 8);
+  if (kk == kNarrowKK) knn_rerank_kernel<T><<<grid, 256, 0, st>>>(X, n, d, cand_idx, k, out_idx, out_d2);
+  else if (kk == kWideKK) knn_wide_rerank_kernel<T><<<grid, 256, 0, st>>>(X, n, d, cand_idx, k, out_idx, out_d2);
+  else if (kk == kLongKK) knn_long_rerank_kernel<T><<<grid, 256, 0, st>>>(X, n, d, cand_idx, k, out_idx, out_d2);
+  else return MDE_E_INVALID;
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+template int knn_dense_rerank<float>(int, const float*, int64_t, int, const int32_t*, int, int32_t*, float*,
+                                     cudaStream_t);
+template int knn_dense_rerank<__half>(int, const __half*, int64_t, int, const int32_t*, int, int32_t*, float*,
+                                      cudaStream_t);
+template int knn_dense_rerank<__nv_bfloat16>(int, const __nv_bfloat16*, int64_t, int, const int32_t*, int, int32_t*,
+                                             float*, cudaStream_t);
 
 }  // namespace mde
 
@@ -526,13 +595,14 @@ int tensor_map_encoder(EncodeTiledFn* out) {
   return 0;
 }
 
-// Tensor map of an n_pad x k_pad bf16 operand, loaded in boxes of box_rows x 64 (128-byte swizzle).
-int make_map(EncodeTiledFn enc, CUtensorMap* map, void* ptr, int64_t n_pad, int k_pad, int box_rows = kTileM) {
+// Tensor map of an n_pad x k_pad 16-bit operand (bf16 or fp16), loaded in boxes of box_rows x 64 (128-byte swizzle).
+int make_map(EncodeTiledFn enc, CUtensorMap* map, void* ptr, int64_t n_pad, int k_pad, int box_rows = kTileM,
+             CUtensorMapDataType type = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16) {
   const cuuint64_t dims[2] = {(cuuint64_t)k_pad, (cuuint64_t)n_pad};
   const cuuint64_t strides[1] = {(cuuint64_t)k_pad * 2};
   const cuuint32_t box[2] = {(cuuint32_t)kBlockK, (cuuint32_t)box_rows};
   const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, ptr, dims, strides, box, estr,
+  const CUresult r = enc(map, type, 2, ptr, dims, strides, box, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? 0 : MDE_E_INVALID;
@@ -543,15 +613,17 @@ struct KnnLayout {
   size_t off_h, off_l, off_norm, off_ci, off_cv, total;
 };
 
-// kk: candidates kept per row (kKK, kWideKK for the wide search, kLongKK for the long one)
-KnnLayout knn_layout(int64_t n, int d, int kk = kKK) {
+// kk: candidates kept per row (kKK, kWideKK for the wide search, kLongKK for the long one); split: fp32 input, whose
+// operand has a lo part (16-bit input has none: off_l == off_h, 2 n_pad k_pad bytes fewer)
+KnnLayout knn_layout(int64_t n, int d, int kk = kKK, bool split = true) {
   KnnLayout L;
   L.n_pad = (n + kTileN - 1) / kTileN * kTileN;
   L.k_pad = (d + kBlockK - 1) / kBlockK * kBlockK;
   auto up = [](size_t x) { return (x + 1023) / 1024 * 1024; };
   size_t o = 0;
   L.off_h = o; o = up(o + (size_t)L.n_pad * L.k_pad * 2);
-  L.off_l = o; o = up(o + (size_t)L.n_pad * L.k_pad * 2);
+  L.off_l = split ? o : L.off_h;
+  if (split) o = up(o + (size_t)L.n_pad * L.k_pad * 2);
   L.off_norm = o; o = up(o + (size_t)L.n_pad * 4);
   L.off_ci = o; o = up(o + (size_t)n * kk * 4);
   L.off_cv = o; o = up(o + (size_t)n * kk * 4);
@@ -559,43 +631,110 @@ KnnLayout knn_layout(int64_t n, int d, int kk = kKK) {
   return L;
 }
 
-// mde_knn_wide (KK = 96, TN = 128) and mde_knn_long (KK = 288, TN = 64): prep, tiles, re-rank of all KK candidates.
-template <int KK, int TN>
-int run_wide(const float* X, int64_t n, int d, int k, int max_k, int32_t* idx_out, float* d2_out, void* ws,
-             size_t ws_bytes, void* stream) {
-  if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > max_k || k > n - 1) return MDE_E_INVALID;
+// mde_knn / mde_knn16: prep, tiles, re-rank of the 32 candidates.
+template <class T>
+int run_narrow(const T* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
+               void* stream) {
+  if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > kMaxK || k > n - 1) return MDE_E_INVALID;
   if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
-  const KnnLayout L = knn_layout(n, d, KK);
+  const KnnLayout L = knn_layout(n, d, kKK, Operand<T>::kSplit);
   if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   EncodeTiledFn enc = nullptr;
   int rc;
   if ((rc = tensor_map_encoder(&enc))) return rc;
   uint8_t* w = static_cast<uint8_t*>(ws);
-  __nv_bfloat16* Xh = reinterpret_cast<__nv_bfloat16*>(w + L.off_h);
+  OpT<T>* Xh = reinterpret_cast<OpT<T>*>(w + L.off_h);
   __nv_bfloat16* Xl = reinterpret_cast<__nv_bfloat16*>(w + L.off_l);
   float* norms = reinterpret_cast<float*>(w + L.off_norm);
   int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
   float* cv = reinterpret_cast<float*>(w + L.off_cv);
+  CUtensorMap mh, ml;
+  if ((rc = make_map(enc, &mh, Xh, L.n_pad, L.k_pad, kTileM, Operand<T>::kMapType))) return rc;
+  if ((rc = make_map(enc, &ml, Xl, L.n_pad, L.k_pad, kTileM, Operand<T>::kMapType))) return rc;
+  knn_prep_kernel<T><<<(unsigned)((L.n_pad + 7) / 8), 256, 0, st>>>(X, n, d, L.n_pad, L.k_pad, Xh, Xl, norms);
+  MDE_LAUNCH_CHECK();
+  static bool attr_set = false;
+  if (!attr_set) {
+    MDE_CUDA_TRY(cudaFuncSetAttribute(knn_tile_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+    attr_set = true;
+  }
+  const unsigned grid = (unsigned)((n + kTileM - 1) / kTileM);
+  knn_tile_kernel<T><<<grid, kThreads, kSmemBytes, st>>>(mh, ml, norms, n, L.n_pad, L.k_pad, ci, cv);
+  MDE_LAUNCH_CHECK();
+  return knn_dense_rerank<T>(kKK, X, n, d, ci, k, idx_out, d2_out, st);
+}
+
+// mde_knn_wide (KK = 96, TN = 128) and mde_knn_long (KK = 288, TN = 64), and their 16-bit entries: prep, tiles,
+// re-rank of all KK candidates.
+template <class T, int KK, int TN>
+int run_wide(const T* X, int64_t n, int d, int k, int max_k, int32_t* idx_out, float* d2_out, void* ws,
+             size_t ws_bytes, void* stream) {
+  if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > max_k || k > n - 1) return MDE_E_INVALID;
+  if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
+  const KnnLayout L = knn_layout(n, d, KK, Operand<T>::kSplit);
+  if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  EncodeTiledFn enc = nullptr;
+  int rc;
+  if ((rc = tensor_map_encoder(&enc))) return rc;
+  uint8_t* w = static_cast<uint8_t*>(ws);
+  OpT<T>* Xh = reinterpret_cast<OpT<T>*>(w + L.off_h);
+  __nv_bfloat16* Xl = reinterpret_cast<__nv_bfloat16*>(w + L.off_l);
+  float* norms = reinterpret_cast<float*>(w + L.off_norm);
+  int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
+  float* cv = reinterpret_cast<float*>(w + L.off_cv);
+  constexpr CUtensorMapDataType kType = Operand<T>::kMapType;
   CUtensorMap mah, mal, mh, ml;  // query operand in 64-row boxes, candidate operand in TN-row boxes
-  if ((rc = make_map(enc, &mah, Xh, L.n_pad, L.k_pad, kWideTileM))) return rc;
-  if ((rc = make_map(enc, &mal, Xl, L.n_pad, L.k_pad, kWideTileM))) return rc;
-  if ((rc = make_map(enc, &mh, Xh, L.n_pad, L.k_pad, TN))) return rc;
-  if ((rc = make_map(enc, &ml, Xl, L.n_pad, L.k_pad, TN))) return rc;
-  knn_prep_kernel<<<(unsigned)((L.n_pad + 7) / 8), 256, 0, st>>>(X, n, d, L.n_pad, L.k_pad, Xh, Xl, norms);
+  if ((rc = make_map(enc, &mah, Xh, L.n_pad, L.k_pad, kWideTileM, kType))) return rc;
+  if ((rc = make_map(enc, &mal, Xl, L.n_pad, L.k_pad, kWideTileM, kType))) return rc;
+  if ((rc = make_map(enc, &mh, Xh, L.n_pad, L.k_pad, TN, kType))) return rc;
+  if ((rc = make_map(enc, &ml, Xl, L.n_pad, L.k_pad, TN, kType))) return rc;
+  knn_prep_kernel<T><<<(unsigned)((L.n_pad + 7) / 8), 256, 0, st>>>(X, n, d, L.n_pad, L.k_pad, Xh, Xl, norms);
   MDE_LAUNCH_CHECK();
   constexpr int kSmem = kWideSmemBytes<KK, TN>;
   static bool attr_set = false;
   if (!attr_set) {
-    MDE_CUDA_TRY(cudaFuncSetAttribute(knn_wide_tile_kernel<KK, TN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+    MDE_CUDA_TRY(cudaFuncSetAttribute(knn_wide_tile_kernel<T, KK, TN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      kSmem));
     attr_set = true;
   }
   const unsigned grid = (unsigned)((n + kWideTileM - 1) / kWideTileM);
-  knn_wide_tile_kernel<KK, TN><<<grid, kWideThreads, kSmem, st>>>(mah, mal, mh, ml, norms, n, L.n_pad, L.k_pad, ci, cv);
+  knn_wide_tile_kernel<T, KK, TN><<<grid, kWideThreads, kSmem, st>>>(mah, mal, mh, ml, norms, n, L.n_pad, L.k_pad, ci,
+                                                                     cv);
   MDE_LAUNCH_CHECK();
-  if constexpr (KK == kWideKK) knn_wide_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(X, n, d, ci, k, idx_out, d2_out);
-  else knn_long_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(X, n, d, ci, k, idx_out, d2_out);
-  MDE_LAUNCH_CHECK();
+  return knn_dense_rerank<T>(KK, X, n, d, ci, k, idx_out, d2_out, st);
+}
+
+// The 16-bit entries: dtype code -> element type, MDE_E_INVALID for an unknown code (before any CUDA call).
+template <template <class> class Run, class... A>
+int by_dtype(const void* X, int dtype, A... args) {
+  if (dtype == MDE_DTYPE_FP16) return Run<__half>::call(static_cast<const __half*>(X), args...);
+  if (dtype == MDE_DTYPE_BF16) return Run<__nv_bfloat16>::call(static_cast<const __nv_bfloat16*>(X), args...);
+  return MDE_E_INVALID;
+}
+template <class T>
+struct Narrow {
+  static int call(const T* X, int64_t n, int d, int k, int32_t* i, float* d2, void* ws, size_t b, void* st) {
+    return run_narrow<T>(X, n, d, k, i, d2, ws, b, st);
+  }
+};
+template <class T>
+struct Wide {
+  static int call(const T* X, int64_t n, int d, int k, int32_t* i, float* d2, void* ws, size_t b, void* st) {
+    return run_wide<T, kWideKK, kTileN>(X, n, d, k, kWideMaxK, i, d2, ws, b, st);
+  }
+};
+template <class T>
+struct Long {
+  static int call(const T* X, int64_t n, int d, int k, int32_t* i, float* d2, void* ws, size_t b, void* st) {
+    return run_wide<T, kLongKK, kLongTileN>(X, n, d, k, kLongMaxK, i, d2, ws, b, st);
+  }
+};
+
+int layout_bytes(int64_t n, int d, int kk, bool split, size_t* bytes) {
+  if (!bytes || n < 2 || d < 1) return MDE_E_INVALID;
+  *bytes = knn_layout(n, d, kk, split).total;
   return 0;
 }
 
@@ -605,70 +744,50 @@ extern "C" {
 
 int mde_knn_max_k(void) { return kMaxK; }
 
-int mde_knn_ws_bytes(int64_t n, int d, size_t* bytes) {
-  if (!bytes || n < 2 || d < 1) return MDE_E_INVALID;
-  *bytes = knn_layout(n, d).total;
-  return 0;
-}
+int mde_knn_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kKK, true, bytes); }
 
 int mde_knn(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
             void* stream) {
-  if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > kMaxK || k > n - 1) return MDE_E_INVALID;
-  if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
-  const KnnLayout L = knn_layout(n, d);
-  if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream;
-  EncodeTiledFn enc = nullptr;
-  int rc;
-  if ((rc = tensor_map_encoder(&enc))) return rc;
-  uint8_t* w = static_cast<uint8_t*>(ws);
-  __nv_bfloat16* Xh = reinterpret_cast<__nv_bfloat16*>(w + L.off_h);
-  __nv_bfloat16* Xl = reinterpret_cast<__nv_bfloat16*>(w + L.off_l);
-  float* norms = reinterpret_cast<float*>(w + L.off_norm);
-  int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
-  float* cv = reinterpret_cast<float*>(w + L.off_cv);
-  CUtensorMap mh, ml;
-  if ((rc = make_map(enc, &mh, Xh, L.n_pad, L.k_pad))) return rc;
-  if ((rc = make_map(enc, &ml, Xl, L.n_pad, L.k_pad))) return rc;
-  knn_prep_kernel<<<(unsigned)((L.n_pad + 7) / 8), 256, 0, st>>>(X, n, d, L.n_pad, L.k_pad, Xh, Xl, norms);
-  MDE_LAUNCH_CHECK();
-  static bool attr_set = false;
-  if (!attr_set) {
-    MDE_CUDA_TRY(cudaFuncSetAttribute(knn_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    attr_set = true;
-  }
-  const unsigned grid = (unsigned)((n + kTileM - 1) / kTileM);
-  knn_tile_kernel<<<grid, kThreads, kSmemBytes, st>>>(mh, ml, norms, n, L.n_pad, L.k_pad, ci, cv);
-  MDE_LAUNCH_CHECK();
-  knn_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(X, n, d, ci, k, idx_out, d2_out);
-  MDE_LAUNCH_CHECK();
-  return 0;
+  return run_narrow<float>(X, n, d, k, idx_out, d2_out, ws, ws_bytes, stream);
 }
 
 int mde_knn_wide_max_k(void) { return kWideMaxK; }
 
-int mde_knn_wide_ws_bytes(int64_t n, int d, size_t* bytes) {
-  if (!bytes || n < 2 || d < 1) return MDE_E_INVALID;
-  *bytes = knn_layout(n, d, kWideKK).total;
-  return 0;
-}
+int mde_knn_wide_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kWideKK, true, bytes); }
 
 int mde_knn_wide(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                  size_t ws_bytes, void* stream) {
-  return run_wide<kWideKK, kTileN>(X, n, d, k, kWideMaxK, idx_out, d2_out, ws, ws_bytes, stream);
+  return run_wide<float, kWideKK, kTileN>(X, n, d, k, kWideMaxK, idx_out, d2_out, ws, ws_bytes, stream);
 }
 
 int mde_knn_long_max_k(void) { return kLongMaxK; }
 
-int mde_knn_long_ws_bytes(int64_t n, int d, size_t* bytes) {
-  if (!bytes || n < 2 || d < 1) return MDE_E_INVALID;
-  *bytes = knn_layout(n, d, kLongKK).total;
-  return 0;
-}
+int mde_knn_long_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kLongKK, true, bytes); }
 
 int mde_knn_long(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                  size_t ws_bytes, void* stream) {
-  return run_wide<kLongKK, kLongTileN>(X, n, d, k, kLongMaxK, idx_out, d2_out, ws, ws_bytes, stream);
+  return run_wide<float, kLongKK, kLongTileN>(X, n, d, k, kLongMaxK, idx_out, d2_out, ws, ws_bytes, stream);
+}
+
+int mde_knn16_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kKK, false, bytes); }
+
+int mde_knn16(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+              size_t ws_bytes, void* stream) {
+  return by_dtype<Narrow>(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream);
+}
+
+int mde_knn16_wide_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kWideKK, false, bytes); }
+
+int mde_knn16_wide(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                   size_t ws_bytes, void* stream) {
+  return by_dtype<Wide>(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream);
+}
+
+int mde_knn16_long_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kLongKK, false, bytes); }
+
+int mde_knn16_long(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                   size_t ws_bytes, void* stream) {
+  return by_dtype<Long>(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream);
 }
 
 }  // extern "C"

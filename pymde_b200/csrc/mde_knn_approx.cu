@@ -16,7 +16,10 @@
 //
 // and the host stops when fewer than 0.001 n KB entries changed or after max(5, ceil(log2 n)) iterations.  The final
 // lists go to the re-rank kernels of mde_knn (knn_rerank_kernel for 32 candidates, knn_wide_rerank_kernel for 96),
-// so the output contract and the distance arithmetic are those of the exact search.
+// so the output contract and the distance arithmetic are those of the exact search.  A 16-bit matrix (IEEE fp16 or
+// bf16, mde_knn16_approx) is read in place: DenseRows, the join and the re-rank take the element type as a template
+// parameter and convert each element to fp32 as they load it, so every distance, and with it the whole search, has
+// the bits of the fp32 search on X.float().
 //
 // Determinism.  Offers and reverse samples arrive in a racy order, so they are collected in cascade reservoirs: R
 // 64-bit keys per row, all ones when empty; inserting x runs y = atomicMin(&r[i], x), x = max(x, y) down the slots.
@@ -68,9 +71,10 @@ __device__ __forceinline__ uint64_t hash4(uint64_t seed, uint64_t a, uint64_t b,
 }
 
 // The one distance of the search: sequential fp32 sum over the features (the join's tiles add in the same order).
-__device__ __forceinline__ float seq_dist(const float* __restrict__ a, const float* __restrict__ b, int d) {
+template <class T>
+__device__ __forceinline__ float seq_dist(const T* __restrict__ a, const T* __restrict__ b, int d) {
   float acc = 0.0f;
-  for (int f = 0; f < d; ++f) { const float t = a[f] - b[f]; acc = fmaf(t, t, acc); }
+  for (int f = 0; f < d; ++f) { const float t = elem_f32(a[f]) - elem_f32(b[f]); acc = fmaf(t, t, acc); }
   return acc;
 }
 
@@ -100,9 +104,10 @@ __device__ __forceinline__ bool in_list(const unsigned long long* __restrict__ l
   return lo < KB && __ldg(l + lo) == x;
 }
 
-// The row formats: the one distance of the search between rows a and b.
+// The row formats: the one distance of the search between rows a and b.  T: the element type of a dense matrix.
+template <class T>
 struct DenseRows {
-  const float* X;
+  const T* X;
   int d;
   __device__ __forceinline__ float dist(int64_t a, int64_t b) const { return seq_dist(X + a * d, X + b * d, d); }
 };
@@ -277,9 +282,9 @@ __device__ __forceinline__ void offer_pair(const unsigned long long* __restrict_
 // join of dense rows: one CTA per row u.  The candidates (join_candidates) are staged in shared memory 64 features at
 // a time; thread t < 100 owns the 4 x 4 pair tile (ta, tb), ta < 8 <= ... tb: every pair with a new member and a < b.
 // ---------------------------------------------------------------------------------------------------------------
-template <int KB>
+template <int KB, class T>
 __global__ void __launch_bounds__(kJoinThreads)
-nnd_join_kernel(const float* __restrict__ X, int64_t n, int d, const unsigned long long* __restrict__ keys,
+nnd_join_kernel(const T* __restrict__ X, int64_t n, int d, const unsigned long long* __restrict__ keys,
                 const int32_t* __restrict__ fwd, unsigned long long* __restrict__ rev, const uint32_t* __restrict__ thr,
                 unsigned long long* __restrict__ offers) {
   __shared__ int s_raw[kCand];
@@ -310,7 +315,7 @@ nnd_join_kernel(const float* __restrict__ X, int64_t n, int d, const unsigned lo
     __syncthreads();  // the previous chunk is consumed
     for (int e = t; e < kCand * kFC; e += kJoinThreads) {
       const int r = e / kFC, f = e % kFC;
-      s_x[r][f] = (f < fc && slot_valid(r)) ? __ldg(X + (int64_t)s_idx[r] * d + f0 + f) : 0.0f;
+      s_x[r][f] = (f < fc && slot_valid(r)) ? load_f32(X + (int64_t)s_idx[r] * d + f0 + f) : 0.0f;
     }
     __syncthreads();
     if (active) {
@@ -519,10 +524,10 @@ ApproxCsrLayout approx_csr_layout(int64_t n, int d, int64_t nnz, int k) {
 }
 
 // The format-specific launches of the driver.
-template <int KB>
-int launch_join(const DenseRows& r, int64_t n, const unsigned long long* keys, const int32_t* fwd,
+template <int KB, class T>
+int launch_join(const DenseRows<T>& r, int64_t n, const unsigned long long* keys, const int32_t* fwd,
                 unsigned long long* rev, const uint32_t* thr, unsigned long long* offers, cudaStream_t st) {
-  nnd_join_kernel<KB><<<(unsigned)n, kJoinThreads, 0, st>>>(r.X, n, r.d, keys, fwd, rev, thr, offers);
+  nnd_join_kernel<KB, T><<<(unsigned)n, kJoinThreads, 0, st>>>(r.X, n, r.d, keys, fwd, rev, thr, offers);
   MDE_LAUNCH_CHECK();
   return 0;
 }
@@ -534,14 +539,10 @@ int launch_join(const CsrRows& r, int64_t n, const unsigned long long* keys, con
   MDE_LAUNCH_CHECK();
   return 0;
 }
-template <int KB>
-int launch_rerank(const DenseRows& r, int64_t n, const int32_t* cand, int k, int32_t* idx_out, float* d2_out,
+template <int KB, class T>
+int launch_rerank(const DenseRows<T>& r, int64_t n, const int32_t* cand, int k, int32_t* idx_out, float* d2_out,
                   cudaStream_t st) {
-  const unsigned grid = (unsigned)((n + 7) / 8);
-  if (KB == kNarrowKK) knn_rerank_kernel<<<grid, 256, 0, st>>>(r.X, n, r.d, cand, k, idx_out, d2_out);
-  else knn_wide_rerank_kernel<<<grid, 256, 0, st>>>(r.X, n, r.d, cand, k, idx_out, d2_out);
-  MDE_LAUNCH_CHECK();
-  return 0;
+  return knn_dense_rerank<T>(KB, r.X, n, r.d, cand, k, idx_out, d2_out, st);
 }
 template <int KB>
 int launch_rerank(const CsrRows& r, int64_t n, const int32_t* cand, int k, int32_t* idx_out, float* d2_out,
@@ -593,6 +594,22 @@ int run_approx(const Rows& rows, int64_t n, int k, uint64_t seed, int32_t* idx_o
   return launch_rerank<KB>(rows, n, cand, k, idx_out, d2_out, st);
 }
 
+// The dense search on a matrix of element type T.
+template <class T>
+int approx_dense(const T* X, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out, float* d2_out, void* ws,
+                 size_t ws_bytes, void* stream, int* iterations) {
+  if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > kWideMaxK || k > n - 1)
+    return MDE_E_INVALID;
+  if (n >= (1ll << 31) - 128) return MDE_E_UNSUPPORTED;
+  const ApproxLayout L = approx_layout(n, k);
+  if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* w = static_cast<uint8_t*>(ws);
+  const DenseRows<T> rows{X, d};
+  if (L.kb == kNarrowKK) return run_approx<kNarrowKK>(rows, n, k, seed, idx_out, d2_out, w, L, st, iterations);
+  return run_approx<kWideKK>(rows, n, k, seed, idx_out, d2_out, w, L, st, iterations);
+}
+
 }  // namespace
 
 extern "C" {
@@ -607,21 +624,30 @@ int mde_knn_approx_ws_bytes(int64_t n, int d, int k, size_t* bytes) {
 
 int mde_knn_approx_ex(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out, float* d2_out,
                       void* ws, size_t ws_bytes, void* stream, int* iterations) {
-  if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > kWideMaxK || k > n - 1)
-    return MDE_E_INVALID;
-  if (n >= (1ll << 31) - 128) return MDE_E_UNSUPPORTED;
-  const ApproxLayout L = approx_layout(n, k);
-  if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream;
-  uint8_t* w = static_cast<uint8_t*>(ws);
-  const DenseRows rows{X, d};
-  if (L.kb == kNarrowKK) return run_approx<kNarrowKK>(rows, n, k, seed, idx_out, d2_out, w, L, st, iterations);
-  return run_approx<kWideKK>(rows, n, k, seed, idx_out, d2_out, w, L, st, iterations);
+  return approx_dense<float>(X, n, d, k, seed, idx_out, d2_out, ws, ws_bytes, stream, iterations);
 }
 
 int mde_knn_approx(const float* X, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out, float* d2_out, void* ws,
                    size_t ws_bytes, void* stream) {
   return mde_knn_approx_ex(X, n, d, k, seed, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
+}
+
+int mde_knn16_approx_ws_bytes(int64_t n, int d, int k, size_t* bytes) { return mde_knn_approx_ws_bytes(n, d, k, bytes); }
+
+int mde_knn16_approx_ex(const void* X, int dtype, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out,
+                        float* d2_out, void* ws, size_t ws_bytes, void* stream, int* iterations) {
+  if (dtype == MDE_DTYPE_FP16)
+    return approx_dense<__half>(static_cast<const __half*>(X), n, d, k, seed, idx_out, d2_out, ws, ws_bytes, stream,
+                                iterations);
+  if (dtype == MDE_DTYPE_BF16)
+    return approx_dense<__nv_bfloat16>(static_cast<const __nv_bfloat16*>(X), n, d, k, seed, idx_out, d2_out, ws,
+                                       ws_bytes, stream, iterations);
+  return MDE_E_INVALID;
+}
+
+int mde_knn16_approx(const void* X, int dtype, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out,
+                     float* d2_out, void* ws, size_t ws_bytes, void* stream) {
+  return mde_knn16_approx_ex(X, dtype, n, d, k, seed, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
 int mde_knn_approx_csr_ws_bytes(int64_t n, int d, int64_t nnz, int k, size_t* bytes) {

@@ -9,10 +9,12 @@
 // (distance, index); the worst is the largest, so the list after a sweep depends on nothing but the order of the
 // offers, never on timing.
 //
-// It also declares the two dense re-rank kernels (defined in mde_knn.cu).  The approximate search
+// It also declares the launcher of the dense re-rank kernels (defined in mde_knn.cu).  The approximate search
 // (mde_knn_approx.cu) hands its final lists to them, so a pair found by the exact and the approximate search carries
 // the same fp32 distance bits.
 #pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -76,14 +78,22 @@ struct WideList {
   }
 };
 
-// Exact fp32 squared distances sum_j (q_j - x_j)^2 (lane-strided fmaf, then a butterfly) of a row's kNarrowKK
-// (knn_rerank_kernel) or kWideKK (knn_wide_rerank_kernel) candidates cand_idx[row][.], -1 for none; the k smallest by
-// (distance, index) go to out_idx / out_d2 [n][k] in ascending order.  One warp per row, 256 threads per block.
-__global__ void __launch_bounds__(256)
-knn_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
-                  int32_t* __restrict__ out_idx, float* __restrict__ out_d2);
-__global__ void __launch_bounds__(256)
-knn_wide_rerank_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
-                       int32_t* __restrict__ out_idx, float* __restrict__ out_d2);
+// Element types of a dense data matrix: fp32, IEEE fp16 and bf16.  The searches read 16-bit matrices in place and
+// compute every distance on the fp32 value of each element, which is exact, so a 16-bit matrix X gives the bits of the
+// fp32 matrix X.float().
+__device__ __forceinline__ float elem_f32(float x) { return x; }
+__device__ __forceinline__ float elem_f32(__half x) { return __half2float(x); }
+__device__ __forceinline__ float elem_f32(__nv_bfloat16 x) { return __bfloat162float(x); }
+template <class T>
+__device__ __forceinline__ float load_f32(const T* p) { return elem_f32(__ldg(p)); }
+
+// Exact fp32 squared distances sum_j (q_j - x_j)^2 (lane-strided fmaf, then a butterfly) of a row's kk candidates
+// cand_idx[row][.], -1 for none, kk = kNarrowKK (knn_rerank_kernel), kWideKK (knn_wide_rerank_kernel) or kLongKK
+// (knn_long_rerank_kernel); the k smallest by (distance, index) go to out_idx / out_d2 [n][k] in ascending order.
+// One warp per row, 256 threads per block; the elements of X are converted to fp32 as they are read.  Defined in
+// mde_knn.cu for T = float, __half and __nv_bfloat16.
+template <class T>
+int knn_dense_rerank(int kk, const T* X, int64_t n, int d, const int32_t* cand_idx, int k, int32_t* out_idx,
+                     float* out_d2, cudaStream_t st);
 
 }  // namespace mde

@@ -13,7 +13,13 @@ exact search is faster (DESIGN section 11.3).  `PYMDE_B200_KNN=approx` leaves sp
 (`mde_knn_csr`, `mde_knn_csr_wide`, `mde_knn_csr_long`, csrc/mde_knn_sparse.cu), and its pair distances come from
 sorted merges of CSR rows (`mde_pair_dist_csr`).  `PYMDE_B200_KNN_SPARSE=approx` opts in to NN-descent over the CSR
 rows for k <= 64 (`mde_knn_approx_csr`, csrc/mde_knn_approx.cu), with the distances of the exact sparse search
-(DESIGN section 11.4); a k above 64 takes the exact long search."""
+(DESIGN section 11.4); a k above 64 takes the exact long search.
+
+A float16 / bfloat16 matrix (a torch tensor on any device, or an np.float16 array) is searched in its own precision,
+without an fp32 copy: the `mde_knn16*` entries use it as the tensor-core operand and convert each element to fp32 as
+the re-rank and NN-descent read it, so neighbours and distances are those of the fp32 search on the upcast matrix
+(DESIGN section 11.7).  The routing by k and PYMDE_B200_KNN is unchanged; the GEMM path, and every other dtype,
+still work on an fp32 copy."""
 import ctypes as C
 import os
 
@@ -26,12 +32,26 @@ from .graph import EdgeListGraph, Graph
 from .preprocess import sample_edges  # noqa: F401  (the reference exposes it here as well)
 
 
-def _to_device_matrix(data, device):
-    if sp.issparse(data):
+# element types the search kernels read in place -> their MDE_DTYPE_* codes (include/mde_b200.h)
+_HALF_DTYPES = {torch.float16: 1, torch.bfloat16: 2}
+
+
+def _to_device_matrix(data, device, keep_half=False):
+    """The dense matrix on `device`, in fp32; with `keep_half`, a dense float16 / bfloat16 matrix keeps its dtype
+    (uploaded at 2 bytes per value)."""
+    sparse = sp.issparse(data)
+    if sparse:
         data = data.toarray()
     if isinstance(data, np.ndarray):
         data = torch.from_numpy(np.ascontiguousarray(data))
+    if keep_half and not sparse and data.dtype in _HALF_DTYPES:
+        return data.to(device=device)
     return data.to(device=device, dtype=torch.float32)
+
+
+def _matrix_args(X):
+    """The leading arguments of a dense search entry: (X,) for fp32, (X, dtype code) for the mde_knn16* entries."""
+    return (X.data_ptr(), _HALF_DTYPES[X.dtype]) if X.dtype in _HALF_DTYPES else (X.data_ptr(),)
 
 
 def _to_device_csr(data, device):
@@ -128,15 +148,16 @@ def _knn_graph(idx, d2, n, max_distance, dev):
 def knn_device(X, k):
     """(indices [n, k] int32, squared distances [n, k] fp32) of the k nearest rows of every row of the CUDA fp32
     matrix X, ascending; the wgmma kernel behind `mde_knn` for k <= 24, `mde_knn_wide` for 24 < k <= 64 and
-    `mde_knn_long` for 64 < k <= 256 (include/mde_b200.h)."""
+    `mde_knn_long` for 64 < k <= 256 (include/mde_b200.h).  A float16 / bfloat16 X is read in place by the
+    `mde_knn16*` entries, with the result of X.float()."""
     from .. import _lib
     lib = _lib.load()
+    name = "knn16" if X.dtype in _HALF_DTYPES else "knn"
     if k > lib.mde_knn_wide_max_k():
-        ws_bytes, search = lib.mde_knn_long_ws_bytes, lib.mde_knn_long
+        name += "_long"
     elif k > lib.mde_knn_max_k():
-        ws_bytes, search = lib.mde_knn_wide_ws_bytes, lib.mde_knn_wide
-    else:
-        ws_bytes, search = lib.mde_knn_ws_bytes, lib.mde_knn
+        name += "_wide"
+    ws_bytes, search = getattr(lib, "mde_%s_ws_bytes" % name), getattr(lib, "mde_" + name)
     X = X.contiguous()
     n, d = X.shape
     need = C.c_size_t(0)
@@ -147,8 +168,8 @@ def knn_device(X, k):
     d2 = torch.empty((n, k), dtype=torch.float32, device=X.device)
     with torch.cuda.device(X.device):
         stream = torch.cuda.current_stream().cuda_stream
-        _lib.check(search(X.data_ptr(), int(n), int(d), int(k), idx.data_ptr(), d2.data_ptr(), ws.data_ptr() + off,
-                          need.value, stream))
+        _lib.check(search(*_matrix_args(X), int(n), int(d), int(k), idx.data_ptr(), d2.data_ptr(),
+                          ws.data_ptr() + off, need.value, stream))
         torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
     return idx, d2
 
@@ -157,23 +178,27 @@ def knn_approx_device(X, k, seed=None):
     """(indices [n, k] int32, squared distances [n, k] fp32) of k rows found for every row of the CUDA fp32 matrix X
     by NN-descent, ascending by (distance, index), with the exact fp32 distances of `knn_device`
     (`mde_knn_approx`, include/mde_b200.h).  `seed` defaults to a draw from the module RNG, so `pymde_b200.seed(s)`
-    reproduces the result."""
+    reproduces the result.  A float16 / bfloat16 X is read in place (`mde_knn16_approx`), with the result of
+    X.float()."""
     from .. import _lib
     lib = _lib.load()
     if seed is None:
         seed = int(util.np_rng().integers(0, 2 ** 62))
     X = X.contiguous()
     n, d = X.shape
+    half = X.dtype in _HALF_DTYPES
+    ws_bytes, search = ((lib.mde_knn16_approx_ws_bytes, lib.mde_knn16_approx) if half else
+                        (lib.mde_knn_approx_ws_bytes, lib.mde_knn_approx))
     need = C.c_size_t(0)
-    _lib.check(lib.mde_knn_approx_ws_bytes(int(n), int(d), int(k), C.byref(need)))
+    _lib.check(ws_bytes(int(n), int(d), int(k), C.byref(need)))
     ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=X.device)
     off = (-ws.data_ptr()) % 1024
     idx = torch.empty((n, k), dtype=torch.int32, device=X.device)
     d2 = torch.empty((n, k), dtype=torch.float32, device=X.device)
     with torch.cuda.device(X.device):
         stream = torch.cuda.current_stream().cuda_stream
-        _lib.check(lib.mde_knn_approx(X.data_ptr(), int(n), int(d), int(k), C.c_uint64(seed), idx.data_ptr(),
-                                      d2.data_ptr(), ws.data_ptr() + off, need.value, stream))
+        _lib.check(search(*_matrix_args(X), int(n), int(d), int(k), C.c_uint64(seed), idx.data_ptr(), d2.data_ptr(),
+                          ws.data_ptr() + off, need.value, stream))
         torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
     return idx, d2
 
@@ -182,7 +207,8 @@ def _search(data, k, dev, chunk_rows=None):
     """The neighbour search of `k_nearest_neighbors`: (idx [n, k'], squared distances [n, k'] fp32, n) of the
     k' = min(k, n - 1) nearest rows of every row, from the search kernels (int32 indices), or from row chunks of a
     library GEMM + top-k (int64 indices) for k' > 256, dense input with 64 < k' <= 256 (unless PYMDE_B200_KNN=approx),
-    `chunk_rows` or PYMDE_B200_KNN=gemm."""
+    `chunk_rows` or PYMDE_B200_KNN=gemm.  A dense float16 / bfloat16 matrix stays in its dtype on the search kernels
+    and is upcast for the GEMM path."""
     from .. import _lib
     lib = _lib.load()
     mode = os.environ.get("PYMDE_B200_KNN", "kernel")
@@ -199,7 +225,7 @@ def _search(data, k, dev, chunk_rows=None):
             else:
                 idx, d2 = knn_sparse_device(csr, shape, k)
             return idx, d2, n
-    X = _to_device_matrix(data, dev)
+    X = _to_device_matrix(data, dev, keep_half=True)
     n = X.shape[0]
     k = int(min(k, n - 1))
     if use_kernel and 1 <= k <= lib.mde_knn_wide_max_k():
@@ -211,6 +237,7 @@ def _search(data, k, dev, chunk_rows=None):
         # on the GEMM path below, which measured faster on 70 000 x 784 at k = 65 .. 256 (DESIGN section 11.6)
         idx, d2 = knn_device(X, k)
         return idx, d2, n
+    X = X.float()
     sq = (X * X).sum(1)
     rows = chunk_rows or max(256, min(n, int(2 ** 27 // max(n, 1))))
     idxs, vals = [], []
@@ -262,12 +289,13 @@ def k_nearest_neighbors_device_long(data, k, max_distance=None, device=None):
 
 def _pair_distances(data, retain_fraction, dev):
     """(pairs [p, 2] int64 with i < j, Euclidean distances [p] fp32, n) of `distances`, on the device: all pairs in
-    row-major order, or `sample_edges`' sample in its draw order."""
+    row-major order, or `sample_edges`' sample in its draw order.  A dense float16 / bfloat16 matrix stays in its
+    dtype; each chunk of pairs is upcast, which gives the distances of the fp32 matrix."""
     if sp.issparse(data):
         csr, shape = _to_device_csr(data, dev)
         n = shape[0]
     else:
-        X = _to_device_matrix(data, dev)
+        X = _to_device_matrix(data, dev, keep_half=True)
         n = X.shape[0]
     n_all = n * (n - 1) // 2
     if retain_fraction >= 1.0:
@@ -280,7 +308,7 @@ def _pair_distances(data, retain_fraction, dev):
     step = 1 << 22
     for s0 in range(0, edges.shape[0], step):
         e = edges[s0:s0 + step]
-        out[s0:s0 + step] = (X[e[:, 0]] - X[e[:, 1]]).norm(dim=1)
+        out[s0:s0 + step] = (X[e[:, 0]].float() - X[e[:, 1]].float()).norm(dim=1)
     return edges, out, n
 
 

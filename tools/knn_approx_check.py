@@ -3,9 +3,11 @@ after a warm-up on a small matrix), NN-descent iterations, peak device memory, r
 against an fp64 brute force over all n rows (chunked GEMM), and at n <= 10^6 the exact mde_knn / mde_knn_wide on the
 same matrix (the exact search is not run at 10^7: it scales as n^2 d).  At 10^7 it also times the host
 `_knn_graph` (Graph.from_edges) on the result.  Data: a Gaussian mixture of `--intrinsic` dimensions embedded in d by
-a random orthonormal map, plus noise of 1e-2 of the cluster spread.  One JSON line per shape, with the GPU name and
-power limit read in the same run.
-Usage: python tools/knn_approx_check.py [--shapes 1e6x50x15,1e6x784x15,1e6x784x50,1e7x50x15,1e7x784x15] [--reps 3]"""
+a random orthonormal map, plus noise of 1e-2 of the cluster spread; `--dtype fp16|bf16` casts it to that type, which
+both searches read in place (mde_knn16_approx, mde_knn16*).  One JSON line per shape, with the GPU name, power limit
+and max SM clock read in the same run.
+Usage: python tools/knn_approx_check.py [--shapes 1e6x50x15,1e6x784x15,1e6x784x50,1e7x50x15,1e7x784x15] [--reps 3]
+       [--dtype fp32|fp16|bf16]"""
 import argparse, ctypes as C, json, os, subprocess, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -13,25 +15,27 @@ from pymde_b200 import _lib
 from pymde_b200.preprocess import data_matrix as dm
 
 dev = torch.device("cuda", 0)
+DTYPES = {"fp32": torch.float32, "fp16": torch.float16, "bf16": torch.bfloat16}
 
 
 def gpu_identity():
-    out = {"gpu": torch.cuda.get_device_name(dev), "power_limit_w": None}
+    out = {"gpu": torch.cuda.get_device_name(dev), "power_limit_w": None, "max_sm_clock_mhz": None}
     try:
-        r = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
-                           capture_output=True, text=True, timeout=10)
-        out["power_limit_w"] = float(r.stdout.strip())
+        r = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit,clocks.max.sm",
+                            "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=10)
+        p, c = r.stdout.strip().split(",")
+        out["power_limit_w"], out["max_sm_clock_mhz"] = float(p), float(c)
     except Exception:
         pass
     return out
 
 
-def mixture(n, d, intrinsic, seed, clusters=100, chunk=1 << 20):
+def mixture(n, d, intrinsic, seed, clusters=100, chunk=1 << 20, dtype=torch.float32):
     """Built in row chunks, so only X itself is n x d sized."""
     g = torch.Generator(device=dev).manual_seed(seed)
     centres = 4.0 * torch.randn((clusters, intrinsic), generator=g, device=dev)
     Q, _ = torch.linalg.qr(torch.randn((d, intrinsic), generator=g, device=dev))
-    X = torch.empty((n, d), dtype=torch.float32, device=dev)
+    X = torch.empty((n, d), dtype=dtype, device=dev)
     for s0 in range(0, n, chunk):
         m = min(chunk, n - s0)
         lab = torch.randint(0, clusters, (m,), generator=g, device=dev)
@@ -64,13 +68,15 @@ def approx(X, k, seed):
     lib = _lib.load()
     n, d = X.shape
     need = C.c_size_t(0)
-    _lib.check(lib.mde_knn_approx_ws_bytes(n, d, k, C.byref(need)))
+    half = X.dtype != torch.float32
+    _lib.check((lib.mde_knn16_approx_ws_bytes if half else lib.mde_knn_approx_ws_bytes)(n, d, k, C.byref(need)))
     ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=dev)
     idx = torch.empty((n, k), dtype=torch.int32, device=dev)
     d2 = torch.empty((n, k), dtype=torch.float32, device=dev)
     it = C.c_int(0)
-    _lib.check(lib.mde_knn_approx_ex(X.data_ptr(), n, d, k, C.c_uint64(seed), idx.data_ptr(), d2.data_ptr(),
-                                     ws.data_ptr() + (-ws.data_ptr()) % 1024, need.value, None, C.byref(it)))
+    search = lib.mde_knn16_approx_ex if half else lib.mde_knn_approx_ex
+    _lib.check(search(*dm._matrix_args(X), n, d, k, C.c_uint64(seed), idx.data_ptr(), d2.data_ptr(),
+                      ws.data_ptr() + (-ws.data_ptr()) % 1024, need.value, None, C.byref(it)))
     torch.cuda.synchronize()
     return idx, d2, need.value, it.value
 
@@ -85,16 +91,16 @@ def timed(fn, reps):
     return min(ts), ts, out
 
 
-def run(n, d, k, reps, intrinsic, seed=0):
+def run(n, d, k, reps, intrinsic, dtype, seed=0):
     lib = _lib.load()
-    X = mixture(n, d, intrinsic, seed)
+    X = mixture(n, d, intrinsic, seed, dtype=DTYPES[dtype])
     torch.cuda.synchronize()
-    rec = {"n": n, "d": d, "k": k, "intrinsic_dim": intrinsic}
+    rec = {"n": n, "d": d, "k": k, "dtype": dtype, "intrinsic_dim": intrinsic}
     torch.cuda.reset_peak_memory_stats(dev)
     base = torch.cuda.memory_allocated(dev)
     best, ts, (idx, d2, ws_bytes, iterations) = timed(lambda: approx(X, k, seed=1), reps)
     rec.update({"approx_s": best, "approx_all_s": ts, "iterations": iterations,
-                "workspace_gb": ws_bytes / 1e9, "X_gb": n * d * 4 / 1e9,
+                "workspace_gb": ws_bytes / 1e9, "X_gb": X.numel() * X.element_size() / 1e9,
                 "peak_device_gb": torch.cuda.max_memory_allocated(dev) / 1e9,
                 "peak_above_X_gb": (torch.cuda.max_memory_allocated(dev) - base) / 1e9})
     g = torch.Generator(device=dev).manual_seed(123)
@@ -106,7 +112,9 @@ def run(n, d, k, reps, intrinsic, seed=0):
     rec["rows_all_found_4096"] = float((hits == k).float().mean())
     if n <= 10 ** 6:
         name = "mde_knn_s" if k <= lib.mde_knn_max_k() else "mde_knn_wide_s"
+        torch.cuda.reset_peak_memory_stats(dev)
         ebest, ets, (ei, ed) = timed(lambda: dm.knn_device(X, k), min(reps, 2))
+        rec["exact_peak_above_X_gb"] = (torch.cuda.max_memory_allocated(dev) - base) / 1e9
         rec.update({name: ebest, name.replace("_s", "_all_s"): ets, "speedup_vs_exact": ebest / best})
         same = (torch.sort(ei.long(), 1)[0] == torch.sort(idx.long(), 1)[0]).all(1)
         rec["rows_identical_to_exact"] = float(same.float().mean())
@@ -132,15 +140,16 @@ def main():
     ap.add_argument("--shapes", default="1e6x50x15,1e6x784x15,1e6x784x50,1e7x50x15,1e7x784x15")
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--intrinsic", type=int, default=16)
+    ap.add_argument("--dtype", default="fp32", choices=sorted(DTYPES))
     a = ap.parse_args()
     # warm-up: module loads of both searches on a small matrix
-    Xw = mixture(20000, 64, a.intrinsic, 99)
+    Xw = mixture(20000, 64, a.intrinsic, 99, dtype=DTYPES[a.dtype])
     for kw in (15, 50):
         approx(Xw, kw, 1); dm.knn_device(Xw, kw)
     del Xw
     for s in a.shapes.split(","):
         n, d, k = s.split("x")
-        run(int(float(n)), int(d), int(k), a.reps, a.intrinsic)
+        run(int(float(n)), int(d), int(k), a.reps, a.intrinsic, a.dtype)
 
 
 if __name__ == "__main__":

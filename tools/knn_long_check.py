@@ -8,7 +8,11 @@ in the same run.
   (b)     the same matrix as CSR (DESIGN section 11.1) at k = 65 and 256 (best of 3 after a warm-up)
   (a)     text-like 3e5 x 1e5 (120 GB dense) at k = 100, one run
 
-Usage: python tools/knn_long_check.py [--parts dense,b,a] [--rows 4096]
+`--dtype fp16|bf16` casts the dense matrix to that type, which mde_knn16_long (and mde_knn16_wide at k = 64) read in
+place; the GEMM path and the parity check work on its fp32 upcast.  Dense lines also carry the peak device memory of
+the search above the input.
+
+Usage: python tools/knn_long_check.py [--parts dense,b,a] [--rows 4096] [--dtype fp32|fp16|bf16]
 """
 import argparse
 import json
@@ -27,6 +31,7 @@ from pymde_b200.preprocess import data_matrix as dm  # noqa: E402
 from tools.knn_sparse_check import host_brute, mnist_like, text_like, timed  # noqa: E402
 
 dev = torch.device("cuda", 0)
+DTYPES = {"fp32": torch.float32, "fp16": torch.float16, "bf16": torch.bfloat16}
 
 
 def gpu_identity():
@@ -83,27 +88,40 @@ def dense_parity(X, idx, d2, rows):
     return out
 
 
-def run_dense(n_rows):
+def peak_above(fn):
+    """Peak device memory allocated by fn() above what was allocated before it, in bytes."""
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats(dev)
+    base = torch.cuda.memory_allocated(dev)
+    out = fn()
+    torch.cuda.synchronize()
+    del out
+    return torch.cuda.max_memory_allocated(dev) - base
+
+
+def run_dense(n_rows, dtype):
     Xn = mnist_like()
-    X = torch.from_numpy(Xn).to(dev)
+    X = torch.from_numpy(Xn).to(dev).to(DTYPES[dtype])
     rows = np.random.default_rng(1).choice(X.shape[0], n_rows, replace=False)
-    w = torch.from_numpy(mnist_like(4096, seed=3)).to(dev)
+    w = torch.from_numpy(mnist_like(4096, seed=3)).to(dev).to(DTYPES[dtype])
     for k in (64, 65, 256):  # warm-up: module loads and the GEMM path's algorithm choice
         dm.knn_device(w, k)
         gemm_topk(w, k)
     res = {}
     t = timed(lambda: res.__setitem__("w", dm.knn_device(X, 64)))
-    emit({"part": "dense", "n": 70000, "d": 784, "k": 64, "kernel": "mde_knn_wide", "search_s": round(t, 4),
-          "timing": "best of 3 after a warm-up"})
+    emit({"part": "dense", "n": 70000, "d": 784, "k": 64, "dtype": dtype, "kernel": "mde_knn_wide",
+          "search_s": round(t, 4), "timing": "best of 3 after a warm-up",
+          "peak_above_input_bytes": peak_above(lambda: dm.knn_device(X, 64))})
     del res["w"]
     for k in (65, 128, 256):
         t_long = timed(lambda: res.__setitem__("long", dm.knn_device(X, k)))
         t_gemm = timed(lambda: res.__setitem__("gemm", gemm_topk(X, k)))
         del res["gemm"]
         idx, d2 = res.pop("long")
-        line = {"part": "dense", "n": 70000, "d": 784, "k": k, "kernel": "mde_knn_long", "search_s": round(t_long, 4),
-                "gemm_topk_s": round(t_gemm, 4), "timing": "best of 3 after a warm-up"}
-        line.update({"parity_" + a: b for a, b in dense_parity(X, idx, d2, rows).items()})
+        line = {"part": "dense", "n": 70000, "d": 784, "k": k, "dtype": dtype, "kernel": "mde_knn_long",
+                "search_s": round(t_long, 4), "gemm_topk_s": round(t_gemm, 4), "timing": "best of 3 after a warm-up",
+                "peak_above_input_bytes": peak_above(lambda: dm.knn_device(X, k))}
+        line.update({"parity_" + a: b for a, b in dense_parity(X.float(), idx, d2, rows).items()})
         emit(line)
         del idx, d2
     torch.cuda.empty_cache()
@@ -147,6 +165,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--parts", default="dense,b,a")
     ap.add_argument("--rows", type=int, default=4096, help="rows sampled for the dense parity check")
+    ap.add_argument("--dtype", default="fp32", choices=sorted(DTYPES), help="element type of the dense matrix")
     a = ap.parse_args()
     torch.cuda.init()
     assert _lib.load().mde_knn_long_max_k() == 256
@@ -156,7 +175,7 @@ def main():
     dm.knn_sparse_device(cw, sw, 100)  # warm-up of the sparse search
     del cw
     if "dense" in parts:
-        run_dense(a.rows)
+        run_dense(a.rows, a.dtype)
     if "b" in parts:
         run_sparse("b_mnist_like_csr", sp.csr_matrix(mnist_like()), [65, 256], 3, 256)
     if "a" in parts:
