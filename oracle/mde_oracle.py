@@ -69,10 +69,10 @@ def _eval_one(fn, sc, d, a, b, dt):
     with np.errstate(all="ignore"):
         if fn == P_LINEAR:  # penalties.py:112-120
             return a * d, a * np.ones_like(d)
-        if fn == P_QUADRATIC:  # :123-131
-            return a * d * d, dt(2.0) * a * d
+        if fn == P_QUADRATIC:  # :123-131  w * d^2: a zero weight times an overflowed d^2 is NaN
+            return a * (d * d), dt(2.0) * a * d
         if fn == P_CUBIC:  # :163-171
-            return a * d * d * d, dt(3.0) * a * d * d
+            return a * (d * d * d), dt(3.0) * a * d * d
         if fn == P_POWER:  # :191-202
             return a * np.power(d, s0), a * s0 * np.power(d, s0 - one)
         if fn == P_HUBER:  # :205-243  (s0 = threshold)
@@ -95,10 +95,22 @@ def _eval_one(fn, sc, d, a, b, dt):
             return f, fp
         if fn == P_INVPOWER:  # :340-353
             aw = np.abs(a)
-            return aw / np.power(d, s0), -aw * s0 * np.power(d, -s0 - one)
+            de = np.power(d, s0)
+            fp = -aw * s0 * np.power(d, -s0 - one)
+            # the reference's chain rule -((|w| / x) / x) (e d^(e-1)), x = d^e, is not finite where an intermediate
+            # overflows or meets inf * 0 (NaN at d = 0 for e > 1); where it is finite and the closed form is not (a zero
+            # weight times d^(-e-1) = inf), its value is the reference's
+            chain = -((aw / de) / de) * (s0 * np.power(d, s0 - one))
+            return aw / de, np.where(np.isfinite(chain) & np.isfinite(fp), fp, chain)
         if fn == P_LOGRATIO:  # :356-369
             de = np.power(d, s0)
-            return a * np.log(de / (one + de)), a * s0 / (d * (one + de))
+            y = de / (one + de)
+            fp = a * s0 / (d * (one + de))
+            # the reference's chain rule ((w / y) / (1 + x) - (w / y) x / (1 + x)^2) (e d^(e-1)), x = d^e, is NaN
+            # where x is 0 (inf * 0) or overflows (y = inf / inf)
+            gy = a / y
+            chain = (gy / (one + de) - gy * de / ((one + de) * (one + de))) * (s0 * np.power(d, s0 - one))
+            return a * np.log(y), np.where(np.isfinite(chain) & np.isfinite(fp), fp, chain)
         # losses: a = deviations
         r = np.abs(a - d)
         sg = _sign(d - a)

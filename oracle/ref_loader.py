@@ -8,11 +8,14 @@ under tests/golden/ (tests/golden/make_golden.py, make_api_golden.py).
 The reference eagerly imports matplotlib (pymde/__init__.py:17 ->
 pymde/experiment_utils.py:1-3) and pynndescent (pymde/preprocess/data_matrix.py:116),
 neither of which is installed here; plotting and approximate k-NN are outside the
-hot path, so empty stub modules are registered in sys.modules before the import.
+hot path, so empty stub modules are registered in sys.modules before the import.  So is the Cython graph
+extension `pymde.preprocess._graph` when the checkout has none built: only the graph preprocessing uses it, and the
+distortion functions import and run without it.
 Nothing in the product (`pymde_b200/`) may import this file.
 """
 import importlib
 import os
+from importlib.machinery import EXTENSION_SUFFIXES
 import sys
 import types
 
@@ -57,6 +60,10 @@ def load_reference():
     _stub("mpl_toolkits.axes_grid1", make_axes_locatable=None)
     _stub("mpl_toolkits.mplot3d")
     _stub("pynndescent")
+    # a checkout whose Cython graph extension was never built: the distortion functions do not use it
+    pre = os.path.join(root, "pymde", "preprocess")
+    if not any(os.path.exists(os.path.join(pre, "_graph" + sfx)) for sfx in EXTENSION_SUFFIXES):
+        sys.modules.setdefault("pymde.preprocess._graph", types.ModuleType("pymde.preprocess._graph"))
     sys.path.insert(0, root)
     try:
         return importlib.import_module("pymde")

@@ -68,10 +68,10 @@ __device__ __forceinline__ void eval_fn_t(float s0, float s1, float d, float a, 
     f = a * d; fp = a;
   }
   else if constexpr (FN == MDE_FN_P_QUADRATIC) {
-    f = a * d * d; fp = 2.0f * a * d;
+    f = a * (d * d); fp = 2.0f * a * d;  // w d^2: a zero weight times an overflowed d^2 is NaN, like the reference
   }
   else if constexpr (FN == MDE_FN_P_CUBIC) {
-    f = a * d * d * d; fp = 3.0f * a * d * d;
+    f = a * (d * d * d); fp = 3.0f * a * d * d;
   }
   else if constexpr (FN == MDE_FN_P_POWER) {
     float de, dem1; pow_pair(d, s0, de, dem1);
@@ -96,12 +96,19 @@ __device__ __forceinline__ void eval_fn_t(float s0, float s1, float d, float a, 
   }
   else if constexpr (FN == MDE_FN_P_INVPOWER) {
     float de, dem1; pow_pair(d, s0, de, dem1);
+      // f' = -|w| e d^(e-1) / d^(2e) along the reference's chain rule ((|w| / d^e) / d^e) (e d^(e-1)): finite exactly
+      // where the reference's is (a form like 1 / (d^e d) underflows and overflows at other d)
       float aw = fabsf(a);
-      f = aw / de; fp = -aw * s0 / (de * d);
+      f = aw / de; fp = -((aw / de) / de) * (s0 * dem1);
   }
   else if constexpr (FN == MDE_FN_P_LOGRATIO) {
     float de, dem1; pow_pair(d, s0, de, dem1);
-      f = a * logf(de / (1.0f + de)); fp = a * s0 / (d * (1.0f + de));
+      // f' = w e d^(e-1) / (d^e (1 + d^e)), evaluated along the reference's chain rule: (w / y) (e d^(e-1)) / (1 + d^e)^2,
+      // y = d^e / (1 + d^e).  It is finite wherever the reference's is (no product like d d^e that underflows first),
+      // and NaN where d^e is 0 or overflows, as the reference's is
+      const float y = de / (1.0f + de);
+      const float r = 1.0f / (1.0f + de);
+      f = a * logf(y); fp = (a / y) * (s0 * dem1) * r * r;
   }
   else if constexpr (FN == MDE_FN_L_ABSOLUTE) {
     f = fabsf(a - d); fp = signf(d - a);
@@ -183,8 +190,9 @@ __device__ __forceinline__ void edge_f_fp(const FnDev& fn, float d, float a, flo
 }
 
 // Per-edge distortion f_k(d) and gradient coefficient g_k = f'_k(d) / (p d), with the
-// reference's guard: non-finite g -> 1.0 (pymde/average_distortion.py:55-62; it only fires
-// when d = 0, where the difference vector is 0 too).
+// reference's guard: non-finite g -> 1.0 (pymde/average_distortion.py:55-62).  At d = 0 the difference vector is 0
+// too; at d > 0 the guard moves the pair by g = 1 wherever the reference's f' is not finite: LogRatio where d^e
+// underflows or overflows, loss Power(delta, e < 1) at d = delta, loss Logistic where exp(|d - delta|) overflows.
 template <int FA, int FR>
 __device__ __forceinline__ void edge_coeff(const FnDev& fn, float d, float a, float b, float inv_p,
                                            float& f, float& g) {
