@@ -103,7 +103,7 @@ int mde_edges_create_ex(mde_edges_t** out, const int64_t* edges, int64_t p, int6
                         int64_t p_total, int embedding_dim, void* stream);
 int mde_edges_destroy(mde_edges_t* e);
 int64_t mde_edges_count(const mde_edges_t* e);
-/* which layout / kernel family the library chose: 0 = sorted SoA (quad / strided / wide kernels), 1 = tile records
+/* which layout / kernel family the library chose: 0 = sorted SoA (owner / quad / wide kernels), 1 = tile records
  * (push kernel, shared-memory dst tile), 2 = pull records (directed entries, no shared-memory atomics), 3 = sorted SoA
  * + ELL pull records (one lane per owner, pymde_b200/csrc/mde_ell.cu: the fused evaluation runs on the ELL kernel,
  * value-only / per-edge outputs / external coefficients on the SoA kernels).

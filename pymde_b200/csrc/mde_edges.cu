@@ -15,10 +15,9 @@
 // Kernel shapes
 //   m <= 4, default (fused value + gradient and external coefficients): distortion_owner_kernel walks the directed
 //            entries `ent` grouped by owner node, 8 lanes per node, sum in registers, one write per row, no atomics.
-//   m <= 4, value only / MDE_B200_DETERMINISTIC / other m: one thread per edge (quad or strided kernel); the lhs
-//            contributions (sorted => runs of equal src) are summed with a warp segmented
-//            reduction and issued as ONE vector red per run; rhs contributions go out as
-//            vector reds (REDG.E.ADD.F32x2/x4).
+//   m <= 4, value only / MDE_B200_DETERMINISTIC / other m: one thread per 4 consecutive edges (quad kernel); the
+//            lhs contributions (sorted => runs of equal src) are summed in registers and issued as ONE vector red
+//            per run; rhs contributions go out as vector reds (REDG.E.ADD.F32x2/x4).
 //   m >= 5 : a group of G lanes (8/16/32) walks a contiguous slice of edges; the lhs row and
 //            its gradient accumulator stay in registers across a run.
 //   5 <= m <= 512, MDE_B200_DETERMINISTIC (fused and external coefficients): distortion_wide_owner_kernel, one group
@@ -37,9 +36,6 @@ unsigned long long g_launch_count = 0;
 }
 
 using namespace mde;
-
-static constexpr int kSmallThreads = 256;
-static constexpr int kRounds = 4;  // 32-edge rounds per warp iteration
 
 // ------------------------------------------------------------------------------------------
 // layout build
@@ -125,91 +121,6 @@ __global__ void fx_apply_kernel(const int* __restrict__ flag, const long long* _
     grad[i] += (float)((double)F[i] * (1.0 / 1099511627776.0));
 }
 
-// MODE 0: fused value + gradient; 1: value only; 2: external per-edge g (gradient only)
-template <int M, int MODE, int FA, int FR>
-__global__ void __launch_bounds__(kSmallThreads)
-distortion_small_kernel(const int32_t* __restrict__ src, const int32_t* __restrict__ dst,
-                        const float* __restrict__ par0, const float* __restrict__ par1,
-                        const int32_t* __restrict__ perm, const float* __restrict__ gext,
-                        int64_t p, const float* __restrict__ X, float* __restrict__ grad,
-                        double* __restrict__ loss_partials, FnDev fn, float inv_p,
-                        const int* __restrict__ flag) {
-  if (flag != nullptr && *flag == 0) return;
-  const int lane = threadIdx.x & 31;
-  const int64_t warp0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  constexpr int64_t kPerWarp = 32 * kRounds;
-  double lsum = 0.0;
-
-  for (int64_t base = warp0 * kPerWarp; base < p; base += nwarps * kPerWarp) {
-    int s[kRounds], t[kRounds];
-    float a[kRounds], b[kRounds];
-    bool ok[kRounds];
-    // Out-of-range lanes re-read the last edge (index clamp) instead of selecting zeros: every lane
-    // then holds valid row indices and no address is formed from a predicated value.
-#pragma unroll
-    for (int r = 0; r < kRounds; ++r) {
-      int64_t k = base + r * 32 + lane;
-      ok[r] = k < p;
-      const int64_t kk = ok[r] ? k : (p - 1);
-      s[r] = __ldg(src + kk);
-      t[r] = __ldg(dst + kk);
-      if (MODE == 2) a[r] = __ldg(gext + __ldg(perm + kk));
-      else a[r] = __ldg(par0 + kk);
-      b[r] = (MODE != 2 && par1 != nullptr) ? __ldg(par1 + kk) : 0.0f;
-    }
-    Row<M> xi[kRounds], xj[kRounds];
-#pragma unroll
-    for (int r = 0; r < kRounds; ++r) {
-      xi[r] = ldg_row<M>(X, s[r]);
-      xj[r] = ldg_row<M>(X, t[r]);
-    }
-#pragma unroll
-    for (int r = 0; r < kRounds; ++r) {
-      float diff[M];
-      float d2 = 0.0f;
-#pragma unroll
-      for (int c = 0; c < M; ++c) { diff[c] = xi[r].v[c] - xj[r].v[c]; d2 += diff[c] * diff[c]; }
-      float g;
-      if (MODE == 2) {
-        g = a[r];
-      } else {
-        float d = sqrtf(d2), f;
-        if (MODE == 0) edge_coeff<FA, FR>(fn, d, a[r], b[r], inv_p, f, g);
-        else { edge_value<FA, FR>(fn, d, a[r], b[r], f); g = 0.0f; }
-        if (ok[r]) lsum += (double)f;
-      }
-      if (MODE != 1) {
-        float v[M];
-#pragma unroll
-        for (int c = 0; c < M; ++c) v[c] = ok[r] ? g * diff[c] : 0.0f;
-        if (ok[r]) red_row<M>(grad, t[r], v, -1.0f);
-        // lhs: sorted => equal keys are adjacent lanes; segmented warp reduction
-        int key = ok[r] ? s[r] : (-1 - lane);
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-          int k2 = __shfl_down_sync(kFull, key, off);
-          bool take = (lane + off < 32) && (k2 == key);
-#pragma unroll
-          for (int c = 0; c < M; ++c) {
-            float o = __shfl_down_sync(kFull, v[c], off);
-            if (take) v[c] += o;
-          }
-        }
-        int kprev = __shfl_up_sync(kFull, key, 1);
-        bool head = (lane == 0) || (kprev != key);
-        if (head && ok[r]) red_row<M>(grad, s[r], v, 1.0f);
-      }
-    }
-  }
-  if (MODE != 2) {
-    __shared__ double sm[32];
-    double v1[1] = {lsum};
-    block_sum<1>(v1, sm);
-    if (threadIdx.x == 0) loss_partials[blockIdx.x] = v1[0];
-  }
-}
-
 // ------------------------------------------------------------------------------------------
 // m <= 4, thread-contiguous variant: each thread owns 4 CONSECUTIVE sorted edges (three 16-byte
 // loads for src/dst/par0), sums the lhs contributions of equal-src runs in registers and issues one
@@ -248,7 +159,7 @@ __device__ __forceinline__ bool edge_contribution(const Row<M>& xs, const Row<M>
   return live;
 }
 
-template <int M, int MODE, int FA, int FR, bool FAST, int NQ>
+template <int M, int MODE, int FA, int FR, bool FAST>
 __global__ void __launch_bounds__(kQuadThreads)
 distortion_quad_kernel(const int32_t* __restrict__ src, const int32_t* __restrict__ dst,
                        const float* __restrict__ par0, const float* __restrict__ par1,
@@ -257,76 +168,63 @@ distortion_quad_kernel(const int32_t* __restrict__ src, const int32_t* __restric
                        double* __restrict__ loss_partials, FnDev fn, float inv_p,
                        const int* __restrict__ flag, long long* __restrict__ fx) {
   if (flag != nullptr && *flag == 0) return;
-  constexpr int E = 4 * NQ;  // consecutive edges owned by a thread per iteration
   const int64_t nquads = (p + 3) >> 2;
-  const int64_t nunits = (nquads + NQ - 1) / NQ;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   float lsum_f = 0.0f;
   double lsum = 0.0;
-  // software pipeline (NQ == 1): the edge record of the NEXT grid-stride iteration is requested before the
+  // software pipeline (MODE 0 and 1): the edge record of the NEXT grid-stride iteration is requested before the
   // vertex rows of the current one are gathered, so its latency overlaps the gathers and the math
   int4 s4n = make_int4(0, 0, 0, 0), t4n = make_int4(0, 0, 0, 0);
   float4 a4n = make_float4(0.f, 0.f, 0.f, 0.f);
-  const bool pipe = (NQ == 1 && MODE != 2);
+  constexpr bool pipe = MODE != 2;
   {
     const int64_t u0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (pipe && u0 < nunits) {
+    if (pipe && u0 < nquads) {
       s4n = __ldg(reinterpret_cast<const int4*>(src) + u0);
       t4n = __ldg(reinterpret_cast<const int4*>(dst) + u0);
       a4n = __ldg(reinterpret_cast<const float4*>(par0) + u0);
     }
   }
-  for (int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; u < nunits; u += stride) {
-    int s[E], t[E];
-    float a[E], b[E];
-#pragma unroll
-    for (int j = 0; j < NQ; ++j) {
-      const int64_t q = u * NQ + j;
-      const int64_t qc = q < nquads ? q : nquads - 1;  // clamped: masked below through `ok`
-      int4 s4, t4;
-      if (pipe) {
-        s4 = s4n; t4 = t4n;
-        const int64_t un = u + stride;
-        if (un < nunits) {
-          s4n = __ldg(reinterpret_cast<const int4*>(src) + un);
-          t4n = __ldg(reinterpret_cast<const int4*>(dst) + un);
-        }
-      } else {
-        s4 = __ldg(reinterpret_cast<const int4*>(src) + qc);
-        t4 = __ldg(reinterpret_cast<const int4*>(dst) + qc);
+  for (int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; u < nquads; u += stride) {
+    int s[4], t[4];
+    float a[4], b[4];
+    int4 s4, t4;
+    if (pipe) {
+      s4 = s4n; t4 = t4n;
+      const int64_t un = u + stride;
+      if (un < nquads) {
+        s4n = __ldg(reinterpret_cast<const int4*>(src) + un);
+        t4n = __ldg(reinterpret_cast<const int4*>(dst) + un);
       }
-      s[4 * j] = s4.x; s[4 * j + 1] = s4.y; s[4 * j + 2] = s4.z; s[4 * j + 3] = s4.w;
-      t[4 * j] = t4.x; t[4 * j + 1] = t4.y; t[4 * j + 2] = t4.z; t[4 * j + 3] = t4.w;
-      if (MODE == 2) {
-        const int4 o4 = __ldg(reinterpret_cast<const int4*>(perm) + qc);  // pad entries repeat the last edge
-        a[4 * j] = __ldg(gext + o4.x); a[4 * j + 1] = __ldg(gext + o4.y);
-        a[4 * j + 2] = __ldg(gext + o4.z); a[4 * j + 3] = __ldg(gext + o4.w);
-      } else {
-        float4 a4;
-        if (pipe) {
-          a4 = a4n;
-          const int64_t un = u + stride;
-          if (un < nunits) a4n = __ldg(reinterpret_cast<const float4*>(par0) + un);
-        } else {
-          a4 = __ldg(reinterpret_cast<const float4*>(par0) + qc);
-        }
-        a[4 * j] = a4.x; a[4 * j + 1] = a4.y; a[4 * j + 2] = a4.z; a[4 * j + 3] = a4.w;
-      }
-      if (MODE != 2 && par1 != nullptr) {
-        const float4 b4 = __ldg(reinterpret_cast<const float4*>(par1) + qc);
-        b[4 * j] = b4.x; b[4 * j + 1] = b4.y; b[4 * j + 2] = b4.z; b[4 * j + 3] = b4.w;
-      } else { b[4 * j] = b[4 * j + 1] = b[4 * j + 2] = b[4 * j + 3] = 0.0f; }
+    } else {
+      s4 = __ldg(reinterpret_cast<const int4*>(src) + u);
+      t4 = __ldg(reinterpret_cast<const int4*>(dst) + u);
     }
-    Row<M> xi[E], xj[E];
+    s[0] = s4.x; s[1] = s4.y; s[2] = s4.z; s[3] = s4.w;
+    t[0] = t4.x; t[1] = t4.y; t[2] = t4.z; t[3] = t4.w;
+    if (MODE == 2) {
+      const int4 o4 = __ldg(reinterpret_cast<const int4*>(perm) + u);  // pad entries repeat the last edge
+      a[0] = __ldg(gext + o4.x); a[1] = __ldg(gext + o4.y); a[2] = __ldg(gext + o4.z); a[3] = __ldg(gext + o4.w);
+    } else {
+      const float4 a4 = a4n;
+      const int64_t un = u + stride;
+      if (un < nquads) a4n = __ldg(reinterpret_cast<const float4*>(par0) + un);
+      a[0] = a4.x; a[1] = a4.y; a[2] = a4.z; a[3] = a4.w;
+    }
+    if (MODE != 2 && par1 != nullptr) {
+      const float4 b4 = __ldg(reinterpret_cast<const float4*>(par1) + u);
+      b[0] = b4.x; b[1] = b4.y; b[2] = b4.z; b[3] = b4.w;
+    } else { b[0] = b[1] = b[2] = b[3] = 0.0f; }
+    Row<M> xi[4], xj[4];
 #pragma unroll
-    for (int e = 0; e < E; ++e) { xi[e] = ldg_row<M>(X, s[e]); xj[e] = ldg_row<M>(X, t[e]); }
+    for (int e = 0; e < 4; ++e) { xi[e] = ldg_row<M>(X, s[e]); xj[e] = ldg_row<M>(X, t[e]); }
     float acc[M];
 #pragma unroll
     for (int c = 0; c < M; ++c) acc[c] = 0.0f;
     int cur = s[0];
 #pragma unroll
-    for (int e = 0; e < E; ++e) {
-      const bool ok = (4 * (u * NQ) + e) < p;
+    for (int e = 0; e < 4; ++e) {
+      const bool ok = 4 * u + e < p;
       float f, v[M];
       const bool live = edge_contribution<M, MODE, FA, FR, FAST>(xi[e], xj[e], a[e], b[e], fn, inv_p, ok, f, v);
       if (MODE != 2 && ok) { if (FAST) lsum_f += f; else lsum += (double)f; }
@@ -837,37 +735,14 @@ __global__ void function_eval_kernel(FnDev fn, const float* __restrict__ par0, i
 // ------------------------------------------------------------------------------------------
 namespace mde {
 
-int loss_blocks_small(int64_t p) {
-  int64_t per_block = (int64_t)(kSmallThreads / 32) * 32 * kRounds;
+// the quad kernel's grid is capped at one resident wave, 4 blocks per SM
+static constexpr int kQuadBlocksPerSM = 4;
+
+int loss_blocks_quad(int64_t p) {
+  int64_t per_block = (int64_t)kQuadThreads * 4;
   int64_t nb = (p + per_block - 1) / per_block;
   if (nb < 1) nb = 1;
-  if (nb > kNumSMs * 8) nb = kNumSMs * 8;
-  return (int)nb;
-}
-
-// A/B switches for measurements, read when a layout is created (mde_edges::kvar / nq / qbps):
-//   MDE_B200_KERNEL=strided   the lane-strided kernel with the warp segmented reduction (sorted SoA)
-//   MDE_B200_KERNEL=precise   the thread-contiguous / tile kernels with IEEE math instead of the MUFU forms
-//   MDE_B200_NQ=2             two consecutive quads per thread in the FAST quad kernel (default 1)
-//   MDE_B200_QUAD_BPS=k       blocks per SM in the quad kernel's grid cap (default 4 = one resident wave)
-static void read_kernel_switches(mde_edges* e) {
-  const char* ev = getenv("MDE_B200_KERNEL");
-  e->kvar = 0;
-  if (ev && !strcmp(ev, "strided")) e->kvar = 1;
-  if (ev && !strcmp(ev, "precise")) e->kvar = 2;
-  ev = getenv("MDE_B200_NQ");
-  e->nq = (ev && ev[0] == '2') ? 2 : 1;
-  int v = env_int("MDE_B200_QUAD_BPS", 4);
-  if (v < 1) v = 1;
-  if (v > 16) v = 16;
-  e->qbps = v;
-}
-
-int loss_blocks_quad(int64_t p, int nq, int bps) {
-  int64_t per_block = (int64_t)kQuadThreads * 4 * nq;
-  int64_t nb = (p + per_block - 1) / per_block;
-  if (nb < 1) nb = 1;
-  if (nb > kNumSMs * bps) nb = kNumSMs * bps;
+  if (nb > kNumSMs * kQuadBlocksPerSM) nb = kNumSMs * kQuadBlocksPerSM;
   return (int)nb;
 }
 
@@ -888,13 +763,10 @@ int loss_blocks_wide(int64_t p, int G) {
   return (int)nb;
 }
 
-// compile-time function pairs of the quad / owner kernels and of the strided kernel (fused mode, m = 2 / 3)
+// compile-time function pairs of the quad / owner kernels (fused mode, m = 2 / 3)
 using QuadPairs = FnList<Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>, Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOGRATIO>, Fn1<MDE_FN_P_QUADRATIC>,
                          Fn1<MDE_FN_L_ABSOLUTE>, Fn1<MDE_FN_L_QUADRATIC>, Fn1<MDE_FN_L_WEIGHTED_QUADRATIC>,
                          Fn1<MDE_FN_L_HUBER>>;
-using StridedPairs = FnList<Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>, Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOGRATIO>,
-                            Fn1<MDE_FN_P_QUADRATIC>, Fn1<MDE_FN_P_LOG1P>, Fn1<MDE_FN_L_ABSOLUTE>, Fn1<MDE_FN_L_QUADRATIC>,
-                            Fn1<MDE_FN_L_WEIGHTED_QUADRATIC>, Fn1<MDE_FN_L_HUBER>>;
 
 // one evaluation on the sorted-SoA layout; the launch helpers return the grid size (= loss partials)
 struct SoaLaunch {
@@ -926,37 +798,23 @@ int launch_quad(const SoaLaunch& l) {
     if (l.owner) return launch_owner<M, MODE, FA, FR, FAST>(l);
   }
   const mde_edges* e = l.e;
-  const int nq = (FAST && e->nq == 2) ? 2 : 1;
-  const int nb = loss_blocks_quad(e->p, nq, e->qbps);
-  auto k = nq == 2 ? &distortion_quad_kernel<M, MODE, FA, FR, FAST, 2> : &distortion_quad_kernel<M, MODE, FA, FR, FAST, 1>;
-  k<<<nb, kQuadThreads, 0, l.st>>>(e->src, e->dst, e->par0, l.par1(), e->perm, l.gext, e->p, l.X, l.grad,
-                                   e->loss_partials, e->fn, l.inv_p, l.flag, l.fx);
-  return nb;
-}
-
-template <int M, int MODE, int FA, int FR>
-int launch_strided(const SoaLaunch& l) {
-  const mde_edges* e = l.e;
-  const int nb = loss_blocks_small(e->p);
-  distortion_small_kernel<M, MODE, FA, FR><<<nb, kSmallThreads, 0, l.st>>>(
-      e->src, e->dst, e->par0, l.par1(), e->perm, l.gext, e->p, l.X, l.grad, e->loss_partials, e->fn, l.inv_p, l.flag);
+  const int nb = loss_blocks_quad(e->p);
+  distortion_quad_kernel<M, MODE, FA, FR, FAST><<<nb, kQuadThreads, 0, l.st>>>(
+      e->src, e->dst, e->par0, l.par1(), e->perm, l.gext, e->p, l.X, l.grad, e->loss_partials, e->fn, l.inv_p, l.flag,
+      l.fx);
   return nb;
 }
 
 template <int M, int MODE>
 int launch_small(const SoaLaunch& l) {
   const FnDev& fn = l.e->fn;
-  if (l.e->kvar == 1) {
-    return select_fn<M, MODE>(fn, false, StridedPairs{},
-                              [&](auto f) { using F = decltype(f); return launch_strided<M, MODE, F::FA, F::FR>(l); });
-  }
   if constexpr (MODE == 0 && (M == 1 || M == 4)) {
     // m = 1, 4: the owner kernel evaluates every edge twice, so the recipe default PushAndPull(Log1p, Log) gets
     // compile-time ids there (IEEE math, as the run-time table) instead of two out-of-line calls
     if (l.owner && Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>::matches(fn))
       return launch_owner<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOG, false>(l);
   }
-  return select_fn<M, MODE>(fn, fast_log1p_log(fn, l.e->kvar == 2), QuadPairs{}, [&](auto f) {
+  return select_fn<M, MODE>(fn, fast_log1p_log(fn, l.e->precise), QuadPairs{}, [&](auto f) {
     using F = decltype(f);
     return launch_quad<M, MODE, F::FA, F::FR, F::FAST>(l);
   });
@@ -1009,7 +867,7 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
   // deterministic mode (m <= 4, sorted-SoA layout): zero the fixed-point buffer, accumulate into it, add it to grad.
   // A deterministic layout built for m >= 5 has no fixed-point buffer: it evaluates its own m on the wide owner kernel
   // (launch_wide).
-  if (e->det && e->fx && MODE != 1 && m <= 4 && m <= e->m_hint && e->kvar != 1) {
+  if (e->det && e->fx && MODE != 1 && m <= 4 && m <= e->m_hint) {
     l.fx = e->fx;
     const int64_t cnt = e->n * m;
     int zb = (int)((cnt + 255) / 256); if (zb > kNumSMs * 8) zb = kNumSMs * 8;
@@ -1017,7 +875,7 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
     ++g_launch_count;
   }
   // default on the sorted-SoA layout: the owner kernel over the directed entries, in place of the quad kernel
-  l.owner = !l.fx && e->ent && MODE != 1 && m == e->m_hint && e->kvar != 1;
+  l.owner = !l.fx && e->ent && MODE != 1 && m == e->m_hint;
   int nb;
   if (m == 1) nb = launch_small<1, MODE>(l);
   else if (m == 2) nb = launch_small<2, MODE>(l);
@@ -1142,7 +1000,7 @@ int mde_edges_create(mde_edges_t** out, const int64_t* edges, int64_t p, int64_t
   return mde_edges_create_ex(out, edges, p, n_items, par0, par1, fn, p_total, 2, stream);
 }
 
-// layout choice: MDE_B200_LAYOUT=soa forces the sorted-SoA layout (quad / strided kernels), =tiles insists on
+// layout choice: MDE_B200_LAYOUT=soa forces the sorted-SoA layout (owner / quad / wide kernels), =tiles insists on
 // the tile-record layout whenever it can be built; default: tiles for m <= 4 without a second parameter array
 static int layout_pref() {  // read at every create: A/B runs build both layouts in one process
   const char* ev = getenv("MDE_B200_LAYOUT");
@@ -1163,7 +1021,7 @@ int mde_edges_create_ex(mde_edges_t** out, const int64_t* edges, int64_t p, int6
   mde_edges* e = new (std::nothrow) mde_edges();
   if (!e) return MDE_E_ALLOC;
   e->p = p; e->n = n_items; e->p_total = p_total; e->fn = to_dev(*fn); e->has_par1 = par1 != nullptr;
-  read_kernel_switches(e);
+  { const char* ev = getenv("MDE_B200_KERNEL"); e->precise = ev && !strcmp(ev, "precise"); }
 
   uint64_t *keys_in = nullptr, *keys_out = nullptr;
   int32_t *vals_in = nullptr, *vals_out = nullptr;

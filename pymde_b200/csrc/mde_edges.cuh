@@ -46,10 +46,9 @@ struct mde_edges {
   mde::FnDev fn;
   int has_par1 = 0;
   int64_t nbytes = 0;
-  // kernel switches, resolved once when the layout is created (layouts built with different settings coexist):
-  int kvar = 0;              // MDE_B200_KERNEL: 0 default, 1 strided (sorted SoA), 2 precise (no MUFU math)
-  int nq = 1;                // MDE_B200_NQ: consecutive quads per thread of the FAST quad kernel (1 or 2)
-  int qbps = 4;              // MDE_B200_QUAD_BPS: blocks per SM in the quad kernel's grid cap (1..16)
+  // MDE_B200_KERNEL=precise: IEEE math in place of the MUFU forms, resolved once when the layout is created (layouts
+  // built with and without it coexist)
+  bool precise = false;
   int det = 0;               // deterministic mode: m <= 4 fixed point (fx), 5 <= m <= 512 the wide owner kernel
   long long* fx = nullptr;   // [n * m_hint] fixed-point accumulator (det, m_hint <= 4 only)
   // sorted-SoA layout, m_hint <= 4 (and deterministic layouts with 5 <= m_hint <= 512): every edge is stored again as
@@ -72,7 +71,6 @@ struct mde_edges {
   int nbkt = 0;            // non-empty buckets
   int32_t* bkt_tile = nullptr;  // [nbkt]     dst tile of bucket b
   int32_t* bkt_wt0 = nullptr;   // [nbkt + 1] first warp-tile of bucket b
-  int gred = 0;                 // kind 1: dst contributions as global reds instead of shared-memory CAS
   int ncta = 0;                 // persistent grid of the tile kernel
   int32_t* cta_wt0 = nullptr;   // [ncta + 1] warp-tile range of CTA c
   int32_t* cta_bkt0 = nullptr;  // [ncta]     bucket holding cta_wt0[c]

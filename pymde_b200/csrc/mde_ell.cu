@@ -53,11 +53,6 @@ static_assert(ell_rec_bytes(4, 2) <= kEllSlotBytes && ell_rec_bytes(8, 1) <= kEl
               ell_rec_bytes(6, 1) <= kEllSlotBytes, "slot size");
 constexpr uint32_t kOwnMask = 0x00ffffffu;
 
-int ell_pack_enabled() {  // MDE_B200_ELL_PACK=0: one lane-slot per lane in every record (A/B)
-  const char* e = getenv("MDE_B200_ELL_PACK");
-  return !(e && e[0] == '0');
-}
-
 // Record directory: everything about the records except their bytes.  Derived from the HISTOGRAM of lane-slot lengths
 // per (tile, class) alone -- lane-slots are consumed longest first inside a (tile, class) -- so the host builder and
 // the device builder (which only brings that histogram back to the host) share it and produce identical layouts.
@@ -72,7 +67,6 @@ struct EllPlan {
 
 // hist[(tile * 2 + cls) * 9 + len]: lane-slots of length len (1..8) in (tile, cls)
 int ell_plan(const uint32_t* hist, int64_t ndt, int max_cta, EllPlan& out) {
-  const int pack = ell_pack_enabled();
   std::vector<int64_t> rec_cost;
   out.rec_off.assign(1, 0u);
   out.rec_hdr.clear(); out.rec_slot0.clear(); out.bkt_tile.clear(); out.bkt_wt0.clear();
@@ -97,7 +91,7 @@ int ell_plan(const uint32_t* hist, int64_t ndt, int max_cta, EllPlan& out) {
         while (i0 >= upto) { --len; upto += h[len]; }
         const int W = (len + 1) & ~1;
         const int64_t left = total - i0;
-        const int K = (int)std::min<int64_t>(pack ? ell_kmax(W) : 1, (left + 31) / 32);
+        const int K = (int)std::min<int64_t>(ell_kmax(W), (left + 31) / 32);
         const int ns = (int)std::min<int64_t>(32ll * K, left);
         out.rec_hdr.push_back(W); out.rec_hdr.push_back((int32_t)c); out.rec_hdr.push_back(K); out.rec_hdr.push_back(ns);
         out.rec_slot0.push_back((int32_t)(slot_base + i0));
@@ -530,7 +524,7 @@ using EllPairs = FnList<Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>, Fn1<MDE_FN_P_QUADRATIC
                         Fn1<MDE_FN_L_HUBER>>;
 
 const void* select_kernel(const mde_edges* e, int m) {
-  const bool fast = fast_log1p_log(e->fn, e->kvar == 2);
+  const bool fast = fast_log1p_log(e->fn, e->precise);
   return with_small_m(m, [&](auto mc) {
     constexpr int M = decltype(mc)::value;
     return select_fn<M, 0>(e->fn, fast, EllPairs{}, [](auto f) {

@@ -402,7 +402,7 @@ using PullPairs = FnList<Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>, Fn<MDE_FN_P_LOG1P, MD
 
 template <int MODE>
 const void* select_kernel(const mde_edges* e, int m, int epl) {
-  const bool fast = fast_log1p_log(e->fn, e->kvar == 2);
+  const bool fast = fast_log1p_log(e->fn, e->precise);
   return with_small_m(m, [&](auto mc) {
     constexpr int M = decltype(mc)::value;
     return select_fn<M, MODE>(e->fn, fast, PullPairs{}, [&](auto f) {

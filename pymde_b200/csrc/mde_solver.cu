@@ -40,6 +40,7 @@ constexpr int kMaxSlices = (kMaxMemory + kPairsPerSlice - 1) / kPairsPerSlice;  
 constexpr int kHeadAcc = kDotsPerSlice + 12;  // step_head_kernel: + g.d, g.g, |g|_1, column sums of g and X (+ pad): fp32 accumulators
 constexpr int kHeadCols = kHeadAcc + 6;       // columns of a partial row: + loss, (g.d, d.d, X.X, max|d|) of the vec kernel, pad (even)
 constexpr int kStatusInts = 12;
+constexpr int kStepsPerGraph = 8;  // steps of the multi-step graph (the one-step graph takes the last few)
 enum { PH_DIR = 0, PH_TRIAL = 1, PH_FRESH = 2, PH_MAT = 3 };  // phase of a step
 
 struct alignas(16) HeadDesc {  // what every block of the next head kernel needs, in 64 bytes (4 broadcast loads)
@@ -313,11 +314,14 @@ ext_coeff_kernel(const int* flag, const float* __restrict__ fpp, const float* __
 // a host-side NCCL call: plain kernel nodes, so the sharded solve runs the same CUDA graph of gated steps as one
 // GPU, and a gated-off step costs nothing.  Every rank sums the peers' partial buffers in RANK ORDER, so all ranks
 // hold bit-identical gradients (the replicated Wolfe / L-BFGS decisions depend on it).
-//   small buffers (<= kOneShotBytes): one-shot -- every rank reads all W partial buffers and writes g;
-//   large buffers: two-shot -- rank r reduces chunk r in place (reduce-scatter), then everybody gathers the
-//   W reduced chunks (all-gather): 2 (W-1)/W of the buffer over NVLink instead of (W-1).
+//   small buffers (<= kOneShotBytes): one-shot -- every rank reads all W partial buffers and writes g
+//   (allreduce_kernel);
+//   large buffers: write-based -- rank r stores chunk q of its partial buffer into rank q's receive slots, rank q
+//   sums its W copies and stores the reduced chunk into the gradient buffer of every rank (allreduce_push_kernel):
+//   every byte crosses NVLink as a posted store.
 // Handshake: monotonically increasing epochs in per-rank flag arrays (st.release.sys / ld.acquire.sys),
-// fa = "my partial buffer is complete", fb = "my chunk is reduced", fd = "I have finished reading the peers".
+// fa = "my partial buffer is complete" (one-shot) / "my chunks are in the peers' receive slots" (write-based),
+// fb = "my reduced chunk is in every rank's g", fd = "I have finished reading the peers".
 // Spins are bounded: a peer that never arrives sets the solver's error word instead of hanging the GPU.
 // ---------------------------------------------------------------------------------------
 constexpr int kMaxWorld = 8;
@@ -389,87 +393,59 @@ __device__ __forceinline__ void comm_reduce_tail(const Comm& c, int64_t npad, fl
   out[1] = (float)(sum - (double)hi);
 }
 
-// One-shot: g[i] = sum_q buf_q[i] (rank order) for i < npad, tail summed in double.  MODE 0 = one-shot,
-// 1 = reduce-scatter phase (chunk `rank` reduced in place), 2 = all-gather phase.
-template <int PHASE>
+// One-shot: g[i] = sum_q buf_q[i] (rank order) for i < npad, tail summed in double.
 __global__ void __launch_bounds__(kCommThreads)
 allreduce_kernel(const int* __restrict__ flag, Comm c, float* __restrict__ g, int64_t npad, int* __restrict__ err) {
   if (off(flag)) return;
   const unsigned ep = *reinterpret_cast<volatile unsigned*>(c.epoch) + 1u;
-  unsigned* const* sig = (PHASE == 2) ? c.fb : c.fa;
-  if (blockIdx.x == 0) comm_signal(sig, c, ep);
-  comm_wait(sig[c.rank], c, ep, err);
+  if (blockIdx.x == 0) comm_signal(c.fa, c, ep);
+  comm_wait(c.fa[c.rank], c, ep, err);
   const int64_t n4 = npad >> 2;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   constexpr int U = 2;  // float4 per thread per trip; all U * world peer loads are issued before the first add
-  if (PHASE == 0 || PHASE == 1) {
-    // chunk q = [q * cs, min((q + 1) * cs, n4)) in float4 units; one-shot reduces everything, reduce-scatter its chunk
-    const int64_t cs = (n4 + c.world - 1) / c.world;
-    const int64_t lo = (PHASE == 0) ? 0 : (int64_t)c.rank * cs;
-    const int64_t hi = (PHASE == 0) ? n4 : ((lo + cs < n4) ? lo + cs : n4);
-    float* out = (PHASE == 0) ? g : c.buf[c.rank];
-    for (int64_t i0 = lo + tid; i0 < hi; i0 += U * stride) {
-      float4 v[kMaxWorld][U];
+  for (int64_t i0 = tid; i0 < n4; i0 += U * stride) {
+    float4 v[kMaxWorld][U];
 #pragma unroll
-      for (int q = 0; q < kMaxWorld; ++q) {
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          const int64_t i = i0 + u * stride;
-          v[q][u] = (q < c.world && i < hi) ? ld_peer_f4(c.buf[q] + 4 * i) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
+    for (int q = 0; q < kMaxWorld; ++q) {
 #pragma unroll
       for (int u = 0; u < U; ++u) {
-        float4 acc = v[0][u];
-#pragma unroll
-        for (int q = 1; q < kMaxWorld; ++q) {  // rank order: bit-identical sums on every rank (absent ranks add +0)
-          if (q < c.world) { acc.x += v[q][u].x; acc.y += v[q][u].y; acc.z += v[q][u].z; acc.w += v[q][u].w; }
-        }
         const int64_t i = i0 + u * stride;
-        if (i < hi) reinterpret_cast<float4*>(out)[i] = acc;
+        v[q][u] = (q < c.world && i < n4) ? ld_peer_f4(c.buf[q] + 4 * i) : make_float4(0.f, 0.f, 0.f, 0.f);
       }
     }
-    if (tid == 0) comm_reduce_tail(c, npad, g + npad);
-  } else {
-    const int64_t cs = (n4 + c.world - 1) / c.world;
-    constexpr int UG = 8;
-    for (int64_t i0 = tid; i0 < n4; i0 += UG * stride) {
-      float4 v[UG];
 #pragma unroll
-      for (int u = 0; u < UG; ++u) {
-        const int64_t i = i0 + u * stride;
-        v[u] = (i < n4) ? ld_peer_f4(c.buf[(int)(i / cs)] + 4 * i) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
+    for (int u = 0; u < U; ++u) {
+      float4 acc = v[0][u];
 #pragma unroll
-      for (int u = 0; u < UG; ++u) {
-        const int64_t i = i0 + u * stride;
-        if (i < n4) reinterpret_cast<float4*>(g)[i] = v[u];
+      for (int q = 1; q < kMaxWorld; ++q) {  // rank order: bit-identical sums on every rank (absent ranks add +0)
+        if (q < c.world) { acc.x += v[q][u].x; acc.y += v[q][u].y; acc.z += v[q][u].z; acc.w += v[q][u].w; }
       }
+      const int64_t i = i0 + u * stride;
+      if (i < n4) reinterpret_cast<float4*>(g)[i] = acc;
     }
   }
-  if (PHASE != 1) {
-    // the last block to finish tells the peers "I am done reading your buffers" and completes the epoch
-    __shared__ int s_last;
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      const unsigned t = atomicAdd(c.ticket, 1u);
-      s_last = (t == gridDim.x - 1u) ? 1 : 0;
-      if (s_last) *c.ticket = 0u;
-    }
-    __syncthreads();
-    if (s_last) {
-      comm_signal(c.fd, c, ep);
-      if (threadIdx.x == 0) *c.epoch = ep;
-    }
+  if (tid == 0) comm_reduce_tail(c, npad, g + npad);
+  // the last block to finish tells the peers "I am done reading your buffers" and completes the epoch
+  __shared__ int s_last;
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const unsigned t = atomicAdd(c.ticket, 1u);
+    s_last = (t == gridDim.x - 1u) ? 1 : 0;
+    if (s_last) *c.ticket = 0u;
+  }
+  __syncthreads();
+  if (s_last) {
+    comm_signal(c.fd, c, ep);
+    if (threadIdx.x == 0) *c.epoch = ep;
   }
 }
 
 // ---------------------------------------------------------------------------------------
-// Large buffers: write-based ("push") all-reduce.  NVLink stores are posted, loads are round trips: the read-based
-// reduce-scatter + all-gather above sustained ~300 GB/s per GPU on 80 MB gradients.  Here every byte crosses NVLink
-// as a store:
+// Large buffers: write-based ("push") all-reduce.  NVLink stores are posted, loads are round trips: a read-based
+// reduce-scatter + all-gather sustained ~300 GB/s per GPU on 80 MB gradients.  Here every byte crosses NVLink as a
+// store:
 //   K<0>  rank r copies chunk q of its partial buffer into rank q's receive slot r (all q != r) and its loss pair
 //         into everybody's tails; last block: fence + flag fa
 //   K<1>  wait fa of all ranks; rank q sums its W copies of chunk q IN RANK ORDER and stores the result into the
@@ -1218,7 +1194,6 @@ struct mde_solver {
   // exported with cudaIpc, the peers' regions mapped by mde_solver_comm_connect
   void* comm_region = nullptr;
   int64_t comm_bytes = 0, comm_flags_off = 0, comm_g_off = 0, comm_recv_off = 0, comm_tails_off = 0, comm_slot_floats = 0;
-  int comm_pull = 0;                 // read-based two-shot instead of the push kernels (A/B switch)
   Comm comm{};
   Comm* comm_dev = nullptr;
   int comm_connected = 0;
@@ -1232,8 +1207,7 @@ struct mde_solver {
   // stream-launched steps (a caller's part is a hook): the caller's parts that are graphs, instantiated
   // (0 distortion function, 1 retraction, 2 tangent projection)
   cudaGraphExec_t part_exec[3] = {nullptr, nullptr, nullptr};
-  // flat step graphs (one step / steps_per_graph steps), no conditional nodes
-  int steps_per_graph = 8;           // MDE_B200_STEPS (1..64)
+  // flat step graphs (one step / kStepsPerGraph steps), no conditional nodes
   cudaGraph_t step_graph = nullptr, steps_graph = nullptr;
   cudaGraphExec_t step_exec = nullptr, steps_exec = nullptr;
   int step_kernels = 0;              // kernel nodes per step
@@ -1334,12 +1308,7 @@ int enqueue_eval(mde_solver* s, const int* flag, cudaStream_t st) {
       if (nb > kNumSMs) nb = kNumSMs;  // one resident 512-thread block per SM (84-100 registers): a single wave
       if (nb < 1) nb = 1;
       if ((s->npad + 4) * (int64_t)sizeof(float) <= kOneShotBytes) {
-        allreduce_kernel<0><<<nb, kCommThreads, 0, st>>>(flag, s->comm, s->g, s->npad, &s->S->error);
-        MDE_LAUNCH_CHECK();
-      } else if (s->comm_pull) {  // MDE_B200_ALLREDUCE=pull: read-based reduce-scatter + all-gather (A/B)
-        allreduce_kernel<1><<<nb, kCommThreads, 0, st>>>(flag, s->comm, s->g, s->npad, &s->S->error);
-        MDE_LAUNCH_CHECK();
-        allreduce_kernel<2><<<nb, kCommThreads, 0, st>>>(flag, s->comm, s->g, s->npad, &s->S->error);
+        allreduce_kernel<<<nb, kCommThreads, 0, st>>>(flag, s->comm, s->g, s->npad, &s->S->error);
         MDE_LAUNCH_CHECK();
       } else {
         allreduce_push_kernel<0><<<nb, kCommThreads, 0, st>>>(flag, s->comm, s->npad, &s->S->error);
@@ -1457,14 +1426,11 @@ void destroy_step_graphs(mde_solver* s) {
   }
 }
 
-// the one-step and the steps_per_graph-step graphs (one GPU, or several once connected)
+// the one-step and the kStepsPerGraph-step graphs (one GPU, or several once connected)
 int build_step_graphs(mde_solver* s) {
   int rc = build_step_graph(s, 1, &s->step_graph, &s->step_exec);
   if (rc) return rc;
-  { const char* ev = getenv("MDE_B200_STEPS"); if (ev) s->steps_per_graph = atoi(ev); }
-  if (s->steps_per_graph < 1) s->steps_per_graph = 1;
-  if (s->steps_per_graph > 64) s->steps_per_graph = 64;
-  return build_step_graph(s, s->steps_per_graph, &s->steps_graph, &s->steps_exec);
+  return build_step_graph(s, kStepsPerGraph, &s->steps_graph, &s->steps_exec);
 }
 
 // a graph the solver can embed as a child node: kernel, memset and memcpy nodes only (no memory-allocation nodes);
@@ -1565,7 +1531,6 @@ int solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m, co
     TRY(cudaMalloc(&s->comm_dev, sizeof(Comm)));
     s->gpart = reinterpret_cast<float*>(s->comm_region);
     s->g = reinterpret_cast<float*>(reinterpret_cast<char*>(s->comm_region) + s->comm_g_off);
-    { const char* ev = getenv("MDE_B200_ALLREDUCE"); if (ev && !strcmp(ev, "pull")) s->comm_pull = 1; }
   } else {
     TRY(cudaMalloc(&s->g, vb));
   }
@@ -1814,18 +1779,17 @@ int mde_solver_run(mde_solver_t* s, int iters, int* iters_done, int* converged, 
     int remaining = target - s->host_iter;
     if (remaining < 1) remaining = 1;
     long long steps = 0;
-    const int spg = s->steps_per_graph;
     if (!s->steps_exec) {
       // host hook (all-reduce, or a callable distortion function in hook mode): stream-launched steps; every rank
       // enqueues the same number of steps (same `remaining`: the replicated state machines agree)
       int n_steps = remaining + remaining / 8 + (round > 0 ? 1 : 0) + 1;
       if (n_steps > 64) n_steps = 64;
       for (int b = 0; b < n_steps; ++b) { if ((rc = enqueue_step(s, st))) return rc; }
-    } else if (remaining >= spg) {
-      int graphs = (remaining + remaining / 8 + 1) / spg;
-      if (graphs * spg > 96) graphs = 96 / spg > 0 ? 96 / spg : 1;  // <= ~96 steps in flight per status read
+    } else if (remaining >= kStepsPerGraph) {
+      int graphs = (remaining + remaining / 8 + 1) / kStepsPerGraph;
+      if (graphs * kStepsPerGraph > 96) graphs = 96 / kStepsPerGraph;  // <= ~96 steps in flight per status read
       for (int b = 0; b < graphs; ++b) MDE_CUDA_TRY(cudaGraphLaunch(s->steps_exec, st));
-      steps = (long long)graphs * spg;
+      steps = (long long)graphs * kStepsPerGraph;
     } else {
       const int singles = remaining + remaining / 4 + (round > 0 ? 1 : 0) + 1;
       for (int b = 0; b < singles; ++b) MDE_CUDA_TRY(cudaGraphLaunch(s->step_exec, st));

@@ -18,7 +18,6 @@
 // Global L2 requests per edge drop from ~3.3 (2 row gathers + 1.3 reds) to the src side only
 // (~0.2 sector reads + <= 1 red).
 #include <cub/cub.cuh>
-#include <cstring>
 #include <vector>
 
 #include "mde_edges.cuh"
@@ -74,7 +73,6 @@ struct TileArgs {
   int rb;
   int x_vec_ok;  // X 16-byte aligned: the dst tile comes by cp.async.bulk
   int g_vec_ok;  // grad 16-byte aligned: the gradient tile is flushed with red.v4
-  int gred;      // 1: dst contributions leave as global reds (no gradient tile, no CAS); the X tile may be twice as large
 };
 
 // One thread, 4 consecutive slots of a warp-tile: src rows from global (L1-cached, sorted => neighbouring lanes
@@ -120,16 +118,7 @@ __device__ __forceinline__ void quad_compute(const TileArgs& a, const float* __r
       float v[M];
 #pragma unroll
       for (int cc = 0; cc < M; ++cc) v[cc] = live ? g * diff[cc] : 0.0f;
-      if (live) {
-        if (a.gred) {
-          float nv[M];
-#pragma unroll
-          for (int cc = 0; cc < M; ++cc) nv[cc] = -v[cc];
-          red_row<M>(a.grad, td[e], nv);
-        } else {
-          smem_sub_row<M>(Gt, dl[e], v);
-        }
-      }
+      if (live) smem_sub_row<M>(Gt, dl[e], v);
       const int se = ok ? s[e] : cur;  // pads never break a run
       if (se != cur) {                 // run of equal src ended: flush its sum
         red_row<M>(a.grad, cur, acc);
@@ -155,8 +144,8 @@ distortion_tile_kernel(const TileArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int R = 1 << a.rb;
   float* Xt = reinterpret_cast<float*>(smem_raw);
-  float* Gt = Xt + R * M;  // (unused when a.gred)
-  unsigned char* slots = reinterpret_cast<unsigned char*>(Xt + (a.gred ? 1 : 2) * R * M);
+  float* Gt = Xt + R * M;
+  unsigned char* slots = reinterpret_cast<unsigned char*>(Xt + 2 * R * M);
   uint64_t* bars = reinterpret_cast<uint64_t*>(slots + kTileWarps * kWtBytes);
   double* red = reinterpret_cast<double*>(bars + kTileWarps + 2);
 
@@ -194,7 +183,7 @@ distortion_tile_kernel(const TileArgs a) {
     seg_end = be < wt1 ? be : wt1;
     if (new_tile == tile) return;  // same dst tile, other src super-tile: keep accumulating
     __syncthreads();               // every warp is done with the old tile
-    if (!first && MODE != 1 && !a.gred) {
+    if (!first && MODE != 1) {
       // flush: grad[tile rows] += Gt, zero Gt (same thread reads and clears an element)
       const int64_t rows_l = a.n - base;
       const int rows = (int)(rows_l < (int64_t)R ? rows_l : (int64_t)R);
@@ -226,7 +215,7 @@ distortion_tile_kernel(const TileArgs a) {
     const int rows = (int)(rows_l < (int64_t)R ? rows_l : (int64_t)R);
     const int nfl = rows * M;
     const float* xsrc = a.X + base * M;
-    if (first && MODE != 1 && !a.gred) {
+    if (first && MODE != 1) {
       float4* G4 = reinterpret_cast<float4*>(Gt);
       for (int i = threadIdx.x; i < ((R * M) >> 2); i += kTileThreads) G4[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     }
@@ -307,7 +296,7 @@ distortion_tile_kernel(const TileArgs a) {
   if (first && wt0 < wt1) { enter_bucket(true); first = false; }
   while (seg_end < wt1) { ++bkt; enter_bucket(false); }
   __syncthreads();
-  if (MODE != 1 && tile >= 0 && !a.gred) {  // final flush
+  if (MODE != 1 && tile >= 0) {  // final flush
     const int64_t rows_l = a.n - base;
     const int rows = (int)(rows_l < (int64_t)R ? rows_l : (int64_t)R);
     const int nfl = rows * M;
@@ -413,8 +402,8 @@ __global__ void tiled_outputs_kernel(const int32_t* __restrict__ rec, const int3
   }
 }
 
-size_t tile_smem_bytes(int rb, int m, int gred) {
-  return (size_t)(gred ? 1 : 2) * ((size_t)1 << rb) * m * sizeof(float) + (size_t)kTileWarps * kWtBytes +
+size_t tile_smem_bytes(int rb, int m) {
+  return (size_t)2 * ((size_t)1 << rb) * m * sizeof(float) + (size_t)kTileWarps * kWtBytes +
          (size_t)(kTileWarps + 2) * sizeof(uint64_t) + 32 * sizeof(double);
 }
 
@@ -424,7 +413,7 @@ using TilePairs = FnList<Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>, Fn<MDE_FN_P_LOG1P, MD
 
 template <int MODE>
 const void* select_kernel(const mde_edges* e, int m) {
-  const bool fast = fast_log1p_log(e->fn, e->kvar == 2);
+  const bool fast = fast_log1p_log(e->fn, e->precise);
   return with_small_m(m, [&](auto mc) {
     constexpr int M = decltype(mc)::value;
     return select_fn<M, MODE>(e->fn, fast, TilePairs{}, [](auto f) {
@@ -455,9 +444,7 @@ int tiled_build(mde_edges* e, const int64_t* edges, const float* par0, const mde
   const int64_t p = e->p, n = e->n;
   if (m < 1 || m > 4) return MDE_E_UNSUPPORTED;
   const int rb = tile_rb(m);
-  int gred = 0;
-  { const char* ev = getenv("MDE_B200_TILE_SCATTER"); if (ev && !strcmp(ev, "global")) gred = 1; }
-  if (tile_smem_bytes(rb, m, gred) > kMaxDynSmem) return MDE_E_UNSUPPORTED;
+  if (tile_smem_bytes(rb, m) > kMaxDynSmem) return MDE_E_UNSUPPORTED;
   // src super-tile: X + gradient rows of one super-tile (2 * m * 4 bytes per row) stay L2-resident; 24 MB leaves
   // about half of the H100's 50 MB L2 to the streamed records and the destination side
   int64_t l2_bytes = (int64_t)env_int("MDE_B200_STILE_MB", 24) << 20;
@@ -555,7 +542,6 @@ int tiled_build(mde_edges* e, const int64_t* edges, const float* par0, const mde
     for (int mode = 0; mode < 3; ++mode) {
       if ((rc = allow_max_smem(select_kernel(e, m, mode)))) goto done;
     }
-    e->gred = gred;
     e->kind = kTiles; e->m_hint = m; e->rb = rb; e->ss = ss; e->nwt = nwt; e->nbkt = nbkt; e->ncta = ncta;
     e->nbytes = nwt * (kWtBytes + 4 * kWtEdges) + 8 * kMaxLossBlocks + 4ll * (2 * nbkt + 2 * ncta + 2);
   }
@@ -575,7 +561,7 @@ done:
 int tiled_launch(int mode, const mde_edges* e, const float* X, int m, float* grad, const float* gext,
                  int* nblocks_out, const int* flag, cudaStream_t st) {
   if (e->kind != kTiles || m < 1 || m > 4) return MDE_E_UNSUPPORTED;
-  const size_t smem = tile_smem_bytes(e->rb, m, e->gred);
+  const size_t smem = tile_smem_bytes(e->rb, m);
   if (smem > kMaxDynSmem) return MDE_E_UNSUPPORTED;  // layout built for a smaller embedding dimension
   TileArgs a;
   a.rec = e->rec; a.perm = e->perm; a.gext = gext; a.bkt_tile = e->bkt_tile; a.bkt_wt0 = e->bkt_wt0;
@@ -583,7 +569,6 @@ int tiled_launch(int mode, const mde_edges* e, const float* X, int m, float* gra
   a.flag = flag; a.fn = e->fn; a.inv_p = 1.0f / (float)e->p_total; a.n = e->n; a.rb = e->rb;
   a.x_vec_ok = ((reinterpret_cast<uintptr_t>(X) & 15u) == 0) ? 1 : 0;
   a.g_vec_ok = ((reinterpret_cast<uintptr_t>(grad) & 15u) == 0) ? 1 : 0;
-  a.gred = e->gred;
   return launch_persistent(select_kernel(e, m, mode), &a, e->ncta, kTileThreads, smem, nblocks_out, st);
 }
 

@@ -91,7 +91,7 @@ if rank == 0:
     conv["rel"] = abs(conv["value"] - conv["single_value"]) / abs(conv["single_value"])
 res["converged"] = conv
 
-# (iv) a gradient above 4 MB (n = 600 000): the write-based ("push") all-reduce, and the read-based one for A/B
+# (iv) a gradient above 4 MB (n = 600 000): the write-based ("push") all-reduce
 n3 = 600_000
 e3, w3 = bench.c5_shard(3, n=n3, p=3_000_000, block=5_000)
 X3 = bench.initial_iterate(4, n3, 2)
@@ -100,27 +100,22 @@ mk3 = lambda lo, hi: pm.penalties.PushAndPull(w3t[lo:hi].to(dev), pm.penalties.L
 spec3 = O.FnSpec(O.P_LOG1P, w3, (1.5, 0, 0), fn_rep=O.P_LOG, rep=(1.0, 0, 0))
 v3_ref, g3_ref = c_oracle.average_distortion(X3, e3, spec3, True)
 r3_ref = float(np.sqrt((g3_ref ** 2).sum()))
-big = {}
 one3 = None
 if rank == 0:
     one = pm.MDE(n3, 2, e3t.to(dev), mk3(0, len(e3)), pm.Centered(), device=dev)
     one.embed(X=torch.tensor(X3, device=dev), max_iter=8, eps=0.0)
     one3 = np.array(one.solve_stats.average_distortions)
     del one
-for mode in ("push", "pull"):
-    os.environ["MDE_B200_ALLREDUCE"] = mode
-    mb = pdist.shard_mde(pm.MDE, n3, 2, e3t, mk3, pm.Centered(), dev, transport="peer")
-    Xb = mb.embed(X=torch.tensor(X3, device=dev), max_iter=8, eps=0.0)
-    sb = mb.solve_stats
-    ab = np.array(sb.average_distortions)
-    rb = {"iterations": sb.iterations, "x_identical": digests_equal(Xb), "loss0_rel": abs(ab[0] - v3_ref) / abs(v3_ref),
-          "resid0_rel": abs(sb.residual_norms[0] - r3_ref) / r3_ref, "decreased": bool(ab[-1] < ab[0])}
-    if rank == 0:
-        rb["first3_rel_vs_single"] = float(np.abs(ab[:3] - one3[:3]).max() / np.abs(one3[:3]).max())
-    big[mode] = rb
-    del mb
-os.environ.pop("MDE_B200_ALLREDUCE", None)
-res["big"] = big
+mb = pdist.shard_mde(pm.MDE, n3, 2, e3t, mk3, pm.Centered(), dev, transport="peer")
+Xb = mb.embed(X=torch.tensor(X3, device=dev), max_iter=8, eps=0.0)
+sb = mb.solve_stats
+ab = np.array(sb.average_distortions)
+rb = {"iterations": sb.iterations, "x_identical": digests_equal(Xb), "loss0_rel": abs(ab[0] - v3_ref) / abs(v3_ref),
+      "resid0_rel": abs(sb.residual_norms[0] - r3_ref) / r3_ref, "decreased": bool(ab[-1] < ab[0])}
+if rank == 0:
+    rb["first3_rel_vs_single"] = float(np.abs(ab[:3] - one3[:3]).max() / np.abs(one3[:3]).max())
+del mb
+res["big"] = {"push": rb}
 
 # (v) a sharded problem the device solver does not take (arbitrary callable): the host-stepped solver must still see
 #     the GLOBAL objective (EdgeLayout all-reduces evaluations), so the replicas stay identical

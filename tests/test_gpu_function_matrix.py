@@ -44,8 +44,7 @@ from tests.test_function_matrix_cpu import GOLD, nonfinite_class, spec_of
 gpu = pytest.mark.gpu
 
 _ENV = ("MDE_B200_LAYOUT", "MDE_B200_TILE_RB", "MDE_B200_STILE_MB", "MDE_B200_TILE_MIN", "MDE_B200_PULL_EPL",
-        "MDE_B200_PULL_REP", "MDE_B200_TILE_SCATTER", "MDE_B200_KERNEL", "MDE_B200_NQ", "MDE_B200_QUAD_BPS",
-        "MDE_B200_DETERMINISTIC", "MDE_B200_ELL_PACK", "MDE_B200_ELL_BUILD")
+        "MDE_B200_PULL_REP", "MDE_B200_KERNEL", "MDE_B200_DETERMINISTIC", "MDE_B200_ELL_BUILD")
 
 TOL = {"mufu_f_abs": 2.0 ** -18, "mufu_f_rel": 2.0 ** -18, "mufu_fp_rel": 2.0 ** -17, "ell_d_rel": 2.0 ** -20,
        "det_abs": 2.0 ** -40, "g_abs": 2.0 ** -126, "ieee_ulp": 16, "ieee_k": 10.0}
@@ -55,7 +54,6 @@ _TILES = {"MDE_B200_TILE_MIN": "0"}
 PATHS = {
     "owner_m1": ({}, 1, 0), "owner_m2": ({}, 2, 0), "owner_m3": ({}, 3, 0), "owner_m4": ({}, 4, 0),
     "precise_owner_m2": ({"MDE_B200_KERNEL": "precise"}, 2, 0),
-    "strided_m2": ({"MDE_B200_KERNEL": "strided"}, 2, 0), "strided_m3": ({"MDE_B200_KERNEL": "strided"}, 3, 0),
     "tiles_m2": (dict(_TILES, MDE_B200_LAYOUT="tiles"), 2, 1), "tiles_m3": (dict(_TILES, MDE_B200_LAYOUT="tiles"), 3, 1),
     "precise_tiles_m2": (dict(_TILES, MDE_B200_LAYOUT="tiles", MDE_B200_KERNEL="precise"), 2, 1),
     "pull_m2": (dict(_TILES, MDE_B200_LAYOUT="pull"), 2, 2), "pull_m3": (dict(_TILES, MDE_B200_LAYOUT="pull"), 3, 2),

@@ -15,7 +15,7 @@ pytestmark = pytest.mark.gpu
 @pytest.fixture(params=["auto", "soa", "tiles", "pull", "ell"], autouse=True)
 def edge_layout(request, monkeypatch):
     """Every test of this file runs on each edge layout / kernel family: the library's own choice, the sorted-SoA
-    layout (quad / strided / wide kernels), tile records (push kernel), pull records and ELL pull records
+    layout (owner / quad / wide kernels), tile records (push kernel), pull records and ELL pull records
     (mde_edges.cuh).  Layouts that
     do not apply (m > 4, WeightedQuadratic's second array) fall back to SoA inside the library."""
     if request.param != "auto":

@@ -30,14 +30,12 @@ gpu = pytest.mark.gpu
 
 # every switch that changes which layout or kernel the library picks; cleared before each test
 _ENV = ("MDE_B200_LAYOUT", "MDE_B200_TILE_RB", "MDE_B200_STILE_MB", "MDE_B200_TILE_MIN", "MDE_B200_PULL_EPL",
-        "MDE_B200_PULL_REP", "MDE_B200_TILE_SCATTER", "MDE_B200_KERNEL", "MDE_B200_NQ", "MDE_B200_QUAD_BPS",
-        "MDE_B200_DETERMINISTIC", "MDE_B200_ELL_PACK", "MDE_B200_ELL_BUILD")
+        "MDE_B200_PULL_REP", "MDE_B200_KERNEL", "MDE_B200_DETERMINISTIC", "MDE_B200_ELL_BUILD")
 
 # layout variant -> (environment, kind it must build)
 LAYOUTS = {
     "soa": ({"MDE_B200_LAYOUT": "soa"}, 0),
     "tiles": ({"MDE_B200_LAYOUT": "tiles"}, 1),
-    "tiles_global": ({"MDE_B200_LAYOUT": "tiles", "MDE_B200_TILE_SCATTER": "global"}, 1),
     "pull4": ({"MDE_B200_LAYOUT": "pull", "MDE_B200_PULL_EPL": "4"}, 2),
     "pull8": ({"MDE_B200_LAYOUT": "pull", "MDE_B200_PULL_EPL": "8"}, 2),
     "pull_push": ({"MDE_B200_LAYOUT": "pull", "MDE_B200_PULL_REP": "push"}, 2),
@@ -452,20 +450,6 @@ def test_precise_and_fast_in_one_process(layout, m, monkeypatch):
     fast, precise, fast2 = run(False), run(True), run(False)
     assert fast == fast2
     assert fast != precise, "MDE_B200_KERNEL=precise did not change the kernel"
-
-
-@gpu
-@pytest.mark.parametrize("name", ["pp_fast_mixed", "loss_huber"])
-@pytest.mark.parametrize("m", [1, 2, 3, 4])
-@pytest.mark.parametrize("switch", [{"MDE_B200_KERNEL": "strided"}, {"MDE_B200_NQ": "2"}, {"MDE_B200_QUAD_BPS": "1"}],
-                         ids=["strided", "nq2", "bps1"])
-def test_soa_kernel_switches(switch, m, name, monkeypatch):
-    """The sorted-SoA kernel variants: the lane-strided kernel, two quads per thread, a one-block-per-SM grid."""
-    import pymde_b200 as pm
-    _setenv(monkeypatch, GEOMETRIES["G1"][1])
-    _setenv(monkeypatch, LAYOUTS["soa"][0])
-    _setenv(monkeypatch, switch)
-    _check_case(pm, "G1", m, name, 0)
 
 
 # ------------------------------------------------------------------------------------------------ oracle self-check

@@ -19,7 +19,7 @@ from tests.test_gpu_owner_pass import _exact_graph
 
 gpu = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "owner_bits.json")
-_ENV = ("MDE_B200_LAYOUT", "MDE_B200_KERNEL", "MDE_B200_NQ", "MDE_B200_QUAD_BPS", "MDE_B200_DETERMINISTIC")
+_ENV = ("MDE_B200_LAYOUT", "MDE_B200_KERNEL", "MDE_B200_DETERMINISTIC")
 
 CASES = (["c2slice-fast", "c2slice-precise"] + ["hub-pushpull-m%d" % m for m in (1, 2, 3, 4)] +
          ["hub-huber-m%d" % m for m in (1, 2, 3, 4)] + ["hub-external-m%d" % m for m in (1, 2, 3, 4)])

@@ -13,7 +13,7 @@ import torch
 
 gpu = pytest.mark.gpu
 
-_ENV = ("MDE_B200_LAYOUT", "MDE_B200_KERNEL", "MDE_B200_NQ", "MDE_B200_QUAD_BPS", "MDE_B200_DETERMINISTIC")
+_ENV = ("MDE_B200_LAYOUT", "MDE_B200_KERNEL", "MDE_B200_DETERMINISTIC")
 
 
 @pytest.fixture(autouse=True)

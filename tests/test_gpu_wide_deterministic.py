@@ -20,8 +20,7 @@ from tests.test_gpu_owner_pass import _exact_expected, _exact_graph
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 
-_ENV = ("MDE_B200_LAYOUT", "MDE_B200_KERNEL", "MDE_B200_NQ", "MDE_B200_QUAD_BPS", "MDE_B200_DETERMINISTIC",
-        "PYMDE_B200_EXTERNAL", "PYMDE_B200_SPECTRAL")
+_ENV = ("MDE_B200_LAYOUT", "MDE_B200_KERNEL", "MDE_B200_DETERMINISTIC", "PYMDE_B200_EXTERNAL", "PYMDE_B200_SPECTRAL")
 SEG = 256  # entries per segment of a long list (kWideSeg)
 
 

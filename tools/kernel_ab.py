@@ -22,8 +22,8 @@ try:
     PEAK = float(json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["hbm_gbs"])
 except Exception:
     pass
-SHORT = {"RB": "MDE_B200_TILE_RB", "STILE": "MDE_B200_STILE_MB", "MIN": "MDE_B200_TILE_MIN", "SC": "MDE_B200_TILE_SCATTER", "EPL": "MDE_B200_PULL_EPL",
-         "REP": "MDE_B200_PULL_REP", "PACK": "MDE_B200_ELL_PACK"}
+SHORT = {"RB": "MDE_B200_TILE_RB", "STILE": "MDE_B200_STILE_MB", "MIN": "MDE_B200_TILE_MIN", "EPL": "MDE_B200_PULL_EPL",
+         "REP": "MDE_B200_PULL_REP"}
 flush = None
 
 
