@@ -334,14 +334,24 @@ int mde_solver_comm_connect(mde_solver_t* s, int rank, const void* handles, int6
  * force below 10 000 rows, the approximate pynndescent above; a third-party dependency either way).  X is a device
  * row-major n x d fp32 matrix.  For every row i the k rows nearest to it in Euclidean distance (i itself excluded)
  * are written to idx_out[i*k .. i*k+k) in ascending distance with their exact fp32 SQUARED distances in d2_out.
- * Cross terms run on the tensor cores (wgmma, bf16 hi/lo split, fp32 accumulate in registers) with a running
- * top-32 per row; the 32 candidates are re-ranked with exact fp32 distances, so the result is that of a brute-force
- * fp32 search (equal-distance ties aside).  1 <= k <= mde_knn_max_k() (24), k <= n - 1.  `ws`: 1024-byte aligned
- * device scratch of mde_knn_ws_bytes(n, d) bytes.  Asynchronous on `stream`. */
+ * The columns are centred on their mean (fp64 sums in a fixed order) when that bounds the score error more tightly
+ * than the raw rows do; cross terms of the (centred) values run on the tensor cores (wgmma, bf16 hi/lo split, fp32
+ * accumulate in registers) with a running top-32 per row; the 32
+ * candidates are re-ranked with exact fp32 distances of the raw rows.  A per-row certificate (a proven bound on the
+ * tensor-core scores' error against the gap between the k-th re-ranked distance and the worst kept score) shows that
+ * no other row can enter the list; a row that fails it is searched directly over all n rows with the re-rank's
+ * arithmetic.  So the k rows are the k smallest (fp32 squared distance, index) pairs in lexicographic order, the
+ * result of a brute-force fp32 search, ties included, whatever the offset or clustering of the data.
+ * 1 <= k <= mde_knn_max_k() (24), k <= n - 1.  `ws`: 1024-byte aligned device scratch of mde_knn_ws_bytes(n, d)
+ * bytes.  Asynchronous on `stream`.  mde_knn_ex also writes the number of rows searched directly to *fallback_rows
+ * (nullable; when not null the call waits for the stream), as do mde_knn_wide_ex, mde_knn_long_ex and the mde_knn16*_ex
+ * entries below. */
 int mde_knn_max_k(void);
 int mde_knn_ws_bytes(int64_t n, int d, size_t* bytes);
 int mde_knn(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
             void* stream);
+int mde_knn_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
+               void* stream, int* fallback_rows);
 
 /* The same search on a sparse data matrix, without densifying it (pymde/preprocess/data_matrix.py:19,99 accepts
  * scipy.sparse input).  Device CSR of an n x d matrix: int64 indptr[n+1] (indptr[0] = 0, indptr[n] = nnz), int32
@@ -366,6 +376,8 @@ int mde_knn_wide_max_k(void);
 int mde_knn_wide_ws_bytes(int64_t n, int d, size_t* bytes);
 int mde_knn_wide(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                  size_t ws_bytes, void* stream);
+int mde_knn_wide_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                    size_t ws_bytes, void* stream, int* fallback_rows);
 int mde_knn_csr_wide_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes);
 int mde_knn_csr_wide(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                      int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream);
@@ -379,6 +391,8 @@ int mde_knn_long_max_k(void);
 int mde_knn_long_ws_bytes(int64_t n, int d, size_t* bytes);
 int mde_knn_long(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                  size_t ws_bytes, void* stream);
+int mde_knn_long_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                    size_t ws_bytes, void* stream, int* fallback_rows);
 int mde_knn_csr_long_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes);
 int mde_knn_csr_long(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                      int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream);
@@ -404,11 +418,10 @@ int mde_knn_approx_ex(const float* X, int64_t n, int d, int k, uint64_t seed, in
  * arguments before any CUDA call.  mde_knn16, mde_knn16_wide, mde_knn16_long and mde_knn16_approx(_ex) take the
  * arguments, bounds on k, return codes, blocking behaviour and output contract of mde_knn, mde_knn_wide, mde_knn_long
  * and mde_knn_approx(_ex), and give the bits those give on the fp32 matrix X.float(): the re-rank and NN-descent
- * convert every element to fp32 as they read it and keep the fp32 arithmetic.  The exact searches' operand is X itself
- * (one wgmma per 16 features, bf16 x bf16 or fp16 x fp16, against three for the bf16 hi / lo split of fp32 input); a
- * bf16 value's lo part is exactly zero, so bf16 input gives the fp32 route's candidate lists, and fp16 input gives
- * them up to rounding of the cross terms, so the results are equal unless more rows than the list's spare slots lie
- * within that rounding of the k-th distance.  `ws`: 1024-byte aligned device scratch of mde_knn16_ws_bytes(n, d),
+ * convert every element to fp32 as they read it and keep the fp32 arithmetic.  The exact searches' operand is X in
+ * its own type (one wgmma per 16 features, bf16 x bf16 or fp16 x fp16, against three for the bf16 hi / lo split of
+ * fp32 input): X itself, exact, or the centred X rounded to 16 bits when data far from the origin makes that the
+ * smaller error bound.  The exact searches give the bits of the fp32 route on X.float(), ties included.  `ws`: 1024-byte aligned device scratch of mde_knn16_ws_bytes(n, d),
  * mde_knn16_wide_ws_bytes(n, d), mde_knn16_long_ws_bytes(n, d) (2 n_pad k_pad bytes less than the fp32 searches,
  * n_pad = n rounded up to 128, k_pad = d rounded up to 64: no lo operand) or mde_knn16_approx_ws_bytes(n, d, k) (that
  * of mde_knn_approx: NN-descent keeps no copy of X) bytes.  Nothing n x d sized in fp32 is allocated. */
@@ -417,12 +430,18 @@ int mde_knn_approx_ex(const float* X, int64_t n, int d, int k, uint64_t seed, in
 int mde_knn16_ws_bytes(int64_t n, int d, size_t* bytes);
 int mde_knn16(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
               size_t ws_bytes, void* stream);
+int mde_knn16_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                 size_t ws_bytes, void* stream, int* fallback_rows);
 int mde_knn16_wide_ws_bytes(int64_t n, int d, size_t* bytes);
 int mde_knn16_wide(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                    size_t ws_bytes, void* stream);
+int mde_knn16_wide_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                      size_t ws_bytes, void* stream, int* fallback_rows);
 int mde_knn16_long_ws_bytes(int64_t n, int d, size_t* bytes);
 int mde_knn16_long(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                    size_t ws_bytes, void* stream);
+int mde_knn16_long_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                      size_t ws_bytes, void* stream, int* fallback_rows);
 int mde_knn16_approx_ws_bytes(int64_t n, int d, int k, size_t* bytes);
 int mde_knn16_approx(const void* X, int dtype, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out,
                      float* d2_out, void* ws, size_t ws_bytes, void* stream);

@@ -115,6 +115,8 @@ SIGNATURES = {
     "mde_knn_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                           C.c_void_p]),
+    "mde_knn_ex": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                             C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
     "mde_knn_csr_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.POINTER(C.c_size_t)]),
     "mde_knn_csr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_void_p,
                               C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -122,6 +124,8 @@ SIGNATURES = {
     "mde_knn_wide_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn_wide": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                C.c_size_t, C.c_void_p]),
+    "mde_knn_wide_ex": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
     "mde_knn_csr_wide_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.POINTER(C.c_size_t)]),
     "mde_knn_csr_wide": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -129,6 +133,8 @@ SIGNATURES = {
     "mde_knn_long_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn_long": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                C.c_size_t, C.c_void_p]),
+    "mde_knn_long_ex": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
     "mde_knn_csr_long_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.POINTER(C.c_size_t)]),
     "mde_knn_csr_long": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -141,12 +147,18 @@ SIGNATURES = {
     "mde_knn16_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn16": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                             C.c_size_t, C.c_void_p]),
+    "mde_knn16_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                               C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
     "mde_knn16_wide_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn16_wide": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn16_wide_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
     "mde_knn16_long_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn16_long": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                  C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn16_long_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
     "mde_knn16_approx_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn16_approx": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -14,9 +14,15 @@
 //              matrix never exists.
 //   re-rank  exact fp32 sum (q - x)^2 of the KK candidates of a row (one warp per row), k smallest, ascending.
 //
-// The bf16 x 3 split leaves an error of ~2^-16 |q||x| on a cross term, far below the gap between the k-th and the
-// (k + 8)-th neighbour of real data, and the re-rank removes it from the result: the neighbour lists are those of a
-// brute-force fp32 search (ties and fp32 rounding aside).  k <= 24.
+// The prep works on the column-centred values x^ = fl(x - mu) (mu: fp64 column sums in a fixed order, rounded to
+// fp32), which removes a global offset from the scores, unless the raw rows give the smaller error bound (knn_centre:
+// a 16-bit element near the origin is its own exact operand); the re-rank reads the raw rows.  The bf16 x 3 split still
+// leaves an error of ~2^-16 |q^||x^| on a cross term, which is noise when clusters lie far apart against their spread.
+//   certify  a proven bound E(q) on the score error (knn_certify_kernel) shows, row by row, that no row the tiles did
+//            not keep can enter the re-ranked list;
+//   direct   the rows that fail are searched over all n rows with the re-rank's arithmetic (knn_direct_kernel).
+// So the result is the k smallest (fp32 distance, index) pairs of a brute-force fp32 search, ties included, on every
+// input; the certificate only decides how much of it the tensor cores do.  k <= 24.
 //
 // mde_knn_wide (24 < k <= 64): knn_wide_tile_kernel does the same sweep for 64 query rows per CTA with one consumer
 // warpgroup and keeps KK = 96 candidates per row in shared memory (mde_knn_select.cuh); knn_wide_rerank_kernel
@@ -144,32 +150,151 @@ __device__ __forceinline__ void cross_step(float (&acc)[TN / 2], uint64_t ah, ui
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// prep: the operand (zero padded to n_pad x k_pad): bf16 hi / lo split of fp32 X, a copy of 16-bit X (Xl unused);
-// squared norms of the fp32 values (+inf on padded rows), the same arithmetic for every element type
+// column mean mu (fp32) of the fp32 values of X: fp64 sums over chunks of kMeanChunk rows, then over the chunks, in a
+// fixed order (the same bits on every run)
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int kMeanChunk = 512;
+constexpr int kMaxGridY = 65535;
+
+template <class T>
+__global__ void __launch_bounds__(128)
+knn_colsum_kernel(const T* __restrict__ X, int64_t n, int d, int chunks, double* __restrict__ part) {
+  const int c = blockIdx.x * 128 + threadIdx.x;
+  if (c >= d) return;
+  for (int64_t ch = blockIdx.y; ch < chunks; ch += gridDim.y) {
+    const int64_t r0 = ch * kMeanChunk;
+    const int64_t r1 = r0 + kMeanChunk < n ? r0 + kMeanChunk : n;
+    double s = 0.0;
+    for (int64_t r = r0; r < r1; ++r) s += (double)elem_f32(X[r * d + c]);
+    part[ch * d + c] = s;
+  }
+}
+
+__global__ void __launch_bounds__(128)
+knn_mean_kernel(const double* __restrict__ part, int chunks, int64_t n, int d, float* __restrict__ mu) {
+  const int c = blockIdx.x * 128 + threadIdx.x;
+  if (c >= d) return;
+  double s = 0.0;
+  for (int i = 0; i < chunks; ++i) s += part[(int64_t)i * d + c];
+  mu[c] = (float)(s / (double)n);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The error bound of the certificate (knn_certify_kernel).  s(y) = ||y^||^2 - 2 <q, y>~ is the score the tiles rank
+// (fp32 norm and tensor-core cross term of the operand y^ = y - mu, or of y itself when the search is not centred),
+// S(y) = ||q - y||^2 - ||q - mu||^2 its exact value.  |s(y) - S(y)| <= E(q) for every y, and the fp32 norm of the
+// query lies within E(q) of ||q - mu||^2, with
+//   E(q) = sigma (2 (a_cross |q^| M + eta (|q^| + M)) + a_norm M^2 + a_abs),   M^2 = max_y ||y^||^2 (fp32):
+//   a_cross  the operand's rounding (bf16 x 3 split: the dropped lo x lo term and the split residual, 3.1 2^-16; a
+//            centred value rounded to 16 bits: 2 eps + eps^2; an uncentred 16-bit element is its own exact operand: 0),
+//            the centring's rounding (2.01 u, centred only), the fp32 accumulation of m products (2 u per addition,
+//            u = 2^-24, allowing truncating tensor-core adds; m = 3 k_pad split, k_pad 16-bit) and the rounding of
+//            the score's fma (u),
+//   eta      fp16 subnormals of a centred operand: 2^-25 sqrt(k_pad) (an absolute error per element),
+//   a_norm   the fp32 norm (ceil(k_pad / 32) + 8) u and the score's fma (u),
+//   a_abs    underflow: 2^-126 per product and per square,
+// and sigma = 2, a safety factor for second-order terms (tests/test_knn_offset_cpu.py derives the bound).
+// ---------------------------------------------------------------------------------------------------------------
+struct CertBound {
+  double a_cen, a_unc;  // a_cross of the centred and of the uncentred operand
+  double eta, a_norm, a_abs, delta;
+};
+constexpr double kCertSafety = 2.0;
+
+template <class T>
+CertBound cert_bound(int d, int k_pad) {
+  const double u = 0x1p-24;
+  CertBound b;
+  double op, op_unc = 0.0;
+  int m = k_pad;
+  if constexpr (Operand<T>::kSplit) { op = op_unc = 3.1 * 0x1p-16; m = 3 * k_pad; }
+  else if constexpr (std::is_same_v<T, __half>) op = (2.0 + 0x1p-11) * 0x1p-11;
+  else op = (2.0 + 0x1p-8) * 0x1p-8;
+  b.a_cen = op + 2.01 * u + 2.0 * u * m + u;
+  b.a_unc = op_unc + 2.0 * u * m + u;
+  b.eta = std::is_same_v<T, __half> ? 0x1p-25 * sqrt((double)k_pad) : 0.0;
+  b.a_norm = ((k_pad + 31) / 32 + 9) * u;
+  b.a_abs = (2.0 * m + k_pad) * 0x1p-126 + (std::is_same_v<T, __half> ? 2.0 * k_pad * 0x1p-50 : 0.0);
+  b.delta = ((d + 31) / 32 + 8) * u;
+  return b;
+}
+
+// The search header in the workspace: uncertified row count, then maxima of squared norms as float bits
+// (non-negative floats order as their bits; NaN orders above +inf) and the centring decision.
+enum { kHdrCount, kHdrMaxNorm, kHdrMaxRaw, kHdrMaxCen, kHdrCentred, kHdrWords };
+
+// ---------------------------------------------------------------------------------------------------------------
+// norms: the largest fp32 squared norm of the raw rows and of the centred rows x - mu, for the centring decision
 // ---------------------------------------------------------------------------------------------------------------
 template <class T>
 __global__ void __launch_bounds__(256)
-knn_prep_kernel(const T* __restrict__ X, int64_t n, int d, int64_t n_pad, int k_pad, OpT<T>* __restrict__ Xh,
-                __nv_bfloat16* __restrict__ Xl, float* __restrict__ norms) {
+knn_maxnorm_kernel(const T* __restrict__ X, int64_t n, int d, const float* __restrict__ mu, unsigned* __restrict__ hdr) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= n) return;
+  float raw = 0.0f, cen = 0.0f;
+  for (int c = lane; c < d; c += 32) {
+    const float x = elem_f32(X[row * d + c]), y = x - mu[c];
+    raw = fmaf(x, x, raw);
+    cen = fmaf(y, y, cen);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    raw += __shfl_xor_sync(kFull, raw, o);
+    cen += __shfl_xor_sync(kFull, cen, o);
+  }
+  if (lane == 0) {
+    atomicMax(hdr + kHdrMaxRaw, __float_as_uint(raw));
+    atomicMax(hdr + kHdrMaxCen, __float_as_uint(cen));
+  }
+}
+
+// Centre when the centred operand's cross-term bound, a_cen M_cen^2, is below the uncentred one, a_unc M_raw^2 (the
+// same decision in every thread).  A 16-bit element is its own exact operand, while its centred value is rounded to
+// 16 bits: data near the origin keeps X, data far from it is centred.
+__device__ __forceinline__ bool knn_centre(const unsigned* hdr, const CertBound& b) {
+  return b.a_cen * (double)__uint_as_float(hdr[kHdrMaxCen]) < b.a_unc * (double)__uint_as_float(hdr[kHdrMaxRaw]);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// prep: the operand (zero padded to n_pad x k_pad) of x^ = fl(x - mu), or of x itself when knn_centre says no: the
+// bf16 hi / lo split of fp32 X, or x^ rounded to the 16-bit type of X (Xl unused; x itself when not centred, exact);
+// squared norms of x^ (+inf on padded rows), the same arithmetic for every element type; their maximum over the rows
+// to the header (+inf when an operand element is not finite, so that no row certifies)
+// ---------------------------------------------------------------------------------------------------------------
+template <class T>
+__global__ void __launch_bounds__(256)
+knn_prep_kernel(const T* __restrict__ X, int64_t n, int d, int64_t n_pad, int k_pad, const float* __restrict__ mu,
+                CertBound b, OpT<T>* __restrict__ Xh, __nv_bfloat16* __restrict__ Xl, float* __restrict__ norms,
+                unsigned* __restrict__ hdr) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= n_pad) return;
+  const bool centre = knn_centre(hdr, b);
+  if (row == 0 && lane == 0) hdr[kHdrCentred] = centre;
   float acc = 0.0f;
+  bool bad = false;
   for (int c = lane; c < k_pad; c += 32) {
-    const float x = (row < n && c < d) ? elem_f32(X[row * d + c]) : 0.0f;
+    const float x = (row < n && c < d) ? elem_f32(X[row * d + c]) - (centre ? mu[c] : 0.0f) : 0.0f;
     if constexpr (Operand<T>::kSplit) {
       const __nv_bfloat16 h = __float2bfloat16_rn(x);
       const __nv_bfloat16 l = __float2bfloat16_rn(x - __bfloat162float(h));
       Xh[row * k_pad + c] = h;
       Xl[row * k_pad + c] = l;
     } else {
-      Xh[row * k_pad + c] = (row < n && c < d) ? X[row * d + c] : T(0.0f);
+      const T o = T(x);  // round to nearest (fp16 overflows to inf beyond 65504); exact when not centred
+      bad |= !isfinite(elem_f32(o));
+      Xh[row * k_pad + c] = o;
     }
     acc += x * x;
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
-  if (lane == 0) norms[row] = (row < n) ? acc : __int_as_float(0x7f800000);
+  bad = __any_sync(kFull, bad);
+  if (lane == 0) {
+    norms[row] = (row < n) ? acc : __int_as_float(0x7f800000);
+    if (row < n) atomicMax(hdr + kHdrMaxNorm, bad ? 0x7f800000u : __float_as_uint(acc));
+  }
 }
 
 // Replace the worst of the KK kept candidates by (dist, col) and find the new worst.  Static indices only, so the
@@ -577,6 +702,111 @@ template int knn_dense_rerank<__nv_bfloat16>(int, const __nv_bfloat16*, int64_t,
 
 namespace {
 
+// ---------------------------------------------------------------------------------------------------------------
+// certificate: is the re-ranked list of a row the k smallest (distance, index) over ALL rows?
+//
+// Every row the tiles did not keep scored at least t, the worst kept score (+inf when the list was never filled:
+// every row was kept).  With the bound E(q) above (cert_bound), a row that was not kept lies at an exact distance of at
+// least t - E(q) + ||q^||^2 - E(q); when that exceeds d2_k (1 + delta) / (1 - delta), where d2_k is the k-th
+// re-ranked fp32 distance and delta bounds the re-rank's relative rounding, its fp32 distance exceeds d2_k and it
+// cannot enter the list.  A row that fails is searched directly (knn_direct_kernel); a false failure costs time
+// only.  The uncertified rows are appended to rows[] (in no particular order: each is searched on its own) and
+// counted in the header.
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+knn_certify_kernel(const float* __restrict__ cand_val, int kk, const float* __restrict__ norms,
+                   const float* __restrict__ d2_out, int k, int64_t n, CertBound b, unsigned* __restrict__ hdr,
+                   int32_t* __restrict__ rows) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= n) return;
+  float t = -__int_as_float(0x7f800000);
+  for (int q = lane; q < kk; q += 32) t = fmaxf(t, cand_val[row * kk + q]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) t = fmaxf(t, __shfl_xor_sync(kFull, t, o));
+  if (lane) return;
+  const bool centred = hdr[kHdrCentred] != 0;
+  const double a_cross = centred ? b.a_cen : b.a_unc, eta = centred ? b.eta : 0.0;
+  const double M2 = (double)__uint_as_float(hdr[kHdrMaxNorm]), M = sqrt(M2);
+  const double qn = (double)norms[row], qa = sqrt(qn);
+  const double E = kCertSafety * (2.0 * (a_cross * qa * M + eta * (qa + M)) + b.a_norm * M2 + b.a_abs);
+  const double lhs = (double)d2_out[row * k + k - 1] * (1.0 + b.delta) / (1.0 - b.delta) - qn + E;
+  if (!(lhs < (double)t - E)) rows[atomicAdd(reinterpret_cast<int*>(hdr + kHdrCount), 1)] = (int32_t)row;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// direct search of the uncertified rows: one warp per row sweeps all n rows with the re-rank's arithmetic (the same
+// fp32 bits) and keeps the k smallest (distance, index) pairs, ascending.  Only pairs up to the re-rank's k-th pair
+// can belong (the re-rank's k rows are k candidates with these very distances), which keeps insertions rare.
+// ---------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool pair_before(float d1, unsigned i1, float d2, unsigned i2) {
+  return d1 < d2 || (d1 == d2 && i1 < i2);
+}
+
+template <class T>
+__global__ void __launch_bounds__(256)
+knn_direct_kernel(const T* __restrict__ X, int64_t n, int d, int k, const unsigned* __restrict__ hdr,
+                  const int32_t* __restrict__ rows, int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+  __shared__ float s_d[8][kLongMaxK];
+  __shared__ unsigned s_i[8][kLongMaxK];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t slot = (int64_t)blockIdx.x * 8 + warp;
+  if (slot >= (int64_t)hdr[kHdrCount]) return;
+  const int64_t row = rows[slot];
+  float* ld = s_d[warp];
+  unsigned* li = s_i[warp];
+  for (int j = lane; j < k; j += 32) { ld[j] = __int_as_float(0x7f800000); li[j] = 0xffffffffu; }
+  __syncwarp();
+  const float bd = out_d2[row * k + k - 1];
+  const unsigned bi = (unsigned)out_idx[row * k + k - 1];
+  float thr = __int_as_float(0x7f800000);
+  unsigned thi = 0xffffffffu;
+  int worst = 0;
+  const T* xq = X + row * d;
+  for (int64_t c = 0; c < n; ++c) {
+    if (c == row) continue;
+    const T* xc = X + c * d;
+    float acc = 0.0f;
+    for (int j = lane; j < d; j += 32) { const float t = elem_f32(xq[j]) - elem_f32(xc[j]); acc = fmaf(t, t, acc); }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
+    // (warp-uniform) at most the re-rank's k-th pair, and before the worst kept pair
+    if (pair_before(bd, bi, acc, (unsigned)c) || !pair_before(acc, (unsigned)c, thr, thi)) continue;
+    if (lane == 0) { ld[worst] = acc; li[worst] = (unsigned)c; }
+    __syncwarp();
+    // the new worst: the largest (distance, index, slot) of the list
+    float m = -__int_as_float(0x7f800000); unsigned mi = 0; int w = -1;
+    for (int j = lane; j < k; j += 32) {
+      if (pair_before(m, mi, ld[j], li[j]) || (m == ld[j] && mi == li[j])) { m = ld[j]; mi = li[j]; w = j; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float om = __shfl_xor_sync(kFull, m, o);
+      const unsigned omi = __shfl_xor_sync(kFull, mi, o);
+      const int ow = __shfl_xor_sync(kFull, w, o);
+      if (pair_before(m, mi, om, omi) || (m == om && mi == omi && ow > w)) { m = om; mi = omi; w = ow; }
+    }
+    thr = m; thi = mi; worst = w;
+    __syncwarp();
+  }
+  // ascending by (distance, index): the rank of every slot among the k
+  int rank[kLongMaxK / 32];
+#pragma unroll
+  for (int s = 0; s < kLongMaxK / 32; ++s) {
+    const int j = lane + 32 * s;
+    rank[s] = 0;
+    if (j < k) for (int q = 0; q < k; ++q) rank[s] += pair_before(ld[q], li[q], ld[j], li[j]);
+  }
+#pragma unroll
+  for (int s = 0; s < kLongMaxK / 32; ++s) {
+    const int j = lane + 32 * s;
+    if (j < k) {
+      out_idx[row * k + rank[s]] = (int32_t)li[j];
+      out_d2[row * k + rank[s]] = ld[j];
+    }
+  }
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -609,8 +839,8 @@ int make_map(EncodeTiledFn enc, CUtensorMap* map, void* ptr, int64_t n_pad, int 
 }
 
 struct KnnLayout {
-  int64_t n_pad; int k_pad;
-  size_t off_h, off_l, off_norm, off_ci, off_cv, total;
+  int64_t n_pad; int k_pad, chunks;
+  size_t off_h, off_l, off_norm, off_ci, off_cv, off_mu, off_part, off_hdr, off_rows, total;
 };
 
 // kk: candidates kept per row (kKK, kWideKK for the wide search, kLongKK for the long one); split: fp32 input, whose
@@ -619,6 +849,7 @@ KnnLayout knn_layout(int64_t n, int d, int kk = kKK, bool split = true) {
   KnnLayout L;
   L.n_pad = (n + kTileN - 1) / kTileN * kTileN;
   L.k_pad = (d + kBlockK - 1) / kBlockK * kBlockK;
+  L.chunks = (int)((n + kMeanChunk - 1) / kMeanChunk);
   auto up = [](size_t x) { return (x + 1023) / 1024 * 1024; };
   size_t o = 0;
   L.off_h = o; o = up(o + (size_t)L.n_pad * L.k_pad * 2);
@@ -627,14 +858,63 @@ KnnLayout knn_layout(int64_t n, int d, int kk = kKK, bool split = true) {
   L.off_norm = o; o = up(o + (size_t)L.n_pad * 4);
   L.off_ci = o; o = up(o + (size_t)n * kk * 4);
   L.off_cv = o; o = up(o + (size_t)n * kk * 4);
+  L.off_mu = o; o = up(o + (size_t)d * 4);                   // column mean
+  L.off_part = o; o = up(o + (size_t)L.chunks * d * 8);      // its per-chunk fp64 sums
+  L.off_hdr = o; o = up(o + 4 * kHdrWords);                  // the search header (kHdr*)
+  L.off_rows = o; o = up(o + (size_t)n * 4);                 // the uncertified rows
   L.total = o;
   return L;
 }
 
-// mde_knn / mde_knn16: prep, tiles, re-rank of the 32 candidates.
+// The tiles' operand and norms: column mean, the centring decision, then prep.
+template <class T>
+int centre_and_prep(const T* X, int64_t n, int d, const KnnLayout& L, uint8_t* w, cudaStream_t st) {
+  double* part = reinterpret_cast<double*>(w + L.off_part);
+  float* mu = reinterpret_cast<float*>(w + L.off_mu);
+  unsigned* hdr = reinterpret_cast<unsigned*>(w + L.off_hdr);
+  MDE_CUDA_TRY(cudaMemsetAsync(hdr, 0, 4 * kHdrWords, st));
+  const unsigned gy = (unsigned)(L.chunks < kMaxGridY ? L.chunks : kMaxGridY);
+  knn_colsum_kernel<T><<<dim3((unsigned)((d + 127) / 128), gy), 128, 0, st>>>(X, n, d, L.chunks, part);
+  MDE_LAUNCH_CHECK();
+  knn_mean_kernel<<<(unsigned)((d + 127) / 128), 128, 0, st>>>(part, L.chunks, n, d, mu);
+  MDE_LAUNCH_CHECK();
+  knn_maxnorm_kernel<T><<<(unsigned)((n + 7) / 8), 256, 0, st>>>(X, n, d, mu, hdr);
+  MDE_LAUNCH_CHECK();
+  knn_prep_kernel<T><<<(unsigned)((L.n_pad + 7) / 8), 256, 0, st>>>(
+      X, n, d, L.n_pad, L.k_pad, mu, cert_bound<T>(d, L.k_pad), reinterpret_cast<OpT<T>*>(w + L.off_h),
+      reinterpret_cast<__nv_bfloat16*>(w + L.off_l), reinterpret_cast<float*>(w + L.off_norm), hdr);
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+
+// After the tiles: re-rank the KK candidates of every row, certify every row, search the uncertified rows directly;
+// with `fallback_rows`, wait for the stream and report how many rows that was.
+template <class T>
+int rerank_certify(int kk, const T* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, const KnnLayout& L,
+                   uint8_t* w, cudaStream_t st, int* fallback_rows) {
+  int rc;
+  if ((rc = knn_dense_rerank<T>(kk, X, n, d, reinterpret_cast<const int32_t*>(w + L.off_ci), k, idx_out, d2_out, st)))
+    return rc;
+  unsigned* hdr = reinterpret_cast<unsigned*>(w + L.off_hdr);
+  int32_t* rows = reinterpret_cast<int32_t*>(w + L.off_rows);
+  const unsigned grid = (unsigned)((n + 7) / 8);
+  knn_certify_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const float*>(w + L.off_cv), kk,
+                                           reinterpret_cast<const float*>(w + L.off_norm), d2_out, k, n,
+                                           cert_bound<T>(d, L.k_pad), hdr, rows);
+  MDE_LAUNCH_CHECK();
+  knn_direct_kernel<T><<<grid, 256, 0, st>>>(X, n, d, k, hdr, rows, idx_out, d2_out);
+  MDE_LAUNCH_CHECK();
+  if (fallback_rows) {
+    MDE_CUDA_TRY(cudaMemcpyAsync(fallback_rows, hdr + kHdrCount, sizeof(int), cudaMemcpyDeviceToHost, st));
+    MDE_CUDA_TRY(cudaStreamSynchronize(st));
+  }
+  return 0;
+}
+
+// mde_knn / mde_knn16: centring and prep, tiles, re-rank of the 32 candidates, certificate and direct search.
 template <class T>
 int run_narrow(const T* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
-               void* stream) {
+               void* stream, int* fallback_rows) {
   if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > kMaxK || k > n - 1) return MDE_E_INVALID;
   if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
   const KnnLayout L = knn_layout(n, d, kKK, Operand<T>::kSplit);
@@ -652,8 +932,7 @@ int run_narrow(const T* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_
   CUtensorMap mh, ml;
   if ((rc = make_map(enc, &mh, Xh, L.n_pad, L.k_pad, kTileM, Operand<T>::kMapType))) return rc;
   if ((rc = make_map(enc, &ml, Xl, L.n_pad, L.k_pad, kTileM, Operand<T>::kMapType))) return rc;
-  knn_prep_kernel<T><<<(unsigned)((L.n_pad + 7) / 8), 256, 0, st>>>(X, n, d, L.n_pad, L.k_pad, Xh, Xl, norms);
-  MDE_LAUNCH_CHECK();
+  if ((rc = centre_and_prep<T>(X, n, d, L, w, st))) return rc;
   static bool attr_set = false;
   if (!attr_set) {
     MDE_CUDA_TRY(cudaFuncSetAttribute(knn_tile_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
@@ -662,14 +941,14 @@ int run_narrow(const T* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_
   const unsigned grid = (unsigned)((n + kTileM - 1) / kTileM);
   knn_tile_kernel<T><<<grid, kThreads, kSmemBytes, st>>>(mh, ml, norms, n, L.n_pad, L.k_pad, ci, cv);
   MDE_LAUNCH_CHECK();
-  return knn_dense_rerank<T>(kKK, X, n, d, ci, k, idx_out, d2_out, st);
+  return rerank_certify<T>(kKK, X, n, d, k, idx_out, d2_out, L, w, st, fallback_rows);
 }
 
-// mde_knn_wide (KK = 96, TN = 128) and mde_knn_long (KK = 288, TN = 64), and their 16-bit entries: prep, tiles,
-// re-rank of all KK candidates.
+// mde_knn_wide (KK = 96, TN = 128) and mde_knn_long (KK = 288, TN = 64), and their 16-bit entries: centring and
+// prep, tiles, re-rank of all KK candidates, certificate and direct search.
 template <class T, int KK, int TN>
 int run_wide(const T* X, int64_t n, int d, int k, int max_k, int32_t* idx_out, float* d2_out, void* ws,
-             size_t ws_bytes, void* stream) {
+             size_t ws_bytes, void* stream, int* fallback_rows) {
   if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > max_k || k > n - 1) return MDE_E_INVALID;
   if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
   const KnnLayout L = knn_layout(n, d, KK, Operand<T>::kSplit);
@@ -690,8 +969,7 @@ int run_wide(const T* X, int64_t n, int d, int k, int max_k, int32_t* idx_out, f
   if ((rc = make_map(enc, &mal, Xl, L.n_pad, L.k_pad, kWideTileM, kType))) return rc;
   if ((rc = make_map(enc, &mh, Xh, L.n_pad, L.k_pad, TN, kType))) return rc;
   if ((rc = make_map(enc, &ml, Xl, L.n_pad, L.k_pad, TN, kType))) return rc;
-  knn_prep_kernel<T><<<(unsigned)((L.n_pad + 7) / 8), 256, 0, st>>>(X, n, d, L.n_pad, L.k_pad, Xh, Xl, norms);
-  MDE_LAUNCH_CHECK();
+  if ((rc = centre_and_prep<T>(X, n, d, L, w, st))) return rc;
   constexpr int kSmem = kWideSmemBytes<KK, TN>;
   static bool attr_set = false;
   if (!attr_set) {
@@ -703,7 +981,7 @@ int run_wide(const T* X, int64_t n, int d, int k, int max_k, int32_t* idx_out, f
   knn_wide_tile_kernel<T, KK, TN><<<grid, kWideThreads, kSmem, st>>>(mah, mal, mh, ml, norms, n, L.n_pad, L.k_pad, ci,
                                                                      cv);
   MDE_LAUNCH_CHECK();
-  return knn_dense_rerank<T>(KK, X, n, d, ci, k, idx_out, d2_out, st);
+  return rerank_certify<T>(KK, X, n, d, k, idx_out, d2_out, L, w, st, fallback_rows);
 }
 
 // The 16-bit entries: dtype code -> element type, MDE_E_INVALID for an unknown code (before any CUDA call).
@@ -715,20 +993,20 @@ int by_dtype(const void* X, int dtype, A... args) {
 }
 template <class T>
 struct Narrow {
-  static int call(const T* X, int64_t n, int d, int k, int32_t* i, float* d2, void* ws, size_t b, void* st) {
-    return run_narrow<T>(X, n, d, k, i, d2, ws, b, st);
+  static int call(const T* X, int64_t n, int d, int k, int32_t* i, float* d2, void* ws, size_t b, void* st, int* fb) {
+    return run_narrow<T>(X, n, d, k, i, d2, ws, b, st, fb);
   }
 };
 template <class T>
 struct Wide {
-  static int call(const T* X, int64_t n, int d, int k, int32_t* i, float* d2, void* ws, size_t b, void* st) {
-    return run_wide<T, kWideKK, kTileN>(X, n, d, k, kWideMaxK, i, d2, ws, b, st);
+  static int call(const T* X, int64_t n, int d, int k, int32_t* i, float* d2, void* ws, size_t b, void* st, int* fb) {
+    return run_wide<T, kWideKK, kTileN>(X, n, d, k, kWideMaxK, i, d2, ws, b, st, fb);
   }
 };
 template <class T>
 struct Long {
-  static int call(const T* X, int64_t n, int d, int k, int32_t* i, float* d2, void* ws, size_t b, void* st) {
-    return run_wide<T, kLongKK, kLongTileN>(X, n, d, k, kLongMaxK, i, d2, ws, b, st);
+  static int call(const T* X, int64_t n, int d, int k, int32_t* i, float* d2, void* ws, size_t b, void* st, int* fb) {
+    return run_wide<T, kLongKK, kLongTileN>(X, n, d, k, kLongMaxK, i, d2, ws, b, st, fb);
   }
 };
 
@@ -746,48 +1024,80 @@ int mde_knn_max_k(void) { return kMaxK; }
 
 int mde_knn_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kKK, true, bytes); }
 
+int mde_knn_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
+               void* stream, int* fallback_rows) {
+  return run_narrow<float>(X, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
+}
+
 int mde_knn(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
             void* stream) {
-  return run_narrow<float>(X, n, d, k, idx_out, d2_out, ws, ws_bytes, stream);
+  return mde_knn_ex(X, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
 int mde_knn_wide_max_k(void) { return kWideMaxK; }
 
 int mde_knn_wide_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kWideKK, true, bytes); }
 
+int mde_knn_wide_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                    size_t ws_bytes, void* stream, int* fallback_rows) {
+  return run_wide<float, kWideKK, kTileN>(X, n, d, k, kWideMaxK, idx_out, d2_out, ws, ws_bytes, stream,
+                                          fallback_rows);
+}
+
 int mde_knn_wide(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                  size_t ws_bytes, void* stream) {
-  return run_wide<float, kWideKK, kTileN>(X, n, d, k, kWideMaxK, idx_out, d2_out, ws, ws_bytes, stream);
+  return mde_knn_wide_ex(X, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
 int mde_knn_long_max_k(void) { return kLongMaxK; }
 
 int mde_knn_long_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kLongKK, true, bytes); }
 
+int mde_knn_long_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                    size_t ws_bytes, void* stream, int* fallback_rows) {
+  return run_wide<float, kLongKK, kLongTileN>(X, n, d, k, kLongMaxK, idx_out, d2_out, ws, ws_bytes, stream,
+                                              fallback_rows);
+}
+
 int mde_knn_long(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                  size_t ws_bytes, void* stream) {
-  return run_wide<float, kLongKK, kLongTileN>(X, n, d, k, kLongMaxK, idx_out, d2_out, ws, ws_bytes, stream);
+  return mde_knn_long_ex(X, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
 int mde_knn16_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kKK, false, bytes); }
 
+int mde_knn16_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                 size_t ws_bytes, void* stream, int* fallback_rows) {
+  return by_dtype<Narrow>(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
+}
+
 int mde_knn16(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
               size_t ws_bytes, void* stream) {
-  return by_dtype<Narrow>(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream);
+  return mde_knn16_ex(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
 int mde_knn16_wide_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kWideKK, false, bytes); }
 
+int mde_knn16_wide_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                      size_t ws_bytes, void* stream, int* fallback_rows) {
+  return by_dtype<Wide>(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
+}
+
 int mde_knn16_wide(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                    size_t ws_bytes, void* stream) {
-  return by_dtype<Wide>(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream);
+  return mde_knn16_wide_ex(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
 int mde_knn16_long_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kLongKK, false, bytes); }
 
+int mde_knn16_long_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                      size_t ws_bytes, void* stream, int* fallback_rows) {
+  return by_dtype<Long>(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
+}
+
 int mde_knn16_long(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                    size_t ws_bytes, void* stream) {
-  return by_dtype<Long>(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream);
+  return mde_knn16_long_ex(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
 }  // extern "C"

@@ -19,7 +19,13 @@ A float16 / bfloat16 matrix (a torch tensor on any device, or an np.float16 arra
 without an fp32 copy: the `mde_knn16*` entries use it as the tensor-core operand and convert each element to fp32 as
 the re-rank and NN-descent read it, so neighbours and distances are those of the fp32 search on the upcast matrix
 (DESIGN section 11.7).  The routing by k and PYMDE_B200_KNN is unchanged; the GEMM path, and every other dtype,
-still work on an fp32 copy."""
+still work on an fp32 copy.
+
+The dense exact searches are exact on data far from the origin and on far-apart clusters: the kernels centre the
+columns when that bounds the score error more tightly (a 16-bit matrix near the origin stays its own exact operand)
+and certify every row, searching the rows that fail directly (DESIGN section 11), and the GEMM path scores
+candidates with fp64 matmuls of the centred matrix, independent of torch's TF32 setting, then re-ranks them by fp32
+distance and index."""
 import ctypes as C
 import os
 
@@ -237,17 +243,38 @@ def _search(data, k, dev, chunk_rows=None):
         # on the GEMM path below, which measured faster on 70 000 x 784 at k = 65 .. 256 (DESIGN section 11.6)
         idx, d2 = knn_device(X, k)
         return idx, d2, n
-    X = X.float()
-    sq = (X * X).sum(1)
-    rows = chunk_rows or max(256, min(n, int(2 ** 27 // max(n, 1))))
+    idx, d2 = _gemm_search(X.float(), k, chunk_rows)
+    return idx, d2, n
+
+
+def _gemm_search(X, k, chunk_rows=None):
+    """(idx [n, k] int64, squared distances [n, k] fp32) of the k nearest rows of every row of the device fp32 matrix
+    X, by row chunks of a library GEMM: candidate scores ||x||^2 - 2 q.x of the fp64 column-centred matrix (fp64
+    matmuls, whatever torch.backends.cuda.matmul.allow_tf32 says; centring keeps the cancellation of data far from the
+    origin out of the scores), the k + 8 best kept, then re-ranked by their fp32 squared distances (sum of squared fp32
+    differences) and index, ascending."""
+    n, d = X.shape
+    dev = X.device
+    Xd = X.double()
+    Xd -= Xd.mean(0)
+    sq = (Xd * Xd).sum(1)
+    kc = min(k + 8, n - 1)
+    rows = chunk_rows or max(256, min(n, int(2 ** 26 // max(n, 1))))
+    sub = max(1, int(2 ** 26 // max(kc * d, 1)))  # rows per fp32 re-rank batch (256 MB of differences)
     idxs, vals = [], []
     for s0 in range(0, n, rows):
-        Q = X[s0:s0 + rows]
-        d2 = (sq[s0:s0 + rows, None] + sq[None, :] - 2.0 * (Q @ X.T)).clamp_(min=0)
-        d2[torch.arange(Q.shape[0], device=dev), torch.arange(s0, s0 + Q.shape[0], device=dev)] = float("inf")
-        val, idx = torch.topk(d2, k, dim=1, largest=False)
-        idxs.append(idx); vals.append(val)
-    return torch.cat(idxs), torch.cat(vals), n
+        Q = Xd[s0:s0 + rows]
+        score = sq[None, :] - 2.0 * (Q @ Xd.T)  # ||q||^2 is constant along a row
+        score[torch.arange(Q.shape[0], device=dev), torch.arange(s0, s0 + Q.shape[0], device=dev)] = float("inf")
+        cand = torch.topk(score, kc, dim=1, largest=False)[1]
+        del score
+        cand = torch.sort(cand, 1)[0]  # index order, so that the stable sort below breaks ties by index
+        for r0 in range(0, cand.shape[0], sub):
+            c = cand[r0:r0 + sub]
+            d2 = ((X[s0 + r0:s0 + r0 + c.shape[0], None, :] - X[c]) ** 2).sum(-1)
+            d2, pos = torch.sort(d2, dim=1, stable=True)
+            idxs.append(torch.gather(c, 1, pos[:, :k])); vals.append(d2[:, :k])
+    return torch.cat(idxs), torch.cat(vals)
 
 
 def k_nearest_neighbors(data, k, max_distance=None, verbose=False, device=None, chunk_rows=None):
