@@ -31,7 +31,7 @@ extern "C" {
 
 /* error codes (negative; positive values are cudaError_t) */
 #define MDE_E_INVALID   (-1)  /* bad argument */
-#define MDE_E_UNSUPPORTED (-2) /* combination not built (e.g. Standardized with m > 32) */
+#define MDE_E_UNSUPPORTED (-2) /* combination not built (e.g. Standardized with m > 1024) */
 #define MDE_E_NAN       (-3)  /* line search: function/gradient stayed NaN/Inf (lbfgs.py:70-80) */
 #define MDE_E_ALLOC     (-4)
 #define MDE_E_COMM      (-5)  /* multi-GPU: a peer never arrived at the all-reduce handshake (bounded spin) */
@@ -183,8 +183,8 @@ int64_t mde_project_ws_bytes(int64_t n, int m);
 int mde_project_centered(float* X, int64_t n, int m, void* ws, void* stream);
 /* _Standardized.project_onto_constraint, constraints.py:194-195 -> util.py:129-171:
  * de-mean, then sqrt(n) * polar factor, computed as X (X^T X)^(-1/2) via the m x m Gram: a Jacobi eigensolver in
- * one warp for m <= 32, a tiled Gram kernel + fp64 Newton-Schulz inverse square root for 32 < m <= 256 (the reference
- * pins m = 250 in pymde/test_util.py:20-71).  m > 256: MDE_E_UNSUPPORTED.  The Gram is taken of X - s, s near the column
+ * one warp for m <= 32, a tiled Gram kernel + fp64 Newton-Schulz inverse square root for 32 < m <= 1024 (the reference
+ * pins m = 250 in pymde/test_util.py:20-71).  m > 1024: MDE_E_UNSUPPORTED.  The Gram is taken of X - s, s near the column
  * means (from the first 32 rows), so columns far from the origin keep their digits.  Asynchronous; a singular Gram is not an error code but a status word in
  * `ws`, read by mde_project_status.  The device solver's own retractions do not read it. */
 int mde_project_standardized(float* X, int64_t n, int m, void* ws, void* stream);
@@ -193,7 +193,7 @@ int mde_project_standardized(float* X, int64_t n, int m, void* ws, void* stream)
  * smallest Gram eigenvalue <= 1e-12 x the largest for m <= 32, or a Newton-Schulz chain that did not converge for
  * m > 32; W and X are then not meaningful).  Returns 0 or an error code. */
 int mde_project_status(const void* ws, int m, int* status, void* stream);
-/* _Standardized.project_onto_tangent_space, constraints.py:186-192: Z -= (1/n) X (Z^T X).  m <= 256. */
+/* _Standardized.project_onto_tangent_space, constraints.py:186-192: Z -= (1/n) X (Z^T X).  m <= 1024. */
 int mde_tangent_standardized(const float* X, float* Z, int64_t n, int m, void* ws, void* stream);
 
 /* ---------------------------------------------------------------------------------------

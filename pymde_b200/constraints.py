@@ -116,12 +116,12 @@ class _Standardized(Constraint):
         _check(out)
         _check(X)
         n, m = out.shape
-        if m <= 256:
+        if m <= 1024:
             lib = _lib.load()
             _lib.check(lib.mde_tangent_standardized(X.data_ptr(), out.data_ptr(), n, m, _ws(out).data_ptr(),
                                                     util.stream_ptr(out.device)))
             return out
-        with torch.no_grad():  # m > 256: plain library GEMMs for the m x m product
+        with torch.no_grad():  # m > 1024: plain library GEMMs for the m x m product
             gtx = out.T @ X
             out.sub_((1.0 / n) * (X @ gtx))
         return out

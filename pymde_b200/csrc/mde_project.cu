@@ -135,10 +135,11 @@ moments_warp_kernel(const float* __restrict__ Z, const float* __restrict__ X, in
   }
 }
 
-// wide rows (m > 32): column sums only.  thread t owns column t % mpad of row-lane t / mpad.
+// wide rows (m > 32): column sums only.  thread t owns column t % mpad of row-lane t / mpad.  shift (nullable): sums
+// of X - s, s = proj_shift(shift), stored in shift_out (see moments_small_kernel).
 __global__ void __launch_bounds__(kProjThreads)
 colsum_wide_kernel(const float* __restrict__ X, int64_t n, int m, int mpad,
-                   double* __restrict__ partials, const int* active) {
+                   double* __restrict__ partials, const float* shift, double* shift_out, const int* active) {
   if (inactive(active)) return;
   __shared__ double sm[kProjThreads];
   const int nrl = mpad >= kProjThreads ? 1 : kProjThreads / mpad;
@@ -147,10 +148,15 @@ colsum_wide_kernel(const float* __restrict__ X, int64_t n, int m, int mpad,
     int c = cb + c0;
     double acc = 0.0;
     if (c < m && rl < nrl) {
+      float s = 0.0f;
+      if (shift) {
+        s = proj_shift(shift, n, m, c);
+        if (blockIdx.x == 0 && rl == 0) shift_out[c] = (double)s;
+      }
       float facc = 0.0f;
       int cnt = 0;
       for (int64_t r = (int64_t)blockIdx.x * nrl + rl; r < n; r += (int64_t)gridDim.x * nrl) {
-        facc += X[r * m + c];
+        facc += shift ? X[r * m + c] - s : X[r * m + c];
         if (++cnt == 64) { acc += (double)facc; facc = 0.0f; cnt = 0; }
       }
       acc += (double)facc;
@@ -167,7 +173,7 @@ colsum_wide_kernel(const float* __restrict__ X, int64_t n, int m, int mpad,
 }
 
 __global__ void colmean_finalize_kernel(const double* __restrict__ partials, int nblocks, int64_t n, int m,
-                                        double* __restrict__ mean, const int* active) {
+                                        const double* shift, double* __restrict__ mean, const int* active) {
   if (inactive(active)) return;
   // one warp per column
   const int lane = threadIdx.x & 31;
@@ -176,7 +182,7 @@ __global__ void colmean_finalize_kernel(const double* __restrict__ partials, int
     double s = 0.0;
     for (int b = lane; b < nblocks; b += 32) s += partials[(int64_t)b * m + k];
     s = warp_sum(s);
-    if (lane == 0) mean[k] = s / (double)n;
+    if (lane == 0) mean[k] = shift ? shift[k] + s / (double)n : s / (double)n;
   }
 }
 
@@ -428,14 +434,15 @@ int launch_rowmat(const float* X, float* Y, int64_t n, int m, const ProjWs& w, c
 
 namespace mde {
 
-int enqueue_colmean_wide(const float* X, int64_t n, int m, const ProjWs& w, const int* active, cudaStream_t st) {
+int enqueue_colmean_wide(const float* X, int64_t n, int m, const ProjWs& w, const int* active, cudaStream_t st,
+                         const float* shift) {
   int mpad = 64;
   while (mpad < m && mpad < kProjThreads) mpad <<= 1;
   int nrl = kProjThreads / mpad;
   const int nb = blocks_for_rows(n, nrl * 8);
-  colsum_wide_kernel<<<nb, kProjThreads, 0, st>>>(X, n, m, mpad, w.partials, active);
+  colsum_wide_kernel<<<nb, kProjThreads, 0, st>>>(X, n, m, mpad, w.partials, shift, w.shift, active);
   MDE_LAUNCH_CHECK();
-  colmean_finalize_kernel<<<(m + 7) / 8, 256, 0, st>>>(w.partials, nb, n, m, w.mean, active);
+  colmean_finalize_kernel<<<(m + 7) / 8, 256, 0, st>>>(w.partials, nb, n, m, shift ? w.shift : nullptr, w.mean, active);
   MDE_LAUNCH_CHECK();
   return 0;
 }

@@ -1,11 +1,12 @@
-// mde_project_wide.cu -- the Standardized constraint for wide embeddings, 32 < m <= 256, on the device.
+// mde_project_wide.cu -- the Standardized constraint for wide embeddings, 32 < m <= 1024, on the device.
 //
 // Reference: pymde/constraints.py:167-200 -> pymde/util.py:129-171 (de-mean, thin SVD of the n x m matrix,
 // sqrt(n) U V^T; pinned at m = 250 by pymde/test_util.py:20-71) and pymde/constraints.py:186-192 (tangent space:
 // Z -= (1/n) X (Z^T X)).  The narrow path (mde_project.cu) eigen-decomposes the m x m Gram matrix in one warp; that
 // does not scale to m = 256.  Here everything is a tiled product:
 //
-//   gram      P[rb] = Z[rows rb]^T X[rows rb]   64 x 64 output tiles, 4 x 4 per thread, fp32 inside a row block
+//   gram      P[rb] = Z[rows rb]^T X[rows rb]   64 x 64 output tiles, 4 x 4 per thread (m <= 256), or 128 x 128, 8 x 8
+//                                               per thread (m > 256); fp32 inside a row block of <= ceil(n / 16) rows
 //   reduce    G = sum_rb P[rb]                  fp64 across row blocks (fixed order)
 //   retraction:   G is the Gram of X - s (s = proj_shift, near the column mean) ;  A = (G - n (mu - s)(mu - s)^T) / n ;
 //                 W = A^(-1/2) by the coupled Newton-Schulz iteration
@@ -13,9 +14,12 @@
 //                 in fp64 with c = ||A||_inf >= lambda_max (so the iteration converges for every positive definite
 //                 A); an embedding that is already nearly standardized -- every trial point of the solver -- has
 //                 A = I + E and needs 4-6 iterations.  The iterations are enqueued as a FIXED chain (CUDA-graph
-//                 capturable) and switch themselves off through a device flag once ||I - Z Y||_F < 1e-9 m.
-//   rowmat    X <- (X - mu) W   or   Z <- Z - X (G / n):  32 rows x all columns per block, the block's rows held
-//             in shared memory (which makes the in-place update safe), the matrix streamed in 16-row slabs.
+//                 capturable) and switch themselves off through a device flag once ||I - Z Y||_F < 1e-9 m.  The
+//                 m x m products run on FFMA up to m = 256 and on the fp64 tensor cores (DMMA) above.
+//   rowmat    X <- (X - mu) W   or   Z <- Z - X (G / n).  m <= 256: 32 rows x all columns per block, the block's rows
+//             held in shared memory (which makes the in-place update safe), the matrix streamed in 16-row slabs.
+//             m > 256: 128 x 128 output tiles like the Gram; the retraction writes each chunk of 16 m rows to the
+//             (then free) fpart region and copies it back.
 //
 // Every kernel takes the solver's `active` gate like the narrow path.
 #include "mde_project.cuh"
@@ -26,68 +30,77 @@ namespace {
 
 __device__ __forceinline__ bool inactive(const int* active) { return active != nullptr && *active == 0; }
 
-constexpr int kGT = 64;   // Gram output tile
 constexpr int kGK = 16;   // rows per shared-memory stage
 
 // P[rb][a][b] = sum over the rows of row block rb of (Z[r][a] - s[a]) (X[r][b] - s[b]);  grid = (tiles*tiles, row
-// blocks).  s = proj_shift(shift) (nullable; the retraction passes X, and s goes to shift_out): the products of the shifted rows
-// keep the fp32 digits that G - n mu mu^T would cancel when the columns sit far from the origin.
-__global__ void __launch_bounds__(256)
+// blocks), T = 16 TM output tiles, TM x TM per thread.  s = proj_shift(shift) (nullable; the retraction passes X, and
+// s goes to shift_out): the products of the shifted rows keep the fp32 digits that G - n mu mu^T would cancel when the
+// columns sit far from the origin.  A thread owns rows (and columns) t * 4 + (i & 3) + 64 (i >> 2), i < TM, of the
+// tile; each of its sums runs over the block's rows in order, so the tile size does not change any P element.
+template <int TM>
+__global__ void __launch_bounds__(256, TM == 8 ? 2 : 0)
 gram_wide_kernel(const float* __restrict__ Z, const float* __restrict__ X, int64_t n, int m, int tiles,
                  int64_t rows_per_block, float* __restrict__ P, const float* shift, double* shift_out,
                  const int* active) {
+  constexpr int T = 16 * TM;
+  constexpr int Q = kGK * T / 256;  // staged elements per thread and operand
   if (inactive(active)) return;
-  __shared__ __align__(16) float sA[kGK][kGT + 4];
-  __shared__ __align__(16) float sB[kGK][kGT + 4];
+  __shared__ __align__(16) float sA[kGK][T + 4];
+  __shared__ __align__(16) float sB[kGK][T + 4];
   const int ta = blockIdx.x / tiles, tb = blockIdx.x % tiles;
   const int ty = threadIdx.x >> 4, tx = threadIdx.x & 15;
-  // every element this thread stages lies in column threadIdx.x & 63 of the two tiles
+  // every element this thread stages lies in column threadIdx.x % T of the two tiles
   float sa = 0.0f, sb = 0.0f;
   if (shift) {
-    const int ca = ta * kGT + (threadIdx.x & 63), cb = tb * kGT + (threadIdx.x & 63);
+    const int ca = ta * T + (threadIdx.x % T), cb = tb * T + (threadIdx.x % T);
     if (ca < m) sa = proj_shift(shift, n, m, ca);
     if (cb < m) sb = proj_shift(shift, n, m, cb);
-    if (blockIdx.y == 0 && tb == 0 && threadIdx.x < kGT && ca < m) shift_out[ca] = (double)sa;
+    if (blockIdx.y == 0 && tb == 0 && threadIdx.x < T && ca < m) shift_out[ca] = (double)sa;
   }
   const int64_t r0 = (int64_t)blockIdx.y * rows_per_block;
   int64_t r1 = r0 + rows_per_block;
   if (r1 > n) r1 = n;
-  float acc[4][4];
+  float acc[TM][TM];
 #pragma unroll
-  for (int i = 0; i < 4; ++i)
+  for (int i = 0; i < TM; ++i)
 #pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j] = 0.0f;
+    for (int j = 0; j < TM; ++j) acc[i][j] = 0.0f;
   for (int64_t r = r0; r < r1; r += kGK) {
-    // 16 rows x 64 columns of each operand: 1024 elements, 4 per thread
+    // kGK rows x T columns of each operand
 #pragma unroll
-    for (int q = 0; q < 4; ++q) {
+    for (int q = 0; q < Q; ++q) {
       const int e = threadIdx.x + 256 * q;
-      const int kk = e >> 6, c = e & 63;
+      const int kk = e / T, c = e % T;
       const int64_t row = r + kk;
-      const int ca = ta * kGT + c, cb = tb * kGT + c;
+      const int ca = ta * T + c, cb = tb * T + c;
       sA[kk][c] = (row < r1 && ca < m) ? Z[row * m + ca] - sa : 0.0f;
       sB[kk][c] = (row < r1 && cb < m) ? X[row * m + cb] - sb : 0.0f;
     }
     __syncthreads();
 #pragma unroll
     for (int kk = 0; kk < kGK; ++kk) {
-      const float4 av = *reinterpret_cast<const float4*>(&sA[kk][ty * 4]);
-      const float4 bv = *reinterpret_cast<const float4*>(&sB[kk][tx * 4]);
-      const float a[4] = {av.x, av.y, av.z, av.w}, b[4] = {bv.x, bv.y, bv.z, bv.w};
+      float a[TM], b[TM];
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
+      for (int h = 0; h < TM / 4; ++h) {
+        const float4 av = *reinterpret_cast<const float4*>(&sA[kk][ty * 4 + 64 * h]);
+        const float4 bv = *reinterpret_cast<const float4*>(&sB[kk][tx * 4 + 64 * h]);
+        a[4 * h] = av.x; a[4 * h + 1] = av.y; a[4 * h + 2] = av.z; a[4 * h + 3] = av.w;
+        b[4 * h] = bv.x; b[4 * h + 1] = bv.y; b[4 * h + 2] = bv.z; b[4 * h + 3] = bv.w;
+      }
 #pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+      for (int i = 0; i < TM; ++i)
+#pragma unroll
+        for (int j = 0; j < TM; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
     }
     __syncthreads();
   }
   float* out = P + (int64_t)blockIdx.y * m * m;
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int a = ta * kGT + ty * 4 + i;
+  for (int i = 0; i < TM; ++i) {
+    const int a = ta * T + ty * 4 + (i & 3) + 64 * (i >> 2);
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int b = tb * kGT + tx * 4 + j;
+    for (int j = 0; j < TM; ++j) {
+      const int b = tb * T + tx * 4 + (j & 3) + 64 * (j >> 2);
       if (a < m && b < m) out[(int64_t)a * m + b] = acc[i][j];
     }
   }
@@ -155,8 +168,8 @@ ns_init_kernel(const double* __restrict__ G, const double* __restrict__ mean, co
   }
 }
 
-// C = alpha A B + beta I on m x m fp64 matrices, 32 x 32 tiles (2 x 2 per thread).  blockIdx.z selects one of two
-// independent products (Y T and T Z in one launch).
+// C = alpha A B + beta I on m x m fp64 matrices.  blockIdx.z selects one of two independent products (Y T and T Z in
+// one launch).
 //
 // Gating of the fixed chain: iteration `it` accumulates r_it = ||I - Z_it Y_it||_F^2 into slot it % 3 (first kernel,
 // RES).  A kernel of iteration it idles when the sticky flag is set (by an EARLIER launch) or when r_(it-1) < tol^2;
@@ -165,19 +178,27 @@ ns_init_kernel(const double* __restrict__ G, const double* __restrict__ mean, co
 // improves the iterate).  The second kernel of an iteration zeroes the slot of the next one.
 struct MmArgs { const double* A; const double* B; double* C; };
 
+// true: this launch of the chain idles
+template <bool RES>
+__device__ __forceinline__ bool ns_gate(const double* res_prev, double* res_zero, double tol2, int* nsflag, int cur) {
+  const bool first = blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0;
+  if (nsflag[0]) return true;
+  if (res_prev != nullptr && *res_prev < tol2) {
+    if (RES && first) { nsflag[1] = cur; __threadfence(); nsflag[0] = 1; }
+    return true;
+  }
+  if (!RES && first && res_zero) *res_zero = 0.0;
+  return false;
+}
+
+// m <= 256: 32 x 32 tiles, 2 x 2 per thread on FFMA
 template <bool RES>
 __global__ void __launch_bounds__(256)
 ns_mm_kernel(MmArgs p0, MmArgs p1, int m, double alpha, double beta, double* __restrict__ res_acc,
              const double* __restrict__ res_prev, double* __restrict__ res_zero, double tol2, int* __restrict__ nsflag,
              int cur, const int* active) {
   if (inactive(active)) return;
-  const bool first = blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0;
-  if (nsflag[0]) return;
-  if (res_prev != nullptr && *res_prev < tol2) {
-    if (RES && first) { nsflag[1] = cur; __threadfence(); nsflag[0] = 1; }
-    return;
-  }
-  if (!RES && first && res_zero) *res_zero = 0.0;
+  if (ns_gate<RES>(res_prev, res_zero, tol2, nsflag, cur)) return;
   const MmArgs p = blockIdx.z ? p1 : p0;
   __shared__ double sA[32][17];
   __shared__ double sB[16][33];
@@ -216,6 +237,85 @@ ns_mm_kernel(MmArgs p0, MmArgs p1, int m, double alpha, double beta, double* __r
   if (RES) {
     r2 = warp_sum(r2);
     if ((threadIdx.x & 31) == 0 && r2 != 0.0) atomicAdd(res_acc, r2);
+  }
+}
+
+// m > 256: 64 x 64 tiles on the fp64 tensor cores, mma.m16n8k16 (DMMA.16x8x16); 4 warps of 32 x 32, k staged 32 at
+// a time.  Fragments (g = lane / 4, t = lane % 4): A a_q at (g + 8 (q & 1), t + 4 (q >> 1)), B b_q at (t + 4 q, g),
+// C c_q at (g + 8 (q >> 1), 2 t + (q & 1)).  Each element is an fp64 sum of the same products as the FFMA kernel's.
+constexpr int kDT = 64, kDK = 32;
+__device__ __forceinline__ void dmma16816(double (&d)[4], const double (&a)[8], const double (&b)[4]) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+               "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
+               : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+               : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]),
+                 "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
+}
+
+template <bool RES>
+__global__ void __launch_bounds__(128)
+ns_dmma_kernel(MmArgs p0, MmArgs p1, int m, double alpha, double beta, double* __restrict__ res_acc,
+               const double* __restrict__ res_prev, double* __restrict__ res_zero, double tol2,
+               int* __restrict__ nsflag, int cur, const int* active) {
+  if (inactive(active)) return;
+  if (ns_gate<RES>(res_prev, res_zero, tol2, nsflag, cur)) return;
+  const MmArgs p = blockIdx.z ? p1 : p0;
+  __shared__ double sA[kDT][kDK + 4];   // A[a0 + r][k0 + c]
+  __shared__ double sB[kDK][kDT + 4];   // B[k0 + r][b0 + c]
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int g = lane >> 2, t = lane & 3;
+  const int wr = (warp >> 1) * 32, wc = (warp & 1) * 32;
+  const int a0 = blockIdx.y * kDT, b0 = blockIdx.x * kDT;
+  double acc[2][4][4];
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) acc[i][j][q] = 0.0;
+  for (int k0 = 0; k0 < m; k0 += kDK) {
+#pragma unroll
+    for (int q = 0; q < kDT * kDK / 128; ++q) {
+      const int e = threadIdx.x + 128 * q;
+      { const int r = e / kDK, c = e % kDK; const int a = a0 + r, k = k0 + c; sA[r][c] = (a < m && k < m) ? p.A[(int64_t)a * m + k] : 0.0; }
+      { const int r = e / kDT, c = e % kDT; const int k = k0 + r, b = b0 + c; sB[r][c] = (k < m && b < m) ? p.B[(int64_t)k * m + b] : 0.0; }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < kDK; kk += 16) {
+      double af[2][8], bf[4][4];
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int q = 0; q < 8; ++q) af[i][q] = sA[wr + 16 * i + g + 8 * (q & 1)][kk + t + 4 * (q >> 1)];
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) bf[j][q] = sB[kk + t + 4 * q][wc + 8 * j + g];
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) dmma16816(acc[i][j], af[i], bf[j]);
+    }
+    __syncthreads();
+  }
+  double r2 = 0.0;
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int a = a0 + wr + 16 * i + g + 8 * (q >> 1), b = b0 + wc + 8 * j + 2 * t + (q & 1);
+        if (a < m && b < m) {
+          const double id = (a == b) ? 1.0 : 0.0;
+          if (RES) { const double e = id - acc[i][j][q]; r2 += e * e; }
+          p.C[(int64_t)a * m + b] = alpha * acc[i][j][q] + beta * id;
+        }
+      }
+  if (RES) {
+    r2 = warp_sum(r2);
+    if (lane == 0 && r2 != 0.0) atomicAdd(res_acc, r2);
   }
 }
 
@@ -296,9 +396,89 @@ rowmat_wide_kernel(const float* __restrict__ X, float* __restrict__ Y, int64_t n
   }
 }
 
+// m > 256: O = (X - mu) W  (MODE 0)  or  O = B - X W  (MODE 1) over `rows` rows, as 128 x 128 output tiles, 8 x 8 per
+// thread, k staged kGK at a time -- the Gram kernel's layout with X as the row operand.  O may be B (the tangent: Z is
+// not read by the product) but not X: the retraction writes its rows to a staging region and copies them back.  Each
+// output is the ascending fp32 sum over k, as in rowmat_wide_kernel.
+template <int MODE>
+__global__ void __launch_bounds__(256, 2)
+rowgemm_kernel(const float* __restrict__ X, const float* B, float* O, int rows, int m,
+               const double* __restrict__ mean, const float* __restrict__ W, const int* active) {
+  constexpr int T = 128;
+  if (inactive(active)) return;
+  __shared__ __align__(16) float sA[kGK][T + 4];  // sA[k][r] = X[r0 + r][k0 + k] (- mu)
+  __shared__ __align__(16) float sB[kGK][T + 4];  // sB[k][c] = W[k0 + k][c0 + c]
+  const int r0 = blockIdx.y * T;  // rows * m < 2^31: a chunk is at most the fpart region
+  const int c0 = blockIdx.x * T;
+  const int ty = threadIdx.x >> 4, tx = threadIdx.x & 15;
+  float acc[8][8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[i][j] = 0.0f;
+  for (int k0 = 0; k0 < m; k0 += kGK) {
+#pragma unroll
+    for (int q = 0; q < kGK * T / 256; ++q) {
+      const int e = threadIdx.x + 256 * q;
+      {
+        const int r = e / kGK, k = e % kGK;
+        const int row = r0 + r;
+        const int kk = k0 + k;
+        float v = 0.0f;
+        if (row < rows && kk < m) {
+          v = X[row * m + kk];
+          if (MODE == 0) v -= (float)mean[kk];
+        }
+        sA[k][r] = v;
+      }
+      {
+        const int k = e / T, c = e % T;
+        const int kk = k0 + k, col = c0 + c;
+        sB[k][c] = (kk < m && col < m) ? W[(int64_t)kk * m + col] : 0.0f;
+      }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < kGK; ++kk) {
+      float a[8], b[8];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float4 av = *reinterpret_cast<const float4*>(&sA[kk][ty * 4 + 64 * h]);
+        const float4 bv = *reinterpret_cast<const float4*>(&sB[kk][tx * 4 + 64 * h]);
+        a[4 * h] = av.x; a[4 * h + 1] = av.y; a[4 * h + 2] = av.z; a[4 * h + 3] = av.w;
+        b[4 * h] = bv.x; b[4 * h + 1] = bv.y; b[4 * h + 2] = bv.z; b[4 * h + 3] = bv.w;
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int row = r0 + ty * 4 + (i & 3) + 64 * (i >> 2);
+    if (row >= rows) continue;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int col = c0 + tx * 4 + (j & 3) + 64 * (j >> 2);
+      if (col < m) O[row * m + col] = (MODE == 0) ? acc[i][j] : B[row * m + col] - acc[i][j];
+    }
+  }
+}
+
+// dst[k] = src[k], k < count (gated: a memcpy node would run in an inactive step too)
+__global__ void __launch_bounds__(256)
+copy_kernel(const float* __restrict__ src, float* __restrict__ dst, int64_t count, const int* active) {
+  if (inactive(active)) return;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < count; k += stride) dst[k] = src[k];
+}
+
 int launch_gram(const float* Z, const float* X, int64_t n, int m, const float* shift, const ProjWs& w,
                 const int* active, cudaStream_t st) {
-  const int tiles = (m + kGT - 1) / kGT;
+  const int T = wide_gram_tile(m);
+  const int tiles = (m + T - 1) / T;
   int rb = wide_row_blocks(m);
   const int64_t max_rb = (n + 255) / 256;  // at least 256 rows per block
   if (rb > max_rb) rb = (int)max_rb;
@@ -307,10 +487,29 @@ int launch_gram(const float* Z, const float* X, int64_t n, int m, const float* s
   rows_per_block = (rows_per_block + kGK - 1) / kGK * kGK;
   rb = (int)((n + rows_per_block - 1) / rows_per_block);
   dim3 grid(tiles * tiles, rb);
-  gram_wide_kernel<<<grid, 256, 0, st>>>(Z, X, n, m, tiles, rows_per_block, w.fpart, shift, w.shift, active);
+  if (T == 64) gram_wide_kernel<4><<<grid, 256, 0, st>>>(Z, X, n, m, tiles, rows_per_block, w.fpart, shift, w.shift, active);
+  else gram_wide_kernel<8><<<grid, 256, 0, st>>>(Z, X, n, m, tiles, rows_per_block, w.fpart, shift, w.shift, active);
   MDE_LAUNCH_CHECK();
   const int64_t mm = (int64_t)m * m;
   gram_reduce_kernel<<<(unsigned)((mm + 255) / 256), 256, 0, st>>>(w.fpart, rb, mm, w.gram, active);
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+
+// one fixed-chain product launch: ZY (RES, one product) or Y T and T Z (two)
+template <bool RES>
+int launch_ns_mm(MmArgs p0, MmArgs p1, int m, double alpha, double beta, double* res_acc, const double* res_prev,
+                 double* res_zero, double tol2, int* nsflag, int cur, const int* active, cudaStream_t st) {
+  const unsigned z = RES ? 1 : 2;
+  if (m <= kWideTileM) {
+    const int g = (m + 31) / 32;
+    ns_mm_kernel<RES><<<dim3(g, g, z), 256, 0, st>>>(p0, p1, m, alpha, beta, res_acc, res_prev, res_zero, tol2,
+                                                      nsflag, cur, active);
+  } else {
+    const int g = (m + kDT - 1) / kDT;
+    ns_dmma_kernel<RES><<<dim3(g, g, z), 128, 0, st>>>(p0, p1, m, alpha, beta, res_acc, res_prev, res_zero, tol2,
+                                                        nsflag, cur, active);
+  }
   MDE_LAUNCH_CHECK();
   return 0;
 }
@@ -332,6 +531,31 @@ int launch_rowmat_wide(const float* X, float* Y, int64_t n, int m, const ProjWs&
   return 0;
 }
 
+// m > 256, in chunks of the rows the fpart region holds (16 m of them, or more; the Gram has been reduced by now):
+// MODE 0 Y = (X - mu) W through fpart and a copy back (Y may be X), MODE 1 Y -= X W (through fpart when Y is X)
+template <int MODE>
+int launch_rowgemm(const float* X, float* Y, int64_t n, int m, const ProjWs& w, const int* active, cudaStream_t st) {
+  const int64_t chunk = wide_fpart_floats(m) / m / 128 * 128;
+  const bool staged = (const float*)Y == X;
+  for (int64_t r0 = 0; r0 < n; r0 += chunk) {
+    const int64_t rows = (n - r0 < chunk) ? n - r0 : chunk;
+    const float* Xc = X + r0 * m;
+    float* Yc = Y + r0 * m;
+    float* O = staged ? w.fpart : Yc;
+    dim3 grid((unsigned)((m + 127) / 128), (unsigned)((rows + 127) / 128));
+    rowgemm_kernel<MODE><<<grid, 256, 0, st>>>(Xc, Yc, O, (int)rows, m, w.mean, w.wf, active);
+    MDE_LAUNCH_CHECK();
+    if (staged) {
+      const int64_t count = rows * m;
+      int nb = (int)((count + 1023) / 1024);
+      if (nb > kNumSMs * 8) nb = kNumSMs * 8;
+      copy_kernel<<<nb, 256, 0, st>>>(w.fpart, Yc, count, active);
+      MDE_LAUNCH_CHECK();
+    }
+  }
+  return 0;
+}
+
 }  // namespace
 
 namespace mde {
@@ -339,7 +563,9 @@ namespace mde {
 int enqueue_project_standardized_wide(float* X, int64_t n, int m, const ProjWs& w, const int* active, cudaStream_t st) {
   if (!proj_wide(m) || !w.fpart) return MDE_E_UNSUPPORTED;
   int rc;
-  if ((rc = enqueue_colmean_wide(X, n, m, w, active, st))) return rc;
+  // above m = 256 the mean is summed around s as well: an fp32 sum of raw columns 1000 standard deviations off-centre
+  // misses mu by ~1e-5 sigma, and A = G_s / n - (mu - s)(mu - s)^T takes that error times |mu - s|
+  if ((rc = enqueue_colmean_wide(X, n, m, w, active, st, m > kWideTileM ? X : nullptr))) return rc;
   if ((rc = launch_gram(X, X, n, m, X, w, active, st))) return rc;
   const int64_t mm = (int64_t)m * m;
   double* Yb[2] = {w.ns, w.ns + mm};
@@ -347,7 +573,6 @@ int enqueue_project_standardized_wide(float* X, int64_t n, int m, const ProjWs& 
   double* T = w.ns + 4 * mm;
   ns_init_kernel<<<1, 1024, 0, st>>>(w.gram, w.mean, w.shift, n, m, Yb[0], Zb[0], w.scal, w.nsflag, w.status, active);
   MDE_LAUNCH_CHECK();
-  const int g = (m + 31) / 32;
   const double tol = 1e-9 * (double)m, tol2 = tol * tol;
   for (int it = 0; it < kWideNsIters; ++it) {
     const int cur = it & 1, nxt = cur ^ 1;
@@ -355,16 +580,14 @@ int enqueue_project_standardized_wide(float* X, int64_t n, int m, const ProjWs& 
     const double* res_prev = it ? w.scal + 1 + (it - 1) % 3 : nullptr;
     double* res_next = w.scal + 1 + (it + 1) % 3;
     MmArgs zy = {Zb[cur], Yb[cur], T}, none = {nullptr, nullptr, nullptr};
-    ns_mm_kernel<true><<<dim3(g, g, 1), 256, 0, st>>>(zy, none, m, -0.5, 1.5, res, res_prev, nullptr, tol2, w.nsflag, cur, active);
-    MDE_LAUNCH_CHECK();
+    if ((rc = launch_ns_mm<true>(zy, none, m, -0.5, 1.5, res, res_prev, nullptr, tol2, w.nsflag, cur, active, st))) return rc;
     MmArgs yt = {Yb[cur], T, Yb[nxt]}, tz = {T, Zb[cur], Zb[nxt]};
-    ns_mm_kernel<false><<<dim3(g, g, 2), 256, 0, st>>>(yt, tz, m, 1.0, 0.0, nullptr, res_prev, res_next, tol2, w.nsflag, cur, active);
-    MDE_LAUNCH_CHECK();
+    if ((rc = launch_ns_mm<false>(yt, tz, m, 1.0, 0.0, nullptr, res_prev, res_next, tol2, w.nsflag, cur, active, st))) return rc;
   }
   ns_finish_kernel<<<(unsigned)((mm + 255) / 256), 256, 0, st>>>(w.ns, mm, w.scal, w.nsflag, kWideNsIters & 1,
                                                                 w.scal + 1 + (kWideNsIters - 1) % 3, tol2, w.wf, w.status, active);
   MDE_LAUNCH_CHECK();
-  return launch_rowmat_wide<0>(X, X, n, m, w, active, st);
+  return m <= kWideTileM ? launch_rowmat_wide<0>(X, X, n, m, w, active, st) : launch_rowgemm<0>(X, X, n, m, w, active, st);
 }
 
 int enqueue_tangent_standardized_wide(const float* X, float* Z, int64_t n, int m, const ProjWs& w,
@@ -375,7 +598,7 @@ int enqueue_tangent_standardized_wide(const float* X, float* Z, int64_t n, int m
   const int64_t mm = (int64_t)m * m;
   tangent_mat_kernel<<<(unsigned)((mm + 255) / 256), 256, 0, st>>>(w.gram, mm, 1.0 / (double)n, w.wf, active);
   MDE_LAUNCH_CHECK();
-  return launch_rowmat_wide<1>(X, Z, n, m, w, active, st);
+  return m <= kWideTileM ? launch_rowmat_wide<1>(X, Z, n, m, w, active, st) : launch_rowgemm<1>(X, Z, n, m, w, active, st);
 }
 
 }  // namespace mde

@@ -1494,7 +1494,6 @@ int solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m, co
                   const mde_external_t* ext, const mde_constraint_part_t* cpart, void* stream) {
   if (!out || !e || !opts || n < 1 || m < 1) return MDE_E_INVALID;
   if (opts->memory_size < 1 || opts->memory_size > kMaxMemory) return MDE_E_UNSUPPORTED;
-  if (opts->constraint == MDE_CONSTRAINT_STANDARDIZED && m > kWideMaxM) return MDE_E_UNSUPPORTED;
   if (opts->constraint < 0 || opts->constraint > MDE_CONSTRAINT_CUSTOM) return MDE_E_INVALID;
   if ((opts->constraint == MDE_CONSTRAINT_CUSTOM) != (cpart != nullptr)) return MDE_E_INVALID;
   if (opts->max_iter < 1) return MDE_E_INVALID;

@@ -1,7 +1,7 @@
 """Host-stepped projected L-BFGS for problems the device-resident solver does not take:
 user-defined constraints (any `Constraint` subclass) unless PYMDE_B200_CONSTRAINT=device|graph|hook
 asks for the device-resident solver (and always on edge-sharded problems), memory_size > 32,
-use_line_search=False or use_cached_loss=False, Standardized with embedding_dim > 256, and Python
+use_line_search=False or use_cached_loss=False, embedding dimensions past the evaluation kernels' caps, and Python
 callables as distortion functions on edge-sharded problems or under PYMDE_B200_EXTERNAL=generic
 (other callables, and opted-in constraints, run on the device-resident solver, pymde_b200/external.py).
 

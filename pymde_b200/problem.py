@@ -315,8 +315,6 @@ class MDE(torch.nn.Module):
         if not constraints.is_builtin(constraint):
             if external.constraint_mode() is None or self.__dict__["_dist"] is not None:
                 return False
-        if isinstance(constraint, constraints._Standardized) and int(self.embedding_dim) > 256:
-            return False
         m = int(self.embedding_dim)
         if (m % 4 == 0 and m > 1024) or (m % 4 != 0 and m > 512):  # mirrors launch_distortion (mde_edges.cu)
             return False

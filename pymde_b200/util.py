@@ -202,13 +202,14 @@ class Workspace(object):
 def proj_standardized(X, demean=False, inplace=False):
     """sqrt(n) * polar factor of X (pymde/util.py:129-171), on the device.
 
-    m <= 32: fused Gram + on-device Jacobi kernels; 32 < m <= 256: tiled Gram, Newton-Schulz inverse square root
-    and row kernel (csrc/mde_project_wide.cu) -- both behind mde_project_standardized.  Larger m: the same Gram /
-    eigen formulation with the m x m eigenproblem handed to cuSOLVER through torch.
+    m <= 32: fused Gram + on-device Jacobi kernels; 32 < m <= 1024: tiled Gram, Newton-Schulz inverse square root
+    and row kernel (csrc/mde_project_wide.cu) -- both behind mde_project_standardized.  m > 1024, or demean=False:
+    the same Gram / eigen formulation with the m x m eigenproblem handed to cuSOLVER through torch.
 
     Raises SolverError when X (de-meaned if asked) is numerically rank deficient: a constant or duplicated column,
-    n <= m with demean, or a Gram too ill conditioned for the device's Newton-Schulz iteration.  X may have been
-    overwritten by then when inplace is set."""
+    n <= m with demean, or, for 32 < m <= 1024, a Gram too ill conditioned for the device's Newton-Schulz iteration
+    (it converges at cond(X_c) = 1e3 and gives up near 1e4).  X may have been overwritten by then when inplace is
+    set."""
     if X.device.type != "cuda":
         raise ValueError("pymde_b200.util.proj_standardized needs a CUDA tensor")
     out = X if inplace else X.detach().clone()
@@ -216,7 +217,7 @@ def proj_standardized(X, demean=False, inplace=False):
         raise ValueError("expected a contiguous float32 tensor")
     n, m = out.shape
     lib = _lib.load()
-    if m <= 256 and demean:
+    if m <= 1024 and demean:
         ws = Workspace.get(out.device, lib.mde_project_ws_bytes(n, m))
         stream = stream_ptr(out.device)
         _lib.check(lib.mde_project_standardized(out.data_ptr(), n, m, ws.data_ptr(), stream))
