@@ -447,6 +447,24 @@ int mde_knn16_approx(const void* X, int dtype, int64_t n, int d, int k, uint64_t
                      float* d2_out, void* ws, size_t ws_bytes, void* stream);
 int mde_knn16_approx_ex(const void* X, int dtype, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out,
                         float* d2_out, void* ws, size_t ws_bytes, void* stream, int* iterations);
+/* The exact dense searches for a range of query rows: rows [row_begin, row_end) of X against all n rows of X (the
+ * row itself excluded), for embedding new rows next to rows already searched.  Row r of idx_out / d2_out (rows x k,
+ * rows = row_end - row_begin) is bit for bit row row_begin + r of mde_knn (k <= 24) or mde_knn_wide (24 < k <= 64)
+ * on the same X and k, ties included; mde_knn16_rows is the same for mde_knn16 / mde_knn16_wide (`dtype` as there).
+ * The cost scales with rows x n, not n^2: the tiles sweep only the query rows, and when those cannot fill the SMs the
+ * candidate sweep is split into S slices (one CTA per query tile and slice; S from the tile counts alone), whose S
+ * lists per row are merged by an exact re-rank and certified against the smallest of their worst kept scores.  The
+ * full searches above are this code with [0, n).  0 <= row_begin < row_end <= n, 1 <= k <= 64, k <= n - 1; an unknown
+ * dtype, a bad argument or a workspace too small or not 1024-byte aligned is MDE_E_INVALID before any CUDA call.
+ * `ws`: 1024-byte aligned device scratch of mde_knn_rows_ws_bytes(n, d, rows, k) or mde_knn16_rows_ws_bytes(n, d,
+ * rows, k) bytes.  Asynchronous on `stream`; *fallback_rows (nullable; when not null the call waits for the stream)
+ * receives the number of query rows searched directly, as for the _ex entries. */
+int mde_knn_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes);
+int mde_knn_rows(const float* X, int64_t n, int d, int64_t row_begin, int64_t row_end, int k, int32_t* idx_out,
+                 float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows);
+int mde_knn16_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes);
+int mde_knn16_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin, int64_t row_end, int k,
+                   int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows);
 /* The same NN-descent search on a sparse data matrix, without densifying it.  Input contract of mde_knn_csr (the
  * device CSR check included: MDE_E_INVALID when malformed); output contract of mde_knn_approx, with the distances of
  * mde_knn_csr / mde_knn_csr_wide: the exact squared distance summed in fp64 and rounded once to fp32, which is also

@@ -16,7 +16,7 @@ from .util import align, all_edges, center, rotate, seed  # noqa: F401
 def __getattr__(name):
     # recipes / preprocessing import scipy & sklearn; load them on first use
     import importlib
-    if name in ("preserve_neighbors", "preserve_distances", "laplacian_embedding", "recipes"):
+    if name in ("preserve_neighbors", "preserve_distances", "laplacian_embedding", "embed_new_points", "recipes"):
         recipes = importlib.import_module(__name__ + ".recipes")
         return recipes if name == "recipes" else getattr(recipes, name)
     if name in ("preprocess", "Graph"):

@@ -159,6 +159,12 @@ SIGNATURES = {
                                  C.c_void_p, C.c_size_t, C.c_void_p]),
     "mde_knn16_long_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                     C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
+    "mde_knn_rows_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
+                               C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
+    "mde_knn16_rows_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn16_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
+                                 C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
     "mde_knn16_approx_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn16_approx": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -216,6 +222,7 @@ DEBUG_SIGNATURES = {
                             C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "mde_dbg_lbfgs_reset": (None, [C.c_void_p]),
     "mde_dbg_lbfgs_cand": (C.c_int, [C.c_void_p]),
+    "mde_dbg_knn_slices": (C.c_int, [C.c_int64, C.c_int64, C.c_int]),
 }
 
 _lib = None

@@ -29,6 +29,11 @@
 // re-ranks all 96 with the arithmetic above.  mde_knn_long (k <= 256) is the same kernel with KK = 288 and candidate
 // tiles of 64 (wgmma.m64n64k16), so that its lists fit in shared memory; knn_long_rerank_kernel re-ranks all 288.
 //
+// mde_knn_rows / mde_knn16_rows search a range of query rows against all n rows with the narrow or wide tiles (every
+// full search is the range [0, n)).  When the query tiles leave SMs idle the candidate tiles are split into S slices
+// (blockIdx.y; S from mde_logic.h::knn_slices), each CTA keeps its own top-KK, knn_merge_rerank_kernel re-ranks the
+// S KK candidates of a row exactly, and the certificate takes the smallest of the S worst kept scores (DESIGN 11.8).
+//
 // 16-bit input (mde_knn16, mde_knn16_wide, mde_knn16_long: IEEE fp16 or bf16, read without an fp32 copy).  The element
 // type T is a template parameter of every kernel above.  The prep copies X into a zero-padded operand of its own type
 // (no lo part) and writes the norms with the arithmetic of the fp32 prep on the upcast values; the tile kernels issue
@@ -50,6 +55,7 @@
 
 #include "mde_common.cuh"
 #include "mde_knn_select.cuh"
+#include "mde_logic.h"
 #include "mde_tma.cuh"
 #include "mde_wgmma.cuh"
 
@@ -93,6 +99,21 @@ constexpr int kWideSmemBytes = kStages * kWideStageBytes<TN> + 1024 /* alignment
 // of 64-wide candidate tiles and a 16.5 KB accumulator (232 256 bytes in all)
 static_assert(kWideSmemBytes<kWideKK, kTileN> <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 static_assert(kWideSmemBytes<kLongKK, kLongTileN> <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
+
+// The query rows of a search, [lo, hi) of X, and the candidate slice of a CTA (mde_knn_rows).  CTA (x, y) takes the
+// query rows base + x TM .. + TM - 1 (base: lo rounded down to 128, so that every query box lies inside the padded
+// operand) against the candidate tiles [slice_begin(T), slice_begin(T, 1)) of the T tiles, and keeps the list of
+// query row r at list(r) = (r - lo) slices + y: the S lists of a row are adjacent.  A full search is [0, n) in one slice.
+struct QueryRange {
+  int64_t base, lo, hi;
+  int slices;
+  __device__ __forceinline__ bool has(int64_t r) const { return r >= lo && r < hi; }
+  __device__ __forceinline__ int64_t list(int64_t r) const { return (r - lo) * slices + blockIdx.y; }
+  __device__ __forceinline__ int slice_begin(int tiles, int next = 0) const {
+    return (int)((int64_t)tiles * (blockIdx.y + next) / slices);
+  }
+};
+constexpr int kMaxSlices = 16;  // S <= 16: the merge keeps a row's S KK <= 1536 candidates in 12 KB of shared memory
 
 // ---------------------------------------------------------------------------------------------------------------
 // PTX wrappers (tensor TMA); mbarriers come from mde_tma.cuh, wgmma from mde_wgmma.cuh
@@ -317,8 +338,8 @@ __device__ __forceinline__ void keep_candidate(float (&bd)[kKK], int (&bi)[kKK],
 template <class T>
 __global__ void __launch_bounds__(kThreads, 1)
 knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_l,
-                const float* __restrict__ norms, int64_t n, int64_t n_pad, int k_pad, int32_t* __restrict__ cand_idx,
-                float* __restrict__ cand_val) {
+                const float* __restrict__ norms, int64_t n, int64_t n_pad, int k_pad, QueryRange qr,
+                int32_t* __restrict__ cand_idx, float* __restrict__ cand_val) {
   extern __shared__ uint8_t smem_raw[];
   // carve: [stages x 64 KB, 1024-aligned] | staged accumulators [128][kAccStride] | norms[2][128] | barriers
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -332,7 +353,8 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_kb = k_pad / kBlockK;
   const int num_tiles = (int)(n_pad / kTileN);
-  const int row0 = blockIdx.x * kTileM;
+  const int t_begin = qr.slice_begin(num_tiles), t_end = qr.slice_begin(num_tiles, 1);
+  const int row0 = (int)qr.base + blockIdx.x * kTileM;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kStages; ++s) { mbar_init(bar0 + 8 * s, 1); mbar_init(bar0 + 16 + 8 * s, kConsumerWarps); }
@@ -344,7 +366,7 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
     // ===== TMA producer =====
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
-      for (int t = 0; t < num_tiles; ++t) {
+      for (int t = t_begin; t < t_end; ++t) {
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(bar0 + 16 + 8 * stage, phase ^ 1);  // slot released by the consumers
           const uint32_t full = bar0 + 8 * stage;
@@ -383,7 +405,7 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
   for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
 
   int stage = 0; uint32_t phase = 0;
-  for (int t = 0; t < num_tiles; ++t) {
+  for (int t = t_begin; t < t_end; ++t) {
     for (int kb = 0; kb < num_kb; ++kb) {
       mbar_wait(bar0 + 8 * stage, phase);  // operands landed
       const uint32_t sa = base + stage * kStageBytes;
@@ -439,11 +461,12 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
       const float dist = xd[q];
       if (dist < thr) keep_candidate(bd, bi, dist, xi[q], thr, worst);
     }
-    if (row < n) {
+    if (qr.has(row)) {
+      const int64_t o = qr.list(row) * kKK;
 #pragma unroll
       for (int q = 0; q < kKK; ++q) {
-        cand_idx[(int64_t)row * kKK + q] = bi[q];
-        cand_val[(int64_t)row * kKK + q] = bd[q];
+        cand_idx[o + q] = bi[q];
+        cand_val[o + q] = bd[q];
       }
     }
   }
@@ -502,7 +525,7 @@ template <class T, int KK, int TN>
 __global__ void __launch_bounds__(kWideThreads, 1)
 knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant__ CUtensorMap map_al,
                      const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_l,
-                     const float* __restrict__ norms, int64_t n, int64_t n_pad, int k_pad,
+                     const float* __restrict__ norms, int64_t n, int64_t n_pad, int k_pad, QueryRange qr,
                      int32_t* __restrict__ cand_idx, float* __restrict__ cand_val) {
   static_assert(TN == 64 || TN == 128, "wgmma.m64n64k16 or m64n128k16");
   constexpr int kBOpBytes = TN * kRowBytes;
@@ -525,7 +548,8 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_kb = k_pad / kBlockK;
   const int num_tiles = (int)(n_pad / TN);
-  const int row0 = blockIdx.x * kWideTileM;
+  const int t_begin = qr.slice_begin(num_tiles), t_end = qr.slice_begin(num_tiles, 1);
+  const int row0 = (int)qr.base + blockIdx.x * kWideTileM;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kStages; ++s) { mbar_init(bar0 + 8 * s, 1); mbar_init(bar0 + 16 + 8 * s, kWideConsumerWarps); }
@@ -537,7 +561,7 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
     // ===== TMA producer =====
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
-      for (int t = 0; t < num_tiles; ++t) {
+      for (int t = t_begin; t < t_end; ++t) {
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(bar0 + 16 + 8 * stage, phase ^ 1);  // slot released by the consumers
           const uint32_t full = bar0 + 8 * stage;
@@ -566,7 +590,7 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
   for (int i = 0; i < TN / 2; ++i) acc[i] = 0.0f;
 
   int stage = 0; uint32_t phase = 0;
-  for (int t = 0; t < num_tiles; ++t) {
+  for (int t = t_begin; t < t_end; ++t) {
     for (int kb = 0; kb < num_kb; ++kb) {
       mbar_wait(bar0 + 8 * stage, phase);  // operands landed
       const uint32_t sa = base + stage * kStageB;
@@ -608,7 +632,7 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
       if (col + 1 != row && col + 1 < n) list.offer(fmaf(-2.0f, a.y, s.y), col + 1);
     }
   }
-  if (row < n) list.store(cand_idx + (int64_t)row * KK, cand_val + (int64_t)row * KK);
+  if (qr.has(row)) list.store(cand_idx + qr.list(row) * KK, cand_val + qr.list(row) * KK);
 }
 
 }  // namespace
@@ -703,10 +727,65 @@ template int knn_dense_rerank<__nv_bfloat16>(int, const __nv_bfloat16*, int64_t,
 namespace {
 
 // ---------------------------------------------------------------------------------------------------------------
+// merge: the re-rank of a row searched in S candidate slices (or of a query range that does not start at row 0).
+// One warp per query row r (global row lo + r) computes the exact fp32 distances of its S KK candidates with the
+// re-rank's arithmetic (the same bits), stages them in shared memory and writes the k smallest (distance, index)
+// pairs, ascending, to row r of the compact output; missing candidates (-1) order last, as in the re-rank.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int kMergeWarps = 4;
+
+template <class T>
+__global__ void __launch_bounds__(kMergeWarps * 32)
+knn_merge_rerank_kernel(const T* __restrict__ X, int d, int64_t lo, int64_t rows,
+                        const int32_t* __restrict__ cand_idx, int cands, int k, int32_t* __restrict__ out_idx,
+                        float* __restrict__ out_d2) {
+  extern __shared__ float s_merge[];  // per warp: distances [cands], indices [cands]
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t r = (int64_t)blockIdx.x * kMergeWarps + warp;
+  if (r >= rows) return;
+  float* sd = s_merge + (size_t)warp * 2 * cands;
+  unsigned* si = reinterpret_cast<unsigned*>(sd + cands);
+  const T* xq = X + (lo + r) * d;
+  for (int b = 0; b < cands; b += 32) {
+    const int mine = cand_idx[r * cands + b + lane];
+    float my_d = __int_as_float(0x7f800000);
+    for (int q = 0; q < 32; ++q) {
+      const int c = __shfl_sync(kFull, mine, q);
+      if (c < 0) continue;  // (warp-uniform)
+      const T* xc = X + (int64_t)c * d;
+      float acc = 0.0f;
+      for (int j = lane; j < d; j += 32) { const float t = elem_f32(xq[j]) - elem_f32(xc[j]); acc = fmaf(t, t, acc); }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
+      if (lane == q) my_d = acc;
+    }
+    sd[b + lane] = my_d;
+    si[b + lane] = (unsigned)mine;
+  }
+  __syncwarp();
+  // rank of each candidate among the S KK: ties broken by index (slices hold disjoint rows), missing candidates last
+  for (int j = lane; j < cands; j += 32) {
+    const float dj = sd[j];
+    const unsigned ij = si[j];
+    int rank = 0;
+    for (int q = 0; q < cands; ++q) rank += (sd[q] < dj || (sd[q] == dj && si[q] < ij));
+    if (rank < k) {
+      out_idx[r * k + rank] = (int32_t)ij;
+      out_d2[r * k + rank] = dj;
+    }
+  }
+}
+
+}  // namespace
+
+namespace {
+
+// ---------------------------------------------------------------------------------------------------------------
 // certificate: is the re-ranked list of a row the k smallest (distance, index) over ALL rows?
 //
 // Every row the tiles did not keep scored at least t, the worst kept score (+inf when the list was never filled:
-// every row was kept).  With the bound E(q) above (cert_bound), a row that was not kept lies at an exact distance of at
+// every row was kept); a row searched in S candidate slices takes the smallest of the S slices' worst kept scores,
+// since every row a slice did not keep scored at least that slice's worst.  With the bound E(q) above (cert_bound), a row that was not kept lies at an exact distance of at
 // least t - E(q) + ||q^||^2 - E(q); when that exceeds d2_k (1 + delta) / (1 - delta), where d2_k is the k-th
 // re-ranked fp32 distance and delta bounds the re-rank's relative rounding, its fp32 distance exceeds d2_k and it
 // cannot enter the list.  A row that fails is searched directly (knn_direct_kernel); a false failure costs time
@@ -714,29 +793,34 @@ namespace {
 // counted in the header.
 // ---------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-knn_certify_kernel(const float* __restrict__ cand_val, int kk, const float* __restrict__ norms,
-                   const float* __restrict__ d2_out, int k, int64_t n, CertBound b, unsigned* __restrict__ hdr,
-                   int32_t* __restrict__ rows) {
+knn_certify_kernel(const float* __restrict__ cand_val, int kk, int slices, const float* __restrict__ norms,
+                   const float* __restrict__ d2_out, int k, int64_t lo, int64_t n, CertBound b,
+                   unsigned* __restrict__ hdr, int32_t* __restrict__ rows) {
   const int lane = threadIdx.x & 31;
-  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);  // of the query range
   if (row >= n) return;
-  float t = -__int_as_float(0x7f800000);
-  for (int q = lane; q < kk; q += 32) t = fmaxf(t, cand_val[row * kk + q]);
+  const float* cv = cand_val + row * slices * kk;
+  float t = __int_as_float(0x7f800000);
+  for (int s = 0; s < slices; ++s, cv += kk) {
+    float ts = -__int_as_float(0x7f800000);
+    for (int q = lane; q < kk; q += 32) ts = fmaxf(ts, cv[q]);
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) t = fmaxf(t, __shfl_xor_sync(kFull, t, o));
+    for (int o = 16; o > 0; o >>= 1) ts = fmaxf(ts, __shfl_xor_sync(kFull, ts, o));
+    t = fminf(t, ts);
+  }
   if (lane) return;
   const bool centred = hdr[kHdrCentred] != 0;
   const double a_cross = centred ? b.a_cen : b.a_unc, eta = centred ? b.eta : 0.0;
   const double M2 = (double)__uint_as_float(hdr[kHdrMaxNorm]), M = sqrt(M2);
-  const double qn = (double)norms[row], qa = sqrt(qn);
+  const double qn = (double)norms[lo + row], qa = sqrt(qn);
   const double E = kCertSafety * (2.0 * (a_cross * qa * M + eta * (qa + M)) + b.a_norm * M2 + b.a_abs);
   const double lhs = (double)d2_out[row * k + k - 1] * (1.0 + b.delta) / (1.0 - b.delta) - qn + E;
   if (!(lhs < (double)t - E)) rows[atomicAdd(reinterpret_cast<int*>(hdr + kHdrCount), 1)] = (int32_t)row;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// direct search of the uncertified rows: one warp per row sweeps all n rows with the re-rank's arithmetic (the same
-// fp32 bits) and keeps the k smallest (distance, index) pairs, ascending.  Only pairs up to the re-rank's k-th pair
+// direct search of the uncertified rows (row r of the query range is row lo + r of X): one warp per row sweeps all n
+// rows with the re-rank's arithmetic (the same fp32 bits) and keeps the k smallest (distance, index) pairs, ascending.  Only pairs up to the re-rank's k-th pair
 // can belong (the re-rank's k rows are k candidates with these very distances), which keeps insertions rare.
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ bool pair_before(float d1, unsigned i1, float d2, unsigned i2) {
@@ -745,7 +829,7 @@ __device__ __forceinline__ bool pair_before(float d1, unsigned i1, float d2, uns
 
 template <class T>
 __global__ void __launch_bounds__(256)
-knn_direct_kernel(const T* __restrict__ X, int64_t n, int d, int k, const unsigned* __restrict__ hdr,
+knn_direct_kernel(const T* __restrict__ X, int64_t n, int d, int k, int64_t lo, const unsigned* __restrict__ hdr,
                   const int32_t* __restrict__ rows, int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
   __shared__ float s_d[8][kLongMaxK];
   __shared__ unsigned s_i[8][kLongMaxK];
@@ -762,9 +846,9 @@ knn_direct_kernel(const T* __restrict__ X, int64_t n, int d, int k, const unsign
   float thr = __int_as_float(0x7f800000);
   unsigned thi = 0xffffffffu;
   int worst = 0;
-  const T* xq = X + row * d;
+  const T* xq = X + (lo + row) * d;
   for (int64_t c = 0; c < n; ++c) {
-    if (c == row) continue;
+    if (c == lo + row) continue;
     const T* xc = X + c * d;
     float acc = 0.0f;
     for (int j = lane; j < d; j += 32) { const float t = elem_f32(xq[j]) - elem_f32(xc[j]); acc = fmaf(t, t, acc); }
@@ -839,29 +923,51 @@ int make_map(EncodeTiledFn enc, CUtensorMap* map, void* ptr, int64_t n_pad, int 
 }
 
 struct KnnLayout {
-  int64_t n_pad; int k_pad, chunks;
+  int64_t n_pad; int k_pad, chunks, slices;
   size_t off_h, off_l, off_norm, off_ci, off_cv, off_mu, off_part, off_hdr, off_rows, total;
 };
 
-// kk: candidates kept per row (kKK, kWideKK for the wide search, kLongKK for the long one); split: fp32 input, whose
-// operand has a lo part (16-bit input has none: off_l == off_h, 2 n_pad k_pad bytes fewer)
-KnnLayout knn_layout(int64_t n, int d, int kk = kKK, bool split = true) {
+// The tile shape of a search: tm query rows per CTA, tn candidates per tile, kk candidates kept per row (kKK, kWideKK
+// for the wide search, kLongKK for the long one).
+struct Shape { int tm, tn, kk; };
+constexpr Shape kNarrow{kTileM, kTileN, kKK}, kWide{kWideTileM, kTileN, kWideKK}, kLong{kWideTileM, kLongTileN, kLongKK};
+
+// Candidate slices of a search of `rows` query rows against the n rows of X (mde_logic.h: knn_slices).  The long
+// search keeps one: the merge of its 288-candidate lists would not fit in shared memory.
+int search_slices(int64_t n, int64_t rows, Shape sh) {
+  if (sh.kk == kLongKK) return 1;
+  const int64_t n_pad = (n + kTileN - 1) / kTileN * kTileN;
+  return knn_slices((rows + sh.tm - 1) / sh.tm, n_pad / sh.tn, kNumSMs, kMaxSlices);
+}
+
+// rows: query rows of the search (n for a full one), each with one list of sh.kk candidates per slice; split: fp32
+// input, whose operand has a lo part (16-bit input has none: off_l == off_h, 2 n_pad k_pad bytes fewer)
+KnnLayout knn_layout(int64_t n, int d, int64_t rows, Shape sh, bool split) {
   KnnLayout L;
   L.n_pad = (n + kTileN - 1) / kTileN * kTileN;
   L.k_pad = (d + kBlockK - 1) / kBlockK * kBlockK;
   L.chunks = (int)((n + kMeanChunk - 1) / kMeanChunk);
+  L.slices = search_slices(n, rows, sh);
+  // room for the lists of rows x S query rows: rows itself, or, when the rule may split, the most a split can hold
+  // (q_tiles S <= kNumSMs, S <= kMaxSlices).  Monotone in rows: a workspace sized for a search fits every smaller one.
+  int64_t cap = rows;
+  if (sh.kk != kLongKK) {
+    const int64_t split = rows * kMaxSlices < (int64_t)kNumSMs * sh.tm ? rows * kMaxSlices : (int64_t)kNumSMs * sh.tm;
+    if (split > cap) cap = split;
+  }
+  const size_t lists = (size_t)cap * sh.kk;
   auto up = [](size_t x) { return (x + 1023) / 1024 * 1024; };
   size_t o = 0;
   L.off_h = o; o = up(o + (size_t)L.n_pad * L.k_pad * 2);
   L.off_l = split ? o : L.off_h;
   if (split) o = up(o + (size_t)L.n_pad * L.k_pad * 2);
   L.off_norm = o; o = up(o + (size_t)L.n_pad * 4);
-  L.off_ci = o; o = up(o + (size_t)n * kk * 4);
-  L.off_cv = o; o = up(o + (size_t)n * kk * 4);
+  L.off_ci = o; o = up(o + lists * 4);
+  L.off_cv = o; o = up(o + lists * 4);
   L.off_mu = o; o = up(o + (size_t)d * 4);                   // column mean
   L.off_part = o; o = up(o + (size_t)L.chunks * d * 8);      // its per-chunk fp64 sums
   L.off_hdr = o; o = up(o + 4 * kHdrWords);                  // the search header (kHdr*)
-  L.off_rows = o; o = up(o + (size_t)n * 4);                 // the uncertified rows
+  L.off_rows = o; o = up(o + (size_t)rows * 4);              // the uncertified rows
   L.total = o;
   return L;
 }
@@ -887,22 +993,31 @@ int centre_and_prep(const T* X, int64_t n, int d, const KnnLayout& L, uint8_t* w
   return 0;
 }
 
-// After the tiles: re-rank the KK candidates of every row, certify every row, search the uncertified rows directly;
-// with `fallback_rows`, wait for the stream and report how many rows that was.
+// After the tiles: re-rank the candidates of every query row (rows lo .. hi - 1 of X; the S KK of a sliced search
+// are merged), certify every row, search the uncertified rows directly; with `fallback_rows`, wait for the stream
+// and report how many rows that was.  Outputs are compact: row r holds row lo + r of X.
 template <class T>
-int rerank_certify(int kk, const T* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, const KnnLayout& L,
-                   uint8_t* w, cudaStream_t st, int* fallback_rows) {
+int rerank_certify(int kk, const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int32_t* idx_out,
+                   float* d2_out, const KnnLayout& L, uint8_t* w, cudaStream_t st, int* fallback_rows) {
+  const int64_t rows = hi - lo;
+  const int32_t* ci = reinterpret_cast<const int32_t*>(w + L.off_ci);
   int rc;
-  if ((rc = knn_dense_rerank<T>(kk, X, n, d, reinterpret_cast<const int32_t*>(w + L.off_ci), k, idx_out, d2_out, st)))
-    return rc;
+  if (L.slices == 1 && lo == 0) {
+    if ((rc = knn_dense_rerank<T>(kk, X, rows, d, ci, k, idx_out, d2_out, st))) return rc;
+  } else {
+    const int cands = L.slices * kk;
+    knn_merge_rerank_kernel<T><<<(unsigned)((rows + kMergeWarps - 1) / kMergeWarps), kMergeWarps * 32,
+                                 (size_t)kMergeWarps * cands * 8, st>>>(X, d, lo, rows, ci, cands, k, idx_out, d2_out);
+    MDE_LAUNCH_CHECK();
+  }
   unsigned* hdr = reinterpret_cast<unsigned*>(w + L.off_hdr);
-  int32_t* rows = reinterpret_cast<int32_t*>(w + L.off_rows);
-  const unsigned grid = (unsigned)((n + 7) / 8);
-  knn_certify_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const float*>(w + L.off_cv), kk,
-                                           reinterpret_cast<const float*>(w + L.off_norm), d2_out, k, n,
-                                           cert_bound<T>(d, L.k_pad), hdr, rows);
+  int32_t* uncert = reinterpret_cast<int32_t*>(w + L.off_rows);
+  const unsigned grid = (unsigned)((rows + 7) / 8);
+  knn_certify_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const float*>(w + L.off_cv), kk, L.slices,
+                                           reinterpret_cast<const float*>(w + L.off_norm), d2_out, k, lo, rows,
+                                           cert_bound<T>(d, L.k_pad), hdr, uncert);
   MDE_LAUNCH_CHECK();
-  knn_direct_kernel<T><<<grid, 256, 0, st>>>(X, n, d, k, hdr, rows, idx_out, d2_out);
+  knn_direct_kernel<T><<<grid, 256, 0, st>>>(X, n, d, k, lo, hdr, uncert, idx_out, d2_out);
   MDE_LAUNCH_CHECK();
   if (fallback_rows) {
     MDE_CUDA_TRY(cudaMemcpyAsync(fallback_rows, hdr + kHdrCount, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -911,13 +1026,21 @@ int rerank_certify(int kk, const T* X, int64_t n, int d, int k, int32_t* idx_out
   return 0;
 }
 
-// mde_knn / mde_knn16: centring and prep, tiles, re-rank of the 32 candidates, certificate and direct search.
+// Arguments shared by every dense exact search: the query rows [lo, hi) of X (a full search is [0, n)).
+bool bad_search_args(const void* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int max_k, const void* idx_out,
+                     const void* d2_out, const void* ws) {
+  return !X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > max_k || k > n - 1 || lo < 0 ||
+         hi > n || lo >= hi;
+}
+
+// mde_knn / mde_knn16 / the narrow mde_knn_rows: centring and prep, tiles (in S candidate slices), re-rank of the 32
+// candidates (merge of the 32 S), certificate and direct search.
 template <class T>
-int run_narrow(const T* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
-               void* stream, int* fallback_rows) {
-  if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > kMaxK || k > n - 1) return MDE_E_INVALID;
+int run_narrow(const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int32_t* idx_out, float* d2_out, void* ws,
+               size_t ws_bytes, void* stream, int* fallback_rows) {
+  if (bad_search_args(X, n, d, lo, hi, k, kMaxK, idx_out, d2_out, ws)) return MDE_E_INVALID;
   if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
-  const KnnLayout L = knn_layout(n, d, kKK, Operand<T>::kSplit);
+  const KnnLayout L = knn_layout(n, d, hi - lo, kNarrow, Operand<T>::kSplit);
   if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   EncodeTiledFn enc = nullptr;
@@ -938,20 +1061,22 @@ int run_narrow(const T* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_
     MDE_CUDA_TRY(cudaFuncSetAttribute(knn_tile_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
     attr_set = true;
   }
-  const unsigned grid = (unsigned)((n + kTileM - 1) / kTileM);
-  knn_tile_kernel<T><<<grid, kThreads, kSmemBytes, st>>>(mh, ml, norms, n, L.n_pad, L.k_pad, ci, cv);
+  const QueryRange qr{lo / kTileN * kTileN, lo, hi, L.slices};
+  const dim3 grid((unsigned)((hi - qr.base + kTileM - 1) / kTileM), (unsigned)L.slices);
+  knn_tile_kernel<T><<<grid, kThreads, kSmemBytes, st>>>(mh, ml, norms, n, L.n_pad, L.k_pad, qr, ci, cv);
   MDE_LAUNCH_CHECK();
-  return rerank_certify<T>(kKK, X, n, d, k, idx_out, d2_out, L, w, st, fallback_rows);
+  return rerank_certify<T>(kKK, X, n, d, lo, hi, k, idx_out, d2_out, L, w, st, fallback_rows);
 }
 
-// mde_knn_wide (KK = 96, TN = 128) and mde_knn_long (KK = 288, TN = 64), and their 16-bit entries: centring and
-// prep, tiles, re-rank of all KK candidates, certificate and direct search.
+// mde_knn_wide (KK = 96, TN = 128) and mde_knn_long (KK = 288, TN = 64), their 16-bit entries and the wide
+// mde_knn_rows: centring and prep, tiles (in S candidate slices), re-rank of all KK candidates (merge of the KK S),
+// certificate and direct search.
 template <class T, int KK, int TN>
-int run_wide(const T* X, int64_t n, int d, int k, int max_k, int32_t* idx_out, float* d2_out, void* ws,
-             size_t ws_bytes, void* stream, int* fallback_rows) {
-  if (!X || !idx_out || !d2_out || !ws || n < 2 || d < 1 || k < 1 || k > max_k || k > n - 1) return MDE_E_INVALID;
+int run_wide(const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int max_k, int32_t* idx_out, float* d2_out,
+             void* ws, size_t ws_bytes, void* stream, int* fallback_rows) {
+  if (bad_search_args(X, n, d, lo, hi, k, max_k, idx_out, d2_out, ws)) return MDE_E_INVALID;
   if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
-  const KnnLayout L = knn_layout(n, d, KK, Operand<T>::kSplit);
+  const KnnLayout L = knn_layout(n, d, hi - lo, Shape{kWideTileM, TN, KK}, Operand<T>::kSplit);
   if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   EncodeTiledFn enc = nullptr;
@@ -977,11 +1102,12 @@ int run_wide(const T* X, int64_t n, int d, int k, int max_k, int32_t* idx_out, f
                                       kSmem));
     attr_set = true;
   }
-  const unsigned grid = (unsigned)((n + kWideTileM - 1) / kWideTileM);
-  knn_wide_tile_kernel<T, KK, TN><<<grid, kWideThreads, kSmem, st>>>(mah, mal, mh, ml, norms, n, L.n_pad, L.k_pad, ci,
-                                                                     cv);
+  const QueryRange qr{lo / kTileN * kTileN, lo, hi, L.slices};
+  const dim3 grid((unsigned)((hi - qr.base + kWideTileM - 1) / kWideTileM), (unsigned)L.slices);
+  knn_wide_tile_kernel<T, KK, TN><<<grid, kWideThreads, kSmem, st>>>(mah, mal, mh, ml, norms, n, L.n_pad, L.k_pad, qr,
+                                                                     ci, cv);
   MDE_LAUNCH_CHECK();
-  return rerank_certify<T>(KK, X, n, d, k, idx_out, d2_out, L, w, st, fallback_rows);
+  return rerank_certify<T>(KK, X, n, d, lo, hi, k, idx_out, d2_out, L, w, st, fallback_rows);
 }
 
 // The 16-bit entries: dtype code -> element type, MDE_E_INVALID for an unknown code (before any CUDA call).
@@ -994,25 +1120,40 @@ int by_dtype(const void* X, int dtype, A... args) {
 template <class T>
 struct Narrow {
   static int call(const T* X, int64_t n, int d, int k, int32_t* i, float* d2, void* ws, size_t b, void* st, int* fb) {
-    return run_narrow<T>(X, n, d, k, i, d2, ws, b, st, fb);
+    return run_narrow<T>(X, n, d, 0, n, k, i, d2, ws, b, st, fb);
   }
 };
 template <class T>
 struct Wide {
   static int call(const T* X, int64_t n, int d, int k, int32_t* i, float* d2, void* ws, size_t b, void* st, int* fb) {
-    return run_wide<T, kWideKK, kTileN>(X, n, d, k, kWideMaxK, i, d2, ws, b, st, fb);
+    return run_wide<T, kWideKK, kTileN>(X, n, d, 0, n, k, kWideMaxK, i, d2, ws, b, st, fb);
   }
 };
 template <class T>
 struct Long {
   static int call(const T* X, int64_t n, int d, int k, int32_t* i, float* d2, void* ws, size_t b, void* st, int* fb) {
-    return run_wide<T, kLongKK, kLongTileN>(X, n, d, k, kLongMaxK, i, d2, ws, b, st, fb);
+    return run_wide<T, kLongKK, kLongTileN>(X, n, d, 0, n, k, kLongMaxK, i, d2, ws, b, st, fb);
+  }
+};
+// mde_knn_rows / mde_knn16_rows: the narrow search for k <= 24, the wide one up to 64
+template <class T>
+struct Rows {
+  static int call(const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int32_t* i, float* d2, void* ws,
+                  size_t b, void* st, int* fb) {
+    if (k > kMaxK) return run_wide<T, kWideKK, kTileN>(X, n, d, lo, hi, k, kWideMaxK, i, d2, ws, b, st, fb);
+    return run_narrow<T>(X, n, d, lo, hi, k, i, d2, ws, b, st, fb);
   }
 };
 
-int layout_bytes(int64_t n, int d, int kk, bool split, size_t* bytes) {
+int layout_bytes(int64_t n, int d, Shape sh, bool split, size_t* bytes) {
   if (!bytes || n < 2 || d < 1) return MDE_E_INVALID;
-  *bytes = knn_layout(n, d, kk, split).total;
+  *bytes = knn_layout(n, d, n, sh, split).total;
+  return 0;
+}
+
+int rows_layout_bytes(int64_t n, int d, int64_t rows, int k, bool split, size_t* bytes) {
+  if (!bytes || n < 2 || d < 1 || rows < 1 || rows > n || k < 1 || k > kWideMaxK || k > n - 1) return MDE_E_INVALID;
+  *bytes = knn_layout(n, d, rows, k > kMaxK ? kWide : kNarrow, split).total;
   return 0;
 }
 
@@ -1022,11 +1163,11 @@ extern "C" {
 
 int mde_knn_max_k(void) { return kMaxK; }
 
-int mde_knn_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kKK, true, bytes); }
+int mde_knn_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kNarrow, true, bytes); }
 
 int mde_knn_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
                void* stream, int* fallback_rows) {
-  return run_narrow<float>(X, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
+  return run_narrow<float>(X, n, d, 0, n, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
 }
 
 int mde_knn(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
@@ -1036,11 +1177,11 @@ int mde_knn(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2
 
 int mde_knn_wide_max_k(void) { return kWideMaxK; }
 
-int mde_knn_wide_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kWideKK, true, bytes); }
+int mde_knn_wide_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kWide, true, bytes); }
 
 int mde_knn_wide_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                     size_t ws_bytes, void* stream, int* fallback_rows) {
-  return run_wide<float, kWideKK, kTileN>(X, n, d, k, kWideMaxK, idx_out, d2_out, ws, ws_bytes, stream,
+  return run_wide<float, kWideKK, kTileN>(X, n, d, 0, n, k, kWideMaxK, idx_out, d2_out, ws, ws_bytes, stream,
                                           fallback_rows);
 }
 
@@ -1051,11 +1192,11 @@ int mde_knn_wide(const float* X, int64_t n, int d, int k, int32_t* idx_out, floa
 
 int mde_knn_long_max_k(void) { return kLongMaxK; }
 
-int mde_knn_long_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kLongKK, true, bytes); }
+int mde_knn_long_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kLong, true, bytes); }
 
 int mde_knn_long_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                     size_t ws_bytes, void* stream, int* fallback_rows) {
-  return run_wide<float, kLongKK, kLongTileN>(X, n, d, k, kLongMaxK, idx_out, d2_out, ws, ws_bytes, stream,
+  return run_wide<float, kLongKK, kLongTileN>(X, n, d, 0, n, k, kLongMaxK, idx_out, d2_out, ws, ws_bytes, stream,
                                               fallback_rows);
 }
 
@@ -1064,7 +1205,16 @@ int mde_knn_long(const float* X, int64_t n, int d, int k, int32_t* idx_out, floa
   return mde_knn_long_ex(X, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
-int mde_knn16_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kKK, false, bytes); }
+int mde_knn_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes) {
+  return rows_layout_bytes(n, d, rows, k, true, bytes);
+}
+
+int mde_knn_rows(const float* X, int64_t n, int d, int64_t row_begin, int64_t row_end, int k, int32_t* idx_out,
+                 float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows) {
+  return Rows<float>::call(X, n, d, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
+}
+
+int mde_knn16_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kNarrow, false, bytes); }
 
 int mde_knn16_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                  size_t ws_bytes, void* stream, int* fallback_rows) {
@@ -1076,7 +1226,7 @@ int mde_knn16(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_ou
   return mde_knn16_ex(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
-int mde_knn16_wide_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kWideKK, false, bytes); }
+int mde_knn16_wide_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kWide, false, bytes); }
 
 int mde_knn16_wide_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                       size_t ws_bytes, void* stream, int* fallback_rows) {
@@ -1088,7 +1238,7 @@ int mde_knn16_wide(const void* X, int dtype, int64_t n, int d, int k, int32_t* i
   return mde_knn16_wide_ex(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
-int mde_knn16_long_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kLongKK, false, bytes); }
+int mde_knn16_long_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kLong, false, bytes); }
 
 int mde_knn16_long_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                       size_t ws_bytes, void* stream, int* fallback_rows) {
@@ -1098,6 +1248,22 @@ int mde_knn16_long_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t
 int mde_knn16_long(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                    size_t ws_bytes, void* stream) {
   return mde_knn16_long_ex(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
+}
+
+int mde_knn16_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes) {
+  return rows_layout_bytes(n, d, rows, k, false, bytes);
+}
+
+int mde_knn16_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin, int64_t row_end, int k,
+                   int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows) {
+  return by_dtype<Rows>(X, dtype, n, d, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
+}
+
+// host-side debug entry point: the candidate slices (mde_logic.h: knn_slices) of a search of `rows` query rows
+// against n rows with k neighbours (the narrow search up to k = 24, the wide one up to 64); -1 for bad arguments
+int mde_dbg_knn_slices(int64_t n, int64_t rows, int k) {
+  if (n < 2 || rows < 1 || rows > n || k < 1 || k > kWideMaxK) return -1;
+  return search_slices(n, rows, k > kMaxK ? kWide : kNarrow);
 }
 
 }  // extern "C"

@@ -319,4 +319,19 @@ MDE_HD inline void lbfgs_direction(LbfgsState& B, double (*SY)[kMaxMemory], doub
   for (int j = 0; j < h; ++j) { B.cs[j] = cc[j]; B.cy[j] = -B.H_diag * al[j]; }
 }
 
+// ---------------------------------------------------------------------------------------
+// exact k-nearest-neighbour search (mde_knn.cu): candidate slices
+// ---------------------------------------------------------------------------------------
+// One CTA per (query tile, candidate slice), one CTA per SM.  When the q_tiles query tiles leave SMs idle, the sweep
+// over the c_tiles candidate tiles is split into S slices: as many as keep q_tiles S within one wave of num_sms CTAs,
+// at most one candidate tile per slice and at most max_slices (the merge re-ranks S times the candidates).  S = 1
+// once the query tiles fill the SMs.
+MDE_HD inline int knn_slices(int64_t q_tiles, int64_t c_tiles, int num_sms, int max_slices) {
+  if (q_tiles < 1 || q_tiles >= num_sms) return 1;
+  int64_t s = num_sms / q_tiles;
+  if (s > c_tiles) s = c_tiles;
+  if (s > max_slices) s = max_slices;
+  return s < 1 ? 1 : (int)s;
+}
+
 }  // namespace mde

@@ -25,7 +25,11 @@ The dense exact searches are exact on data far from the origin and on far-apart 
 columns when that bounds the score error more tightly (a 16-bit matrix near the origin stays its own exact operand)
 and certify every row, searching the rows that fail directly (DESIGN section 11), and the GEMM path scores
 candidates with fp64 matmuls of the centred matrix, independent of torch's TF32 setting, then re-ranks them by fp32
-distance and index."""
+distance and index.
+
+`knn_rows_device` searches only a range of rows against all rows (`mde_knn_rows`, `mde_knn16_rows`), exactly, at a
+cost that scales with the rows searched: `pymde_b200.embed_new_points` searches the new rows of a stacked matrix with
+it (DESIGN section 11.8)."""
 import ctypes as C
 import os
 
@@ -180,6 +184,53 @@ def knn_device(X, k):
     return idx, d2
 
 
+def knn_rows_device(X, k, row_begin, row_end):
+    """(indices [r, k], squared distances [r, k] fp32), r = row_end - row_begin: row r of the result is row
+    row_begin + r of the exact search of X (its k nearest rows among all n rows of X, itself excluded, ascending by
+    (distance, index)).  Always exact: PYMDE_B200_KNN does not apply.  Routes:
+      * a CUDA fp32 / float16 / bfloat16 matrix with k <= 64: `mde_knn_rows` / `mde_knn16_rows` (int32 indices), bit
+        for bit the rows of `knn_device`, at a cost of about r n d rather than n^2 d (other float dtypes are searched
+        in fp32);
+      * a dense matrix with k > 64: the row range of `_gemm_search` (int64 indices), the rows it gives on all of X;
+      * a scipy.sparse matrix: the whole matrix is searched with `knn_sparse_device` (k <= 256; above that the GEMM
+        path on the dense matrix) and the rows are sliced out.  Exact, but it costs the full search."""
+    from .. import _lib
+    lib = _lib.load()
+    n = int(X.shape[0])
+    row_begin, row_end, k = int(row_begin), int(row_end), int(k)
+    if not 0 <= row_begin < row_end <= n:
+        raise ValueError("need 0 <= row_begin < row_end <= n; got [%d, %d) with n = %d" % (row_begin, row_end, n))
+    if not 1 <= k <= n - 1:
+        raise ValueError("need 1 <= k <= n - 1; got k = %d with n = %d" % (k, n))
+    if sp.issparse(X):
+        dev = util.cuda_device()
+        if k > lib.mde_knn_long_max_k():
+            return _gemm_search(_to_device_matrix(X, dev), k, row_begin=row_begin, row_end=row_end)
+        idx, d2 = knn_sparse_device(*_to_device_csr(X, dev), k)
+        return idx[row_begin:row_end].contiguous(), d2[row_begin:row_end].contiguous()
+    if X.dtype not in _HALF_DTYPES:
+        X = X.float()
+    X = X.contiguous()
+    if k > lib.mde_knn_wide_max_k():
+        return _gemm_search(X.float(), k, row_begin=row_begin, row_end=row_end)
+    half = X.dtype in _HALF_DTYPES
+    ws_bytes, search = ((lib.mde_knn16_rows_ws_bytes, lib.mde_knn16_rows) if half else
+                        (lib.mde_knn_rows_ws_bytes, lib.mde_knn_rows))
+    d, r = int(X.shape[1]), row_end - row_begin
+    need = C.c_size_t(0)
+    _lib.check(ws_bytes(n, d, r, k, C.byref(need)))
+    ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=X.device)
+    off = (-ws.data_ptr()) % 1024
+    idx = torch.empty((r, k), dtype=torch.int32, device=X.device)
+    d2 = torch.empty((r, k), dtype=torch.float32, device=X.device)
+    with torch.cuda.device(X.device):
+        stream = torch.cuda.current_stream().cuda_stream
+        _lib.check(search(*_matrix_args(X), n, d, row_begin, row_end, k, idx.data_ptr(), d2.data_ptr(),
+                          ws.data_ptr() + off, need.value, stream, None))
+        torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
+    return idx, d2
+
+
 def knn_approx_device(X, k, seed=None):
     """(indices [n, k] int32, squared distances [n, k] fp32) of k rows found for every row of the CUDA fp32 matrix X
     by NN-descent, ascending by (distance, index), with the exact fp32 distances of `knn_device`
@@ -247,13 +298,16 @@ def _search(data, k, dev, chunk_rows=None):
     return idx, d2, n
 
 
-def _gemm_search(X, k, chunk_rows=None):
+def _gemm_search(X, k, chunk_rows=None, row_begin=0, row_end=None):
     """(idx [n, k] int64, squared distances [n, k] fp32) of the k nearest rows of every row of the device fp32 matrix
     X, by row chunks of a library GEMM: candidate scores ||x||^2 - 2 q.x of the fp64 column-centred matrix (fp64
     matmuls, whatever torch.backends.cuda.matmul.allow_tf32 says; centring keeps the cancellation of data far from the
     origin out of the scores), the k + 8 best kept, then re-ranked by their fp32 squared distances (sum of squared fp32
-    differences) and index, ascending."""
+    differences) and index, ascending.  With a row range, only the chunks of the full search that hold rows
+    [row_begin, row_end) are searched (against all n rows), with the same arithmetic, and those rows returned: the
+    rows the full search gives, bit for bit."""
     n, d = X.shape
+    row_end = n if row_end is None else row_end
     dev = X.device
     Xd = X.double()
     Xd -= Xd.mean(0)
@@ -262,7 +316,8 @@ def _gemm_search(X, k, chunk_rows=None):
     rows = chunk_rows or max(256, min(n, int(2 ** 26 // max(n, 1))))
     sub = max(1, int(2 ** 26 // max(kc * d, 1)))  # rows per fp32 re-rank batch (256 MB of differences)
     idxs, vals = [], []
-    for s0 in range(0, n, rows):
+    first = row_begin // rows * rows
+    for s0 in range(first, row_end, rows):
         Q = Xd[s0:s0 + rows]
         score = sq[None, :] - 2.0 * (Q @ Xd.T)  # ||q||^2 is constant along a row
         score[torch.arange(Q.shape[0], device=dev), torch.arange(s0, s0 + Q.shape[0], device=dev)] = float("inf")
@@ -274,7 +329,8 @@ def _gemm_search(X, k, chunk_rows=None):
             d2 = ((X[s0 + r0:s0 + r0 + c.shape[0], None, :] - X[c]) ** 2).sum(-1)
             d2, pos = torch.sort(d2, dim=1, stable=True)
             idxs.append(torch.gather(c, 1, pos[:, :k])); vals.append(d2[:, :k])
-    return torch.cat(idxs), torch.cat(vals)
+    lo, hi = row_begin - first, row_end - first
+    return torch.cat(idxs)[lo:hi], torch.cat(vals)[lo:hi]
 
 
 def k_nearest_neighbors(data, k, max_distance=None, verbose=False, device=None, chunk_rows=None):

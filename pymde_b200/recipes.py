@@ -136,3 +136,167 @@ def laplacian_embedding(data, embedding_dim=2, n_neighbors=None, max_distance=No
     return preserve_neighbors(data, embedding_dim=embedding_dim, attractive_penalty=penalties.Quadratic,
                               repulsive_penalty=None, n_neighbors=n_neighbors, max_distance=max_distance,
                               init=init, device=device, verbose=verbose)
+
+
+# ---- embedding new points next to a fitted embedding ------------------------------------------------------------------
+
+def _lists_graph(lists, n):
+    """(edges [p, 2] int64, weights [p] fp32) of `Graph.from_edges` on the directed pairs (i, lists[i, s]) (-1 = no
+    entry): on the device by `graph.knn_edge_list` for CUDA lists of up to 256 columns, else the host `Graph`."""
+    from .preprocess.graph import knn_edge_list
+    if lists.is_cuda and lists.shape[1] <= _knn_graph_max_k(long=True):
+        g = knn_edge_list(lists, n)
+        return g.edges, g.weights
+    keep = lists >= 0
+    rows = torch.arange(n, device=lists.device)[:, None].expand_as(lists)
+    e = torch.stack([rows[keep], lists[keep].long()], 1).cpu()
+    g = Graph.from_edges(e, None, n_items=n)
+    return g.edges.to(lists.device).long(), g.weights.to(lists.device).float()
+
+
+def _new_points_graph(idx, n_old, repulsive_fraction):
+    """Steps 2-4 of `embed_new_points` on the neighbour lists idx [n_new, k] of the new points (global ids: old points
+    0 .. n_old - 1, new points n_old .. n - 1; -1 = no entry), on idx's device.  `repulsive_fraction` None: no
+    repulsive edges.  Returns (items, lists, edges, weights):
+      items    [n_local] global id of every local item: the new points (local 0 .. n_new - 1), then the old points
+               the lists or the repulsive edges reference, ascending;
+      lists    [n_local, k] int32 local lists (old rows -1);
+      edges    [p, 2] local pairs i < j: the attractive edges of `Graph.from_edges` on the lists (a mutual new-new
+               pair weighs 2, a new-old pair 1), then the repulsive pairs (weight -1);
+      weights  [p] fp32."""
+    n_new, k = int(idx.shape[0]), int(idx.shape[1])
+    n = n_old + n_new
+    dev = idx.device
+    idx = idx.long()
+    valid = idx >= 0
+    new = torch.arange(n_old, n, device=dev)
+    att = torch.stack([new[:, None].expand_as(idx)[valid], idx[valid]], 1)
+    att_keys = torch.unique(preprocess.preprocess._keys(att, n))
+    rep = torch.empty((0, 2), dtype=torch.int64, device=dev)
+    if repulsive_fraction is not None:
+        p_att = int(att_keys.numel())
+        available = n_new * (n - 1) - n_new * (n_new - 1) // 2 - p_att
+        n_rep = min(int(repulsive_fraction * p_att), available)
+        exclude = torch.stack([att_keys // n, att_keys % n], 1)
+        rep = preprocess.preprocess.sample_edges_touching(n, n_old, n_rep, exclude=exclude, device=dev)
+    ends = torch.cat([idx[valid], rep.reshape(-1)])
+    items = torch.cat([new, torch.unique(ends[ends < n_old])])
+    local = torch.full((n,), -1, dtype=torch.int64, device=dev)
+    local[items] = torch.arange(items.numel(), device=dev)
+    lists = torch.full((items.numel(), k), -1, dtype=torch.int32, device=dev)
+    lists[:n_new] = torch.where(valid, local[idx.clamp(min=0)], -1).to(torch.int32)
+    edges, weights = _lists_graph(lists, items.numel())
+    rep = torch.sort(local[rep], dim=1).values
+    edges = torch.cat([edges.long(), rep])
+    weights = torch.cat([weights.float(), -torch.ones(rep.shape[0], dtype=torch.float32, device=dev)])
+    return items, lists, edges, weights
+
+
+def _new_points_init(items, lists, n_new, embedding, att_edges):
+    """Step 5 of `embed_new_points`: the initial iterate [n_local, m] fp32.  Old rows are exactly their `embedding`
+    rows; a new point starts at the mean of the embedding rows of its old neighbours, or at the column mean of
+    `embedding` when it has none; when an attractive edge (local pairs `att_edges`) then has length 0, 1e-4 randn is
+    added to the new rows only (pymde/recipes.py:438-447 perturbs every row)."""
+    emb = embedding.float()
+    X = torch.empty((int(items.numel()), emb.shape[1]), dtype=torch.float32, device=emb.device)
+    X[n_new:] = emb[items[n_new:]]
+    nb = lists[:n_new].long()
+    old = nb >= n_new
+    cnt = old.sum(1, keepdim=True)
+    sums = torch.where(old[..., None], X[nb.clamp(min=0)], 0.0).sum(1)
+    X[:n_new] = torch.where(cnt > 0, sums / cnt.clamp(min=1), emb.mean(0))
+    if att_edges.shape[0] and bool(((X[att_edges[:, 0]] - X[att_edges[:, 1]]).norm(dim=1) == 0).any()):
+        X[:n_new] += 1e-4 * torch.randn_like(X[:n_new])
+    return X
+
+
+def _stacked_matrix(data, new_data, dev):
+    """[data; new_data] for the search: a scipy.sparse CSR matrix when either is sparse, else a device tensor (fp32
+    when the two dtypes differ; a float16 / bfloat16 pair stays 16-bit)."""
+    if scipy.sparse.issparse(data) or scipy.sparse.issparse(new_data):
+        return scipy.sparse.vstack([scipy.sparse.csr_matrix(data), scipy.sparse.csr_matrix(new_data)]).tocsr()
+    a, b = (torch.as_tensor(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x for x in (data, new_data))
+    if a.dtype != b.dtype:
+        a, b = a.float(), b.float()
+    return torch.cat([a.to(dev), b.to(dev)])
+
+
+def _new_points_mde(data, embedding, new_data, n_neighbors=None, attractive_penalty=penalties.Log1p,
+                    repulsive_penalty=penalties.Log, repulsive_fraction=None, max_distance=None, device=None):
+    """Steps 1-5 of `embed_new_points`: (the anchored `MDE` over the new points and the old points they reference,
+    with its initial iterate in `_X_init`; items, the global id of each of its items: new points n_old .. n - 1
+    first), or (None, None) when there are no new rows."""
+    for x in (data, new_data):
+        if isinstance(x, Graph):
+            raise ValueError("embed_new_points takes data matrices; a Graph is not supported")
+    if not isinstance(embedding, (np.ndarray, torch.Tensor)) or embedding.ndim != 2:
+        raise ValueError("`embedding` must be a 2-D array (n_old x embedding_dim)")
+    if len(data.shape) != 2 or len(new_data.shape) != 2:
+        raise ValueError("`data` and `new_data` must be 2-D matrices")
+    n_old, n_new = int(data.shape[0]), int(new_data.shape[0])
+    if int(embedding.shape[0]) != n_old:
+        raise ValueError("`embedding` has %d rows; `data` has %d" % (int(embedding.shape[0]), n_old))
+    if int(new_data.shape[1]) != int(data.shape[1]):
+        raise ValueError("`new_data` has %d columns; `data` has %d" % (int(new_data.shape[1]), int(data.shape[1])))
+    if n_new == 0:
+        return None, None
+    if n_old < 1:
+        raise ValueError("`data` must hold at least one fitted row")
+    dev = util.cuda_device(device)
+    n = n_old + n_new
+    if n_neighbors is None:
+        n_neighbors = int(max(min(15, (n * (n - 1) / 2) * 0.01 / n), 5))
+    k = int(min(n_neighbors, n - 1))
+    idx, d2 = preprocess.data_matrix.knn_rows_device(_stacked_matrix(data, new_data, dev), k, n_old, n)
+    idx = idx.to(dev)
+    if max_distance is not None:
+        idx = torch.where(d2.to(dev).sqrt() <= max_distance, idx, -1)  # (a NaN distance is dropped)
+    if repulsive_penalty is not None and repulsive_fraction is None:
+        repulsive_fraction = 1
+    items, lists, edges, weights = _new_points_graph(
+        idx, n_old, repulsive_fraction if repulsive_penalty is not None else None)
+    emb = torch.as_tensor(embedding).to(device=dev, dtype=torch.float32)
+    n_att = int((weights > 0).sum())
+    X_init = _new_points_init(items, lists, n_new, emb, edges[:n_att])
+    if repulsive_penalty is not None:
+        f = penalties.PushAndPull(weights, attractive_penalty=attractive_penalty, repulsive_penalty=repulsive_penalty)
+    else:
+        f = attractive_penalty(weights)
+    anchors = torch.arange(n_new, int(items.numel()), device=dev)
+    constraint = constraints.Anchored(anchors, X_init[n_new:].clone())
+    mde = problem.MDE(n_items=int(items.numel()), embedding_dim=int(emb.shape[1]), edges=edges,
+                      distortion_function=f, constraint=constraint, device=dev)
+    mde._X_init = X_init.contiguous()
+    return mde, items
+
+
+def embed_new_points(data, embedding, new_data, n_neighbors=None, attractive_penalty=penalties.Log1p,
+                     repulsive_penalty=penalties.Log, repulsive_fraction=None, max_distance=None, eps=1e-5,
+                     max_iter=300, device=None, verbose=False):
+    """Embed the rows of `new_data` next to `embedding`, the fitted embedding of the rows of `data`, leaving
+    `embedding` untouched: the "transform" step of an embedding.  Returns the new rows' embedding, an
+    (n_new x embedding_dim) fp32 tensor on the device.
+
+    The workflow the reference documents (docs "Embedding new points") runs `preserve_neighbors` on the stacked data
+    with every fitted row anchored, and so pays for a search, a spectral initialisation and a solve over all rows.
+    Here only the new rows are searched, against all rows (`data_matrix.knn_rows_device`: exact, with a cost of about
+    n_new n d), and only the new points and the fitted points they touch enter the solve:
+      * attractive edges: `Graph.from_edges` on the new points' lists of their min(n_neighbors, n - 1) nearest rows
+        (`n_neighbors` defaults to `preserve_neighbors`' rule at n = n_old + n_new; entries beyond `max_distance`
+        dropped): a mutual new-new pair weighs 2, a new-old pair 1.  Unlike the reference workflow, the fitted points'
+        own neighbour lists add no edges (that would need their n^2 search);
+      * repulsive edges (none when `repulsive_penalty` is None): repulsive_fraction (default 1) times as many pairs
+        as attractive ones, each with a uniform new point at one end and a uniform row at the other, distinct and not
+        attractive, drawn from the module RNG (`pymde_b200.seed(s)` reproduces them);
+      * the fitted points are anchored at their `embedding` rows; a new point starts at the mean of its fitted
+        neighbours' rows (the column mean of `embedding` when it has none);
+      * the anchored problem is solved on the device (`MDE.embed(eps, max_iter)`).
+    `data` and `new_data` are dense (numpy, torch; fp32, or float16 / bfloat16 searched in place) or scipy.sparse
+    matrices with the same columns; a Graph is not supported."""
+    mde, _ = _new_points_mde(data, embedding, new_data, n_neighbors=n_neighbors,
+                             attractive_penalty=attractive_penalty, repulsive_penalty=repulsive_penalty,
+                             repulsive_fraction=repulsive_fraction, max_distance=max_distance, device=device)
+    if mde is None:
+        return torch.empty((0, int(embedding.shape[1])), dtype=torch.float32, device=util.cuda_device(device))
+    X = mde.embed(eps=eps, max_iter=max_iter, verbose=verbose)
+    return X[:int(new_data.shape[0])].contiguous()
