@@ -465,6 +465,24 @@ int mde_knn_rows(const float* X, int64_t n, int d, int64_t row_begin, int64_t ro
 int mde_knn16_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes);
 int mde_knn16_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin, int64_t row_end, int k,
                    int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows);
+/* The exact sparse searches for a range of query rows: rows [row_begin, row_end) of a device CSR matrix against all
+ * n rows (the row itself excluded).  Row r of idx_out / d2_out (rows x k, rows = row_end - row_begin) is bit for bit
+ * row row_begin + r of mde_knn_csr (k <= 24), mde_knn_csr_wide (24 < k <= 64) or mde_knn_csr_long (64 < k <= 256) on
+ * the same matrix and k, ties included.  The preparation (CSR check, feature order, re-sorted rows, tile bitmaps)
+ * covers the whole matrix, since every row is a candidate; the tiles sweep only the query tiles, and when those
+ * cannot fill the SMs the candidate sweep of the narrow and wide searches is split into S slices (one CTA per query
+ * tile and slice; S from the tile counts alone).  A row's S lists are merged by taking their KK smallest pairs in the
+ * tiles' own (approximate score, index) order, which are exactly the full search's KK candidates, before the exact
+ * re-rank.  Input contract, CSR check and return codes of mde_knn_csr (a malformed CSR is MDE_E_INVALID);
+ * 0 <= row_begin < row_end <= n, 1 <= k <= 256, k <= n - 1; a bad argument or a workspace too small or not 1024-byte
+ * aligned is MDE_E_INVALID before any CUDA call.  `ws`: 1024-byte aligned device scratch of
+ * mde_knn_csr_rows_ws_bytes(n, d, nnz, rows, k) bytes (host arithmetic alone: the preparation's, with a bound on the
+ * sort scratch, plus the candidate lists of the query rows; it grows with n and with rows; MDE_E_ALLOC should the
+ * sort need more scratch than that bound).  Blocking as mde_knn_csr. */
+int mde_knn_csr_rows_ws_bytes(int64_t n, int d, int64_t nnz, int64_t rows, int k, size_t* bytes);
+int mde_knn_csr_rows(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                     int64_t nnz, int64_t row_begin, int64_t row_end, int k, int32_t* idx_out, float* d2_out, void* ws,
+                     size_t ws_bytes, void* stream);
 /* The same NN-descent search on a sparse data matrix, without densifying it.  Input contract of mde_knn_csr (the
  * device CSR check included: MDE_E_INVALID when malformed); output contract of mde_knn_approx, with the distances of
  * mde_knn_csr / mde_knn_csr_wide: the exact squared distance summed in fp64 and rounded once to fp32, which is also

@@ -165,6 +165,10 @@ SIGNATURES = {
     "mde_knn16_rows_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn16_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
+    "mde_knn_csr_rows_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int,
+                                            C.POINTER(C.c_size_t)]),
+    "mde_knn_csr_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int64,
+                                   C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mde_knn16_approx_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn16_approx": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -223,6 +227,7 @@ DEBUG_SIGNATURES = {
     "mde_dbg_lbfgs_reset": (None, [C.c_void_p]),
     "mde_dbg_lbfgs_cand": (C.c_int, [C.c_void_p]),
     "mde_dbg_knn_slices": (C.c_int, [C.c_int64, C.c_int64, C.c_int]),
+    "mde_dbg_knn_csr_slices": (C.c_int, [C.c_int64, C.c_int64, C.c_int]),
 }
 
 _lib = None

@@ -100,20 +100,8 @@ constexpr int kWideSmemBytes = kStages * kWideStageBytes<TN> + 1024 /* alignment
 static_assert(kWideSmemBytes<kWideKK, kTileN> <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 static_assert(kWideSmemBytes<kLongKK, kLongTileN> <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 
-// The query rows of a search, [lo, hi) of X, and the candidate slice of a CTA (mde_knn_rows).  CTA (x, y) takes the
-// query rows base + x TM .. + TM - 1 (base: lo rounded down to 128, so that every query box lies inside the padded
-// operand) against the candidate tiles [slice_begin(T), slice_begin(T, 1)) of the T tiles, and keeps the list of
-// query row r at list(r) = (r - lo) slices + y: the S lists of a row are adjacent.  A full search is [0, n) in one slice.
-struct QueryRange {
-  int64_t base, lo, hi;
-  int slices;
-  __device__ __forceinline__ bool has(int64_t r) const { return r >= lo && r < hi; }
-  __device__ __forceinline__ int64_t list(int64_t r) const { return (r - lo) * slices + blockIdx.y; }
-  __device__ __forceinline__ int slice_begin(int tiles, int next = 0) const {
-    return (int)((int64_t)tiles * (blockIdx.y + next) / slices);
-  }
-};
-constexpr int kMaxSlices = 16;  // S <= 16: the merge keeps a row's S KK <= 1536 candidates in 12 KB of shared memory
+// Query ranges and candidate slices: QueryRange, kMaxSlices (mde_knn_select.cuh).  The dense searches take base = lo
+// rounded down to 128, so that every query box also lies inside the padded operand.
 
 // ---------------------------------------------------------------------------------------------------------------
 // PTX wrappers (tensor TMA); mbarriers come from mde_tma.cuh, wgmma from mde_wgmma.cuh

@@ -505,9 +505,8 @@ ApproxLayout approx_layout(int64_t n, int k) {
 }
 
 // CSR search: prepare_csr's workspace (without candidate lists), then the lists.  The workspace size is host
-// arithmetic alone, so the sort scratch is reserved as a bound: 16 bytes per item of the larger sort (the alternate
-// key and value buffers take 12, CUB's look-back at most 4) plus 8 MB of histograms; the call checks CUB's exact
-// figure against it.
+// arithmetic alone, so the sort scratch is reserved as csr_sort_scratch_bound; the call checks CUB's exact figure
+// against it.
 struct ApproxCsrLayout {
   CsrKnnLayout prep;
   ApproxLayout lists;  // offsets from prep.total
@@ -516,8 +515,7 @@ struct ApproxCsrLayout {
 
 ApproxCsrLayout approx_csr_layout(int64_t n, int d, int64_t nnz, int k) {
   ApproxCsrLayout A;
-  const size_t items = (size_t)(nnz > (int64_t)d ? nnz : (int64_t)d);
-  csr_knn_carve(n, d, nnz, 0, 16 * items + (8u << 20), &A.prep);
+  csr_knn_carve(n, d, nnz, 0, csr_sort_scratch_bound(d, nnz), &A.prep);
   A.lists = approx_layout(n, k);
   A.total = A.prep.total + A.lists.total;
   return A;
@@ -548,8 +546,9 @@ template <int KB>
 int launch_rerank(const CsrRows& r, int64_t n, const int32_t* cand, int k, int32_t* idx_out, float* d2_out,
                   cudaStream_t st) {
   const unsigned grid = (unsigned)((n + 7) / 8);
-  if (KB == kNarrowKK) knn_csr_rerank_kernel<<<grid, 256, 0, st>>>(r.indptr, r.cols, r.vals, n, cand, k, idx_out, d2_out);
-  else knn_csr_wide_rerank_kernel<<<grid, 256, 0, st>>>(r.indptr, r.cols, r.vals, n, cand, k, idx_out, d2_out);
+  if (KB == kNarrowKK)
+    knn_csr_rerank_kernel<<<grid, 256, 0, st>>>(r.indptr, r.cols, r.vals, 0, n, cand, k, idx_out, d2_out);
+  else knn_csr_wide_rerank_kernel<<<grid, 256, 0, st>>>(r.indptr, r.cols, r.vals, 0, n, cand, k, idx_out, d2_out);
   MDE_LAUNCH_CHECK();
   return 0;
 }

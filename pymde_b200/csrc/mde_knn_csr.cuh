@@ -19,6 +19,10 @@ struct CsrKnnLayout {
 
 // Scratch bytes of the two CUB radix sorts of prepare_csr: a query that needs a device but does no device work.
 int csr_sort_scratch(int64_t n, int d, int64_t nnz, size_t* bytes);
+// A bound on that scratch in host arithmetic alone, for workspace queries that must not need a device: 16 bytes per
+// item of the larger sort (the alternate key and value buffers take 12, CUB's look-back at most 4) plus 8 MB of
+// histograms.  A search sized by it checks csr_sort_scratch against it before it starts.
+size_t csr_sort_scratch_bound(int d, int64_t nnz);
 // The layout for a given sort scratch (host arithmetic only).  kk: candidates kept per row (kNarrowKK, or kWideKK for
 // the wide search; 0 when the caller keeps its own lists elsewhere).
 void csr_knn_carve(int64_t n, int d, int64_t nnz, int kk, size_t tmp_bytes, CsrKnnLayout* L);
@@ -62,15 +66,16 @@ __device__ __forceinline__ double merge_dist2(const int64_t* __restrict__ indptr
 }
 
 // (float)merge_dist2 of a row's kNarrowKK (knn_csr_rerank_kernel) or kWideKK (knn_csr_wide_rerank_kernel) candidates
-// cand_idx[row][.], -1 for none; the k smallest by (distance, index) go to out_idx / out_d2 [n][k] in ascending order.
-// One warp per row, 256 threads per block.
+// cand_idx[r][.], -1 for none, for the query rows lo + r, 0 <= r < rows; the k smallest by (distance, index) go to
+// out_idx / out_d2 [rows][k] in ascending order.  One warp per row, 256 threads per block.
 __global__ void __launch_bounds__(256)
 knn_csr_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
-                      const float* __restrict__ vals, int64_t n, const int32_t* __restrict__ cand_idx, int k,
-                      int32_t* __restrict__ out_idx, float* __restrict__ out_d2);
+                      const float* __restrict__ vals, int64_t lo, int64_t rows, const int32_t* __restrict__ cand_idx,
+                      int k, int32_t* __restrict__ out_idx, float* __restrict__ out_d2);
 __global__ void __launch_bounds__(256)
 knn_csr_wide_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
-                           const float* __restrict__ vals, int64_t n, const int32_t* __restrict__ cand_idx, int k,
-                           int32_t* __restrict__ out_idx, float* __restrict__ out_d2);
+                           const float* __restrict__ vals, int64_t lo, int64_t rows,
+                           const int32_t* __restrict__ cand_idx, int k, int32_t* __restrict__ out_idx,
+                           float* __restrict__ out_d2);
 
 }  // namespace mde

@@ -32,6 +32,22 @@ __device__ __forceinline__ bool knn_before(float d1, int i1, float d2, int i2) {
   return d1 < d2 || (d1 == d2 && i1 < i2);
 }
 
+// The query rows of a search, [lo, hi) of the matrix, and the candidate slice of a CTA (mde_knn_rows,
+// mde_knn_csr_rows).  CTA (x, y) takes the query rows base + x TM .. + TM - 1 (base: lo rounded down to a tile of the
+// full search, so that every query tile is one of the full search's) against the candidate tiles
+// [slice_begin(T), slice_begin(T, 1)) of the T tiles, and keeps the list of query row r at
+// list(r) = (r - lo) slices + y: the S lists of a row are adjacent.  A full search is [0, n) in one slice.
+struct QueryRange {
+  int64_t base, lo, hi;
+  int slices;
+  __device__ __forceinline__ bool has(int64_t r) const { return r >= lo && r < hi; }
+  __device__ __forceinline__ int64_t list(int64_t r) const { return (r - lo) * slices + blockIdx.y; }
+  __device__ __forceinline__ int slice_begin(int tiles, int next = 0) const {
+    return (int)((int64_t)tiles * (blockIdx.y + next) / slices);
+  }
+};
+constexpr int kMaxSlices = 16;  // S <= 16: a merge keeps a row's S KK <= 1536 candidates in 12 KB of shared memory
+
 // Per-lane copy of its row's threshold: the worst kept pair and its slot (identical in both lanes of the pair).
 template <int KK>
 struct WideList {

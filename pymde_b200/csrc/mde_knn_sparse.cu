@@ -27,6 +27,13 @@
 // mde_knn_csr_long (k <= 256): the same kernel with KK = 288 on candidate tiles of 64 rows (one warpgroup); the
 // re-rank merges all 288.
 //
+// mde_knn_csr_rows searches a range of query rows against all n rows with the narrow, wide or long tiles (every full
+// search is the range [0, n) in one slice).  The preparation still covers the whole matrix; the tiles sweep only the
+// query tiles, aligned as in the full search.  When those leave SMs idle the narrow and wide sweeps are split into S
+// candidate slices (blockIdx.y; S from mde_logic.h::knn_slices), and knn_csr_merge_kernel keeps the KK smallest of a
+// row's S lists by the tiles' own (score, index) order -- the full search's candidates -- for the re-rank
+// (DESIGN 11.8).
+//
 // mde_pair_dist_csr: ||a - b|| of given pairs by the same sorted merge, fp64, sqrt in fp64, one rounding.
 #include <cub/cub.cuh>
 #include <cuda_bf16.h>
@@ -37,6 +44,7 @@
 #include "mde_common.cuh"
 #include "mde_knn_csr.cuh"
 #include "mde_knn_select.cuh"
+#include "mde_logic.h"
 #include "mde_tma.cuh"
 #include "mde_wgmma.cuh"
 
@@ -174,10 +182,12 @@ __global__ void key_to_col_kernel(const uint64_t* __restrict__ keys, int64_t nnz
 // ---------------------------------------------------------------------------------------------------------------
 // tiles
 // ---------------------------------------------------------------------------------------------------------------
+// CTA (x, y) sweeps query tile qr.base / 128 + x against candidate slice y (QueryRange); query rows outside
+// [qr.lo, qr.hi) write nothing.
 __global__ void __launch_bounds__(kThreads, 1)
 knn_csr_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
                     const float* __restrict__ vals, const float* __restrict__ norms,
-                    const uint32_t* __restrict__ bitmap, int nwords, int64_t n, int num_tiles,
+                    const uint32_t* __restrict__ bitmap, int nwords, int64_t n, int num_tiles, QueryRange qr,
                     int32_t* __restrict__ cand_idx, float* __restrict__ cand_val) {
   extern __shared__ uint8_t smem_raw[];
   // carve: [stages x 64 KB, 1024-aligned] | staged accumulators [128][kAccStride] | norms[128] | visited blocks
@@ -190,8 +200,9 @@ knn_csr_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __restric
   __shared__ typename Scan::TempStorage scan_tmp;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int64_t row0 = (int64_t)blockIdx.x * kTileM;
-  const uint32_t* abm = bitmap + (int64_t)blockIdx.x * nwords;
+  const int64_t row0 = qr.base + (int64_t)blockIdx.x * kTileM;
+  const uint32_t* abm = bitmap + (row0 / kTileM) * nwords;
+  const int t_begin = qr.slice_begin(num_tiles), t_end = qr.slice_begin(num_tiles, 1);
 
   // ----- builder role: thread tid owns operand row tid & 127 of A (query tile, tid < 128) or B (candidate tile)
   const bool is_b = tid >= 128;
@@ -218,7 +229,7 @@ knn_csr_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __restric
   float acc[64];
 
   int stage = 0;
-  for (int t = 0; t < num_tiles; ++t) {
+  for (int t = t_begin; t < t_end; ++t) {
     int64_t p = a_beg, end = a_end;
     if (is_b) {
       const int64_t r = (int64_t)t * kTileN + orow;
@@ -314,11 +325,12 @@ knn_csr_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __restric
     for (int q = 0; q < kKK; ++q) {
       if (before(xd[q], xi[q], thr, thi)) keep_candidate(bd, bi, xd[q], xi[q], thr, thi, worst);
     }
-    if (row < n) {
+    if (qr.has(row)) {
+      const int64_t o = qr.list(row) * kKK;
 #pragma unroll
       for (int q = 0; q < kKK; ++q) {
-        cand_idx[row * kKK + q] = bi[q] == INT_MAX ? -1 : bi[q];
-        cand_val[row * kKK + q] = bd[q];
+        cand_idx[o + q] = bi[q] == INT_MAX ? -1 : bi[q];
+        cand_val[o + q] = bd[q];
       }
     }
   }
@@ -332,16 +344,17 @@ knn_csr_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __restric
 // ---------------------------------------------------------------------------------------------------------------
 namespace mde {
 
-// One warp per row, lane q re-ranks candidate q; the k smallest (distance, index) in ascending order.
+// One warp per row r of rows (query row lo + r), lane q re-ranks candidate q; the k smallest (distance, index) in
+// ascending order.
 __global__ void __launch_bounds__(256)
 knn_csr_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
-                      const float* __restrict__ vals, int64_t n, const int32_t* __restrict__ cand_idx, int k,
-                      int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+                      const float* __restrict__ vals, int64_t lo, int64_t rows, const int32_t* __restrict__ cand_idx,
+                      int k, int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (row >= n) return;
+  if (row >= rows) return;
   const int c = cand_idx[row * kKK + lane];
-  const float my_d = c >= 0 ? (float)merge_dist2(indptr, cols, vals, row, c) : kInf;
+  const float my_d = c >= 0 ? (float)merge_dist2(indptr, cols, vals, lo + row, c) : kInf;
   const int mine = c >= 0 ? c : INT_MAX;  // missing candidates last
   int rank = 0;
   for (int q = 0; q < kKK; ++q) {
@@ -362,13 +375,14 @@ namespace {
 // ---------------------------------------------------------------------------------------------------------------
 // wide tiles (k <= 64, KK = 96, TN = 128) and long tiles (k <= 256, KK = 288, TN = 64): as knn_csr_tile_kernel for
 // 64 query rows, one running top-KK per row in shared memory; warpgroup wg issues wgmma.m64n64k16 on candidates
-// 64 wg .. 64 wg + 63 of the tile
+// 64 wg .. 64 wg + 63 of the tile.  CTA (x, y) sweeps the 64 query rows qr.base + 64 x .. against candidate slice y
+// (QueryRange); query rows outside [qr.lo, qr.hi) write nothing.
 // ---------------------------------------------------------------------------------------------------------------
 template <int KK, int TN>
 __global__ void __launch_bounds__(2 * TN, 1)
 knn_csr_wide_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
                          const float* __restrict__ vals, const float* __restrict__ norms,
-                         const uint32_t* __restrict__ bitmap, int nwords, int64_t n, int num_tiles,
+                         const uint32_t* __restrict__ bitmap, int nwords, int64_t n, int num_tiles, QueryRange qr,
                          int32_t* __restrict__ cand_idx, float* __restrict__ cand_val) {
   static_assert(TN == 64 || TN == 128, "one or two warpgroups");
   constexpr int kThreadsT = 2 * TN;                  // one warpgroup per 64 candidates of a tile
@@ -393,10 +407,11 @@ knn_csr_wide_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __re
   __shared__ typename Scan::TempStorage scan_tmp;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int64_t row0 = (int64_t)blockIdx.x * kWideTileM;
+  const int64_t row0 = qr.base + (int64_t)blockIdx.x * kWideTileM;
   // the query rows use the bitmap of their 128-row tile, and so do the candidate rows: a superset of their own
   // blocks (a block only other rows of that tile occupy is built with zero rows and adds exactly 0)
   const uint32_t* abm = bitmap + (row0 / kTileM) * nwords;
+  const int t_begin = qr.slice_begin(num_tiles), t_end = qr.slice_begin(num_tiles, 1);
 
   // ----- builder role: thread tid owns operand row tid of A (query rows, tid < 64) or row tid - 64 of B (up to
   // tid 64 + TN - 1); with TN = 128, warps 6 and 7 build nothing
@@ -421,7 +436,7 @@ knn_csr_wide_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __re
   float acc[32];
 
   int stage = 0;
-  for (int t = 0; t < num_tiles; ++t) {
+  for (int t = t_begin; t < t_end; ++t) {
     int64_t p = a_beg, end = a_end;
     if (is_b) {
       const int64_t r = (int64_t)t * TN + orow;
@@ -511,30 +526,30 @@ knn_csr_wide_tile_kernel(const int64_t* __restrict__ indptr, const int32_t* __re
       }
     }
   }
-  if (scanner && row < n) list.store(cand_idx + row * KK, cand_val + row * KK);
+  if (scanner && qr.has(row)) list.store(cand_idx + qr.list(row) * KK, cand_val + qr.list(row) * KK);
 }
 
 }  // namespace
 
 namespace mde {
 
-// One warp per row, lane q re-ranks candidates q, q + 32, q + 64, ... by the merge of knn_csr_rerank_kernel; the k
-// smallest (distance, index) of the KK in ascending order.
+// One warp per row r of rows (query row lo + r), lane q re-ranks candidates q, q + 32, q + 64, ... by the merge of
+// knn_csr_rerank_kernel; the k smallest (distance, index) of the KK in ascending order.
 template <int KK>
 __device__ __forceinline__ void csr_wide_rerank_row(const int64_t* __restrict__ indptr,
                                                     const int32_t* __restrict__ cols, const float* __restrict__ vals,
-                                                    int64_t n, const int32_t* __restrict__ cand_idx, int k,
-                                                    int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+                                                    int64_t lo, int64_t rows, const int32_t* __restrict__ cand_idx,
+                                                    int k, int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (row >= n) return;
+  if (row >= rows) return;
   constexpr int kPer = KK / 32;
   float my_d[kPer];
   int mine[kPer];
 #pragma unroll
   for (int s = 0; s < kPer; ++s) {
     const int c = cand_idx[row * KK + 32 * s + lane];
-    my_d[s] = c >= 0 ? (float)merge_dist2(indptr, cols, vals, row, c) : kInf;
+    my_d[s] = c >= 0 ? (float)merge_dist2(indptr, cols, vals, lo + row, c) : kInf;
     mine[s] = c >= 0 ? c : INT_MAX;  // missing candidates last
   }
   int rank[kPer] = {};
@@ -558,20 +573,66 @@ __device__ __forceinline__ void csr_wide_rerank_row(const int64_t* __restrict__ 
 
 __global__ void __launch_bounds__(256)
 knn_csr_wide_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
-                           const float* __restrict__ vals, int64_t n, const int32_t* __restrict__ cand_idx, int k,
-                           int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
-  csr_wide_rerank_row<kWideKK>(indptr, cols, vals, n, cand_idx, k, out_idx, out_d2);
+                           const float* __restrict__ vals, int64_t lo, int64_t rows,
+                           const int32_t* __restrict__ cand_idx, int k, int32_t* __restrict__ out_idx,
+                           float* __restrict__ out_d2) {
+  csr_wide_rerank_row<kWideKK>(indptr, cols, vals, lo, rows, cand_idx, k, out_idx, out_d2);
 }
 
 // the 288 candidates of the long search, with the same merge
 __global__ void __launch_bounds__(256)
 knn_csr_long_rerank_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
-                           const float* __restrict__ vals, int64_t n, const int32_t* __restrict__ cand_idx, int k,
-                           int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
-  csr_wide_rerank_row<kLongKK>(indptr, cols, vals, n, cand_idx, k, out_idx, out_d2);
+                           const float* __restrict__ vals, int64_t lo, int64_t rows,
+                           const int32_t* __restrict__ cand_idx, int k, int32_t* __restrict__ out_idx,
+                           float* __restrict__ out_d2) {
+  csr_wide_rerank_row<kLongKK>(indptr, cols, vals, lo, rows, cand_idx, k, out_idx, out_d2);
 }
 
 }  // namespace mde
+
+namespace {
+
+// ---------------------------------------------------------------------------------------------------------------
+// merge of a row searched in S candidate slices (mde_knn_csr_rows).  The tiles keep, per slice, the top KK of the
+// slice by (approximate score, index); the full search keeps the top KK of all candidates by the same order and
+// re-ranks exactly those.  Every member of the global top KK is in its own slice's top KK, so the KK smallest of the
+// S KK pairs, in the order of before() (-0 == +0, ties by index, an empty slot as (+inf, INT_MAX)), are the full
+// search's candidates.  Re-ranking the whole union instead could return a better list than the full search's.
+// One warp per query row r stages the row's S KK pairs in shared memory, ranks each among all of them (equal pairs,
+// only ever empty slots, by slot) and writes those of rank < KK to sel[r][rank], -1 for empty; the re-rank kernels
+// then take sel as the full search's lists.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int kMergeWarps = 4;
+
+__global__ void __launch_bounds__(kMergeWarps * 32)
+knn_csr_merge_kernel(int64_t rows, const int32_t* __restrict__ cand_idx, const float* __restrict__ cand_val,
+                     int cands, int kk, int32_t* __restrict__ sel) {
+  extern __shared__ float s_merge[];  // per warp: scores [cands], indices [cands]
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t r = (int64_t)blockIdx.x * kMergeWarps + warp;
+  if (r >= rows) return;
+  float* sd = s_merge + (size_t)warp * 2 * cands;
+  int* si = reinterpret_cast<int*>(sd + cands);
+  for (int j = lane; j < cands; j += 32) {
+    const int c = cand_idx[r * cands + j];
+    sd[j] = c >= 0 ? cand_val[r * cands + j] : kInf;
+    si[j] = c >= 0 ? c : INT_MAX;
+  }
+  __syncwarp();
+  for (int j = lane; j < cands; j += 32) {
+    const float dj = sd[j];
+    const int ij = si[j];
+    int rank = 0;
+    for (int q = 0; q < cands; ++q) {
+      const float dq = sd[q];
+      const int iq = si[q];
+      rank += before(dq, iq, dj, ij) || (q < j && !before(dj, ij, dq, iq));
+    }
+    if (rank < kk) sel[r * kk + rank] = ij == INT_MAX ? -1 : ij;
+  }
+}
+
+}  // namespace
 
 namespace {
 
@@ -607,6 +668,11 @@ int csr_sort_scratch(int64_t n, int d, int64_t nnz, size_t* bytes) {
                                                bits_for((uint64_t)n) + bits_for((uint64_t)d)));
   *bytes = t1 > t2 ? t1 : t2;
   return 0;
+}
+
+size_t csr_sort_scratch_bound(int d, int64_t nnz) {
+  const size_t items = (size_t)(nnz > (int64_t)d ? nnz : (int64_t)d);
+  return 16 * items + (8u << 20);
 }
 
 int csr_knn_layout(int64_t n, int d, int64_t nnz, CsrKnnLayout* L, int kk) {
@@ -708,7 +774,122 @@ int prepare_csr(const int64_t* indptr, const int32_t* indices, const float* valu
 
 namespace {
 
-int csr_wide_ws_bytes(int64_t n, int d, int64_t nnz, int kk, size_t* bytes) {
+// The tile shape of a search: tm query rows per CTA, tn candidates per tile, kk candidates kept per row.
+struct CsrShape { int tm, tn, kk; };
+constexpr CsrShape kCsrNarrow{kTileM, kTileN, kKK}, kCsrWide{kWideTileM, kTileN, kWideKK},
+    kCsrLong{kWideTileM, kLongTileN, kLongKK};
+
+CsrShape csr_shape(int k) { return k > kWideMaxK ? kCsrLong : k > kMaxK ? kCsrWide : kCsrNarrow; }
+
+// Candidate slices of a search of `rows` query rows against the n rows (mde_logic.h: knn_slices).  The long search
+// keeps one: the merge of its 288-candidate lists would not fit in shared memory.
+int csr_search_slices(int64_t n, int64_t rows, CsrShape sh) {
+  if (sh.kk == kLongKK) return 1;
+  const int64_t n_pad = (n + kTileN - 1) / kTileN * kTileN;
+  return knn_slices((rows + sh.tm - 1) / sh.tm, n_pad / sh.tn, kNumSMs, kMaxSlices);
+}
+
+// mde_knn_csr_rows: prepare_csr's workspace (without candidate lists, its sort scratch reserved as
+// csr_sort_scratch_bound, so that the size is host arithmetic alone), then the lists of the query rows, S per row,
+// and the KK candidates per row the merge selects.  The lists take room for rows, or, when the rule may split, the
+// most a split can hold (q_tiles S <= kNumSMs, S <= kMaxSlices): a workspace sized for a search fits every search of
+// fewer rows, and grows with n.
+struct CsrRowsLayout {
+  CsrKnnLayout prep;
+  int slices;
+  size_t off_ci, off_cv, off_sel, total;
+};
+
+CsrRowsLayout csr_rows_layout(int64_t n, int d, int64_t nnz, int64_t rows, CsrShape sh) {
+  CsrRowsLayout R;
+  csr_knn_carve(n, d, nnz, 0, csr_sort_scratch_bound(d, nnz), &R.prep);
+  R.slices = csr_search_slices(n, rows, sh);
+  int64_t cap = rows;
+  if (sh.kk != kLongKK) {
+    const int64_t split = rows * kMaxSlices < (int64_t)kNumSMs * sh.tm ? rows * kMaxSlices : (int64_t)kNumSMs * sh.tm;
+    if (split > cap) cap = split;
+  }
+  auto up = [](size_t x) { return (x + 1023) / 1024 * 1024; };
+  size_t o = R.prep.total;
+  R.off_ci = o; o = up(o + (size_t)cap * sh.kk * 4);
+  R.off_cv = o; o = up(o + (size_t)cap * sh.kk * 4);
+  R.off_sel = o; o = up(o + (size_t)rows * sh.kk * 4);
+  R.total = o;
+  return R;
+}
+
+// The prepared rows and the bitmaps of a workspace laid out by L.
+struct CsrPrepared {
+  const float* norms;
+  const uint32_t* bm;
+  const int32_t* cols;
+  const float* vals;
+};
+
+CsrPrepared prepared(const CsrKnnLayout& L, const uint8_t* w) {
+  return {reinterpret_cast<const float*>(w + L.off_norm), reinterpret_cast<const uint32_t*>(w + L.off_bm),
+          reinterpret_cast<const int32_t*>(w + L.off_kin), reinterpret_cast<const float*>(w + L.off_val)};
+}
+
+// The tiles of the query range qr (one CTA per query tile and candidate slice) into lists of sh.kk per row and slice.
+int launch_tiles(CsrShape sh, const int64_t* indptr, const CsrPrepared& P, const CsrKnnLayout& L, int64_t n,
+                 const QueryRange& qr, int32_t* ci, float* cv, cudaStream_t st) {
+  const dim3 grid((unsigned)((qr.hi - qr.base + sh.tm - 1) / sh.tm), (unsigned)qr.slices);
+  const int num_tiles = (int)(L.n_pad / sh.tn);
+  if (sh.kk == kKK) {
+    static bool attr_set = false;
+    if (!attr_set) {
+      MDE_CUDA_TRY(cudaFuncSetAttribute(knn_csr_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
+      attr_set = true;
+    }
+    knn_csr_tile_kernel<<<grid, kThreads, kSmemBytes, st>>>(indptr, P.cols, P.vals, P.norms, P.bm, L.nwords, n,
+                                                            num_tiles, qr, ci, cv);
+  } else if (sh.kk == kWideKK) {
+    constexpr int kSmem = kWideSmemBytes<kWideKK, kTileN>;
+    static bool attr_set = false;
+    if (!attr_set) {
+      MDE_CUDA_TRY(cudaFuncSetAttribute(knn_csr_wide_tile_kernel<kWideKK, kTileN>,
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+      attr_set = true;
+    }
+    knn_csr_wide_tile_kernel<kWideKK, kTileN><<<grid, 2 * kTileN, kSmem, st>>>(indptr, P.cols, P.vals, P.norms, P.bm,
+                                                                              L.nwords, n, num_tiles, qr, ci, cv);
+  } else {
+    constexpr int kSmem = kWideSmemBytes<kLongKK, kLongTileN>;
+    static bool attr_set = false;
+    if (!attr_set) {
+      MDE_CUDA_TRY(cudaFuncSetAttribute(knn_csr_wide_tile_kernel<kLongKK, kLongTileN>,
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+      attr_set = true;
+    }
+    knn_csr_wide_tile_kernel<kLongKK, kLongTileN><<<grid, 2 * kLongTileN, kSmem, st>>>(
+        indptr, P.cols, P.vals, P.norms, P.bm, L.nwords, n, num_tiles, qr, ci, cv);
+  }
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+
+// The exact re-rank of kk candidates per query row lo + r, 0 <= r < rows, into the compact outputs [rows][k].
+int launch_rerank(int kk, const int64_t* indptr, const CsrPrepared& P, int64_t lo, int64_t rows, const int32_t* ci,
+                  int k, int32_t* idx_out, float* d2_out, cudaStream_t st) {
+  const unsigned grid = (unsigned)((rows + 7) / 8);
+  if (kk == kKK)
+    knn_csr_rerank_kernel<<<grid, 256, 0, st>>>(indptr, P.cols, P.vals, lo, rows, ci, k, idx_out, d2_out);
+  else if (kk == kWideKK)
+    knn_csr_wide_rerank_kernel<<<grid, 256, 0, st>>>(indptr, P.cols, P.vals, lo, rows, ci, k, idx_out, d2_out);
+  else
+    knn_csr_long_rerank_kernel<<<grid, 256, 0, st>>>(indptr, P.cols, P.vals, lo, rows, ci, k, idx_out, d2_out);
+  MDE_LAUNCH_CHECK();
+  return 0;
+}
+
+bool bad_csr_args(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
+                  int k, int max_k, const void* idx_out, const void* d2_out, const void* ws) {
+  return !indptr || !idx_out || !d2_out || !ws || n < 2 || d < 1 || nnz < 0 || k < 1 || k > max_k || k > n - 1 ||
+         (nnz > 0 && (!indices || !values));
+}
+
+int csr_full_ws_bytes(int64_t n, int d, int64_t nnz, int kk, size_t* bytes) {
   if (!bytes || n < 2 || d < 1 || nnz < 0) return MDE_E_INVALID;
   CsrKnnLayout L;
   int rc = csr_knn_layout(n, d, nnz, &L, kk);
@@ -717,45 +898,63 @@ int csr_wide_ws_bytes(int64_t n, int d, int64_t nnz, int kk, size_t* bytes) {
   return 0;
 }
 
-// mde_knn_csr_wide (KK = 96, TN = 128) and mde_knn_csr_long (KK = 288, TN = 64): prep, tiles, re-rank of all KK.
-template <int KK, int TN>
-int run_csr_wide(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
-                 int k, int max_k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream) {
-  if (!indptr || !idx_out || !d2_out || !ws || n < 2 || d < 1 || nnz < 0 || k < 1 || k > max_k || k > n - 1)
-    return MDE_E_INVALID;
-  if (nnz > 0 && (!indices || !values)) return MDE_E_INVALID;
+// mde_knn_csr (k <= 24), mde_knn_csr_wide (k <= 64), mde_knn_csr_long (k <= 256): prep, the tiles of [0, n) in one
+// slice, re-rank of all KK candidates of every row.
+int run_csr_full(CsrShape sh, const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                 int64_t nnz, int k, int max_k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
+                 void* stream) {
+  if (bad_csr_args(indptr, indices, values, n, d, nnz, k, max_k, idx_out, d2_out, ws)) return MDE_E_INVALID;
   if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
   CsrKnnLayout L;
-  int rc = csr_knn_layout(n, d, nnz, &L, KK);
+  int rc = csr_knn_layout(n, d, nnz, &L, sh.kk);
   if (rc) return rc;
   if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   uint8_t* w = static_cast<uint8_t*>(ws);
   if ((rc = prepare_csr(indptr, indices, values, n, d, nnz, L, w, st))) return rc;
-  const float* norms = reinterpret_cast<const float*>(w + L.off_norm);
+  const CsrPrepared P = prepared(L, w);
   int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
   float* cv = reinterpret_cast<float*>(w + L.off_cv);
-  const uint32_t* bm = reinterpret_cast<const uint32_t*>(w + L.off_bm);
-  const int32_t* cols = reinterpret_cast<const int32_t*>(w + L.off_kin);
-  const float* vals = reinterpret_cast<const float*>(w + L.off_val);
-  constexpr int kSmem = kWideSmemBytes<KK, TN>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    MDE_CUDA_TRY(cudaFuncSetAttribute(knn_csr_wide_tile_kernel<KK, TN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      kSmem));
-    attr_set = true;
+  if ((rc = launch_tiles(sh, indptr, P, L, n, QueryRange{0, 0, n, 1}, ci, cv, st))) return rc;
+  return launch_rerank(sh.kk, indptr, P, 0, n, ci, k, idx_out, d2_out, st);
+}
+
+// mde_knn_csr_rows: prep of the whole matrix, the tiles of the query tiles only (in S candidate slices), the merge
+// of the S lists of a row when S > 1, re-rank.  Query tiles keep the full search's alignment (base: lo rounded down
+// to sh.tm), so that every (query tile, candidate tile) pair, and with it every score, is the full search's.
+int run_csr_rows(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
+                 int64_t lo, int64_t hi, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
+                 void* stream) {
+  if (bad_csr_args(indptr, indices, values, n, d, nnz, k, kLongMaxK, idx_out, d2_out, ws) || lo < 0 || hi > n ||
+      lo >= hi)
+    return MDE_E_INVALID;
+  if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
+  const CsrShape sh = csr_shape(k);
+  const int64_t rows = hi - lo;
+  const CsrRowsLayout R = csr_rows_layout(n, d, nnz, rows, sh);
+  if (ws_bytes < R.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
+  size_t sort_bytes = 0;
+  int rc = csr_sort_scratch(n, d, nnz, &sort_bytes);
+  if (rc) return rc;
+  if (sort_bytes > R.prep.tmp_bytes) return MDE_E_ALLOC;
+  cudaStream_t st = (cudaStream_t)stream;
+  uint8_t* w = static_cast<uint8_t*>(ws);
+  if ((rc = prepare_csr(indptr, indices, values, n, d, nnz, R.prep, w, st))) return rc;
+  const CsrPrepared P = prepared(R.prep, w);
+  int32_t* ci = reinterpret_cast<int32_t*>(w + R.off_ci);
+  float* cv = reinterpret_cast<float*>(w + R.off_cv);
+  const QueryRange qr{lo / sh.tm * sh.tm, lo, hi, R.slices};
+  if ((rc = launch_tiles(sh, indptr, P, R.prep, n, qr, ci, cv, st))) return rc;
+  const int32_t* lists = ci;
+  if (R.slices > 1) {
+    int32_t* sel = reinterpret_cast<int32_t*>(w + R.off_sel);
+    const int cands = R.slices * sh.kk;
+    knn_csr_merge_kernel<<<(unsigned)((rows + kMergeWarps - 1) / kMergeWarps), kMergeWarps * 32,
+                           (size_t)kMergeWarps * cands * 8, st>>>(rows, ci, cv, cands, sh.kk, sel);
+    MDE_LAUNCH_CHECK();
+    lists = sel;
   }
-  const unsigned grid = (unsigned)((n + kWideTileM - 1) / kWideTileM);
-  const int num_tiles = (int)(L.n_pad / TN);
-  knn_csr_wide_tile_kernel<KK, TN><<<grid, 2 * TN, kSmem, st>>>(indptr, cols, vals, norms, bm, L.nwords, n, num_tiles,
-                                                                ci, cv);
-  MDE_LAUNCH_CHECK();
-  if constexpr (KK == kWideKK)
-    knn_csr_wide_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(indptr, cols, vals, n, ci, k, idx_out, d2_out);
-  else
-    knn_csr_long_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(indptr, cols, vals, n, ci, k, idx_out, d2_out);
-  MDE_LAUNCH_CHECK();
-  return 0;
+  return launch_rerank(sh.kk, indptr, P, lo, rows, lists, k, idx_out, d2_out, st);
 }
 
 }  // namespace
@@ -763,64 +962,55 @@ int run_csr_wide(const int64_t* indptr, const int32_t* indices, const float* val
 extern "C" {
 
 int mde_knn_csr_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes) {
-  if (!bytes || n < 2 || d < 1 || nnz < 0) return MDE_E_INVALID;
-  CsrKnnLayout L;
-  int rc = csr_knn_layout(n, d, nnz, &L);
-  if (rc) return rc;
-  *bytes = L.total;
-  return 0;
+  return csr_full_ws_bytes(n, d, nnz, kKK, bytes);
 }
 
 int mde_knn_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
                 int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream) {
-  if (!indptr || !idx_out || !d2_out || !ws || n < 2 || d < 1 || nnz < 0 || k < 1 || k > kMaxK || k > n - 1)
-    return MDE_E_INVALID;
-  if (nnz > 0 && (!indices || !values)) return MDE_E_INVALID;
-  if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
-  CsrKnnLayout L;
-  int rc = csr_knn_layout(n, d, nnz, &L);
-  if (rc) return rc;
-  if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream;
-  uint8_t* w = static_cast<uint8_t*>(ws);
-  if ((rc = prepare_csr(indptr, indices, values, n, d, nnz, L, w, st))) return rc;
-  const float* norms = reinterpret_cast<const float*>(w + L.off_norm);
-  int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
-  float* cv = reinterpret_cast<float*>(w + L.off_cv);
-  const uint32_t* bm = reinterpret_cast<const uint32_t*>(w + L.off_bm);
-  const int32_t* cols = reinterpret_cast<const int32_t*>(w + L.off_kin);
-  const float* vals = reinterpret_cast<const float*>(w + L.off_val);
-  static bool attr_set = false;
-  if (!attr_set) {
-    MDE_CUDA_TRY(cudaFuncSetAttribute(knn_csr_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-    attr_set = true;
-  }
-  knn_csr_tile_kernel<<<(unsigned)L.num_tiles, kThreads, kSmemBytes, st>>>(indptr, cols, vals, norms, bm, L.nwords, n,
-                                                                           L.num_tiles, ci, cv);
-  MDE_LAUNCH_CHECK();
-  knn_csr_rerank_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(indptr, cols, vals, n, ci, k, idx_out, d2_out);
-  MDE_LAUNCH_CHECK();
-  return 0;
+  return run_csr_full(kCsrNarrow, indptr, indices, values, n, d, nnz, k, kMaxK, idx_out, d2_out, ws, ws_bytes,
+                      stream);
 }
 
 int mde_knn_csr_wide_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes) {
-  return csr_wide_ws_bytes(n, d, nnz, kWideKK, bytes);
+  return csr_full_ws_bytes(n, d, nnz, kWideKK, bytes);
 }
 
 int mde_knn_csr_wide(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                      int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream) {
-  return run_csr_wide<kWideKK, kTileN>(indptr, indices, values, n, d, nnz, k, kWideMaxK, idx_out, d2_out, ws, ws_bytes,
-                                       stream);
+  return run_csr_full(kCsrWide, indptr, indices, values, n, d, nnz, k, kWideMaxK, idx_out, d2_out, ws, ws_bytes,
+                      stream);
 }
 
 int mde_knn_csr_long_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes) {
-  return csr_wide_ws_bytes(n, d, nnz, kLongKK, bytes);
+  return csr_full_ws_bytes(n, d, nnz, kLongKK, bytes);
 }
 
 int mde_knn_csr_long(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                      int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream) {
-  return run_csr_wide<kLongKK, kLongTileN>(indptr, indices, values, n, d, nnz, k, kLongMaxK, idx_out, d2_out, ws,
-                                           ws_bytes, stream);
+  return run_csr_full(kCsrLong, indptr, indices, values, n, d, nnz, k, kLongMaxK, idx_out, d2_out, ws, ws_bytes,
+                      stream);
+}
+
+int mde_knn_csr_rows_ws_bytes(int64_t n, int d, int64_t nnz, int64_t rows, int k, size_t* bytes) {
+  if (!bytes || n < 2 || d < 1 || nnz < 0 || rows < 1 || rows > n || k < 1 || k > kLongMaxK || k > n - 1)
+    return MDE_E_INVALID;
+  *bytes = csr_rows_layout(n, d, nnz, rows, csr_shape(k)).total;
+  return 0;
+}
+
+int mde_knn_csr_rows(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                     int64_t nnz, int64_t row_begin, int64_t row_end, int k, int32_t* idx_out, float* d2_out, void* ws,
+                     size_t ws_bytes, void* stream) {
+  return run_csr_rows(indptr, indices, values, n, d, nnz, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes,
+                      stream);
+}
+
+// host-side debug entry point: the candidate slices (mde_logic.h: knn_slices) of mde_knn_csr_rows for `rows` query
+// rows against n rows with k neighbours (narrow tiles up to k = 24, wide up to 64, long, in one slice, up to 256);
+// -1 for bad arguments
+int mde_dbg_knn_csr_slices(int64_t n, int64_t rows, int k) {
+  if (n < 2 || rows < 1 || rows > n || k < 1 || k > kLongMaxK) return -1;
+  return csr_search_slices(n, rows, csr_shape(k));
 }
 
 int mde_pair_dist_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,

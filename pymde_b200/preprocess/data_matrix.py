@@ -27,9 +27,9 @@ and certify every row, searching the rows that fail directly (DESIGN section 11)
 candidates with fp64 matmuls of the centred matrix, independent of torch's TF32 setting, then re-ranks them by fp32
 distance and index.
 
-`knn_rows_device` searches only a range of rows against all rows (`mde_knn_rows`, `mde_knn16_rows`), exactly, at a
-cost that scales with the rows searched: `pymde_b200.embed_new_points` searches the new rows of a stacked matrix with
-it (DESIGN section 11.8)."""
+`knn_rows_device` searches only a range of rows against all rows (`mde_knn_rows`, `mde_knn16_rows`, and
+`mde_knn_csr_rows` for a scipy.sparse matrix), exactly, at a cost that scales with the rows searched:
+`pymde_b200.embed_new_points` searches the new rows of a stacked matrix with it (DESIGN section 11.8)."""
 import ctypes as C
 import os
 
@@ -101,6 +101,34 @@ def knn_sparse_device(csr, shape, k):
         stream = torch.cuda.current_stream().cuda_stream
         _lib.check(search(indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), int(n), int(d), nnz, int(k),
                           idx.data_ptr(), d2.data_ptr(), ws.data_ptr() + off, need.value, stream))
+        torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
+    return idx, d2
+
+
+def knn_sparse_rows_device(csr, shape, k, row_begin, row_end):
+    """(indices [r, k] int32, squared distances [r, k] fp32), r = row_end - row_begin: row r of the result is row
+    row_begin + r of `knn_sparse_device` on the same device CSR matrix and k, bit for bit, ties included
+    (`mde_knn_csr_rows`, include/mde_b200.h; 1 <= k <= 256).  The tiles sweep only the query rows, so the cost of the
+    search proper scales with r n rather than n^2; the preparation still covers the whole matrix."""
+    from .. import _lib
+    lib = _lib.load()
+    indptr, indices, values = csr
+    n, d = int(shape[0]), int(shape[1])
+    row_begin, row_end, k = int(row_begin), int(row_end), int(k)
+    nnz = int(indices.shape[0])
+    dev = indptr.device
+    r = row_end - row_begin
+    need = C.c_size_t(0)
+    _lib.check(lib.mde_knn_csr_rows_ws_bytes(n, d, nnz, r, k, C.byref(need)))
+    ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=dev)
+    off = (-ws.data_ptr()) % 1024
+    idx = torch.empty((r, k), dtype=torch.int32, device=dev)
+    d2 = torch.empty((r, k), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        stream = torch.cuda.current_stream().cuda_stream
+        _lib.check(lib.mde_knn_csr_rows(indptr.data_ptr(), indices.data_ptr(), values.data_ptr(), n, d, nnz,
+                                        row_begin, row_end, k, idx.data_ptr(), d2.data_ptr(), ws.data_ptr() + off,
+                                        need.value, stream))
         torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
     return idx, d2
 
@@ -192,8 +220,9 @@ def knn_rows_device(X, k, row_begin, row_end):
         for bit the rows of `knn_device`, at a cost of about r n d rather than n^2 d (other float dtypes are searched
         in fp32);
       * a dense matrix with k > 64: the row range of `_gemm_search` (int64 indices), the rows it gives on all of X;
-      * a scipy.sparse matrix: the whole matrix is searched with `knn_sparse_device` (k <= 256; above that the GEMM
-        path on the dense matrix) and the rows are sliced out.  Exact, but it costs the full search."""
+      * a scipy.sparse matrix with k <= 256: `knn_sparse_rows_device` (`mde_knn_csr_rows`, int32 indices), bit for
+        bit the rows of `knn_sparse_device`, at a cost of about r n rather than n^2 in the tiles, without densifying;
+      * a scipy.sparse matrix with k > 256: the row range of `_gemm_search` on the dense matrix."""
     from .. import _lib
     lib = _lib.load()
     n = int(X.shape[0])
@@ -206,8 +235,7 @@ def knn_rows_device(X, k, row_begin, row_end):
         dev = util.cuda_device()
         if k > lib.mde_knn_long_max_k():
             return _gemm_search(_to_device_matrix(X, dev), k, row_begin=row_begin, row_end=row_end)
-        idx, d2 = knn_sparse_device(*_to_device_csr(X, dev), k)
-        return idx[row_begin:row_end].contiguous(), d2[row_begin:row_end].contiguous()
+        return knn_sparse_rows_device(*_to_device_csr(X, dev), k, row_begin, row_end)
     if X.dtype not in _HALF_DTYPES:
         X = X.float()
     X = X.contiguous()

@@ -292,7 +292,9 @@ def embed_new_points(data, embedding, new_data, n_neighbors=None, attractive_pen
         neighbours' rows (the column mean of `embedding` when it has none);
       * the anchored problem is solved on the device (`MDE.embed(eps, max_iter)`).
     `data` and `new_data` are dense (numpy, torch; fp32, or float16 / bfloat16 searched in place) or scipy.sparse
-    matrices with the same columns; a Graph is not supported."""
+    matrices with the same columns; a Graph is not supported.  Sparse input is stacked on the host and searched
+    without densifying it (`mde_knn_csr_rows`, k <= 256): the tiles sweep only the new rows, and the result is that
+    of the full sparse search."""
     mde, _ = _new_points_mde(data, embedding, new_data, n_neighbors=n_neighbors,
                              attractive_penalty=attractive_penalty, repulsive_penalty=repulsive_penalty,
                              repulsive_fraction=repulsive_fraction, max_distance=max_distance, device=device)
