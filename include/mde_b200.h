@@ -358,14 +358,23 @@ int mde_knn_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, float*
  * indices[nnz] strictly increasing within a row and below d, fp32 values[nnz]; nnz may exceed 2^31.  Output contract
  * of mde_knn, except that the distances are the exact squared distances summed in fp64 and rounded once to fp32, and
  * the k rows are the k smallest (distance, index) pairs in lexicographic order: the result is fully determined,
- * ties included.  Cross terms run on the tensor cores over the 64-feature blocks both tiles occupy (features ordered
- * by descending document frequency); nothing n x d sized is allocated.  1 <= k <= mde_knn_max_k() (24),
- * k <= n - 1.  `ws`: 1024-byte aligned device scratch of mde_knn_csr_ws_bytes(n, d, nnz) bytes (about 20 bytes per
- * non-zero and 260 per row, plus 20 per feature and the sort's scratch).  MDE_E_INVALID also when the CSR is malformed (checked on the device).
- * Blocking (one status read after the check). */
+ * ties included, whatever the offset or clustering of the data.  Cross terms run on the tensor cores over the
+ * 64-feature blocks both tiles occupy (features ordered by descending document frequency); nothing n x d sized is
+ * allocated, and the columns are not centred (that would densify the matrix).  A per-row certificate (a bound on the
+ * scores' error in terms of the row's non-zeros, over the rows near enough to enter its list) shows that no other row
+ * can enter the list; a row that fails it is searched directly over all n rows with the re-rank's sorted merge.
+ * 1 <= k <= mde_knn_max_k() (24), k <= n - 1.  `ws`: 1024-byte aligned device scratch of
+ * mde_knn_csr_ws_bytes(n, d, nnz) bytes (about 20 bytes per non-zero and 264 per row, plus 20 per feature and the
+ * sort's scratch).  MDE_E_INVALID also when the CSR is malformed (checked on the device).  Blocking (one status read
+ * after the check).  mde_knn_csr_ex also writes the number of rows searched directly to *fallback_rows (nullable;
+ * when not null the call waits for the stream), as do mde_knn_csr_wide_ex, mde_knn_csr_long_ex and
+ * mde_knn_csr_rows_ex below. */
 int mde_knn_csr_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes);
 int mde_knn_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
                 int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream);
+int mde_knn_csr_ex(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
+                   int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream,
+                   int* fallback_rows);
 /* The same two searches for 1 <= k <= mde_knn_wide_max_k() (64), k <= n - 1: arguments, output contract, tie rules
  * and return codes of mde_knn and mde_knn_csr (the CSR check included).  A running top-96 per row, kept in shared
  * memory, feeds the exact re-rank.  For k <= 24 the result is that of mde_knn / mde_knn_csr, which remain the faster
@@ -381,6 +390,9 @@ int mde_knn_wide_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, f
 int mde_knn_csr_wide_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes);
 int mde_knn_csr_wide(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                      int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream);
+int mde_knn_csr_wide_ex(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                        int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream,
+                        int* fallback_rows);
 /* The same two searches for 1 <= k <= mde_knn_long_max_k() (256), k <= n - 1: arguments, output contract, tie rules,
  * CSR check and return codes of mde_knn_wide and mde_knn_csr_wide.  A running top-288 per row feeds the exact
  * re-rank.  For k <= 64 the result is that of mde_knn_wide (the same distance bits; indices may differ only inside
@@ -396,6 +408,9 @@ int mde_knn_long_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, f
 int mde_knn_csr_long_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes);
 int mde_knn_csr_long(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                      int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream);
+int mde_knn_csr_long_ex(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                        int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream,
+                        int* fallback_rows);
 /* APPROXIMATE k-nearest neighbours of a dense matrix by NN-descent, for n too large for the exact O(n^2 d) search.
  * Output contract of mde_knn with "the k nearest rows" replaced by "k rows found by the search": k distinct rows per
  * row, never the row itself, ascending by (squared distance, index), with the exact fp32 squared distances of the
@@ -473,7 +488,8 @@ int mde_knn16_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin
  * cannot fill the SMs the candidate sweep of the narrow and wide searches is split into S slices (one CTA per query
  * tile and slice; S from the tile counts alone).  A row's S lists are merged by taking their KK smallest pairs in the
  * tiles' own (approximate score, index) order, which are exactly the full search's KK candidates, before the exact
- * re-rank.  Input contract, CSR check and return codes of mde_knn_csr (a malformed CSR is MDE_E_INVALID);
+ * re-rank; the certificate takes the worst of those KK scores, as the full search does, so both search the same rows
+ * directly.  Input contract, CSR check and return codes of mde_knn_csr (a malformed CSR is MDE_E_INVALID);
  * 0 <= row_begin < row_end <= n, 1 <= k <= 256, k <= n - 1; a bad argument or a workspace too small or not 1024-byte
  * aligned is MDE_E_INVALID before any CUDA call.  `ws`: 1024-byte aligned device scratch of
  * mde_knn_csr_rows_ws_bytes(n, d, nnz, rows, k) bytes (host arithmetic alone: the preparation's, with a bound on the
@@ -483,6 +499,9 @@ int mde_knn_csr_rows_ws_bytes(int64_t n, int d, int64_t nnz, int64_t rows, int k
 int mde_knn_csr_rows(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                      int64_t nnz, int64_t row_begin, int64_t row_end, int k, int32_t* idx_out, float* d2_out, void* ws,
                      size_t ws_bytes, void* stream);
+int mde_knn_csr_rows_ex(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                        int64_t nnz, int64_t row_begin, int64_t row_end, int k, int32_t* idx_out, float* d2_out,
+                        void* ws, size_t ws_bytes, void* stream, int* fallback_rows);
 /* The same NN-descent search on a sparse data matrix, without densifying it.  Input contract of mde_knn_csr (the
  * device CSR check included: MDE_E_INVALID when malformed); output contract of mde_knn_approx, with the distances of
  * mde_knn_csr / mde_knn_csr_wide: the exact squared distance summed in fp64 and rounded once to fp32, which is also

@@ -120,6 +120,8 @@ SIGNATURES = {
     "mde_knn_csr_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.POINTER(C.c_size_t)]),
     "mde_knn_csr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int, C.c_void_p,
                               C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn_csr_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int,
+                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
     "mde_knn_wide_max_k": (C.c_int, []),
     "mde_knn_wide_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn_wide": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -129,6 +131,8 @@ SIGNATURES = {
     "mde_knn_csr_wide_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.POINTER(C.c_size_t)]),
     "mde_knn_csr_wide": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn_csr_wide_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
     "mde_knn_long_max_k": (C.c_int, []),
     "mde_knn_long_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn_long": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -138,6 +142,8 @@ SIGNATURES = {
     "mde_knn_csr_long_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.POINTER(C.c_size_t)]),
     "mde_knn_csr_long": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn_csr_long_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
     "mde_knn_approx_max_k": (C.c_int, []),
     "mde_knn_approx_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn_approx": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_void_p, C.c_void_p,
@@ -169,6 +175,9 @@ SIGNATURES = {
                                             C.POINTER(C.c_size_t)]),
     "mde_knn_csr_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int64,
                                    C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn_csr_rows_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int64,
+                                      C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                      C.POINTER(C.c_int)]),
     "mde_knn16_approx_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn16_approx": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

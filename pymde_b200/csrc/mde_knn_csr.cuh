@@ -10,11 +10,12 @@
 
 namespace mde {
 
-// Workspace of the preparation (and of the exact searches' candidate lists, kk per row), 1024-byte aligned offsets.
+// Workspace of the preparation (and of the exact searches' candidate lists, kk per row, and their certificate: a
+// header and n row ids, at the end), 1024-byte aligned offsets.
 struct CsrKnnLayout {
   int64_t n_pad; int num_tiles, nwords, row_bits, col_bits;
   size_t off_flag, off_norm, off_ci, off_cv, off_cnt, off_cnt_s, off_iota, off_col_s, off_perm, off_bm, off_kin,
-      off_kout, off_val, off_tmp, tmp_bytes, total;
+      off_kout, off_val, off_tmp, tmp_bytes, off_hdr, off_rows, total;
 };
 
 // Scratch bytes of the two CUB radix sorts of prepare_csr: a query that needs a device but does no device work.
@@ -24,7 +25,7 @@ int csr_sort_scratch(int64_t n, int d, int64_t nnz, size_t* bytes);
 // histograms.  A search sized by it checks csr_sort_scratch against it before it starts.
 size_t csr_sort_scratch_bound(int d, int64_t nnz);
 // The layout for a given sort scratch (host arithmetic only).  kk: candidates kept per row (kNarrowKK, or kWideKK for
-// the wide search; 0 when the caller keeps its own lists elsewhere).
+// the wide search; 0 when the caller keeps its own lists, and its own certificate state, elsewhere).
 void csr_knn_carve(int64_t n, int d, int64_t nnz, int kk, size_t tmp_bytes, CsrKnnLayout* L);
 // csr_knn_carve with the scratch csr_sort_scratch reports.
 int csr_knn_layout(int64_t n, int d, int64_t nnz, CsrKnnLayout* L, int kk = kNarrowKK);

@@ -600,13 +600,13 @@ namespace {
 // search's candidates.  Re-ranking the whole union instead could return a better list than the full search's.
 // One warp per query row r stages the row's S KK pairs in shared memory, ranks each among all of them (equal pairs,
 // only ever empty slots, by slot) and writes those of rank < KK to sel[r][rank], -1 for empty; the re-rank kernels
-// then take sel as the full search's lists.
+// then take sel as the full search's lists, and the certificate takes sel_val, their scores, as the full search's.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int kMergeWarps = 4;
 
 __global__ void __launch_bounds__(kMergeWarps * 32)
 knn_csr_merge_kernel(int64_t rows, const int32_t* __restrict__ cand_idx, const float* __restrict__ cand_val,
-                     int cands, int kk, int32_t* __restrict__ sel) {
+                     int cands, int kk, int32_t* __restrict__ sel, float* __restrict__ sel_val) {
   extern __shared__ float s_merge[];  // per warp: scores [cands], indices [cands]
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int64_t r = (int64_t)blockIdx.x * kMergeWarps + warp;
@@ -628,7 +628,147 @@ knn_csr_merge_kernel(int64_t rows, const int32_t* __restrict__ cand_idx, const f
       const int iq = si[q];
       rank += before(dq, iq, dj, ij) || (q < j && !before(dj, ij, dq, iq));
     }
-    if (rank < kk) sel[r * kk + rank] = ij == INT_MAX ? -1 : ij;
+    if (rank < kk) {
+      sel[r * kk + rank] = ij == INT_MAX ? -1 : ij;
+      sel_val[r * kk + rank] = dj;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// certificate: is the re-ranked list of a row the k smallest (distance, index) over ALL rows?
+//
+// The tiles rank candidate x of query q by s(x) = fl(||x||^2~ - 2 <q, x>~): the fp32 norm (the fp64 sum rounded once)
+// and the cross term of the bf16 hi / lo split accumulated in fp32.  S(x) = ||x||^2 - 2 <q, x> is its exact value, so
+// ||q - x||^2 = S(x) + ||q||^2.  For every x with ||x|| <= R, |s(x) - S(x)| <= E(q), and the fp32 norm of q lies
+// within E(q) of ||q||^2, with
+//   E(q) = sigma (2 (a_cross |q| R + eta (|q| + R)) + a_norm R^2 + a_abs),
+//   a_cross  the split (the dropped lo x lo term and the split residuals, 3.1 2^-16), the fp32 accumulation of
+//            m = 3 nnz(q) products (2 u per addition, u = 2^-24, allowing truncating tensor-core adds; a product with a
+//            zero element of q is an exact zero, and adding an exact zero adds no error) and the score's fma (u),
+//   eta      bf16 subnormals of the split, flushed or not: 2^-126 sqrt(nnz(q)) (an absolute error per element),
+//   a_norm   the fp64 sum of at most d squares and its fp32 rounding (u + (d + 6) 2^-53) and the score's fma (u),
+//   a_abs    underflow: 2^-126 per product, 2^-149 per norm,
+// and sigma = 2, a safety factor for second-order terms (tests/test_knn_csr_offset_cpu.py derives the bound).  None of
+// these depends on d through the products, so a row of a 10^5-feature matrix certifies as one of 100 features does.
+//
+// R need not cover every row: a row x can enter the list only if its fp32 distance is at most d2_k, the k-th re-ranked
+// one, so that ||x|| <= ||q|| + ||q - x|| <= R = sqrt((qn + 2^-149) / (1 - a_norm)) + sqrt((d2_k + 2^-149) /
+// (1 - delta)) (qn: the fp32 norm of q; slack 2^-40 for the fp64 arithmetic).  A few long rows elsewhere in the matrix
+// therefore cost nothing, and R^2 < 2^125 keeps every score of a row within R finite (otherwise the row fails).
+//
+// Every row the tiles did not keep scored at least t, the KK-th kept score (+inf when the list was never filled:
+// every row was kept).  A search in S candidate slices takes t from the merged list, which is the full search's list,
+// so both make the same decision.  A row not kept with ||x|| <= R lies at an exact distance D >= t - E + qn - E; when
+// that exceeds (d2_k + 2^-149) (1 + delta) / (1 - delta), delta = u + (d + 2) 2^-53 bounding the re-rank's relative
+// rounding, its fp32 distance exceeds d2_k and it cannot enter the list.  A row that fails (NaN and +inf included) is
+// searched directly (knn_csr_direct_kernel); a false failure costs time only.  The uncertified rows are appended to
+// rows[] (in no particular order: each is searched on its own) and counted in the header.
+// ---------------------------------------------------------------------------------------------------------------
+enum { kCertCount, kCertHdrWords };
+constexpr double kCertSafety = 2.0;
+
+__global__ void __launch_bounds__(256)
+knn_csr_certify_kernel(const int64_t* __restrict__ indptr, const float* __restrict__ cand_val, int kk,
+                       const float* __restrict__ norms, const float* __restrict__ d2_out, int k, int64_t lo,
+                       int64_t rows, int d, unsigned* __restrict__ hdr, int32_t* __restrict__ uncert) {
+  const int lane = threadIdx.x & 31;
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);  // of the query range
+  if (row >= rows) return;
+  float t = -kInf;
+  for (int q = lane; q < kk; q += 32) t = fmaxf(t, cand_val[row * kk + q]);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) t = fmaxf(t, __shfl_xor_sync(kFull, t, o));
+  if (lane) return;
+  const double u = 0x1p-24, tiny = 0x1p-149;
+  const double m = 3.0 * (double)(indptr[lo + row + 1] - indptr[lo + row]);
+  const double a_cross = 3.1 * 0x1p-16 + 2.0 * u * m + u;
+  const double eta = 0x1p-126 * sqrt(m / 3.0);
+  const double a_norm = 2.0 * u + (d + 6.0) * 0x1p-53;
+  const double a_abs = 2.0 * m * 0x1p-126 + 2.0 * tiny;
+  const double delta = u + (d + 2.0) * 0x1p-53;
+  const double qn = (double)norms[lo + row], d2k = (double)d2_out[row * k + k - 1];
+  const double qa = sqrt((qn + tiny) / (1.0 - a_norm)) * (1.0 + 0x1p-40);
+  const double R = qa + sqrt((d2k + tiny) / (1.0 - delta)) * (1.0 + 0x1p-40);
+  const double E = kCertSafety * (2.0 * (a_cross * qa * R + eta * (qa + R)) + a_norm * R * R + a_abs);
+  const double lhs = (d2k + tiny) * (1.0 + delta) / (1.0 - delta) - qn + E;
+  if (!(lhs < (double)t - E) || !(R * R < 0x1p125))
+    uncert[atomicAdd(reinterpret_cast<int*>(hdr + kCertCount), 1)] = (int32_t)row;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// direct search of the uncertified rows (row r of the query range is row lo + r): one warp per row sweeps all n rows,
+// 32 at a time, one candidate per lane, with the re-rank's merge_dist2 (a function of the unordered pair: the re-rank's
+// bits), and keeps the k smallest (distance, index) pairs, ascending.  Only pairs up to the re-rank's k-th pair can
+// belong (the re-rank's k rows are k candidates with these very distances), which keeps insertions rare.
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+knn_csr_direct_kernel(const int64_t* __restrict__ indptr, const int32_t* __restrict__ cols,
+                      const float* __restrict__ vals, int64_t n, int k, int64_t lo,
+                      const unsigned* __restrict__ hdr, const int32_t* __restrict__ uncert,
+                      int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+  __shared__ float s_d[8][kLongMaxK];
+  __shared__ int s_i[8][kLongMaxK];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t slot = (int64_t)blockIdx.x * 8 + warp;
+  if (slot >= (int64_t)hdr[kCertCount]) return;
+  const int64_t row = uncert[slot], q = lo + row;
+  float* ld = s_d[warp];
+  int* li = s_i[warp];
+  for (int j = lane; j < k; j += 32) { ld[j] = kInf; li[j] = INT_MAX; }
+  __syncwarp();
+  const float bd = out_d2[row * k + k - 1];
+  const int bi = out_idx[row * k + k - 1];
+  float thr = kInf;
+  int thi = INT_MAX, worst = 0;
+  for (int64_t c0 = 0; c0 < n; c0 += 32) {
+    const int64_t c = c0 + lane;
+    float dist = kInf;
+    // at most the re-rank's k-th pair
+    bool offer = c < n && c != q;
+    if (offer) {
+      dist = (float)merge_dist2(indptr, cols, vals, q, c);
+      offer = !before(bd, bi, dist, (int)c);
+    }
+    // the offers of this chunk in index order, each against the worst kept pair (warp-uniform)
+    for (unsigned b = __ballot_sync(kFull, offer); b; b &= b - 1) {
+      const int src = __ffs(b) - 1;
+      const float od = __shfl_sync(kFull, dist, src);
+      const int oi = (int)(c0 + src);
+      if (!before(od, oi, thr, thi)) continue;
+      if (lane == 0) { ld[worst] = od; li[worst] = oi; }
+      __syncwarp();
+      // the new worst: the largest (distance, index, slot) of the list
+      float mx = -kInf; int mi = INT_MIN, w = -1;
+      for (int j = lane; j < k; j += 32) {
+        if (before(mx, mi, ld[j], li[j]) || (mx == ld[j] && mi == li[j])) { mx = ld[j]; mi = li[j]; w = j; }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const float om = __shfl_xor_sync(kFull, mx, o);
+        const int omi = __shfl_xor_sync(kFull, mi, o), ow = __shfl_xor_sync(kFull, w, o);
+        if (before(mx, mi, om, omi) || (mx == om && mi == omi && ow > w)) { mx = om; mi = omi; w = ow; }
+      }
+      thr = mx; thi = mi; worst = w;
+      __syncwarp();
+    }
+  }
+  // ascending by (distance, index): the rank of every slot among the k
+  int rank[kLongMaxK / 32];
+#pragma unroll
+  for (int s = 0; s < kLongMaxK / 32; ++s) {
+    const int j = lane + 32 * s;
+    rank[s] = 0;
+    if (j < k) for (int p = 0; p < k; ++p) rank[s] += before(ld[p], li[p], ld[j], li[j]);
+  }
+  __syncwarp();
+#pragma unroll
+  for (int s = 0; s < kLongMaxK / 32; ++s) {
+    const int j = lane + 32 * s;
+    if (j < k) {
+      out_idx[row * k + rank[s]] = li[j];
+      out_d2[row * k + rank[s]] = ld[j];
+    }
   }
 }
 
@@ -707,6 +847,11 @@ void csr_knn_carve(int64_t n, int d, int64_t nnz, int kk, size_t tmp_bytes, CsrK
   L->off_kout = o; o = up(o + (size_t)nnz * 8);
   L->off_val = o; o = up(o + (size_t)nnz * 4);
   L->off_tmp = o; o = up(o + L->tmp_bytes);
+  L->off_hdr = L->off_rows = 0;
+  if (kk > 0) {
+    L->off_hdr = o; o = up(o + 4 * kCertHdrWords);  // the certificate's header
+    L->off_rows = o; o = up(o + (size_t)n * 4);     // the uncertified rows
+  }
   L->total = o;
 }
 
@@ -791,13 +936,13 @@ int csr_search_slices(int64_t n, int64_t rows, CsrShape sh) {
 
 // mde_knn_csr_rows: prepare_csr's workspace (without candidate lists, its sort scratch reserved as
 // csr_sort_scratch_bound, so that the size is host arithmetic alone), then the lists of the query rows, S per row,
-// and the KK candidates per row the merge selects.  The lists take room for rows, or, when the rule may split, the
+// the KK candidates per row the merge selects with their scores, and the certificate's header and row ids.  The lists take room for rows, or, when the rule may split, the
 // most a split can hold (q_tiles S <= kNumSMs, S <= kMaxSlices): a workspace sized for a search fits every search of
 // fewer rows, and grows with n.
 struct CsrRowsLayout {
   CsrKnnLayout prep;
   int slices;
-  size_t off_ci, off_cv, off_sel, total;
+  size_t off_ci, off_cv, off_sel, off_selv, off_hdr, off_rows, total;
 };
 
 CsrRowsLayout csr_rows_layout(int64_t n, int d, int64_t nnz, int64_t rows, CsrShape sh) {
@@ -814,6 +959,9 @@ CsrRowsLayout csr_rows_layout(int64_t n, int d, int64_t nnz, int64_t rows, CsrSh
   R.off_ci = o; o = up(o + (size_t)cap * sh.kk * 4);
   R.off_cv = o; o = up(o + (size_t)cap * sh.kk * 4);
   R.off_sel = o; o = up(o + (size_t)rows * sh.kk * 4);
+  R.off_selv = o; o = up(o + (size_t)rows * sh.kk * 4);     // their scores, for the certificate
+  R.off_hdr = o; o = up(o + 4 * kCertHdrWords);             // the certificate's header
+  R.off_rows = o; o = up(o + (size_t)rows * 4);             // the uncertified rows
   R.total = o;
   return R;
 }
@@ -883,6 +1031,24 @@ int launch_rerank(int kk, const int64_t* indptr, const CsrPrepared& P, int64_t l
   return 0;
 }
 
+// After the re-rank of the query rows lo + r, 0 <= r < rows: certify every row against its kk kept scores cv[r][.],
+// search the uncertified rows directly; with `fallback_rows`, wait for the stream and report how many rows that was.
+int certify_direct(const int64_t* indptr, const CsrPrepared& P, int64_t n, int d, int64_t lo, int64_t rows, int kk,
+                   const float* cv, int k, int32_t* idx_out, float* d2_out, unsigned* hdr, int32_t* uncert,
+                   cudaStream_t st, int* fallback_rows) {
+  MDE_CUDA_TRY(cudaMemsetAsync(hdr, 0, 4 * kCertHdrWords, st));
+  const unsigned grid = (unsigned)((rows + 7) / 8);
+  knn_csr_certify_kernel<<<grid, 256, 0, st>>>(indptr, cv, kk, P.norms, d2_out, k, lo, rows, d, hdr, uncert);
+  MDE_LAUNCH_CHECK();
+  knn_csr_direct_kernel<<<grid, 256, 0, st>>>(indptr, P.cols, P.vals, n, k, lo, hdr, uncert, idx_out, d2_out);
+  MDE_LAUNCH_CHECK();
+  if (fallback_rows) {
+    MDE_CUDA_TRY(cudaMemcpyAsync(fallback_rows, hdr + kCertCount, sizeof(int), cudaMemcpyDeviceToHost, st));
+    MDE_CUDA_TRY(cudaStreamSynchronize(st));
+  }
+  return 0;
+}
+
 bool bad_csr_args(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
                   int k, int max_k, const void* idx_out, const void* d2_out, const void* ws) {
   return !indptr || !idx_out || !d2_out || !ws || n < 2 || d < 1 || nnz < 0 || k < 1 || k > max_k || k > n - 1 ||
@@ -902,7 +1068,7 @@ int csr_full_ws_bytes(int64_t n, int d, int64_t nnz, int kk, size_t* bytes) {
 // slice, re-rank of all KK candidates of every row.
 int run_csr_full(CsrShape sh, const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                  int64_t nnz, int k, int max_k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
-                 void* stream) {
+                 void* stream, int* fallback_rows) {
   if (bad_csr_args(indptr, indices, values, n, d, nnz, k, max_k, idx_out, d2_out, ws)) return MDE_E_INVALID;
   if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
   CsrKnnLayout L;
@@ -916,7 +1082,10 @@ int run_csr_full(CsrShape sh, const int64_t* indptr, const int32_t* indices, con
   int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
   float* cv = reinterpret_cast<float*>(w + L.off_cv);
   if ((rc = launch_tiles(sh, indptr, P, L, n, QueryRange{0, 0, n, 1}, ci, cv, st))) return rc;
-  return launch_rerank(sh.kk, indptr, P, 0, n, ci, k, idx_out, d2_out, st);
+  if ((rc = launch_rerank(sh.kk, indptr, P, 0, n, ci, k, idx_out, d2_out, st))) return rc;
+  return certify_direct(indptr, P, n, d, 0, n, sh.kk, cv, k, idx_out, d2_out,
+                        reinterpret_cast<unsigned*>(w + L.off_hdr), reinterpret_cast<int32_t*>(w + L.off_rows), st,
+                        fallback_rows);
 }
 
 // mde_knn_csr_rows: prep of the whole matrix, the tiles of the query tiles only (in S candidate slices), the merge
@@ -924,7 +1093,7 @@ int run_csr_full(CsrShape sh, const int64_t* indptr, const int32_t* indices, con
 // to sh.tm), so that every (query tile, candidate tile) pair, and with it every score, is the full search's.
 int run_csr_rows(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
                  int64_t lo, int64_t hi, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
-                 void* stream) {
+                 void* stream, int* fallback_rows) {
   if (bad_csr_args(indptr, indices, values, n, d, nnz, k, kLongMaxK, idx_out, d2_out, ws) || lo < 0 || hi > n ||
       lo >= hi)
     return MDE_E_INVALID;
@@ -946,15 +1115,21 @@ int run_csr_rows(const int64_t* indptr, const int32_t* indices, const float* val
   const QueryRange qr{lo / sh.tm * sh.tm, lo, hi, R.slices};
   if ((rc = launch_tiles(sh, indptr, P, R.prep, n, qr, ci, cv, st))) return rc;
   const int32_t* lists = ci;
+  const float* scores = cv;
   if (R.slices > 1) {
     int32_t* sel = reinterpret_cast<int32_t*>(w + R.off_sel);
+    float* sel_val = reinterpret_cast<float*>(w + R.off_selv);
     const int cands = R.slices * sh.kk;
     knn_csr_merge_kernel<<<(unsigned)((rows + kMergeWarps - 1) / kMergeWarps), kMergeWarps * 32,
-                           (size_t)kMergeWarps * cands * 8, st>>>(rows, ci, cv, cands, sh.kk, sel);
+                           (size_t)kMergeWarps * cands * 8, st>>>(rows, ci, cv, cands, sh.kk, sel, sel_val);
     MDE_LAUNCH_CHECK();
     lists = sel;
+    scores = sel_val;
   }
-  return launch_rerank(sh.kk, indptr, P, lo, rows, lists, k, idx_out, d2_out, st);
+  if ((rc = launch_rerank(sh.kk, indptr, P, lo, rows, lists, k, idx_out, d2_out, st))) return rc;
+  return certify_direct(indptr, P, n, d, lo, rows, sh.kk, scores, k, idx_out, d2_out,
+                        reinterpret_cast<unsigned*>(w + R.off_hdr), reinterpret_cast<int32_t*>(w + R.off_rows), st,
+                        fallback_rows);
 }
 
 }  // namespace
@@ -965,30 +1140,48 @@ int mde_knn_csr_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes) {
   return csr_full_ws_bytes(n, d, nnz, kKK, bytes);
 }
 
+int mde_knn_csr_ex(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
+                   int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream,
+                   int* fallback_rows) {
+  return run_csr_full(kCsrNarrow, indptr, indices, values, n, d, nnz, k, kMaxK, idx_out, d2_out, ws, ws_bytes,
+                      stream, fallback_rows);
+}
+
 int mde_knn_csr(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d, int64_t nnz,
                 int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream) {
-  return run_csr_full(kCsrNarrow, indptr, indices, values, n, d, nnz, k, kMaxK, idx_out, d2_out, ws, ws_bytes,
-                      stream);
+  return mde_knn_csr_ex(indptr, indices, values, n, d, nnz, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
 int mde_knn_csr_wide_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes) {
   return csr_full_ws_bytes(n, d, nnz, kWideKK, bytes);
 }
 
+int mde_knn_csr_wide_ex(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                        int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream,
+                        int* fallback_rows) {
+  return run_csr_full(kCsrWide, indptr, indices, values, n, d, nnz, k, kWideMaxK, idx_out, d2_out, ws, ws_bytes,
+                      stream, fallback_rows);
+}
+
 int mde_knn_csr_wide(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                      int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream) {
-  return run_csr_full(kCsrWide, indptr, indices, values, n, d, nnz, k, kWideMaxK, idx_out, d2_out, ws, ws_bytes,
-                      stream);
+  return mde_knn_csr_wide_ex(indptr, indices, values, n, d, nnz, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
 int mde_knn_csr_long_ws_bytes(int64_t n, int d, int64_t nnz, size_t* bytes) {
   return csr_full_ws_bytes(n, d, nnz, kLongKK, bytes);
 }
 
+int mde_knn_csr_long_ex(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                        int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream,
+                        int* fallback_rows) {
+  return run_csr_full(kCsrLong, indptr, indices, values, n, d, nnz, k, kLongMaxK, idx_out, d2_out, ws, ws_bytes,
+                      stream, fallback_rows);
+}
+
 int mde_knn_csr_long(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                      int64_t nnz, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream) {
-  return run_csr_full(kCsrLong, indptr, indices, values, n, d, nnz, k, kLongMaxK, idx_out, d2_out, ws, ws_bytes,
-                      stream);
+  return mde_knn_csr_long_ex(indptr, indices, values, n, d, nnz, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
 int mde_knn_csr_rows_ws_bytes(int64_t n, int d, int64_t nnz, int64_t rows, int k, size_t* bytes) {
@@ -998,11 +1191,18 @@ int mde_knn_csr_rows_ws_bytes(int64_t n, int d, int64_t nnz, int64_t rows, int k
   return 0;
 }
 
+int mde_knn_csr_rows_ex(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
+                        int64_t nnz, int64_t row_begin, int64_t row_end, int k, int32_t* idx_out, float* d2_out,
+                        void* ws, size_t ws_bytes, void* stream, int* fallback_rows) {
+  return run_csr_rows(indptr, indices, values, n, d, nnz, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes,
+                      stream, fallback_rows);
+}
+
 int mde_knn_csr_rows(const int64_t* indptr, const int32_t* indices, const float* values, int64_t n, int d,
                      int64_t nnz, int64_t row_begin, int64_t row_end, int k, int32_t* idx_out, float* d2_out, void* ws,
                      size_t ws_bytes, void* stream) {
-  return run_csr_rows(indptr, indices, values, n, d, nnz, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes,
-                      stream);
+  return mde_knn_csr_rows_ex(indptr, indices, values, n, d, nnz, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes,
+                             stream, nullptr);
 }
 
 // host-side debug entry point: the candidate slices (mde_logic.h: knn_slices) of mde_knn_csr_rows for `rows` query
