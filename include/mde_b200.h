@@ -112,8 +112,12 @@ int mde_edges_kind(const mde_edges_t* e);
 /* 1 when the layout was created with MDE_B200_DETERMINISTIC=1 and 1 <= embedding_dim <= 512: value AND gradient of
  * fused and external-coefficient evaluations at that m are bit-reproducible run to run and independent of scheduling
  * -- the reference's scatter_add_ is not (pymde/average_distortion.py:75-76).
- *   m <= 4: gradient contributions are accumulated as 64-bit fixed point (2^-40 resolution); two 64-bit reds per row
- *           update instead of one vector red.
+ *   m <= 4: every fp32 contribution is added at both of its ends as a 64-bit fixed-point integer, at a power-of-two
+ *           scale per row picked in each evaluation from the row's largest finite |contribution| M and its degree d
+ *           (quantum at most 2^(ceil(log2 d) - 61) M): no term is clamped and no row sum wraps at any magnitude, and
+ *           each gradient entry is the exact sum of its row's contributions within half a quantum per term, rounded
+ *           once to fp32.  A non-finite contribution makes its entries NaN.  A scan pass over the edges precedes
+ *           the accumulation; 64-bit reds per contribution instead of one vector red per row update.
  *   5 <= m <= 512: owner-complete rows -- every node's directed entries are evaluated by one group of lanes in a fixed
  *           order and its row is written once, with no atomics (lists longer than 256 entries in segments added in
  *           order); two row gathers per edge instead of one plus a row of reds. */

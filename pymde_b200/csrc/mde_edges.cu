@@ -72,18 +72,47 @@ __global__ void unpack_kernel(const uint64_t* __restrict__ keys, const int32_t* 
 // ------------------------------------------------------------------------------------------
 // m <= 4: thread-per-edge kernel
 // ------------------------------------------------------------------------------------------
-// Deterministic mode: contributions are accumulated as 64-bit fixed point (scale 2^40, resolution 9e-13, range
-// +-8.4e6 -- the entries are f'/p-sized).  Integer addition is associative, so the sums do not depend on the order in
-// which the reds land (the float reds of the default mode, like the reference's scatter_add_, do:
-// pymde/average_distortion.py:75-76).
-constexpr float kFxScale = 1099511627776.0f;  // 2^40
+// Deterministic mode: contributions are accumulated as 64-bit fixed point.  Integer addition is associative, so the
+// sums do not depend on the order in which the reds land (the float reds of the default mode, like the reference's
+// scatter_add_, do: pymde/average_distortion.py:75-76).  Every row has its own power-of-two scale 2^S, picked per
+// evaluation: a scan pass finds the row's largest finite |contribution| M < 2^eM (an integer atomicMax, order-free),
+// and S = kFxHeadroom - ceil(log2(deg)) - eM.  Every contribution is added on its own at both ends (no fp32
+// pre-sums), so the row adds deg <= 2^lgdeg terms of magnitude at most M: every term, every partial sum and the
+// final sum stay below 2^62 after scaling, no term is clamped and no sum wraps, and the gradient is the exact sum
+// of the fp32 contributions up to half a quantum per term and the final rounding.  The quantum 2^-S is at most
+// 2^(lgdeg - 61) M, so it tracks the row's contributions (f'/p, or the difference vector where the guard set g = 1)
+// instead of being an absolute 2^-40.  A non-finite term makes its gradient entry NaN, as a non-finite contribution
+// makes the default mode's entry non-finite.
+constexpr int kFxHeadroom = 61;
+// 2^S (inverse = false) or 2^-S (inverse = true) of a row; S lies in [-98, 187], a normal double either way
+__device__ __forceinline__ double fx_scale(unsigned mbits, int lgdeg, bool inverse) {
+  const int em = max((int)(mbits >> 23), 1) - 126;  // M < 2^em (mbits = 0: every contribution is 0)
+  const int s = kFxHeadroom - lgdeg - em;
+  return __hiloint2double((1023 + (inverse ? -s : s)) << 20, 0);
+}
 template <int M>
-__device__ __forceinline__ void red_row_fx(long long* __restrict__ F, int r, const float (&v)[M], float sgn) {
+__device__ __forceinline__ void red_row_fx(long long* __restrict__ F, float* __restrict__ grad, int r,
+                                           const float (&v)[M], float sgn, const unsigned* __restrict__ fmax,
+                                           const uint8_t* __restrict__ lgdeg) {
+  const double sc = fx_scale(__ldcg(fmax + r), (int)__ldg(lgdeg + r), false);
 #pragma unroll
   for (int c = 0; c < M; ++c) {
-    const long long q = __float2ll_rn(sgn * v[c] * kFxScale);
-    atomicAdd(reinterpret_cast<unsigned long long*>(F + (int64_t)r * M + c), (unsigned long long)q);
+    if (isfinite(v[c])) {
+      const long long q = __double2ll_rn((double)(sgn * v[c]) * sc);
+      atomicAdd(reinterpret_cast<unsigned long long*>(F + (int64_t)r * M + c), (unsigned long long)q);
+    } else {
+      grad[(int64_t)r * M + c] = __int_as_float(0x7fffffff);  // NaN survives fx_apply_kernel's addition
+    }
   }
+}
+// the scan pass: the largest finite |v_c| of a contribution, as bits (non-negative floats order like their bits)
+template <int M>
+__device__ __forceinline__ unsigned max_bits_fx(const float (&v)[M]) {
+  unsigned mx = 0u;
+#pragma unroll
+  for (int c = 0; c < M; ++c)
+    if (isfinite(v[c])) mx = max(mx, __float_as_uint(fabsf(v[c])));
+  return mx;
 }
 // incidence entries of the sorted edges: (node, (k << 1) | endpoint is dst); the per-node counts on the side
 __global__ void inc_keys_kernel(const int32_t* __restrict__ src, const int32_t* __restrict__ dst, int64_t p,
@@ -95,6 +124,19 @@ __global__ void inc_keys_kernel(const int32_t* __restrict__ src, const int32_t* 
   keys[j] = (uint32_t)node;
   vals[j] = ((uint32_t)k << 1) | (j < p ? 0u : 1u);
   atomicAdd(count + node, 1);
+}
+// node degrees of the sorted edges (pads excluded)
+__global__ void degree_kernel(const int32_t* __restrict__ src, const int32_t* __restrict__ dst, int64_t p,
+                              int* __restrict__ count) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= 2 * p) return;
+  atomicAdd(count + (j < p ? src[j] : dst[j - p]), 1);
+}
+__global__ void lgdeg_kernel(const int* __restrict__ count, int64_t n, uint8_t* __restrict__ lg) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int d = count[i];
+  lg[i] = (uint8_t)(d <= 1 ? 0 : 32 - __clz(d - 1));  // ceil(log2(d))
 }
 // directed entries in the order of `inc`: (neighbour row | endpoint is dst << 31, bits of par0[k])
 __global__ void ent_fill_kernel(const uint32_t* __restrict__ inc, const int32_t* __restrict__ src,
@@ -108,17 +150,26 @@ __global__ void ent_fill_kernel(const uint32_t* __restrict__ inc, const int32_t*
   const uint32_t nbr = (uint32_t)(is_dst ? src[k] : dst[k]);
   ent[j] = make_uint2(nbr | (is_dst << 31), __float_as_uint(par0[k]));
 }
-__global__ void fx_zero_kernel(const int* __restrict__ flag, long long* __restrict__ F, int64_t count) {
+__global__ void fx_zero_kernel(const int* __restrict__ flag, long long* __restrict__ F, unsigned* __restrict__ fmax,
+                               int64_t n, int m) {
   if (flag != nullptr && *flag == 0) return;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += stride) F[i] = 0ll;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n * m; i += stride) {
+    F[i] = 0ll;
+    if (i < n) fmax[i] = 0u;
+  }
 }
-__global__ void fx_apply_kernel(const int* __restrict__ flag, const long long* __restrict__ F, float* __restrict__ grad,
-                                int64_t count) {
+// grad += F 2^-S: F (|F| < 2^62) is rounded to a double, scaled exactly (S may exceed the float range) and rounded
+// to fp32 once
+__global__ void fx_apply_kernel(const int* __restrict__ flag, const long long* __restrict__ F,
+                                const unsigned* __restrict__ fmax, const uint8_t* __restrict__ lgdeg,
+                                float* __restrict__ grad, int64_t count, int m) {
   if (flag != nullptr && *flag == 0) return;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += stride)
-    grad[i] += (float)((double)F[i] * (1.0 / 1099511627776.0));
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += stride) {
+    const int64_t r = i / m;
+    grad[i] += __double2float_rn(__ll2double_rn(F[i]) * fx_scale(fmax[r], (int)lgdeg[r], true));
+  }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -166,8 +217,12 @@ distortion_quad_kernel(const int32_t* __restrict__ src, const int32_t* __restric
                        const int32_t* __restrict__ perm, const float* __restrict__ gext,
                        int64_t p, const float* __restrict__ X, float* __restrict__ grad,
                        double* __restrict__ loss_partials, FnDev fn, float inv_p,
-                       const int* __restrict__ flag, long long* __restrict__ fx) {
+                       const int* __restrict__ flag, long long* __restrict__ fx, unsigned* __restrict__ fxm,
+                       const uint8_t* __restrict__ fxd, int fx_scan) {
   if (flag != nullptr && *flag == 0) return;
+  // deterministic mode (fx set): the scan pass (fx_scan) only finds every row's largest finite |v| into fxm (one
+  // atomicMax per dst end and per run of equal src); the accumulating pass reads it back as the row's scale
+  unsigned fx_mx = 0u;
   const int64_t nquads = (p + 3) >> 2;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   float lsum_f = 0.0f;
@@ -228,10 +283,21 @@ distortion_quad_kernel(const int32_t* __restrict__ src, const int32_t* __restric
       float f, v[M];
       const bool live = edge_contribution<M, MODE, FA, FR, FAST>(xi[e], xj[e], a[e], b[e], fn, inv_p, ok, f, v);
       if (MODE != 2 && ok) { if (FAST) lsum_f += f; else lsum += (double)f; }
-      if (MODE != 1) {
-        if (live) { if (fx) red_row_fx<M>(fx, t[e], v, -1.0f); else red_row<M>(grad, t[e], v, -1.0f); }
+      if (MODE != 1 && fx_scan) {
+        const unsigned mx = live ? max_bits_fx<M>(v) : 0u;
+        if (mx) atomicMax(fxm + t[e], mx);
+        if (s[e] != cur) {
+          if (fx_mx) atomicMax(fxm + cur, fx_mx);
+          cur = s[e];
+          fx_mx = 0u;
+        }
+        fx_mx = max(fx_mx, mx);
+      } else if (MODE != 1 && fx) {  // every contribution is rounded once and added exactly at both ends
+        if (live) { red_row_fx<M>(fx, grad, t[e], v, -1.0f, fxm, fxd); red_row_fx<M>(fx, grad, s[e], v, 1.0f, fxm, fxd); }
+      } else if (MODE != 1) {
+        if (live) red_row<M>(grad, t[e], v, -1.0f);
         if (s[e] != cur) {  // run of equal src ended: flush its sum
-          if (fx) red_row_fx<M>(fx, cur, acc, 1.0f); else red_row<M>(grad, cur, acc, 1.0f);
+          red_row<M>(grad, cur, acc, 1.0f);
           cur = s[e];
 #pragma unroll
           for (int c = 0; c < M; ++c) acc[c] = 0.0f;
@@ -240,9 +306,15 @@ distortion_quad_kernel(const int32_t* __restrict__ src, const int32_t* __restric
         for (int c = 0; c < M; ++c) acc[c] += v[c];
       }
     }
-    if (MODE != 1) { if (fx) red_row_fx<M>(fx, cur, acc, 1.0f); else red_row<M>(grad, cur, acc, 1.0f); }
+    if (MODE != 1 && fx_scan) {
+      if (fx_mx) atomicMax(fxm + cur, fx_mx);
+      fx_mx = 0u;
+    } else if (MODE != 1 && !fx) {
+      red_row<M>(grad, cur, acc, 1.0f);
+    }
     if (FAST) { lsum += (double)lsum_f; lsum_f = 0.0f; }
   }
+  if (MODE != 1 && fx_scan) return;
   if (MODE != 2) {
     __shared__ double sm[32];
     double v1[1] = {lsum};
@@ -780,6 +852,7 @@ struct SoaLaunch {
   float inv_p;
   long long* fx;  // deterministic mode: the fixed-point accumulator
   bool owner;     // the owner kernel runs in place of the quad kernel
+  bool fx_scan;   // deterministic mode: the scan pass that picks the fixed-point scale
   const float* par1() const { return e->has_par1 ? e->par1 : nullptr; }
 };
 
@@ -801,7 +874,7 @@ int launch_quad(const SoaLaunch& l) {
   const int nb = loss_blocks_quad(e->p);
   distortion_quad_kernel<M, MODE, FA, FR, FAST><<<nb, kQuadThreads, 0, l.st>>>(
       e->src, e->dst, e->par0, l.par1(), e->perm, l.gext, e->p, l.X, l.grad, e->loss_partials, e->fn, l.inv_p, l.flag,
-      l.fx);
+      l.fx, e->fx_max, e->fx_lgdeg, l.fx_scan ? 1 : 0);
   return nb;
 }
 
@@ -813,6 +886,10 @@ int launch_small(const SoaLaunch& l) {
     // compile-time ids there (IEEE math, as the run-time table) instead of two out-of-line calls
     if (l.owner && Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>::matches(fn))
       return launch_owner<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOG, false>(l);
+    // deterministic mode: the same IEEE math on the quad kernel, so that its contributions are the default mode's
+    // and only the accumulation differs
+    if (l.fx && Fn<MDE_FN_P_LOG1P, MDE_FN_P_LOG>::matches(fn))
+      return launch_quad<M, MODE, MDE_FN_P_LOG1P, MDE_FN_P_LOG, false>(l);
   }
   return select_fn<M, MODE>(fn, fast_log1p_log(fn, l.e->precise), QuadPairs{}, [&](auto f) {
     using F = decltype(f);
@@ -863,16 +940,23 @@ int launch_wide(const SoaLaunch& l) {
 template <int MODE>
 int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, const float* gext,
                       int* nblocks_out, const int* flag, cudaStream_t st) {
-  SoaLaunch l{e, X, m, grad, gext, flag, st, 1.0f / (float)e->p_total, nullptr, false};
-  // deterministic mode (m <= 4, sorted-SoA layout): zero the fixed-point buffer, accumulate into it, add it to grad.
-  // A deterministic layout built for m >= 5 has no fixed-point buffer: it evaluates its own m on the wide owner kernel
-  // (launch_wide).
+  SoaLaunch l{e, X, m, grad, gext, flag, st, 1.0f / (float)e->p_total, nullptr, false, false};
+  // deterministic mode (m <= 4, sorted-SoA layout): zero the fixed-point buffer, scan the contributions for the
+  // scale, accumulate into the buffer, add it to grad.  A deterministic layout built for m >= 5 has no fixed-point
+  // buffer: it evaluates its own m on the wide owner kernel (launch_wide).
   if (e->det && e->fx && MODE != 1 && m <= 4 && m <= e->m_hint) {
     l.fx = e->fx;
     const int64_t cnt = e->n * m;
     int zb = (int)((cnt + 255) / 256); if (zb > kNumSMs * 8) zb = kNumSMs * 8;
-    fx_zero_kernel<<<zb, 256, 0, st>>>(flag, l.fx, cnt);
+    fx_zero_kernel<<<zb, 256, 0, st>>>(flag, l.fx, e->fx_max, e->n, m);
     ++g_launch_count;
+    l.fx_scan = true;
+    if (m == 1) launch_small<1, MODE>(l);
+    else if (m == 2) launch_small<2, MODE>(l);
+    else if (m == 3) launch_small<3, MODE>(l);
+    else launch_small<4, MODE>(l);
+    MDE_LAUNCH_CHECK();
+    l.fx_scan = false;
   }
   // default on the sorted-SoA layout: the owner kernel over the directed entries, in place of the quad kernel
   l.owner = !l.fx && e->ent && MODE != 1 && m == e->m_hint;
@@ -904,7 +988,7 @@ int launch_distortion(const mde_edges* e, const float* X, int m, float* grad, co
   if (l.fx) {
     const int64_t cnt = e->n * m;
     int zb = (int)((cnt + 255) / 256); if (zb > kNumSMs * 8) zb = kNumSMs * 8;
-    fx_apply_kernel<<<zb, 256, 0, st>>>(flag, l.fx, grad, cnt);
+    fx_apply_kernel<<<zb, 256, 0, st>>>(flag, l.fx, e->fx_max, e->fx_lgdeg, grad, cnt, m);
     MDE_LAUNCH_CHECK();
   }
   if (nblocks_out) *nblocks_out = nb;
@@ -1093,6 +1177,21 @@ int mde_edges_create_ex(mde_edges_t** out, const int64_t* edges, int64_t p, int6
   }
   cudaFree(keys_in); cudaFree(keys_out); cudaFree(vals_in); cudaFree(vals_out); cudaFree(tmp);
   keys_in = keys_out = nullptr; vals_in = vals_out = nullptr; tmp = nullptr;
+  if (e->fx) {  // the fixed-point scale bounds a row's sum by its degree: keep ceil(log2(degree)) of every row
+    int* cnt = nullptr;
+    TRY(cudaMalloc(&e->fx_max, sizeof(unsigned) * n_items));
+    TRY(cudaMalloc(&e->fx_lgdeg, n_items));
+    TRY(cudaMalloc(&cnt, sizeof(int) * n_items));
+    TRY(cudaMemsetAsync(cnt, 0, sizeof(int) * n_items, st));
+    degree_kernel<<<ceil_div_i64(2 * p, 256), 256, 0, st>>>(e->src, e->dst, p, cnt);
+    ++g_launch_count;
+    TRY(cudaPeekAtLastError());
+    lgdeg_kernel<<<ceil_div_i64(n_items, 256), 256, 0, st>>>(cnt, n_items, e->fx_lgdeg);
+    ++g_launch_count;
+    TRY(cudaPeekAtLastError());
+    TRY(cudaStreamSynchronize(st));
+    cudaFree(cnt);
+  }
   if (((!e->det && embedding_dim >= 1 && embedding_dim <= 4) || (e->det && embedding_dim >= 5)) && !want_ell &&
       2 * p < (1ll << 31)) {
     // incidence lists of the sorted edges: a stable radix sort by node keeps each node's entries in the order
@@ -1175,7 +1274,7 @@ fail:
 int mde_edges_destroy(mde_edges_t* e) {
   if (!e) return 0;
   cudaFree(e->src); cudaFree(e->dst); cudaFree(e->perm); cudaFree(e->par0); cudaFree(e->par1);
-  cudaFree(e->loss_partials); cudaFree(e->fx); cudaFree(e->ent); cudaFree(e->inc); cudaFree(e->inc_off);
+  cudaFree(e->loss_partials); cudaFree(e->fx); cudaFree(e->fx_max); cudaFree(e->fx_lgdeg); cudaFree(e->ent); cudaFree(e->inc); cudaFree(e->inc_off);
   cudaFree(e->wseg); cudaFree(e->whub); cudaFree(e->wpart);
   tiled_free(e);
   pull_free(e);

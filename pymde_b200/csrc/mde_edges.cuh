@@ -51,6 +51,8 @@ struct mde_edges {
   bool precise = false;
   int det = 0;               // deterministic mode: m <= 4 fixed point (fx), 5 <= m <= 512 the wide owner kernel
   long long* fx = nullptr;   // [n * m_hint] fixed-point accumulator (det, m_hint <= 4 only)
+  unsigned* fx_max = nullptr;     // [n] det, m_hint <= 4: bits of the row's largest finite |contribution| (per evaluation)
+  uint8_t* fx_lgdeg = nullptr;    // [n] det, m_hint <= 4: ceil(log2(degree)) of every row
   // sorted-SoA layout, m_hint <= 4 (and deterministic layouts with 5 <= m_hint <= 512): every edge is stored again as
   // two directed entries grouped by owner node, and the owner kernels visit each node's entries in this fixed order,
   // keep the sum in registers and write the row once (no atomics) -- a gradient that is the same bits from run to run
