@@ -15,7 +15,7 @@
  *  - `stream` is a cudaStream_t passed as void*; all work is enqueued on it and no call
  *    synchronises the device unless documented ("blocking");
  *  - matrices are row-major contiguous float32: X[n_items][m] (the mde_knn16* searches also read
- *    16-bit data matrices, tagged with an MDE_DTYPE_* code).
+ *    16-bit data matrices and the mde_knn8* searches 8-bit ones, tagged with an MDE_DTYPE_* code).
  */
 #ifndef MDE_B200_H
 #define MDE_B200_H
@@ -466,6 +466,49 @@ int mde_knn16_approx(const void* X, int dtype, int64_t n, int d, int k, uint64_t
                      float* d2_out, void* ws, size_t ws_bytes, void* stream);
 int mde_knn16_approx_ex(const void* X, int dtype, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out,
                         float* d2_out, void* ws, size_t ws_bytes, void* stream, int* iterations);
+/* The dense searches on an 8-bit data matrix, read in place: `X` is a device row-major n x d matrix of uint8
+ * (`dtype` = MDE_DTYPE_U8) or int8 (MDE_DTYPE_S8) values; any other code is MDE_E_INVALID, checked with the other
+ * arguments before any CUDA call.  mde_knn8, mde_knn8_wide, mde_knn8_long, mde_knn8_approx(_ex) and mde_knn8_rows
+ * take the arguments, bounds on k, return codes, blocking behaviour, fallback-row reporting and output contract of
+ * mde_knn16, mde_knn16_wide, mde_knn16_long, mde_knn16_approx(_ex) and mde_knn16_rows, and give the bits the fp32
+ * entries give on X.float(), ties included: the re-rank, the direct search and NN-descent convert every element to
+ * fp32 as they read it and keep the fp32 arithmetic.  The exact searches' operand is X itself, exact and never
+ * centred: one wgmma.k32 with int32 accumulation per 32 features, candidates ranked by their exact integer score
+ * ||y||^2 - 2 <q, y>, and each row certified by comparing its k-th fp32 distance with the exact distance of the worst
+ * row it kept.  That needs every tile sum to be exact in int32: d <= d_max = mde_knn8_max_d(dtype) (16 512 for uint8,
+ * 43 919 for int8; MDE_E_INVALID for another code); the exact searches return MDE_E_UNSUPPORTED for a wider matrix
+ * (search X.float() instead), NN-descent takes any d.  `ws`: 1024-byte aligned device scratch of
+ * mde_knn8_ws_bytes(n, d), mde_knn8_wide_ws_bytes(n, d), mde_knn8_long_ws_bytes(n, d) or mde_knn8_rows_ws_bytes(n, d,
+ * rows, k) bytes: the layout of the fp32 searches without a lo operand, with 1 byte per operand element (n_pad x
+ * k_pad8, n_pad = n rounded up to 128, k_pad8 = d rounded up to 128) and without the column mean's n d / 64 bytes of
+ * sums; or mde_knn8_approx_ws_bytes(n, d, k) (that of mde_knn_approx: NN-descent keeps no copy of X).  Nothing n x d
+ * sized in fp32 is allocated. */
+#define MDE_DTYPE_U8 3
+#define MDE_DTYPE_S8 4
+int mde_knn8_max_d(int dtype);
+int mde_knn8_ws_bytes(int64_t n, int d, size_t* bytes);
+int mde_knn8(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+             size_t ws_bytes, void* stream);
+int mde_knn8_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                size_t ws_bytes, void* stream, int* fallback_rows);
+int mde_knn8_wide_ws_bytes(int64_t n, int d, size_t* bytes);
+int mde_knn8_wide(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                  size_t ws_bytes, void* stream);
+int mde_knn8_wide_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                     size_t ws_bytes, void* stream, int* fallback_rows);
+int mde_knn8_long_ws_bytes(int64_t n, int d, size_t* bytes);
+int mde_knn8_long(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                  size_t ws_bytes, void* stream);
+int mde_knn8_long_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                     size_t ws_bytes, void* stream, int* fallback_rows);
+int mde_knn8_approx_ws_bytes(int64_t n, int d, int k, size_t* bytes);
+int mde_knn8_approx(const void* X, int dtype, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out,
+                    float* d2_out, void* ws, size_t ws_bytes, void* stream);
+int mde_knn8_approx_ex(const void* X, int dtype, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out,
+                       float* d2_out, void* ws, size_t ws_bytes, void* stream, int* iterations);
+int mde_knn8_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes);
+int mde_knn8_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin, int64_t row_end, int k,
+                  int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows);
 /* The exact dense searches for a range of query rows: rows [row_begin, row_end) of X against all n rows of X (the
  * row itself excluded), for embedding new rows next to rows already searched.  Row r of idx_out / d2_out (rows x k,
  * rows = row_end - row_begin) is bit for bit row row_begin + r of mde_knn (k <= 24) or mde_knn_wide (24 < k <= 64)

@@ -15,6 +15,7 @@ MDE_E_INVALID, MDE_E_UNSUPPORTED, MDE_E_NAN, MDE_E_ALLOC, MDE_E_COMM = -1, -2, -
 IPC_HANDLE_BYTES = 64
 CONSTRAINT_CENTERED, CONSTRAINT_STANDARDIZED, CONSTRAINT_ANCHORED, CONSTRAINT_CUSTOM = 0, 1, 2, 3
 DTYPE_FP16, DTYPE_BF16 = 1, 2  # MDE_DTYPE_* element codes of the mde_knn16* searches
+DTYPE_U8, DTYPE_S8 = 3, 4  # and of the mde_knn8* searches
 
 
 class MdeError(RuntimeError):
@@ -183,6 +184,30 @@ SIGNATURES = {
                                    C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "mde_knn16_approx_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
+    "mde_knn8_max_d": (C.c_int, [C.c_int]),
+    "mde_knn8_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn8": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                           C.c_size_t, C.c_void_p]),
+    "mde_knn8_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                              C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
+    "mde_knn8_wide_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn8_wide": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn8_wide_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
+    "mde_knn8_long_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn8_long": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn8_long_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
+    "mde_knn8_approx_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn8_approx": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "mde_knn8_approx_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
+    "mde_knn8_rows_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn8_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
+                                C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
     "mde_knn_approx_csr_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn_approx_csr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int,
                                      C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -237,6 +262,7 @@ DEBUG_SIGNATURES = {
     "mde_dbg_lbfgs_cand": (C.c_int, [C.c_void_p]),
     "mde_dbg_knn_slices": (C.c_int, [C.c_int64, C.c_int64, C.c_int]),
     "mde_dbg_knn_csr_slices": (C.c_int, [C.c_int64, C.c_int64, C.c_int]),
+    "mde_dbg_knn8_gamma": (C.c_double, [C.c_int]),
 }
 
 _lib = None

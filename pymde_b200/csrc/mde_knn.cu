@@ -44,11 +44,21 @@
 // unchanged arithmetic gives the bits of the fp32 route on X.float() (near-ties at the list's edge aside, DESIGN
 // section 11.7).
 //
+// 8-bit input (mde_knn8, mde_knn8_wide, mde_knn8_long, mde_knn8_rows: uint8 or int8, read without an fp32 copy).  The
+// element is its own operand, exact wherever the data sits, so nothing is centred: the prep copies X into a zero-padded
+// operand (K blocks of 128 elements, one 128-byte swizzle row) and writes exact int32 squared norms (INT_MAX on padded
+// rows); the tile kernels issue one wgmma.m64n{128,64}k32.s32.{u8,s8} per 32 features, four per K block, on the same
+// stage layout, and rank candidates by the exact integer score ||y||^2 - 2 <q, y>.  Every accumulator, norm and score
+// is exact in int32 up to d_max (knn8_max_d); the entries refuse wider matrices.  The lists hold the KK smallest exact
+// distances, the re-rank is the fp32 one, and the certificate compares the k-th re-ranked distance with the exact
+// KK-th (knn_certify_kernel), so the result is again the brute-force fp32 result on X.float() (DESIGN section 11.9).
+//
 // Hangs are not an option on a shared GPU: every mbarrier wait is bounded (mde_tma.cuh) and traps.
 #include <cuda.h>  // CUtensorMap and its enums (types only: the encoder is fetched with cudaGetDriverEntryPoint)
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include <climits>
 #include <cstdint>
 #include <cstdlib>
 #include <type_traits>
@@ -65,12 +75,11 @@ namespace {
 
 constexpr int kTileM = 128;                 // query rows per CTA (two warpgroups of 64)
 constexpr int kTileN = 128;                 // candidates per tile = wgmma N
-constexpr int kBlockK = 64;                 // bf16 elements per 128-byte swizzle row
-constexpr int kWgmmaK = 16;                 // K of one wgmma.m64n128k16
 constexpr int kStages = 2;
 constexpr int kKK = kNarrowKK;              // candidates kept per row before the exact re-rank (32)
 constexpr int kMaxK = 24;
-constexpr int kRowBytes = kBlockK * 2;      // 128
+constexpr int kRowBytes = 128;              // one K block: a 128-byte swizzle row (64 16-bit or 128 8-bit elements)
+constexpr int kKSteps = kRowBytes / 32;     // wgmma K steps per block: k16 on 16-bit operands, k32 on 8-bit ones
 constexpr int kOpBytes = 128 * kRowBytes;   // 16 KB: one 128-row operand block (hi or lo)
 constexpr int kStageBytes = 4 * kOpBytes;   // A hi, A lo, B hi, B lo = 64 KB
 constexpr int kConsumerWarps = 8;           // warps 0-7: two consumer warpgroups; warp 8: TMA producer
@@ -120,33 +129,73 @@ __device__ __forceinline__ void named_bar_sync(int id, int count) {
 }
 
 // The tensor-core operand of an element type: fp32 is split into bf16 hi and lo parts (three products per k16 step),
-// a 16-bit element is its own operand (one product).
+// a 16-bit or 8-bit element is its own operand (one product).  Acc: the type of the accumulators, norms and scores
+// (int32 for 8-bit operands, whose products and sums are exact integers); kBlockK: elements per 128-byte K block.
 template <class T>
 struct Operand {
   using type = __nv_bfloat16;
+  using Acc = float;
   static constexpr bool kSplit = true;
+  static constexpr int kBlockK = 64;
   static constexpr CUtensorMapDataType kMapType = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
 };
 template <>
 struct Operand<__nv_bfloat16> {
   using type = __nv_bfloat16;
+  using Acc = float;
   static constexpr bool kSplit = false;
+  static constexpr int kBlockK = 64;
   static constexpr CUtensorMapDataType kMapType = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
 };
 template <>
 struct Operand<__half> {
   using type = __half;
+  using Acc = float;
   static constexpr bool kSplit = false;
+  static constexpr int kBlockK = 64;
   static constexpr CUtensorMapDataType kMapType = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+};
+template <>
+struct Operand<uint8_t> {
+  using type = uint8_t;
+  using Acc = int;
+  static constexpr bool kSplit = false;
+  static constexpr int kBlockK = 128;
+  static constexpr CUtensorMapDataType kMapType = CU_TENSOR_MAP_DATA_TYPE_UINT8;
+};
+template <>
+struct Operand<int8_t> {
+  using type = int8_t;
+  using Acc = int;
+  static constexpr bool kSplit = false;
+  static constexpr int kBlockK = 128;
+  static constexpr CUtensorMapDataType kMapType = CU_TENSOR_MAP_DATA_TYPE_UINT8;  // (TMA copies bytes)
 };
 template <class T>
 using OpT = typename Operand<T>::type;
+template <class T>
+using AccT = typename Operand<T>::Acc;
+template <class T>
+constexpr bool kInt8 = std::is_same_v<AccT<T>, int>;
 
-// One k16 step of the cross terms of 64 query rows and TN candidates, D (+)= Ah Bh^T (+ Ah Bl^T + Al Bh^T for fp32).
+// The score ||y||^2 - 2 <q, y> of a candidate from its norm s and cross term a: one fp32 fma, or exact in int32.
+__device__ __forceinline__ float tile_score(float a, float s) { return fmaf(-2.0f, a, s); }
+__device__ __forceinline__ int tile_score(int a, int s) { return s - 2 * a; }
+// two adjacent staged accumulators or norms
+template <class A>
+using Pair = std::conditional_t<std::is_same_v<A, int>, int2, float2>;
+
+// One K step of the cross terms of 64 query rows and TN candidates, D (+)= Ah Bh^T (+ Ah Bl^T + Al Bh^T for fp32).
 template <class T, int TN>
-__device__ __forceinline__ void cross_step(float (&acc)[TN / 2], uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl,
+__device__ __forceinline__ void cross_step(AccT<T> (&acc)[TN / 2], uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl,
                                            uint32_t accumulate) {
-  if constexpr (std::is_same_v<T, __half>) {
+  if constexpr (std::is_same_v<T, uint8_t>) {
+    if constexpr (TN == 128) wgmma_u8(acc, ah, bh, accumulate);
+    else wgmma_u8_n64(acc, ah, bh, accumulate);
+  } else if constexpr (std::is_same_v<T, int8_t>) {
+    if constexpr (TN == 128) wgmma_s8(acc, ah, bh, accumulate);
+    else wgmma_s8_n64(acc, ah, bh, accumulate);
+  } else if constexpr (std::is_same_v<T, __half>) {
     if constexpr (TN == 128) wgmma_f16(acc, ah, bh, accumulate);
     else wgmma_f16_n64(acc, ah, bh, accumulate);
   } else if constexpr (TN == 128) {
@@ -203,17 +252,49 @@ knn_mean_kernel(const double* __restrict__ part, int chunks, int64_t n, int d, f
 //   a_norm   the fp32 norm (ceil(k_pad / 32) + 8) u and the score's fma (u),
 //   a_abs    underflow: 2^-126 per product and per square,
 // and sigma = 2, a safety factor for second-order terms (tests/test_knn_offset_cpu.py derives the bound).
+//
+// 8-bit input.  The tiles rank by the exact score S(y), so the list holds the KK smallest exact distances and every
+// row y it did not keep has D(y) = ||q - y||^2 >= D_KK = t + ||q||^2 (t: the worst kept score, exact).  The re-rank's
+// value r(y) is an fp32 sum of d exact squared differences (each below 2^16, so exact in fp32) with at most
+// L = ceil(d / 32) + 5 roundings on any path (the lane's fma chain, then five butterfly levels); a sum of non-negative
+// terms so rounded lies within gamma = L u / (1 - L u) of its value, relatively, so r(y) >= (1 - gamma) D(y).  The row
+// certifies when r_k < (1 - gamma) D_KK: no row outside the list can displace its k-th pair (ties fail and go to the
+// direct search).  Every partial sum is an integer below 2^24, so exact, when d 255^2 <= 2^24 (d <= 258 for both
+// 8-bit types): then gamma = 0 and the test is r_k < D_KK.  2^-50 covers the fp64 rounding of (1 - gamma) D_KK.
+// tests/test_knn_int8_cpu.py derives gamma again and checks it against mde_dbg_knn8_gamma.
 // ---------------------------------------------------------------------------------------------------------------
 struct CertBound {
   double a_cen, a_unc;  // a_cross of the centred and of the uncentred operand
   double eta, a_norm, a_abs, delta;
+  double gamma;         // 8-bit input: the re-rank's relative error bound
 };
 constexpr double kCertSafety = 2.0;
+
+double knn8_gamma(int d) {
+  if ((int64_t)d * 255 * 255 <= (1 << 24)) return 0.0;
+  const double u = 0x1p-24, L = (double)((d + 31) / 32 + 5);
+  return L * u / (1.0 - L * u) + 0x1p-50;
+}
+
+// d_max of an 8-bit type: the largest d for which every accumulator, norm and score of the tiles is exact in int32
+// and every score stays below INT_MAX, the key of padded rows and empty list slots.  uint8: |2 <q, y>| <= 2 d 255^2
+// and 0 <= ||y||^2 <= d 255^2, so 2 d 255^2 < 2^31 gives d <= 16 512.  int8: |<q, y>| <= d 128^2, so 2 <q, y> fits
+// for d < 2^16, and the score ||y||^2 - 2 <q, y> <= d (128^2 + 2 128 127) = 48 896 d < 2^31 - 1 gives d <= 43 919.
+template <class T>
+constexpr int knn8_max_d() {
+  if constexpr (std::is_same_v<T, uint8_t>) return (int)(((1ll << 31) - 1) / (2 * 255 * 255));
+  else return (int)(((1ll << 31) - 2) / (128 * 128 + 2 * 128 * 127));
+}
+static_assert(knn8_max_d<uint8_t>() == 16512 && knn8_max_d<int8_t>() == 43919, "DESIGN section 11.9");
 
 template <class T>
 CertBound cert_bound(int d, int k_pad) {
   const double u = 0x1p-24;
-  CertBound b;
+  CertBound b{};
+  if constexpr (kInt8<T>) {
+    b.gamma = knn8_gamma(d);
+    return b;
+  }
   double op, op_unc = 0.0;
   int m = k_pad;
   if constexpr (Operand<T>::kSplit) { op = op_unc = 3.1 * 0x1p-16; m = 3 * k_pad; }
@@ -271,14 +352,28 @@ __device__ __forceinline__ bool knn_centre(const unsigned* hdr, const CertBound&
 // squared norms of x^ (+inf on padded rows), the same arithmetic for every element type; their maximum over the rows
 // to the header (+inf when an operand element is not finite, so that no row certifies)
 // ---------------------------------------------------------------------------------------------------------------
+// 8-bit input: X itself, zero padded, exact int32 squared norms and INT_MAX on padded rows (their score INT_MAX is
+// never kept); mu, b and the header are not read.
 template <class T>
 __global__ void __launch_bounds__(256)
 knn_prep_kernel(const T* __restrict__ X, int64_t n, int d, int64_t n_pad, int k_pad, const float* __restrict__ mu,
-                CertBound b, OpT<T>* __restrict__ Xh, __nv_bfloat16* __restrict__ Xl, float* __restrict__ norms,
+                CertBound b, OpT<T>* __restrict__ Xh, __nv_bfloat16* __restrict__ Xl, AccT<T>* __restrict__ norms,
                 unsigned* __restrict__ hdr) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= n_pad) return;
+  if constexpr (kInt8<T>) {
+    int acc = 0;
+    for (int c = lane; c < k_pad; c += 32) {
+      const T x = (row < n && c < d) ? X[row * d + c] : T(0);
+      Xh[row * k_pad + c] = x;
+      acc += (int)x * (int)x;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(kFull, acc, o);
+    if (lane == 0) norms[row] = (row < n) ? acc : INT_MAX;
+    return;
+  }
   const bool centre = knn_centre(hdr, b);
   if (row == 0 && lane == 0) hdr[kHdrCentred] = centre;
   float acc = 0.0f;
@@ -308,13 +403,13 @@ knn_prep_kernel(const T* __restrict__ X, int64_t n, int d, int64_t n_pad, int k_
 
 // Replace the worst of the KK kept candidates by (dist, col) and find the new worst.  Static indices only, so the
 // lists stay in registers.
-__device__ __forceinline__ void keep_candidate(float (&bd)[kKK], int (&bi)[kKK], float dist, int col, float& thr,
-                                               int& worst) {
+template <class K>
+__device__ __forceinline__ void keep_candidate(K (&bd)[kKK], int (&bi)[kKK], K dist, int col, K& thr, int& worst) {
 #pragma unroll
   for (int q = 0; q < kKK; ++q) {
     if (q == worst) { bd[q] = dist; bi[q] = col; }
   }
-  float m = bd[0]; int w = 0;
+  K m = bd[0]; int w = 0;
 #pragma unroll
   for (int q = 1; q < kKK; ++q) { if (bd[q] > m) { m = bd[q]; w = q; } }
   thr = m; worst = w;
@@ -326,20 +421,22 @@ __device__ __forceinline__ void keep_candidate(float (&bd)[kKK], int (&bi)[kKK],
 template <class T>
 __global__ void __launch_bounds__(kThreads, 1)
 knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_l,
-                const float* __restrict__ norms, int64_t n, int64_t n_pad, int k_pad, QueryRange qr,
-                int32_t* __restrict__ cand_idx, float* __restrict__ cand_val) {
+                const AccT<T>* __restrict__ norms, int64_t n, int64_t n_pad, int k_pad, QueryRange qr,
+                int32_t* __restrict__ cand_idx, AccT<T>* __restrict__ cand_val) {
+  using A = AccT<T>;
+  constexpr int kBK = Operand<T>::kBlockK;
   extern __shared__ uint8_t smem_raw[];
   // carve: [stages x 64 KB, 1024-aligned] | staged accumulators [128][kAccStride] | norms[2][128] | barriers
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
-  float* s_acc = reinterpret_cast<float*>(gen + kStages * kStageBytes);
-  float* s_norm = s_acc + kTileM * kAccStride;
+  A* s_acc = reinterpret_cast<A*>(gen + kStages * kStageBytes);
+  A* s_norm = s_acc + kTileM * kAccStride;
   uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_norm + 2 * kTileN);
   const uint32_t bar0 = smem_u32(s_bar);
   // barriers: full[s] = bar0 + 8 s (TMA bytes landed), empty[s] = bar0 + 16 + 8 s (every consumer warp is done)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_kb = k_pad / kBlockK;
+  const int num_kb = k_pad / kBK;
   const int num_tiles = (int)(n_pad / kTileN);
   const int t_begin = qr.slice_begin(num_tiles), t_end = qr.slice_begin(num_tiles, 1);
   const int row0 = (int)qr.base + blockIdx.x * kTileM;
@@ -359,11 +456,11 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
           mbar_wait(bar0 + 16 + 8 * stage, phase ^ 1);  // slot released by the consumers
           const uint32_t full = bar0 + 8 * stage;
           const uint32_t dst = base + stage * kStageBytes;
-          mbar_expect_tx(full, Operand<T>::kSplit ? kStageBytes : 2 * kOpBytes);  // 16-bit input: no lo parts
-          tma_load_2d(dst, &map_h, kb * kBlockK, row0, full);
-          if (Operand<T>::kSplit) tma_load_2d(dst + kOpBytes, &map_l, kb * kBlockK, row0, full);
-          tma_load_2d(dst + 2 * kOpBytes, &map_h, kb * kBlockK, t * kTileN, full);
-          if (Operand<T>::kSplit) tma_load_2d(dst + 3 * kOpBytes, &map_l, kb * kBlockK, t * kTileN, full);
+          mbar_expect_tx(full, Operand<T>::kSplit ? kStageBytes : 2 * kOpBytes);  // 16/8-bit input: no lo parts
+          tma_load_2d(dst, &map_h, kb * kBK, row0, full);
+          if (Operand<T>::kSplit) tma_load_2d(dst + kOpBytes, &map_l, kb * kBK, row0, full);
+          tma_load_2d(dst + 2 * kOpBytes, &map_h, kb * kBK, t * kTileN, full);
+          if (Operand<T>::kSplit) tma_load_2d(dst + 3 * kOpBytes, &map_l, kb * kBK, t * kTileN, full);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
@@ -374,23 +471,23 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
   // ===== consumers: warpgroup wg owns query rows row0 + 64 wg .. + 63 =====
   const int wg = warp >> 2;
   const int et = threadIdx.x & 127;            // thread within the warpgroup
-  float* acc_s = s_acc + wg * 64 * kAccStride;
-  float* sn = s_norm + wg * kTileN;
+  A* acc_s = s_acc + wg * 64 * kAccStride;
+  A* sn = s_norm + wg * kTileN;
   // scan: two threads per query row, columns half, half + 2, half + 4, ...
   const int lrow = et >> 1, half = et & 1;
   const int row = row0 + wg * 64 + lrow;
   // accumulator fragment rows / columns of this thread (see wgmma_bf16)
   const int frow = 16 * (warp & 3) + (lane >> 2), fcol = 2 * (lane & 3);
 
-  float bd[kKK];
+  A bd[kKK];
   int bi[kKK];
 #pragma unroll
-  for (int q = 0; q < kKK; ++q) { bd[q] = __int_as_float(0x7f800000); bi[q] = -1; }
-  float thr = __int_as_float(0x7f800000);
+  for (int q = 0; q < kKK; ++q) { bd[q] = key_inf<A>(); bi[q] = -1; }
+  A thr = key_inf<A>();
   int worst = 0;
-  float acc[64];
+  A acc[64];
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+  for (int i = 0; i < 64; ++i) acc[i] = 0;
 
   int stage = 0; uint32_t phase = 0;
   for (int t = t_begin; t < t_end; ++t) {
@@ -403,8 +500,8 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
       for (int i = 0; i < 64; ++i) fence_operand(acc[i]);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
-        const uint64_t adv = (uint64_t)((k * kWgmmaK * 2) >> 4);  // 32 bytes per K step inside the swizzle atom
+      for (int k = 0; k < kKSteps; ++k) {
+        const uint64_t adv = (uint64_t)((k * 32) >> 4);  // 32 bytes per K step inside the swizzle atom
         cross_step<T, kTileN>(acc, ah + adv, al + adv, bh + adv, bl + adv, (kb | k) != 0);
       }
       wgmma_commit();
@@ -419,16 +516,16 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
     named_bar_sync(1 + wg, 128);
 #pragma unroll
     for (int j = 0; j < kTileN / 8; ++j) {
-      *reinterpret_cast<float2*>(acc_s + frow * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
-      *reinterpret_cast<float2*>(acc_s + (frow + 8) * kAccStride + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      *reinterpret_cast<Pair<A>*>(acc_s + frow * kAccStride + 8 * j + fcol) = Pair<A>{acc[4 * j], acc[4 * j + 1]};
+      *reinterpret_cast<Pair<A>*>(acc_s + (frow + 8) * kAccStride + 8 * j + fcol) = Pair<A>{acc[4 * j + 2], acc[4 * j + 3]};
     }
     sn[et] = __ldg(norms + (int64_t)t * kTileN + et);
     named_bar_sync(1 + wg, 128);
-    const float* arow = acc_s + lrow * kAccStride;
+    const A* arow = acc_s + lrow * kAccStride;
 #pragma unroll 4
     for (int i = 0; i < kTileN / 2; ++i) {
       const int c = 2 * i + half;
-      const float dist = fmaf(-2.0f, arow[c], sn[c]);
+      const A dist = tile_score(arow[c], sn[c]);
       if (dist < thr) {
         const int col = t * kTileN + c;
         if (col != row) keep_candidate(bd, bi, dist, col, thr, worst);
@@ -437,7 +534,7 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
   }
   // merge the two half-row lists: the odd-column thread hands its list to the even-column thread
   named_bar_sync(1 + wg, 128);
-  float* xd = acc_s + lrow * kAccStride;
+  A* xd = acc_s + lrow * kAccStride;
   int* xi = reinterpret_cast<int*>(xd + kKK);
   if (half) {
 #pragma unroll
@@ -446,7 +543,7 @@ knn_tile_kernel(const __grid_constant__ CUtensorMap map_h, const __grid_constant
   named_bar_sync(1 + wg, 128);
   if (!half) {
     for (int q = 0; q < kKK; ++q) {
-      const float dist = xd[q];
+      const A dist = xd[q];
       if (dist < thr) keep_candidate(bd, bi, dist, xi[q], thr, worst);
     }
     if (qr.has(row)) {
@@ -513,9 +610,11 @@ template <class T, int KK, int TN>
 __global__ void __launch_bounds__(kWideThreads, 1)
 knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_constant__ CUtensorMap map_al,
                      const __grid_constant__ CUtensorMap map_h, const __grid_constant__ CUtensorMap map_l,
-                     const float* __restrict__ norms, int64_t n, int64_t n_pad, int k_pad, QueryRange qr,
-                     int32_t* __restrict__ cand_idx, float* __restrict__ cand_val) {
-  static_assert(TN == 64 || TN == 128, "wgmma.m64n64k16 or m64n128k16");
+                     const AccT<T>* __restrict__ norms, int64_t n, int64_t n_pad, int k_pad, QueryRange qr,
+                     int32_t* __restrict__ cand_idx, AccT<T>* __restrict__ cand_val) {
+  static_assert(TN == 64 || TN == 128, "wgmma.m64n64 or m64n128");
+  using A = AccT<T>;
+  constexpr int kBK = Operand<T>::kBlockK;
   constexpr int kBOpBytes = TN * kRowBytes;
   constexpr int kStageB = kWideStageBytes<TN>;
   constexpr int kAccS = TN + 2;  // floats per staged accumulator row: the scan's float2 reads are conflict-free
@@ -525,16 +624,16 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
   //        list distances [64][kStride] | list indices [64][kStride] | barriers
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* gen = smem_raw + (base - smem_u32(smem_raw));
-  float* s_acc = reinterpret_cast<float*>(gen + kStages * kStageB);
-  float* s_norm = s_acc + kWideTileM * kAccS;
-  float* s_ld = s_norm + TN;
+  A* s_acc = reinterpret_cast<A*>(gen + kStages * kStageB);
+  A* s_norm = s_acc + kWideTileM * kAccS;
+  A* s_ld = s_norm + TN;
   int* s_li = reinterpret_cast<int*>(s_ld + kWideTileM * kStride);
   uint64_t* s_bar = reinterpret_cast<uint64_t*>(s_li + kWideTileM * kStride);
   const uint32_t bar0 = smem_u32(s_bar);
   // barriers: full[s] = bar0 + 8 s (TMA bytes landed), empty[s] = bar0 + 16 + 8 s (every consumer warp is done)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_kb = k_pad / kBlockK;
+  const int num_kb = k_pad / kBK;
   const int num_tiles = (int)(n_pad / TN);
   const int t_begin = qr.slice_begin(num_tiles), t_end = qr.slice_begin(num_tiles, 1);
   const int row0 = (int)qr.base + blockIdx.x * kWideTileM;
@@ -554,11 +653,11 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
           mbar_wait(bar0 + 16 + 8 * stage, phase ^ 1);  // slot released by the consumers
           const uint32_t full = bar0 + 8 * stage;
           const uint32_t dst = base + stage * kStageB;
-          mbar_expect_tx(full, Operand<T>::kSplit ? kStageB : kAOpBytes + kBOpBytes);  // 16-bit input: no lo parts
-          tma_load_2d(dst, &map_ah, kb * kBlockK, row0, full);
-          if (Operand<T>::kSplit) tma_load_2d(dst + kAOpBytes, &map_al, kb * kBlockK, row0, full);
-          tma_load_2d(dst + 2 * kAOpBytes, &map_h, kb * kBlockK, t * TN, full);
-          if (Operand<T>::kSplit) tma_load_2d(dst + 2 * kAOpBytes + kBOpBytes, &map_l, kb * kBlockK, t * TN, full);
+          mbar_expect_tx(full, Operand<T>::kSplit ? kStageB : kAOpBytes + kBOpBytes);  // 16/8-bit input: no lo parts
+          tma_load_2d(dst, &map_ah, kb * kBK, row0, full);
+          if (Operand<T>::kSplit) tma_load_2d(dst + kAOpBytes, &map_al, kb * kBK, row0, full);
+          tma_load_2d(dst + 2 * kAOpBytes, &map_h, kb * kBK, t * TN, full);
+          if (Operand<T>::kSplit) tma_load_2d(dst + 2 * kAOpBytes + kBOpBytes, &map_l, kb * kBK, t * TN, full);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
@@ -571,11 +670,11 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
   const int lrow = et >> 1, half = et & 1;
   const int row = row0 + lrow;
   const int frow = 16 * warp + (lane >> 2), fcol = 2 * (lane & 3);
-  WideList<KK> list;
+  WideList<KK, A> list;
   list.init(s_ld + lrow * kStride, s_li + lrow * kStride, half);
-  float acc[TN / 2];
+  A acc[TN / 2];
 #pragma unroll
-  for (int i = 0; i < TN / 2; ++i) acc[i] = 0.0f;
+  for (int i = 0; i < TN / 2; ++i) acc[i] = 0;
 
   int stage = 0; uint32_t phase = 0;
   for (int t = t_begin; t < t_end; ++t) {
@@ -588,8 +687,8 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
       for (int i = 0; i < TN / 2; ++i) fence_operand(acc[i]);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
-        const uint64_t adv = (uint64_t)((k * kWgmmaK * 2) >> 4);
+      for (int k = 0; k < kKSteps; ++k) {
+        const uint64_t adv = (uint64_t)((k * 32) >> 4);
         cross_step<T, TN>(acc, ah + adv, al + adv, bh + adv, bl + adv, (kb | k) != 0);
       }
       wgmma_commit();
@@ -604,20 +703,20 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
     named_bar_sync(1, 128);
 #pragma unroll
     for (int j = 0; j < TN / 8; ++j) {
-      *reinterpret_cast<float2*>(s_acc + frow * kAccS + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
-      *reinterpret_cast<float2*>(s_acc + (frow + 8) * kAccS + 8 * j + fcol) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      *reinterpret_cast<Pair<A>*>(s_acc + frow * kAccS + 8 * j + fcol) = Pair<A>{acc[4 * j], acc[4 * j + 1]};
+      *reinterpret_cast<Pair<A>*>(s_acc + (frow + 8) * kAccS + 8 * j + fcol) = Pair<A>{acc[4 * j + 2], acc[4 * j + 3]};
     }
     if (et < TN) s_norm[et] = __ldg(norms + (int64_t)t * TN + et);
     named_bar_sync(1, 128);
     // both lanes of the row offer every column, in column order
-    const float2* arow = reinterpret_cast<const float2*>(s_acc + lrow * kAccS);
-    const float2* sn = reinterpret_cast<const float2*>(s_norm);
+    const Pair<A>* arow = reinterpret_cast<const Pair<A>*>(s_acc + lrow * kAccS);
+    const Pair<A>* sn = reinterpret_cast<const Pair<A>*>(s_norm);
 #pragma unroll 2
     for (int i = 0; i < TN / 2; ++i) {
-      const float2 a = arow[i], s = sn[i];
+      const Pair<A> a = arow[i], s = sn[i];
       const int col = t * TN + 2 * i;
-      if (col != row && col < n) list.offer(fmaf(-2.0f, a.x, s.x), col);
-      if (col + 1 != row && col + 1 < n) list.offer(fmaf(-2.0f, a.y, s.y), col + 1);
+      if (col != row && col < n) list.offer(tile_score(a.x, s.x), col);
+      if (col + 1 != row && col + 1 < n) list.offer(tile_score(a.y, s.y), col + 1);
     }
   }
   if (qr.has(row)) list.store(cand_idx + qr.list(row) * KK, cand_val + qr.list(row) * KK);
@@ -709,6 +808,10 @@ template int knn_dense_rerank<__half>(int, const __half*, int64_t, int, const in
                                       cudaStream_t);
 template int knn_dense_rerank<__nv_bfloat16>(int, const __nv_bfloat16*, int64_t, int, const int32_t*, int, int32_t*,
                                              float*, cudaStream_t);
+template int knn_dense_rerank<uint8_t>(int, const uint8_t*, int64_t, int, const int32_t*, int, int32_t*, float*,
+                                       cudaStream_t);
+template int knn_dense_rerank<int8_t>(int, const int8_t*, int64_t, int, const int32_t*, int, int32_t*, float*,
+                                      cudaStream_t);
 
 }  // namespace mde
 
@@ -778,16 +881,33 @@ namespace {
 // re-ranked fp32 distance and delta bounds the re-rank's relative rounding, its fp32 distance exceeds d2_k and it
 // cannot enter the list.  A row that fails is searched directly (knn_direct_kernel); a false failure costs time
 // only.  The uncertified rows are appended to rows[] (in no particular order: each is searched on its own) and
-// counted in the header.
+// counted in the header.  8-bit input (A = int): t is exact, and the row certifies when d2_k < (1 - gamma) (t +
+// ||q||^2) (cert_bound), or when t = INT_MAX (no list was ever full: every row was kept).
 // ---------------------------------------------------------------------------------------------------------------
+template <class A>
 __global__ void __launch_bounds__(256)
-knn_certify_kernel(const float* __restrict__ cand_val, int kk, int slices, const float* __restrict__ norms,
+knn_certify_kernel(const A* __restrict__ cand_val, int kk, int slices, const A* __restrict__ norms,
                    const float* __restrict__ d2_out, int k, int64_t lo, int64_t n, CertBound b,
                    unsigned* __restrict__ hdr, int32_t* __restrict__ rows) {
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);  // of the query range
   if (row >= n) return;
-  const float* cv = cand_val + row * slices * kk;
+  const A* cv = cand_val + row * slices * kk;
+  if constexpr (std::is_same_v<A, int>) {
+    int t = INT_MAX;
+    for (int s = 0; s < slices; ++s, cv += kk) {
+      int ts = INT_MIN;
+      for (int q = lane; q < kk; q += 32) ts = max(ts, cv[q]);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) ts = max(ts, __shfl_xor_sync(kFull, ts, o));
+      t = min(t, ts);
+    }
+    if (lane || t == INT_MAX) return;
+    const double D = (double)((int64_t)t + norms[lo + row]);
+    if (!((double)d2_out[row * k + k - 1] < (1.0 - b.gamma) * D))
+      rows[atomicAdd(reinterpret_cast<int*>(hdr + kHdrCount), 1)] = (int32_t)row;
+    return;
+  }
   float t = __int_as_float(0x7f800000);
   for (int s = 0; s < slices; ++s, cv += kk) {
     float ts = -__int_as_float(0x7f800000);
@@ -897,12 +1017,14 @@ int tensor_map_encoder(EncodeTiledFn* out) {
   return 0;
 }
 
-// Tensor map of an n_pad x k_pad 16-bit operand (bf16 or fp16), loaded in boxes of box_rows x 64 (128-byte swizzle).
+// Tensor map of an n_pad x k_pad 16-bit (bf16, fp16) or 8-bit operand, loaded in boxes of box_rows x 128 bytes
+// (128-byte swizzle).
 int make_map(EncodeTiledFn enc, CUtensorMap* map, void* ptr, int64_t n_pad, int k_pad, int box_rows = kTileM,
              CUtensorMapDataType type = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16) {
+  const int elem = type == CU_TENSOR_MAP_DATA_TYPE_UINT8 ? 1 : 2;
   const cuuint64_t dims[2] = {(cuuint64_t)k_pad, (cuuint64_t)n_pad};
-  const cuuint64_t strides[1] = {(cuuint64_t)k_pad * 2};
-  const cuuint32_t box[2] = {(cuuint32_t)kBlockK, (cuuint32_t)box_rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)k_pad * elem};
+  const cuuint32_t box[2] = {(cuuint32_t)(kRowBytes / elem), (cuuint32_t)box_rows};
   const cuuint32_t estr[2] = {1, 1};
   const CUresult r = enc(map, type, 2, ptr, dims, strides, box, estr,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -928,13 +1050,21 @@ int search_slices(int64_t n, int64_t rows, Shape sh) {
   return knn_slices((rows + sh.tm - 1) / sh.tm, n_pad / sh.tn, kNumSMs, kMaxSlices);
 }
 
-// rows: query rows of the search (n for a full one), each with one list of sh.kk candidates per slice; split: fp32
-// input, whose operand has a lo part (16-bit input has none: off_l == off_h, 2 n_pad k_pad bytes fewer)
-KnnLayout knn_layout(int64_t n, int d, int64_t rows, Shape sh, bool split) {
+// The operand of an element type: the bf16 hi / lo split of fp32 input, a 16-bit operand (no lo part: off_l == off_h,
+// 2 n_pad k_pad bytes fewer), or an 8-bit one (1 byte per element, k_pad a multiple of 128, and no centring: no column
+// mean or its sums).
+enum OpKind { kOpSplit, kOp16, kOp8 };
+template <class T>
+constexpr OpKind kOpKind = kInt8<T> ? kOp8 : Operand<T>::kSplit ? kOpSplit : kOp16;
+
+// rows: query rows of the search (n for a full one), each with one list of sh.kk candidates per slice
+KnnLayout knn_layout(int64_t n, int d, int64_t rows, Shape sh, OpKind op) {
   KnnLayout L;
+  const int elem = op == kOp8 ? 1 : 2, block_k = kRowBytes / elem;
+  const bool split = op == kOpSplit, centring = op != kOp8;
   L.n_pad = (n + kTileN - 1) / kTileN * kTileN;
-  L.k_pad = (d + kBlockK - 1) / kBlockK * kBlockK;
-  L.chunks = (int)((n + kMeanChunk - 1) / kMeanChunk);
+  L.k_pad = (d + block_k - 1) / block_k * block_k;
+  L.chunks = centring ? (int)((n + kMeanChunk - 1) / kMeanChunk) : 0;
   L.slices = search_slices(n, rows, sh);
   // room for the lists of rows x S query rows: rows itself, or, when the rule may split, the most a split can hold
   // (q_tiles S <= kNumSMs, S <= kMaxSlices).  Monotone in rows: a workspace sized for a search fits every smaller one.
@@ -946,13 +1076,13 @@ KnnLayout knn_layout(int64_t n, int d, int64_t rows, Shape sh, bool split) {
   const size_t lists = (size_t)cap * sh.kk;
   auto up = [](size_t x) { return (x + 1023) / 1024 * 1024; };
   size_t o = 0;
-  L.off_h = o; o = up(o + (size_t)L.n_pad * L.k_pad * 2);
+  L.off_h = o; o = up(o + (size_t)L.n_pad * L.k_pad * elem);
   L.off_l = split ? o : L.off_h;
   if (split) o = up(o + (size_t)L.n_pad * L.k_pad * 2);
   L.off_norm = o; o = up(o + (size_t)L.n_pad * 4);
   L.off_ci = o; o = up(o + lists * 4);
   L.off_cv = o; o = up(o + lists * 4);
-  L.off_mu = o; o = up(o + (size_t)d * 4);                   // column mean
+  L.off_mu = o; o = up(o + (centring ? (size_t)d * 4 : 0));  // column mean
   L.off_part = o; o = up(o + (size_t)L.chunks * d * 8);      // its per-chunk fp64 sums
   L.off_hdr = o; o = up(o + 4 * kHdrWords);                  // the search header (kHdr*)
   L.off_rows = o; o = up(o + (size_t)rows * 4);              // the uncertified rows
@@ -967,16 +1097,18 @@ int centre_and_prep(const T* X, int64_t n, int d, const KnnLayout& L, uint8_t* w
   float* mu = reinterpret_cast<float*>(w + L.off_mu);
   unsigned* hdr = reinterpret_cast<unsigned*>(w + L.off_hdr);
   MDE_CUDA_TRY(cudaMemsetAsync(hdr, 0, 4 * kHdrWords, st));
-  const unsigned gy = (unsigned)(L.chunks < kMaxGridY ? L.chunks : kMaxGridY);
-  knn_colsum_kernel<T><<<dim3((unsigned)((d + 127) / 128), gy), 128, 0, st>>>(X, n, d, L.chunks, part);
-  MDE_LAUNCH_CHECK();
-  knn_mean_kernel<<<(unsigned)((d + 127) / 128), 128, 0, st>>>(part, L.chunks, n, d, mu);
-  MDE_LAUNCH_CHECK();
-  knn_maxnorm_kernel<T><<<(unsigned)((n + 7) / 8), 256, 0, st>>>(X, n, d, mu, hdr);
-  MDE_LAUNCH_CHECK();
+  if constexpr (!kInt8<T>) {  // an 8-bit operand is exact wherever the data sits: no centring
+    const unsigned gy = (unsigned)(L.chunks < kMaxGridY ? L.chunks : kMaxGridY);
+    knn_colsum_kernel<T><<<dim3((unsigned)((d + 127) / 128), gy), 128, 0, st>>>(X, n, d, L.chunks, part);
+    MDE_LAUNCH_CHECK();
+    knn_mean_kernel<<<(unsigned)((d + 127) / 128), 128, 0, st>>>(part, L.chunks, n, d, mu);
+    MDE_LAUNCH_CHECK();
+    knn_maxnorm_kernel<T><<<(unsigned)((n + 7) / 8), 256, 0, st>>>(X, n, d, mu, hdr);
+    MDE_LAUNCH_CHECK();
+  }
   knn_prep_kernel<T><<<(unsigned)((L.n_pad + 7) / 8), 256, 0, st>>>(
       X, n, d, L.n_pad, L.k_pad, mu, cert_bound<T>(d, L.k_pad), reinterpret_cast<OpT<T>*>(w + L.off_h),
-      reinterpret_cast<__nv_bfloat16*>(w + L.off_l), reinterpret_cast<float*>(w + L.off_norm), hdr);
+      reinterpret_cast<__nv_bfloat16*>(w + L.off_l), reinterpret_cast<AccT<T>*>(w + L.off_norm), hdr);
   MDE_LAUNCH_CHECK();
   return 0;
 }
@@ -1001,9 +1133,9 @@ int rerank_certify(int kk, const T* X, int64_t n, int d, int64_t lo, int64_t hi,
   unsigned* hdr = reinterpret_cast<unsigned*>(w + L.off_hdr);
   int32_t* uncert = reinterpret_cast<int32_t*>(w + L.off_rows);
   const unsigned grid = (unsigned)((rows + 7) / 8);
-  knn_certify_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const float*>(w + L.off_cv), kk, L.slices,
-                                           reinterpret_cast<const float*>(w + L.off_norm), d2_out, k, lo, rows,
-                                           cert_bound<T>(d, L.k_pad), hdr, uncert);
+  knn_certify_kernel<AccT<T>><<<grid, 256, 0, st>>>(reinterpret_cast<const AccT<T>*>(w + L.off_cv), kk, L.slices,
+                                                    reinterpret_cast<const AccT<T>*>(w + L.off_norm), d2_out, k, lo,
+                                                    rows, cert_bound<T>(d, L.k_pad), hdr, uncert);
   MDE_LAUNCH_CHECK();
   knn_direct_kernel<T><<<grid, 256, 0, st>>>(X, n, d, k, lo, hdr, uncert, idx_out, d2_out);
   MDE_LAUNCH_CHECK();
@@ -1021,14 +1153,21 @@ bool bad_search_args(const void* X, int64_t n, int d, int64_t lo, int64_t hi, in
          hi > n || lo >= hi;
 }
 
-// mde_knn / mde_knn16 / the narrow mde_knn_rows: centring and prep, tiles (in S candidate slices), re-rank of the 32
+// 8-bit input wider than d_max: its tile sums could leave int32 (the caller searches X.float() instead)
+template <class T>
+bool too_wide(int d) {
+  if constexpr (kInt8<T>) return d > knn8_max_d<T>();
+  else return false;
+}
+
+// mde_knn / mde_knn16 / mde_knn8 / the narrow mde_knn_rows: centring and prep, tiles (in S candidate slices), re-rank of the 32
 // candidates (merge of the 32 S), certificate and direct search.
 template <class T>
 int run_narrow(const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int32_t* idx_out, float* d2_out, void* ws,
                size_t ws_bytes, void* stream, int* fallback_rows) {
   if (bad_search_args(X, n, d, lo, hi, k, kMaxK, idx_out, d2_out, ws)) return MDE_E_INVALID;
-  if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
-  const KnnLayout L = knn_layout(n, d, hi - lo, kNarrow, Operand<T>::kSplit);
+  if (n > (1ll << 31) - kTileN || too_wide<T>(d)) return MDE_E_UNSUPPORTED;
+  const KnnLayout L = knn_layout(n, d, hi - lo, kNarrow, kOpKind<T>);
   if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   EncodeTiledFn enc = nullptr;
@@ -1037,9 +1176,9 @@ int run_narrow(const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int3
   uint8_t* w = static_cast<uint8_t*>(ws);
   OpT<T>* Xh = reinterpret_cast<OpT<T>*>(w + L.off_h);
   __nv_bfloat16* Xl = reinterpret_cast<__nv_bfloat16*>(w + L.off_l);
-  float* norms = reinterpret_cast<float*>(w + L.off_norm);
+  AccT<T>* norms = reinterpret_cast<AccT<T>*>(w + L.off_norm);
   int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
-  float* cv = reinterpret_cast<float*>(w + L.off_cv);
+  AccT<T>* cv = reinterpret_cast<AccT<T>*>(w + L.off_cv);
   CUtensorMap mh, ml;
   if ((rc = make_map(enc, &mh, Xh, L.n_pad, L.k_pad, kTileM, Operand<T>::kMapType))) return rc;
   if ((rc = make_map(enc, &ml, Xl, L.n_pad, L.k_pad, kTileM, Operand<T>::kMapType))) return rc;
@@ -1063,8 +1202,8 @@ template <class T, int KK, int TN>
 int run_wide(const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int max_k, int32_t* idx_out, float* d2_out,
              void* ws, size_t ws_bytes, void* stream, int* fallback_rows) {
   if (bad_search_args(X, n, d, lo, hi, k, max_k, idx_out, d2_out, ws)) return MDE_E_INVALID;
-  if (n > (1ll << 31) - kTileN) return MDE_E_UNSUPPORTED;
-  const KnnLayout L = knn_layout(n, d, hi - lo, Shape{kWideTileM, TN, KK}, Operand<T>::kSplit);
+  if (n > (1ll << 31) - kTileN || too_wide<T>(d)) return MDE_E_UNSUPPORTED;
+  const KnnLayout L = knn_layout(n, d, hi - lo, Shape{kWideTileM, TN, KK}, kOpKind<T>);
   if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   EncodeTiledFn enc = nullptr;
@@ -1073,9 +1212,9 @@ int run_wide(const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int ma
   uint8_t* w = static_cast<uint8_t*>(ws);
   OpT<T>* Xh = reinterpret_cast<OpT<T>*>(w + L.off_h);
   __nv_bfloat16* Xl = reinterpret_cast<__nv_bfloat16*>(w + L.off_l);
-  float* norms = reinterpret_cast<float*>(w + L.off_norm);
+  AccT<T>* norms = reinterpret_cast<AccT<T>*>(w + L.off_norm);
   int32_t* ci = reinterpret_cast<int32_t*>(w + L.off_ci);
-  float* cv = reinterpret_cast<float*>(w + L.off_cv);
+  AccT<T>* cv = reinterpret_cast<AccT<T>*>(w + L.off_cv);
   constexpr CUtensorMapDataType kType = Operand<T>::kMapType;
   CUtensorMap mah, mal, mh, ml;  // query operand in 64-row boxes, candidate operand in TN-row boxes
   if ((rc = make_map(enc, &mah, Xh, L.n_pad, L.k_pad, kWideTileM, kType))) return rc;
@@ -1098,11 +1237,17 @@ int run_wide(const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int ma
   return rerank_certify<T>(KK, X, n, d, lo, hi, k, idx_out, d2_out, L, w, st, fallback_rows);
 }
 
-// The 16-bit entries: dtype code -> element type, MDE_E_INVALID for an unknown code (before any CUDA call).
+// The 16-bit and 8-bit entries: dtype code -> element type, MDE_E_INVALID for an unknown code (before any CUDA call).
 template <template <class> class Run, class... A>
 int by_dtype(const void* X, int dtype, A... args) {
   if (dtype == MDE_DTYPE_FP16) return Run<__half>::call(static_cast<const __half*>(X), args...);
   if (dtype == MDE_DTYPE_BF16) return Run<__nv_bfloat16>::call(static_cast<const __nv_bfloat16*>(X), args...);
+  return MDE_E_INVALID;
+}
+template <template <class> class Run, class... A>
+int by_dtype8(const void* X, int dtype, A... args) {
+  if (dtype == MDE_DTYPE_U8) return Run<uint8_t>::call(static_cast<const uint8_t*>(X), args...);
+  if (dtype == MDE_DTYPE_S8) return Run<int8_t>::call(static_cast<const int8_t*>(X), args...);
   return MDE_E_INVALID;
 }
 template <class T>
@@ -1123,7 +1268,7 @@ struct Long {
     return run_wide<T, kLongKK, kLongTileN>(X, n, d, 0, n, k, kLongMaxK, i, d2, ws, b, st, fb);
   }
 };
-// mde_knn_rows / mde_knn16_rows: the narrow search for k <= 24, the wide one up to 64
+// mde_knn_rows / mde_knn16_rows / mde_knn8_rows: the narrow search for k <= 24, the wide one up to 64
 template <class T>
 struct Rows {
   static int call(const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int32_t* i, float* d2, void* ws,
@@ -1133,15 +1278,15 @@ struct Rows {
   }
 };
 
-int layout_bytes(int64_t n, int d, Shape sh, bool split, size_t* bytes) {
+int layout_bytes(int64_t n, int d, Shape sh, OpKind op, size_t* bytes) {
   if (!bytes || n < 2 || d < 1) return MDE_E_INVALID;
-  *bytes = knn_layout(n, d, n, sh, split).total;
+  *bytes = knn_layout(n, d, n, sh, op).total;
   return 0;
 }
 
-int rows_layout_bytes(int64_t n, int d, int64_t rows, int k, bool split, size_t* bytes) {
+int rows_layout_bytes(int64_t n, int d, int64_t rows, int k, OpKind op, size_t* bytes) {
   if (!bytes || n < 2 || d < 1 || rows < 1 || rows > n || k < 1 || k > kWideMaxK || k > n - 1) return MDE_E_INVALID;
-  *bytes = knn_layout(n, d, rows, k > kMaxK ? kWide : kNarrow, split).total;
+  *bytes = knn_layout(n, d, rows, k > kMaxK ? kWide : kNarrow, op).total;
   return 0;
 }
 
@@ -1151,7 +1296,7 @@ extern "C" {
 
 int mde_knn_max_k(void) { return kMaxK; }
 
-int mde_knn_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kNarrow, true, bytes); }
+int mde_knn_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kNarrow, kOpSplit, bytes); }
 
 int mde_knn_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes,
                void* stream, int* fallback_rows) {
@@ -1165,7 +1310,7 @@ int mde_knn(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2
 
 int mde_knn_wide_max_k(void) { return kWideMaxK; }
 
-int mde_knn_wide_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kWide, true, bytes); }
+int mde_knn_wide_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kWide, kOpSplit, bytes); }
 
 int mde_knn_wide_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                     size_t ws_bytes, void* stream, int* fallback_rows) {
@@ -1180,7 +1325,7 @@ int mde_knn_wide(const float* X, int64_t n, int d, int k, int32_t* idx_out, floa
 
 int mde_knn_long_max_k(void) { return kLongMaxK; }
 
-int mde_knn_long_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kLong, true, bytes); }
+int mde_knn_long_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kLong, kOpSplit, bytes); }
 
 int mde_knn_long_ex(const float* X, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                     size_t ws_bytes, void* stream, int* fallback_rows) {
@@ -1194,7 +1339,7 @@ int mde_knn_long(const float* X, int64_t n, int d, int k, int32_t* idx_out, floa
 }
 
 int mde_knn_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes) {
-  return rows_layout_bytes(n, d, rows, k, true, bytes);
+  return rows_layout_bytes(n, d, rows, k, kOpSplit, bytes);
 }
 
 int mde_knn_rows(const float* X, int64_t n, int d, int64_t row_begin, int64_t row_end, int k, int32_t* idx_out,
@@ -1202,7 +1347,7 @@ int mde_knn_rows(const float* X, int64_t n, int d, int64_t row_begin, int64_t ro
   return Rows<float>::call(X, n, d, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
 }
 
-int mde_knn16_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kNarrow, false, bytes); }
+int mde_knn16_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kNarrow, kOp16, bytes); }
 
 int mde_knn16_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                  size_t ws_bytes, void* stream, int* fallback_rows) {
@@ -1214,7 +1359,7 @@ int mde_knn16(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_ou
   return mde_knn16_ex(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
-int mde_knn16_wide_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kWide, false, bytes); }
+int mde_knn16_wide_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kWide, kOp16, bytes); }
 
 int mde_knn16_wide_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                       size_t ws_bytes, void* stream, int* fallback_rows) {
@@ -1226,7 +1371,7 @@ int mde_knn16_wide(const void* X, int dtype, int64_t n, int d, int k, int32_t* i
   return mde_knn16_wide_ex(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
-int mde_knn16_long_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kLong, false, bytes); }
+int mde_knn16_long_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kLong, kOp16, bytes); }
 
 int mde_knn16_long_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
                       size_t ws_bytes, void* stream, int* fallback_rows) {
@@ -1239,13 +1384,67 @@ int mde_knn16_long(const void* X, int dtype, int64_t n, int d, int k, int32_t* i
 }
 
 int mde_knn16_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes) {
-  return rows_layout_bytes(n, d, rows, k, false, bytes);
+  return rows_layout_bytes(n, d, rows, k, kOp16, bytes);
 }
 
 int mde_knn16_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin, int64_t row_end, int k,
                    int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows) {
   return by_dtype<Rows>(X, dtype, n, d, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
 }
+
+int mde_knn8_max_d(int dtype) {
+  if (dtype == MDE_DTYPE_U8) return knn8_max_d<uint8_t>();
+  if (dtype == MDE_DTYPE_S8) return knn8_max_d<int8_t>();
+  return MDE_E_INVALID;
+}
+
+int mde_knn8_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kNarrow, kOp8, bytes); }
+
+int mde_knn8_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                size_t ws_bytes, void* stream, int* fallback_rows) {
+  return by_dtype8<Narrow>(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
+}
+
+int mde_knn8(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+             size_t ws_bytes, void* stream) {
+  return mde_knn8_ex(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
+}
+
+int mde_knn8_wide_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kWide, kOp8, bytes); }
+
+int mde_knn8_wide_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                     size_t ws_bytes, void* stream, int* fallback_rows) {
+  return by_dtype8<Wide>(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
+}
+
+int mde_knn8_wide(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                  size_t ws_bytes, void* stream) {
+  return mde_knn8_wide_ex(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
+}
+
+int mde_knn8_long_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kLong, kOp8, bytes); }
+
+int mde_knn8_long_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                     size_t ws_bytes, void* stream, int* fallback_rows) {
+  return by_dtype8<Long>(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
+}
+
+int mde_knn8_long(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
+                  size_t ws_bytes, void* stream) {
+  return mde_knn8_long_ex(X, dtype, n, d, k, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
+}
+
+int mde_knn8_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes) {
+  return rows_layout_bytes(n, d, rows, k, kOp8, bytes);
+}
+
+int mde_knn8_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin, int64_t row_end, int k,
+                  int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows) {
+  return by_dtype8<Rows>(X, dtype, n, d, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
+}
+
+// host-side debug entry point: the certificate's gamma for 8-bit input of d columns (cert_bound); -1 for d < 1
+double mde_dbg_knn8_gamma(int d) { return d < 1 ? -1.0 : knn8_gamma(d); }
 
 // host-side debug entry point: the candidate slices (mde_logic.h: knn_slices) of a search of `rows` query rows
 // against n rows with k neighbours (the narrow search up to k = 24, the wide one up to 64); -1 for bad arguments

@@ -17,9 +17,9 @@
 // and the host stops when fewer than 0.001 n KB entries changed or after max(5, ceil(log2 n)) iterations.  The final
 // lists go to the re-rank kernels of mde_knn (knn_rerank_kernel for 32 candidates, knn_wide_rerank_kernel for 96),
 // so the output contract and the distance arithmetic are those of the exact search.  A 16-bit matrix (IEEE fp16 or
-// bf16, mde_knn16_approx) is read in place: DenseRows, the join and the re-rank take the element type as a template
-// parameter and convert each element to fp32 as they load it, so every distance, and with it the whole search, has
-// the bits of the fp32 search on X.float().
+// bf16, mde_knn16_approx) or an 8-bit one (uint8 or int8, mde_knn8_approx) is read in place: DenseRows, the join and
+// the re-rank take the element type as a template parameter and convert each element to fp32 as they load it, so
+// every distance, and with it the whole search, has the bits of the fp32 search on X.float().
 //
 // Determinism.  Offers and reverse samples arrive in a racy order, so they are collected in cascade reservoirs: R
 // 64-bit keys per row, all ones when empty; inserting x runs y = atomicMin(&r[i], x), x = max(x, y) down the slots.
@@ -647,6 +647,24 @@ int mde_knn16_approx_ex(const void* X, int dtype, int64_t n, int d, int k, uint6
 int mde_knn16_approx(const void* X, int dtype, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out,
                      float* d2_out, void* ws, size_t ws_bytes, void* stream) {
   return mde_knn16_approx_ex(X, dtype, n, d, k, seed, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
+}
+
+int mde_knn8_approx_ws_bytes(int64_t n, int d, int k, size_t* bytes) { return mde_knn_approx_ws_bytes(n, d, k, bytes); }
+
+int mde_knn8_approx_ex(const void* X, int dtype, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out,
+                       float* d2_out, void* ws, size_t ws_bytes, void* stream, int* iterations) {
+  if (dtype == MDE_DTYPE_U8)
+    return approx_dense<uint8_t>(static_cast<const uint8_t*>(X), n, d, k, seed, idx_out, d2_out, ws, ws_bytes, stream,
+                                 iterations);
+  if (dtype == MDE_DTYPE_S8)
+    return approx_dense<int8_t>(static_cast<const int8_t*>(X), n, d, k, seed, idx_out, d2_out, ws, ws_bytes, stream,
+                                iterations);
+  return MDE_E_INVALID;
+}
+
+int mde_knn8_approx(const void* X, int dtype, int64_t n, int d, int k, uint64_t seed, int32_t* idx_out,
+                    float* d2_out, void* ws, size_t ws_bytes, void* stream) {
+  return mde_knn8_approx_ex(X, dtype, n, d, k, seed, idx_out, d2_out, ws, ws_bytes, stream, nullptr);
 }
 
 int mde_knn_approx_csr_ws_bytes(int64_t n, int d, int64_t nnz, int k, size_t* bytes) {

@@ -18,8 +18,10 @@ rows for k <= 64 (`mde_knn_approx_csr`, csrc/mde_knn_approx.cu), with the distan
 A float16 / bfloat16 matrix (a torch tensor on any device, or an np.float16 array) is searched in its own precision,
 without an fp32 copy: the `mde_knn16*` entries use it as the tensor-core operand and convert each element to fp32 as
 the re-rank and NN-descent read it, so neighbours and distances are those of the fp32 search on the upcast matrix
-(DESIGN section 11.7).  The routing by k and PYMDE_B200_KNN is unchanged; the GEMM path, and every other dtype,
-still work on an fp32 copy.
+(DESIGN section 11.7).  A uint8 / int8 matrix (raw pixels, genotypes, quantised embeddings) is searched the same way
+by the `mde_knn8*` entries, whose tiles multiply the 8-bit values exactly on the integer tensor cores (DESIGN section
+11.9), up to `mde_knn8_max_d` columns (16 512 for uint8, 43 919 for int8); a wider one is upcast.  The routing by k
+and PYMDE_B200_KNN is unchanged; the GEMM path, and every other dtype, still work on an fp32 copy.
 
 The dense exact searches are exact on data far from the origin and on far-apart clusters: the kernels centre the
 columns when that bounds the score error more tightly (a 16-bit matrix near the origin stays its own exact operand)
@@ -27,8 +29,8 @@ and certify every row, searching the rows that fail directly (DESIGN section 11)
 candidates with fp64 matmuls of the centred matrix, independent of torch's TF32 setting, then re-ranks them by fp32
 distance and index.
 
-`knn_rows_device` searches only a range of rows against all rows (`mde_knn_rows`, `mde_knn16_rows`, and
-`mde_knn_csr_rows` for a scipy.sparse matrix), exactly, at a cost that scales with the rows searched:
+`knn_rows_device` searches only a range of rows against all rows (`mde_knn_rows`, `mde_knn16_rows`,
+`mde_knn8_rows`, and `mde_knn_csr_rows` for a scipy.sparse matrix), exactly, at a cost that scales with the rows searched:
 `pymde_b200.embed_new_points` searches the new rows of a stacked matrix with it (DESIGN section 11.8)."""
 import ctypes as C
 import os
@@ -42,26 +44,42 @@ from .graph import EdgeListGraph, Graph
 from .preprocess import sample_edges  # noqa: F401  (the reference exposes it here as well)
 
 
-# element types the search kernels read in place -> their MDE_DTYPE_* codes (include/mde_b200.h)
-_HALF_DTYPES = {torch.float16: 1, torch.bfloat16: 2}
+# element types the dense search kernels read in place -> (prefix of their C entries, MDE_DTYPE_* code or None for
+# the fp32 entries, which take none; include/mde_b200.h)
+_SEARCH_DTYPES = {torch.float32: ("knn", None), torch.float16: ("knn16", 1), torch.bfloat16: ("knn16", 2),
+                  torch.uint8: ("knn8", 3), torch.int8: ("knn8", 4)}
 
 
-def _to_device_matrix(data, device, keep_half=False):
-    """The dense matrix on `device`, in fp32; with `keep_half`, a dense float16 / bfloat16 matrix keeps its dtype
-    (uploaded at 2 bytes per value)."""
+def _kernel_dtype(X):
+    """Whether the dense search entries read X (a tensor) in its own dtype: fp32, 16-bit, or 8-bit with at most
+    `mde_knn8_max_d` columns (beyond that the integer tile sums could leave int32)."""
+    fam = _SEARCH_DTYPES.get(X.dtype)
+    if fam is None or fam[0] != "knn8":
+        return fam is not None
+    from .. import _lib
+    return X.shape[-1] <= _lib.load().mde_knn8_max_d(fam[1])
+
+
+def _to_device_matrix(data, device, keep_dtype=False):
+    """The dense matrix on `device`, in fp32; with `keep_dtype`, a dense matrix whose dtype the search kernels read
+    in place (`_kernel_dtype`: float16 / bfloat16, uint8 / int8) keeps it (uploaded at 2 or 1 bytes per value)."""
     sparse = sp.issparse(data)
     if sparse:
         data = data.toarray()
     if isinstance(data, np.ndarray):
         data = torch.from_numpy(np.ascontiguousarray(data))
-    if keep_half and not sparse and data.dtype in _HALF_DTYPES:
+    if keep_dtype and not sparse and _kernel_dtype(data):
         return data.to(device=device)
     return data.to(device=device, dtype=torch.float32)
 
 
-def _matrix_args(X):
-    """The leading arguments of a dense search entry: (X,) for fp32, (X, dtype code) for the mde_knn16* entries."""
-    return (X.data_ptr(), _HALF_DTYPES[X.dtype]) if X.dtype in _HALF_DTYPES else (X.data_ptr(),)
+def _entries(lib, X, suffix=""):
+    """(workspace-size function, search function, leading arguments) of the dense search entry `suffix` ("", "_wide",
+    "_long", "_rows", "_approx") of X's dtype: (X,) for the fp32 entries, (X, dtype code) for the others."""
+    prefix, code = _SEARCH_DTYPES[X.dtype]
+    name = "mde_%s%s" % (prefix, suffix)
+    args = (X.data_ptr(),) if code is None else (X.data_ptr(), code)
+    return getattr(lib, name + "_ws_bytes"), getattr(lib, name), args
 
 
 def _to_device_csr(data, device):
@@ -187,16 +205,13 @@ def knn_device(X, k):
     """(indices [n, k] int32, squared distances [n, k] fp32) of the k nearest rows of every row of the CUDA fp32
     matrix X, ascending; the wgmma kernel behind `mde_knn` for k <= 24, `mde_knn_wide` for 24 < k <= 64 and
     `mde_knn_long` for 64 < k <= 256 (include/mde_b200.h).  A float16 / bfloat16 X is read in place by the
-    `mde_knn16*` entries, with the result of X.float()."""
+    `mde_knn16*` entries and a uint8 / int8 X by the `mde_knn8*` entries (upcast above `mde_knn8_max_d` columns),
+    with the result of X.float()."""
     from .. import _lib
     lib = _lib.load()
-    name = "knn16" if X.dtype in _HALF_DTYPES else "knn"
-    if k > lib.mde_knn_wide_max_k():
-        name += "_long"
-    elif k > lib.mde_knn_max_k():
-        name += "_wide"
-    ws_bytes, search = getattr(lib, "mde_%s_ws_bytes" % name), getattr(lib, "mde_" + name)
-    X = X.contiguous()
+    X = (X if _kernel_dtype(X) else X.float()).contiguous()
+    suffix = "_long" if k > lib.mde_knn_wide_max_k() else "_wide" if k > lib.mde_knn_max_k() else ""
+    ws_bytes, search, args = _entries(lib, X, suffix)
     n, d = X.shape
     need = C.c_size_t(0)
     _lib.check(ws_bytes(int(n), int(d), C.byref(need)))
@@ -206,8 +221,8 @@ def knn_device(X, k):
     d2 = torch.empty((n, k), dtype=torch.float32, device=X.device)
     with torch.cuda.device(X.device):
         stream = torch.cuda.current_stream().cuda_stream
-        _lib.check(search(*_matrix_args(X), int(n), int(d), int(k), idx.data_ptr(), d2.data_ptr(),
-                          ws.data_ptr() + off, need.value, stream))
+        _lib.check(search(*args, int(n), int(d), int(k), idx.data_ptr(), d2.data_ptr(), ws.data_ptr() + off,
+                          need.value, stream))
         torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
     return idx, d2
 
@@ -216,9 +231,9 @@ def knn_rows_device(X, k, row_begin, row_end):
     """(indices [r, k], squared distances [r, k] fp32), r = row_end - row_begin: row r of the result is row
     row_begin + r of the exact search of X (its k nearest rows among all n rows of X, itself excluded, ascending by
     (distance, index)).  Always exact: PYMDE_B200_KNN does not apply.  Routes:
-      * a CUDA fp32 / float16 / bfloat16 matrix with k <= 64: `mde_knn_rows` / `mde_knn16_rows` (int32 indices), bit
-        for bit the rows of `knn_device`, at a cost of about r n d rather than n^2 d (other float dtypes are searched
-        in fp32);
+      * a CUDA fp32 / float16 / bfloat16 / uint8 / int8 matrix with k <= 64: `mde_knn_rows` / `mde_knn16_rows` /
+        `mde_knn8_rows` (int32 indices), bit for bit the rows of `knn_device`, at a cost of about r n d rather than
+        n^2 d (other dtypes, and 8-bit matrices wider than `mde_knn8_max_d`, are searched in fp32);
       * a dense matrix with k > 64: the row range of `_gemm_search` (int64 indices), the rows it gives on all of X;
       * a scipy.sparse matrix with k <= 256: `knn_sparse_rows_device` (`mde_knn_csr_rows`, int32 indices), bit for
         bit the rows of `knn_sparse_device`, at a cost of about r n rather than n^2 in the tiles, without densifying;
@@ -236,14 +251,10 @@ def knn_rows_device(X, k, row_begin, row_end):
         if k > lib.mde_knn_long_max_k():
             return _gemm_search(_to_device_matrix(X, dev), k, row_begin=row_begin, row_end=row_end)
         return knn_sparse_rows_device(*_to_device_csr(X, dev), k, row_begin, row_end)
-    if X.dtype not in _HALF_DTYPES:
-        X = X.float()
-    X = X.contiguous()
+    X = (X if _kernel_dtype(X) else X.float()).contiguous()
     if k > lib.mde_knn_wide_max_k():
         return _gemm_search(X.float(), k, row_begin=row_begin, row_end=row_end)
-    half = X.dtype in _HALF_DTYPES
-    ws_bytes, search = ((lib.mde_knn16_rows_ws_bytes, lib.mde_knn16_rows) if half else
-                        (lib.mde_knn_rows_ws_bytes, lib.mde_knn_rows))
+    ws_bytes, search, args = _entries(lib, X, "_rows")
     d, r = int(X.shape[1]), row_end - row_begin
     need = C.c_size_t(0)
     _lib.check(ws_bytes(n, d, r, k, C.byref(need)))
@@ -253,8 +264,8 @@ def knn_rows_device(X, k, row_begin, row_end):
     d2 = torch.empty((r, k), dtype=torch.float32, device=X.device)
     with torch.cuda.device(X.device):
         stream = torch.cuda.current_stream().cuda_stream
-        _lib.check(search(*_matrix_args(X), n, d, row_begin, row_end, k, idx.data_ptr(), d2.data_ptr(),
-                          ws.data_ptr() + off, need.value, stream, None))
+        _lib.check(search(*args, n, d, row_begin, row_end, k, idx.data_ptr(), d2.data_ptr(), ws.data_ptr() + off,
+                          need.value, stream, None))
         torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
     return idx, d2
 
@@ -263,17 +274,15 @@ def knn_approx_device(X, k, seed=None):
     """(indices [n, k] int32, squared distances [n, k] fp32) of k rows found for every row of the CUDA fp32 matrix X
     by NN-descent, ascending by (distance, index), with the exact fp32 distances of `knn_device`
     (`mde_knn_approx`, include/mde_b200.h).  `seed` defaults to a draw from the module RNG, so `pymde_b200.seed(s)`
-    reproduces the result.  A float16 / bfloat16 X is read in place (`mde_knn16_approx`), with the result of
-    X.float()."""
+    reproduces the result.  A float16 / bfloat16 X is read in place (`mde_knn16_approx`), and so is a uint8 / int8 X
+    (`mde_knn8_approx`), with the result of X.float()."""
     from .. import _lib
     lib = _lib.load()
     if seed is None:
         seed = int(util.np_rng().integers(0, 2 ** 62))
-    X = X.contiguous()
+    X = (X if _kernel_dtype(X) else X.float()).contiguous()
     n, d = X.shape
-    half = X.dtype in _HALF_DTYPES
-    ws_bytes, search = ((lib.mde_knn16_approx_ws_bytes, lib.mde_knn16_approx) if half else
-                        (lib.mde_knn_approx_ws_bytes, lib.mde_knn_approx))
+    ws_bytes, search, args = _entries(lib, X, "_approx")
     need = C.c_size_t(0)
     _lib.check(ws_bytes(int(n), int(d), int(k), C.byref(need)))
     ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=X.device)
@@ -282,7 +291,7 @@ def knn_approx_device(X, k, seed=None):
     d2 = torch.empty((n, k), dtype=torch.float32, device=X.device)
     with torch.cuda.device(X.device):
         stream = torch.cuda.current_stream().cuda_stream
-        _lib.check(search(*_matrix_args(X), int(n), int(d), int(k), C.c_uint64(seed), idx.data_ptr(), d2.data_ptr(),
+        _lib.check(search(*args, int(n), int(d), int(k), C.c_uint64(seed), idx.data_ptr(), d2.data_ptr(),
                           ws.data_ptr() + off, need.value, stream))
         torch.cuda.current_stream().synchronize()  # (the scratch buffer is released on return)
     return idx, d2
@@ -292,8 +301,8 @@ def _search(data, k, dev, chunk_rows=None):
     """The neighbour search of `k_nearest_neighbors`: (idx [n, k'], squared distances [n, k'] fp32, n) of the
     k' = min(k, n - 1) nearest rows of every row, from the search kernels (int32 indices), or from row chunks of a
     library GEMM + top-k (int64 indices) for k' > 256, dense input with 64 < k' <= 256 (unless PYMDE_B200_KNN=approx),
-    `chunk_rows` or PYMDE_B200_KNN=gemm.  A dense float16 / bfloat16 matrix stays in its dtype on the search kernels
-    and is upcast for the GEMM path."""
+    `chunk_rows` or PYMDE_B200_KNN=gemm.  A dense float16 / bfloat16 / uint8 / int8 matrix stays in its dtype on the
+    search kernels (`_kernel_dtype`) and is upcast for the GEMM path."""
     from .. import _lib
     lib = _lib.load()
     mode = os.environ.get("PYMDE_B200_KNN", "kernel")
@@ -310,7 +319,7 @@ def _search(data, k, dev, chunk_rows=None):
             else:
                 idx, d2 = knn_sparse_device(csr, shape, k)
             return idx, d2, n
-    X = _to_device_matrix(data, dev, keep_half=True)
+    X = _to_device_matrix(data, dev, keep_dtype=True)
     n = X.shape[0]
     k = int(min(k, n - 1))
     if use_kernel and 1 <= k <= lib.mde_knn_wide_max_k():
@@ -400,13 +409,13 @@ def k_nearest_neighbors_device_long(data, k, max_distance=None, device=None):
 
 def _pair_distances(data, retain_fraction, dev):
     """(pairs [p, 2] int64 with i < j, Euclidean distances [p] fp32, n) of `distances`, on the device: all pairs in
-    row-major order, or `sample_edges`' sample in its draw order.  A dense float16 / bfloat16 matrix stays in its
-    dtype; each chunk of pairs is upcast, which gives the distances of the fp32 matrix."""
+    row-major order, or `sample_edges`' sample in its draw order.  A dense float16 / bfloat16 / uint8 / int8 matrix
+    stays in its dtype; each chunk of pairs is upcast, which gives the distances of the fp32 matrix."""
     if sp.issparse(data):
         csr, shape = _to_device_csr(data, dev)
         n = shape[0]
     else:
-        X = _to_device_matrix(data, dev, keep_half=True)
+        X = _to_device_matrix(data, dev, keep_dtype=True)
         n = X.shape[0]
     n_all = n * (n - 1) // 2
     if retain_fraction >= 1.0:

@@ -212,7 +212,7 @@ def _new_points_init(items, lists, n_new, embedding, att_edges):
 
 def _stacked_matrix(data, new_data, dev):
     """[data; new_data] for the search: a scipy.sparse CSR matrix when either is sparse, else a device tensor (fp32
-    when the two dtypes differ; a float16 / bfloat16 pair stays 16-bit)."""
+    when the two dtypes differ; a float16 / bfloat16 pair stays 16-bit and a uint8 / int8 pair 8-bit)."""
     if scipy.sparse.issparse(data) or scipy.sparse.issparse(new_data):
         return scipy.sparse.vstack([scipy.sparse.csr_matrix(data), scipy.sparse.csr_matrix(new_data)]).tocsr()
     a, b = (torch.as_tensor(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x for x in (data, new_data))

@@ -68,14 +68,14 @@ def approx(X, k, seed):
     lib = _lib.load()
     n, d = X.shape
     need = C.c_size_t(0)
-    half = X.dtype != torch.float32
-    _lib.check((lib.mde_knn16_approx_ws_bytes if half else lib.mde_knn_approx_ws_bytes)(n, d, k, C.byref(need)))
+    ws_bytes, _, args = dm._entries(lib, X, "_approx")
+    _lib.check(ws_bytes(n, d, k, C.byref(need)))
     ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=dev)
     idx = torch.empty((n, k), dtype=torch.int32, device=dev)
     d2 = torch.empty((n, k), dtype=torch.float32, device=dev)
     it = C.c_int(0)
-    search = lib.mde_knn16_approx_ex if half else lib.mde_knn_approx_ex
-    _lib.check(search(*dm._matrix_args(X), n, d, k, C.c_uint64(seed), idx.data_ptr(), d2.data_ptr(),
+    search = getattr(lib, "mde_%s_approx_ex" % dm._SEARCH_DTYPES[X.dtype][0])
+    _lib.check(search(*args, n, d, k, C.c_uint64(seed), idx.data_ptr(), d2.data_ptr(),
                       ws.data_ptr() + (-ws.data_ptr()) % 1024, need.value, None, C.byref(it)))
     torch.cuda.synchronize()
     return idx, d2, need.value, it.value

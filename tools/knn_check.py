@@ -52,14 +52,14 @@ def wide_only(X, k):
     from pymde_b200 import _lib
     lib = _lib.load()
     n, d = X.shape
-    name = "knn_wide" if X.dtype == torch.float32 else "knn16_wide"
+    ws_bytes, search, args = dm._entries(lib, X, "_wide")
     need = C.c_size_t(0)
-    _lib.check(getattr(lib, "mde_%s_ws_bytes" % name)(n, d, C.byref(need)))
+    _lib.check(ws_bytes(n, d, C.byref(need)))
     ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=X.device)
     idx = torch.empty((n, k), dtype=torch.int32, device=X.device)
     d2 = torch.empty((n, k), dtype=torch.float32, device=X.device)
-    _lib.check(getattr(lib, "mde_" + name)(*dm._matrix_args(X), n, d, k, idx.data_ptr(), d2.data_ptr(),
-                                           ws.data_ptr() + (-ws.data_ptr()) % 1024, need.value, None))
+    _lib.check(search(*args, n, d, k, idx.data_ptr(), d2.data_ptr(), ws.data_ptr() + (-ws.data_ptr()) % 1024,
+                      need.value, None))
     torch.cuda.synchronize()
     return idx, d2
 
