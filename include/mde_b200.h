@@ -650,6 +650,16 @@ int mde_graph_knn_max_k(void);
 int64_t mde_graph_knn_ws_bytes(int64_t n, int batch);
 int mde_graph_knn(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n, int k,
                   double max_distance, int32_t* out_idx, float* out_len, void* ws, int64_t ws_bytes, void* stream);
+/* The same search for the sources [s_begin, s_end) only: output row r (out_idx[r*k .. r*k+k), out_len likewise) is
+ * row s_begin + r of mde_graph_knn on the same CSR, k and max_distance, bit for bit, whatever batch `ws_bytes`
+ * allows (the batch is path_batch of s_end - s_begin sources).  The workspace is sized by mde_graph_knn_ws_bytes; its
+ * distance tile holds n B entries with B >= 32, and each call clears it, so even one source costs O(n) memory and
+ * memset time.  MDE_E_INVALID, before any CUDA call, for a null pointer, n < 1 or n >= 2^31, s_begin < 0,
+ * s_end > n, s_begin > s_end, k outside [1, mde_graph_knn_max_k()] or ws_bytes < mde_graph_knn_ws_bytes(n, 32).
+ * An empty range returns 0 without a launch.  Blocking. */
+int mde_graph_knn_rows(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n,
+                       int64_t s_begin, int64_t s_end, int k, double max_distance, int32_t* out_idx, float* out_len,
+                       void* ws, int64_t ws_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -240,6 +240,8 @@ SIGNATURES = {
     "mde_graph_knn_ws_bytes": (C.c_int64, [C.c_int64, C.c_int]),
     "mde_graph_knn": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_double, C.c_void_p,
                                 C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "mde_graph_knn_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int,
+                                     C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "mde_solver_comm_export": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64]),
     "mde_solver_comm_connect": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]),
 }

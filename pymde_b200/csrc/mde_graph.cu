@@ -346,9 +346,10 @@ __device__ __forceinline__ bool key_less(unsigned long long d0, int v0, unsigned
   return d0 < d1 || (d0 == d1 && v0 < v1);
 }
 
-// step 4: one warp per source; k rounds of a warp-wide minimum of (length, node) above the last one chosen
+// step 4: one warp per source; k rounds of a warp-wide minimum of (length, node) above the last one chosen.
+// Source s0 + b is written to output row s0 + b - row0 (row0: the first source of the call's range).
 __global__ void __launch_bounds__(256)
-knn_select_kernel(PathWs w, int64_t B, int64_t s0, int nsrc, int k, int32_t* __restrict__ out_idx,
+knn_select_kernel(PathWs w, int64_t B, int64_t s0, int64_t row0, int nsrc, int k, int32_t* __restrict__ out_idx,
                   float* __restrict__ out_len) {
   const int b = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
   const int lane = threadIdx.x & 31;
@@ -357,8 +358,8 @@ knn_select_kernel(PathWs w, int64_t B, int64_t s0, int nsrc, int k, int32_t* __r
   const int64_t lo = (int64_t)w.seg_off[b], hi = (int64_t)w.seg_off[b + 1];
   unsigned long long last_d = 0ull;
   int last_v = -1;
-  int32_t* oi = out_idx + (s0 + b) * (int64_t)k;
-  float* ol = out_len + (s0 + b) * (int64_t)k;
+  int32_t* oi = out_idx + (s0 - row0 + b) * (int64_t)k;
+  float* ol = out_len + (s0 - row0 + b) * (int64_t)k;
   for (int j = 0; j < k; ++j) {
     unsigned long long best_d = kUnreached;
     int best_v = 0x7fffffff;
@@ -429,6 +430,28 @@ inline double length_limit(double max_length) {
   return (max_length > 0.0 && max_length < INFINITY) ? max_length : INFINITY;
 }
 
+// k-NN lists of the sources [s_begin, s_end) into output rows 0 .. s_end - s_begin - 1.  Every list is a function of
+// its source alone (the lengths are the schedule-free fixed point, ties break by node index), so it does not depend
+// on the batch size or on where the batches start.
+int graph_knn_range(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n, int64_t s_begin,
+                    int64_t s_end, int k, double max_distance, int32_t* out_idx, float* out_len, void* ws,
+                    int64_t ws_bytes, cudaStream_t st) {
+  const int64_t B = path_batch(n, s_end - s_begin, ws_bytes);
+  const PathWs w = path_ws(ws, n, B);
+  return run_batches(indptr, indices, weights, n, s_begin, s_end, length_limit(max_distance), w, B, st,
+                     [&](int64_t s0, int nsrc) -> int {
+                       MDE_CUDA_TRY(cudaMemsetAsync(w.seg_count, 0, (size_t)B * sizeof(int), st));
+                       knn_count_kernel<<<kRelaxBlocks, 256, 0, st>>>(w, s0);
+                       knn_scan_kernel<<<1, 1024, 0, st>>>(w, (int)B);
+                       knn_scatter_kernel<<<kRelaxBlocks, 256, 0, st>>>(w, s0);
+                       knn_select_kernel<<<(nsrc * 32 + 255) / 256, 256, 0, st>>>(w, B, s0, s_begin, nsrc, k,
+                                                                                  out_idx, out_len);
+                       path_reset_kernel<<<kRelaxBlocks, 256, 0, st>>>(w, B);
+                       g_launch_count += 5;
+                       return 0;
+                     });
+}
+
 }  // namespace
 
 extern "C" {
@@ -470,21 +493,20 @@ int mde_graph_knn(const int32_t* indptr, const int32_t* indices, const float* we
                   double max_distance, int32_t* out_idx, float* out_len, void* ws, int64_t ws_bytes, void* stream) {
   if (!indptr || !indices || n < 1 || n >= (1ll << 31) || k < 1 || k > kKnnMaxK || !out_idx || !out_len || !ws)
     return MDE_E_INVALID;
-  const int64_t B = path_batch(n, n, ws_bytes);
-  if (B < 32) return MDE_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream;
-  const PathWs w = path_ws(ws, n, B);
-  return run_batches(indptr, indices, weights, n, 0, n, length_limit(max_distance), w, B, st,
-                     [&](int64_t s0, int nsrc) -> int {
-                       MDE_CUDA_TRY(cudaMemsetAsync(w.seg_count, 0, (size_t)B * sizeof(int), st));
-                       knn_count_kernel<<<kRelaxBlocks, 256, 0, st>>>(w, s0);
-                       knn_scan_kernel<<<1, 1024, 0, st>>>(w, (int)B);
-                       knn_scatter_kernel<<<kRelaxBlocks, 256, 0, st>>>(w, s0);
-                       knn_select_kernel<<<(nsrc * 32 + 255) / 256, 256, 0, st>>>(w, B, s0, nsrc, k, out_idx, out_len);
-                       path_reset_kernel<<<kRelaxBlocks, 256, 0, st>>>(w, B);
-                       g_launch_count += 5;
-                       return 0;
-                     });
+  if (path_batch(n, n, ws_bytes) < 32) return MDE_E_INVALID;
+  return graph_knn_range(indptr, indices, weights, n, 0, n, k, max_distance, out_idx, out_len, ws, ws_bytes,
+                         (cudaStream_t)stream);
+}
+
+int mde_graph_knn_rows(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n,
+                       int64_t s_begin, int64_t s_end, int k, double max_distance, int32_t* out_idx, float* out_len,
+                       void* ws, int64_t ws_bytes, void* stream) {
+  if (!indptr || !indices || n < 1 || n >= (1ll << 31) || s_begin < 0 || s_end > n || s_begin > s_end || k < 1 ||
+      k > kKnnMaxK || !out_idx || !out_len || !ws || ws_bytes < path_ws_bytes(n, 32))
+    return MDE_E_INVALID;
+  if (s_begin == s_end) return 0;
+  return graph_knn_range(indptr, indices, weights, n, s_begin, s_end, k, max_distance, out_idx, out_len, ws,
+                         ws_bytes, (cudaStream_t)stream);
 }
 
 int mde_graph_hops(const int32_t* indptr, const int32_t* indices, int64_t n, int64_t s_begin, int64_t s_end,

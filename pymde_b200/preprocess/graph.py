@@ -273,6 +273,92 @@ def k_nearest_neighbors_device(graph, k, max_distance=None, device=None):
     return knn_edge_list(idx.view(n, k), n)
 
 
+def _knn_limit(max_distance):
+    """The search radius of `mde_graph_knn`: None, inf or a value <= 0 mean unlimited."""
+    if max_distance is None or not np.isfinite(max_distance) or float(max_distance) <= 0:
+        return np.inf
+    return float(max_distance)
+
+
+def knn_rows_device(graph, k, s_begin, s_end, max_distance=None, device=None):
+    """Shortest-path k-nearest neighbours of the nodes s_begin .. s_end - 1 only, on the GPU (`mde_graph_knn_rows`):
+    (idx [rows, k] int32, len [rows, k] fp32) on the device, row r being row s_begin + r of `mde_graph_knn` bit for
+    bit -- the k smallest (length, node index) pairs within `max_distance`, the node itself excluded, padded with
+    -1 / inf.  The workspace still holds an n x B distance tile (B >= 32), so the memory is that of the full search
+    on the same graph; the time is that of the searched rows."""
+    from .. import _lib, util
+    A = graph.adjacency_matrix if isinstance(graph, Graph) else Graph(graph).adjacency_matrix
+    n = A.shape[0]
+    k, s_begin, s_end = int(k), int(s_begin), int(s_end)
+    dev = util.cuda_device(device)
+    lib = _lib.load()
+    if not 1 <= k <= int(lib.mde_graph_knn_max_k()):
+        raise ValueError("k must be between 1 and %d" % int(lib.mde_graph_knn_max_k()))
+    if not 0 <= s_begin <= s_end <= n:
+        raise ValueError("the rows [%d, %d) are not a range of the %d nodes" % (s_begin, s_end, n))
+    rows = s_end - s_begin
+    idx = torch.empty((rows, k), dtype=torch.int32, device=dev)
+    ln = torch.empty((rows, k), dtype=torch.float32, device=dev)
+    if rows == 0:
+        return idx, ln
+    indptr, indices, weights = _device_csr(A, dev)
+    wptr = None if _is_unweighted(A) else weights.data_ptr()
+    ws = _path_ws(lib.mde_graph_knn_ws_bytes, n, rows, dev)
+    limit = _knn_limit(max_distance)
+    with torch.cuda.device(dev):
+        _lib.check(lib.mde_graph_knn_rows(indptr.data_ptr(), indices.data_ptr(), wptr, n, s_begin, s_end, k,
+                                          0.0 if np.isinf(limit) else limit, idx.data_ptr(), ln.data_ptr(),
+                                          ws.data_ptr(), ws.numel(), util.stream_ptr(dev)))
+    return idx, ln
+
+
+def _smallest_pairs(D, rows, k):
+    """Per row of D [c, n] (fp64, inf = unreached), the k smallest finite (D, column) pairs in lexicographic order,
+    the column rows[i] of row i excluded: (idx [c, k] int32, len [c, k] fp64), padded with -1 / inf."""
+    c, n = D.shape
+    D = D.copy()
+    D[np.arange(c), rows] = np.inf
+    idx = np.full((c, k), -1, dtype=np.int32)
+    ln = np.full((c, k), np.inf)
+    kth = np.partition(D, k - 1, axis=1)[:, k - 1] if k < n else np.full(c, np.inf)
+    r, j = np.nonzero((D <= kth[:, None]) & np.isfinite(D))  # every pair at most the k-th length, ties included
+    d = D[r, j]
+    order = np.lexsort((j, d, r))
+    r, j, d = r[order], j[order], d[order]
+    start = np.searchsorted(r, np.arange(c))
+    slot = np.arange(r.size) - start[r]
+    keep = slot < k
+    idx[r[keep], slot[keep]] = j[keep]
+    ln[r[keep], slot[keep]] = d[keep]
+    return idx, ln
+
+
+def knn_rows_host(graph, k, s_begin, s_end, max_distance=None):
+    """The host restatement of `knn_rows_device` for any k >= 1: scipy's Dijkstra (undirected, `limit` =
+    max_distance) from the nodes s_begin .. s_end - 1 in row chunks, then per row the k smallest (fp64 length, node
+    index) pairs, the node itself excluded.  Returns numpy (idx [rows, k] int32, len [rows, k] fp32), padded with
+    -1 / inf: the device search's lists exactly, since its lengths are scipy's."""
+    A = graph.adjacency_matrix if isinstance(graph, Graph) else Graph(graph).adjacency_matrix
+    n = A.shape[0]
+    k, s_begin, s_end = int(k), int(s_begin), int(s_end)
+    if k < 1:
+        raise ValueError("k must be at least 1")
+    if not 0 <= s_begin <= s_end <= n:
+        raise ValueError("the rows [%d, %d) are not a range of the %d nodes" % (s_begin, s_end, n))
+    A = A.astype(np.float64)  # (float64: parallel entries count as the shortest one, as on the device)
+    limit = _knn_limit(max_distance)
+    idx = np.full((s_end - s_begin, k), -1, dtype=np.int32)
+    ln = np.full((s_end - s_begin, k), np.inf, dtype=np.float32)
+    chunk = max(1, min(n, int(2e7 // max(n, 1))))
+    for r0 in range(s_begin, s_end, chunk):
+        rows = np.arange(r0, min(s_end, r0 + chunk))
+        D = csgraph.dijkstra(A, directed=False, indices=rows, limit=limit)
+        i, d = _smallest_pairs(D, rows, k)
+        idx[r0 - s_begin:r0 - s_begin + rows.size] = i
+        ln[r0 - s_begin:r0 - s_begin + rows.size] = d.astype(np.float32)
+    return idx, ln
+
+
 def knn_edge_list(idx, n):
     """`EdgeListGraph` of the neighbour lists idx [n, k] (device int32, -1 = no entry, 1 <= k <= 256) on their
     device: the edges and weights `Graph.from_edges` gives for the directed pairs (i, idx[i, s]) -- every unordered

@@ -221,23 +221,76 @@ def _stacked_matrix(data, new_data, dev):
     return torch.cat([a.to(dev), b.to(dev)])
 
 
+def _check_new_graph(data, new_data):
+    """`new_data` must span the n_old nodes of `data` and the new ones after them, and hold only edges that touch a
+    new node (ValueError otherwise)."""
+    n_old, n = data.n_items, new_data.n_items
+    if n < n_old:
+        raise ValueError("`new_data` has %d nodes; it must hold the %d nodes of `data` and the new ones after them"
+                         % (n, n_old))
+    B = new_data.adjacency_matrix.tocoo()
+    if bool(((B.row < n_old) & (B.col < n_old)).any()):
+        raise ValueError("`new_data` holds an edge between two fitted nodes (both < %d); pass only the edges that "
+                         "touch a new node" % n_old)
+
+
+def _union_graph(data, new_data):
+    """Adjacency matrix [n, n] of the graph the new nodes are searched in: `data`'s matrix (n_old nodes) padded to
+    n = new_data.n_items, plus `new_data`'s.  After `_check_new_graph` the two share no entry, so the sum is their
+    union."""
+    n_old, n = data.n_items, new_data.n_items
+    A = data.adjacency_matrix
+    indptr = np.concatenate([A.indptr, np.full(n - n_old, A.indptr[-1], dtype=A.indptr.dtype)])
+    padded = scipy.sparse.csr_matrix((A.data, A.indices, indptr), shape=(n, n))
+    return (padded + new_data.adjacency_matrix.tocsr()).tocsr()
+
+
+def _graph_new_lists(data, new_data, k, max_distance, dev):
+    """Neighbour lists [n_new, k] (global ids, -1 = none, on `dev`) of the new nodes n_old .. n - 1 in the union of
+    the two graphs: `graph.knn_rows_device` when the graph searches run on the device and k <= 64, else the host
+    row search (`graph.knn_rows_host`), which gives the same lists.  `max_distance` None: preserve_neighbors' rule,
+    3 times the 75th percentile of the union's edge lengths."""
+    from .preprocess import generic
+    from .preprocess import graph as G
+    n_old, n = data.n_items, new_data.n_items
+    union = _union_graph(data, new_data)
+    if max_distance is None:
+        # the union's edges are those of `data` and of `new_data`, disjoint: the same lengths as Graph(union).distances
+        lengths = torch.cat([data.distances, new_data.distances])
+        max_distance = (3 * torch.quantile(lengths, 0.75)).item() if lengths.numel() else np.inf
+    if generic._graph_on_device(union) and k <= generic._graph_knn_max_k():
+        idx, _ = G.knn_rows_device(union, k, n_old, n, max_distance=max_distance, device=dev)
+        return idx
+    idx, _ = G.knn_rows_host(union, k, n_old, n, max_distance=max_distance)
+    return torch.from_numpy(idx).to(dev)
+
+
 def _new_points_mde(data, embedding, new_data, n_neighbors=None, attractive_penalty=penalties.Log1p,
                     repulsive_penalty=penalties.Log, repulsive_fraction=None, max_distance=None, device=None):
     """Steps 1-5 of `embed_new_points`: (the anchored `MDE` over the new points and the old points they reference,
     with its initial iterate in `_X_init`; items, the global id of each of its items: new points n_old .. n - 1
-    first), or (None, None) when there are no new rows."""
-    for x in (data, new_data):
-        if isinstance(x, Graph):
-            raise ValueError("embed_new_points takes data matrices; a Graph is not supported")
+    first), or (None, None) when there are no new rows.  `data` and `new_data` are two data matrices, or two Graphs
+    (`new_data` over the n_old fitted and the new nodes, holding only edges that touch a new node); every check
+    runs before the device is touched."""
+    graph = isinstance(data, Graph)
+    if graph != isinstance(new_data, Graph):
+        raise ValueError("`data` and `new_data` must both be data matrices or both be Graphs")
     if not isinstance(embedding, (np.ndarray, torch.Tensor)) or embedding.ndim != 2:
         raise ValueError("`embedding` must be a 2-D array (n_old x embedding_dim)")
-    if len(data.shape) != 2 or len(new_data.shape) != 2:
-        raise ValueError("`data` and `new_data` must be 2-D matrices")
-    n_old, n_new = int(data.shape[0]), int(new_data.shape[0])
-    if int(embedding.shape[0]) != n_old:
-        raise ValueError("`embedding` has %d rows; `data` has %d" % (int(embedding.shape[0]), n_old))
-    if int(new_data.shape[1]) != int(data.shape[1]):
-        raise ValueError("`new_data` has %d columns; `data` has %d" % (int(new_data.shape[1]), int(data.shape[1])))
+    if graph:
+        n_old, n_new = data.n_items, new_data.n_items - data.n_items
+        _check_new_graph(data, new_data)
+        if int(embedding.shape[0]) != n_old:
+            raise ValueError("`embedding` has %d rows; `data` has %d nodes" % (int(embedding.shape[0]), n_old))
+    else:
+        if len(data.shape) != 2 or len(new_data.shape) != 2:
+            raise ValueError("`data` and `new_data` must be 2-D matrices")
+        n_old, n_new = int(data.shape[0]), int(new_data.shape[0])
+        if int(embedding.shape[0]) != n_old:
+            raise ValueError("`embedding` has %d rows; `data` has %d" % (int(embedding.shape[0]), n_old))
+        if int(new_data.shape[1]) != int(data.shape[1]):
+            raise ValueError("`new_data` has %d columns; `data` has %d" % (int(new_data.shape[1]),
+                                                                          int(data.shape[1])))
     if n_new == 0:
         return None, None
     if n_old < 1:
@@ -247,10 +300,13 @@ def _new_points_mde(data, embedding, new_data, n_neighbors=None, attractive_pena
     if n_neighbors is None:
         n_neighbors = int(max(min(15, (n * (n - 1) / 2) * 0.01 / n), 5))
     k = int(min(n_neighbors, n - 1))
-    idx, d2 = preprocess.data_matrix.knn_rows_device(_stacked_matrix(data, new_data, dev), k, n_old, n)
-    idx = idx.to(dev)
-    if max_distance is not None:
-        idx = torch.where(d2.to(dev).sqrt() <= max_distance, idx, -1)  # (a NaN distance is dropped)
+    if graph:
+        idx = _graph_new_lists(data, new_data, k, max_distance, dev)
+    else:
+        idx, d2 = preprocess.data_matrix.knn_rows_device(_stacked_matrix(data, new_data, dev), k, n_old, n)
+        idx = idx.to(dev)
+        if max_distance is not None:
+            idx = torch.where(d2.to(dev).sqrt() <= max_distance, idx, -1)  # (a NaN distance is dropped)
     if repulsive_penalty is not None and repulsive_fraction is None:
         repulsive_fraction = 1
     items, lists, edges, weights = _new_points_graph(
@@ -292,13 +348,23 @@ def embed_new_points(data, embedding, new_data, n_neighbors=None, attractive_pen
         neighbours' rows (the column mean of `embedding` when it has none);
       * the anchored problem is solved on the device (`MDE.embed(eps, max_iter)`).
     `data` and `new_data` are dense (numpy, torch; fp32, or float16 / bfloat16 searched in place) or scipy.sparse
-    matrices with the same columns; a Graph is not supported.  Sparse input is stacked on the host and searched
-    without densifying it (`mde_knn_csr_rows`, k <= 256): the tiles sweep only the new rows, and the result is that
-    of the full sparse search."""
+    matrices with the same columns.  Sparse input is stacked on the host and searched without densifying it
+    (`mde_knn_csr_rows`, k <= 256): the tiles sweep only the new rows, and the result is that of the full sparse
+    search.
+
+    Graphs: `data` is the `Graph` of the n_old fitted nodes, and `new_data` a `Graph` over n_old + n_new nodes that
+    holds the edges of the new nodes n_old .. n - 1 -- every edge has at least one end >= n_old, and a new node
+    without edges is allowed -- e.g. `Graph.from_edges(new_edges, weights, n_items=n_old + n_new)`.  The new nodes'
+    lists are their nearest nodes under the shortest-path metric of the union of the two graphs, within
+    `max_distance` (default: 3 times the 75th percentile of the union's edge lengths, `preserve_neighbors`' rule;
+    inf: unlimited), ties broken by node index.  Only the new nodes are searched: `graph.knn_rows_device`
+    (`mde_graph_knn_rows`, the rows of the full device search bit for bit) for k <= 64 on graphs the device searches
+    take, otherwise the host row search `graph.knn_rows_host` (scipy's Dijkstra), which gives the same lists."""
     mde, _ = _new_points_mde(data, embedding, new_data, n_neighbors=n_neighbors,
                              attractive_penalty=attractive_penalty, repulsive_penalty=repulsive_penalty,
                              repulsive_fraction=repulsive_fraction, max_distance=max_distance, device=device)
     if mde is None:
         return torch.empty((0, int(embedding.shape[1])), dtype=torch.float32, device=util.cuda_device(device))
     X = mde.embed(eps=eps, max_iter=max_iter, verbose=verbose)
-    return X[:int(new_data.shape[0])].contiguous()
+    n_new = new_data.n_items - data.n_items if isinstance(new_data, Graph) else int(new_data.shape[0])
+    return X[:n_new].contiguous()
