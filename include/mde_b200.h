@@ -660,6 +660,19 @@ int mde_graph_knn(const int32_t* indptr, const int32_t* indices, const float* we
 int mde_graph_knn_rows(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n,
                        int64_t s_begin, int64_t s_end, int k, double max_distance, int32_t* out_idx, float* out_len,
                        void* ws, int64_t ws_bytes, void* stream);
+/* The same two searches for 1 <= k <= mde_graph_knn_long_max_k() (256): arguments, workspace, output contract, tie
+ * rule, return codes and blocking behaviour of mde_graph_knn and mde_graph_knn_rows, with that bound on k.  For
+ * k <= 64 the lists equal mde_graph_knn's bit for bit; row r of mde_graph_knn_long_rows is row s_begin + r of
+ * mde_graph_knn_long whatever batch `ws_bytes` allows.  The selection takes one block per source and sorts the
+ * source's (length, node) keys in shared memory, or radix-selects the k smallest over a longer segment in the
+ * workspace, so its work per source does not grow with k times the nodes within the radius. */
+int mde_graph_knn_long_max_k(void);
+int mde_graph_knn_long(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n, int k,
+                       double max_distance, int32_t* out_idx, float* out_len, void* ws, int64_t ws_bytes,
+                       void* stream);
+int mde_graph_knn_long_rows(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n,
+                            int64_t s_begin, int64_t s_end, int k, double max_distance, int32_t* out_idx,
+                            float* out_len, void* ws, int64_t ws_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -242,6 +242,12 @@ SIGNATURES = {
                                 C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "mde_graph_knn_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int,
                                      C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "mde_graph_knn_long_max_k": (C.c_int, []),
+    "mde_graph_knn_long": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_double, C.c_void_p,
+                                     C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "mde_graph_knn_long_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64,
+                                          C.c_int, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                          C.c_void_p]),
     "mde_solver_comm_export": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64]),
     "mde_solver_comm_connect": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]),
 }

@@ -384,6 +384,156 @@ knn_select_kernel(PathWs w, int64_t B, int64_t s0, int64_t row0, int nsrc, int k
   }
 }
 
+// step 4 for 1 <= k <= kKnnLongMaxK (mde_graph_knn_long*): one CTA per source, the same lists as knn_select_kernel.
+// A selection key is the 96-bit (fp64 length bits, node index) pair, unique within a source.  Segments of at most
+// kLongSmem entries are sorted whole in shared memory.  Longer ones (a hub, an unlimited radius) never sit in shared
+// memory: an MSB radix select, 8 bits per pass over the segment in global memory, finds the k-th key, starting below
+// the common prefix of the segment's smallest and largest keys and stopping at the first digit whose bin holds exactly
+// the keys still wanted; the <= k winners are then compacted into shared memory and sorted.  So the work per source is
+// O(passes x segment) whatever k, and ties cost at most the 4 passes over the node-index bits.
+constexpr int kKnnLongMaxK = 256;
+constexpr int kLongThreads = 256;
+constexpr int kLongSmem = 2048;   // keys sorted whole in shared memory: 24 KB
+
+typedef unsigned __int128 u128;
+
+__device__ __forceinline__ u128 long_key(const PathWs& w, int64_t B, int b, int v) {
+  return ((u128)w.dist[(int64_t)v * B + b] << 32) | (uint32_t)v;
+}
+
+// ascending bitonic sort of sd / sv [0, len) in shared memory, len a power of two; ends with a barrier
+__device__ void long_sort(unsigned long long* sd, int* sv, int len) {
+  for (int size = 2; size <= len; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int i = threadIdx.x; i < (len >> 1); i += kLongThreads) {
+        const int lo = 2 * stride * (i / stride) + (i % stride), hi = lo + stride;
+        const bool up = (lo & size) == 0;
+        if (key_less(sd[hi], sv[hi], sd[lo], sv[lo]) == up) {
+          const unsigned long long td = sd[lo]; sd[lo] = sd[hi]; sd[hi] = td;
+          const int tv = sv[lo]; sv[lo] = sv[hi]; sv[hi] = tv;
+        }
+      }
+      __syncthreads();
+    }
+  }
+}
+
+__device__ __forceinline__ u128 shfl_xor_u128(u128 x, int off) {
+  const unsigned long long hi = __shfl_xor_sync(kFull, (unsigned long long)(x >> 64), off);
+  const unsigned long long lo = __shfl_xor_sync(kFull, (unsigned long long)x, off);
+  return ((u128)hi << 64) | lo;
+}
+
+__global__ void __launch_bounds__(kLongThreads)
+knn_select_long_kernel(PathWs w, int64_t B, int64_t s0, int64_t row0, int k, int32_t* __restrict__ out_idx,
+                       float* __restrict__ out_len) {
+  __shared__ unsigned long long sd[kLongSmem];
+  __shared__ int sv[kLongSmem];
+  __shared__ int hist[256];
+  __shared__ u128 red[2][kLongThreads / 32];
+  __shared__ int sel_bin, sel_below, sel_cnt, n_win;
+  const int b = blockIdx.x, t = threadIdx.x, lane = t & 31, wid = t >> 5;
+  const int32_t* seg = reinterpret_cast<const int32_t*>(w.queue[0]);
+  const int64_t lo = (int64_t)w.seg_off[b], len = (int64_t)w.seg_off[b + 1] - lo;
+  int m;  // keys in sd / sv to sort: the whole segment, or the k winners
+  if (len <= kLongSmem) {
+    for (int i = t; i < (int)len; i += kLongThreads) {
+      const int v = seg[lo + i];
+      sd[i] = w.dist[(int64_t)v * B + b];
+      sv[i] = v;
+    }
+    m = (int)len;
+  } else {
+    // the smallest and largest key: every key shares their common prefix
+    u128 kmin = ~(u128)0, kmax = 0;
+    for (int64_t i = t; i < len; i += kLongThreads) {
+      const u128 key = long_key(w, B, b, seg[lo + i]);
+      kmin = key < kmin ? key : kmin;
+      kmax = key > kmax ? key : kmax;
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      const u128 a = shfl_xor_u128(kmin, off), c = shfl_xor_u128(kmax, off);
+      kmin = a < kmin ? a : kmin;
+      kmax = c > kmax ? c : kmax;
+    }
+    if (lane == 0) { red[0][wid] = kmin; red[1][wid] = kmax; }
+    __syncthreads();
+    kmin = red[0][0]; kmax = red[1][0];
+    for (int i = 1; i < kLongThreads / 32; ++i) {
+      kmin = red[0][i] < kmin ? red[0][i] : kmin;
+      kmax = red[1][i] > kmax ? red[1][i] : kmax;
+    }
+    // keys are distinct and len > k, so kmin != kmax; s is the digit holding the highest differing bit
+    const u128 diff = kmin ^ kmax;
+    const unsigned long long dh = (unsigned long long)(diff >> 64), dl = (unsigned long long)diff;
+    const int top = dh ? 128 - __clzll((long long)dh) : 64 - __clzll((long long)dl);
+    int s = ((top - 1) / 8) * 8;
+    u128 prefix = (kmin >> (s + 8)) << (s + 8);
+    int want = k;
+    for (;;) {
+      hist[t] = 0;
+      __syncthreads();
+      for (int64_t base = 0; base < len; base += kLongThreads) {  // block-uniform trip count: whole warps below
+        const int64_t i = base + t;
+        int digit = -1;
+        if (i < len) {
+          const u128 key = long_key(w, B, b, seg[lo + i]);
+          if ((key >> (s + 8)) == (prefix >> (s + 8))) digit = (int)((unsigned)(key >> s) & 255u);
+        }
+        const unsigned peers = __match_any_sync(kFull, digit);
+        if (digit >= 0 && lane == __ffs(peers) - 1) atomicAdd(&hist[digit], __popc(peers));
+      }
+      __syncthreads();
+      // exclusive scan of the 256 bins; the thread whose bin holds the want-th key publishes it
+      const int c = hist[t];
+      int incl = c;
+#pragma unroll
+      for (int off = 1; off < 32; off <<= 1) {
+        const int o = __shfl_up_sync(kFull, incl, off);
+        if (lane >= off) incl += o;
+      }
+      __syncthreads();  // every hist[t] read before the warp totals overwrite hist[0 .. 7]
+      if (lane == 31) hist[wid] = incl;
+      __syncthreads();
+      int ex = incl - c;
+      for (int i = 0; i < wid; ++i) ex += hist[i];
+      if (ex < want && want <= ex + c) { sel_bin = t; sel_below = ex; sel_cnt = c; }
+      __syncthreads();
+      prefix |= (u128)sel_bin << s;
+      want -= sel_below;
+      if (sel_cnt == want) break;  // (at s = 0 a bin holds one key, so the loop ends there at the latest)
+      s -= 8;
+    }
+    // the winners: every key whose digits down to s are at most the prefix's, exactly k of them
+    if (t == 0) n_win = 0;
+    __syncthreads();
+    const u128 bound = prefix >> s;
+    for (int64_t i = t; i < len; i += kLongThreads) {
+      const int v = seg[lo + i];
+      const u128 key = long_key(w, B, b, v);
+      if ((key >> s) <= bound) {
+        const int p = atomicAdd(&n_win, 1);
+        sd[p] = (unsigned long long)(key >> 32);
+        sv[p] = v;
+      }
+    }
+    m = k;
+  }
+  int len2 = 32;
+  while (len2 < m) len2 <<= 1;
+  for (int i = m + t; i < len2; i += kLongThreads) { sd[i] = kUnreached; sv[i] = 0x7fffffff; }
+  __syncthreads();
+  long_sort(sd, sv, len2);
+  int32_t* oi = out_idx + (s0 - row0 + b) * (int64_t)k;
+  float* ol = out_len + (s0 - row0 + b) * (int64_t)k;
+  for (int j = t; j < k; j += kLongThreads) {
+    const bool found = j < m;
+    oi[j] = found ? sv[j] : -1;
+    ol[j] = found ? (float)__longlong_as_double((long long)sd[j]) : __int_as_float(0x7f800000);
+  }
+}
+
 __global__ void path_reset_kernel(PathWs w, int64_t B) {
   const unsigned long long nt = w.ctr->touched;
   for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < nt;
@@ -432,10 +582,10 @@ inline double length_limit(double max_length) {
 
 // k-NN lists of the sources [s_begin, s_end) into output rows 0 .. s_end - s_begin - 1.  Every list is a function of
 // its source alone (the lengths are the schedule-free fixed point, ties break by node index), so it does not depend
-// on the batch size or on where the batches start.
+// on the batch size or on where the batches start.  `long_select`: knn_select_long_kernel instead of knn_select_kernel.
 int graph_knn_range(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n, int64_t s_begin,
                     int64_t s_end, int k, double max_distance, int32_t* out_idx, float* out_len, void* ws,
-                    int64_t ws_bytes, cudaStream_t st) {
+                    int64_t ws_bytes, bool long_select, cudaStream_t st) {
   const int64_t B = path_batch(n, s_end - s_begin, ws_bytes);
   const PathWs w = path_ws(ws, n, B);
   return run_batches(indptr, indices, weights, n, s_begin, s_end, length_limit(max_distance), w, B, st,
@@ -444,8 +594,12 @@ int graph_knn_range(const int32_t* indptr, const int32_t* indices, const float* 
                        knn_count_kernel<<<kRelaxBlocks, 256, 0, st>>>(w, s0);
                        knn_scan_kernel<<<1, 1024, 0, st>>>(w, (int)B);
                        knn_scatter_kernel<<<kRelaxBlocks, 256, 0, st>>>(w, s0);
-                       knn_select_kernel<<<(nsrc * 32 + 255) / 256, 256, 0, st>>>(w, B, s0, s_begin, nsrc, k,
-                                                                                  out_idx, out_len);
+                       if (long_select)
+                         knn_select_long_kernel<<<nsrc, kLongThreads, 0, st>>>(w, B, s0, s_begin, k, out_idx,
+                                                                              out_len);
+                       else
+                         knn_select_kernel<<<(nsrc * 32 + 255) / 256, 256, 0, st>>>(w, B, s0, s_begin, nsrc, k,
+                                                                                    out_idx, out_len);
                        path_reset_kernel<<<kRelaxBlocks, 256, 0, st>>>(w, B);
                        g_launch_count += 5;
                        return 0;
@@ -494,7 +648,7 @@ int mde_graph_knn(const int32_t* indptr, const int32_t* indices, const float* we
   if (!indptr || !indices || n < 1 || n >= (1ll << 31) || k < 1 || k > kKnnMaxK || !out_idx || !out_len || !ws)
     return MDE_E_INVALID;
   if (path_batch(n, n, ws_bytes) < 32) return MDE_E_INVALID;
-  return graph_knn_range(indptr, indices, weights, n, 0, n, k, max_distance, out_idx, out_len, ws, ws_bytes,
+  return graph_knn_range(indptr, indices, weights, n, 0, n, k, max_distance, out_idx, out_len, ws, ws_bytes, false,
                          (cudaStream_t)stream);
 }
 
@@ -506,7 +660,30 @@ int mde_graph_knn_rows(const int32_t* indptr, const int32_t* indices, const floa
     return MDE_E_INVALID;
   if (s_begin == s_end) return 0;
   return graph_knn_range(indptr, indices, weights, n, s_begin, s_end, k, max_distance, out_idx, out_len, ws,
-                         ws_bytes, (cudaStream_t)stream);
+                         ws_bytes, false, (cudaStream_t)stream);
+}
+
+int mde_graph_knn_long_max_k(void) { return kKnnLongMaxK; }
+
+int mde_graph_knn_long(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n, int k,
+                       double max_distance, int32_t* out_idx, float* out_len, void* ws, int64_t ws_bytes,
+                       void* stream) {
+  if (!indptr || !indices || n < 1 || n >= (1ll << 31) || k < 1 || k > kKnnLongMaxK || !out_idx || !out_len || !ws)
+    return MDE_E_INVALID;
+  if (path_batch(n, n, ws_bytes) < 32) return MDE_E_INVALID;
+  return graph_knn_range(indptr, indices, weights, n, 0, n, k, max_distance, out_idx, out_len, ws, ws_bytes, true,
+                         (cudaStream_t)stream);
+}
+
+int mde_graph_knn_long_rows(const int32_t* indptr, const int32_t* indices, const float* weights, int64_t n,
+                            int64_t s_begin, int64_t s_end, int k, double max_distance, int32_t* out_idx,
+                            float* out_len, void* ws, int64_t ws_bytes, void* stream) {
+  if (!indptr || !indices || n < 1 || n >= (1ll << 31) || s_begin < 0 || s_end > n || s_begin > s_end || k < 1 ||
+      k > kKnnLongMaxK || !out_idx || !out_len || !ws || ws_bytes < path_ws_bytes(n, 32))
+    return MDE_E_INVALID;
+  if (s_begin == s_end) return 0;
+  return graph_knn_range(indptr, indices, weights, n, s_begin, s_end, k, max_distance, out_idx, out_len, ws,
+                         ws_bytes, true, (cudaStream_t)stream);
 }
 
 int mde_graph_hops(const int32_t* indptr, const int32_t* indices, int64_t n, int64_t s_begin, int64_t s_end,

@@ -252,23 +252,36 @@ def k_nearest_neighbors_device(graph, k, max_distance=None, device=None):
     nearest nodes within `max_distance` (ties broken by node index), as undirected pairs (i < j) sorted by (i, j);
     a pair that is a neighbour in both directions gets weight 2, otherwise 1 -- the edges and weights that
     `k_nearest_neighbors` gives when no lengths tie.  Returns an `EdgeListGraph` on the device."""
+    return _knn_device(graph, k, max_distance, device, long=False)
+
+
+def k_nearest_neighbors_device_long(graph, k, max_distance=None, device=None):
+    """`k_nearest_neighbors_device` for 1 <= k <= 256 (`mde_graph_knn_long`, the same lists as `mde_graph_knn` for
+    k <= 64).  Where lengths tie at the k-th place the lowest node indices are kept, where the host
+    `k_nearest_neighbors` keeps an arbitrary subset of the tied nodes."""
+    return _knn_device(graph, k, max_distance, device, long=True)
+
+
+def _knn_device(graph, k, max_distance, device, long):
     from .. import _lib, util
     A = graph.adjacency_matrix if isinstance(graph, Graph) else Graph(graph).adjacency_matrix
     n = A.shape[0]
     k = int(k)
-    dev = util.cuda_device(device)
     lib = _lib.load()
-    if not 1 <= k <= int(lib.mde_graph_knn_max_k()):
-        raise ValueError("k must be between 1 and %d" % int(lib.mde_graph_knn_max_k()))
+    max_k = int(lib.mde_graph_knn_long_max_k() if long else lib.mde_graph_knn_max_k())
+    if not 1 <= k <= max_k:
+        raise ValueError("k must be between 1 and %d" % max_k)
+    dev = util.cuda_device(device)
     indptr, indices, weights = _device_csr(A, dev)
     wptr = None if _is_unweighted(A) else weights.data_ptr()
     ws = _path_ws(lib.mde_graph_knn_ws_bytes, n, n, dev)
     idx = torch.empty(n * k, dtype=torch.int32, device=dev)
     ln = torch.empty(n * k, dtype=torch.float32, device=dev)
     limit = 0.0 if (max_distance is None or not np.isfinite(max_distance)) else float(max_distance)
+    search = lib.mde_graph_knn_long if long else lib.mde_graph_knn
     with torch.cuda.device(dev):
-        _lib.check(lib.mde_graph_knn(indptr.data_ptr(), indices.data_ptr(), wptr, n, k, limit, idx.data_ptr(),
-                                     ln.data_ptr(), ws.data_ptr(), ws.numel(), util.stream_ptr(dev)))
+        _lib.check(search(indptr.data_ptr(), indices.data_ptr(), wptr, n, k, limit, idx.data_ptr(), ln.data_ptr(),
+                          ws.data_ptr(), ws.numel(), util.stream_ptr(dev)))
     del ws, ln
     return knn_edge_list(idx.view(n, k), n)
 
@@ -286,16 +299,27 @@ def knn_rows_device(graph, k, s_begin, s_end, max_distance=None, device=None):
     bit -- the k smallest (length, node index) pairs within `max_distance`, the node itself excluded, padded with
     -1 / inf.  The workspace still holds an n x B distance tile (B >= 32), so the memory is that of the full search
     on the same graph; the time is that of the searched rows."""
+    return _knn_rows_device(graph, k, s_begin, s_end, max_distance, device, long=False)
+
+
+def knn_rows_device_long(graph, k, s_begin, s_end, max_distance=None, device=None):
+    """`knn_rows_device` for 1 <= k <= 256 (`mde_graph_knn_long_rows`): row r is row s_begin + r of
+    `mde_graph_knn_long` bit for bit, and equals `knn_rows_host`."""
+    return _knn_rows_device(graph, k, s_begin, s_end, max_distance, device, long=True)
+
+
+def _knn_rows_device(graph, k, s_begin, s_end, max_distance, device, long):
     from .. import _lib, util
     A = graph.adjacency_matrix if isinstance(graph, Graph) else Graph(graph).adjacency_matrix
     n = A.shape[0]
     k, s_begin, s_end = int(k), int(s_begin), int(s_end)
-    dev = util.cuda_device(device)
     lib = _lib.load()
-    if not 1 <= k <= int(lib.mde_graph_knn_max_k()):
-        raise ValueError("k must be between 1 and %d" % int(lib.mde_graph_knn_max_k()))
+    max_k = int(lib.mde_graph_knn_long_max_k() if long else lib.mde_graph_knn_max_k())
+    if not 1 <= k <= max_k:
+        raise ValueError("k must be between 1 and %d" % max_k)
     if not 0 <= s_begin <= s_end <= n:
         raise ValueError("the rows [%d, %d) are not a range of the %d nodes" % (s_begin, s_end, n))
+    dev = util.cuda_device(device)
     rows = s_end - s_begin
     idx = torch.empty((rows, k), dtype=torch.int32, device=dev)
     ln = torch.empty((rows, k), dtype=torch.float32, device=dev)
@@ -305,10 +329,11 @@ def knn_rows_device(graph, k, s_begin, s_end, max_distance=None, device=None):
     wptr = None if _is_unweighted(A) else weights.data_ptr()
     ws = _path_ws(lib.mde_graph_knn_ws_bytes, n, rows, dev)
     limit = _knn_limit(max_distance)
+    search = lib.mde_graph_knn_long_rows if long else lib.mde_graph_knn_rows
     with torch.cuda.device(dev):
-        _lib.check(lib.mde_graph_knn_rows(indptr.data_ptr(), indices.data_ptr(), wptr, n, s_begin, s_end, k,
-                                          0.0 if np.isinf(limit) else limit, idx.data_ptr(), ln.data_ptr(),
-                                          ws.data_ptr(), ws.numel(), util.stream_ptr(dev)))
+        _lib.check(search(indptr.data_ptr(), indices.data_ptr(), wptr, n, s_begin, s_end, k,
+                          0.0 if np.isinf(limit) else limit, idx.data_ptr(), ln.data_ptr(), ws.data_ptr(), ws.numel(),
+                          util.stream_ptr(dev)))
     return idx, ln
 
 

@@ -27,6 +27,16 @@ def _knn_graph_max_k(long=False):
     return int(lib.mde_knn_graph_long_max_k() if long else lib.mde_knn_graph_max_k())
 
 
+def _graph_knn_long(A, k):
+    """A graph's k-NN search above mde_graph_knn_max_k() takes the long device search (`mde_graph_knn_long*`) when
+    the graph searches run on the device and k <= mde_graph_knn_long_max_k()."""
+    from . import _lib
+    from .preprocess import generic
+    lib = _lib.load()
+    return (generic._graph_on_device(A)
+            and int(lib.mde_graph_knn_max_k()) < k <= int(lib.mde_graph_knn_long_max_k()))
+
+
 def preserve_distances(data, embedding_dim=2, loss=losses.Absolute, constraint=None, max_distances=5e7,
                        device=None, verbose=False):
     """MDE problem preserving original distances (pymde/recipes.py:103-218).  For a data matrix the pair distances
@@ -58,7 +68,10 @@ def preserve_neighbors(data, embedding_dim=2, attractive_penalty=penalties.Log1p
     """MDE problem preserving local structure (pymde/recipes.py:221-448).  For a data matrix the neighbour graph is
     assembled on the device from the search's lists (`data_matrix.k_nearest_neighbors_device`, or
     `k_nearest_neighbors_device_long` above 64) when min(n_neighbors, n - 1) <= 256; larger n_neighbors keep the
-    chunked GEMM search and the host `Graph`."""
+    chunked GEMM search and the host `Graph`.  For a `Graph` whose searches run on the device, k <= 64 takes
+    `graph.k_nearest_neighbors_device` and 64 < k <= 256 `graph.k_nearest_neighbors_device_long`; both keep the
+    lowest node indices where shortest-path lengths tie at the k-th place (scipy's route, for larger k, tiny graphs
+    or PYMDE_B200_SHORTEST_PATHS=host, keeps an arbitrary subset of the tied nodes)."""
     dev = util.cuda_device(device)
     if isinstance(data, Graph):
         n = data.n_items
@@ -80,7 +93,9 @@ def preserve_neighbors(data, embedding_dim=2, attractive_penalty=penalties.Log1p
         problem.LOGGER.info("Computing %d-nearest neighbors, with max_distance=%s" % (n_neighbors, max_distance))
 
     k = min(n_neighbors, n - 1)
-    if isinstance(data, Graph) or k > _knn_graph_max_k(long=True):
+    if isinstance(data, Graph) and _graph_knn_long(data.adjacency_matrix, k):
+        knn = preprocess.graph.k_nearest_neighbors_device_long(data, k, max_distance=max_distance, device=dev)
+    elif isinstance(data, Graph) or k > _knn_graph_max_k(long=True):
         knn = preprocess.k_nearest_neighbors(data, k=n_neighbors, max_distance=max_distance, verbose=verbose,
                                              device=dev)
     else:
@@ -247,9 +262,10 @@ def _union_graph(data, new_data):
 
 def _graph_new_lists(data, new_data, k, max_distance, dev):
     """Neighbour lists [n_new, k] (global ids, -1 = none, on `dev`) of the new nodes n_old .. n - 1 in the union of
-    the two graphs: `graph.knn_rows_device` when the graph searches run on the device and k <= 64, else the host
-    row search (`graph.knn_rows_host`), which gives the same lists.  `max_distance` None: preserve_neighbors' rule,
-    3 times the 75th percentile of the union's edge lengths."""
+    the two graphs: when the graph searches run on the device, `graph.knn_rows_device` for k <= 64 and
+    `graph.knn_rows_device_long` for k <= 256, else the host row search (`graph.knn_rows_host`), which gives the
+    same lists.  `max_distance` None: preserve_neighbors' rule, 3 times the 75th percentile of the union's edge
+    lengths."""
     from .preprocess import generic
     from .preprocess import graph as G
     n_old, n = data.n_items, new_data.n_items
@@ -260,6 +276,9 @@ def _graph_new_lists(data, new_data, k, max_distance, dev):
         max_distance = (3 * torch.quantile(lengths, 0.75)).item() if lengths.numel() else np.inf
     if generic._graph_on_device(union) and k <= generic._graph_knn_max_k():
         idx, _ = G.knn_rows_device(union, k, n_old, n, max_distance=max_distance, device=dev)
+        return idx
+    if _graph_knn_long(union, k):
+        idx, _ = G.knn_rows_device_long(union, k, n_old, n, max_distance=max_distance, device=dev)
         return idx
     idx, _ = G.knn_rows_host(union, k, n_old, n, max_distance=max_distance)
     return torch.from_numpy(idx).to(dev)
@@ -357,9 +376,10 @@ def embed_new_points(data, embedding, new_data, n_neighbors=None, attractive_pen
     without edges is allowed -- e.g. `Graph.from_edges(new_edges, weights, n_items=n_old + n_new)`.  The new nodes'
     lists are their nearest nodes under the shortest-path metric of the union of the two graphs, within
     `max_distance` (default: 3 times the 75th percentile of the union's edge lengths, `preserve_neighbors`' rule;
-    inf: unlimited), ties broken by node index.  Only the new nodes are searched: `graph.knn_rows_device`
-    (`mde_graph_knn_rows`, the rows of the full device search bit for bit) for k <= 64 on graphs the device searches
-    take, otherwise the host row search `graph.knn_rows_host` (scipy's Dijkstra), which gives the same lists."""
+    inf: unlimited), ties broken by node index.  Only the new nodes are searched: on graphs the device searches take,
+    `graph.knn_rows_device` (`mde_graph_knn_rows`, the rows of the full device search bit for bit) for k <= 64 and
+    `graph.knn_rows_device_long` (`mde_graph_knn_long_rows`) for 64 < k <= 256; otherwise the host row search
+    `graph.knn_rows_host` (scipy's Dijkstra), which gives the same lists."""
     mde, _ = _new_points_mde(data, embedding, new_data, n_neighbors=n_neighbors,
                              attractive_penalty=attractive_penalty, repulsive_penalty=repulsive_penalty,
                              repulsive_fraction=repulsive_fraction, max_distance=max_distance, device=device)
