@@ -527,6 +527,34 @@ int mde_knn_rows(const float* X, int64_t n, int d, int64_t row_begin, int64_t ro
 int mde_knn16_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes);
 int mde_knn16_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin, int64_t row_end, int k,
                    int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows);
+/* The long exact dense searches for a range of query rows: rows [row_begin, row_end) of X against all n rows of X (the
+ * row itself excluded).  Row r of idx_out / d2_out (rows x k, rows = row_end - row_begin) is bit for bit row
+ * row_begin + r of mde_knn_long, mde_knn16_long or mde_knn8_long on the same X and k, ties included (`dtype` as
+ * there).  The cost scales with rows x n, not n^2: the tiles sweep only the query rows, and when those cannot fill
+ * the SMs the candidate sweep is split into S slices (one CTA per query tile and slice; S from the tile counts alone,
+ * mde_dbg_knn_long_slices).  A row's S lists of 288 are merged by selecting their 288 smallest pairs in the tiles' own
+ * (score, index) order, which are exactly the full search's 288 candidates, before the exact re-rank; the certificate
+ * takes the worst of those 288 scores, as the full search does, so both search the same rows directly and report the
+ * same fallback rows.  0 <= row_begin < row_end <= n, 1 <= k <= 256, k <= n - 1; an unknown dtype, a bad argument or
+ * a workspace too small or not 1024-byte aligned is MDE_E_INVALID, and an 8-bit X wider than mde_knn8_max_d(dtype)
+ * MDE_E_UNSUPPORTED, before any CUDA call.  `ws`: 1024-byte aligned device scratch of
+ * mde_knn{,16,8}_long_rows_ws_bytes(n, d, rows, k) bytes (host arithmetic: the operand of the full search, plus
+ * 2.3 KB of candidate lists per query row and slice and 2.3 KB of merged lists per query row; it grows with n and with
+ * rows).  Asynchronous on `stream`; *fallback_rows (nullable; when not null the call waits for the stream) receives
+ * the number of query rows searched directly, as for the _ex entries. */
+int mde_knn_long_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes);
+int mde_knn_long_rows(const float* X, int64_t n, int d, int64_t row_begin, int64_t row_end, int k,
+                      int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows);
+int mde_knn16_long_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes);
+int mde_knn16_long_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin, int64_t row_end, int k,
+                        int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows);
+int mde_knn8_long_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes);
+int mde_knn8_long_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin, int64_t row_end, int k,
+                       int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows);
+/* Host-only: the candidate slices S of mde_knn_long_rows for `rows` query rows against n rows (1 <= k <= 256): as
+ * many as keep q_tiles S within one wave of 132 CTAs, q_tiles = ceil(rows / 64), at most c_tiles = n_pad / 64
+ * (n_pad = n rounded up to 128) and 16; 1 once q_tiles >= 132.  -1 for bad arguments.  For CPU tests. */
+int mde_dbg_knn_long_slices(int64_t n, int64_t rows, int k);
 /* The exact sparse searches for a range of query rows: rows [row_begin, row_end) of a device CSR matrix against all
  * n rows (the row itself excluded).  Row r of idx_out / d2_out (rows x k, rows = row_end - row_begin) is bit for bit
  * row row_begin + r of mde_knn_csr (k <= 24), mde_knn_csr_wide (24 < k <= 64) or mde_knn_csr_long (64 < k <= 256) on

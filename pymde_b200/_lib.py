@@ -169,6 +169,16 @@ SIGNATURES = {
     "mde_knn_rows_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
                                C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
+    "mde_knn_long_rows_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn_long_rows": (C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
+    "mde_dbg_knn_long_slices": (C.c_int, [C.c_int64, C.c_int64, C.c_int]),  # host-only (CPU tests)
+    "mde_knn16_long_rows_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn16_long_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
+    "mde_knn8_long_rows_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
+    "mde_knn8_long_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),
     "mde_knn16_rows_ws_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "mde_knn16_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p,
                                  C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int)]),

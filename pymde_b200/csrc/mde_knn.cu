@@ -33,6 +33,8 @@
 // full search is the range [0, n)).  When the query tiles leave SMs idle the candidate tiles are split into S slices
 // (blockIdx.y; S from mde_logic.h::knn_slices), each CTA keeps its own top-KK, knn_merge_rerank_kernel re-ranks the
 // S KK candidates of a row exactly, and the certificate takes the smallest of the S worst kept scores (DESIGN 11.8).
+// mde_knn_long_rows / mde_knn16_long_rows / mde_knn8_long_rows split the long search the same way; their merge
+// (knn_long_select_kernel) radix-selects the full search's 288 candidates from a row's S 288 before the long re-rank.
 //
 // 16-bit input (mde_knn16, mde_knn16_wide, mde_knn16_long: IEEE fp16 or bf16, read without an fp32 copy).  The element
 // type T is a template parameter of every kernel above.  The prep copies X into a zero-padded operand of its own type
@@ -727,9 +729,10 @@ knn_wide_tile_kernel(const __grid_constant__ CUtensorMap map_ah, const __grid_co
 namespace mde {
 
 // Exact fp32 squared distances of a row's KK candidates (the arithmetic of knn_rerank_kernel), the k smallest in
-// ascending order; lane q owns candidates q, q + 32, q + 64, ..., ranks are taken over all KK.
+// ascending order; lane q owns candidates q, q + 32, q + 64, ..., ranks are taken over all KK.  Row r of the n lists
+// and of the output is row lo + r of X.
 template <class T, int KK>
-__device__ __forceinline__ void wide_rerank_row(const T* __restrict__ X, int64_t n, int d,
+__device__ __forceinline__ void wide_rerank_row(const T* __restrict__ X, int64_t lo, int64_t n, int d,
                                                 const int32_t* __restrict__ cand_idx, int k,
                                                 int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
   const int lane = threadIdx.x & 31;
@@ -738,7 +741,7 @@ __device__ __forceinline__ void wide_rerank_row(const T* __restrict__ X, int64_t
   constexpr int kPer = KK / 32;
   int mine[kPer];
   float my_d[kPer];
-  const T* xq = X + row * d;
+  const T* xq = X + (lo + row) * d;
 #pragma unroll
   for (int s = 0; s < kPer; ++s) {
     mine[s] = cand_idx[row * KK + 32 * s + lane];
@@ -780,15 +783,16 @@ template <class T>
 __global__ void __launch_bounds__(256)
 knn_wide_rerank_kernel(const T* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
                        int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
-  wide_rerank_row<T, kWideKK>(X, n, d, cand_idx, k, out_idx, out_d2);
+  wide_rerank_row<T, kWideKK>(X, 0, n, d, cand_idx, k, out_idx, out_d2);
 }
 
-// the 288 candidates of the long search, with the same arithmetic
+// the 288 candidates of the long search, with the same arithmetic, for the n query rows lo .. lo + n - 1 of X
+// (lo = 0 but for the long row search)
 template <class T>
 __global__ void __launch_bounds__(256)
-knn_long_rerank_kernel(const T* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ cand_idx, int k,
-                       int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
-  wide_rerank_row<T, kLongKK>(X, n, d, cand_idx, k, out_idx, out_d2);
+knn_long_rerank_kernel(const T* __restrict__ X, int64_t lo, int64_t n, int d, const int32_t* __restrict__ cand_idx,
+                       int k, int32_t* __restrict__ out_idx, float* __restrict__ out_d2) {
+  wide_rerank_row<T, kLongKK>(X, lo, n, d, cand_idx, k, out_idx, out_d2);
 }
 
 template <class T>
@@ -797,7 +801,7 @@ int knn_dense_rerank(int kk, const T* X, int64_t n, int d, const int32_t* cand_i
   const unsigned grid = (unsigned)((n + 7) / 8);
   if (kk == kNarrowKK) knn_rerank_kernel<T><<<grid, 256, 0, st>>>(X, n, d, cand_idx, k, out_idx, out_d2);
   else if (kk == kWideKK) knn_wide_rerank_kernel<T><<<grid, 256, 0, st>>>(X, n, d, cand_idx, k, out_idx, out_d2);
-  else if (kk == kLongKK) knn_long_rerank_kernel<T><<<grid, 256, 0, st>>>(X, n, d, cand_idx, k, out_idx, out_d2);
+  else if (kk == kLongKK) knn_long_rerank_kernel<T><<<grid, 256, 0, st>>>(X, 0, n, d, cand_idx, k, out_idx, out_d2);
   else return MDE_E_INVALID;
   MDE_LAUNCH_CHECK();
   return 0;
@@ -864,6 +868,109 @@ knn_merge_rerank_kernel(const T* __restrict__ X, int d, int64_t lo, int64_t rows
       out_idx[r * k + rank] = (int32_t)ij;
       out_d2[r * k + rank] = dj;
     }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// long merge: the candidates of a row searched in S candidate slices by the long tiles (mde_knn_long_rows; DESIGN
+// section 11.8).  Slice y keeps the 288 smallest (score, index) pairs of its candidates in WideList's order (-0 == +0,
+// ties by index, an empty slot as (key_inf, INT_MAX)), a strict total order, so the kept set does not depend on the
+// order of the offers.  Every member of the full search's 288 is among its own slice's 288, so the 288 smallest of
+// the S 288 pairs in the same order are exactly the full search's candidates, and their worst score is the full
+// search's worst kept score.  Ranking S 288 <= 4 608 pairs against each other would cost 21 M comparisons per row, so
+// one CTA per row radix-selects them instead: each pair becomes the 64-bit key (order-preserving bits of the score,
+// index; an empty slot's -1 as 0xffffffff), the keys stay in registers (18 per thread at S = 16), and an MSB-first
+// select over 8-bit digits narrows the prefix of the 288-th key, stopping at the first digit whose bin holds exactly
+// the keys still needed.  Shared memory: a 256-bin histogram and four control words.  The pairs below the prefix, then
+// enough pairs equal to it (only ever identical empty slots), are copied, as the tiles wrote them, to sel[r][.]; their
+// order there is free (the re-rank ranks all 288 and the certificate takes their maximum).
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int kSelThreads = 256;
+constexpr int kSelPer = kMaxSlices * kLongKK / kSelThreads;  // keys per thread at S = kMaxSlices
+static_assert(kMaxSlices * kLongKK % kSelThreads == 0, "whole keys per thread");
+
+// order-preserving unsigned bits of a tile score: -0 and +0 map to the same key
+__device__ __forceinline__ uint32_t score_bits(float v) {
+  uint32_t b = __float_as_uint(v);
+  if (b == 0x80000000u) b = 0u;
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ uint32_t score_bits(int v) { return (uint32_t)v ^ 0x80000000u; }
+
+template <class A>
+__global__ void __launch_bounds__(kSelThreads)
+knn_long_select_kernel(const int32_t* __restrict__ cand_idx, const A* __restrict__ cand_val, int slices,
+                       int32_t* __restrict__ sel, A* __restrict__ sel_val) {
+  __shared__ unsigned s_hist[256];
+  __shared__ unsigned s_ctl[4];  // bin of the 288-th key, keys still needed, count of that bin | output counters
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int64_t r = blockIdx.x;
+  const int cands = slices * kLongKK;
+  const int32_t* ri = cand_idx + r * cands;
+  const A* rv = cand_val + r * cands;
+  uint64_t key[kSelPer];
+#pragma unroll
+  for (int j = 0; j < kSelPer; ++j) {
+    const int c = tid + j * kSelThreads;
+    key[j] = c < cands ? ((uint64_t)score_bits(rv[c]) << 32) | (uint32_t)ri[c] : ~0ull;
+  }
+  uint64_t prefix = 0, mask = 0;
+  unsigned need = kLongKK;  // of the keys that match the prefix
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    s_hist[tid] = 0u;
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < kSelPer; ++j) {
+      const bool in = tid + j * kSelThreads < cands && (key[j] & mask) == prefix;
+      const unsigned bin = in ? (unsigned)(key[j] >> shift) & 255u : 256u;
+      const unsigned peers = __match_any_sync(kFull, bin);  // one shared-memory atomic per bin and warp
+      if (in && lane == __ffs(peers) - 1) atomicAdd(&s_hist[bin], (unsigned)__popc(peers));
+    }
+    __syncthreads();
+    if (tid < 32) {
+      // lane l scans bins 8 l .. 8 l + 7; the lane whose range holds the need-th key finds its bin
+      unsigned h[8], sum = 0;
+#pragma unroll
+      for (int b = 0; b < 8; ++b) { h[b] = s_hist[8 * lane + b]; sum += h[b]; }
+      unsigned incl = sum;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned v = __shfl_up_sync(kFull, incl, o);
+        if (lane >= o) incl += v;
+      }
+      unsigned below = incl - sum;
+      if (below < need && need <= incl) {
+        int b = 0;
+        while (below + h[b] < need) below += h[b++];
+        s_ctl[0] = 8 * lane + b; s_ctl[1] = need - below; s_ctl[2] = h[b];
+      }
+    }
+    __syncthreads();
+    prefix |= (uint64_t)s_ctl[0] << shift;
+    mask |= 0xffull << shift;
+    need = s_ctl[1];
+    const bool done = s_ctl[2] == need;  // the bin holds exactly the keys still needed
+    __syncthreads();                      // (s_ctl and s_hist are rewritten below)
+    if (done) break;
+  }
+  // kLongKK - need keys lie below the prefix; `need` more match it
+  if (tid == 0) { s_ctl[2] = 0u; s_ctl[3] = 0u; }
+  __syncthreads();
+  int32_t* so = sel + r * kLongKK;
+  A* vo = sel_val + r * kLongKK;
+#pragma unroll
+  for (int j = 0; j < kSelPer; ++j) {
+    const int c = tid + j * kSelThreads;
+    if (c >= cands) continue;
+    const uint64_t m = key[j] & mask;
+    int o = -1;
+    if (m < prefix) {
+      o = (int)atomicAdd(&s_ctl[2], 1u);
+    } else if (m == prefix) {
+      const unsigned t = atomicAdd(&s_ctl[3], 1u);
+      if (t < need) o = (int)(kLongKK - need + t);
+    }
+    if (o >= 0) { so[o] = ri[c]; vo[o] = rv[c]; }
   }
 }
 
@@ -1034,18 +1141,20 @@ int make_map(EncodeTiledFn enc, CUtensorMap* map, void* ptr, int64_t n_pad, int 
 
 struct KnnLayout {
   int64_t n_pad; int k_pad, chunks, slices;
-  size_t off_h, off_l, off_norm, off_ci, off_cv, off_mu, off_part, off_hdr, off_rows, total;
+  size_t off_h, off_l, off_norm, off_ci, off_cv, off_sel, off_selv, off_mu, off_part, off_hdr, off_rows, total;
 };
 
 // The tile shape of a search: tm query rows per CTA, tn candidates per tile, kk candidates kept per row (kKK, kWideKK
-// for the wide search, kLongKK for the long one).
-struct Shape { int tm, tn, kk; };
-constexpr Shape kNarrow{kTileM, kTileN, kKK}, kWide{kWideTileM, kTileN, kWideKK}, kLong{kWideTileM, kLongTileN, kLongKK};
+// for the wide search, kLongKK for the long one); split: whether the candidate sweep may be split into slices.
+struct Shape { int tm, tn, kk; bool split; };
+constexpr Shape kNarrow{kTileM, kTileN, kKK, true}, kWide{kWideTileM, kTileN, kWideKK, true};
+// The full long searches keep one slice (their query tiles fill the SMs from n = 8 448 on, and their bits, fallback
+// counts and times stay those of the one-slice sweep); the long row search splits and merges (knn_long_select_kernel).
+constexpr Shape kLong{kWideTileM, kLongTileN, kLongKK, false}, kLongRows{kWideTileM, kLongTileN, kLongKK, true};
 
-// Candidate slices of a search of `rows` query rows against the n rows of X (mde_logic.h: knn_slices).  The long
-// search keeps one: the merge of its 288-candidate lists would not fit in shared memory.
+// Candidate slices of a search of `rows` query rows against the n rows of X (mde_logic.h: knn_slices).
 int search_slices(int64_t n, int64_t rows, Shape sh) {
-  if (sh.kk == kLongKK) return 1;
+  if (!sh.split) return 1;
   const int64_t n_pad = (n + kTileN - 1) / kTileN * kTileN;
   return knn_slices((rows + sh.tm - 1) / sh.tm, n_pad / sh.tn, kNumSMs, kMaxSlices);
 }
@@ -1069,11 +1178,13 @@ KnnLayout knn_layout(int64_t n, int d, int64_t rows, Shape sh, OpKind op) {
   // room for the lists of rows x S query rows: rows itself, or, when the rule may split, the most a split can hold
   // (q_tiles S <= kNumSMs, S <= kMaxSlices).  Monotone in rows: a workspace sized for a search fits every smaller one.
   int64_t cap = rows;
-  if (sh.kk != kLongKK) {
+  if (sh.split) {
     const int64_t split = rows * kMaxSlices < (int64_t)kNumSMs * sh.tm ? rows * kMaxSlices : (int64_t)kNumSMs * sh.tm;
     if (split > cap) cap = split;
   }
   const size_t lists = (size_t)cap * sh.kk;
+  // the long row search's merged lists: one list of kLongKK per query row (knn_long_select_kernel)
+  const size_t merged = sh.split && sh.kk == kLongKK ? (size_t)rows * kLongKK : 0;
   auto up = [](size_t x) { return (x + 1023) / 1024 * 1024; };
   size_t o = 0;
   L.off_h = o; o = up(o + (size_t)L.n_pad * L.k_pad * elem);
@@ -1082,6 +1193,8 @@ KnnLayout knn_layout(int64_t n, int d, int64_t rows, Shape sh, OpKind op) {
   L.off_norm = o; o = up(o + (size_t)L.n_pad * 4);
   L.off_ci = o; o = up(o + lists * 4);
   L.off_cv = o; o = up(o + lists * 4);
+  L.off_sel = o; o = up(o + merged * 4);
+  L.off_selv = o; o = up(o + merged * 4);
   L.off_mu = o; o = up(o + (centring ? (size_t)d * 4 : 0));  // column mean
   L.off_part = o; o = up(o + (size_t)L.chunks * d * 8);      // its per-chunk fp64 sums
   L.off_hdr = o; o = up(o + 4 * kHdrWords);                  // the search header (kHdr*)
@@ -1114,15 +1227,28 @@ int centre_and_prep(const T* X, int64_t n, int d, const KnnLayout& L, uint8_t* w
 }
 
 // After the tiles: re-rank the candidates of every query row (rows lo .. hi - 1 of X; the S KK of a sliced search
-// are merged), certify every row, search the uncertified rows directly; with `fallback_rows`, wait for the stream
+// are merged: by an exact re-rank of all S KK for the narrow and wide searches, by selecting the full search's 288
+// before the long re-rank for the long one), certify every row, search the uncertified rows directly; with `fallback_rows`, wait for the stream
 // and report how many rows that was.  Outputs are compact: row r holds row lo + r of X.
 template <class T>
 int rerank_certify(int kk, const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int32_t* idx_out,
                    float* d2_out, const KnnLayout& L, uint8_t* w, cudaStream_t st, int* fallback_rows) {
+  using A = AccT<T>;
   const int64_t rows = hi - lo;
   const int32_t* ci = reinterpret_cast<const int32_t*>(w + L.off_ci);
-  int rc;
-  if (L.slices == 1 && lo == 0) {
+  const A* cv = reinterpret_cast<const A*>(w + L.off_cv);
+  int slices = L.slices, rc;
+  if (kk == kLongKK) {
+    if (slices > 1) {  // the full search's 288 candidates of each row, from its S lists
+      int32_t* sel = reinterpret_cast<int32_t*>(w + L.off_sel);
+      A* selv = reinterpret_cast<A*>(w + L.off_selv);
+      knn_long_select_kernel<A><<<(unsigned)rows, kSelThreads, 0, st>>>(ci, cv, slices, sel, selv);
+      MDE_LAUNCH_CHECK();
+      ci = sel; cv = selv; slices = 1;
+    }
+    knn_long_rerank_kernel<T><<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(X, lo, rows, d, ci, k, idx_out, d2_out);
+    MDE_LAUNCH_CHECK();
+  } else if (L.slices == 1 && lo == 0) {
     if ((rc = knn_dense_rerank<T>(kk, X, rows, d, ci, k, idx_out, d2_out, st))) return rc;
   } else {
     const int cands = L.slices * kk;
@@ -1133,9 +1259,8 @@ int rerank_certify(int kk, const T* X, int64_t n, int d, int64_t lo, int64_t hi,
   unsigned* hdr = reinterpret_cast<unsigned*>(w + L.off_hdr);
   int32_t* uncert = reinterpret_cast<int32_t*>(w + L.off_rows);
   const unsigned grid = (unsigned)((rows + 7) / 8);
-  knn_certify_kernel<AccT<T>><<<grid, 256, 0, st>>>(reinterpret_cast<const AccT<T>*>(w + L.off_cv), kk, L.slices,
-                                                    reinterpret_cast<const AccT<T>*>(w + L.off_norm), d2_out, k, lo,
-                                                    rows, cert_bound<T>(d, L.k_pad), hdr, uncert);
+  knn_certify_kernel<A><<<grid, 256, 0, st>>>(cv, kk, slices, reinterpret_cast<const A*>(w + L.off_norm), d2_out, k,
+                                             lo, rows, cert_bound<T>(d, L.k_pad), hdr, uncert);
   MDE_LAUNCH_CHECK();
   knn_direct_kernel<T><<<grid, 256, 0, st>>>(X, n, d, k, lo, hdr, uncert, idx_out, d2_out);
   MDE_LAUNCH_CHECK();
@@ -1200,10 +1325,10 @@ int run_narrow(const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int3
 // certificate and direct search.
 template <class T, int KK, int TN>
 int run_wide(const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int max_k, int32_t* idx_out, float* d2_out,
-             void* ws, size_t ws_bytes, void* stream, int* fallback_rows) {
+             void* ws, size_t ws_bytes, void* stream, int* fallback_rows, bool split = KK != kLongKK) {
   if (bad_search_args(X, n, d, lo, hi, k, max_k, idx_out, d2_out, ws)) return MDE_E_INVALID;
   if (n > (1ll << 31) - kTileN || too_wide<T>(d)) return MDE_E_UNSUPPORTED;
-  const KnnLayout L = knn_layout(n, d, hi - lo, Shape{kWideTileM, TN, KK}, kOpKind<T>);
+  const KnnLayout L = knn_layout(n, d, hi - lo, Shape{kWideTileM, TN, KK, split}, kOpKind<T>);
   if (ws_bytes < L.total || (reinterpret_cast<uintptr_t>(ws) & 1023)) return MDE_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   EncodeTiledFn enc = nullptr;
@@ -1268,6 +1393,14 @@ struct Long {
     return run_wide<T, kLongKK, kLongTileN>(X, n, d, 0, n, k, kLongMaxK, i, d2, ws, b, st, fb);
   }
 };
+// mde_knn_long_rows / mde_knn16_long_rows / mde_knn8_long_rows: the long search, split into candidate slices
+template <class T>
+struct LongRows {
+  static int call(const T* X, int64_t n, int d, int64_t lo, int64_t hi, int k, int32_t* i, float* d2, void* ws,
+                  size_t b, void* st, int* fb) {
+    return run_wide<T, kLongKK, kLongTileN>(X, n, d, lo, hi, k, kLongMaxK, i, d2, ws, b, st, fb, true);
+  }
+};
 // mde_knn_rows / mde_knn16_rows / mde_knn8_rows: the narrow search for k <= 24, the wide one up to 64
 template <class T>
 struct Rows {
@@ -1287,6 +1420,12 @@ int layout_bytes(int64_t n, int d, Shape sh, OpKind op, size_t* bytes) {
 int rows_layout_bytes(int64_t n, int d, int64_t rows, int k, OpKind op, size_t* bytes) {
   if (!bytes || n < 2 || d < 1 || rows < 1 || rows > n || k < 1 || k > kWideMaxK || k > n - 1) return MDE_E_INVALID;
   *bytes = knn_layout(n, d, rows, k > kMaxK ? kWide : kNarrow, op).total;
+  return 0;
+}
+
+int long_rows_layout_bytes(int64_t n, int d, int64_t rows, int k, OpKind op, size_t* bytes) {
+  if (!bytes || n < 2 || d < 1 || rows < 1 || rows > n || k < 1 || k > kLongMaxK || k > n - 1) return MDE_E_INVALID;
+  *bytes = knn_layout(n, d, rows, kLongRows, op).total;
   return 0;
 }
 
@@ -1347,6 +1486,15 @@ int mde_knn_rows(const float* X, int64_t n, int d, int64_t row_begin, int64_t ro
   return Rows<float>::call(X, n, d, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
 }
 
+int mde_knn_long_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes) {
+  return long_rows_layout_bytes(n, d, rows, k, kOpSplit, bytes);
+}
+
+int mde_knn_long_rows(const float* X, int64_t n, int d, int64_t row_begin, int64_t row_end, int k, int32_t* idx_out,
+                      float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows) {
+  return LongRows<float>::call(X, n, d, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
+}
+
 int mde_knn16_ws_bytes(int64_t n, int d, size_t* bytes) { return layout_bytes(n, d, kNarrow, kOp16, bytes); }
 
 int mde_knn16_ex(const void* X, int dtype, int64_t n, int d, int k, int32_t* idx_out, float* d2_out, void* ws,
@@ -1390,6 +1538,16 @@ int mde_knn16_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes
 int mde_knn16_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin, int64_t row_end, int k,
                    int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows) {
   return by_dtype<Rows>(X, dtype, n, d, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
+}
+
+int mde_knn16_long_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes) {
+  return long_rows_layout_bytes(n, d, rows, k, kOp16, bytes);
+}
+
+int mde_knn16_long_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin, int64_t row_end, int k,
+                        int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows) {
+  return by_dtype<LongRows>(X, dtype, n, d, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes, stream,
+                            fallback_rows);
 }
 
 int mde_knn8_max_d(int dtype) {
@@ -1443,6 +1601,16 @@ int mde_knn8_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin,
   return by_dtype8<Rows>(X, dtype, n, d, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes, stream, fallback_rows);
 }
 
+int mde_knn8_long_rows_ws_bytes(int64_t n, int d, int64_t rows, int k, size_t* bytes) {
+  return long_rows_layout_bytes(n, d, rows, k, kOp8, bytes);
+}
+
+int mde_knn8_long_rows(const void* X, int dtype, int64_t n, int d, int64_t row_begin, int64_t row_end, int k,
+                       int32_t* idx_out, float* d2_out, void* ws, size_t ws_bytes, void* stream, int* fallback_rows) {
+  return by_dtype8<LongRows>(X, dtype, n, d, row_begin, row_end, k, idx_out, d2_out, ws, ws_bytes, stream,
+                             fallback_rows);
+}
+
 // host-side debug entry point: the certificate's gamma for 8-bit input of d columns (cert_bound); -1 for d < 1
 double mde_dbg_knn8_gamma(int d) { return d < 1 ? -1.0 : knn8_gamma(d); }
 
@@ -1451,6 +1619,13 @@ double mde_dbg_knn8_gamma(int d) { return d < 1 ? -1.0 : knn8_gamma(d); }
 int mde_dbg_knn_slices(int64_t n, int64_t rows, int k) {
   if (n < 2 || rows < 1 || rows > n || k < 1 || k > kWideMaxK) return -1;
   return search_slices(n, rows, k > kMaxK ? kWide : kNarrow);
+}
+
+// host-side debug entry point: the candidate slices of the long row search (mde_knn_long_rows) of `rows` query rows
+// against n rows, 1 <= k <= 256: knn_slices with TM = TN = 64; -1 for bad arguments
+int mde_dbg_knn_long_slices(int64_t n, int64_t rows, int k) {
+  if (n < 2 || rows < 1 || rows > n || k < 1 || k > kLongMaxK) return -1;
+  return search_slices(n, rows, kLongRows);
 }
 
 }  // extern "C"

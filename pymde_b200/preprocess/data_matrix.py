@@ -31,7 +31,10 @@ distance and index.
 
 `knn_rows_device` searches only a range of rows against all rows (`mde_knn_rows`, `mde_knn16_rows`,
 `mde_knn8_rows`, and `mde_knn_csr_rows` for a scipy.sparse matrix), exactly, at a cost that scales with the rows searched:
-`pymde_b200.embed_new_points` searches the new rows of a stacked matrix with it (DESIGN section 11.8)."""
+`pymde_b200.embed_new_points` searches the new rows of a stacked matrix with it (DESIGN section 11.8).  Its dense
+route for k > 64 is the row range of the GEMM path; `knn_rows_device_long` instead takes a dense matrix up to k = 256
+to the long row search (`mde_knn_long_rows`, `mde_knn16_long_rows`, `mde_knn8_long_rows`), which reads a 16-bit or
+8-bit matrix in place and gives the rows of the full long search, certified, bit for bit."""
 import ctypes as C
 import os
 
@@ -254,8 +257,44 @@ def knn_rows_device(X, k, row_begin, row_end):
     X = (X if _kernel_dtype(X) else X.float()).contiguous()
     if k > lib.mde_knn_wide_max_k():
         return _gemm_search(X.float(), k, row_begin=row_begin, row_end=row_end)
-    ws_bytes, search, args = _entries(lib, X, "_rows")
-    d, r = int(X.shape[1]), row_end - row_begin
+    return _dense_rows(lib, X, k, row_begin, row_end, "_rows")
+
+
+def knn_rows_device_long(X, k, row_begin, row_end):
+    """(indices [r, k] int32, squared distances [r, k] fp32), r = row_end - row_begin, for 1 <= k <= 256: row r of
+    the result is row row_begin + r of the full long search of X (`knn_device` at k > 64), bit for bit, ties included;
+    always exact (PYMDE_B200_KNN does not apply).  Routes:
+      * a CUDA fp32 / float16 / bfloat16 / uint8 / int8 matrix: `mde_knn_long_rows` / `mde_knn16_long_rows` /
+        `mde_knn8_long_rows`, read in place, at a cost of about r n d (the candidate sweep is split across the SMs
+        when the query rows are few, DESIGN section 11.8); other dtypes, and 8-bit matrices wider than
+        `mde_knn8_max_d`, are searched in fp32;
+      * a scipy.sparse matrix: `knn_sparse_rows_device` (`mde_knn_csr_rows`), without densifying it.
+    ValueError for a bad range or a k outside [1, min(256, n - 1)]."""
+    from .. import _lib
+    lib = _lib.load()
+    n = int(X.shape[0])
+    row_begin, row_end, k = int(row_begin), int(row_end), int(k)
+    max_k = int(lib.mde_knn_long_max_k())
+    if not 1 <= k <= max_k:
+        raise ValueError("need 1 <= k <= %d; got k = %d" % (max_k, k))
+    if not 0 <= row_begin < row_end <= n:
+        raise ValueError("need 0 <= row_begin < row_end <= n; got [%d, %d) with n = %d" % (row_begin, row_end, n))
+    if k > n - 1:
+        raise ValueError("need 1 <= k <= n - 1; got k = %d with n = %d" % (k, n))
+    if sp.issparse(X):
+        return knn_sparse_rows_device(*_to_device_csr(X, util.cuda_device()), k, row_begin, row_end)
+    if not (isinstance(X, torch.Tensor) and X.is_cuda):  # a host matrix is uploaded in its own dtype
+        X = _to_device_matrix(X, util.cuda_device(), keep_dtype=True)
+    X = (X if _kernel_dtype(X) else X.float()).contiguous()
+    return _dense_rows(lib, X, k, row_begin, row_end, "_long_rows")
+
+
+def _dense_rows(lib, X, k, row_begin, row_end, suffix):
+    """The row-range entry `suffix` ("_rows" or "_long_rows") of X's dtype on rows [row_begin, row_end) of the CUDA
+    matrix X: (indices [r, k] int32, squared distances [r, k] fp32)."""
+    from .. import _lib
+    ws_bytes, search, args = _entries(lib, X, suffix)
+    n, d, r = int(X.shape[0]), int(X.shape[1]), row_end - row_begin
     need = C.c_size_t(0)
     _lib.check(ws_bytes(n, d, r, k, C.byref(need)))
     ws = torch.empty(need.value + 1024, dtype=torch.uint8, device=X.device)

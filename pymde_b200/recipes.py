@@ -284,6 +284,21 @@ def _graph_new_lists(data, new_data, k, max_distance, dev):
     return torch.from_numpy(idx).to(dev)
 
 
+def _dense_new_lists(X, k, n_old, n):
+    """(indices, squared distances) of the new rows n_old .. n - 1 of the stacked matrix X: a float16 / bfloat16 /
+    uint8 / int8 matrix with 64 < k <= 256 takes the long row search (`data_matrix.knn_rows_device_long`, read in
+    place), every other case `data_matrix.knn_rows_device` (k <= 64, sparse input, and the GEMM rows for fp32 at
+    k > 64 and for k > 256).  fp32 stays on the GEMM rows because they measured faster on it (DESIGN section 11.8);
+    for a 16-bit or 8-bit matrix they would make an fp32 and an fp64 copy of the whole stack."""
+    dm = preprocess.data_matrix
+    from . import _lib
+    lib = _lib.load()
+    narrow = isinstance(X, torch.Tensor) and X.dtype in (torch.float16, torch.bfloat16, torch.uint8, torch.int8)
+    if narrow and lib.mde_knn_wide_max_k() < k <= lib.mde_knn_long_max_k():
+        return dm.knn_rows_device_long(X, k, n_old, n)
+    return dm.knn_rows_device(X, k, n_old, n)
+
+
 def _new_points_mde(data, embedding, new_data, n_neighbors=None, attractive_penalty=penalties.Log1p,
                     repulsive_penalty=penalties.Log, repulsive_fraction=None, max_distance=None, device=None):
     """Steps 1-5 of `embed_new_points`: (the anchored `MDE` over the new points and the old points they reference,
@@ -322,7 +337,7 @@ def _new_points_mde(data, embedding, new_data, n_neighbors=None, attractive_pena
     if graph:
         idx = _graph_new_lists(data, new_data, k, max_distance, dev)
     else:
-        idx, d2 = preprocess.data_matrix.knn_rows_device(_stacked_matrix(data, new_data, dev), k, n_old, n)
+        idx, d2 = _dense_new_lists(_stacked_matrix(data, new_data, dev), k, n_old, n)
         idx = idx.to(dev)
         if max_distance is not None:
             idx = torch.where(d2.to(dev).sqrt() <= max_distance, idx, -1)  # (a NaN distance is dropped)
@@ -366,8 +381,12 @@ def embed_new_points(data, embedding, new_data, n_neighbors=None, attractive_pen
       * the fitted points are anchored at their `embedding` rows; a new point starts at the mean of its fitted
         neighbours' rows (the column mean of `embedding` when it has none);
       * the anchored problem is solved on the device (`MDE.embed(eps, max_iter)`).
-    `data` and `new_data` are dense (numpy, torch; fp32, or float16 / bfloat16 searched in place) or scipy.sparse
-    matrices with the same columns.  Sparse input is stacked on the host and searched without densifying it
+    `data` and `new_data` are dense (numpy, torch; fp32, or float16 / bfloat16 / uint8 / int8 searched in place) or
+    scipy.sparse matrices with the same columns.  Dense input is searched by the row-range tensor-core search
+    `mde_knn_rows` up to k = 64, which gives the rows of the full exact search bit for bit.  Above that a 16-bit or
+    8-bit matrix takes the long row search up to k = 256 (`data_matrix.knn_rows_device_long`: the rows of the full
+    long search bit for bit, read in place, without an fp32 copy), and an fp32 matrix, or any k > 256, the row range
+    of the GEMM path.  Sparse input is stacked on the host and searched without densifying it
     (`mde_knn_csr_rows`, k <= 256): the tiles sweep only the new rows, and the result is that of the full sparse
     search.
 
