@@ -229,9 +229,10 @@ int mde_solver_begin(mde_solver_t* s, const float* X0, double eps, void* stream)
  * statistics buffers): one solver object serves embed() calls with different `max_iter`. */
 int mde_solver_begin_ex(mde_solver_t* s, const float* X0, double eps, int max_iter, void* stream);
 /* Run up to `iters` further iterations; stops early on convergence (||grad||_F <= eps,
- * optim.py:165).  Blocking.  On return *iters_done = total iterations so far,
+ * optim.py:165).  Returns once the solve has stopped: *iters_done = total iterations so far,
  * *converged = 1 if the residual test fired.  Returns MDE_E_NAN where the reference raises
- * SolverError. */
+ * SolverError.  Work it enqueued may still be queued on `stream` at return (kernels gated off after the
+ * stop, which write nothing); reads of X, the statistics or the state on `stream` come after it. */
 int mde_solver_run(mde_solver_t* s, int iters, int* iters_done, int* converged, void* stream);
 
 /* Diagnostics: %globaltimer stamps (ns) of the last step that started an iteration:
@@ -239,6 +240,9 @@ int mde_solver_run(mde_solver_t* s, int iters, int* iters_done, int* converged, 
  * [3] partials reduced, [4] previous step finished / phase chosen, [5] history update + two-loop done,
  * [6] before the state is written back, [7] first block of the vector kernel that follows.  No reference counterpart. */
 int mde_solver_debug_times(mde_solver_t* s, unsigned long long* out8, void* stream);
+/* Diagnostics: the steps the last mde_solver_run call that ran the solve enqueued (*launched) and how many of them ran (*ran); the others
+ * exited at their gates after the solve stopped.  No reference counterpart. */
+int mde_solver_debug_run_steps(mde_solver_t* s, int64_t* launched, int64_t* ran);
 /* Diagnostics: the L-BFGS state of a solve paused between two mde_solver_run calls, copied to host buffers (blocking;
  * MDE_E_INVALID when the solve is not paused).  g: (n*m) gradient of the last evaluation; g_prev, d: (n*m) gradient
  * and direction of the last completed iteration; S, Y: (memory_size, n*m) receive the *count stored pairs in logical

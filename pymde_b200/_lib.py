@@ -99,6 +99,7 @@ SIGNATURES = {
     "mde_solver_begin_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_void_p]),
     "mde_solver_run": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_void_p]),
     "mde_solver_debug_times": (C.c_int, [C.c_void_p, C.POINTER(C.c_ulonglong), C.c_void_p]),
+    "mde_solver_debug_run_steps": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "mde_solver_debug_lbfgs": (C.c_int, [C.c_void_p] + [C.c_void_p] * 5 + [C.POINTER(C.c_int), C.POINTER(C.c_double),
                                                                           C.POINTER(C.c_int), C.c_void_p]),
     "mde_solver_x": (C.c_void_p, [C.c_void_p]),
@@ -266,6 +267,7 @@ SIGNATURES = {
 DEBUG_SIGNATURES = {
     "mde_dbg_ls_new": (C.c_void_p, [C.c_double, C.c_double, C.c_float, C.c_float]),
     "mde_dbg_ls_free": (None, [C.c_void_p]),
+    "mde_dbg_feed_policy": (C.c_int, [C.c_int64, C.c_int64]),
     "mde_dbg_ls_t": (C.c_double, [C.c_void_p]),
     "mde_dbg_ls_step": (C.c_int, [C.c_void_p, C.c_double, C.c_float, C.c_int]),
     "mde_dbg_ls_result": (None, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double),

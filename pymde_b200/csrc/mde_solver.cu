@@ -19,6 +19,7 @@
 //  * reference quirk kept on purpose (SURVEY section 7.5): the gradient seen by iteration k+1 is
 //    the one left by the LAST trial of iteration k's line search, the loss is the ACCEPTED
 //    trial's loss.
+#include <chrono>
 #include <cstddef>
 #include <cstdlib>
 #include <cstring>
@@ -67,6 +68,8 @@ struct SolverState {
   int g_eval;      // gates of the next step, written by the head kernel's epilogue: closure evaluation runs
   int g_proj;      //   the iterate moved: retraction kernels run
   unsigned int ticket;  // last-block-done counter of the head kernel
+  int run_seq;     // of the mde_solver_run call that armed the solver (progress word)
+  int run_steps;   // head kernels that ran their scalar stage since that call armed it
   // ---- scalars ----
   double eps;
   double loss;     // f at the current iterate (cached loss, lbfgs.py:418-426,550)
@@ -89,6 +92,34 @@ struct SolverState {
 };
 
 __device__ __forceinline__ bool off(const int* flag) { return *flag == 0; }
+
+// Progress word: one 64-bit word in mapped host memory that resume_kernel and every head kernel's scalar stage
+// overwrite, so that mde_solver_run can keep the step queue fed, and see the solve stop, without synchronising.  One
+// 8-byte store is single-copy atomic, so the host always reads one consistent snapshot and the store needs no fence.
+// Layout: [63] stopped (not active), [62] paused, [61] converged, [60] failed, [59:53] run sequence number,
+// [52:32] steps of this run modulo 2^21, [31:0] completed iterations.
+constexpr int kProgSeqMask = 0x7f;
+constexpr long long kProgStepsMask = (1ll << 21) - 1;
+
+__device__ __forceinline__ void publish_progress(unsigned long long* p, const SolverState* S) {
+  const unsigned long long w =
+      ((unsigned long long)(S->active ? 0 : 1) << 63) | ((unsigned long long)(S->paused ? 1 : 0) << 62) |
+      ((unsigned long long)(S->converged ? 1 : 0) << 61) | ((unsigned long long)(S->error ? 1 : 0) << 60) |
+      ((unsigned long long)(S->run_seq & kProgSeqMask) << 53) | ((unsigned long long)(S->run_steps & kProgStepsMask) << 32) |
+      (unsigned long long)(unsigned)S->iter;
+  asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(p), "l"(w) : "memory");
+}
+
+struct Progress {
+  bool stopped, paused, converged, failed;
+  int seq, iter;
+  long long steps;
+};
+
+inline Progress decode_progress(unsigned long long w) {
+  return {(w >> 63 & 1) != 0, (w >> 62 & 1) != 0, (w >> 61 & 1) != 0, (w >> 60 & 1) != 0,
+          (int)(w >> 53 & kProgSeqMask), (int)(unsigned)w, (long long)(w >> 32 & kProgStepsMask)};
+}
 
 // Fixed-order reduction of K sums over nb block partials into smem out[K]; all threads of the block call.
 // Stage 1: thread t owns (k = t % K, segment = t / K) and walks blocks segment, segment + S, ... in batches of
@@ -695,7 +726,8 @@ __device__ void reduce_head_rows(const double* __restrict__ part, int nb, double
 }
 
 __device__ void step_head_body(SolverState* __restrict__ S, const double* __restrict__ part, int nblocks, Tail tl,
-                               unsigned char* smem, float tpass, int count, unsigned long long t_entry) {
+                               unsigned char* smem, float tpass, int count, unsigned long long t_entry,
+                               unsigned long long* progress) {
   SolverState* sS = reinterpret_cast<SolverState*>(smem);
   double* sums = reinterpret_cast<double*>(smem + sizeof(SolverState));
   double* dots = sums + kMaxSlices * kHeadCols;
@@ -767,6 +799,8 @@ __device__ void step_head_body(SolverState* __restrict__ S, const double* __rest
     }
     s_go = (sS->active && sS->phase == PH_DIR) ? 1 : 0;
     s_dirty = (s_go || sS->lb.n_iter != n_iter) ? 1 : 0;  // (opt.reset() at the end of an iteration)
+    sS->run_steps += 1;
+    publish_progress(progress, sS);
     s_t[3] = gtime();
   }
   __syncthreads();
@@ -860,7 +894,7 @@ __global__ void __launch_bounds__(kVecThreads, 2)
 step_head_kernel(SolverState* __restrict__ S, const float* __restrict__ g, const float* __restrict__ gprev,
                  const float* __restrict__ d, const float* __restrict__ X, float* __restrict__ Sb,
                  float* __restrict__ Yb, int64_t npad, int mcols, double* __restrict__ part,
-                 const double* __restrict__ vpart, Tail tl) {
+                 const double* __restrict__ vpart, Tail tl, unsigned long long* progress) {
   if (off(&S->active)) return;
   __shared__ __align__(16) unsigned char raw[(kHeadSmemBytes + 15) / 16 * 16];  // warp sums, then the scalar stage
   static_assert(sizeof(raw) >= sizeof(float) * kHeadAcc * (kVecThreads / 32), "warp sums must fit");
@@ -1028,7 +1062,7 @@ step_head_kernel(SolverState* __restrict__ S, const float* __restrict__ g, const
       if (lane == 4) o[kHeadCols - 1] = 0.0;
     }
   }
-  if (last_block_done(&S->ticket)) step_head_body(S, part, gridDim.x, tl, raw, t, count, t_entry);
+  if (last_block_done(&S->ticket)) step_head_body(S, part, gridDim.x, tl, raw, t, count, t_entry, progress);
 }
 
 // the vector kernel of a step (see above).  `gz` is the buffer the scatter kernel adds into: g itself
@@ -1132,13 +1166,15 @@ step_vec_kernel(SolverState* __restrict__ S, const float* g, float* __restrict__
   }
 }
 
-// (re)arm the solver for iterations up to `limit`
-__global__ void resume_kernel(SolverState* __restrict__ S, int limit) {
+// (re)arm the solver for iterations up to `limit`, for the mde_solver_run call numbered `seq`
+__global__ void resume_kernel(SolverState* __restrict__ S, int limit, int seq, unsigned long long* progress) {
   if (threadIdx.x != 0) return;
   S->iter_limit = limit;
   if (S->paused && S->iter < limit) { S->paused = 0; S->active = 1; }
   else if (S->active && S->iter >= limit) { S->active = 0; S->paused = 1; }
   set_phase(S, S->phase);
+  S->run_seq = seq; S->run_steps = 0;
+  publish_progress(progress, S);
 }
 
 __global__ void init_state_kernel(SolverState* S, double eps, int memory, int max_stats, int world,
@@ -1149,6 +1185,7 @@ __global__ void init_state_kernel(SolverState* S, double eps, int memory, int ma
   S->dd = 0.0; S->xx = 0.0; S->t_last = 0.0; S->t_eval = 0.0; S->func_evals = 0;
   S->max_stats = max_stats; S->world = world;
   S->paused = 0; S->iter_limit = max_stats; S->pend = 0;
+  S->run_seq = 0; S->run_steps = 0;
   S->t_cur = 0.0;
   for (int c = 0; c < 4; ++c) { S->cs_g[c] = 0.0; S->cs_d[c] = 0.0; S->mu_x[c] = 0.0f; S->mu_d[c] = 0.0f; }
   for (int q = 0; q < kSlots; ++q) for (int c = 0; c < 4; ++c) { S->cs_S[q][c] = 0.0; S->cs_Y[q][c] = 0.0; }
@@ -1177,6 +1214,10 @@ struct mde_solver {
   mde_solver_opts_t opts{};
   SolverState* S = nullptr;          // device
   int* status_host = nullptr;        // pinned, kStatusInts ints
+  unsigned long long* progress = nullptr;      // pinned and mapped: the progress word (host view)
+  unsigned long long* progress_dev = nullptr;  //   ... and its device address
+  int run_seq = 0;                   // sequence number of the last mde_solver_run call, modulo kProgSeqMask + 1
+  long long run_launched = 0;        // steps that call enqueued
   float *X = nullptr, *xinit = nullptr, *d = nullptr, *g = nullptr, *gprev = nullptr, *Sb = nullptr, *Yb = nullptr;
   float* gpart = nullptr;            // multi-GPU: this rank's partial [gradient | loss] before the all-reduce
   double *dpart = nullptr;           // partial rows of the head kernel
@@ -1222,6 +1263,51 @@ int read_status(mde_solver* s, cudaStream_t st) {
   MDE_CUDA_TRY(cudaMemcpyAsync(s->status_host, s->S, kStatusInts * sizeof(int), cudaMemcpyDeviceToHost, st));
   MDE_CUDA_TRY(cudaStreamSynchronize(st));
   return 0;
+}
+
+// Steps to enqueue now (kStepsPerGraph, 1 or 0), with `in_flight` steps enqueued whose head kernel has not run and
+// `left` iterations before the pause, as of one snapshot of the progress word.  An iteration ends in a head kernel and
+// takes at least one step, so the next `left` steps all run: an eight-step graph goes in while in_flight + 8 <= left
+// (about two of them queued), closer to the pause a one-step graph while in_flight < left (and < 8).  With nothing in
+// flight and the solve not stopped, the next step runs too.  So no step is enqueued after the pause.  Near it the queue is one step deep when
+// an iteration takes more steps than it has left: the head kernel's result reaches the host while that step's vector
+// and distortion kernels run.  (Convergence or an error cannot be foreseen: up to 2 kStepsPerGraph steps are queued
+// when one stops the solve, and they exit at their gates.)
+int feed_policy(long long in_flight, long long left) {
+  if (in_flight <= kStepsPerGraph && in_flight + kStepsPerGraph <= left) return kStepsPerGraph;
+  return ((in_flight < left && in_flight < kStepsPerGraph) || in_flight == 0) ? 1 : 0;
+}
+
+// Enqueue step graphs as the progress word reports the device's steps, until it reports a stop; *stop = that word.
+// Returns with *stop.stopped false when the word has not changed for a second (a step that long, or a stream still
+// busy with earlier work): the caller then synchronises and reads the status.  `launched` counts the steps of this run.
+int feed_steps(mde_solver* s, int target, int seq, long long* launched, Progress* stop, cudaStream_t st) {
+  using clock = std::chrono::steady_clock;
+  unsigned long long last = ~0ull;
+  clock::time_point since = clock::now();
+  *stop = Progress{};
+  for (;;) {
+    const unsigned long long w = *static_cast<volatile unsigned long long*>(s->progress);
+    const Progress pg = decode_progress(w);
+    long long done = 0;
+    int iter = s->host_iter;
+    if (pg.seq == seq) {  // (else resume_kernel of this run has not run yet)
+      if (pg.stopped) { *stop = pg; return 0; }
+      done = pg.steps;
+      iter = pg.iter;
+    }
+    const int k = feed_policy((*launched - done) & kProgStepsMask, (long long)target - iter);
+    if (k) {
+      MDE_CUDA_TRY(cudaGraphLaunch(k == 1 ? s->step_exec : s->steps_exec, st));
+      *launched += k;
+      g_launch_count += (unsigned long long)k * s->step_kernels;
+    } else if (w != last) {
+      last = w;
+      since = clock::now();
+    } else if (clock::now() - since > std::chrono::seconds(1)) {
+      return 0;
+    }
+  }
 }
 
 // callable distortion function: distances -> the caller's torch code -> coefficients -> scatter.  The caller's part is
@@ -1354,7 +1440,8 @@ int enqueue_step(mde_solver* s, cudaStream_t st) {
   tl.lpart = s->edges->loss_partials; tl.nl = s->nl; tl.tail = s->g + s->npad;
   tl.p_total = (double)s->edges->p_total; tl.inv_n = 1.0 / (double)s->n;
   step_head_kernel<<<dim3(s->nvb, slices), kVecThreads, 0, st>>>(S, s->g, s->gprev, s->d, s->X, s->Sb, s->Yb, s->npad,
-                                                                 s->center_m, s->dpart, s->vpart, tl);
+                                                                 s->center_m, s->dpart, s->vpart, tl,
+                                                                 s->progress_dev);
   MDE_LAUNCH_CHECK();
   step_vec_kernel<<<s->nvb, kVecThreads, 0, st>>>(S, s->g, s->gprev, s->d, s->X, s->xinit, s->Sb, s->Yb, s->npad,
                                                   s->N, s->center_m, s->opts.world_size > 1 ? s->gpart : s->g,
@@ -1510,6 +1597,9 @@ int solver_create(mde_solver_t** out, const mde_edges_t* e, int64_t n, int m, co
 #define TRY(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { rc = (int)_e; goto fail; } } while (0)
   TRY(cudaMalloc(&s->S, sizeof(SolverState)));
   TRY(cudaMallocHost(&s->status_host, kStatusInts * sizeof(int)));
+  TRY(cudaHostAlloc(&s->progress, sizeof(unsigned long long), cudaHostAllocMapped));
+  *s->progress = 0ull;
+  TRY(cudaHostGetDevicePointer(&s->progress_dev, s->progress, 0));
   TRY(cudaMalloc(&s->X, vb)); TRY(cudaMalloc(&s->xinit, vb)); TRY(cudaMalloc(&s->d, vb));
   TRY(cudaMalloc(&s->gprev, vb));
   if (opts->world_size > 1) {
@@ -1626,7 +1716,7 @@ int mde_solver_set_external(mde_solver_t* s, const mde_external_t* ext, void* st
 
 int mde_solver_destroy(mde_solver_t* s) {
   if (!s) return 0;
-  cudaFree(s->S); cudaFreeHost(s->status_host);
+  cudaFree(s->S); cudaFreeHost(s->status_host); cudaFreeHost(s->progress);
   cudaFree(s->X); cudaFree(s->xinit); cudaFree(s->d); cudaFree(s->gprev);
   if (!s->comm_region) cudaFree(s->g);  // (several GPUs: g lives inside the peer-visible region)
   for (int q = 0; q < kMaxWorld; ++q) if (s->peer_base[q]) cudaIpcCloseMemHandle(s->peer_base[q]);
@@ -1771,19 +1861,40 @@ int mde_solver_run(mde_solver_t* s, int iters, int* iters_done, int* converged, 
   }
   int target = s->host_iter + iters;
   if (target > s->cur_max_iter) target = s->cur_max_iter;
-  resume_kernel<<<1, 32, 0, st>>>(s->S, target);
+  const int seq = s->run_seq = (s->run_seq + 1) & kProgSeqMask;
+  resume_kernel<<<1, 32, 0, st>>>(s->S, target, seq, s->progress_dev);
   MDE_LAUNCH_CHECK();
+  // One GPU with step graphs: the host keeps the queue fed from the progress word and takes the result of a clean stop
+  // (pause, convergence, iteration cap) from it, without synchronising: what is still queued then is the rest of the
+  // stopping step and the steps after a convergence, all gated off, and they complete in stream order.  After an
+  // error or a stall it reads the status.  Stream-launched steps and sharded solves read the status after every
+  // batch (every rank must enqueue the same steps, decided from the same status).
+  const bool fed = s->steps_exec && s->opts.world_size == 1;
+  long long launched = 0;
   for (int round = 0;; ++round) {
     if (round > (1 << 18)) return MDE_E_INVALID;
     int remaining = target - s->host_iter;
     if (remaining < 1) remaining = 1;
     long long steps = 0;
-    if (!s->steps_exec) {
+    if (fed) {
+      Progress stop;
+      rc = feed_steps(s, target, seq, &launched, &stop, st);
+      s->run_launched = launched;
+      if (rc) return rc;
+      if (stop.stopped && !stop.failed) {
+        s->host_iter = stop.iter;
+        s->host_active = stop.paused;  // only a pause can be resumed
+        if (iters_done) *iters_done = stop.iter;
+        if (converged) *converged = stop.converged;
+        return 0;
+      }
+    } else if (!s->steps_exec) {
       // host hook (all-reduce, or a callable distortion function in hook mode): stream-launched steps; every rank
       // enqueues the same number of steps (same `remaining`: the replicated state machines agree)
       int n_steps = remaining + remaining / 8 + (round > 0 ? 1 : 0) + 1;
       if (n_steps > 64) n_steps = 64;
       for (int b = 0; b < n_steps; ++b) { if ((rc = enqueue_step(s, st))) return rc; }
+      launched += n_steps;
     } else if (remaining >= kStepsPerGraph) {
       int graphs = (remaining + remaining / 8 + 1) / kStepsPerGraph;
       if (graphs * kStepsPerGraph > 96) graphs = 96 / kStepsPerGraph;  // <= ~96 steps in flight per status read
@@ -1795,6 +1906,8 @@ int mde_solver_run(mde_solver_t* s, int iters, int* iters_done, int* converged, 
       steps = singles;
     }
     g_launch_count += (unsigned long long)steps * s->step_kernels;  // (stream-launched steps count themselves)
+    launched += steps;
+    s->run_launched = launched;
     if ((rc = read_status(s, st))) return rc;
     s->host_iter = s->status_host[2];
     if (s->status_host[3]) { s->host_active = 0; if (iters_done) *iters_done = s->status_host[2]; return s->status_host[3]; }
@@ -1802,9 +1915,20 @@ int mde_solver_run(mde_solver_t* s, int iters, int* iters_done, int* converged, 
       s->host_active = s->status_host[8];  // only a pause can be resumed
       break;
     }
+    // still active after a stall: every step enqueued has run, and each one published the word
+    const Progress pg = decode_progress(*static_cast<volatile unsigned long long*>(s->progress));
+    if (fed && (pg.seq != seq || pg.steps != (launched & kProgStepsMask))) return MDE_E_INVALID;
   }
   if (iters_done) *iters_done = s->status_host[2];
   if (converged) *converged = s->status_host[1];
+  return 0;
+}
+
+int mde_solver_debug_run_steps(mde_solver_t* s, int64_t* launched, int64_t* ran) {
+  if (!s || !launched || !ran) return MDE_E_INVALID;
+  const Progress pg = decode_progress(*static_cast<volatile unsigned long long*>(s->progress));
+  *launched = s->run_launched;
+  *ran = pg.seq == s->run_seq ? pg.steps : 0;
   return 0;
 }
 
@@ -1840,6 +1964,7 @@ void* mde_dbg_ls_new(double t0, double f0, float gtd0, float d_norm) {
   return L;
 }
 void mde_dbg_ls_free(void* p) { delete (LsState*)p; }
+int mde_dbg_feed_policy(int64_t in_flight, int64_t left) { return feed_policy(in_flight, left); }
 double mde_dbg_ls_t(void* p) { return ((LsState*)p)->t; }
 int mde_dbg_ls_step(void* p, double f_new, float gtd_new, int grad_finite) {
   LsState* L = (LsState*)p;
